@@ -1,17 +1,17 @@
 #!/usr/bin/env python
-"""Benchmark of the fused tri-plane render (BASELINE.json metric: rays/s at 128x128, 64 coarse +
-64 fine samples per ray).
+"""Benchmark of the fused tri-plane render (metric: rays/s at 128x128, 64 coarse + 64 fine samples
+per ray).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
-                    [--config 2|3|4|5] [--scaling weak|strong]
+                    [--config 2|3|4|5] [--scaling weak|strong] [--dump-outputs DIR]
 
-Workloads (BASELINE.json `configs`):
+Workloads:
   --config 2 (default)  p3d_car generator forward: batch 32 per GPU, 256^2 x 32ch fp32 tri-planes
              -> 128x128 rays x (64 + 64) samples -> rgb / depth / mask.
-               value     render with the planes resident in HBM in the layout the sm_100a plane
+               value     render with the planes resident in HBM in the layout the sm_90a plane
                          producer emits (channel-last), CUDA events, max over ranks
                e2e       w -> image through the public API: latents in pinned host memory -> H2D
-                         -> synthesis network (tcgen05 kernels) -> render -> D2H of rgb/depth/mask
+                         -> synthesis network (wgmma kernels) -> render -> D2H of rgb/depth/mask
                roofline  render_forward_pipe against the algorithmic tensor-FLOP bound (SURVEY 8d)
                cpu_baseline / --impl reference: the reference's own render on the host cores
   --config 3  cub --run_inversion: orthographic, scene_range 2, GLOBAL batch 16 sharded over the
@@ -22,8 +22,11 @@ Workloads (BASELINE.json `configs`):
   --config 5  inversion sweep: resolution {128, 256} x samples/ray {32, 64, 128}, forward and
              forward+backward, 8 images per GPU; one JSON line with a `sweep` list.
 --scaling strong (config 2): global batch 32 split over the GPUs instead of 32 per GPU.
+--dump-outputs DIR (config 2): after the timed steps, rank 0 writes the rgb / depth / mask of the
+             last timed step as DIR/rgb.npy, DIR/depth.npy, DIR/mask.npy (float32, 10.5 MB at the
+             default batch); the inputs are seeded, so two builds can be compared output for output.
 
-Inputs (>= 0.8 GB per GPU at config 2) are far larger than the 126 MB L2, so consecutive steps
+Inputs (>= 0.8 GB per GPU at config 2) are far larger than the 50 MB L2, so consecutive steps
 cannot be served from cache.
 """
 import argparse
@@ -65,20 +68,8 @@ def peaks():
         p = json.load(open(path))
         return dict(hbm_gbs=p['hbm_gbs'], tflops=p.get('bf16_tflops_sustained', p['bf16_tflops']),
                     source='measured (MEASURED_PEAKS.json, bf16 sustained)')
-    return dict(hbm_gbs=6650.0, tflops=1590.0, source='fallback (B200_PROFILING.md)')
-
-
-def measured_traffic(kernel, batch):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of `kernel` from the committed
-    `ncu --set full` capture (profiles/traffic.json: written from the raw csv by
-    tools/ncu_summary.py); None when no capture of this batch size exists."""
-    path = os.path.join(ROOT, 'profiles', 'traffic.json')
-    if not os.path.isfile(path):
-        return None, None
-    for row in json.load(open(path)):
-        if row['kernel'] == kernel and row['batch'] == batch:
-            return row['dram_bytes'], row['source']
-    return None, None
+    return dict(hbm_gbs=3350.0, tflops=989.0,
+                source='H100 SXM data sheet (dense BF16, 700 W card), not measured')
 
 
 class ClockSampler(threading.Thread):
@@ -146,8 +137,8 @@ def _cpu_case(n_images):
 
 
 def reference_kind():
-    """'reference' when the unmodified reference can run here (staged into baseline/_ref by
-    tools/stage_reference.py, or /root/reference itself), else 'port' (the oracle)."""
+    """'reference' when the unmodified reference can run here (installed into oracle/_ref by
+    oracle/stage_reference.py), else 'port' (the oracle)."""
     from oracle import reference_lift as RL
     return 'reference' if RL.available() else 'port'
 
@@ -250,7 +241,7 @@ def run_reference(args):
                          'sample': '%d image(s) of the batch per step (same geometry; images are '
                                    'independent, the rate is per ray), torch CPU fp32, no_grad; %s'
                                    % (n_img, 'unmodified reference render (run.py:176-350 lifted '
-                                      'from baseline/_ref), planes given' if kind == 'reference'
+                                      'from oracle/_ref), planes given' if kind == 'reference'
                                       else 'oracle port of the reference ops')},
         'e2e': {'value': value, 'unit': UNIT, 'h2d_bytes_per_step': 0, 'd2h_bytes_per_step': 0},
         'gpu_launches': 0,
@@ -258,7 +249,7 @@ def run_reference(args):
     print(json.dumps(line))
 
 
-# ------------------------------------------------------------------ the B200 arm
+# ------------------------------------------------------------------ the fused (CUDA) arm
 class Bench:
     def __init__(self, args):
         import torch.distributed as dist
@@ -316,7 +307,7 @@ class Bench:
                             attention_values=CFG['attention_values'], scene_range=ds['scene_range'],
                             white_background=ds['white_background'],
                             object_radius=ds['object_radius'], device=self.dev)
-        if layout == 'channel_last':   # what the sm_100a plane producer emits
+        if layout == 'channel_last':   # what the sm_90a plane producer emits
             sc['planes'] = sc['planes'].permute(0, 1, 3, 4, 2).contiguous()
         cams = syn.make_cameras(seed, batch, ortho=ds['ortho'], radius=ds['radius'], device=self.dev)
         nt, nu = syn.make_noise(seed, batch, H, W, S, device=self.dev)
@@ -413,6 +404,12 @@ class Bench:
         clocks = sampler.summary() if rank == 0 else None
         ms_step = self.max_over_ranks(ev0.elapsed_time(ev1)) / a.steps
         rays_step = gb * H * W
+        if a.dump_outputs and rank == 0:
+            import numpy as np
+            os.makedirs(a.dump_outputs, exist_ok=True)
+            for name, t in zip(('rgb', 'depth', 'mask'), last):
+                np.save(os.path.join(a.dump_outputs, name + '.npy'),
+                        t.detach().float().cpu().numpy())
         value = rays_step / (ms_step * 1e-3)
         k_ms = sum(x.elapsed_time(y) for x, y in kernel_events) / max(1, len(kernel_events))
         coll_ms = (self.max_over_ranks(sum(x.elapsed_time(y) for x, y in gather_events)
@@ -466,10 +463,9 @@ class Bench:
         flops_launch = float(B * H * W) * (2 * S) * FLOPS_PER_POINT
         hbm_bytes_launch = float(B) * 3 * 32 * CFG['plane_res'] ** 2 * 4 + B * H * W * 20.0
         achieved_tf = flops_launch / (k_ms * 1e-3) / 1e12 if k_ms > 0 else 0.0
-        traffic, traffic_src = measured_traffic('render_forward_pipe', B)
         roofline = {
             'bound': 'tensor', 'achieved': achieved_tf, 'peak': pk['tflops'], 'unit': 'TFLOP/s',
-            'frac': achieved_tf / pk['tflops'], 'traffic': traffic, 'traffic_source': traffic_src,
+            'frac': achieved_tf / pk['tflops'],
             'kernel': 'render_forward_pipe (dominant kernel of the step)', 'kernel_ms': k_ms,
             'kernel_share_of_step': k_ms / ms_step if ms_step > 0 else None,
             'algorithmic_flops_per_launch': flops_launch,
@@ -489,7 +485,7 @@ class Bench:
                 'algorithmic_flops_per_step': flops_launch + bwd_flops,
                 'what': 'render_forward_pipe + render_backward_pipe (pose gradients on) of one '
                         'inversion step; the backward is bound by its three line-rate passes per '
-                        'point -- gather, red.global.add.v4 scatter, pose re-read (DESIGN.md 8.2)'}
+                        'point -- gather, red.global.add.v4 scatter, pose re-read'}
         cpu_baseline = parity = eager = None
         if world == 1 and not a.no_cpu_baseline:
             cpu_baseline, parity = self.cpu_baseline_and_parity(cfg, H, W, S)
@@ -513,7 +509,7 @@ class Bench:
     def e2e_generator_forward(self, B, gb, H, W, S):
         """w -> image end to end: the per-step inputs (latents, cameras) start in pinned host
         memory, the image ends in pinned host memory; synthesis network and render both on the
-        sm_100a kernels.  With the reference files staged the call is the public drop-in
+        sm_90a kernels.  With the reference files staged the call is the public drop-in
         ``render()`` on the reference's own Generator; otherwise the same two stages are called
         directly on seeded synthesis parameters."""
         from nerf_from_image_b200 import render as R
@@ -557,7 +553,7 @@ class Bench:
                 torch.cuda.synchronize()
             api = ('nerf_from_image_b200.render.render (drop-in of run.py:176-350) on the reference '
                    'Generator with enable_fused_synthesis: mapping-free w input -> texture mapper -> '
-                   'FusedSynthesis (tcgen05) -> fused render')
+                   'FusedSynthesis (wgmma) -> fused render')
             fs_only = FusedSynthesis(g.synthesis_network)
             ws_dev = host['ws'].to(dev)
             synth_only = lambda: fs_only(ws_dev[:, :14])
@@ -621,7 +617,7 @@ class Bench:
                 'd2h_bytes_per_step': d2h, 'ms_per_step': dt * 1e3,
                 'mask_mean': host['mask'].mean().item(), 'api': api, 'synthesis': synthesis,
                 'what': 'generator forward, w -> image: latents + cameras H2D from pinned memory, '
-                        'synthesis network and render on the sm_100a kernels (both random draws '
+                        'synthesis network and render on the sm_90a kernels (both random draws '
                         'made on the device like the reference), rgb/depth/mask D2H; wall clock '
                         'incl. synchronisation, max over ranks'}
 
@@ -635,7 +631,7 @@ class Bench:
         from nerf_from_image_b200.synthesis import FusedSynthesis
         from oracle import reference_lift as RL  # availability probe + module import only
         if not RL.available():
-            return {'unavailable': 'reference files not staged (tools/stage_reference.py)'}
+            return {'unavailable': 'reference not installed (oracle/stage_reference.py)'}
         try:
             import types
             dev = self.dev
@@ -758,7 +754,7 @@ class Bench:
         return {'value': gb * H * W / (ms_b * 1e-3), 'unit': UNIT, 'ms_per_step': ms_b,
                 'what': 'fused_render forward + backward through the autograd.Function (grads to '
                         'planes, palette, %s)' % (
-                            'decoder weights (render_wgrad_pipe, tcgen05), beta, alpha (+ their '
+                            'decoder weights (render_wgrad_pipe, wgmma), beta, alpha (+ their '
                             'all-reduce); cameras are data' if weights
                             else 'tform_cam2world; decoder frozen')}
 
@@ -777,7 +773,7 @@ class Bench:
         cpu = {'value': rate, 'unit': UNIT, 'cores': cores, 'host_cores': os.cpu_count(), 'kind': kind,
                'sample': '%d of the 32 images (same geometry) x %d passes, %.1f s, torch CPU fp32 '
                          'no_grad, %s' % (n_img, reps, dt, 'unmodified reference render lifted from '
-                                          'baseline/_ref' if kind == 'reference' else 'oracle port')}
+                                          'oracle/_ref' if kind == 'reference' else 'oracle port')}
         # parity of the CUDA path on exactly those images, against the oracle with the same
         # injected noise (the reference draws its own: same distribution, different numbers)
         from oracle import render_oracle as O
@@ -855,7 +851,7 @@ class Bench:
             'data': 'synthetic', 'config': config_block(a, world, B, gb), 'clocks': clocks,
             'forward_only': {'value': gb * H * W / (ms_f * 1e-3), 'unit': UNIT, 'ms_per_step': ms_f},
             'images_per_gpu': B,
-            'tiles_per_gpu': tiles, 'waves_of_148_ctas': tiles / 148.0,
+            'tiles_per_gpu': tiles, 'waves_of_132_ctas': tiles / 132.0,
             # per step: weight image + render_forward_pipe, weight images + render_backward_pipe,
             # with decoder gradients also weight images + render_wgrad_pipe
             'what': res['what'], 'gpu_launches': (5 if inv else 8) * steps,
@@ -917,6 +913,8 @@ def main():
     ap.add_argument('--quick', action='store_true', help='skip the side legs (ncu, A/B runs)')
     ap.add_argument('--e2e-steps', type=int, default=3)
     ap.add_argument('--mlp-mode', type=lambda x: int(x, 0), default=0)
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='config 2: write rgb / depth / mask of the last timed step as DIR/<name>.npy')
     args = ap.parse_args()
     args.steps_given = args.steps is not None
     if args.steps is None:

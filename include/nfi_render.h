@@ -1,5 +1,5 @@
 /*
- * nfi_render.h -- C ABI of the B200 (sm_100a) fused tri-plane volume renderer.
+ * nfi_render.h -- C ABI of the H100 (sm_90a) fused tri-plane volume renderer.
  *
  * Drop-in boundary for ONE hot path of google-research/nerf-from-image: the
  * per-ray render (SURVEY.md section 8).  The reference has no FFI of its own
@@ -71,11 +71,12 @@ enum nfi_noise_mode {
 enum nfi_mlp_mode {
   NFI_MLP_AUTO = 0,
   NFI_MLP_FP32_SIMT = 1, /* fp32 FFMA on CUDA cores                      */
-  NFI_MLP_TC_3XTF32 = 2, /* tcgen05.mma kind::tf32, hi/lo split (3 MMAs), lockstep tile groups */
+  NFI_MLP_TC_3XTF32 = 2, /* wgmma tf32, hi/lo split (3 MMAs), lockstep tile groups */
   NFI_MLP_TC_WARPSPEC = 3, /* alias of NFI_MLP_TC_PIPE (the first warp-specialised kernel, whose two
                               roles shared one ring stage per chain, was retired) */
   NFI_MLP_TC_PIPE = 4 /* same arithmetic, fully pipelined: A stages released at MMA completion,
-                         hidden activations stay in TMEM, consumers software-pipelined (default) */
+                         hidden activations stay in registers, consumers software-pipelined
+                         (default) */
 };
 
 typedef struct nfi_render_params {
@@ -197,7 +198,7 @@ typedef struct nfi_render_grads {
 
 /* library / build identification */
 NFI_API int nfi_abi_version(void);
-NFI_API const char *nfi_build_info(void); /* "sm_100a ..." */
+NFI_API const char *nfi_build_info(void); /* "sm_90a ..." */
 NFI_API const char *nfi_last_error(void);
 
 /* Scratch the forward / backward kernels need for `params` (bytes). */
@@ -229,8 +230,8 @@ NFI_API int nfi_decoder_forward(const float *features, int64_t n_points, const f
 
 /* autograd of the above (SURVEY.md section 8 row a13): recomputes the samples.
  * With params->workspace >= 64 KiB, no semantics output and S <= 128, S % 4 == 0 the four GEMMs of
- * a sample step run on tcgen05 (render_backward_pipe).  Decoder-weight gradients (grad_w1 / b1 /
- * w2 / b2) come from render_wgrad_pipe (MN-major bf16-pair GEMMs on tcgen05), which needs
+ * a sample step run on the tensor cores (render_backward_pipe).  Decoder-weight gradients (grad_w1 /
+ * b1 / w2 / b2) come from render_wgrad_pipe (MN-major bf16-pair GEMMs on wgmma), which needs
  * params->workspace >= NFI_BACKWARD_WORKSPACE_BYTES: without pose gradients (the GAN generator
  * step) it is the WHOLE backward in one sweep, with them it runs beside render_backward_pipe.
  * Everything outside that envelope: the fp32 SIMT kernel. */

@@ -1,5 +1,5 @@
 /*
- * nfi_synth.h -- C ABI of the B200 (sm_100a) tri-plane producer: the StyleGAN2 synthesis
+ * nfi_synth.h -- C ABI of the H100 (sm_90a) tri-plane producer: the StyleGAN2 synthesis
  * network that google-research/nerf-from-image runs in front of its per-ray render
  * (SURVEY.md section 8f, N1; the "a5" row of section 8a).
  *
@@ -12,11 +12,11 @@
  * (nerf_from_image_b200/synthesis.py), and it emits the planes CHANNEL-LAST ([B,3,R,R,32]), the
  * layout nfi_render_forward gathers from, so no re-layout pass sits between the two.
  *
- * Arithmetic: every convolution is an implicit GEMM on tcgen05 (kind::f16 on bf16 operands: the
- * activations and weights are kept as bf16 hi + lo pairs -- 16 significant bits, 4 bytes per element
- * like the fp32 they stand for -- three MMAs per product, fp32 accumulation in TMEM; measured
- * 1.4e-4 relative L2 against the fp64 network at the full 512-channel size, bounded by the tensor
- * core's accumulation, not by the operands), operands staged by TMA (cp.async.bulk.tensor),
+ * Arithmetic: every convolution is an implicit GEMM on wgmma (bf16 operands: the activations and
+ * weights are kept as bf16 hi + lo pairs -- 16 significant bits, 4 bytes per element like the fp32
+ * they stand for -- three MMAs per product, fp32 accumulation in registers; the error against the
+ * fp64 network is bounded by the tensor core's accumulation, not by the operands; the tests hold it
+ * under 3e-4 relative L2 at the full 512-channel size), operands staged by TMA (cp.async.bulk.tensor),
  * prologue (style scaling) folded into the producing layer's epilogue, epilogue (demodulation,
  * noise, bias, gain, leaky-relu, next layer's style, hi/lo split) fused.  Conventions as in nfi_render.h:
  * device pointers, fp32, stream as void*, 0 = success, text via nfi_last_error().

@@ -167,7 +167,7 @@ class NfiError(RuntimeError):
 
 
 def build(verbose=False):
-    """Compiles the library in-tree (nvcc, sm_100a)."""
+    """Compiles the library in-tree (nvcc, sm_90a)."""
     script = os.path.join(_HERE, 'csrc', 'build.sh')
     res = subprocess.run(['bash', script], capture_output=True, text=True)
     if verbose or res.returncode != 0:

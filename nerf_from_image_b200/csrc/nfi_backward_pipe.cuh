@@ -2,7 +2,7 @@
 //
 // Same mathematics as nfi_backward.cuh (single front-to-back sweep over the merged
 // depth order, field re-evaluated at every sample, no saved per-sample tensor) but
-// all four GEMMs of a sample step run on tcgen05 with 3xTF32 operands:
+// all four GEMMs of a sample step run on the tensor cores (wgmma) with 3xTF32 operands:
 //
 //   MMA1  D1 = F  W1^T          [128 x 32] x [32 x 64]   pre-activations (x log2 e)
 //   MMA2  D2 = H  W2^T          [128 x 64] x [64 x 16]   decoder outputs
@@ -14,52 +14,52 @@
 //           forward kernel does and, when D4 of such a step is ready, scatters it
 //           into the plane gradient (red.global.add.v4, 8 lanes per texel) and
 //           accumulates the camera gradient of its rays;
-//   P       four MMA issuer warps, one per GEMM;
-//   P+1     shading, thread = ray: decoder outputs -> density / colour ->
-//           reverse compositing -> dOut (hi/lo split into TMEM), palette / beta /
-//           alpha gradients;
-//   P+2     activation, thread = TMEM lane: softplus forward (D1 -> H) and its
-//           reverse (D3, H -> dpre = D3 * (1 - exp(-H))).
-// TMEM: two slots of 240 columns,
-//   [0,64)  D1 -> H_lo -> D4 ([0,32))     [64,128) H_hi -> dpre_hi     [128,144) D2
-//   [144,176) dOut hi | lo                [176,240) D3 -> dpre_lo
-// Decoder-weight gradients (GAN generator step) are NOT produced here: that case
-// stays on render_backward_simt.
+//   P       shading, thread = ray: decoder outputs -> density / colour ->
+//           reverse compositing -> dOut, palette / beta / alpha gradients;
+//   P+1     activation: issues all four GEMMs (accumulators in its registers, one 64-row half
+//           of the tile after the other) with softplus forward (D1 -> H) and its reverse
+//           (D3, H -> dpre = D3 * (1 - exp(-H))) on the accumulator registers.  Its order is
+//           fwd(m+1) before bwd(m), so that the shading chain of step m overlaps the forward
+//           GEMMs of step m+1; bwd(m) recomputes D1 from the stage, which stays resident until
+//           then (a stored H would not fit the shared memory).
+// Shared-memory slots (two of each): D2 -> dOut ([128 x 20] fp32: the shading thread reads its
+// row of D2 and writes its row of dOut in its place) and D4 ([128 x 36] fp32).
+// Decoder-weight gradients (GAN generator step) are NOT produced here (nfi_wgrad_pipe.cuh).
 #pragma once
 #include "nfi_forward_pipe.cuh"
 
 namespace nfi {
 
 constexpr int kBwdSlots = 2;
-constexpr int kBwdSlotCols = 240;
 constexpr int kBwdStages = 3;
+constexpr int kD4Ld = 36;  // floats per row of a D4 slot
+constexpr int kD4SlotBytes = kThreads * kD4Ld * 4;
 // backward weight image (bytes), appended to the forward image
 constexpr int kWbW2tHi = 0;      // [64 rows = hidden j][32 k = output o, 16 used] SW128, 8 KB
 constexpr int kWbW2tLo = 8192;
 constexpr int kWbW1tHi = 16384;  // [32 rows = channel c][64 k = hidden j] as two [32 x 32] k-blocks
-constexpr int kWbW1tLo = 24576;
+constexpr int kWbW1tLo = 24576;  //   (K positions in register-fragment order: tc::kpos_of_hidden)
 constexpr int kWbBytes = 32768;
 
 template <int P>
 struct BwdCfg {
-  static constexpr int kThreadsTotal = 384 + 128 * P;
+  static constexpr int kThreadsTotal = 256 + 128 * P;
   static constexpr int kSmWb = 25600;                      // backward weight image
   static constexpr int kSmA = kSmWb + kWbBytes;            // 58368 = 57 * 1024
-  static constexpr int kSmStage = kSmA + kBwdStages * kPipeStageBytes;  // per-warp scatter staging
-  static constexpr int kStageWarp = 32 * 36 * 4 + 32 * 4 * 4;           // [32][36] dF + [32][4] coord grads
+  static constexpr int kSmD2 = kSmA + kBwdStages * kPipeStageBytes;  // D2 / dOut slots
+  static constexpr int kSmD4 = kSmD2 + kBwdSlots * kD2SlotBytes;     // D4 slots
+  static constexpr int kSmStage = kSmD4 + kBwdSlots * kD4SlotBytes;  // per-warp coord-grad staging
+  static constexpr int kStageWarp = 32 * 4 * 4;                      // [32][4] coord grads
   static constexpr int kSmPal = kSmStage + P * 4 * kStageWarp;
   static constexpr int kSmFrac = kSmPal + 48 * 4;
   static constexpr int kSmBars = kSmFrac + 128 * 4;
-  // full[3], a_free[3], per slot: d1_full, h_ready, d2_full, dout_ready, d3_full, dpre_ready,
-  // d4_full, slot_free; weights x2
-  static constexpr int kNumBars = 2 * kBwdStages + 8 * kBwdSlots + 2;
-  static constexpr int kSmTmemPtr = kSmBars + kNumBars * 8;
-  static constexpr int kSmBytes = kSmTmemPtr + 16;
-  // P = 2: 640 x 96 = 61440 = 128 x (88 + 112 + 24) + 256 x 128
-  static constexpr int kActRegs = 88;
+  // full[3], a_free[3], per slot: d2_full, dout_ready, d4_full, slot_free; weights x2
+  static constexpr int kNumBars = 2 * kBwdStages + 4 * kBwdSlots + 2;
+  static constexpr int kSmBytes = kSmBars + kNumBars * 8;
+  // P = 2: 512 x 128 = 65536 = 128 x (144 + 112) + 256 x 128 (the producers keep the launch
+  // allocation)
+  static constexpr int kActRegs = 144;
   static constexpr int kShadeRegs = 112;
-  static constexpr int kAuxRegs = 24;
-  static constexpr int kProducerRegs = 128;
 };
 
 // W2^T (padded to K = 32) and W1^T / 3, split into TF32 hi/lo, K-major SWIZZLE_128B.
@@ -77,37 +77,54 @@ static __global__ void prep_weight_image_bwd(const float* __restrict__ w1, const
     const int c = i / kHid, j = i % kHid;  // B4[c][j] = W1[j][c] / 3 (features = mean of 3 planes)
     const float w = w1[j * kC + c] * (1.f / 3.f);
     const float hi = tc::tf32_hi(w);
-    const uint32_t off = (j >> 5) * 4096 + tc::sw128_offset(c, (j & 31) >> 2) + (j & 3) * 4;
+    const int jp = tc::kpos_of_hidden(j);
+    const uint32_t off = (jp >> 5) * 4096 + tc::sw128_offset(c, (jp & 31) >> 2) + (jp & 3) * 4;
     *reinterpret_cast<float*>(img + kWbW1tHi + off) = hi;
     *reinterpret_cast<float*>(img + kWbW1tLo + off) = w - hi;
   }
 }
 
-// D3 = dOut_lo*B_hi + dOut_hi*B_lo + dOut_hi*B_hi   (K = 16: two k-steps)
-__device__ __forceinline__ void issue_mma3(uint32_t d3, uint32_t dout_hi, uint32_t dout_lo,
-                                           uint64_t b_hi, uint64_t b_lo) {
-  constexpr uint32_t idesc = tc::umma_idesc_tf32(128, 64);
-  tc::umma_ts<false>(d3, dout_lo, b_hi, idesc);
-  tc::umma_ts<true>(d3, dout_lo + 8, b_hi + 2, idesc);
-  tc::umma_ts<true>(d3, dout_hi, b_lo, idesc);
-  tc::umma_ts<true>(d3, dout_hi + 8, b_lo + 2, idesc);
-  tc::umma_ts<true>(d3, dout_hi, b_hi, idesc);
-  tc::umma_ts<true>(d3, dout_hi + 8, b_hi + 2, idesc);
+// dOut rows of one 64-row block (row-major slot, kD2Ld floats per row) as TF32 hi / lo register
+// A fragments of the two k-blocks of K = 16
+__device__ __forceinline__ void load_dout_frags(const float* rows, int warp, int lane,
+                                                uint32_t (&hi)[2][4], uint32_t (&lo)[2][4]) {
+  const int g = lane >> 2, t = lane & 3;
+  const float* r0 = rows + (16 * warp + g) * kD2Ld + t;
+#pragma unroll
+  for (int kb = 0; kb < 2; ++kb) {
+    tc::put_split(hi, lo, kb, 0, r0[8 * kb]);
+    tc::put_split(hi, lo, kb, 1, r0[8 * kD2Ld + 8 * kb]);
+    tc::put_split(hi, lo, kb, 2, r0[8 * kb + 4]);
+    tc::put_split(hi, lo, kb, 3, r0[8 * kD2Ld + 8 * kb + 4]);
+  }
+}
+// D3 = dOut_lo*B_hi + dOut_hi*B_lo + dOut_hi*B_hi   (K = 16: two k-steps), one 64-row block
+__device__ __forceinline__ void mma3_mb(float (&d3)[32], const uint32_t (&hi)[2][4],
+                                        const uint32_t (&lo)[2][4], uint64_t b_hi, uint64_t b_lo) {
+  tc::wgmma_tf32_rs_n64(d3, lo[0], b_hi, 0);
+  tc::wgmma_tf32_rs_n64(d3, lo[1], b_hi + 2, 1);
+  tc::wgmma_tf32_rs_n64(d3, hi[0], b_lo, 1);
+  tc::wgmma_tf32_rs_n64(d3, hi[1], b_lo + 2, 1);
+  tc::wgmma_tf32_rs_n64(d3, hi[0], b_hi, 1);
+  tc::wgmma_tf32_rs_n64(d3, hi[1], b_hi + 2, 1);
 }
 // D4 = dpre_lo*B_hi + dpre_hi*B_lo + dpre_hi*B_hi   (K = 64: two k-blocks of 4 k-steps)
-__device__ __forceinline__ void issue_mma4(uint32_t d4, uint32_t dpre_hi, uint32_t dpre_lo,
-                                           uint64_t b_hi, uint64_t b_lo) {
-  constexpr uint32_t idesc = tc::umma_idesc_tf32(128, 32);
-  tc::umma_ts<false>(d4, dpre_lo, b_hi, idesc);
-#pragma unroll
-  for (int ks = 1; ks < 8; ++ks)
-    tc::umma_ts<true>(d4, dpre_lo + 8 * ks, b_hi + (ks >> 2) * 256 + (ks & 3) * 2, idesc);
+__device__ __forceinline__ void mma4_mb(float (&d4)[16], const uint32_t (&hi)[8][4],
+                                        const uint32_t (&lo)[8][4], uint64_t b_hi, uint64_t b_lo) {
 #pragma unroll
   for (int ks = 0; ks < 8; ++ks)
-    tc::umma_ts<true>(d4, dpre_hi + 8 * ks, b_lo + (ks >> 2) * 256 + (ks & 3) * 2, idesc);
+    tc::wgmma_tf32_rs_n32(d4, lo[ks], b_hi + (ks >> 2) * 256 + (ks & 3) * 2, ks != 0);
 #pragma unroll
   for (int ks = 0; ks < 8; ++ks)
-    tc::umma_ts<true>(d4, dpre_hi + 8 * ks, b_hi + (ks >> 2) * 256 + (ks & 3) * 2, idesc);
+    tc::wgmma_tf32_rs_n32(d4, hi[ks], b_lo + (ks >> 2) * 256 + (ks & 3) * 2, 1);
+#pragma unroll
+  for (int ks = 0; ks < 8; ++ks)
+    tc::wgmma_tf32_rs_n32(d4, hi[ks], b_hi + (ks >> 2) * 256 + (ks & 3) * 2, 1);
+}
+template <int R>
+__device__ __forceinline__ void zero(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) d[i] = 0.f;
 }
 
 // byte_taps plus the "gradient flows" flags of make_taps (coordinate strictly inside
@@ -195,26 +212,23 @@ render_backward_pipe(const nfi_render_params p, const nfi_render_grads g,
   unsigned char* base = smem_raw;
   const int tid = threadIdx.x, lane = tid & 31;
   const int hw_wg = __shfl_sync(kFull, tid >> 7, 0);
-  // logical role: 0 activation, 1 shading, 2 MMA issuers, 3.. producer sets (see nfi_forward_pipe.cuh)
-  const int wg = (hw_wg < P) ? hw_wg + 3 : (P + 2 - hw_wg);
+  // logical role: 0 activation, 1 shading, 3.. producer sets (see nfi_forward_pipe.cuh)
+  const int wg = (hw_wg < P) ? hw_wg + 3 : (P + 1 - hw_wg);
   const int gt = tid & 127;
   const int wig = __shfl_sync(kFull, gt >> 5, 0);
   const int S = p.num_samples;
   const int n_total = (p.fine_sampling ? 2 : 1) * S;  // steps per tile
 
   uint64_t* bars = reinterpret_cast<uint64_t*>(base + Cfg::kSmBars);
-  uint64_t* full = bars;                     // [3] stage gathered (4 warps)
-  uint64_t* a_free = full + NS;              // [3] stage read by MMA1 (commit)
-  uint64_t* d1_full = a_free + NS;           // [2] commit
-  uint64_t* h_ready = d1_full + kBwdSlots;   // [2] 4 warps
-  uint64_t* d2_full = h_ready + kBwdSlots;   // [2] commit
-  uint64_t* dout_ready = d2_full + kBwdSlots;   // [2] 4 warps
-  uint64_t* d3_full = dout_ready + kBwdSlots;   // [2] commit
-  uint64_t* dpre_ready = d3_full + kBwdSlots;   // [2] 4 warps
-  uint64_t* d4_full = dpre_ready + kBwdSlots;   // [2] commit
-  uint64_t* slot_free = d4_full + kBwdSlots;    // [2] 4 warps (D4 read)
+  uint64_t* full = bars;                        // [3] stage gathered (4 warps)
+  uint64_t* a_free = full + NS;                 // [3] stage read by the last GEMM using it (4 warps)
+  uint64_t* d2_full = a_free + NS;              // [2] D2 in its slot (4 warps)
+  uint64_t* dout_ready = d2_full + kBwdSlots;   // [2] dOut in the same slot (4 warps)
+  uint64_t* d4_full = dout_ready + kBwdSlots;   // [2] D4 in its slot (4 warps)
+  uint64_t* slot_free = d4_full + kBwdSlots;    // [2] D4 scattered (4 warps)
   uint64_t* wbar = slot_free + kBwdSlots;       // [2] weight images landed
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(base + Cfg::kSmTmemPtr);
+  float* d2s = reinterpret_cast<float*>(base + Cfg::kSmD2);  // [2][128][kD2Ld]
+  float* d4s = reinterpret_cast<float*>(base + Cfg::kSmD4);  // [2][128][kD4Ld]
   const float* b1s = reinterpret_cast<const float*>(base + kWiB1);
   const float* b2s = reinterpret_cast<const float*>(base + kWiB2);
   float* pal = reinterpret_cast<float*>(base + Cfg::kSmPal);
@@ -224,28 +238,20 @@ render_backward_pipe(const nfi_render_params p, const nfi_render_grads g,
   if (tid == 0) {
     if (tc::smem_u32(base) & 1023u) __trap();
     for (int i = 0; i < NS; ++i) {
-      tc::mbar_init(&full[i], 4);
-      tc::mbar_init(&a_free[i], 1);
+      tc::mbar_init(&full[i], kWarps);
+      tc::mbar_init(&a_free[i], kWarps);
     }
     for (int i = 0; i < kBwdSlots; ++i) {
-      tc::mbar_init(&d1_full[i], 1);
-      tc::mbar_init(&h_ready[i], kWarps);
-      tc::mbar_init(&d2_full[i], 1);
+      tc::mbar_init(&d2_full[i], kWarps);
       tc::mbar_init(&dout_ready[i], kWarps);
-      tc::mbar_init(&d3_full[i], 1);
-      tc::mbar_init(&dpre_ready[i], kWarps);
-      tc::mbar_init(&d4_full[i], 1);
+      tc::mbar_init(&d4_full[i], kWarps);
       tc::mbar_init(&slot_free[i], kWarps);
     }
     tc::mbar_init(&wbar[0], 1);
     tc::mbar_init(&wbar[1], 1);
     tc::fence_mbar_init();
   }
-  if (tid < 32) tc::tmem_alloc(tmem_ptr, 512);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(kFull, *tmem_ptr, 0);
   if (tid == 0) {
     tc::mbar_expect_tx(&wbar[0], kWiBytes);
     tc::tma_bulk_g2s(base, wimg, kWiBytes, &wbar[0]);
@@ -255,7 +261,6 @@ render_backward_pipe(const nfi_render_params p, const nfi_render_grads g,
   tc::mbar_wait(&wbar[0], 0);
   tc::mbar_wait(&wbar[1], 0);
 
-  const uint32_t base_s = tc::smem_u32(base);
   const int tiles_x = (p.width + kTileW - 1) / kTileW;
   const int tiles_y = (p.height + kTileH - 1) / kTileH;
   const int n_tiles = tiles_x * tiles_y * p.batch;
@@ -265,14 +270,11 @@ render_backward_pipe(const nfi_render_params p, const nfi_render_grads g,
   const int R = p.plane_res;
   const float inv_range = 1.f / p.scene_range;
   const uint32_t plane_bytes = (uint32_t)R * (uint32_t)R * 128u;
-  const uint32_t lane_addr = (uint32_t)(32 * wig) << 16;
 
   if (wg >= 3) {
     // ================================ PRODUCER / SCATTER ================================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(Cfg::kProducerRegs));
     const int set = wg - 3;
-    float* Dw = reinterpret_cast<float*>(base + Cfg::kSmStage + (set * 4 + wig) * Cfg::kStageWarp);
-    float* Gw = Dw + 32 * 36;
+    float* Gw = reinterpret_cast<float*>(base + Cfg::kSmStage + (set * 4 + wig) * Cfg::kStageWarp);
     const int q = lane >> 3, kq = lane & 7;
     const uint32_t row_units = (uint32_t)R * 8u;
     uint32_t n0 = 0;  // ring position of the tile's first step
@@ -335,36 +337,14 @@ render_backward_pipe(const nfi_render_params p, const nfi_render_grads g,
         // ---- scatter step i: D4 -> plane gradient (and camera gradient)
         const uint32_t m = n0 + (uint32_t)i;
         const uint32_t sl = m % kBwdSlots, v = m / kBwdSlots;
-        const uint32_t d4 = tmem_base + sl * kBwdSlotCols + lane_addr;
+        // this warp's 32 rows of the D4 slot, read in place (released after the scatter)
+        const float* Dw = d4s + sl * (kThreads * kD4Ld) + 32 * wig * kD4Ld;
         NFI_STEP_WAIT(&d4_full[sl], v & 1);
-        tc::tc_fence_after();
-        {
-          uint32_t ra[16], rb[16];
-          tc::tmem_ld16_nowait(d4, ra);
-          tc::tmem_ld16_nowait(d4 + 16, rb);
-          tc::tmem_wait_ld();
-          tc::tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&slot_free[sl]);
-          if ((p.mlp_mode & 0x4000) && p.normals != nullptr && ray == (size_t)p.noise_seed && valid) {
-            float* d32 = p.normals + (size_t)n_total * 8 + (size_t)i * 32;   // debug trace
+        if ((p.mlp_mode & 0x4000) && p.normals != nullptr && ray == (size_t)p.noise_seed && valid) {
+          float* d32 = p.normals + (size_t)n_total * 8 + (size_t)i * 32;   // debug trace
 #pragma unroll
-            for (int k = 0; k < 16; ++k) {
-              d32[k] = __uint_as_float(ra[k]);
-              d32[16 + k] = __uint_as_float(rb[k]);
-            }
-          }
-#pragma unroll
-          for (int c4 = 0; c4 < 4; ++c4) {
-            *reinterpret_cast<float4*>(Dw + lane * 36 + 4 * c4) =
-                make_float4(__uint_as_float(ra[4 * c4]), __uint_as_float(ra[4 * c4 + 1]),
-                            __uint_as_float(ra[4 * c4 + 2]), __uint_as_float(ra[4 * c4 + 3]));
-            *reinterpret_cast<float4*>(Dw + lane * 36 + 16 + 4 * c4) =
-                make_float4(__uint_as_float(rb[4 * c4]), __uint_as_float(rb[4 * c4 + 1]),
-                            __uint_as_float(rb[4 * c4 + 2]), __uint_as_float(rb[4 * c4 + 3]));
-          }
+          for (int k = 0; k < 32; ++k) d32[k] = Dw[lane * kD4Ld + k];
         }
-        __syncwarp();
         const ByteTaps& tp = cur;
 #ifdef NFI_BWD_NO_SCATTER   // timing experiment: D4 is read and dropped
 #pragma unroll 1
@@ -375,7 +355,7 @@ render_backward_pipe(const nfi_render_params p, const nfi_render_grads g,
 #endif
           const int src = 4 * gq + q;
           const uint32_t in6 = CAM ? __shfl_sync(kFull, cur_in, src) : 0u;
-          const float4 d4v = *reinterpret_cast<const float4*>(Dw + src * 36 + 4 * kq);
+          const float4 d4v = *reinterpret_cast<const float4*>(Dw + src * kD4Ld + 4 * kq);
           float gc0 = 0.f, gc1 = 0.f, gc2 = 0.f;
           // nw texel clamped to R-2: all four taps of a plane exist at fixed offsets
           const uint32_t dx = 8u;
@@ -460,6 +440,7 @@ render_backward_pipe(const nfi_render_params p, const nfi_render_grads g,
           }
         }
         __syncwarp();
+        if (lane == 0) mbar_arrive(&slot_free[sl]);
         if (CAM) {
           // D4 carries the 1/3 of the plane mean already
           const float dpx = Gw[lane * 4 + 0] * inv_range, dpy = Gw[lane * 4 + 1] * inv_range,
@@ -482,125 +463,78 @@ render_backward_pipe(const nfi_render_params p, const nfi_render_grads g,
         atomicAdd(g.grad_dirs + ray * 3 + 2, gdz);
       }
     }
-  } else if (wg == 2) {
-    // ================================ MMA ISSUERS ================================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::kAuxRegs));
-    if (wig == 0) {
-      const uint64_t dsc_w1_hi = tc::umma_desc_sw128(base_s + kWiW1Hi);
-      const uint64_t dsc_w1_lo = tc::umma_desc_sw128(base_s + kWiW1Lo);
-      const uint64_t dsc_a0 = tc::umma_desc_sw128(base_s + Cfg::kSmA);
-      uint32_t st = 0, u = 0, sl = 0, v = 0;
-      for (uint32_t m = 0; m < total_steps; ++m) {
-        NFI_STEP_WAIT(&full[st], u & 1);
-        NFI_STEP_WAIT(&slot_free[sl], (v & 1) ^ 1);
-        if (elect_one()) {
-          tc::tc_fence_after();
-          const uint64_t dsc_a = dsc_a0 + (uint64_t)st * (kPipeStageBytes >> 4);
-          tc::issue_layer1_d(tmem_base + sl * kBwdSlotCols, dsc_a, dsc_a + (16384 >> 4),
-                             dsc_w1_hi, dsc_w1_lo);
-          tc::umma_commit(&d1_full[sl]);
-          tc::umma_commit(&a_free[st]);
-        }
-        __syncwarp();
-        if (++st == NS) { st = 0; ++u; }
-        if (++sl == kBwdSlots) { sl = 0; ++v; }
-      }
-    } else if (wig == 1) {
-      const uint64_t dsc_w2_hi = tc::umma_desc_sw128(base_s + kWiW2Hi);
-      const uint64_t dsc_w2_lo = tc::umma_desc_sw128(base_s + kWiW2Lo);
-      uint32_t sl = 0, v = 0;
-      for (uint32_t m = 0; m < total_steps; ++m) {
-        NFI_STEP_WAIT(&h_ready[sl], v & 1);
-        if (elect_one()) {
-          tc::tc_fence_after();
-          const uint32_t d = tmem_base + sl * kBwdSlotCols;
-          issue_layer2_tt(d + 128, d, d + 64, dsc_w2_hi, dsc_w2_lo);
-          tc::umma_commit(&d2_full[sl]);
-        }
-        __syncwarp();
-        if (++sl == kBwdSlots) { sl = 0; ++v; }
-      }
-    } else if (wig == 2) {
-      const uint64_t b_hi = tc::umma_desc_sw128(base_s + Cfg::kSmWb + kWbW2tHi);
-      const uint64_t b_lo = tc::umma_desc_sw128(base_s + Cfg::kSmWb + kWbW2tLo);
-      uint32_t sl = 0, v = 0;
-      for (uint32_t m = 0; m < total_steps; ++m) {
-        NFI_STEP_WAIT(&dout_ready[sl], v & 1);
-        if (elect_one()) {
-          tc::tc_fence_after();
-          const uint32_t d = tmem_base + sl * kBwdSlotCols;
-          issue_mma3(d + 176, d + 144, d + 160, b_hi, b_lo);
-          tc::umma_commit(&d3_full[sl]);
-        }
-        __syncwarp();
-        if (++sl == kBwdSlots) { sl = 0; ++v; }
-      }
-    } else {
-      const uint64_t b_hi = tc::umma_desc_sw128(base_s + Cfg::kSmWb + kWbW1tHi);
-      const uint64_t b_lo = tc::umma_desc_sw128(base_s + Cfg::kSmWb + kWbW1tLo);
-      uint32_t sl = 0, v = 0;
-      for (uint32_t m = 0; m < total_steps; ++m) {
-        NFI_STEP_WAIT(&dpre_ready[sl], v & 1);
-        if (elect_one()) {
-          tc::tc_fence_after();
-          const uint32_t d = tmem_base + sl * kBwdSlotCols;
-          issue_mma4(d, d + 64, d + 176, b_hi, b_lo);
-          tc::umma_commit(&d4_full[sl]);
-        }
-        __syncwarp();
-        if (++sl == kBwdSlots) { sl = 0; ++v; }
-      }
-    }
   } else if (wg == 0) {
-    // ================================ ACTIVATION (forward and reverse) ================================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::kActRegs));
+    // ================================ ACTIVATION: the four GEMMs ================================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(Cfg::kActRegs));
+    const uint32_t base_s = tc::smem_u32(base);
+    const uint64_t w1_hi = tc::gmma_desc_sw128(base_s + kWiW1Hi);
+    const uint64_t w1_lo = tc::gmma_desc_sw128(base_s + kWiW1Lo);
+    const uint64_t w2_hi = tc::gmma_desc_sw128(base_s + kWiW2Hi);
+    const uint64_t w2_lo = tc::gmma_desc_sw128(base_s + kWiW2Lo);
+    const uint64_t b3_hi = tc::gmma_desc_sw128(base_s + Cfg::kSmWb + kWbW2tHi);
+    const uint64_t b3_lo = tc::gmma_desc_sw128(base_s + Cfg::kSmWb + kWbW2tLo);
+    const uint64_t b4_hi = tc::gmma_desc_sw128(base_s + Cfg::kSmWb + kWbW1tHi);
+    const uint64_t b4_lo = tc::gmma_desc_sw128(base_s + Cfg::kSmWb + kWbW1tLo);
+    const uint64_t dsc_a0 = tc::gmma_desc_sw128(base_s + Cfg::kSmA);
+    const int t = lane & 3;
+    // D1 -> softplus -> D2 into the slot
     auto act_fwd = [&](uint32_t m) {
-      const uint32_t sl = m % kBwdSlots, v = m / kBwdSlots;
-      const uint32_t d1 = tmem_base + sl * kBwdSlotCols + lane_addr;
-      NFI_STEP_WAIT(&d1_full[sl], v & 1);
-      tc::tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        float lo[16], hi[16];
-        tc::tmem_ld16(d1 + 16 * c, lo);
-        softplus_split16(lo, hi, b1s + 16 * c);
-        tc::tmem_st16(d1 + 16 * c, lo);
-        tc::tmem_st16(d1 + 64 + 16 * c, hi);
-      }
-      tc::tmem_wait_st();
-      tc::tc_fence_before();
+      const uint32_t st = m % NS, u = m / NS, sl = m % kBwdSlots;
+      NFI_STEP_WAIT(&full[st], u & 1);
+      decoder_step(dsc_a0 + (uint64_t)st * (kPipeStageBytes >> 4), w1_hi, w1_lo, w2_hi, w2_lo, b1s,
+                   d2s + sl * (kThreads * kD2Ld), wig, lane, []() {});
       __syncwarp();
-      if (lane == 0) mbar_arrive(&h_ready[sl]);
+      if (lane == 0) mbar_arrive(&d2_full[sl]);
     };
-    // dpre = dH * sigmoid(pre),  sigmoid(pre) = 1 - exp(-softplus(pre)) = 1 - 2^(-H log2 e)
+    // D1 again, D3 = dOut W2, dpre = D3 * sigmoid(pre), D4 = dpre (W1 / 3) into the slot
+    //   sigmoid(pre) = 1 - exp(-softplus(pre)) = 1 - 2^(-H log2 e)
     auto act_bwd = [&](uint32_t m) {
-      const uint32_t sl = m % kBwdSlots, v = m / kBwdSlots;
-      const uint32_t d = tmem_base + sl * kBwdSlotCols + lane_addr;
-      NFI_STEP_WAIT(&d3_full[sl], v & 1);
-      tc::tc_fence_after();
+      const uint32_t st = m % NS, sl = m % kBwdSlots, v = m / kBwdSlots;
+      const uint64_t dsc_a = dsc_a0 + (uint64_t)st * (kPipeStageBytes >> 4);
+      const float* dout = d2s + sl * (kThreads * kD2Ld);
+      float* d4 = d4s + sl * (kThreads * kD4Ld);
+      NFI_STEP_WAIT(&dout_ready[sl], v & 1);
+      NFI_STEP_WAIT(&slot_free[sl], (v & 1) ^ 1);  // D4 of step m - 2 scattered
 #pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        uint32_t r3[16], rh[16], rl[16];
-        tc::tmem_ld16_nowait(d + 176 + 16 * c, r3);
-        tc::tmem_ld16_nowait(d + 64 + 16 * c, rh);
-        tc::tmem_ld16_nowait(d + 16 * c, rl);
-        tc::tmem_wait_ld();
-        float lo[16], hi[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const float h = __uint_as_float(rh[i]) + __uint_as_float(rl[i]);
-          const float sg = 1.f - tc::ex2_approx(-h * kLog2e);
-          const float dp = __uint_as_float(r3[i]) * sg;
-          hi[i] = tc::tf32_hi(dp);
-          lo[i] = dp - hi[i];
+      for (int mb = 0; mb < 2; ++mb) {
+        float d[32], d3[32];
+        zero(d);
+        zero(d3);
+        uint32_t ohi[2][4], olo[2][4];
+        load_dout_frags(dout + 64 * mb * kD2Ld, wig, lane, ohi, olo);
+        tc::wgmma_fence();
+        tc::layer1_mb(d, dsc_a + mb * (8192 >> 4), dsc_a + ((16384 + mb * 8192) >> 4), w1_hi, w1_lo);
+        mma3_mb(d3, ohi, olo, b3_hi, b3_lo);
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::reg_fence(d);
+        tc::reg_fence(d3);
+        if (mb == 1) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&a_free[st]);
         }
-        tc::tmem_st16(d + 176 + 16 * c, lo);  // dpre_lo over D3
-        tc::tmem_st16(d + 64 + 16 * c, hi);   // dpre_hi over H_hi
+        uint32_t phi[8][4], plo[8][4];
+#pragma unroll
+        for (int kb = 0; kb < 8; ++kb) {
+          const float2 bb = *reinterpret_cast<const float2*>(b1s + 8 * kb + 2 * t);
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const float h = tc::softplus_mufu<true>(d[4 * kb + e] + ((e & 1) ? bb.y : bb.x));
+            const float sg = 1.f - tc::ex2_approx(-h * kLog2e);
+            tc::put_split(phi, plo, kb, tc::afrag_slot(e), d3[4 * kb + e] * sg);
+          }
+        }
+        float d4v[16];
+        zero(d4v);
+        tc::wgmma_fence();
+        mma4_mb(d4v, phi, plo, b4_hi, b4_lo);
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::reg_fence(d4v);
+        tc::store_frag_rows(d4v, d4 + 64 * mb * kD4Ld, kD4Ld, wig, lane);
       }
-      tc::tmem_wait_st();
-      tc::tc_fence_before();
       __syncwarp();
-      if (lane == 0) mbar_arrive(&dpre_ready[sl]);
+      if (lane == 0) mbar_arrive(&d4_full[sl]);
     };
     if (total_steps > 0) act_fwd(0);
     for (uint32_t m = 0; m < total_steps; ++m) {
@@ -609,7 +543,7 @@ render_backward_pipe(const nfi_render_params p, const nfi_render_grads g,
     }
   } else {
     // ================================ SHADING (forward and reverse) ================================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(Cfg::kShadeRegs));
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::kShadeRegs));
     FieldConst fc;
     fc.A = p.n_attention;
     fc.use_sdf = p.use_sdf;
@@ -675,15 +609,15 @@ render_backward_pipe(const nfi_render_params p, const nfi_render_grads g,
         const float zn = has_next ? mw.pop() : z;
         const float delta = has_next ? (zn - z) * r.dn : 0.f;
         const uint32_t sl = m % kBwdSlots, v = m / kBwdSlots;
-        const uint32_t d = tmem_base + sl * kBwdSlotCols + lane_addr;
+        float* const row = d2s + sl * (kThreads * kD2Ld) + gt * kD2Ld;  // D2 in, dOut out
         // ---- forward at this sample
         const float wx = r.ox + r.dx * z, wy = r.oy + r.dy * z, wz = r.oz + r.dz * z;
         const float x0 = wx * inv_range, x1 = wy * inv_range, x2 = wz * inv_range;
         const float keep = (fabsf(x0) > 1.f || fabsf(x1) > 1.f || fabsf(x2) > 1.f) ? 0.f : 1.f;
         NFI_STEP_WAIT(&d2_full[sl], v & 1);
-        tc::tc_fence_after();
         float o16[16];
-        tc::tmem_ld16(d + 128, o16);
+#pragma unroll
+        for (int o = 0; o < 16; ++o) o16[o] = row[o];
         float out[NOUT_PAD];
 #pragma unroll
         for (int o = 0; o < NOUT_PAD; ++o) out[o] = o16[o] + b2s[o];
@@ -697,7 +631,7 @@ render_backward_pipe(const nfi_render_params p, const nfi_render_grads g,
           // d cdf / d(-d) = e / (2 beta), also AT the zero crossing: autograd of the reference's
           // 0.5 + 0.5 sign(x)(1 - exp(-|x|/beta)) returns 0 for x == 0.0 exactly (sign(0) = 0),
           // which fp32 does produce (out[0] = D2 + b2 cancels to 0.0 on a few samples per
-          // million: profiles/r2_grad_trace_exact_zero_sdf.txt); the analytic limit is used
+          // million); the analytic limit is used
           dsig_dout0 = -(fc.inv_alpha * keep) * 0.5f * e_sdf * fc.inv_beta;
         } else {
           const float x = out[0] - 1.f;
@@ -780,21 +714,13 @@ render_backward_pipe(const nfi_render_params p, const nfi_render_grads g,
           q8[0] = z; q8[1] = sigma; q8[2] = w; q8[3] = T; q8[4] = dsig; q8[5] = dOut[0];
           q8[6] = s_i; q8[7] = delta;
         }
-        // ---- hand dOut to the tensor core (hi/lo split)
-        {
-          float hi[16], lo[16];
+        // ---- hand dOut to the tensor core (split into TF32 hi/lo by the activation group)
 #pragma unroll
-          for (int o = 0; o < 16; ++o) {
-            hi[o] = tc::tf32_hi(dOut[o]);
-            lo[o] = dOut[o] - hi[o];
-          }
-          tc::tmem_st16(d + 144, hi);
-          tc::tmem_st16(d + 160, lo);
-          tc::tmem_wait_st();
-          tc::tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&dout_ready[sl]);
-        }
+        for (int o4 = 0; o4 < 4; ++o4)
+          *reinterpret_cast<float4*>(row + 4 * o4) =
+              make_float4(dOut[4 * o4], dOut[4 * o4 + 1], dOut[4 * o4 + 2], dOut[4 * o4 + 3]);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&dout_ready[sl]);
         if (EXTRA == 1) {  // coords output: d(w x)/dx = w
           const float dpx = w * ge0, dpy = w * ge1, dpz = w * ge2;
           gox += dpx; goy += dpy; goz += dpz;
@@ -833,9 +759,6 @@ render_backward_pipe(const nfi_render_params p, const nfi_render_grads g,
       }
     }
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (tid < 32) tc::tmem_dealloc(tmem_base, 512);
 }
 
 }  // namespace nfi

@@ -1,4 +1,4 @@
-// Shared device helpers for the fused tri-plane renderer (sm_100a).
+// Shared device helpers for the fused tri-plane renderer (sm_90a).
 //
 // Everything here mirrors, stage by stage, the reference's per-ray render
 // (citations into /root/reference).  The file is compiled with --fmad=false so

@@ -1,41 +1,33 @@
 // Forward render kernel, pipelined tensor-core variant (NFI_MLP_TC_PIPE, the default).
 //
-// Same arithmetic as nfi_forward_tc.cuh (3xTF32 decoder on tcgen05, thread = ray
+// Same arithmetic as nfi_forward_tc.cuh (3xTF32 decoder on wgmma, thread = ray
 // for everything per-ray), but the per-step chain
 //     gather -> MMA1 -> softplus/split -> MMA2 -> density/colour/composite
 // is cut so that NO resource is held across more than one link of it, and every
 // role only ever does its own kind of work:
 //
 //   persistent CTA (one per SM), one 16x8-pixel tile (128 rays) in flight:
-//     warpgroup 0   ACTIVATION  thread = TMEM lane: D1 -> softplus -> H_hi / H_lo (stateless,
-//                   throughput-bound: FMA pipe + one MUFU per hidden unit)
-//     warpgroup 1   SHADING     thread = ray = TMEM lane: D2 -> density / colour -> coarse
+//     warpgroup 0   ACTIVATION  issues both decoder layers (wgmma, accumulators in its
+//                   registers, one 64-row half of the tile after the other): D1 -> softplus ->
+//                   H_hi / H_lo register A fragments -> D2 -> D2 slot in shared memory
+//     warpgroup 1   SHADING     thread = ray: D2 -> density / colour -> coarse
 //                   weights or sorted merge + compositing (latency-bound chains);
 //                   the two groups put two independent instruction streams on
 //                   every SM sub-partition
-//     warpgroup 2   warp 8 issues every layer-1 tcgen05.mma, warp 9 every layer-2
-//                   tcgen05.mma (the ~25-50 cycles an MMA takes to issue are
-//                   nobody else's problem); warps 10-11 idle
-//     warpgroups 3+ P PRODUCER sets of 4 warps; set q gathers the steps n = q (mod P)
+//     warpgroups 2+ P PRODUCER sets of 4 warps; set q gathers the steps n = q (mod P)
 //                   into A stage n mod (P+1) (A_hi/A_lo, 32 KB, SWIZZLE_128B)
 //
-//   stage   : producers --full[q]--> MMA1 --a_free[q] (tcgen05.commit)--> producers
-//             (a stage is released as soon as the tensor core has READ it; the
+//   stage   : producers --full[q]--> activation --a_free[q]--> producers
+//             (a stage is released as soon as layer 1 has READ it; the
 //             hidden activations never come back to shared memory)
-//   TMEM    : three slots of 160 columns: [0,64) D1 then H_lo, [64,128) H_hi,
-//             [128,144) D2;  MMA1 --d1_full--> activation --h_ready--> MMA2
-//             --d2_full--> shading --slot_free--> MMA1
+//   D2 slot : three [128 x 20] fp32 slots: activation --d2_full--> shading --slot_free-->
+//             activation
 //   softplus: ln2 * (max(x', 0) + lg2(1 + 2^-|x'|)) with x' = x log2 e: two MUFU ops (ex2, lg2)
-//             per hidden unit, 8 unit pairs side by side; log2(e) is folded into W1/b1 by
-//             prep_weight_image (a degree-8 FMA-pipe log1p instead of lg2 was measured slower:
-//             DESIGN.md section 5);
+//             per hidden unit; log2(e) is folded into W1/b1 by prep_weight_image;
 //   resample: the S uniforms of a ray are sorted by a bitonic network across the
 //             warp (2 per lane) and pushed through the inverse CDF with shuffle
 //             binary searches: one warp-pass per ray instead of a serial per-thread
 //             walk (run.py:259-281, lib/nerf_utils.py:183-222).
-// What bounds the kernel after this: the L1 data pipe (12 texel lines of 128 bytes per point plus
-// the A-tile stores) at 65 %, issue slots at 55 %, and a consumer chain that alone needs two
-// thirds of a step (DESIGN.md section 5).
 #pragma once
 #include <type_traits>
 
@@ -110,20 +102,10 @@ __device__ __forceinline__ TileCoord tile_coord(int tile, int tiles_x, int tiles
 }
 
 constexpr int kPipeSlots = 3;
-constexpr int kPipeSlotCols = 160;  // [0,64) D1 then H_lo, [64,128) H_hi, [128,144) D2
 constexpr int kPipeStageBytes = 32768;
-// NFI_L1_BF16: layer 1 of the forward kernel on bf16 hi/lo pairs (operands exact to 2^-17
-// instead of 3xTF32's 2^-22, as nfi_wgrad_pipe.cuh and the synthesis convolutions): the A stage
-// shrinks from 32 KB to 16 KB (two [128][32 bf16] SWIZZLE_64B tiles: half the stores of the
-// gather, 64 KB of shared memory back to the L1), six K16 MMAs instead of twelve K8.
-// Measured (profiles/r2_ab_forward_bf16_l1.txt): 8.52 vs 8.69 ms, 1.9 % -- and the importance-
-// resampled depths move from <= 2e-5 to > 2e-5 of the oracle's (the coarse densities feed an
-// inverse CDF), which costs the gradient tests their margin.  Not worth it: off by default; the
-// weight-gradient kernel, which resamples nothing, uses the bf16 form (nfi_wgrad_pipe.cuh).
-#ifndef NFI_L1_BF16
-#define NFI_L1_BF16 0
-#endif
-constexpr int kFwdStageBytes = NFI_L1_BF16 ? 16384 : 32768;
+constexpr int kFwdStageBytes = 32768;
+constexpr int kD2Ld = 20;  // floats per row of a D2 slot (80-byte rows: row reads are conflict-free)
+constexpr int kD2SlotBytes = kThreads * kD2Ld * 4;
 
 // scratch per CTA: the tc_scratch layout plus NES parked extras per coarse sample
 __host__ __device__ inline size_t pipe_scratch_floats(int S, int nes) {
@@ -132,32 +114,23 @@ __host__ __device__ inline size_t pipe_scratch_floats(int S, int nes) {
 
 template <int P>
 struct PipeCfg {
-  static constexpr int kThreadsTotal = 384 + 128 * P;
+  static constexpr int kThreadsTotal = 256 + 128 * P;
   static constexpr int kStages = P + 1;  // one spare: a set never waits for its own MMA
   static constexpr int kSmA = 25600;
-  static constexpr int kSmPal = kSmA + kStages * kFwdStageBytes;
+  static constexpr int kSmD2 = kSmA + kStages * kFwdStageBytes;
+  static constexpr int kSmPal = kSmD2 + kPipeSlots * kD2SlotBytes;
   static constexpr int kSmFrac = kSmPal + 48 * 4;  // s / S for s < 128 (one IEEE division each)
   static constexpr int kSmBars = kSmFrac + 128 * 4;
-  // full[P], a_free[P], d1_full[3], h_ready[3], d2_full[3], slot_free[3], cw_ready, zf_ready,
-  // weights
-  static constexpr int kNumBars = 2 * kStages + 4 * kPipeSlots + 3;
-  static constexpr int kSmTmemPtr = kSmBars + kNumBars * 8;
-  static constexpr int kSmBytes = kSmTmemPtr + 16;
+  // full[P+1], a_free[P+1], d2_full[3], slot_free[3], cw_ready, zf_ready, weights
+  static constexpr int kNumBars = 2 * kStages + 2 * kPipeSlots + 3;
+  static constexpr int kSmBytes = kSmBars + kNumBars * 8;
   // setmaxnreg moves registers inside the CTA's launch allocation (threads x launch regs):
-  //   P = 3: 768 x 80 = 61440 = 128 x (88 + 80 + 24) + 384 x 96 (12 texel loads in flight per
-  //   producer warp: 48 data registers + 64-bit addresses + taps).  A 256-bit variant
-  //   (ld.global.nc.v8.f32, 4 lanes per texel, 8 points per iteration: 23 instead of 37
-  //   instructions per point) assembles for sm_100a but traps as an illegal instruction
-  //   on the B200, so 128-bit loads it is.
-#ifndef NFI_ACT_REGS
-#define NFI_ACT_REGS 88
-#define NFI_SHADE_REGS 80
-#define NFI_PROD_REGS 96
-#endif
-  static constexpr int kActRegs = NFI_ACT_REGS;
-  static constexpr int kShadeRegs = NFI_SHADE_REGS;
-  static constexpr int kAuxRegs = 24;
-  static constexpr int kProducerRegs = NFI_PROD_REGS;
+  //   P = 3: 640 x 96 = 61440 = 128 x (136 + 80) + 384 x 88 (12 texel loads in flight per
+  //   producer warp: 48 data registers + 64-bit addresses + taps; the activation group holds a
+  //   64 x 64 accumulator block and its hi / lo split).
+  static constexpr int kActRegs = 136;
+  static constexpr int kShadeRegs = 80;
+  static constexpr int kProducerRegs = 88;
 };
 
 // this kernel's weight image has log2(e) folded into layer 1 (the softplus works
@@ -166,63 +139,44 @@ constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kLn2 = 0.6931471805599453f;
 constexpr float kPadLogit = -1e30f;
 
-// D2 = H_lo*W2_hi + H_hi*W2_lo + H_hi*W2_hi, both halves of H read from TMEM.
-__device__ __forceinline__ void issue_layer2_tt(uint32_t d2_tmem, uint32_t hlo_tmem,
-                                                uint32_t hhi_tmem, uint64_t w2_hi,
-                                                uint64_t w2_lo) {
-  constexpr uint32_t idesc = tc::umma_idesc_tf32(128, 16);
-  tc::umma_ts<false>(d2_tmem, hlo_tmem, w2_hi, idesc);
+// The decoder of one 128-point step, issued by the whole (activation) warpgroup: per 64-row
+// half, layer 1 from the A stage (3xTF32, 12 wgmma), softplus on the accumulator registers,
+// layer 2 with H as register A fragments (24 wgmma).  `on_stage_read` runs once layer 1 of both
+// halves has completed (the stage may be refilled); D2 goes to `d2` ([128][kD2Ld]).
+template <typename F>
+__device__ __forceinline__ void decoder_step(uint64_t dsc_a, uint64_t w1_hi, uint64_t w1_lo,
+                                             uint64_t w2_hi, uint64_t w2_lo,
+                                             const float* __restrict__ b1, float* d2, int warp,
+                                             int lane, F&& on_stage_read) {
+#pragma unroll 1
+  for (int mb = 0; mb < 2; ++mb) {
+    float d[32];
 #pragma unroll
-  for (int ks = 1; ks < 8; ++ks)
-    tc::umma_ts<true>(d2_tmem, hlo_tmem + 8 * ks, w2_hi + (ks >> 2) * 128 + (ks & 3) * 2, idesc);
+    for (int i = 0; i < 32; ++i) d[i] = 0.f;
+    tc::wgmma_fence();
+    tc::layer1_mb(d, dsc_a + mb * (8192 >> 4), dsc_a + ((16384 + mb * 8192) >> 4), w1_hi, w1_lo);
+    tc::wgmma_commit();
+    tc::wgmma_wait<0>();
+    tc::reg_fence(d);
+    if (mb == 1) on_stage_read();
+    uint32_t hi[8][4], lo[8][4];
+    tc::softplus_frag<true>(d, b1, lane & 3, hi, lo);
+    float o[8];
 #pragma unroll
-  for (int ks = 0; ks < 8; ++ks)
-    tc::umma_ts<true>(d2_tmem, hhi_tmem + 8 * ks, w2_lo + (ks >> 2) * 128 + (ks & 3) * 2, idesc);
-#pragma unroll
-  for (int ks = 0; ks < 8; ++ks)
-    tc::umma_ts<true>(d2_tmem, hhi_tmem + 8 * ks, w2_hi + (ks >> 2) * 128 + (ks & 3) * 2, idesc);
+    for (int i = 0; i < 8; ++i) o[i] = 0.f;
+    tc::wgmma_fence();
+    tc::layer2_mb(o, hi, lo, w2_hi, w2_lo);
+    tc::wgmma_commit();
+    tc::wgmma_wait<0>();
+    tc::reg_fence(o);
+    tc::store_frag_rows(o, d2 + 64 * mb * kD2Ld, kD2Ld, warp, lane);
+  }
 }
 
 __device__ __forceinline__ float ldcg(const float* p) {
   float v;
   asm volatile("ld.global.cg.f32 %0, [%1];" : "=f"(v) : "l"(p));
   return v;
-}
-
-// Hidden activations of 16 TMEM columns: v = log2(e) * (W1 f) (the accumulator),
-// bias16 pre-scaled by log2(e).  Returns h split into TF32 hi (hi[]) and the
-// remainder (in place, v[]).
-//   softplus(x) = ln2 * (max(x', 0) + lg2(1 + 2^-|x'|)),  x' = x log2 e
-// 13 instructions per unit pair (2 ex2 + 2 lg2 on the MUFU pipe, which the
-// gather does not use); the 8 pairs advance side by side through every stage.
-__device__ __forceinline__ void softplus_split16(float (&v)[16], float (&hi)[16],
-                                                 const float* __restrict__ bias16) {
-  float2 x[8], l[8];
-#pragma unroll
-  for (int i4 = 0; i4 < 4; ++i4) {
-    const float4 bb = *reinterpret_cast<const float4*>(bias16 + 4 * i4);
-    x[2 * i4] = __fadd2_rn(make_float2(v[4 * i4], v[4 * i4 + 1]), make_float2(bb.x, bb.y));
-    x[2 * i4 + 1] = __fadd2_rn(make_float2(v[4 * i4 + 2], v[4 * i4 + 3]), make_float2(bb.z, bb.w));
-  }
-#pragma unroll
-  for (int k = 0; k < 8; ++k)
-    l[k] = make_float2(tc::ex2_approx(-fabsf(x[k].x)), tc::ex2_approx(-fabsf(x[k].y)));
-#pragma unroll
-  for (int k = 0; k < 8; ++k) l[k] = __fadd2_rn(l[k], make_float2(1.f, 1.f));
-#pragma unroll
-  for (int k = 0; k < 8; ++k) l[k] = make_float2(tc::lg2_approx(l[k].x), tc::lg2_approx(l[k].y));
-#pragma unroll
-  for (int k = 0; k < 8; ++k)
-    l[k] = __fadd2_rn(l[k], make_float2(fmaxf(x[k].x, 0.f), fmaxf(x[k].y, 0.f)));
-#pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    const float2 h = __fmul2_rn(l[k], make_float2(kLn2, kLn2));
-    hi[2 * k] = tc::tf32_hi(h.x);
-    hi[2 * k + 1] = tc::tf32_hi(h.y);
-    const float2 lo2 = __fadd2_rn(h, make_float2(-hi[2 * k], -hi[2 * k + 1]));
-    v[2 * k] = lo2.x;
-    v[2 * k + 1] = lo2.y;
-  }
 }
 
 // Density and colour from the decoder outputs, branch-free over the palette
@@ -494,28 +448,26 @@ render_forward_pipe(const nfi_render_params p, const unsigned char* __restrict__
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   unsigned char* base = smem_raw;
   const int tid = threadIdx.x, lane = tid & 31;
-  // Role by warpgroup.  The arbiter favours high warp ids, so the two consumer roles --
-  // one warp each per sub-partition, nothing to hide their latency behind -- sit above the
-  // producers: hardware wg 0..P-1 producer sets, P MMA issuers, P+1 shading, P+2 activation.
-  // `wg` below is the logical role: 0 activation, 1 shading, 2 MMA issuers, 3.. producer sets.
+  // Role by warpgroup.  The two consumer roles -- one warp each per sub-partition, nothing to
+  // hide their latency behind -- sit above the producers: hardware wg 0..P-1 producer sets, P
+  // shading, P+1 activation.  `wg` below is the logical role: 0 activation, 1 shading, 3..
+  // producer sets (2 is unused).
   const int hw_wg = __shfl_sync(kFull, tid >> 7, 0);
-  const int wg = (hw_wg < P) ? hw_wg + 3 : (P + 2 - hw_wg);
-  const int gt = tid & 127;                        // row of the tile = ray = TMEM lane
-  const int wig = __shfl_sync(kFull, gt >> 5, 0);  // warp in warpgroup = TMEM lane quadrant
+  const int wg = (hw_wg < P) ? hw_wg + 3 : (P + 1 - hw_wg);
+  const int gt = tid & 127;                        // row of the tile = ray
+  const int wig = __shfl_sync(kFull, gt >> 5, 0);  // warp in warpgroup
   const int S = p.num_samples;
 
   uint64_t* bars = reinterpret_cast<uint64_t*>(base + Cfg::kSmBars);
   constexpr int NS = Cfg::kStages;
   uint64_t* full = bars;                         // [NS] stage gathered            (4 warps)
-  uint64_t* a_free = full + NS;                  // [NS] stage read by the tensor core (commit)
-  uint64_t* d1_full = a_free + NS;               // [3]  layer-1 accumulator ready (commit)
-  uint64_t* h_ready = d1_full + kPipeSlots;      // [3]  H_hi/H_lo in TMEM         (4 warps)
-  uint64_t* d2_full = h_ready + kPipeSlots;      // [3]  layer-2 accumulator ready (commit)
+  uint64_t* a_free = full + NS;                  // [NS] stage read by layer 1     (4 warps)
+  uint64_t* d2_full = a_free + NS;               // [3]  D2 slot written           (4 warps)
   uint64_t* slot_free = d2_full + kPipeSlots;    // [3]  D2 read                   (4 warps)
   uint64_t* cw_ready = slot_free + kPipeSlots;   //      coarse weights of the tile written (4 warps)
   uint64_t* zf_ready = cw_ready + 1;             //      fine depths of the tile written (every resampling warp)
   uint64_t* wbar = zf_ready + 1;                 //      weight image landed
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(base + Cfg::kSmTmemPtr);
+  float* d2s = reinterpret_cast<float*>(base + Cfg::kSmD2);  // [3][128][kD2Ld]
   const float* b1s = reinterpret_cast<const float*>(base + kWiB1);
   const float* b2s = reinterpret_cast<const float*>(base + kWiB2);
   float* pal = reinterpret_cast<float*>(base + Cfg::kSmPal);
@@ -524,16 +476,14 @@ render_forward_pipe(const nfi_render_params p, const unsigned char* __restrict__
 
   if (tid == 0) {
     if (tc::smem_u32(base) & 1023u) __trap();
+    // barriers count WARPS: a warp-wide mbarrier.arrive is 32 serialised shared-memory atomics
+    // on one word (L1 data-pipe wavefronts the gather needs)
     for (int i = 0; i < NS; ++i) {
-      tc::mbar_init(&full[i], 4);
-      tc::mbar_init(&a_free[i], 1);
+      tc::mbar_init(&full[i], kWarps);
+      tc::mbar_init(&a_free[i], kWarps);
     }
     for (int i = 0; i < kPipeSlots; ++i) {
-      tc::mbar_init(&d1_full[i], 1);
-      // consumer barriers count WARPS: a warp-wide mbarrier.arrive is 32 serialised
-      // shared-memory atomics on one word (L1 data-pipe wavefronts the gather needs)
-      tc::mbar_init(&h_ready[i], kWarps);
-      tc::mbar_init(&d2_full[i], 1);
+      tc::mbar_init(&d2_full[i], kWarps);
       tc::mbar_init(&slot_free[i], kWarps);
     }
     tc::mbar_init(cw_ready, kWarps);
@@ -541,34 +491,13 @@ render_forward_pipe(const nfi_render_params p, const unsigned char* __restrict__
     tc::mbar_init(wbar, 1);
     tc::fence_mbar_init();
   }
-  if (tid < 32) tc::tmem_alloc(tmem_ptr, 512);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(kFull, *tmem_ptr, 0);
   if (tid == 0) {
     tc::mbar_expect_tx(wbar, kWiBytes);
     tc::tma_bulk_g2s(base, wimg, kWiBytes, wbar);
   }
   tc::mbar_wait(wbar, 0);
-#if NFI_L1_BF16
-  // layer 1's weights (x log2 e, as the image has them in TF32) as a bf16 hi / lo pair over the
-  // image's W1 region: [64 rows = hidden unit][32 k] K-major SWIZZLE_64B, 4 KB each
-  __syncthreads();
-  for (int i = tid; i < kHid * kC; i += Cfg::kThreadsTotal) {
-    const int j = i / kC, c = i % kC;
-    const float w = p.w1[i] * kLog2e;
-    const uint32_t hi = tc::bf16x2_rn(w, 0.f) & 0xFFFFu;
-    const uint32_t lo = tc::bf16x2_rn(w - __uint_as_float(hi << 16), 0.f) & 0xFFFFu;
-    const uint32_t off = tc::sw64_offset(j, c >> 3) + (c & 7) * 2;
-    *reinterpret_cast<unsigned short*>(base + kWiW1Hi + off) = (unsigned short)hi;
-    *reinterpret_cast<unsigned short*>(base + kWiW1Hi + 4096 + off) = (unsigned short)lo;
-  }
-  tc::fence_async_smem();
-  __syncthreads();
-#endif
 
-  const uint32_t base_s = tc::smem_u32(base);
   const int tiles_x = (p.width + kTileW - 1) / kTileW;
   const int tiles_y = (p.height + kTileH - 1) / kTileH;
   const int n_tiles = tiles_x * tiles_y * p.batch;
@@ -583,10 +512,9 @@ render_forward_pipe(const nfi_render_params p, const unsigned char* __restrict__
   const bool dbg_skip_consumer = (p.mlp_mode & 0x200) != 0;
   const bool dbg_window = (p.mlp_mode & 0x800) != 0;
   // phase timers (DBG instantiation, mlp_mode & 0x1000, buffer in p.normals): lane 0 of
-  // producer set 0 warp 0 -> [0..], activation warp 0 -> [16..], shading warp 0 -> [32..],
-  // issuer warps -> [48..], [64..]
+  // producer set 0 warp 0 -> [0..], activation warp 0 -> [16..], shading warp 0 -> [32..]
   const bool dbg_time = DBG && (p.mlp_mode & 0x1000) && p.normals != nullptr && blockIdx.x == 0 &&
-                        lane == 0 && (wg <= 3) && (wg == 2 ? wig < 2 : wig == 0);
+                        lane == 0 && (wg <= 3) && wg != 2 && wig == 0;
   long long tacc[DBG ? 10 : 1];
   long long tprev = 0;
   if (DBG)
@@ -610,8 +538,7 @@ render_forward_pipe(const nfi_render_params p, const unsigned char* __restrict__
   // activation and one warp of every producer set -- the producers would otherwise idle
   // between the coarse and the fine pass): a warp-pass is a chain of dependent shuffles at
   // ~0.1 IPC, so five warps per sub-partition get through the tile's 128 rays sooner than
-  // two (measured per tile: 78 k -> 46 k cycles until the fine depths are complete; kernel
-  // 8.78 -> 8.65 ms at config 2; profiles/r1_phase_times_v8_pipe.txt).
+  // two.
   constexpr int kRsParts = 2 + P;
   auto rs_first = [](int part) {  // part: 0 shading, 1 activation, 2.. producer sets
     constexpr int base_rows = 32 / kRsParts, rem = 32 % kRsParts;
@@ -636,10 +563,7 @@ render_forward_pipe(const nfi_render_params p, const unsigned char* __restrict__
   // region, and a block reachable from two branches gets the smaller count.
   if (wg >= 3) {
     // ================================ PRODUCER ================================
-    if (Cfg::kProducerRegs * Cfg::kThreadsTotal > 65536)  // above the launch allocation per thread
-      asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(Cfg::kProducerRegs));
-    else
-      asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::kProducerRegs));
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::kProducerRegs));
     const int set = wg - 3;
     uint32_t n = 0;        // ring position at the start of the pass, identical in every role
     uint32_t tile_it = 0;  // tiles done by this CTA (parity of zf_ready)
@@ -702,13 +626,8 @@ render_forward_pipe(const nfi_render_params p, const unsigned char* __restrict__
             tp.o[1] &= 0x7FFu;
             tp.o[2] &= 0x7FFu;
           }
-          if (!dbg_skip_gather) {
-#if NFI_L1_BF16
-            gather_to_tiles_lean<true>(planes_b, R, tp, stage, stage + 8192, 32 * wig, lane);
-#else
+          if (!dbg_skip_gather)
             gather_to_tiles_lean(planes_b, R, tp, stage, stage + 16384, 32 * wig, lane);
-#endif
-          }
           NFI_T(2)
           tc::fence_async_smem();
           __syncwarp();
@@ -721,117 +640,37 @@ render_forward_pipe(const nfi_render_params p, const unsigned char* __restrict__
     }
     if (DBG && dbg_time)
       for (int i = 0; i < 10; ++i) p.normals[i] = (float)tacc[i];
-  } else if (wg == 2) {
-    // ================================ MMA ISSUERS ================================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::kAuxRegs));
-    if (wig == 0) {
-      // layer 1: full[set] + slot_free[slot] -> 12 MMAs -> d1_full[slot], a_free[set]
-#if NFI_L1_BF16
-      constexpr uint32_t idesc1 = tc::umma_idesc_bf16(128, 64, false, false);
-      const uint64_t dsc_w1_hi = tc::umma_desc(base_s + kWiW1Hi, 4, 16, 512);
-      const uint64_t dsc_w1_lo = tc::umma_desc(base_s + kWiW1Hi + 4096, 4, 16, 512);
-      const uint64_t dsc_a0 = tc::umma_desc(base_s + Cfg::kSmA, 4, 16, 512);
-#else
-      const uint64_t dsc_w1_hi = tc::umma_desc_sw128(base_s + kWiW1Hi);
-      const uint64_t dsc_w1_lo = tc::umma_desc_sw128(base_s + kWiW1Lo);
-      const uint64_t dsc_a0 = tc::umma_desc_sw128(base_s + Cfg::kSmA);
-#endif
-      uint32_t st = 0, u = 0, sl = 0, v = 0;
-      for (uint32_t m = 0; m < total_steps; ++m) {
-        if (DBG && dbg_time && tprev == 0) tprev = clock64();
-        NFI_STEP_WAIT(&full[st], u & 1);
-        NFI_T(0)
-        NFI_STEP_WAIT(&slot_free[sl], (v & 1) ^ 1);
-        NFI_T(1)
-        if (elect_one()) {
-          tc::tc_fence_after();
-          const uint64_t dsc_a = dsc_a0 + (uint64_t)st * (kFwdStageBytes >> 4);
-#if NFI_L1_BF16
-          // D1 = F_lo W1_hi + F_hi W1_lo + F_hi W1_hi, K = 32 = two K16 steps of 32 bytes
-          const uint32_t d1 = tmem_base + sl * kPipeSlotCols;
-          const uint64_t a_lo = dsc_a + (8192 >> 4);
-          tc::umma_f16_ss<false>(d1, a_lo, dsc_w1_hi, idesc1);
-          tc::umma_f16_ss<true>(d1, a_lo + 2, dsc_w1_hi + 2, idesc1);
-          tc::umma_f16_ss<true>(d1, dsc_a, dsc_w1_lo, idesc1);
-          tc::umma_f16_ss<true>(d1, dsc_a + 2, dsc_w1_lo + 2, idesc1);
-          tc::umma_f16_ss<true>(d1, dsc_a, dsc_w1_hi, idesc1);
-          tc::umma_f16_ss<true>(d1, dsc_a + 2, dsc_w1_hi + 2, idesc1);
-#else
-          tc::issue_layer1_d(tmem_base + sl * kPipeSlotCols, dsc_a, dsc_a + (16384 >> 4),
-                             dsc_w1_hi, dsc_w1_lo);
-#endif
-          tc::umma_commit(&d1_full[sl]);
-          tc::umma_commit(&a_free[st]);
-        }
-        __syncwarp();
-        NFI_T(2)
-        if (++st == NS) { st = 0; ++u; }
-        if (++sl == kPipeSlots) { sl = 0; ++v; }
-      }
-      if (DBG && dbg_time)
-        for (int i = 0; i < 10; ++i) p.normals[48 + i] = (float)tacc[i];
-    } else if (wig == 1) {
-      // layer 2: h_ready[slot] -> 24 MMAs (A from TMEM) -> d2_full[slot]
-      const uint64_t dsc_w2_hi = tc::umma_desc_sw128(base_s + kWiW2Hi);
-      const uint64_t dsc_w2_lo = tc::umma_desc_sw128(base_s + kWiW2Lo);
-      uint32_t sl = 0, v = 0;
-      for (uint32_t m = 0; m < total_steps; ++m) {
-        if (DBG && dbg_time && tprev == 0) tprev = clock64();
-        NFI_STEP_WAIT(&h_ready[sl], v & 1);
-        NFI_T(0)
-        if (elect_one()) {
-          tc::tc_fence_after();
-          const uint32_t d_col = tmem_base + sl * kPipeSlotCols;
-          issue_layer2_tt(d_col + 128, d_col, d_col + 64, dsc_w2_hi, dsc_w2_lo);
-          tc::umma_commit(&d2_full[sl]);
-        }
-        __syncwarp();
-        NFI_T(1)
-        if (++sl == kPipeSlots) { sl = 0; ++v; }
-      }
-      if (DBG && dbg_time)
-        for (int i = 0; i < 10; ++i) p.normals[64 + i] = (float)tacc[i];
-    }
   } else if (wg == 0) {
     // ================================ ACTIVATION ================================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(Cfg::kActRegs));
-    uint32_t sl = 0, v = 0;
-    const uint32_t lane_addr = (uint32_t)(32 * wig) << 16;
-    // D1 of the slot -> bias + softplus -> H_lo over D1, H_hi next to it -> h_ready
+    const uint32_t base_s = tc::smem_u32(base);
+    const uint64_t dsc_w1_hi = tc::gmma_desc_sw128(base_s + kWiW1Hi);
+    const uint64_t dsc_w1_lo = tc::gmma_desc_sw128(base_s + kWiW1Lo);
+    const uint64_t dsc_w2_hi = tc::gmma_desc_sw128(base_s + kWiW2Hi);
+    const uint64_t dsc_w2_lo = tc::gmma_desc_sw128(base_s + kWiW2Lo);
+    const uint64_t dsc_a0 = tc::gmma_desc_sw128(base_s + Cfg::kSmA);
+    uint32_t st = 0, u = 0, sl = 0, v = 0;
+    // the next ring position: stage + D2 slot -> decoder -> d2_full, a_free
     auto activate = [&]() {
-      const uint32_t d1 = tmem_base + sl * kPipeSlotCols + lane_addr;
       if (DBG && dbg_time && tprev == 0) tprev = clock64();
       NFI_T(2)
-      NFI_STEP_WAIT(&d1_full[sl], v & 1);
-      tc::tc_fence_after();
+      NFI_STEP_WAIT(&full[st], u & 1);
+      NFI_STEP_WAIT(&slot_free[sl], (v & 1) ^ 1);
       NFI_T(0)
+      float* d2 = d2s + sl * (kThreads * kD2Ld);
       if (!dbg_skip_consumer) {
-        uint32_t ra[16], rb[16];
-        float lo[16], hi[16];
-        tc::tmem_ld16_nowait(d1, ra);
-        tc::tmem_ld16_nowait(d1 + 16, rb);
-        tc::tmem_wait_ld();
-#pragma unroll 1
-        for (int c2 = 0; c2 < 2; ++c2) {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) lo[i] = __uint_as_float(ra[i]);
-          if (c2 == 0) tc::tmem_ld16_nowait(d1 + 32, ra);  // next 32 columns while these compute
-          softplus_split16(lo, hi, b1s + 32 * c2);
-          tc::tmem_st16(d1 + 32 * c2, lo);
-          tc::tmem_st16(d1 + 64 + 32 * c2, hi);
-#pragma unroll
-          for (int i = 0; i < 16; ++i) lo[i] = __uint_as_float(rb[i]);
-          if (c2 == 0) tc::tmem_ld16_nowait(d1 + 48, rb);
-          softplus_split16(lo, hi, b1s + 32 * c2 + 16);
-          tc::tmem_st16(d1 + 32 * c2 + 16, lo);
-          tc::tmem_st16(d1 + 64 + 32 * c2 + 16, hi);
-          if (c2 == 0) tc::tmem_wait_ld();
-        }
-        tc::tmem_wait_st();
+        decoder_step(dsc_a0 + (uint64_t)st * (kFwdStageBytes >> 4), dsc_w1_hi, dsc_w1_lo, dsc_w2_hi,
+                     dsc_w2_lo, b1s, d2, wig, lane, [&]() {
+                       __syncwarp();
+                       if (lane == 0) mbar_arrive(&a_free[st]);
+                     });
+      } else {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&a_free[st]);
       }
-      tc::tc_fence_before();
       __syncwarp();
-      if (lane == 0) mbar_arrive(&h_ready[sl]);
+      if (lane == 0) mbar_arrive(&d2_full[sl]);
+      if (++st == NS) { st = 0; ++u; }
       if (++sl == kPipeSlots) { sl = 0; ++v; }
       NFI_T(1)
       if (DBG && dbg_time) tacc[9] += 1;
@@ -865,9 +704,8 @@ render_forward_pipe(const nfi_render_params p, const unsigned char* __restrict__
       for (int i = 0; i < 10; ++i) p.normals[16 + i] = (float)tacc[i];
   } else {
     // ================================ SHADING ================================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(Cfg::kShadeRegs));
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::kShadeRegs));
     uint32_t sl = 0, v = 0;
-    const uint32_t lane_addr = (uint32_t)(32 * wig) << 16;
     FieldConst fc;
     fc.A = p.n_attention;
     fc.use_sdf = p.use_sdf;
@@ -899,15 +737,20 @@ render_forward_pipe(const nfi_render_params p, const unsigned char* __restrict__
 
       // decoder outputs of the next ring position -> density and colour at depth t
       auto shade = [&](float t, float& sigma, float& cr, float& cg, float& cb, float* ex) {
-        const uint32_t d2 = tmem_base + sl * kPipeSlotCols + 128 + lane_addr;
+        const float* d2 = d2s + sl * (kThreads * kD2Ld) + gt * kD2Ld;
         if (DBG && dbg_time && tprev == 0) tprev = clock64();
         NFI_T(2)
         NFI_STEP_WAIT(&d2_full[sl], v & 1);
-        tc::tc_fence_after();
         NFI_T(0)
         float o16[16];
-        tc::tmem_ld16(d2, o16);
-        tc::tc_fence_before();
+#pragma unroll
+        for (int o4 = 0; o4 < 4; ++o4) {
+          const float4 x = *reinterpret_cast<const float4*>(d2 + 4 * o4);
+          o16[4 * o4] = x.x;
+          o16[4 * o4 + 1] = x.y;
+          o16[4 * o4 + 2] = x.z;
+          o16[4 * o4 + 3] = x.w;
+        }
         __syncwarp();
         if (lane == 0) mbar_arrive(&slot_free[sl]);
         if (++sl == kPipeSlots) { sl = 0; ++v; }
@@ -1065,7 +908,6 @@ render_forward_pipe(const nfi_render_params p, const unsigned char* __restrict__
       for (int i = 0; i < 10; ++i) p.normals[32 + i] = (float)tacc[i];
   }
 #undef NFI_T
-  tc::tc_fence_before();
   __syncthreads();
   if (p.n_peers > 0 && p.peer_done != nullptr && tid == 0) {
     // Completion handshake of the fused exchange.  Every CTA: its threads' peer stores are ordered
@@ -1093,7 +935,6 @@ render_forward_pipe(const nfi_render_params p, const unsigned char* __restrict__
       }
     }
   }
-  if (tid < 32) tc::tmem_dealloc(tmem_base, 512);
 }
 
 }  // namespace nfi

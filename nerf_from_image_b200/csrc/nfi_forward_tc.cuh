@@ -1,24 +1,22 @@
 // Forward render kernel, tensor-core variant (NFI_MLP_TC_3XTF32).
 //
-// CTA = 512 threads = 4 independent "tile groups" of 128 threads; a group owns
-// one 16x8 pixel tile (thread = ray, exactly as in nfi_forward.cuh) and the four
-// groups of a CTA cover a 32x16 pixel block of one image.  One CTA per SM:
-// 16 resident warps, ~150 KB of shared memory, all 512 TMEM columns.
+// CTA = 512 threads = 4 independent "tile groups" of 128 threads (one warpgroup each); a group
+// owns one 16x8 pixel tile (thread = ray, exactly as in nfi_forward.cuh) and the four groups of
+// a CTA cover a 32x16 pixel block of one image.  One CTA per SM: 16 resident warps, ~195 KB of
+// shared memory.
 //
 // Per sample step and group:
 //   1. every thread places its point and computes its 3x(offset, fx, fy) taps;
 //   2. the group's four warps gather features cooperatively (8 lanes x float4
 //      = one 128-byte channel-last texel per tap) and write them, split into
-//      TF32 hi/lo parts, straight into the group's A tiles in the UMMA
+//      TF32 hi/lo parts, straight into the group's A tiles in the wgmma
 //      SWIZZLE_128B K-major layout -- features never exist anywhere else;
-//   3. one thread issues 12 tcgen05.mma (3xTF32, M=128 N=64 K=32) into the
-//      group's first 64 TMEM columns and commits to the group's mbarrier;
-//   4. every thread reads its own TMEM lane (tcgen05.ld), applies bias +
-//      softplus, and hands the hidden activations back to the tensor core split
-//      as H_hi (shared memory, in the space of the now idle A tiles) and H_lo
-//      (tcgen05.st over the D1 columns it just read);
-//   5. 24 more tcgen05.mma (N=16, K=64; H_lo read from TMEM, H_hi from shared
-//      memory) produce the 1+A decoder outputs in 16 further TMEM columns;
+//   3. the warpgroup issues, per 64-row half of the tile, 12 wgmma (3xTF32, M=64 N=64 K=32)
+//      with the accumulator in registers;
+//   4. bias + softplus on those registers; the hidden activations go back to the tensor core as
+//      register A fragments, split as H_hi / H_lo;
+//   5. 24 more wgmma (N=16, K=64) produce the 1+A decoder outputs, which pass through a
+//      [128 x 20] shared-memory tile to the thread that owns the ray;
 //   6. density / softmax-palette colour / alpha compositing in registers.
 // Decoder weights arrive pre-split and pre-swizzled ("weight image", built by
 // prep_weight_image) through ONE TMA bulk copy per CTA.
@@ -49,20 +47,20 @@ constexpr int kWiBytes = kWiB2 + 64;       // 24896
 // shared memory map (bytes from the 1024-aligned base)
 constexpr int kSmA = 25600;                // 25 * 1024
 constexpr int kSmAGroup = 32768;           // A_hi (16 KB) + A_lo (16 KB); later H_hi k-blocks 0/1
-constexpr int kSmPal = kSmA + kGroups * kSmAGroup;
-constexpr int kSmBars = kSmPal + 48 * 4;   // 5 mbarriers
-constexpr int kSmTmemPtr = kSmBars + 8 * 8;
-constexpr int kSmTcBytes = kSmTmemPtr + 16;
-// TMEM columns of group g: [128 g, +64) D1 then H_lo, [128 g + 64, +16) D2
+constexpr int kOutLd = 20;                 // decoder-output tile: [128 rays][20] floats per group
+constexpr int kSmOut = kSmA + kGroups * kSmAGroup;
+constexpr int kSmPal = kSmOut + kGroups * kThreads * kOutLd * 4;
+constexpr int kSmBars = kSmPal + 48 * 4;   // 1 mbarrier (weights)
+constexpr int kSmTcBytes = kSmBars + 8;
 
 // scratch per group-tile: float4 srgb[S][128], float t[S][128], w[S][128], zf[S][128]
 __host__ __device__ inline size_t tc_scratch_floats_per_group(int S) {
   return (size_t)S * kThreads * 7;
 }
 
-// Builds the weight image: W1 split into TF32 hi/lo and laid out as the UMMA
+// Builds the weight image: W1 split into TF32 hi/lo and laid out as the wgmma
 // B operand ([64 rows = hidden unit][32 k] fp32, K-major, SWIZZLE_128B), W2
-// transposed/padded, biases.
+// padded to 16 rows with its K positions in register-fragment order (tc::kpos_of_hidden), biases.
 static __global__ void prep_weight_image(const float* __restrict__ w1, const float* __restrict__ b1,
                                   const float* __restrict__ w2, const float* __restrict__ b2,
                                   int nout, unsigned char* __restrict__ img, float scale1,
@@ -82,7 +80,8 @@ static __global__ void prep_weight_image(const float* __restrict__ w1, const flo
     const int o = i / kHid, j = i % kHid;  // W2[o][j], rows >= nout are zero
     const float w = (o < nout) ? w2[o * kHid + j] * (o >= 1 ? scale2 : 1.f) : 0.f;
     const float hi = tc::tf32_hi(w);
-    const uint32_t off = (j >> 5) * 2048 + tc::sw128_offset(o, (j & 31) >> 2) + (j & 3) * 4;
+    const int jp = tc::kpos_of_hidden(j);
+    const uint32_t off = (jp >> 5) * 2048 + tc::sw128_offset(o, (jp & 31) >> 2) + (jp & 3) * 4;
     *reinterpret_cast<float*>(img + kWiW2Hi + off) = hi;
     *reinterpret_cast<float*>(img + kWiW2Lo + off) = w - hi;
   }
@@ -113,7 +112,7 @@ __device__ __forceinline__ void pack_taps(float gx, float gy, int R, uint32_t& o
 }
 
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-  return __ffma2_rn(a, b, c);
+  return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
 }
 
 // interpolates one plane's 4 taps for this lane's 4 channels, accumulating into acc
@@ -332,8 +331,7 @@ struct ByteTaps {
 // The nw texel is clamped to R-2, so that all four taps always exist at fixed offsets (+128 B, +one
 // row): at the far edge the fraction becomes 1 instead of 0 on the next cell, the interpolated value
 // is the same bit for bit (0 * finite + 1 * v), and the serving lanes need two address computations
-// per plane instead of four (round 1 carried two "neighbour exists" flag bits: 8.75 -> 8.66 ms,
-// profiles/r2_ab_forward_fixed_offset_taps.txt).
+// per plane instead of four (instead of two "neighbour exists" flag bits per tap).
 __device__ __forceinline__ void byte_taps(float gx, float gy, int R, uint32_t plane_units,
                                           uint32_t& o, float& fx, float& fy) {
   const float m = (float)(R - 1);
@@ -429,8 +427,7 @@ struct TcShared {
   const float* b1;
   const float* b2;
   float* pal;
-  uint64_t* bars;        // [0..3] group MMA barriers, [4] weights
-  uint32_t* tmem_ptr;
+  uint64_t* bars;        // [0] weights
 };
 
 __device__ __forceinline__ TcShared tc_shared_map(unsigned char* raw) {
@@ -440,162 +437,93 @@ __device__ __forceinline__ TcShared tc_shared_map(unsigned char* raw) {
   s.b2 = reinterpret_cast<const float*>(raw + kWiB2);
   s.pal = reinterpret_cast<float*>(raw + kSmPal);
   s.bars = reinterpret_cast<uint64_t*>(raw + kSmBars);
-  s.tmem_ptr = reinterpret_cast<uint32_t*>(raw + kSmTmemPtr);
   return s;
 }
 
 // per-thread view of its tile group
 struct TcGroup {
   int g, gt, wig;
-  unsigned char* a_hi;   // A_hi tile  / H_hi k-block 0
-  unsigned char* a_lo;   // A_lo tile  / H_hi k-block 1
-  uint64_t dsc_a, dsc_w1_hi, dsc_w1_lo, dsc_w2_hi, dsc_w2_lo;  // UMMA descriptor bases
-  uint32_t d_tmem;       // group's first TMEM column, lane 0
-  uint32_t d_lane;       // same, this warp's lane quadrant
-  uint64_t* bar;
+  unsigned char* a_hi;   // A_hi tile
+  unsigned char* a_lo;   // A_lo tile
+  float* out;            // decoder outputs, [128][kOutLd]
+  uint64_t dsc_a, dsc_w1_hi, dsc_w1_lo, dsc_w2_hi, dsc_w2_lo;  // wgmma descriptor bases
 };
 
-__device__ __forceinline__ bool tc_elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n.reg .pred p;\nelect.sync _|p, 0xffffffff;\nselp.u32 %0, 1, 0, p;\n}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
-
-__device__ __forceinline__ TcGroup tc_group(const TcShared& sm, uint32_t tmem_base, int tid) {
+__device__ __forceinline__ TcGroup tc_group(const TcShared& sm, int tid) {
   TcGroup q;
   // warp-uniform by construction AND known to the compiler as such (shfl from lane 0):
-  // lets ptxas keep the UMMA operands in uniform registers instead of a
-  // per-instruction ELECT / R2UR waterfall loop.
+  // lets ptxas keep the wgmma operands in uniform registers
   q.g = __shfl_sync(kFull, tid >> 7, 0);
   q.gt = tid & 127;
   q.wig = __shfl_sync(kFull, q.gt >> 5, 0);
   q.a_hi = sm.base + kSmA + q.g * kSmAGroup;
   q.a_lo = q.a_hi + 16384;
+  q.out = reinterpret_cast<float*>(sm.base + kSmOut) + q.g * kThreads * kOutLd;
   const uint32_t base_s = tc::smem_u32(sm.base);
-  q.dsc_a = tc::umma_desc_sw128(base_s + kSmA + q.g * kSmAGroup);
-  q.dsc_w1_hi = tc::umma_desc_sw128(base_s + kWiW1Hi);
-  q.dsc_w1_lo = tc::umma_desc_sw128(base_s + kWiW1Lo);
-  q.dsc_w2_hi = tc::umma_desc_sw128(base_s + kWiW2Hi);
-  q.dsc_w2_lo = tc::umma_desc_sw128(base_s + kWiW2Lo);
-  q.d_tmem = __shfl_sync(kFull, tmem_base, 0) + q.g * 128;
-  q.d_lane = q.d_tmem + ((uint32_t)(32 * q.wig) << 16);
-  q.bar = &sm.bars[q.g];
+  q.dsc_a = tc::gmma_desc_sw128(base_s + kSmA + q.g * kSmAGroup);
+  q.dsc_w1_hi = tc::gmma_desc_sw128(base_s + kWiW1Hi);
+  q.dsc_w1_lo = tc::gmma_desc_sw128(base_s + kWiW1Lo);
+  q.dsc_w2_hi = tc::gmma_desc_sw128(base_s + kWiW2Hi);
+  q.dsc_w2_lo = tc::gmma_desc_sw128(base_s + kWiW2Lo);
   return q;
 }
 
 // The decoder on one 128-point tile whose features already sit (hi/lo split)
-// in the group's A tiles.  Both linear layers run on the tensor core:
-//   MMA batch 1: D1 = A * W1^T                       (12 x tcgen05.mma, N = 64)
-//   epilogue 1 : h = softplus(D1 + b1); H_hi -> shared memory (re-using the A
-//                tiles as two K-blocks), H_lo -> TMEM in place of D1
-//   MMA batch 2: D2 = H * W2^T                       (24 x tcgen05.mma, N = 16)
-//   epilogue 2 : out = D2 + b2
+// in the group's A tiles.  Both linear layers run on the tensor core, one
+// 64-row half of the tile after the other (the group is one warpgroup):
+//   layer 1    : D1 = A * W1^T                      (12 x wgmma, N = 64, registers)
+//   epilogue 1 : h = softplus(D1 + b1) -> H_hi / H_lo register A fragments
+//   layer 2    : D2 = H * W2^T                      (24 x wgmma, N = 16)
+//   epilogue 2 : D2 -> the group's output tile; out = D2 + b2 of this thread's row
 template <int NOUT_PAD>
-__device__ __forceinline__ void tile_mlp(const TcGroup& q, const TcShared& sm, uint32_t& phase,
+__device__ __forceinline__ void tile_mlp(const TcGroup& q, const TcShared& sm,
                                          float (&out)[NOUT_PAD]) {
+  const int lane = q.gt & 31;
   tc::fence_async_smem();
-  tc::tc_fence_before();
-  tc::bar_sync(1 + q.g, kThreads);
-  if (q.wig == 0) {
-    if (tc_elect_one()) {
-      tc::tc_fence_after();
-      tc::issue_layer1_d(q.d_tmem, q.dsc_a, q.dsc_a + (16384 >> 4), q.dsc_w1_hi, q.dsc_w1_lo);
-      tc::umma_commit(q.bar);
-    }
-    __syncwarp();
-  }
-  tc::mbar_wait(q.bar, phase);
-  phase ^= 1;
-  tc::tc_fence_after();
+  tc::bar_sync(1 + q.g, kThreads);  // A tiles complete, previous outputs consumed
 #pragma unroll 1
-  for (int c2 = 0; c2 < 2; ++c2) {  // two 16-column TMEM loads in flight
-    uint32_t ra[16], rb[16];
-    tc::tmem_ld16_nowait(q.d_lane + 32 * c2, ra);
-    tc::tmem_ld16_nowait(q.d_lane + 32 * c2 + 16, rb);
-    tc::tmem_wait_ld();
-    unsigned char* hrow = (c2 == 0) ? q.a_hi : q.a_lo;
+  for (int mb = 0; mb < 2; ++mb) {
+    float d[32];
 #pragma unroll
-    for (int half = 0; half < 2; ++half) {
-      float v[16];
+    for (int i = 0; i < 32; ++i) d[i] = 0.f;
+    tc::wgmma_fence();
+    tc::layer1_mb(d, q.dsc_a + mb * (8192 >> 4), q.dsc_a + ((16384 + mb * 8192) >> 4), q.dsc_w1_hi,
+                  q.dsc_w1_lo);
+    tc::wgmma_commit();
+    tc::wgmma_wait<0>();
+    tc::reg_fence(d);
+    uint32_t hi[8][4], lo[8][4];
+    tc::softplus_frag<false>(d, sm.b1, lane & 3, hi, lo);
+    float o[8];
 #pragma unroll
-      for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(half ? rb[i] : ra[i]);
-#pragma unroll
-      for (int i4 = 0; i4 < 4; ++i4) {
-        const float4 bb = *reinterpret_cast<const float4*>(sm.b1 + 32 * c2 + 16 * half + 4 * i4);
-        const float bv[4] = {bb.x, bb.y, bb.z, bb.w};
-        float hi[4];
-#pragma unroll
-        for (int i = 0; i < 4; i += 2) {
-          // softplus(x) = max(x,0) + ln2 * lg2(1 + 2^(-|x| log2 e)); two lanes packed (FFMA2 etc.)
-          const float2 x = __fadd2_rn(make_float2(v[4 * i4 + i], v[4 * i4 + i + 1]),
-                                      make_float2(bv[i], bv[i + 1]));
-          const float2 ax = __fmul2_rn(make_float2(fabsf(x.x), fabsf(x.y)),
-                                       make_float2(-1.4426950408889634f, -1.4426950408889634f));
-          const float2 l = make_float2(tc::lg2_approx(1.f + tc::ex2_approx(ax.x)),
-                                       tc::lg2_approx(1.f + tc::ex2_approx(ax.y)));
-          const float2 h = __ffma2_rn(l, make_float2(0.6931471805599453f, 0.6931471805599453f),
-                                      make_float2(fmaxf(x.x, 0.f), fmaxf(x.y, 0.f)));
-          hi[i] = tc::tf32_hi(h.x);
-          hi[i + 1] = tc::tf32_hi(h.y);
-          const float2 lo2 = __fadd2_rn(h, make_float2(-hi[i], -hi[i + 1]));
-          v[4 * i4 + i] = lo2.x;
-          v[4 * i4 + i + 1] = lo2.y;
-        }
-        const uint32_t off = tc::sw128_offset(q.gt, half * 4 + i4);
-        *reinterpret_cast<float4*>(hrow + off) = make_float4(hi[0], hi[1], hi[2], hi[3]);
-      }
-      tc::tmem_st16(q.d_lane + 32 * c2 + 16 * half, v);  // H_lo over the D1 columns just read
-    }
+    for (int i = 0; i < 8; ++i) o[i] = 0.f;
+    tc::wgmma_fence();
+    tc::layer2_mb(o, hi, lo, q.dsc_w2_hi, q.dsc_w2_lo);
+    tc::wgmma_commit();
+    tc::wgmma_wait<0>();
+    tc::reg_fence(o);
+    tc::store_frag_rows(o, q.out + 64 * mb * kOutLd, kOutLd, q.wig, lane);
   }
-  tc::tmem_wait_st();
-  tc::fence_async_smem();
-  tc::tc_fence_before();
   tc::bar_sync(1 + q.g, kThreads);
-  if (q.wig == 0) {
-    if (tc_elect_one()) {
-      tc::tc_fence_after();
-      tc::issue_layer2_d(q.d_tmem + 64, q.d_tmem, q.dsc_a, q.dsc_w2_hi, q.dsc_w2_lo);
-      tc::umma_commit(q.bar);
-    }
-    __syncwarp();
-  }
-  tc::mbar_wait(q.bar, phase);
-  phase ^= 1;
-  tc::tc_fence_after();
-  float v[16];
-  tc::tmem_ld16(q.d_lane + 64, v);
+  const float* row = q.out + q.gt * kOutLd;
 #pragma unroll
-  for (int o = 0; o < NOUT_PAD; ++o) out[o] = v[o] + sm.b2[o];
+  for (int o = 0; o < NOUT_PAD; ++o) out[o] = row[o] + sm.b2[o];
 }
 
-// common prologue: barriers, TMEM, weight image via TMA bulk copy
-__device__ __forceinline__ uint32_t tc_prologue(const TcShared& sm, const unsigned char* wimg,
-                                                int tid) {
+// common prologue: barrier, weight image via TMA bulk copy
+__device__ __forceinline__ void tc_prologue(const TcShared& sm, const unsigned char* wimg,
+                                            int tid) {
   if (tid == 0) {
     if (tc::smem_u32(sm.base) & 1023u) __trap();  // SWIZZLE_128B tiles need 1024-byte alignment
-    for (int i = 0; i < kGroups; ++i) tc::mbar_init(&sm.bars[i], 1);
-    tc::mbar_init(&sm.bars[4], 1);
+    tc::mbar_init(&sm.bars[0], 1);
     tc::fence_mbar_init();
   }
-  if (tid < 32) tc::tmem_alloc(sm.tmem_ptr, 512);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem_base = *sm.tmem_ptr;
   if (tid == 0) {
-    tc::mbar_expect_tx(&sm.bars[4], kWiBytes);
-    tc::tma_bulk_g2s(sm.base, wimg, kWiBytes, &sm.bars[4]);
+    tc::mbar_expect_tx(&sm.bars[0], kWiBytes);
+    tc::tma_bulk_g2s(sm.base, wimg, kWiBytes, &sm.bars[0]);
   }
-  tc::mbar_wait(&sm.bars[4], 0);
-  return tmem_base;
-}
-
-__device__ __forceinline__ void tc_epilogue_free(const TcShared& sm, uint32_t tmem_base, int tid) {
-  tc::tc_fence_before();
-  __syncthreads();
-  if (tid < 32) tc::tmem_dealloc(tmem_base, 512);
+  tc::mbar_wait(&sm.bars[0], 0);
 }
 
 // ---------------------------------------------------------------------------
@@ -610,10 +538,9 @@ decoder_forward_tc(const float* __restrict__ feats, long long n_points, int nout
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   const TcShared sm = tc_shared_map(smem_raw);
   const int tid = threadIdx.x;
-  const uint32_t tmem_base = tc_prologue(sm, wimg, tid);
-  const TcGroup q = tc_group(sm, tmem_base, tid);
+  tc_prologue(sm, wimg, tid);
+  const TcGroup q = tc_group(sm, tid);
   const long long n_tiles = (n_points + 127) / 128;
-  uint32_t phase = 0;
   for (long long tile = (long long)blockIdx.x * kGroups + q.g; tile < n_tiles;
        tile += (long long)gridDim.x * kGroups) {
     const long long row = tile * 128 + q.gt;  // thread gt stages row gt: 8 x 16 bytes
@@ -629,12 +556,11 @@ decoder_forward_tc(const float* __restrict__ feats, long long n_points, int nout
       *reinterpret_cast<float4*>(q.a_lo + off) = fl;
     }
     float out[NOUT_PAD];
-    tile_mlp<NOUT_PAD>(q, sm, phase, out);
+    tile_mlp<NOUT_PAD>(q, sm, out);
     if (row < n_points)
       for (int o = 0; o < NOUT_PAD; ++o)
         if (o < nout) outp[row * nout + o] = out[o];
   }
-  tc_epilogue_free(sm, tmem_base, tid);
 }
 
 // ---------------------------------------------------------------------------
@@ -649,8 +575,8 @@ render_forward_tc(const nfi_render_params p, const unsigned char* __restrict__ w
   const TcShared sm = tc_shared_map(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31;
   const int S = p.num_samples;
-  const uint32_t tmem_base = tc_prologue(sm, wimg, tid);
-  const TcGroup q = tc_group(sm, tmem_base, tid);
+  tc_prologue(sm, wimg, tid);
+  const TcGroup q = tc_group(sm, tid);
   const int g = q.g, gt = q.gt, wig = q.wig;
 
   // CTA -> 2x2 block of 16x8 tiles of one image
@@ -691,7 +617,6 @@ render_forward_tc(const nfi_render_params p, const unsigned char* __restrict__ w
 
     unsigned char* a_hi = q.a_hi;
     unsigned char* a_lo = q.a_lo;
-    uint32_t phase = 0;
 
     const size_t group_slot = (size_t)blockIdx.x * kGroups + g;
     float* slab = scratch + group_slot * tc_scratch_floats_per_group(S);
@@ -714,7 +639,7 @@ render_forward_tc(const nfi_render_params p, const unsigned char* __restrict__ w
       pack_taps(x1, x2, R, tp.o[2], tp.fx[2], tp.fy[2]);
       gather_to_tiles_deep(planes_b, R, tp, a_hi, a_lo, 32 * wig, lane);
       float out[NOUT_PAD];
-      tile_mlp<NOUT_PAD>(q, sm, phase, out);
+      tile_mlp<NOUT_PAD>(q, sm, out);
       float probs[NOUT_PAD];
       field_head<NOUT_PAD, true>(out, fc, sm.pal, keep, sigma, cr, cg, cb, probs);
       if (EXTRA == 1) {
@@ -865,7 +790,6 @@ render_forward_tc(const nfi_render_params p, const unsigned char* __restrict__ w
         for (int a = 0; a < 3; ++a) p.extra[ray * 3 + a] = comp.ae[a];
     }
   }
-  tc_epilogue_free(sm, tmem_base, tid);
 }
 
 }  // namespace nfi

@@ -9,6 +9,8 @@
 // This kernel is that kernel with the reverse compositing taken out: one sweep over the merged
 // samples of a ray (fine depths from the forward pass's z_fine), gather -> MMA1 -> softplus ->
 // MMA2 -> (shading: w_i) and -> s -> MMA4 -> (producers: re-read, dot, normalise, weight, sum).
+// s needs nothing from the shading group, so the activation group issues all three GEMMs of a
+// step back to back and releases the stage after layer 1.
 // It runs after render_forward_pipe (which wrote z_fine and mask) and fills `normals`.
 #pragma once
 #include "nfi_backward_pipe.cuh"
@@ -27,26 +29,23 @@ render_normals_pipe(const nfi_render_params p, const unsigned char* __restrict__
   unsigned char* base = smem_raw;
   const int tid = threadIdx.x, lane = tid & 31;
   const int hw_wg = __shfl_sync(kFull, tid >> 7, 0);
-  // logical role: 0 activation, 1 shading, 2 MMA issuers, 3.. producer sets (see nfi_forward_pipe.cuh)
-  const int wg = (hw_wg < P) ? hw_wg + 3 : (P + 2 - hw_wg);
+  // logical role: 0 activation, 1 shading, 3.. producer sets (see nfi_forward_pipe.cuh)
+  const int wg = (hw_wg < P) ? hw_wg + 3 : (P + 1 - hw_wg);
   const int gt = tid & 127;
   const int wig = __shfl_sync(kFull, gt >> 5, 0);
   const int S = p.num_samples;
   const int n_total = (p.fine_sampling ? 2 : 1) * S;  // steps per tile
 
   uint64_t* bars = reinterpret_cast<uint64_t*>(base + Cfg::kSmBars);
-  uint64_t* full = bars;                     // [3] stage gathered (4 warps)
-  uint64_t* a_free = full + NS;              // [3] stage read by MMA1 (commit)
-  uint64_t* d1_full = a_free + NS;           // [2] commit
-  uint64_t* h_ready = d1_full + kBwdSlots;   // [2] 4 warps
-  uint64_t* d2_full = h_ready + kBwdSlots;   // [2] commit
-  uint64_t* dout_ready = d2_full + kBwdSlots;   // [2] 4 warps
-  uint64_t* d3_full = dout_ready + kBwdSlots;   // [2] commit
-  uint64_t* dpre_ready = d3_full + kBwdSlots;   // [2] 4 warps
-  uint64_t* d4_full = dpre_ready + kBwdSlots;   // [2] commit
-  uint64_t* slot_free = d4_full + kBwdSlots;    // [2] 4 warps (D4 read)
+  uint64_t* full = bars;                        // [3] stage gathered (4 warps)
+  uint64_t* a_free = full + NS;                 // [3] stage read by layer 1 (4 warps)
+  uint64_t* d2_full = a_free + NS;              // [2] D2 in its slot (4 warps)
+  uint64_t* dout_ready = d2_full + kBwdSlots;   // [2] D2 read, sample weight written (4 warps)
+  uint64_t* d4_full = dout_ready + kBwdSlots;   // [2] D4 in its slot (4 warps)
+  uint64_t* slot_free = d4_full + kBwdSlots;    // [2] D4 used (4 warps)
   uint64_t* wbar = slot_free + kBwdSlots;       // [2] weight images landed
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(base + Cfg::kSmTmemPtr);
+  float* d2s = reinterpret_cast<float*>(base + Cfg::kSmD2);  // [2][128][kD2Ld]
+  float* d4s = reinterpret_cast<float*>(base + Cfg::kSmD4);  // [2][128][kD4Ld]
   const float* b1s = reinterpret_cast<const float*>(base + kWiB1);
   const float* b2s = reinterpret_cast<const float*>(base + kWiB2);
   float* pal = reinterpret_cast<float*>(base + Cfg::kSmPal);
@@ -59,28 +58,20 @@ render_normals_pipe(const nfi_render_params p, const unsigned char* __restrict__
   if (tid == 0) {
     if (tc::smem_u32(base) & 1023u) __trap();
     for (int i = 0; i < NS; ++i) {
-      tc::mbar_init(&full[i], 4);
-      tc::mbar_init(&a_free[i], 1);
+      tc::mbar_init(&full[i], kWarps);
+      tc::mbar_init(&a_free[i], kWarps);
     }
     for (int i = 0; i < kBwdSlots; ++i) {
-      tc::mbar_init(&d1_full[i], 1);
-      tc::mbar_init(&h_ready[i], kWarps);
-      tc::mbar_init(&d2_full[i], 1);
+      tc::mbar_init(&d2_full[i], kWarps);
       tc::mbar_init(&dout_ready[i], kWarps);
-      tc::mbar_init(&d3_full[i], 1);
-      tc::mbar_init(&dpre_ready[i], kWarps);
-      tc::mbar_init(&d4_full[i], 1);
+      tc::mbar_init(&d4_full[i], kWarps);
       tc::mbar_init(&slot_free[i], kWarps);
     }
     tc::mbar_init(&wbar[0], 1);
     tc::mbar_init(&wbar[1], 1);
     tc::fence_mbar_init();
   }
-  if (tid < 32) tc::tmem_alloc(tmem_ptr, 512);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(kFull, *tmem_ptr, 0);
   if (tid == 0) {
     tc::mbar_expect_tx(&wbar[0], kWiBytes);
     tc::tma_bulk_g2s(base, wimg, kWiBytes, &wbar[0]);
@@ -90,7 +81,6 @@ render_normals_pipe(const nfi_render_params p, const unsigned char* __restrict__
   tc::mbar_wait(&wbar[0], 0);
   tc::mbar_wait(&wbar[1], 0);
 
-  const uint32_t base_s = tc::smem_u32(base);
   const int tiles_x = (p.width + kTileW - 1) / kTileW;
   const int tiles_y = (p.height + kTileH - 1) / kTileH;
   const int n_tiles = tiles_x * tiles_y * p.batch;
@@ -100,14 +90,11 @@ render_normals_pipe(const nfi_render_params p, const unsigned char* __restrict__
   const int R = p.plane_res;
   const float inv_range = 1.f / p.scene_range;
   const uint32_t plane_bytes = (uint32_t)R * (uint32_t)R * 128u;
-  const uint32_t lane_addr = (uint32_t)(32 * wig) << 16;
 
   if (wg >= 3) {
     // ================================ PRODUCER / SCATTER ================================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(Cfg::kProducerRegs));
     const int set = wg - 3;
-    float* Dw = reinterpret_cast<float*>(base + Cfg::kSmStage + (set * 4 + wig) * Cfg::kStageWarp);
-    float* Gw = Dw + 32 * 36;
+    float* Gw = reinterpret_cast<float*>(base + Cfg::kSmStage + (set * 4 + wig) * Cfg::kStageWarp);
     const int q = lane >> 3, kq = lane & 7;
     const uint32_t row_units = (uint32_t)R * 8u;
     uint32_t n0 = 0;  // ring position of the tile's first step
@@ -169,30 +156,11 @@ render_normals_pipe(const nfi_render_params p, const unsigned char* __restrict__
         // ---- scatter step i: D4 -> plane gradient (and camera gradient)
         const uint32_t m = n0 + (uint32_t)i;
         const uint32_t sl = m % kBwdSlots, v = m / kBwdSlots;
-        const uint32_t d4 = tmem_base + sl * kBwdSlotCols + lane_addr;
+        // this warp's 32 rows of the D4 slot, read in place (released after the scatter)
+        const float* Dw = d4s + sl * (kThreads * kD4Ld) + 32 * wig * kD4Ld;
         NFI_STEP_WAIT(&d4_full[sl], v & 1);
         NFI_STEP_WAIT(&dout_ready[sl], v & 1);  // the shading thread's weight of this sample
         const float wgt = wbuf[sl * 128 + 32 * wig + lane];
-        tc::tc_fence_after();
-        {
-          uint32_t ra[16], rb[16];
-          tc::tmem_ld16_nowait(d4, ra);
-          tc::tmem_ld16_nowait(d4 + 16, rb);
-          tc::tmem_wait_ld();
-          tc::tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&slot_free[sl]);
-#pragma unroll
-          for (int c4 = 0; c4 < 4; ++c4) {
-            *reinterpret_cast<float4*>(Dw + lane * 36 + 4 * c4) =
-                make_float4(__uint_as_float(ra[4 * c4]), __uint_as_float(ra[4 * c4 + 1]),
-                            __uint_as_float(ra[4 * c4 + 2]), __uint_as_float(ra[4 * c4 + 3]));
-            *reinterpret_cast<float4*>(Dw + lane * 36 + 16 + 4 * c4) =
-                make_float4(__uint_as_float(rb[4 * c4]), __uint_as_float(rb[4 * c4 + 1]),
-                            __uint_as_float(rb[4 * c4 + 2]), __uint_as_float(rb[4 * c4 + 3]));
-          }
-        }
-        __syncwarp();
         const ByteTaps& tp = cur;
 #ifdef NFI_BWD_NO_SCATTER   // timing experiment: D4 is read and dropped
 #pragma unroll 1
@@ -203,7 +171,7 @@ render_normals_pipe(const nfi_render_params p, const unsigned char* __restrict__
 #endif
           const int src = 4 * gq + q;
           const uint32_t in6 = CAM ? __shfl_sync(kFull, cur_in, src) : 0u;
-          const float4 d4v = *reinterpret_cast<const float4*>(Dw + src * 36 + 4 * kq);
+          const float4 d4v = *reinterpret_cast<const float4*>(Dw + src * kD4Ld + 4 * kq);
           float gc0 = 0.f, gc1 = 0.f, gc2 = 0.f;
           // nw texel clamped to R-2: all four taps of a plane exist at fixed offsets
           const uint32_t dx = 8u;
@@ -267,6 +235,7 @@ render_normals_pipe(const nfi_render_params p, const unsigned char* __restrict__
           }
         }
         __syncwarp();
+        if (lane == 0) mbar_arrive(&slot_free[sl]);  // (the sample weight was read before)
         {
           // grad_x sdf of this thread's sample (D4 carries the 1/3 of the plane mean already),
           // F.normalize (generator.py:620), weighted with the detached compositing weight
@@ -290,120 +259,82 @@ render_normals_pipe(const nfi_render_params p, const unsigned char* __restrict__
         atomicAdd(p.normals + ray * 3 + 2, an2 + bg);
       }
     }
-  } else if (wg == 2) {
-    // ================================ MMA ISSUERS ================================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::kAuxRegs));
-    if (wig == 0) {
-      const uint64_t dsc_w1_hi = tc::umma_desc_sw128(base_s + kWiW1Hi);
-      const uint64_t dsc_w1_lo = tc::umma_desc_sw128(base_s + kWiW1Lo);
-      const uint64_t dsc_a0 = tc::umma_desc_sw128(base_s + Cfg::kSmA);
-      uint32_t st = 0, u = 0, sl = 0, v = 0;
-      for (uint32_t m = 0; m < total_steps; ++m) {
-        NFI_STEP_WAIT(&full[st], u & 1);
-        NFI_STEP_WAIT(&slot_free[sl], (v & 1) ^ 1);
-        if (elect_one()) {
-          tc::tc_fence_after();
-          const uint64_t dsc_a = dsc_a0 + (uint64_t)st * (kPipeStageBytes >> 4);
-          tc::issue_layer1_d(tmem_base + sl * kBwdSlotCols, dsc_a, dsc_a + (16384 >> 4),
-                             dsc_w1_hi, dsc_w1_lo);
-          tc::umma_commit(&d1_full[sl]);
-          tc::umma_commit(&a_free[st]);
-        }
-        __syncwarp();
-        if (++st == NS) { st = 0; ++u; }
-        if (++sl == kBwdSlots) { sl = 0; ++v; }
-      }
-    } else if (wig == 1) {
-      const uint64_t dsc_w2_hi = tc::umma_desc_sw128(base_s + kWiW2Hi);
-      const uint64_t dsc_w2_lo = tc::umma_desc_sw128(base_s + kWiW2Lo);
-      uint32_t sl = 0, v = 0;
-      for (uint32_t m = 0; m < total_steps; ++m) {
-        NFI_STEP_WAIT(&h_ready[sl], v & 1);
-        if (elect_one()) {
-          tc::tc_fence_after();
-          const uint32_t d = tmem_base + sl * kBwdSlotCols;
-          issue_layer2_tt(d + 128, d, d + 64, dsc_w2_hi, dsc_w2_lo);
-          tc::umma_commit(&d2_full[sl]);
-        }
-        __syncwarp();
-        if (++sl == kBwdSlots) { sl = 0; ++v; }
-      }
-    } else if (wig == 2) {
-      // (no dL/dH product here: s = W2[0,:] sigmoid(pre) comes straight from the activations)
-    } else {
-      const uint64_t b_hi = tc::umma_desc_sw128(base_s + Cfg::kSmWb + kWbW1tHi);
-      const uint64_t b_lo = tc::umma_desc_sw128(base_s + Cfg::kSmWb + kWbW1tLo);
-      uint32_t sl = 0, v = 0;
-      for (uint32_t m = 0; m < total_steps; ++m) {
-        NFI_STEP_WAIT(&dpre_ready[sl], v & 1);
-        if (elect_one()) {
-          tc::tc_fence_after();
-          const uint32_t d = tmem_base + sl * kBwdSlotCols;
-          issue_mma4(d, d + 64, d + 176, b_hi, b_lo);
-          tc::umma_commit(&d4_full[sl]);
-        }
-        __syncwarp();
-        if (++sl == kBwdSlots) { sl = 0; ++v; }
-      }
-    }
   } else if (wg == 0) {
-    // ================================ ACTIVATION (forward and reverse) ================================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::kActRegs));
-    auto act_fwd = [&](uint32_t m) {
-      const uint32_t sl = m % kBwdSlots, v = m / kBwdSlots;
-      const uint32_t d1 = tmem_base + sl * kBwdSlotCols + lane_addr;
-      NFI_STEP_WAIT(&d1_full[sl], v & 1);
-      tc::tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        float lo[16], hi[16];
-        tc::tmem_ld16(d1 + 16 * c, lo);
-        softplus_split16(lo, hi, b1s + 16 * c);
-        tc::tmem_st16(d1 + 16 * c, lo);
-        tc::tmem_st16(d1 + 64 + 16 * c, hi);
-      }
-      tc::tmem_wait_st();
-      tc::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&h_ready[sl]);
-    };
-    // dpre = dH * sigmoid(pre),  sigmoid(pre) = 1 - exp(-softplus(pre)) = 1 - 2^(-H log2 e)
-    auto act_bwd = [&](uint32_t m) {
-      const uint32_t sl = m % kBwdSlots, v = m / kBwdSlots;
-      const uint32_t d = tmem_base + sl * kBwdSlotCols + lane_addr;
-      NFI_STEP_WAIT(&d2_full[sl], v & 1);   // layer 2 has read H: H_hi's columns may be reused
-      tc::tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        uint32_t rh[16], rl[16];
-        tc::tmem_ld16_nowait(d + 64 + 16 * c, rh);
-        tc::tmem_ld16_nowait(d + 16 * c, rl);
-        tc::tmem_wait_ld();
-        float lo[16], hi[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const float h = __uint_as_float(rh[i]) + __uint_as_float(rl[i]);
-          const float sg = 1.f - tc::ex2_approx(-h * kLog2e);
-          const float dp = w2r0[16 * c + i] * sg;   // d sdf / d pre_j
-          hi[i] = tc::tf32_hi(dp);
-          lo[i] = dp - hi[i];
-        }
-        tc::tmem_st16(d + 176 + 16 * c, lo);  // dpre_lo over D3
-        tc::tmem_st16(d + 64 + 16 * c, hi);   // dpre_hi over H_hi
-      }
-      tc::tmem_wait_st();
-      tc::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&dpre_ready[sl]);
-    };
-    if (total_steps > 0) act_fwd(0);
+    // ================================ ACTIVATION: the three GEMMs ================================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(Cfg::kActRegs));
+    const uint32_t base_s = tc::smem_u32(base);
+    const uint64_t w1_hi = tc::gmma_desc_sw128(base_s + kWiW1Hi);
+    const uint64_t w1_lo = tc::gmma_desc_sw128(base_s + kWiW1Lo);
+    const uint64_t w2_hi = tc::gmma_desc_sw128(base_s + kWiW2Hi);
+    const uint64_t w2_lo = tc::gmma_desc_sw128(base_s + kWiW2Lo);
+    const uint64_t b4_hi = tc::gmma_desc_sw128(base_s + Cfg::kSmWb + kWbW1tHi);
+    const uint64_t b4_lo = tc::gmma_desc_sw128(base_s + Cfg::kSmWb + kWbW1tLo);
+    const uint64_t dsc_a0 = tc::gmma_desc_sw128(base_s + Cfg::kSmA);
+    const int t = lane & 3;
     for (uint32_t m = 0; m < total_steps; ++m) {
-      if (m + 1 < total_steps) act_fwd(m + 1);
-      act_bwd(m);
+      const uint32_t st = m % NS, u = m / NS, sl = m % kBwdSlots, v = m / kBwdSlots;
+      const uint64_t dsc_a = dsc_a0 + (uint64_t)st * (kPipeStageBytes >> 4);
+      float* d2 = d2s + sl * (kThreads * kD2Ld);
+      float* d4 = d4s + sl * (kThreads * kD4Ld);
+      NFI_STEP_WAIT(&full[st], u & 1);
+      NFI_STEP_WAIT(&dout_ready[sl], (v & 1) ^ 1);  // D2 of step m - 2 read
+      NFI_STEP_WAIT(&slot_free[sl], (v & 1) ^ 1);   // D4 of step m - 2 used
+#pragma unroll 1
+      for (int mb = 0; mb < 2; ++mb) {
+        float d[32];
+        zero(d);
+        tc::wgmma_fence();
+        tc::layer1_mb(d, dsc_a + mb * (8192 >> 4), dsc_a + ((16384 + mb * 8192) >> 4), w1_hi, w1_lo);
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::reg_fence(d);
+        if (mb == 1) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&a_free[st]);
+        }
+        {
+          uint32_t hi[8][4], lo[8][4];
+          tc::softplus_frag<true>(d, b1s, t, hi, lo);
+          float o[8];
+          zero(o);
+          tc::wgmma_fence();
+          tc::layer2_mb(o, hi, lo, w2_hi, w2_lo);
+          tc::wgmma_commit();
+          tc::wgmma_wait<0>();
+          tc::reg_fence(o);
+          tc::store_frag_rows(o, d2 + 64 * mb * kD2Ld, kD2Ld, wig, lane);
+        }
+        // d sdf / d pre_j = W2[0, j] sigmoid(pre_j),  sigmoid(pre) = 1 - 2^(-H log2 e)
+        uint32_t shi[8][4], slo[8][4];
+#pragma unroll
+        for (int kb = 0; kb < 8; ++kb) {
+          const float2 bb = *reinterpret_cast<const float2*>(b1s + 8 * kb + 2 * t);
+          const float2 ww = *reinterpret_cast<const float2*>(w2r0 + 8 * kb + 2 * t);
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const float h = tc::softplus_mufu<true>(d[4 * kb + e] + ((e & 1) ? bb.y : bb.x));
+            const float sg = 1.f - tc::ex2_approx(-h * kLog2e);
+            tc::put_split(shi, slo, kb, tc::afrag_slot(e), ((e & 1) ? ww.y : ww.x) * sg);
+          }
+        }
+        float d4v[16];
+        zero(d4v);
+        tc::wgmma_fence();
+        mma4_mb(d4v, shi, slo, b4_hi, b4_lo);
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::reg_fence(d4v);
+        tc::store_frag_rows(d4v, d4 + 64 * mb * kD4Ld, kD4Ld, wig, lane);
+      }
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(&d2_full[sl]);
+        mbar_arrive(&d4_full[sl]);
+      }
     }
   } else {
     // ================================ SHADING (forward and reverse) ================================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(Cfg::kShadeRegs));
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::kShadeRegs));
     FieldConst fc;
     fc.A = p.n_attention;
     fc.use_sdf = p.use_sdf;
@@ -438,15 +369,15 @@ render_normals_pipe(const nfi_render_params p, const unsigned char* __restrict__
         const float zn = has_next ? mw.pop() : z;
         const float delta = has_next ? (zn - z) * r.dn : 0.f;
         const uint32_t sl = m % kBwdSlots, v = m / kBwdSlots;
-        const uint32_t d = tmem_base + sl * kBwdSlotCols + lane_addr;
+        const float* row = d2s + sl * (kThreads * kD2Ld) + gt * kD2Ld;
         // ---- forward at this sample
         const float wx = r.ox + r.dx * z, wy = r.oy + r.dy * z, wz = r.oz + r.dz * z;
         const float x0 = wx * inv_range, x1 = wy * inv_range, x2 = wz * inv_range;
         const float keep = (fabsf(x0) > 1.f || fabsf(x1) > 1.f || fabsf(x2) > 1.f) ? 0.f : 1.f;
         NFI_STEP_WAIT(&d2_full[sl], v & 1);
-        tc::tc_fence_after();
         float o16[16];
-        tc::tmem_ld16(d + 128, o16);
+#pragma unroll
+        for (int o = 0; o < 16; ++o) o16[o] = row[o];
         float out[NOUT_PAD];
 #pragma unroll
         for (int o = 0; o < NOUT_PAD; ++o) out[o] = o16[o] + b2s[o];
@@ -464,16 +395,12 @@ render_normals_pipe(const nfi_render_params p, const unsigned char* __restrict__
         const float a = 1.f - __expf(-sigma * delta);
         wbuf[sl * 128 + gt] = a * T;
         T = T * ((1.f - a) + 1e-10f);
-        tc::tc_fence_before();
         __syncwarp();
         if (lane == 0) mbar_arrive(&dout_ready[sl]);
         z = zn;
       }
     }
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (tid < 32) tc::tmem_dealloc(tmem_base, 512);
 }
 
 }  // namespace nfi

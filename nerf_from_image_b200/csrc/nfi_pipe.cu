@@ -1,6 +1,6 @@
-// Translation unit of the pipelined tcgen05 kernels: forward (nfi_forward_pipe.cuh) and
-// backward (nfi_backward_pipe.cuh).  Compiled WITHOUT --split-compile: the forward kernel's
-// schedule is ~3 % slower with it (measured).
+// Translation unit of the pipelined tensor-core kernels: forward (nfi_forward_pipe.cuh),
+// backward (nfi_backward_pipe.cuh), surface normals (nfi_normals_pipe.cuh) and decoder-weight
+// gradients (nfi_wgrad_pipe.cuh).
 #include <cuda_runtime.h>
 #include <stdio.h>
 
@@ -133,7 +133,8 @@ int launch_pipe_backward(const nfi_render_params& p, const nfi_render_grads& g, 
   return bwd_np<16>(p, g, wimg, grid, st, err, err_len);
 }
 
-// decoder-weight gradients on tcgen05 (nfi_wgrad_pipe.cuh): both weight images + render_wgrad_pipe
+// decoder-weight gradients on the tensor cores (nfi_wgrad_pipe.cuh): both weight images +
+// render_wgrad_pipe
 int launch_pipe_wgrad(const nfi_render_params& p, const nfi_render_grads& g, int nout_pad,
                       unsigned char* wimg, unsigned grid, bool planes, cudaStream_t st, char* err,
                       size_t err_len) {

@@ -1,4 +1,4 @@
-// Launchers of the pipelined tcgen05 kernels (nfi_pipe.cu), a translation unit of its own so
+// Launchers of the pipelined tensor-core kernels (nfi_pipe.cu), a translation unit of its own so
 // that build.sh can compile it in parallel with the rest of the library.
 #pragma once
 #include <cuda_runtime.h>
@@ -16,7 +16,7 @@ int launch_pipe_forward(const nfi_render_params& p, int nout_pad, const unsigned
 int launch_pipe_backward(const nfi_render_params& p, const nfi_render_grads& g, int nout_pad,
                          unsigned char* wimg, unsigned grid, cudaStream_t st, char* err,
                          size_t err_len);
-// decoder-weight gradients (grad_w1 / b1 / w2 / b2 of `g`, accumulated) on tcgen05: both weight
+// decoder-weight gradients (grad_w1 / b1 / w2 / b2 of `g`, accumulated) on the tensor cores: both weight
 // images + render_wgrad_pipe; the other gradients of `g` are NOT produced (launch_pipe_backward)
 // (workspace at `wimg`: the two weight images, then one accumulator row buffer per CTA:
 // pipe_wgrad_workspace_bytes(grid) in all)

@@ -1,8 +1,8 @@
 // C-ABI entry points of libnfi_render.so (see include/nfi_render.h).
 //
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a --fmad=false -lineinfo
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a --fmad=false -lineinfo
 //        (nerf_from_image_b200/csrc/build.sh).  No torch, no CPU fallback: on a
-//        machine without an sm_100 device every launch returns an error.
+//        machine without an sm_90 device every launch returns an error.
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <string.h>
@@ -94,7 +94,7 @@ size_t num_ctas(const nfi_render_params* p) {
 constexpr size_t kWeightImageBytes = 32768;  // workspace header (nfi::kWiBytes rounded up)
 constexpr size_t kBackwardWorkspaceBytes = 65536;  // forward + backward weight images
 
-constexpr size_t kMaxPersistentCtas = 160;  // >= SM count of any sm_100 part (B200: 148)
+constexpr size_t kMaxPersistentCtas = 160;  // >= SM count of any sm_90 part (H100 SXM: 132)
 
 // persistent pipelined kernels (nfi_pipe.cu): one CTA per SM, one scratch slab per CTA
 size_t num_tc_ctas(const nfi_render_params* p) {  // persistent grid: at most one CTA per SM
@@ -345,7 +345,7 @@ extern "C" {
 int nfi_abi_version(void) { return NFI_ABI_VERSION; }
 
 const char* nfi_build_info(void) {
-  return "libnfi_render sm_100a (compute_100a) nvcc " NFI_STR(__CUDACC_VER_MAJOR__) "." NFI_STR(
+  return "libnfi_render sm_90a (compute_90a) nvcc " NFI_STR(__CUDACC_VER_MAJOR__) "." NFI_STR(
       __CUDACC_VER_MINOR__) " fmad=false";
 }
 
@@ -484,7 +484,7 @@ int nfi_decoder_forward(const float* features, int64_t n_points, const float* w1
   nfi::prep_weight_image<<<1, 256, 0, st>>>(w1, b1, w2, b2, nout, wimg, 1.f, 0.f, 1.f);
   NFI_CUDA(cudaGetLastError());
   const long long tiles = (n_points + 127) / 128;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const unsigned grid = (unsigned)((tiles + nfi::kGroups - 1) / nfi::kGroups < sms
@@ -526,7 +526,7 @@ int nfi_render_backward(const nfi_render_params* params, const nfi_render_grads*
                       (!p.fine_sampling || p.z_fine != nullptr) && g.out_rgb && g.out_mask &&
                       (!g.g_extra || g.out_extra) &&
                       ((g.grad_origins == nullptr) == (g.grad_dirs == nullptr));
-  // decoder-weight gradients (the GAN generator step, run.py:1044) on tcgen05 too: a second
+  // decoder-weight gradients (the GAN generator step, run.py:1044) on the tensor cores too: a second
   // kernel (render_wgrad_pipe) beside render_backward_pipe, which then sees a frozen decoder.
   // An upstream gradient of the coords output stays on the SIMT kernel.
   const bool tc_ok = tc_env && (!wgrad || (!g.g_extra &&

@@ -1,5 +1,5 @@
-// Tri-plane producer on sm_100a: the StyleGAN2 synthesis network of
-// /root/reference/models/stylegan.py:293-490 as tcgen05 implicit GEMMs (C ABI: include/nfi_synth.h).
+// Tri-plane producer on sm_90a: the StyleGAN2 synthesis network of the reference's
+// models/stylegan.py:293-490 as TMA-fed wgmma implicit GEMMs (C ABI: include/nfi_synth.h).
 //
 // Data layout.  Activations are channel-last ([B,H,W,C]) and exist as a PAIR of bf16 tensors,
 // hi = bf16(value) and lo = bf16(value - hi) (16 significant bits between them, 4 bytes per element
@@ -8,23 +8,21 @@
 // re-laid-out per call to [tap][Cout][Cin] (K-major rows for the B operand), also as hi / lo.  One
 // 3x3 tap of one 64-channel block is then ONE TMA box per operand: a [1 x 8 x 16 x 64] box of the
 // activation tensor at the tile origin shifted by the tap (out-of-range rows / columns / channels
-// arrive as zeros = the conv padding) is a 128-row x 128-byte SWIZZLE_128B tile = the K-major A
-// operand of a 128 x BN x 64 UMMA; no im2col buffer, no register staging.  D accumulates over taps
-// x channel blocks in TMEM as A_lo W_hi + A_hi W_lo + A_hi W_hi (kind::f16 on bf16 operands, fp32
-// accumulate): the dropped lo x lo term is 2^-18 of a product.  [The first version of this kernel
-// ran the same three products as 3xTF32 (kind::tf32, fp32 hi/lo pairs): twice the tensor time for
-// operands exact to 2^-22 -- but the result was no more accurate (1.35e-4 vs the fp64 network at
-// K = 9 x 512, DESIGN.md 4.8): the tensor core adds the products of one output into its fp32
-// accumulator with truncation, and that bias, which grows with K, dominates either way.]
+// arrive as zeros = the conv padding) is a 256-row x 128-byte SWIZZLE_128B tile = the K-major A
+// operand of four 64 x BN x 64 wgmma row blocks; no im2col buffer, no register staging.  D
+// accumulates over taps x channel blocks in registers as A_lo W_hi + A_hi W_lo + A_hi W_hi (bf16
+// operands, fp32 accumulate): the dropped lo x lo term is 2^-18 of a product.  (3xTF32 on fp32
+// pairs would double the tensor time for operands exact to 2^-22 without a more accurate result:
+// the tensor core adds the products of one output into its fp32 accumulator with truncation, and
+// that bias, which grows with K, dominates either way.)
 //
-// conv_tc_kernel (persistent, 320 threads):
-//   warp 0    TMA producer   : 4 boxes per k-iteration (A_hi, A_lo 32 KB each, W_hi, W_lo) into a 2-stage ring
-//   warp 1    MMA issuer     : 2 x 12 tcgen05.mma (kind::f16 / bf16, M128 N<=128 K16) per stage,
-//                              tcgen05.commit -> stage free / accumulator full
-//   warps 2-9 epilogue       : tcgen05.ld of one of the two TMEM accumulator PAIRS (the other is being
-//                              filled) -> fused epilogue -> global; two warps per TMEM lane quadrant,
-//                              half of the columns each (the ToRGB / ACT epilogues are bound by the
-//                              loads and stores in flight, not by arithmetic)
+// conv_tc_kernel (persistent, 384 threads):
+//   warpgroup 0    TMA producer : 4 boxes per k-iteration (A_hi, A_lo 32 KB each, W_hi, W_lo) into a
+//                                 2-stage ring (one elected thread)
+//   warpgroups 1-2 consumers    : rows 128c .. 128c + 127 of the position tile as two 64-row wgmma
+//                                 blocks, 24 wgmma (bf16, M64 N<=128 K16) per stage, the stage released
+//                                 once the next one's are in flight; then the fused epilogue straight
+//                                 from the accumulator registers -> global
 // Epilogues: ACT  x*dcoef + noise + bias, *sqrt(2), leaky-relu 0.2, then for up to two consumers
 //                 (next conv, ToRGB) * their style -> hi / lo           (stylegan.py:137-142,349-356)
 //            RAW  plain store at (2a+py, 2b+px) of the (2H+1)x(2W+1) transposed-conv result; the
@@ -47,11 +45,12 @@
 namespace nfi {
 namespace synth {
 
-constexpr int kTileH = 16, kTileW = 16;  // 256 output positions = two UMMA M = 128 halves (rows 0-7 / 8-15)
+constexpr int kTileH = 16, kTileW = 16;  // 256 output positions = four wgmma M = 64 blocks
 constexpr int kKBlock = 64;             // bf16 channels per k-iteration: 128-byte rows
 constexpr int kStages = 2;
 constexpr int kATile = 256 * 128;       // bytes of one A box: 256 rows of 128 bytes
-constexpr int kConvThreads = 320;      // TMA warp, MMA warp, 8 epilogue warps
+constexpr int kConvThreads = 384;      // TMA warpgroup, two consumer warpgroups
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;  // 384 x 168 = 128 x (40 + 2 x 232) + 512
 constexpr int kMaxPhases = 4, kMaxTaps = 9;
 
 enum { kModeRaw = 0, kModeAct = 1, kModeRgb = 2 };
@@ -127,23 +126,6 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(tc::smem_u32(bar)) : "memory");
 }
 
-// Instruction descriptor, kind::f16 with bf16 operands, fp32 accumulate, A and B K-major:
-//   [4,6) c_format=1 (F32)  [7,10) a_format=1 (BF16)  [10,13) b_format=1  [17,23) N>>3  [24,29) M>>4
-__device__ __forceinline__ uint32_t umma_idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_bf16_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                             uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
 struct TileCoord {
   int phase, img, ty, tx, nt;
 };
@@ -182,6 +164,34 @@ __device__ __forceinline__ void store_split4(__nv_bfloat16* hi, __nv_bfloat16* l
 }
 __device__ __forceinline__ float lrelu(float x) { return x > 0.f ? x : 0.2f * x; }
 
+// value -> (value * style) as a bf16 hi / lo pair, 2 channels (4 bytes per tensor) at a time
+__device__ __forceinline__ void store_split2(__nv_bfloat16* hi, __nv_bfloat16* lo, size_t idx,
+                                             float2 v, float2 s) {
+  __align__(4) __nv_bfloat16 h[2], l[2];
+  split_bf16(v.x * s.x, h[0], l[0]);
+  split_bf16(v.y * s.y, h[1], l[1]);
+  *reinterpret_cast<uint32_t*>(hi + idx) = *reinterpret_cast<const uint32_t*>(h);
+  *reinterpret_cast<uint32_t*>(lo + idx) = *reinterpret_cast<const uint32_t*>(l);
+}
+// The ACT epilogue on 2 consecutive channels n, n+1 of position `pos` (the conv kernel's register
+// fragments hold channel pairs).
+__device__ __forceinline__ void act_store2(const ActEpilogue& e, int img, size_t pos, int N, int n,
+                                           float2 acc, float noise) {
+  const float2 d = __ldg(reinterpret_cast<const float2*>(e.dcoef + (size_t)img * N + n));
+  const float2 b = __ldg(reinterpret_cast<const float2*>(e.bias + n));
+  float2 v;
+  v.x = lrelu(((acc.x * d.x + noise) + b.x) * e.gain);
+  v.y = lrelu(((acc.y * d.y + noise) + b.y) * e.gain);
+  const float2 one = make_float2(1.f, 1.f);
+  if (e.a_hi != nullptr) {
+    const float2 s = e.style_a ? __ldg(reinterpret_cast<const float2*>(e.style_a + (size_t)img * N + n)) : one;
+    store_split2(e.a_hi, e.a_lo, pos * N + n, v, s);
+  }
+  if (e.b_hi != nullptr) {
+    const float2 s = e.style_b ? __ldg(reinterpret_cast<const float2*>(e.style_b + (size_t)img * N + n)) : one;
+    store_split2(e.b_hi, e.b_lo, pos * N + n, v, s);
+  }
+}
 // The ACT epilogue on 4 consecutive channels n..n+3 of position `pos` (= (img*H + y)*W + x).
 __device__ __forceinline__ void act_store4(const ActEpilogue& e, int img, size_t pos, int N, int n,
                                            float4 acc, float noise) {
@@ -203,32 +213,177 @@ __device__ __forceinline__ void act_store4(const ActEpilogue& e, int img, size_t
   }
 }
 
+template <int BN>
+__device__ __forceinline__ void wgmma_bn(float (&d)[BN / 2], uint64_t a, uint64_t b) {
+  if constexpr (BN == 32) tc::wgmma_bf16_ss_n32<0, 0>(d, a, b, 1);
+  else if constexpr (BN == 64) tc::wgmma_bf16_ss_n64<0, 0>(d, a, b, 1);
+  else if constexpr (BN == 96) tc::wgmma_bf16_ss_n96<0, 0>(d, a, b, 1);
+  else tc::wgmma_bf16_ss_n128<0, 0>(d, a, b, 1);
+}
+
+// Consumer warpgroup c (0, 1): rows 128c .. 128c + 127 of each position tile, BN columns.
+template <int BN>
+__device__ __forceinline__ void conv_consume(const ConvArgs& a, int n_tiles, unsigned char* smem,
+                                             uint64_t* full, uint64_t* empty, float4* skip_sm,
+                                             int c, int ctid) {
+  const int lane = ctid & 31, warp = ctid >> 5 & 3;
+  const int g4 = lane >> 2, t = lane & 3;
+  const int w_tile = BN * 128;
+  const int stage_bytes = 2 * kATile + 2 * w_tile;
+  const int kblocks = (a.C + kKBlock - 1) / kKBlock;  // a partial last block is zero-filled by TMA
+  const uint32_t smem_s = tc::smem_u32(smem);
+  uint32_t st = 0, ph = 0;
+  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const TileCoord tl = decode_tile(a, tile);
+    const int n0 = tl.nt * BN;
+    const bool staged = (a.mode == kModeRgb) && (a.skip != nullptr);
+    if (staged) {
+      // before the MMAs of this tile: the 10x10 low-resolution footprint of the tile, zeros
+      // outside the image (a missing neighbour contributes nothing, stylegan.py:71-75)
+      const int hh = a.H >> 1, hw = a.W >> 1;
+      const int gy0 = tl.ty * (kTileH / 2) - 1, gx0 = tl.tx * (kTileW / 2) - 1;
+      const int c4n = a.N >> 2;   // float4 per position (24)
+      tc::bar_sync(1, 256);       // the previous tile's readers are done
+      for (int i = ctid; i < kSkipDim * kSkipDim * c4n; i += 256) {
+        const int pxl = i / c4n, c4 = i - pxl * c4n;
+        const int gy = gy0 + pxl / kSkipDim, gx = gx0 + pxl % kSkipDim;
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (gy >= 0 && gy < hh && gx >= 0 && gx < hw)
+          v = __ldg(reinterpret_cast<const float4*>(a.skip + (((size_t)tl.img * hh + gy) * hw + gx) * a.N) + c4);
+        skip_sm[pxl * kSkipRow4 + c4] = v;
+      }
+      tc::bar_sync(1, 256);
+    }
+    float acc[2][BN / 2];
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[mb][i] = 0.f;
+    tc::wgmma_fence();
+    const int iters = a.ph_taps[tl.phase] * kblocks;
+    uint32_t prev_st = 0;
+    for (int k = 0; k < iters; ++k) {
+      tc::mbar_wait(&full[st], ph);
+      const uint32_t sb = smem_s + st * stage_bytes;
+      const uint64_t w_hi = tc::gmma_desc_sw128(sb + 2 * kATile);
+      const uint64_t w_lo = tc::gmma_desc_sw128(sb + 2 * kATile + w_tile);
+      // the W boxes of the stage serve both row blocks of this warpgroup
+#pragma unroll
+      for (int mb = 0; mb < 2; ++mb) {
+        const uint32_t rows = (uint32_t)(128 * c + 64 * mb) * 128;
+        const uint64_t a_hi = tc::gmma_desc_sw128(sb + rows);
+        const uint64_t a_lo = tc::gmma_desc_sw128(sb + kATile + rows);
+        // small terms first; a K step of 16 bf16 = 32 bytes = +2 in the descriptor's address field
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) wgmma_bn<BN>(acc[mb], a_lo + 2 * ks, w_hi + 2 * ks);
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) wgmma_bn<BN>(acc[mb], a_hi + 2 * ks, w_lo + 2 * ks);
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) wgmma_bn<BN>(acc[mb], a_hi + 2 * ks, w_hi + 2 * ks);
+      }
+      tc::wgmma_commit();
+      // the previous stage's products are complete once at most this one's are in flight
+      tc::wgmma_wait<1>();
+      if (k > 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[prev_st]);
+      }
+      prev_st = st;
+      if (++st == kStages) { st = 0; ph ^= 1; }
+    }
+    tc::wgmma_wait<0>();
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb) tc::reg_fence(acc[mb]);
+    __syncwarp();
+    if (iters > 0 && lane == 0) mbar_arrive(&empty[prev_st]);
+
+    // ================================ EPILOGUE ================================
+    const float* skipf = reinterpret_cast<const float*>(skip_sm);
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb) {
+#pragma unroll
+      for (int half = 0; half < 2; ++half) {
+        const int row = 128 * c + 64 * mb + 16 * warp + g4 + 8 * half;  // position (row / 16, row % 16)
+        const int y = tl.ty * kTileH + row / kTileW, x = tl.tx * kTileW + row % kTileW;
+        const bool valid = (y < a.ph_DH[tl.phase]) && (x < a.ph_DW[tl.phase]);
+        if (!valid) continue;
+        float noise = 0.f;
+        size_t pos = 0;
+        float wsk[4] = {0.f, 0.f, 0.f, 0.f};
+        int psk[4] = {0, 0, 0, 0};
+        if (a.mode == kModeRaw) {
+          const int oy = a.out_stride * y + a.ph_oy[tl.phase], ox = a.out_stride * x + a.ph_ox[tl.phase];
+          pos = ((size_t)tl.img * a.out_H + oy) * a.out_W + ox;
+        } else {
+          pos = ((size_t)tl.img * a.H + y) * a.W + x;
+          if (a.mode == kModeAct && a.act.noise != nullptr) noise = __ldg(a.act.noise + pos);
+          if (staged) {
+            // upsample2d (stylegan.py:71-75): out[2i] = 3/4 in[i] + 1/4 in[i-1], out[2i+1] = 3/4 in[i]
+            // + 1/4 in[i+1] per axis; positions inside the staged footprint (its origin is one
+            // low-res position up / left of the tile); out-of-image neighbours are staged as zeros,
+            // so the weights need no masking
+            const int iy = y >> 1, ix = x >> 1;
+            const int jy = (y & 1) ? iy + 1 : iy - 1, jx = (x & 1) ? ix + 1 : ix - 1;
+            const int ly = iy - (tl.ty * (kTileH / 2) - 1), lx = ix - (tl.tx * (kTileW / 2) - 1);
+            const int my = jy - (tl.ty * (kTileH / 2) - 1), mx = jx - (tl.tx * (kTileW / 2) - 1);
+            wsk[0] = 0.75f * 0.75f; psk[0] = ly * kSkipDim + lx;
+            wsk[1] = 0.75f * 0.25f; psk[1] = ly * kSkipDim + mx;
+            wsk[2] = 0.25f * 0.75f; psk[2] = my * kSkipDim + lx;
+            wsk[3] = 0.25f * 0.25f; psk[3] = my * kSkipDim + mx;
+          }
+        }
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          float2 v = make_float2(acc[mb][4 * j + 2 * half], acc[mb][4 * j + 2 * half + 1]);
+          const int nn = n0 + 8 * j + 2 * t;
+          if (a.mode == kModeRaw) {
+            *reinterpret_cast<float2*>(a.out_raw + pos * a.N + nn) = v;
+          } else if (a.mode == kModeAct) {
+            act_store2(a.act, tl.img, pos, a.N, nn, v, noise);
+          } else {
+            const float2 b = __ldg(reinterpret_cast<const float2*>(a.act.bias + nn));
+            v.x += b.x;
+            v.y += b.y;
+            if (staged) {
+#pragma unroll
+              for (int q = 0; q < 4; ++q) {
+                const float2 k2 = *reinterpret_cast<const float2*>(skipf + (psk[q] * kSkipRow4) * 4 + nn);
+                v.x = fmaf(wsk[q], k2.x, v.x);
+                v.y = fmaf(wsk[q], k2.y, v.y);
+              }
+            }
+            if (a.img != nullptr) *reinterpret_cast<float2*>(a.img + pos * a.N + nn) = v;
+            if (a.planes != nullptr) {
+              const int pl = nn >> 5, ch = nn & 31;
+              const size_t o = ((((size_t)tl.img * 3 + pl) * a.H + y) * a.W + x) * 32 + ch;
+              *reinterpret_cast<float2*>(a.planes + o) = v;
+            }
+          }
+        }
+      }
+    }
+  }
+}
+
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
                const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl,
                const __grid_constant__ ConvArgs a, int n_tiles) {
   extern __shared__ __align__(1024) unsigned char smem[];
-  const int tid = threadIdx.x, lane = tid & 31;
-  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
+  const int tid = threadIdx.x;
+  const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);
   const int w_tile = a.BN * 128;                 // bytes of one W box
   const int stage_bytes = 2 * kATile + 2 * w_tile;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * stage_bytes);
   uint64_t* full = bars;                // [kStages] TMA landed
-  uint64_t* empty = full + kStages;     // [kStages] MMAs of the stage complete
-  uint64_t* acc_full = empty + kStages; // [2]
-  uint64_t* acc_empty = acc_full + 2;   // [2]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(acc_empty + 2);
+  uint64_t* empty = full + kStages;     // [kStages] wgmma of the stage complete (8 consumer warps)
   float4* skip_sm = reinterpret_cast<float4*>(smem + kStages * stage_bytes + 128);  // RGB + skip only
 
   if (tid == 0) {
     if (tc::smem_u32(smem) & 1023u) __trap();
     for (int i = 0; i < kStages; ++i) {
       tc::mbar_init(&full[i], 1);
-      tc::mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      tc::mbar_init(&acc_full[i], 1);
-      tc::mbar_init(&acc_empty[i], 8);
+      tc::mbar_init(&empty[i], 8);
     }
     tc::fence_mbar_init();
     prefetch_tmap(&tmAh);
@@ -236,16 +391,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
     prefetch_tmap(&tmWh);
     prefetch_tmap(&tmWl);
   }
-  if (warp == 1) tc::tmem_alloc(tmem_ptr, 512);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   const int kblocks = (a.C + kKBlock - 1) / kKBlock;  // a partial last block is zero-filled by TMA
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ================================ TMA PRODUCER ================================
-    if (elect_one()) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
+    if (tid < 32 && elect_one()) {
       uint32_t st = 0, ph = 0;
       for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const TileCoord t = decode_tile(a, tile);
@@ -266,157 +418,17 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
         }
       }
     }
-  } else if (warp == 1) {
-    // ================================ MMA ISSUER ================================
-    const uint32_t idesc = umma_idesc_bf16(128, a.BN);
-    const uint32_t smem_s = tc::smem_u32(smem);
-    uint32_t st = 0, ph = 0, it = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-      const TileCoord t = decode_tile(a, tile);
-      const uint32_t acc = it & 1;
-      tc::mbar_wait(&acc_empty[acc], ((it >> 1) & 1) ^ 1);
-      tc::tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * 256;  // two 128-column accumulators: rows 0-127, 128-255
-      const int iters = a.ph_taps[t.phase] * kblocks;
-      for (int k = 0; k < iters; ++k) {
-        tc::mbar_wait(&full[st], ph);
-        tc::tc_fence_after();
-        if (elect_one()) {
-          const uint32_t sb = smem_s + st * stage_bytes;
-          const uint64_t w_hi = tc::umma_desc_sw128(sb + 2 * kATile);
-          const uint64_t w_lo = tc::umma_desc_sw128(sb + 2 * kATile + w_tile);
-          // the W boxes of the stage serve both halves of the position tile
-#pragma unroll
-          for (int sub = 0; sub < 2; ++sub) {
-            const uint64_t a_hi = tc::umma_desc_sw128(sb + sub * (kATile / 2));
-            const uint64_t a_lo = tc::umma_desc_sw128(sb + kATile + sub * (kATile / 2));
-            const uint32_t d = d_tmem + sub * 128;
-            // small terms first; a K step of 16 bf16 = 32 bytes = +2 in the descriptor's address field
-#pragma unroll
-            for (int ks = 0; ks < 4; ++ks)
-              umma_bf16_ss(d, a_lo + 2 * ks, w_hi + 2 * ks, idesc, (k | ks) ? 1u : 0u);
-#pragma unroll
-            for (int ks = 0; ks < 4; ++ks) umma_bf16_ss(d, a_hi + 2 * ks, w_lo + 2 * ks, idesc, 1u);
-#pragma unroll
-            for (int ks = 0; ks < 4; ++ks) umma_bf16_ss(d, a_hi + 2 * ks, w_hi + 2 * ks, idesc, 1u);
-          }
-          tc::umma_commit(&empty[st]);
-          if (k == iters - 1) tc::umma_commit(&acc_full[acc]);
-        }
-        __syncwarp();
-        if (++st == kStages) { st = 0; ph ^= 1; }
-      }
-    }
   } else {
-    // ================================ EPILOGUE ================================
-    const int q = warp & 3;                 // TMEM lane quadrant this warp may read
-    const int half = (warp - 2) >> 2;       // which half of the tile's columns this warp handles
-    const int chunks = a.BN / 32;           // 16-column chunks per half (BN = 32, 64, 96, 128)
-    const int row = 32 * q + lane;          // row of a half tile = position (row / 16, row % 16)
-    const int py = row / kTileW, px = row % kTileW;
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-      const TileCoord t = decode_tile(a, tile);
-      const uint32_t acc = it & 1;
-      const int n0 = t.nt * a.BN;
-      const bool staged = (a.mode == kModeRgb) && (a.skip != nullptr);
-      if (staged) {
-        // while the MMAs of this tile run: the 10x10 low-resolution footprint of the tile, zeros
-        // outside the image (a missing neighbour contributes nothing, stylegan.py:71-75)
-        const int hh = a.H >> 1, hw = a.W >> 1;
-        const int gy0 = t.ty * (kTileH / 2) - 1, gx0 = t.tx * (kTileW / 2) - 1;
-        const int c4n = a.N >> 2;   // float4 per position (24)
-        tc::bar_sync(1, 256);       // the previous tile's readers are done
-        for (int i = tid - 64; i < kSkipDim * kSkipDim * c4n; i += 256) {
-          const int pxl = i / c4n, c4 = i - pxl * c4n;
-          const int gy = gy0 + pxl / kSkipDim, gx = gx0 + pxl % kSkipDim;
-          float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (gy >= 0 && gy < hh && gx >= 0 && gx < hw)
-            v = __ldg(reinterpret_cast<const float4*>(a.skip + (((size_t)t.img * hh + gy) * hw + gx) * a.N) + c4);
-          skip_sm[pxl * kSkipRow4 + c4] = v;
-        }
-        tc::bar_sync(1, 256);
-      }
-      tc::mbar_wait(&acc_full[acc], (it >> 1) & 1);
-      tc::tc_fence_after();
-#pragma unroll 1
-      for (int sub = 0; sub < 2; ++sub) {
-      const int y = t.ty * kTileH + 8 * sub + py, x = t.tx * kTileW + px;
-      const bool valid = (y < a.ph_DH[t.phase]) && (x < a.ph_DW[t.phase]);
-      const uint32_t taddr = tmem_base + acc * 256 + sub * 128 + ((uint32_t)(32 * q) << 16);
-      float noise = 0.f;
-      size_t pos = 0;
-      float wsk[4] = {0.f, 0.f, 0.f, 0.f};
-      size_t psk[4] = {0, 0, 0, 0};
-      if (a.mode == kModeRaw) {
-        const int oy = a.out_stride * y + a.ph_oy[t.phase], ox = a.out_stride * x + a.ph_ox[t.phase];
-        pos = ((size_t)t.img * a.out_H + oy) * a.out_W + ox;
-      } else {
-        pos = ((size_t)t.img * a.H + y) * a.W + x;
-        if (a.mode == kModeAct && a.act.noise != nullptr && valid) noise = __ldg(a.act.noise + pos);
-        if (a.mode == kModeRgb && a.skip != nullptr && valid) {
-          // upsample2d (stylegan.py:71-75): out[2i] = 3/4 in[i] + 1/4 in[i-1], out[2i+1] = 3/4 in[i]
-          // + 1/4 in[i+1] per axis, missing neighbours contribute nothing
-          const int hh = a.H >> 1, hw = a.W >> 1;
-          const int iy = y >> 1, ix = x >> 1;
-          const int jy = (y & 1) ? iy + 1 : iy - 1, jx = (x & 1) ? ix + 1 : ix - 1;
-          const float wy1 = (jy >= 0 && jy < hh) ? 0.25f : 0.f, wx1 = (jx >= 0 && jx < hw) ? 0.25f : 0.f;
-          const int cy = min(max(jy, 0), hh - 1), cx = min(max(jx, 0), hw - 1);
-          // positions inside the staged footprint (its origin is one low-res position up / left of
-          // the tile); out-of-image neighbours are staged as zeros, so the weights need no masking
-          const int ly = iy - (t.ty * (kTileH / 2) - 1), lx = ix - (t.tx * (kTileW / 2) - 1);
-          const int my = jy - (t.ty * (kTileH / 2) - 1), mx = jx - (t.tx * (kTileW / 2) - 1);
-          (void)wy1; (void)wx1; (void)cy; (void)cx;
-          wsk[0] = 0.75f * 0.75f; psk[0] = (size_t)(ly * kSkipDim + lx);
-          wsk[1] = 0.75f * 0.25f; psk[1] = (size_t)(ly * kSkipDim + mx);
-          wsk[2] = 0.25f * 0.75f; psk[2] = (size_t)(my * kSkipDim + lx);
-          wsk[3] = 0.25f * 0.25f; psk[3] = (size_t)(my * kSkipDim + mx);
-        }
-      }
-      for (int j = half * chunks; j < (half + 1) * chunks; ++j) {
-        float v[16];
-        tc::tmem_ld16(taddr + 16 * j, v);
-        if (!valid) continue;
-        const int n = n0 + 16 * j;
-#pragma unroll
-        for (int i4 = 0; i4 < 4; ++i4) {
-          float4 acc4 = make_float4(v[4 * i4], v[4 * i4 + 1], v[4 * i4 + 2], v[4 * i4 + 3]);
-          const int nn = n + 4 * i4;
-          if (a.mode == kModeRaw) {
-            *reinterpret_cast<float4*>(a.out_raw + pos * a.N + nn) = acc4;
-          } else if (a.mode == kModeAct) {
-            act_store4(a.act, t.img, pos, a.N, nn, acc4, noise);
-          } else {
-            const float4 b = __ldg(reinterpret_cast<const float4*>(a.act.bias + nn));
-            acc4.x += b.x; acc4.y += b.y; acc4.z += b.z; acc4.w += b.w;
-            if (a.skip != nullptr) {
-#pragma unroll
-              for (int s = 0; s < 4; ++s) {
-                const float4 k = skip_sm[psk[s] * kSkipRow4 + (nn >> 2)];
-                acc4.x = fmaf(wsk[s], k.x, acc4.x);
-                acc4.y = fmaf(wsk[s], k.y, acc4.y);
-                acc4.z = fmaf(wsk[s], k.z, acc4.z);
-                acc4.w = fmaf(wsk[s], k.w, acc4.w);
-              }
-            }
-            if (a.img != nullptr) *reinterpret_cast<float4*>(a.img + pos * a.N + nn) = acc4;
-            if (a.planes != nullptr) {
-              const int pl = nn >> 5, ch = nn & 31;
-              const size_t o = ((((size_t)t.img * 3 + pl) * a.H + y) * a.W + x) * 32 + ch;
-              *reinterpret_cast<float4*>(a.planes + o) = acc4;
-            }
-          }
-        }
-      }
-      }
-      tc::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[acc]);
+    // ================================ CONSUMERS ================================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
+    const int c = wg - 1, ctid = tid - 128;
+    switch (a.BN) {
+      case 32: conv_consume<32>(a, n_tiles, smem, full, empty, skip_sm, c, ctid); break;
+      case 64: conv_consume<64>(a, n_tiles, smem, full, empty, skip_sm, c, ctid); break;
+      case 96: conv_consume<96>(a, n_tiles, smem, full, empty, skip_sm, c, ctid); break;
+      default: conv_consume<128>(a, n_tiles, smem, full, empty, skip_sm, c, ctid); break;
     }
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tc::tmem_dealloc(tmem_base, 512);
 }
 
 // 4x4 FIR (outer([1,3,3,1]) / 16 = the reference's filter * gain 4, pad 1) over the (2H+1)x(2W+1)
@@ -598,7 +610,7 @@ struct Pair {
 
 static int sm_count() {
   static int n = []() {
-    int dev = 0, v = 148;
+    int dev = 0, v = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
     return v;
@@ -807,7 +819,7 @@ static int run(const nfi_synth_params& P, Bump& ws, cudaStream_t st, bool dry, c
         e.style_a = style1[i]; e.a_hi = y.hi; e.a_lo = y.lo;
         const size_t total = (size_t)B * (res / 2) * (res / 2) * (cout / 4);
         unsigned grid = blocks(total, 256);
-        if (grid > 148u * 16u) grid = 148u * 16u;
+        if (grid > (unsigned)sm_count() * 16u) grid = (unsigned)sm_count() * 16u;
         fir_act_kernel<<<grid, 256, 0, st>>>(raw, B, res, res, cout, e);
         NFI_SCUDA(cudaGetLastError());
       }

@@ -1,16 +1,20 @@
-// tcgen05 / TMEM / mbarrier / TMA-bulk primitives used by the tensor-core
-// variant of the decoder MLP (sm_100a only; hand-written PTX, no CUTLASS).
+// Hopper (sm_90a) tensor-core, mbarrier and TMA-bulk primitives of the tensor-core kernels
+// (hand-written PTX, no CUTLASS).
 //
 // Layer 1 of the decoder (models/generator.py:294-299: Linear(32->64)) runs as
-// D[128 points x 64] = A[128 x 32] * W1^T on the 5th-generation tensor cores
-// with fp32 accuracy recovered by the hi/lo split ("3xTF32"):
+// D[128 points x 64] = A[128 x 32] * W1^T on the tensor cores (wgmma, two M = 64 halves per
+// warpgroup) with fp32 accuracy recovered by the hi/lo split ("3xTF32"):
 //     a = a_hi + a_lo,  a_hi = a with the low 13 mantissa bits cleared (exactly
 //     representable in TF32), a_lo = a - a_hi (exact in fp32);
 //     A*W ~= A_lo*W_hi + A_hi*W_lo + A_hi*W_hi       (error ~2^-21 relative)
-// Operands live in shared memory in the canonical K-major SWIZZLE_128B layout
-// (a row of 32 fp32 = 128 B = one swizzle row; 8 rows = one 1024-B atom); the
-// accumulator lives in TMEM (lane = point, column = hidden unit) and is read
-// back with tcgen05.ld for the softplus / layer-2 epilogue.
+// Operands live in shared memory in the canonical K-major SWIZZLE_128B layout (a row of 32 fp32 =
+// 128 B = one swizzle row; 8 rows = one 1024-B atom); the accumulator lives in the registers of
+// the warpgroup that issued the wgmma.  The softplus epilogue works on those registers and hands
+// the hidden activations straight back to layer 2 as register A fragments (wgmma's A operand may
+// come from registers): a fragment holds, in each k-block of 8, the hidden units 8kb + 2t and
+// 8kb + 2t + 1 of lane t = lane % 4, which wgmma reads as K positions t and t + 4.  The B operand
+// of every GEMM whose A is such a fragment is stored with its K positions permuted to match
+// (kpos_of_hidden below).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -71,7 +75,10 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
                "r"(bytes)
                : "memory");
 }
-// TMA bulk copy global -> shared (SASS: UBLKCP), completion on an mbarrier.
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+// TMA bulk copy global -> shared, completion on an mbarrier.
 __device__ __forceinline__ void tma_bulk_g2s(void* dst_smem, const void* src_gmem, uint32_t bytes,
                                              uint64_t* bar) {
   asm volatile(
@@ -82,138 +89,168 @@ __device__ __forceinline__ void tma_bulk_g2s(void* dst_smem, const void* src_gme
 }
 
 // ------------------------------------------------------------- fences
-// generic-proxy shared-memory writes -> visible to the async proxy (UMMA reads)
+// generic-proxy shared-memory writes -> visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 }
 // named barrier over `count` threads (ids 1..15; 0 is __syncthreads)
 __device__ __forceinline__ void bar_sync(uint32_t id, uint32_t count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
-// ------------------------------------------------------------- TMEM
-// One warp allocates `ncols` (power of two >= 32) and publishes the base
-// address through shared memory.
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-
-// 16 consecutive fp32 columns of this thread's TMEM lane (lane = 32*(warp%4)+laneid)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-// same without the wait: issue several, then tmem_wait_ld() once
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const float (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-      "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])),
-      "r"(__float_as_uint(v[3])), "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])),
-      "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])), "r"(__float_as_uint(v[8])),
-      "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-      "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])),
-      "r"(__float_as_uint(v[15]))
-      : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-
-// ------------------------------------------------------------- UMMA
-// Shared-memory matrix descriptor, K-major, SWIZZLE_128B, fp32 rows of 128 B:
-//   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4 (=1)
-//   bits [32,46) stride byte offset >> 4 (1024 B between 8-row groups)
-//   bits [46,48) version = 1 (sm_100)      bits [61,64) layout = 2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
+// ------------------------------------------------------------- wgmma
+// Shared-memory matrix descriptor (sm_90): bits [0,14) start address >> 4, [16,30) leading byte
+// offset >> 4, [32,46) stride byte offset >> 4, [62,64) layout: 1 = SWIZZLE_128B, 2 = SWIZZLE_64B,
+// 3 = SWIZZLE_32B.  K-major: rows = M / N, `sbo` = bytes between 8-row groups (the leading offset
+// is unused).  MN-major: rows = K, a row holds 64 / 32 / 16 elements of M / N, `lbo` = bytes
+// between such atoms along M / N, `sbo` = bytes between 8-row K groups.  A K step inside a
+// swizzle atom adds its byte offset >> 4 to the start address.
+constexpr uint32_t kSw128 = 1, kSw64 = 2, kSw32 = 3;
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t smem_addr, uint32_t layout, uint32_t lbo,
+                                              uint32_t sbo) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
+  d |= (uint64_t)((sbo >> 4) & 0x3FFF) << 32;
+  d |= (uint64_t)layout << 62;
   return d;
 }
-
-// Instruction descriptor, kind::tf32, fp32 accumulate, A and B K-major:
-//   [4,6) c_format=1 (F32)  [7,10) a_format=2 (TF32)  [10,13) b_format=2
-//   [17,23) N>>3            [24,29) M>>4
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) |
-         ((uint32_t)(M >> 4) << 24);
+// K-major, SWIZZLE_128B, 1024 B between 8-row groups: the fp32 [rows x 32] tiles of this project
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr) {
+  return gmma_desc(smem_addr, kSw128, 16, 1024);
+}
+__device__ __forceinline__ void wgmma_fence() {
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+}
+__device__ __forceinline__ void wgmma_commit() {
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+}
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// register fragments must not be touched by the compiler across an in-flight wgmma
+template <int R>
+__device__ __forceinline__ void reg_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// D[tmem] (+)= A[smem] * B[smem]^T ; issued by ONE thread.
-__device__ __forceinline__ void umma_tf32_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                             uint32_t idesc, uint32_t accumulate) {
+// wgmma wrappers: D[64 x N] (+)= A[64 x K] * B[K x N], fp32 accumulators in registers
+// (fragment layout of the PTX ISA: warp w of the warpgroup holds rows 16w + lane/4 and
+// 16w + lane/4 + 8, columns 8j + 2 (lane % 4) + {0, 1}: d[4j .. 4j+3]).
+
+__device__ __forceinline__ void wgmma_tf32_ss_n64(float (&d)[32], uint64_t a, uint64_t b, int acc) {
   asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(acc)
       : "memory");
 }
-// D[tmem] (+)= A[tmem] * B[smem]^T : A read from TMEM (lane = row, one 32-bit
-// column per K element), no output lane disabled.
-__device__ __forceinline__ void umma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc,
-                                             uint32_t idesc, uint32_t accumulate) {
+
+__device__ __forceinline__ void wgmma_tf32_rs_n16(float (&d)[8], const uint32_t (&a)[4], uint64_t b,
+                                                   int acc) {
   asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, {%5, %5, %5, %5}, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate), "r"(0u)
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %13, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc)
       : "memory");
 }
-// All MMAs issued so far by this thread arrive on `bar` when they complete.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::
-                   "r"(smem_u32(bar))
-               : "memory");
+
+__device__ __forceinline__ void wgmma_tf32_rs_n32(float (&d)[16], const uint32_t (&a)[4], uint64_t b,
+                                                   int acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %21, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc)
+      : "memory");
+}
+
+__device__ __forceinline__ void wgmma_tf32_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t b,
+                                                   int acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc)
+      : "memory");
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16_ss_n8(float (&d)[4], uint64_t a, uint64_t b, int acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %6, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n8k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3}, %4, %5, p, 1, 1, %7, %8;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB)
+      : "memory");
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16_ss_n16(float (&d)[8], uint64_t a, uint64_t b, int acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB)
+      : "memory");
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16_ss_n32(float (&d)[16], uint64_t a, uint64_t b, int acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB)
+      : "memory");
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16_ss_n64(float (&d)[32], uint64_t a, uint64_t b, int acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB)
+      : "memory");
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16_ss_n96(float (&d)[48], uint64_t a, uint64_t b, int acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %50, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, %51, %52;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+      : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB)
+      : "memory");
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16_ss_n128(float (&d)[64], uint64_t a, uint64_t b, int acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB)
+      : "memory");
 }
 
 // byte offset of (row, 16-byte chunk) inside a [rows x 128 B] SWIZZLE_128B tile
-__device__ __forceinline__ uint32_t sw128_offset(int row, int chunk) {
+__host__ __device__ __forceinline__ uint32_t sw128_offset(int row, int chunk) {
   return (uint32_t)((row >> 3) * 1024 + (row & 7) * 128 + ((chunk ^ (row & 7)) << 4));
 }
 
@@ -226,124 +263,22 @@ __device__ __forceinline__ uint32_t sw32_offset(int row, int chunk) {
   return (uint32_t)(row * 32 + ((chunk ^ ((row >> 2) & 1)) << 4));
 }
 
-__device__ __forceinline__ float tf32_hi(float x) {
+__host__ __device__ __forceinline__ float tf32_hi(float x) {
+#ifdef __CUDA_ARCH__
   return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u);
+#else
+  return x;
+#endif
 }
 
-// accumulate / overwrite variants without the setp (the flag is known at compile time)
-template <bool ACC>
-__device__ __forceinline__ void umma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                        uint32_t idesc) {
-  if (ACC)
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.eq.u32 p, 0, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc)
-        : "memory");
-  else
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.u32 p, 0, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc)
-        : "memory");
+// K position, inside its block of 8, at which a register A fragment holds hidden unit j (see the
+// header): units 2t and 2t + 1 of the block sit at positions t and t + 4
+__host__ __device__ constexpr int kpos_of_hidden(int j) {
+  return (j & ~7) | ((j & 1) ? 4 + ((j >> 1) & 3) : ((j >> 1) & 3));
 }
-template <bool ACC>
-__device__ __forceinline__ void umma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc,
-                                        uint32_t idesc) {
-  if (ACC)
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.eq.u32 p, 0, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, {%4, %4, %4, %4}, p;\n}\n" ::"r"(
-            d_tmem),
-        "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(0u)
-        : "memory");
-  else
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.u32 p, 0, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, {%4, %4, %4, %4}, p;\n}\n" ::"r"(
-            d_tmem),
-        "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(0u)
-        : "memory");
-}
-
-// Issues the 12 MMAs of one 128x64x32 3xTF32 product (small terms first).
-// Arguments are descriptor BASES (umma_desc_sw128 of the tile start); a K-step
-// of 8 tf32 = 32 bytes adds 2 to the start-address field.
-__device__ __forceinline__ void issue_layer1_d(uint32_t d_tmem, uint64_t a_hi, uint64_t a_lo,
-                                               uint64_t w_hi, uint64_t w_lo) {
-  constexpr uint32_t idesc = umma_idesc_tf32(128, 64);
-  umma_ss<false>(d_tmem, a_lo, w_hi, idesc);
-#pragma unroll
-  for (int ks = 1; ks < 4; ++ks) umma_ss<true>(d_tmem, a_lo + 2 * ks, w_hi + 2 * ks, idesc);
-#pragma unroll
-  for (int ks = 0; ks < 4; ++ks) umma_ss<true>(d_tmem, a_hi + 2 * ks, w_lo + 2 * ks, idesc);
-#pragma unroll
-  for (int ks = 0; ks < 4; ++ks) umma_ss<true>(d_tmem, a_hi + 2 * ks, w_hi + 2 * ks, idesc);
-}
-// D2 = H_lo*W2_hi (TS) + H_hi*W2_lo (SS) + H_hi*W2_hi (SS); H_hi k-block 1 is
-// 16 KB (1024 descriptor units) after k-block 0, W2 k-block 1 is 2 KB (128) after.
-__device__ __forceinline__ void issue_layer2_d(uint32_t d2_tmem, uint32_t hlo_tmem, uint64_t hhi,
-                                               uint64_t w2_hi, uint64_t w2_lo) {
-  constexpr uint32_t idesc = umma_idesc_tf32(128, 16);
-  umma_ts<false>(d2_tmem, hlo_tmem, w2_hi, idesc);
-#pragma unroll
-  for (int ks = 1; ks < 8; ++ks)
-    umma_ts<true>(d2_tmem, hlo_tmem + 8 * ks, w2_hi + (ks >> 2) * 128 + (ks & 3) * 2, idesc);
-#pragma unroll
-  for (int ks = 0; ks < 8; ++ks)
-    umma_ss<true>(d2_tmem, hhi + (ks >> 2) * 1024 + (ks & 3) * 2,
-                  w2_lo + (ks >> 2) * 128 + (ks & 3) * 2, idesc);
-#pragma unroll
-  for (int ks = 0; ks < 8; ++ks)
-    umma_ss<true>(d2_tmem, hhi + (ks >> 2) * 1024 + (ks & 3) * 2,
-                  w2_hi + (ks >> 2) * 128 + (ks & 3) * 2, idesc);
-}
-
-// Issues the 12 MMAs of one 128x64x32 3xTF32 product (small terms first).
-// a_hi/a_lo: [128 x 32] tiles, w_hi/w_lo: [64 x 32] tiles (shared addresses).
-__device__ __forceinline__ void issue_layer1(uint32_t d_tmem, uint32_t a_hi, uint32_t a_lo,
-                                             uint32_t w_hi, uint32_t w_lo) {
-  constexpr uint32_t idesc = umma_idesc_tf32(128, 64);
-  uint32_t acc = 0;
-#pragma unroll
-  for (int term = 0; term < 3; ++term) {
-    const uint32_t a = (term == 0) ? a_lo : a_hi;
-    const uint32_t w = (term == 1) ? w_lo : w_hi;
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {  // K = 32 = 4 x (8 tf32 = 32 bytes)
-      umma_tf32_ss(d_tmem, umma_desc_sw128(a + 32 * ks), umma_desc_sw128(w + 32 * ks), idesc,
-                   acc);
-      acc = 1;
-    }
-  }
-}
-
-// Layer 2 (64 -> 16 padded outputs), 3xTF32 with the hidden activations split
-// as H = H_hi + H_lo: H_hi lives in shared memory (two [128 x 32] K-blocks in
-// the space of the layer-1 A tiles), H_lo lives in TMEM where D1 was.
-//   D2 = H_lo*W2_hi (TS) + H_hi*W2_lo (SS) + H_hi*W2_hi (SS)
-// w2_hi / w2_lo: [16 x 64] fp32 as two [16 x 32] K-blocks of 2048 bytes.
-__device__ __forceinline__ void issue_layer2(uint32_t d2_tmem, uint32_t hlo_tmem, uint32_t hhi_k0,
-                                             uint32_t hhi_k1, uint32_t w2_hi, uint32_t w2_lo) {
-  constexpr uint32_t idesc = umma_idesc_tf32(128, 16);
-  uint32_t acc = 0;
-#pragma unroll
-  for (int ks = 0; ks < 8; ++ks) {  // K = 64 = 8 x 8
-    const uint32_t wb = w2_hi + (ks >> 2) * 2048 + (ks & 3) * 32;
-    umma_tf32_ts(d2_tmem, hlo_tmem + 8 * ks, umma_desc_sw128(wb), idesc, acc);
-    acc = 1;
-  }
-#pragma unroll
-  for (int term = 0; term < 2; ++term) {
-    const uint32_t w = (term == 0) ? w2_lo : w2_hi;
-#pragma unroll
-    for (int ks = 0; ks < 8; ++ks) {
-      const uint32_t a = ((ks >> 2) ? hhi_k1 : hhi_k0) + (ks & 3) * 32;
-      const uint32_t wb = w + (ks >> 2) * 2048 + (ks & 3) * 32;
-      umma_tf32_ss(d2_tmem, umma_desc_sw128(a), umma_desc_sw128(wb), idesc, 1);
-    }
-  }
-}
+// accumulator register e of a column block (rows g / g + 8, columns 2t / 2t + 1) -> A-fragment
+// register of the same element: a0 = (g, t), a1 = (g + 8, t), a2 = (g, t + 4), a3 = (g + 8, t + 4)
+__host__ __device__ constexpr int afrag_slot(int e) { return ((e & 1) << 1) | (e >> 1); }
 
 __device__ __forceinline__ void prefetch_l1(const void* p) {
   asm volatile("prefetch.global.L1 [%0];" ::"l"(p));
@@ -360,50 +295,93 @@ __device__ __forceinline__ float lg2_approx(float x) {
   return y;
 }
 
-// ------------------------------------------------------------- 16-bit operands (kind::f16)
 // two floats -> packed bf16 pair (round-to-nearest-even), `lo` in the low half (lower address)
 __device__ __forceinline__ uint32_t bf16x2_rn(float lo, float hi) {
   uint32_t y;
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(y) : "f"(hi), "f"(lo));
   return y;
 }
-// Shared-memory matrix descriptors for 16-bit operands.  `layout`: 2 = SWIZZLE_128B (128-byte
-// rows), 4 = SWIZZLE_64B (64-byte rows), 6 = SWIZZLE_32B (32-byte rows).  K-major: rows = M / N,
-// `sbo` = bytes between 8-row groups.  MN-major: rows = K, a row holds 64 / 32 / 16 elements of
-// M / N; `lbo` = bytes between such atoms along M / N, `sbo` = bytes between 8-row K groups (a
-// K16 instruction reads two of them).
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr, uint32_t layout, uint32_t lbo,
-                                              uint32_t sbo) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)layout << 61;
-  return d;
+
+// ------------------------------------------------------------- decoder GEMMs of one M = 64 block
+// Layer 1, D[64 x 64] = A W1^T in 3xTF32: 12 wgmma (small terms first).  Arguments are descriptor
+// bases of the block's A_hi / A_lo rows and of W1 hi / lo; a K step of 8 tf32 = 32 bytes = +2.
+__device__ __forceinline__ void layer1_mb(float (&d)[32], uint64_t a_hi, uint64_t a_lo,
+                                          uint64_t w_hi, uint64_t w_lo) {
+  wgmma_tf32_ss_n64(d, a_lo, w_hi, 0);
+#pragma unroll
+  for (int ks = 1; ks < 4; ++ks) wgmma_tf32_ss_n64(d, a_lo + 2 * ks, w_hi + 2 * ks, 1);
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) wgmma_tf32_ss_n64(d, a_hi + 2 * ks, w_lo + 2 * ks, 1);
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) wgmma_tf32_ss_n64(d, a_hi + 2 * ks, w_hi + 2 * ks, 1);
 }
-// Instruction descriptor, kind::f16 with bf16 operands, fp32 accumulate:
-//   [4,6) c_format=1 (F32)  [7,10) a_format=1 (BF16)  [10,13) b_format=1
-//   [15] A MN-major  [16] B MN-major  [17,23) N>>3  [24,29) M>>4
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N, bool a_mn, bool b_mn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((a_mn ? 1u : 0u) << 15) | ((b_mn ? 1u : 0u) << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// Layer 2, D[64 x 16] = H W2^T with H as register fragments (hi / lo, 8 k-blocks): 24 wgmma.
+// W2 hi / lo: [16 x 64] as two [16 x 32] SWIZZLE_128B K-blocks of 2048 bytes.
+__device__ __forceinline__ void layer2_mb(float (&o)[8], const uint32_t (&hhi)[8][4],
+                                          const uint32_t (&hlo)[8][4], uint64_t w2_hi,
+                                          uint64_t w2_lo) {
+#pragma unroll
+  for (int ks = 0; ks < 8; ++ks)
+    wgmma_tf32_rs_n16(o, hlo[ks], w2_hi + (ks >> 2) * 128 + (ks & 3) * 2, ks != 0);
+#pragma unroll
+  for (int ks = 0; ks < 8; ++ks)
+    wgmma_tf32_rs_n16(o, hhi[ks], w2_lo + (ks >> 2) * 128 + (ks & 3) * 2, 1);
+#pragma unroll
+  for (int ks = 0; ks < 8; ++ks)
+    wgmma_tf32_rs_n16(o, hhi[ks], w2_hi + (ks >> 2) * 128 + (ks & 3) * 2, 1);
 }
-template <bool ACC>
-__device__ __forceinline__ void umma_f16_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                            uint32_t idesc) {
-  if (ACC)
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.eq.u32 p, 0, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc)
-        : "memory");
-  else
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.u32 p, 0, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc)
-        : "memory");
+
+// split v into TF32 hi / remainder and place both at A-fragment register `slot` of k-block kb
+template <int KB>
+__device__ __forceinline__ void put_split(uint32_t (&hi)[KB][4], uint32_t (&lo)[KB][4], int kb,
+                                          int slot, float v) {
+  const float h = tf32_hi(v);
+  hi[kb][slot] = __float_as_uint(h);
+  lo[kb][slot] = __float_as_uint(v - h);
+}
+
+// Hidden activations of a layer-1 accumulator block: h = softplus(D1 + b1), returned split as
+// TF32 hi / lo A fragments of layer 2.  PRESCALED: D1 and b1 carry log2(e) (the pipelined
+// kernels' weight image), softplus(x) = ln2 * (max(x', 0) + lg2(1 + 2^-|x'|)), x' = x log2 e;
+// otherwise softplus(x) = max(x, 0) + ln2 * lg2(1 + 2^(-|x| log2 e)).  Two MUFU ops per unit.
+template <bool PRESCALED>
+__device__ __forceinline__ float softplus_mufu(float x) {
+  if (PRESCALED) {
+    float l = ex2_approx(-fabsf(x));
+    l = lg2_approx(l + 1.f);
+    l = l + fmaxf(x, 0.f);
+    return l * 0.6931471805599453f;
+  }
+  const float ax = fabsf(x) * -1.4426950408889634f;
+  const float l = lg2_approx(1.f + ex2_approx(ax));
+  return fmaf(l, 0.6931471805599453f, fmaxf(x, 0.f));
+}
+template <bool PRESCALED>
+__device__ __forceinline__ void softplus_frag(const float (&d)[32], const float* __restrict__ b1,
+                                              int t, uint32_t (&hi)[8][4], uint32_t (&lo)[8][4]) {
+#pragma unroll
+  for (int kb = 0; kb < 8; ++kb) {
+    const float2 bb = *reinterpret_cast<const float2*>(b1 + 8 * kb + 2 * t);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const float h = softplus_mufu<PRESCALED>(d[4 * kb + e] + ((e & 1) ? bb.y : bb.x));
+      put_split(hi, lo, kb, afrag_slot(e), h);
+    }
+  }
+}
+
+// An accumulator block of 64 rows x 2N columns (N/8 column blocks) -> rows of a row-major
+// shared-memory array (`ld` floats per row; the block's row 0 at `rows`)
+template <int R>
+__device__ __forceinline__ void store_frag_rows(const float (&d)[R], float* rows, int ld, int warp,
+                                                int lane) {
+  const int g = lane >> 2, t = lane & 3;
+  float* r0 = rows + (16 * warp + g) * ld + 2 * t;
+#pragma unroll
+  for (int j = 0; j < R / 4; ++j) {
+    *reinterpret_cast<float2*>(r0 + 8 * j) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(r0 + 8 * ld + 8 * j) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+  }
 }
 
 }  // namespace tc

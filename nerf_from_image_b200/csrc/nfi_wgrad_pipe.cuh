@@ -1,40 +1,37 @@
-// Decoder-weight gradients on tcgen05 (SURVEY.md section 8 row a13; the GAN generator step,
-// run.py:1044: loss.backward() with the decoder trainable).
+// Decoder-weight gradients on the tensor cores (SURVEY.md section 8 row a13; the GAN generator
+// step, run.py:1044: loss.backward() with the decoder trainable).
 //
 //   dW1[j][c] = sum_points dpre[p][j] F[p][c]      db1[j] = sum_points dpre[p][j]
 //   dW2[o][j] = sum_points dOut[p][o] H[p][j]      db2[o] = sum_points dOut[p][o]
 //
 // are contractions over the POINTS, i.e. over what the other GEMMs of the path keep as the M
-// dimension (TMEM lane = point).  tcgen05 reads MN-major ("transposed") operands from shared
-// memory -- for 16-bit types with every swizzle; TF32 would need the 32-byte-atomicity layout,
-// which a K-major feature tile cannot double as -- so every operand of a step is laid down
-// point-major as a bf16 hi/lo PAIR (2^-17: these sums are dominated by a few very large terms,
-// single bf16 operands left 1e-3 at every size; with pairs 3e-5 against the fp32 kernel,
-// profiles/r2_wgrad_tc_accuracy.txt) and five accumulating kind::f16 MMAs per 16 points form
+// dimension.  wgmma reads MN-major ("transposed") operands from shared memory for 16-bit types,
+// so every operand of a step is laid down point-major as a bf16 hi/lo PAIR (2^-17: these sums are
+// dominated by a few very large terms; single bf16 operands leave 1e-3, pairs 3e-5 against the
+// fp32 kernel) and five accumulating wgmma per 16 points and 64 rows form
 //
-//   XA = [ dpre_hi (64) | dpre_lo (64) ]   XB = [ H_hi (64) | H_lo (64) ]      (A operands, M = 128)
-//   [448,480) += XA^T F_hi,  += XA^T F_lo      rows j and 64 + j together: dW1[j][.]
-//   [480,496) += XB^T dOut_hi, += XB^T dOut_lo   rows j and 64 + j together: dW2[.][j]
-//   [496,504) += XA^T 1                          db1[j]
+//   XA = [ dpre_hi (64) | dpre_lo (64) ]   XB = [ H_hi (64) | H_lo (64) ]      (A operands)
+//   += XA^T F_hi,  += XA^T F_lo      rows j and 64 + j together: dW1[j][.]
+//   += XB^T dOut_hi, += XB^T dOut_lo   rows j and 64 + j together: dW2[.][j]
+//   += XA^T 1                          db1[j]
 //
-// in 56 TMEM columns, cut into chains of kWgFlush steps that are banked in fp32 (below) and added
-// to the global gradients once per CTA.  db2 is summed in fp32 registers by the shading threads.
+// in the registers of a warpgroup of their own (56 accumulators per thread), cut into chains of
+// kWgFlush steps that are banked in fp32 (below) and added to the global gradients once per CTA.
+// db2 is summed in fp32 registers by the shading threads.
 //
 // To make room for the pair tiles, layer 1 of the recompute chain runs on bf16 pairs too (as the
 // synthesis convolutions do): the gather writes the features as two [128][32 bf16] SWIZZLE_64B
 // tiles (16 KB per stage instead of 32) that are BOTH the K-major A operand of MMA1 and, rows = K,
 // the MN-major B operand of the dW1 products.  The rest of the chain is render_backward_pipe's
-// (MMA2 / MMA3 in 3xTF32, softplus and its reverse, reverse compositing).  Two forms:
+// (MMA2 / MMA3 / MMA4 in 3xTF32 with register A fragments, softplus and its reverse, reverse
+// compositing, issued by the activation warpgroup).  Two forms:
 //   PLANES = true  (the generator step: decoder AND planes / palette / beta / alpha gradients,
 //                   cameras are data): MMA4 and the scatter of render_backward_pipe are folded
-//                   in -- ONE sweep, 26.0 ms per 32 images at config 2 against 21.7 + 16.7 ms of
-//                   the two kernels (profiles/r2_time_wgrad.txt);
+//                   in -- ONE sweep;
 //   PLANES = false (decoder gradients only, or a pose gradient is wanted too): this kernel beside
 //                   render_backward_pipe, which then sees the decoder as a constant.
-// TMEM: two slots of 224 columns
-//   [0,64) D1 -> H_lo (-> D4)   [64,128) H_hi (-> dpre_hi)   [128,144) D2 -> dOut_hi
-//   [144,160) dOut_lo   [160,224) D3 (-> dpre_lo)
-// and the accumulators at [448,504).
+// The accumulator warpgroup costs the register file what a second producer set would need, so
+// one producer set serves the sweep.
 #pragma once
 #include <cuda_bf16.h>
 
@@ -43,12 +40,9 @@
 namespace nfi {
 
 constexpr int kWgSlots = 2;
-constexpr int kWgSlotCols = 224;
-constexpr int kWgAccCol = 448;
 constexpr int kWgStages = 3;
-// The tensor core adds into a TMEM accumulator with truncation, a bias that grows with the length
-// of the chain (DESIGN.md section 2, finding 3: 1.35e-4 after 4,608 terms in the synthesis
-// convolutions); a CTA of config 2 would chain 28,000 accumulating MMAs = 450,000 terms.  The
+// The tensor core adds into its accumulator with truncation, a bias that grows with the length
+// of the chain; a CTA of config 2 would chain 28,000 accumulating MMAs = 450,000 terms.  The
 // chain is therefore cut every kWgFlush steps (2,048 terms): the accumulator is added, in fp32
 // round-to-nearest, to a per-CTA row buffer in global memory (L2-resident, single writer per
 // element) and the next chain starts from zero.
@@ -60,8 +54,8 @@ constexpr size_t kWgAccBytesPerCta = 128 * 64 * sizeof(float);
 // of the GAN generator step in one sweep (no pose gradient: cameras are data there).
 template <bool PLANES>
 struct WgCfgT {
-  static constexpr int P = 2;
-  static constexpr int kThreadsTotal = 384 + 128 * P;
+  static constexpr int P = 1;
+  static constexpr int kThreadsTotal = 384 + 128 * P;  // producers, accumulators, shading, activation
   static constexpr int kStageBytes = 16384;                           // F_hi | F_lo, 8 KB each
   static constexpr int kWbBytes = PLANES ? 32768 : 16384;             // W2^T hi/lo (+ W1^T/3 hi/lo)
   static constexpr int kSmWb = 25600;
@@ -70,21 +64,20 @@ struct WgCfgT {
   static constexpr int kSmX = kSmA + kWgStages * kStageBytes;         // 4 x 16 KB
   static constexpr int kSmE = kSmX + 65536;                           // dOut hi | lo
   static constexpr int kSmOnes = kSmE + 8192;                         // 1 KB of 1.0
-  static constexpr int kStageWarp = 32 * 36 * 4;                      // per-warp scatter staging
-  static constexpr int kSmStage = kSmOnes + 1024;
-  static constexpr int kSmPal = kSmStage + (PLANES ? P * 4 * kStageWarp : 0);
+  static constexpr int kSmD2 = kSmOnes + 1024;                        // D2 / dOut slots
+  static constexpr int kSmD4 = kSmD2 + kWgSlots * kD2SlotBytes;       // one D4 slot (PLANES)
+  static constexpr int kSmPal = kSmD4 + (PLANES ? kD4SlotBytes : 0);
   static constexpr int kSmFrac = kSmPal + 48 * 4;
   static constexpr int kSmBars = kSmFrac + 128 * 4;
-  // full[3], a_free[3], per slot: d1_full, h_ready, d2_full, dout_ready, d3_full, slot_free,
-  // dpre_ready, d4_full; x_ready, x_free; weights x2
-  static constexpr int kNumBars = 2 * kWgStages + 8 * kWgSlots + 2 + 2;
-  static constexpr int kSmTmemPtr = kSmBars + kNumBars * 8;
-  static constexpr int kSmBytes = kSmTmemPtr + 16;
-  // 640 x 96 = 61440 = 256 x 96 + 128 x (128 + 136 + 24) = 256 x 112 + 128 x (96 + 136 + 24)
+  // full[3], a_free[3], per slot: d2_full, dout_ready; d4_full, d4_free; x_ready, x_free;
+  // weights x2
+  static constexpr int kNumBars = 2 * kWgStages + 2 * kWgSlots + 2 + 2 + 2;
+  static constexpr int kSmBytes = kSmBars + kNumBars * 8;
+  // 512 x 128 = 65536 = 128 x (112 + 120 + 136 + 144) = 128 x (96 + 120 + 136 + 160)
   static constexpr int kProdRegs = PLANES ? 112 : 96;
-  static constexpr int kActRegs = PLANES ? 96 : 128;
+  static constexpr int kAccRegs = 120;
   static constexpr int kShadeRegs = 136;
-  static constexpr int kAuxRegs = 24;
+  static constexpr int kActRegs = PLANES ? 144 : 160;
 };
 using WgCfg = WgCfgT<false>;
 static_assert(WgCfgT<true>::kSmBytes <= 227 * 1024, "shared memory budget");
@@ -107,7 +100,7 @@ render_wgrad_pipe(const nfi_render_params p, const nfi_render_grads g,
   unsigned char* base = smem_raw;
   const int tid = threadIdx.x, lane = tid & 31;
   const int hw_wg = __shfl_sync(kFull, tid >> 7, 0);
-  // logical role: 0 activation, 1 shading, 2 MMA issuers, 3.. producer sets
+  // logical role: 0 activation, 1 shading, 2 weight-gradient accumulators, 3.. producer sets
   const int wg = (hw_wg < P) ? hw_wg + 3 : (P + 2 - hw_wg);
   const int gt = tid & 127;
   const int wig = __shfl_sync(kFull, gt >> 5, 0);
@@ -116,19 +109,16 @@ render_wgrad_pipe(const nfi_render_params p, const nfi_render_grads g,
 
   uint64_t* bars = reinterpret_cast<uint64_t*>(base + Cfg::kSmBars);
   uint64_t* full = bars;                      // [3] stage gathered (4 warps)
-  uint64_t* a_free = full + NS;               // [3] stage read by the dW MMAs (commit)
-  uint64_t* d1_full = a_free + NS;            // [2] commit
-  uint64_t* h_ready = d1_full + kWgSlots;     // [2] 4 warps
-  uint64_t* d2_full = h_ready + kWgSlots;     // [2] commit
-  uint64_t* dout_ready = d2_full + kWgSlots;  // [2] 4 warps (dOut in TMEM and in the E tiles)
-  uint64_t* d3_full = dout_ready + kWgSlots;  // [2] commit
-  uint64_t* slot_free = d3_full + kWgSlots;   // [2] 4 warps (D3 / H read)
-  uint64_t* dpre_ready = slot_free + kWgSlots;  // [2] 4 warps (PLANES: dpre hi/lo in TMEM)
-  uint64_t* d4_full = dpre_ready + kWgSlots;    // [2] commit (PLANES)
-  uint64_t* x_ready = d4_full + kWgSlots;     // X tile written (4 warps)
-  uint64_t* x_free = x_ready + 1;             // X and E tiles read by the dW MMAs (commit)
+  uint64_t* a_free = full + NS;               // [3] stage read by the activation AND dW GEMMs (8 warps)
+  uint64_t* d2_full = a_free + NS;            // [2] D2 in its slot (4 warps)
+  uint64_t* dout_ready = d2_full + kWgSlots;  // [2] dOut in the slot and in the E tiles (4 warps)
+  uint64_t* d4_full = dout_ready + kWgSlots;  //     D4 in its slot (PLANES, 4 warps)
+  uint64_t* d4_free = d4_full + 1;            //     D4 scattered (PLANES, 4 warps)
+  uint64_t* x_ready = d4_free + 1;            //     X tiles written (4 warps)
+  uint64_t* x_free = x_ready + 1;             //     X and E tiles read by the dW GEMMs (4 warps)
   uint64_t* wbar = x_free + 1;                // [2] weight images landed
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(base + Cfg::kSmTmemPtr);
+  float* d2s = reinterpret_cast<float*>(base + Cfg::kSmD2);  // [2][128][kD2Ld]
+  float* d4s = reinterpret_cast<float*>(base + Cfg::kSmD4);  // [128][kD4Ld]
   const float* b1s = reinterpret_cast<const float*>(base + kWiB1);
   const float* b2s = reinterpret_cast<const float*>(base + kWiB2);
   float* pal = reinterpret_cast<float*>(base + Cfg::kSmPal);
@@ -152,30 +142,22 @@ render_wgrad_pipe(const nfi_render_params p, const nfi_render_grads g,
   if (tid == 0) {
     if (tc::smem_u32(base) & 1023u) __trap();
     for (int i = 0; i < NS; ++i) {
-      tc::mbar_init(&full[i], 4);
-      tc::mbar_init(&a_free[i], 1);
+      tc::mbar_init(&full[i], kWarps);
+      tc::mbar_init(&a_free[i], 2 * kWarps);
     }
     for (int i = 0; i < kWgSlots; ++i) {
-      tc::mbar_init(&d1_full[i], 1);
-      tc::mbar_init(&h_ready[i], kWarps);
-      tc::mbar_init(&d2_full[i], 1);
+      tc::mbar_init(&d2_full[i], kWarps);
       tc::mbar_init(&dout_ready[i], kWarps);
-      tc::mbar_init(&d3_full[i], 1);
-      tc::mbar_init(&slot_free[i], kWarps);
-      tc::mbar_init(&dpre_ready[i], kWarps);
-      tc::mbar_init(&d4_full[i], 1);
     }
+    tc::mbar_init(d4_full, kWarps);
+    tc::mbar_init(d4_free, kWarps);
     tc::mbar_init(x_ready, kWarps);
-    tc::mbar_init(x_free, 1);
+    tc::mbar_init(x_free, kWarps);
     tc::mbar_init(&wbar[0], 1);
     tc::mbar_init(&wbar[1], 1);
     tc::fence_mbar_init();
   }
-  if (tid < 32) tc::tmem_alloc(tmem_ptr, 512);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(kFull, *tmem_ptr, 0);
   if (tid == 0) {
     tc::mbar_expect_tx(&wbar[0], kWiBytes);
     tc::tma_bulk_g2s(base, wimg, kWiBytes, &wbar[0]);
@@ -185,7 +167,6 @@ render_wgrad_pipe(const nfi_render_params p, const nfi_render_grads g,
   tc::mbar_wait(&wbar[0], 0);
   tc::mbar_wait(&wbar[1], 0);
 
-  const uint32_t base_s = tc::smem_u32(base);
   const int tiles_x = (p.width + kTileW - 1) / kTileW;
   const int tiles_y = (p.height + kTileH - 1) / kTileH;
   const int n_tiles = tiles_x * tiles_y * p.batch;
@@ -195,13 +176,11 @@ render_wgrad_pipe(const nfi_render_params p, const nfi_render_grads g,
   const int R = p.plane_res;
   const float inv_range = 1.f / p.scene_range;
   const uint32_t plane_bytes = (uint32_t)R * (uint32_t)R * 128u;
-  const uint32_t lane_addr = (uint32_t)(32 * wig) << 16;
 
   if (wg >= 3) {
     // ================================ PRODUCERS (gather; PLANES: also the scatter) ================
-    if (PLANES) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(Cfg::kProdRegs));
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::kProdRegs));
     const int set = wg - 3;
-    float* Dw = reinterpret_cast<float*>(base + Cfg::kSmStage + (set * 4 + wig) * Cfg::kStageWarp);
     const int q = lane >> 3, kq = lane & 7;
     const uint32_t row_units = (uint32_t)R * 8u;
     uint32_t n0 = 0;  // ring position of the tile's first step
@@ -251,34 +230,14 @@ render_wgrad_pipe(const nfi_render_params p, const nfi_render_grads g,
           if (i + P < n_total) gather_step(i + P, nxt);
           // ---- scatter step i: D4 -> plane gradient (as render_backward_pipe, no pose gradient)
           const uint32_t m = n0 + (uint32_t)i;
-          const uint32_t sl = m % kWgSlots, v = m / kWgSlots;
-          const uint32_t d4 = tmem_base + sl * kWgSlotCols + lane_addr;
-          NFI_STEP_WAIT(&d4_full[sl], v & 1);
-          tc::tc_fence_after();
-          {
-            uint32_t ra[16], rb[16];
-            tc::tmem_ld16_nowait(d4, ra);
-            tc::tmem_ld16_nowait(d4 + 16, rb);
-            tc::tmem_wait_ld();
-            tc::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&slot_free[sl]);
-#pragma unroll
-            for (int c4 = 0; c4 < 4; ++c4) {
-              *reinterpret_cast<float4*>(Dw + lane * 36 + 4 * c4) =
-                  make_float4(__uint_as_float(ra[4 * c4]), __uint_as_float(ra[4 * c4 + 1]),
-                              __uint_as_float(ra[4 * c4 + 2]), __uint_as_float(ra[4 * c4 + 3]));
-              *reinterpret_cast<float4*>(Dw + lane * 36 + 16 + 4 * c4) =
-                  make_float4(__uint_as_float(rb[4 * c4]), __uint_as_float(rb[4 * c4 + 1]),
-                              __uint_as_float(rb[4 * c4 + 2]), __uint_as_float(rb[4 * c4 + 3]));
-            }
-          }
-          __syncwarp();
+          // this warp's 32 rows of the D4 slot, read in place (released after the scatter)
+          const float* Dw = d4s + 32 * wig * kD4Ld;
+          NFI_STEP_WAIT(d4_full, m & 1);
           if (gplanes_b != nullptr) {
 #pragma unroll 1
             for (int gq = 0; gq < 8; ++gq) {
               const int src = 4 * gq + q;
-              const float4 d4v = *reinterpret_cast<const float4*>(Dw + src * 36 + 4 * kq);
+              const float4 d4v = *reinterpret_cast<const float4*>(Dw + src * kD4Ld + 4 * kq);
 #pragma unroll
               for (int pl = 0; pl < 3; ++pl) {
                 const uint32_t a00 = __shfl_sync(kFull, cur.o[pl], src) | (uint32_t)kq;
@@ -298,276 +257,253 @@ render_wgrad_pipe(const nfi_render_params p, const nfi_render_grads g,
             }
           }
           __syncwarp();
+          if (lane == 0) mbar_arrive(d4_free);
           cur = nxt;
         }
       }
     }
   } else if (wg == 2) {
-    // ================================ MMA ISSUERS ================================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::kAuxRegs));
-    if (wig == 0) {
-      // layer 1 on bf16 pairs: D1 = F_lo W1_hi + F_hi W1_lo + F_hi W1_hi, K = 32 = two K16 steps
-      constexpr uint32_t idesc1 = tc::umma_idesc_bf16(128, 64, false, false);
-      const uint64_t dsc_w1_hi = tc::umma_desc(base_s + Cfg::kSmW1, 4, 16, 512);
-      const uint64_t dsc_w1_lo = tc::umma_desc(base_s + Cfg::kSmW1 + 4096, 4, 16, 512);
-      uint32_t st = 0, u = 0, sl = 0, v = 0;
-      for (uint32_t m = 0; m < total_steps; ++m) {
-        NFI_STEP_WAIT(&full[st], u & 1);
-        NFI_STEP_WAIT(&slot_free[sl], (v & 1) ^ 1);
-        if (elect_one()) {
-          tc::tc_fence_after();
-          const uint32_t stage_s = base_s + Cfg::kSmA + st * Cfg::kStageBytes;
-          const uint64_t a_hi = tc::umma_desc(stage_s, 4, 16, 512);
-          const uint64_t a_lo = tc::umma_desc(stage_s + 8192, 4, 16, 512);
-          const uint32_t d1 = tmem_base + sl * kWgSlotCols;
-          tc::umma_f16_ss<false>(d1, a_lo, dsc_w1_hi, idesc1);
-          tc::umma_f16_ss<true>(d1, a_lo + 2, dsc_w1_hi + 2, idesc1);
-          tc::umma_f16_ss<true>(d1, a_hi, dsc_w1_lo, idesc1);
-          tc::umma_f16_ss<true>(d1, a_hi + 2, dsc_w1_lo + 2, idesc1);
-          tc::umma_f16_ss<true>(d1, a_hi, dsc_w1_hi, idesc1);
-          tc::umma_f16_ss<true>(d1, a_hi + 2, dsc_w1_hi + 2, idesc1);
-          tc::umma_commit(&d1_full[sl]);
-        }
-        __syncwarp();
-        if (++st == NS) { st = 0; ++u; }
-        if (++sl == kWgSlots) { sl = 0; ++v; }
-      }
-    } else if (wig == 1) {
-      const uint64_t dsc_w2_hi = tc::umma_desc_sw128(base_s + kWiW2Hi);
-      const uint64_t dsc_w2_lo = tc::umma_desc_sw128(base_s + kWiW2Lo);
-      uint32_t sl = 0, v = 0;
-      for (uint32_t m = 0; m < total_steps; ++m) {
-        NFI_STEP_WAIT(&h_ready[sl], v & 1);
-        if (elect_one()) {
-          tc::tc_fence_after();
-          const uint32_t d = tmem_base + sl * kWgSlotCols;
-          issue_layer2_tt(d + 128, d, d + 64, dsc_w2_hi, dsc_w2_lo);
-          tc::umma_commit(&d2_full[sl]);
-        }
-        __syncwarp();
-        if (++sl == kWgSlots) { sl = 0; ++v; }
-      }
-    } else if (wig == 2) {
-      const uint64_t b_hi = tc::umma_desc_sw128(base_s + Cfg::kSmWb + kWbW2tHi);
-      const uint64_t b_lo = tc::umma_desc_sw128(base_s + Cfg::kSmWb + kWbW2tLo);
-      uint32_t sl = 0, v = 0;
-      for (uint32_t m = 0; m < total_steps; ++m) {
-        NFI_STEP_WAIT(&dout_ready[sl], v & 1);
-        if (elect_one()) {
-          tc::tc_fence_after();
-          const uint32_t d = tmem_base + sl * kWgSlotCols;
-          issue_mma3(d + 160, d + 128, d + 144, b_hi, b_lo);
-          tc::umma_commit(&d3_full[sl]);
-        }
-        __syncwarp();
-        if (++sl == kWgSlots) { sl = 0; ++v; }
-      }
-    } else {
-      // the weight-gradient chain: 8 k-steps of 16 points, five MMAs each
-      constexpr uint32_t id_w1 = tc::umma_idesc_bf16(128, 32, true, true);
-      constexpr uint32_t id_w2 = tc::umma_idesc_bf16(128, 16, true, true);
-      constexpr uint32_t id_b1 = tc::umma_idesc_bf16(128, 8, true, false);
-      const uint64_t dsc_xa = tc::umma_desc(base_s + Cfg::kSmX, 2, 16384, 1024);
-      const uint64_t dsc_xb = tc::umma_desc(base_s + Cfg::kSmX + 32768, 2, 16384, 1024);
-      const uint64_t dsc_ehi = tc::umma_desc(base_s + Cfg::kSmE, 6, 16, 256);
-      const uint64_t dsc_elo = tc::umma_desc(base_s + Cfg::kSmE + 4096, 6, 16, 256);
-      const uint64_t dsc_one = tc::umma_desc(base_s + Cfg::kSmOnes, 6, 16, 256);  // K-major [8][16]
-      const uint32_t d_w1 = tmem_base + kWgAccCol, d_w2 = d_w1 + 32, d_b1 = d_w1 + 48;
-      const uint64_t w1t_hi = tc::umma_desc_sw128(base_s + Cfg::kSmWb + kWbW1tHi);
-      const uint64_t w1t_lo = tc::umma_desc_sw128(base_s + Cfg::kSmWb + kWbW1tLo);
-      uint32_t st = 0, u = 0, sl = 0, v = 0;
-      for (uint32_t m = 0; m < total_steps; ++m) {
-        if constexpr (PLANES) {  // MMA4: D4 = dpre (W1 / 3) over D1 / H_lo, 3xTF32 as render_backward_pipe
-          NFI_STEP_WAIT(&dpre_ready[sl], v & 1);
-          if (elect_one()) {
-            tc::tc_fence_after();
-            const uint32_t d = tmem_base + sl * kWgSlotCols;
-            issue_mma4(d, d + 64, d + 160, w1t_hi, w1t_lo);
-            tc::umma_commit(&d4_full[sl]);
-          }
-          __syncwarp();
-        }
-        NFI_STEP_WAIT(&full[st], u & 1);
-        NFI_STEP_WAIT(&dout_ready[sl], v & 1);
-        NFI_STEP_WAIT(x_ready, m & 1);
-        if (elect_one()) {
-          tc::tc_fence_after();
-          const uint32_t stage_s = base_s + Cfg::kSmA + st * Cfg::kStageBytes;
-          const uint64_t dsc_fhi = tc::umma_desc(stage_s, 4, 16, 512);        // MN-major: rows = K
-          const uint64_t dsc_flo = tc::umma_desc(stage_s + 8192, 4, 16, 512);
-          const bool fresh = (m % kWgFlush == 0);  // new chain: the first MMA into each accumulator overwrites
+    // ================================ WEIGHT-GRADIENT ACCUMULATORS ================================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::kAccRegs));
+    const uint32_t base_s = tc::smem_u32(base);
+    const int g4 = lane >> 2, t = lane & 3;
+    // accumulator row r = 64 mb + 16 wig + g4 (+ 8) = hidden unit j (mb 0: dpre_hi / H_hi rows, 1:
+    // the lo halves): dW1[j][c] at columns c, dW2[o][j] at o, db1[j] (all 8 columns equal)
+    float w1a[2][16], w2a[2][8], b1a[2][4];
+    auto clear = [&]() {
 #pragma unroll
-          for (int ks = 0; ks < 8; ++ks) {  // 16 points: 2048 B of X, 1024 B of F, 512 B of dOut
-            const uint64_t xa = dsc_xa + 128 * ks, xb = dsc_xb + 128 * ks;
-            if (ks == 0 && fresh) {
-              tc::umma_f16_ss<false>(d_w1, xa, dsc_fhi, id_w1);
-              tc::umma_f16_ss<false>(d_w2, xb, dsc_ehi, id_w2);
-              tc::umma_f16_ss<false>(d_b1, xa, dsc_one, id_b1);
-            } else {
-              tc::umma_f16_ss<true>(d_w1, xa, dsc_fhi + 64 * ks, id_w1);
-              tc::umma_f16_ss<true>(d_w2, xb, dsc_ehi + 32 * ks, id_w2);
-              tc::umma_f16_ss<true>(d_b1, xa, dsc_one, id_b1);
-            }
-            tc::umma_f16_ss<true>(d_w1, xa, dsc_flo + 64 * ks, id_w1);
-            tc::umma_f16_ss<true>(d_w2, xb, dsc_elo + 32 * ks, id_w2);
-          }
-          tc::umma_commit(&a_free[st]);
-          tc::umma_commit(x_free);
-        }
-        __syncwarp();
-        if (++st == NS) { st = 0; ++u; }
-        if (++sl == kWgSlots) { sl = 0; ++v; }
+      for (int mb = 0; mb < 2; ++mb) {
+        zero(w1a[mb]);
+        zero(w2a[mb]);
+        zero(b1a[mb]);
       }
+    };
+    // the row buffer of this CTA ([128][64]: columns 0..31 dW1, 32..47 dW2, 48 db1): `first`: it
+    // is written, not added to; `final`: the total goes to the global gradients instead
+    const int nout_w = 1 + (p.n_attention > 0 ? p.n_attention : 3);
+    auto flush = [&](bool first, bool final) {
+#pragma unroll
+      for (int mb = 0; mb < 2; ++mb) {
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+          const int row = 64 * mb + 16 * wig + g4 + 8 * half, j = row & (kHid - 1);
+          float* const myrow = acc_ws + ((size_t)blockIdx.x * 128 + row) * 64;
+          auto put = [&](int col, float a, float b, float* gdst0, float* gdst1) {
+            float2 v2 = make_float2(a, b);
+            if (!first) {
+              const float2 o = *reinterpret_cast<const float2*>(myrow + col);
+              v2.x += o.x;
+              v2.y += o.y;
+            }
+            if (!final) {
+              *reinterpret_cast<float2*>(myrow + col) = v2;
+            } else {
+              if (gdst0) atomicAdd(gdst0, v2.x);
+              if (gdst1) atomicAdd(gdst1, v2.y);
+            }
+          };
+#pragma unroll
+          for (int jb = 0; jb < 4; ++jb) {
+            const int c = 8 * jb + 2 * t;
+            put(c, w1a[mb][4 * jb + 2 * half], w1a[mb][4 * jb + 2 * half + 1],
+                g.grad_w1 ? g.grad_w1 + j * kC + c : nullptr,
+                g.grad_w1 ? g.grad_w1 + j * kC + c + 1 : nullptr);
+          }
+#pragma unroll
+          for (int jb = 0; jb < 2; ++jb) {
+            const int o = 8 * jb + 2 * t;
+            put(32 + o, w2a[mb][4 * jb + 2 * half], w2a[mb][4 * jb + 2 * half + 1],
+                (g.grad_w2 && o < nout_w) ? g.grad_w2 + o * kHid + j : nullptr,
+                (g.grad_w2 && o + 1 < nout_w) ? g.grad_w2 + (o + 1) * kHid + j : nullptr);
+          }
+          if (t == 0) put(48, b1a[mb][2 * half], 0.f, g.grad_b1 ? g.grad_b1 + j : nullptr, nullptr);
+        }
+      }
+    };
+    clear();
+    const uint64_t dsc_one = tc::gmma_desc(base_s + Cfg::kSmOnes, tc::kSw32, 16, 256);
+    uint32_t st = 0, u = 0, sl = 0, v = 0;
+    for (uint32_t m = 0; m < total_steps; ++m) {
+      NFI_STEP_WAIT(&full[st], u & 1);
+      NFI_STEP_WAIT(&dout_ready[sl], v & 1);
+      NFI_STEP_WAIT(x_ready, m & 1);
+      const uint32_t stage_s = base_s + Cfg::kSmA + st * Cfg::kStageBytes;
+      tc::wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < 8; ++ks) {  // 16 points: 2048 B of X, 1024 B of F, 512 B of dOut
+        // MN-major operands: rows = points (K)
+        const uint64_t f_hi = tc::gmma_desc(stage_s + 1024 * ks, tc::kSw64, 16, 512);
+        const uint64_t f_lo = tc::gmma_desc(stage_s + 8192 + 1024 * ks, tc::kSw64, 16, 512);
+        const uint64_t e_hi = tc::gmma_desc(base_s + Cfg::kSmE + 512 * ks, tc::kSw32, 16, 256);
+        const uint64_t e_lo = tc::gmma_desc(base_s + Cfg::kSmE + 4096 + 512 * ks, tc::kSw32, 16, 256);
+#pragma unroll
+        for (int mb = 0; mb < 2; ++mb) {
+          const uint32_t xa_s = base_s + Cfg::kSmX + 16384 * mb + 2048 * ks;
+          const uint64_t xa = tc::gmma_desc(xa_s, tc::kSw128, 16, 1024);
+          const uint64_t xb = tc::gmma_desc(xa_s + 32768, tc::kSw128, 16, 1024);
+          tc::wgmma_bf16_ss_n32<1, 1>(w1a[mb], xa, f_hi, 1);
+          tc::wgmma_bf16_ss_n32<1, 1>(w1a[mb], xa, f_lo, 1);
+          tc::wgmma_bf16_ss_n8<1, 0>(b1a[mb], xa, dsc_one, 1);
+          tc::wgmma_bf16_ss_n16<1, 1>(w2a[mb], xb, e_hi, 1);
+          tc::wgmma_bf16_ss_n16<1, 1>(w2a[mb], xb, e_lo, 1);
+        }
+      }
+      tc::wgmma_commit();
+      tc::wgmma_wait<0>();
+#pragma unroll
+      for (int mb = 0; mb < 2; ++mb) {
+        tc::reg_fence(w1a[mb]);
+        tc::reg_fence(w2a[mb]);
+        tc::reg_fence(b1a[mb]);
+      }
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(&a_free[st]);
+        mbar_arrive(x_free);
+      }
+      if ((m + 1) % kWgFlush == 0 && m + 1 < total_steps) {
+        flush(m + 1 == (uint32_t)kWgFlush, false);
+        clear();
+      }
+      if (++st == NS) { st = 0; ++u; }
+      if (++sl == kWgSlots) { sl = 0; ++v; }
     }
+    // ---- the last chain + the banked ones -> global gradients (one atomic per entry per CTA)
+    if (total_steps > 0) flush(total_steps <= (uint32_t)kWgFlush, true);
   } else if (wg == 0) {
     // ================================ ACTIVATION (forward and reverse) ================================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(Cfg::kActRegs));
     unsigned char* const xrow = base + Cfg::kSmX;
-    // Accumulator row of this thread (TMEM lane gt), hidden unit j = gt % 64 (rows 64.. are the
-    // products of the lo halves): columns 0..31 dW1[j][.], 32..47 dW2[.][j], 48 db1[j].
-    // `first`: the row buffer is written, not added to; `final`: the total goes to the global
-    // gradients instead.
-    float* const myrow = acc_ws + ((size_t)blockIdx.x * 128 + gt) * 64;
-    const int nout_w = 1 + (p.n_attention > 0 ? p.n_attention : 3);
-    auto flush = [&](bool first, bool final) {
-      const uint32_t dacc = tmem_base + kWgAccCol + lane_addr;
-      const int j = gt & (kHid - 1);
-#pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        float v16[16];
-        tc::tmem_ld16(dacc + 16 * c, v16);  // (c == 3: only column 48 is an accumulator)
-        float4* row4 = reinterpret_cast<float4*>(myrow + 16 * c);
-        if (!first) {
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            if (c == 3 && q > 0) break;
-            const float4 o = row4[q];
-            v16[4 * q] += o.x;
-            v16[4 * q + 1] += o.y;
-            v16[4 * q + 2] += o.z;
-            v16[4 * q + 3] += o.w;
-          }
-        }
-        if (!final) {
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            if (c == 3 && q > 0) break;
-            row4[q] = make_float4(v16[4 * q], v16[4 * q + 1], v16[4 * q + 2], v16[4 * q + 3]);
-          }
-        } else if (c < 2) {
-          if (g.grad_w1) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) atomicAdd(g.grad_w1 + j * kC + 16 * c + i, v16[i]);
-          }
-        } else if (c == 2) {
-          if (g.grad_w2) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i)
-              if (i < nout_w) atomicAdd(g.grad_w2 + i * kHid + j, v16[i]);
-          }
-        } else if (g.grad_b1) {
-          atomicAdd(g.grad_b1 + j, v16[0]);
-        }
-      }
+    const uint32_t base_s = tc::smem_u32(base);
+    const uint64_t w1_hi = tc::gmma_desc(base_s + Cfg::kSmW1, tc::kSw64, 16, 512);
+    const uint64_t w1_lo = tc::gmma_desc(base_s + Cfg::kSmW1 + 4096, tc::kSw64, 16, 512);
+    const uint64_t w2_hi = tc::gmma_desc_sw128(base_s + kWiW2Hi);
+    const uint64_t w2_lo = tc::gmma_desc_sw128(base_s + kWiW2Lo);
+    const uint64_t b3_hi = tc::gmma_desc_sw128(base_s + Cfg::kSmWb + kWbW2tHi);
+    const uint64_t b3_lo = tc::gmma_desc_sw128(base_s + Cfg::kSmWb + kWbW2tLo);
+    const uint64_t b4_hi = tc::gmma_desc_sw128(base_s + Cfg::kSmWb + kWbW1tHi);
+    const uint64_t b4_lo = tc::gmma_desc_sw128(base_s + Cfg::kSmWb + kWbW1tLo);
+    const int g4 = lane >> 2, t = lane & 3;
+    // layer 1 on bf16 pairs for the 64 rows of block mb: D1 = F_lo W1_hi + F_hi W1_lo + F_hi W1_hi,
+    // K = 32 = two K16 steps of 32 bytes
+    auto layer1 = [&](float (&d)[32], uint32_t stage_s, int mb) {
+      const uint64_t a_hi = tc::gmma_desc(stage_s + 4096 * mb, tc::kSw64, 16, 512);
+      const uint64_t a_lo = tc::gmma_desc(stage_s + 8192 + 4096 * mb, tc::kSw64, 16, 512);
+      tc::wgmma_bf16_ss_n64<0, 0>(d, a_lo, w1_hi, 0);
+      tc::wgmma_bf16_ss_n64<0, 0>(d, a_lo + 2, w1_hi + 2, 1);
+      tc::wgmma_bf16_ss_n64<0, 0>(d, a_hi, w1_lo, 1);
+      tc::wgmma_bf16_ss_n64<0, 0>(d, a_hi + 2, w1_lo + 2, 1);
+      tc::wgmma_bf16_ss_n64<0, 0>(d, a_hi, w1_hi, 1);
+      tc::wgmma_bf16_ss_n64<0, 0>(d, a_hi + 2, w1_hi + 2, 1);
     };
     auto act_fwd = [&](uint32_t m) {
-      const uint32_t sl = m % kWgSlots, v = m / kWgSlots;
-      const uint32_t d1 = tmem_base + sl * kWgSlotCols + lane_addr;
-      NFI_STEP_WAIT(&d1_full[sl], v & 1);
-      tc::tc_fence_after();
+      const uint32_t st = m % NS, u = m / NS, sl = m % kWgSlots;
+      const uint32_t stage_s = base_s + Cfg::kSmA + st * Cfg::kStageBytes;
+      float* d2 = d2s + sl * (kThreads * kD2Ld);
+      NFI_STEP_WAIT(&full[st], u & 1);
 #pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        float lo[16], hi[16];
-        tc::tmem_ld16(d1 + 16 * c, lo);
-        softplus_split16(lo, hi, b1s + 16 * c);
-        tc::tmem_st16(d1 + 16 * c, lo);
-        tc::tmem_st16(d1 + 64 + 16 * c, hi);
+      for (int mb = 0; mb < 2; ++mb) {
+        float d[32];
+        zero(d);
+        tc::wgmma_fence();
+        layer1(d, stage_s, mb);
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::reg_fence(d);
+        uint32_t hi[8][4], lo[8][4];
+        tc::softplus_frag<true>(d, b1s, t, hi, lo);
+        float o[8];
+        zero(o);
+        tc::wgmma_fence();
+        tc::layer2_mb(o, hi, lo, w2_hi, w2_lo);
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::reg_fence(o);
+        tc::store_frag_rows(o, d2 + 64 * mb * kD2Ld, kD2Ld, wig, lane);
       }
-      tc::tmem_wait_st();
-      tc::tc_fence_before();
       __syncwarp();
-      if (lane == 0) mbar_arrive(&h_ready[sl]);
+      if (lane == 0) mbar_arrive(&d2_full[sl]);
     };
     // dpre = dH * sigmoid(pre),  sigmoid(pre) = 1 - exp(-softplus(pre)); dpre and H go to the
-    // X tiles as bf16 hi / lo pairs (row = point = this thread, MN-major atoms of 64 columns)
+    // X tiles as bf16 hi / lo pairs (row = point, MN-major atoms of 64 columns); PLANES: D4 too
     auto act_bwd = [&](uint32_t m) {
-      const uint32_t sl = m % kWgSlots, v = m / kWgSlots;
-      const uint32_t d = tmem_base + sl * kWgSlotCols + lane_addr;
-      NFI_STEP_WAIT(&d3_full[sl], v & 1);
-      NFI_STEP_WAIT(x_free, (m & 1) ^ 1);  // the previous step's dW MMAs have read the X tile
-      tc::tc_fence_after();
-      // the chain of steps [m - kWgFlush, m) is complete and the next one cannot start before
-      // this step's x_ready: the accumulator is quiescent -> bank it
-      if (m > 0 && m % kWgFlush == 0) flush(m == kWgFlush, false);
+      const uint32_t st = m % NS, sl = m % kWgSlots, v = m / kWgSlots;
+      const uint32_t stage_s = base_s + Cfg::kSmA + st * Cfg::kStageBytes;
+      const float* dout = d2s + sl * (kThreads * kD2Ld);
+      NFI_STEP_WAIT(&dout_ready[sl], v & 1);
+      NFI_STEP_WAIT(x_free, (m & 1) ^ 1);  // the previous step's dW GEMMs have read the X tiles
+      if constexpr (PLANES) NFI_STEP_WAIT(d4_free, (m & 1) ^ 1);  // D4 of step m - 1 scattered
 #pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        uint32_t r3[16], rh[16], rl[16];
-        tc::tmem_ld16_nowait(d + 160 + 16 * c, r3);
-        tc::tmem_ld16_nowait(d + 64 + 16 * c, rh);
-        tc::tmem_ld16_nowait(d + 16 * c, rl);
-        tc::tmem_wait_ld();
-        float dp[16], hh[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const float h = __uint_as_float(rh[i]) + __uint_as_float(rl[i]);
-          const float sg = 1.f - tc::ex2_approx(-h * kLog2e);
-          dp[i] = __uint_as_float(r3[i]) * sg;
-          hh[i] = h;
+      for (int mb = 0; mb < 2; ++mb) {
+        float d[32], d3[32];
+        zero(d);
+        zero(d3);
+        uint32_t ohi[2][4], olo[2][4];
+        load_dout_frags(dout + 64 * mb * kD2Ld, wig, lane, ohi, olo);
+        tc::wgmma_fence();
+        layer1(d, stage_s, mb);
+        mma3_mb(d3, ohi, olo, b3_hi, b3_lo);
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::reg_fence(d);
+        tc::reg_fence(d3);
+        if (mb == 1) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&a_free[st]);
         }
-        if constexpr (PLANES) {  // dpre as a TF32 pair for MMA4: hi over H_hi, lo over D3
-          float thi[16], tlo[16];
+        uint32_t phi[8][4], plo[8][4];
 #pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            thi[i] = tc::tf32_hi(dp[i]);
-            tlo[i] = dp[i] - thi[i];
+        for (int kb = 0; kb < 8; ++kb) {
+          const float2 bb = *reinterpret_cast<const float2*>(b1s + 8 * kb + 2 * t);
+#pragma unroll
+          for (int half = 0; half < 2; ++half) {
+            float hv[2], dp[2];
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+              const int e = 2 * half + c;
+              hv[c] = tc::softplus_mufu<true>(d[4 * kb + e] + (c ? bb.y : bb.x));
+              const float sg = 1.f - tc::ex2_approx(-hv[c] * kLog2e);
+              dp[c] = d3[4 * kb + e] * sg;
+              if constexpr (PLANES) tc::put_split(phi, plo, kb, tc::afrag_slot(e), dp[c]);
+            }
+            // columns 8kb + 2t, +1 of this thread's row in dpre_hi / dpre_lo (tiles 0, 1) and
+            // H_hi / H_lo (tiles 2, 3)
+            const int row = 64 * mb + 16 * wig + g4 + 8 * half;
+            const uint32_t off = tc::sw128_offset(row, kb) + 4 * t;
+            const uint32_t dh = tc::bf16x2_rn(dp[0], dp[1]);
+            const uint32_t dl = tc::bf16x2_rn(dp[0] - __uint_as_float(dh << 16),
+                                              dp[1] - __uint_as_float(dh & 0xFFFF0000u));
+            const uint32_t hh = tc::bf16x2_rn(hv[0], hv[1]);
+            const uint32_t hl = tc::bf16x2_rn(hv[0] - __uint_as_float(hh << 16),
+                                              hv[1] - __uint_as_float(hh & 0xFFFF0000u));
+            *reinterpret_cast<uint32_t*>(xrow + off) = dh;
+            *reinterpret_cast<uint32_t*>(xrow + 16384 + off) = dl;
+            *reinterpret_cast<uint32_t*>(xrow + 32768 + off) = hh;
+            *reinterpret_cast<uint32_t*>(xrow + 49152 + off) = hl;
           }
-          tc::tmem_st16(d + 160 + 16 * c, tlo);
-          tc::tmem_st16(d + 64 + 16 * c, thi);
         }
-        // columns 16c .. 16c+15 of dpre_hi / dpre_lo (tiles 0, 1) and H_hi / H_lo (tiles 2, 3):
-        // two 16-byte chunks of this point's 128-byte row in each
-#pragma unroll
-        for (int q = 0; q < 2; ++q) {
-          const uint32_t off = tc::sw128_offset(gt, 2 * c + q);
-          uint32_t dh[4], dl[4], hh2[4], hl[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float a0 = dp[8 * q + 2 * i], a1 = dp[8 * q + 2 * i + 1];
-            dh[i] = tc::bf16x2_rn(a0, a1);
-            dl[i] = tc::bf16x2_rn(a0 - __uint_as_float(dh[i] << 16),
-                                  a1 - __uint_as_float(dh[i] & 0xFFFF0000u));
-            const float b0 = hh[8 * q + 2 * i], b1v = hh[8 * q + 2 * i + 1];
-            hh2[i] = tc::bf16x2_rn(b0, b1v);
-            hl[i] = tc::bf16x2_rn(b0 - __uint_as_float(hh2[i] << 16),
-                                  b1v - __uint_as_float(hh2[i] & 0xFFFF0000u));
-          }
-          *reinterpret_cast<uint4*>(xrow + off) = make_uint4(dh[0], dh[1], dh[2], dh[3]);
-          *reinterpret_cast<uint4*>(xrow + 16384 + off) = make_uint4(dl[0], dl[1], dl[2], dl[3]);
-          *reinterpret_cast<uint4*>(xrow + 32768 + off) = make_uint4(hh2[0], hh2[1], hh2[2], hh2[3]);
-          *reinterpret_cast<uint4*>(xrow + 49152 + off) = make_uint4(hl[0], hl[1], hl[2], hl[3]);
+        if constexpr (PLANES) {  // MMA4: D4 = dpre (W1 / 3), 3xTF32 as render_backward_pipe
+          float d4v[16];
+          zero(d4v);
+          tc::wgmma_fence();
+          mma4_mb(d4v, phi, plo, b4_hi, b4_lo);
+          tc::wgmma_commit();
+          tc::wgmma_wait<0>();
+          tc::reg_fence(d4v);
+          tc::store_frag_rows(d4v, d4s + 64 * mb * kD4Ld, kD4Ld, wig, lane);
         }
       }
-      if constexpr (PLANES) tc::tmem_wait_st();
-      tc::tc_fence_before();
       tc::fence_async_smem();
       __syncwarp();
       if (lane == 0) {
         mbar_arrive(x_ready);
-        if constexpr (PLANES) mbar_arrive(&dpre_ready[sl]);  // (the slot is freed by the scatter)
-        else mbar_arrive(&slot_free[sl]);
+        if constexpr (PLANES) mbar_arrive(d4_full);
       }
     };
     if (total_steps > 0) act_fwd(0);
     for (uint32_t m = 0; m < total_steps; ++m) {
       if (m + 1 < total_steps) act_fwd(m + 1);
       act_bwd(m);
-    }
-    // ---- the last chain + the banked ones -> global gradients (one atomic per entry per CTA)
-    if (total_steps > 0) {
-      NFI_STEP_WAIT(x_free, (total_steps - 1) & 1);
-      tc::tc_fence_after();
-      flush(total_steps <= (uint32_t)kWgFlush, true);
-      tc::tc_fence_before();
     }
   } else {
     // ================================ SHADING (forward and reverse) ================================
@@ -630,14 +566,14 @@ render_wgrad_pipe(const nfi_render_params p, const nfi_render_grads g,
         const float zn = has_next ? mw.pop() : z;
         const float delta = has_next ? (zn - z) * r.dn : 0.f;
         const uint32_t sl = m % kWgSlots, v = m / kWgSlots;
-        const uint32_t d = tmem_base + sl * kWgSlotCols + lane_addr;
+        float* const row = d2s + sl * (kThreads * kD2Ld) + gt * kD2Ld;  // D2 in, dOut out
         const float wx = r.ox + r.dx * z, wy = r.oy + r.dy * z, wz = r.oz + r.dz * z;
         const float x0 = wx * inv_range, x1 = wy * inv_range, x2 = wz * inv_range;
         const float keep = (fabsf(x0) > 1.f || fabsf(x1) > 1.f || fabsf(x2) > 1.f) ? 0.f : 1.f;
         NFI_STEP_WAIT(&d2_full[sl], v & 1);
-        tc::tc_fence_after();
         float o16[16];
-        tc::tmem_ld16(d + 128, o16);
+#pragma unroll
+        for (int o = 0; o < 16; ++o) o16[o] = row[o];
         float out[NOUT_PAD];
 #pragma unroll
         for (int o = 0; o < NOUT_PAD; ++o) out[o] = o16[o] + b2s[o];
@@ -724,18 +660,14 @@ render_wgrad_pipe(const nfi_render_params p, const nfi_render_grads g,
         }
 #pragma unroll
         for (int o = 0; o < NOUT_PAD; ++o) acc_b2[o] += dOut[o];
-        // ---- hand dOut to the tensor core: TF32 hi/lo into TMEM (MMA3), a bf16 hi/lo pair into
+        // ---- hand dOut to the tensor core: fp32 into the slot (MMA3), a bf16 hi/lo pair into
         //      the two [128][16] SWIZZLE_32B tiles the dW2 products read (once the previous
         //      step's chain has read them)
         {
-          float hi[16], lo[16];
 #pragma unroll
-          for (int o = 0; o < 16; ++o) {
-            hi[o] = tc::tf32_hi(dOut[o]);
-            lo[o] = dOut[o] - hi[o];
-          }
-          tc::tmem_st16(d + 128, hi);
-          tc::tmem_st16(d + 144, lo);
+          for (int o4 = 0; o4 < 4; ++o4)
+            *reinterpret_cast<float4*>(row + 4 * o4) =
+                make_float4(dOut[4 * o4], dOut[4 * o4 + 1], dOut[4 * o4 + 2], dOut[4 * o4 + 3]);
           NFI_STEP_WAIT(x_free, (m & 1) ^ 1);
           unsigned char* const et = base + Cfg::kSmE;
 #pragma unroll
@@ -752,8 +684,6 @@ render_wgrad_pipe(const nfi_render_params p, const nfi_render_grads g,
             *reinterpret_cast<uint4*>(et + off) = make_uint4(eh[0], eh[1], eh[2], eh[3]);
             *reinterpret_cast<uint4*>(et + 4096 + off) = make_uint4(el[0], el[1], el[2], el[3]);
           }
-          tc::tmem_wait_st();
-          tc::tc_fence_before();
           tc::fence_async_smem();
           __syncwarp();
           if (lane == 0) mbar_arrive(&dout_ready[sl]);
@@ -792,9 +722,6 @@ render_wgrad_pipe(const nfi_render_params p, const nfi_render_grads g,
       }
     }
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (tid < 32) tc::tmem_dealloc(tmem_base, 512);
 }
 
 }  // namespace nfi

@@ -1,9 +1,9 @@
-"""Generator front-end with the plane producer on sm_100a.
+"""Generator front-end with the plane producer on sm_90a.
 
 ``FusedGeneratorFront(G)`` is the part of the reference's ``Generator.forward``
 (/root/reference/models/generator.py:407-477,500-502) that turns the model input into the
 radiance field -- latent selection / mapping network, palette (texture mapper), synthesis
-network -- with the synthesis network run by ``synthesis.FusedSynthesis`` (tcgen05 kernels,
+network -- with the synthesis network run by ``synthesis.FusedSynthesis`` (wgmma kernels,
 planes emitted channel-last).  ``G`` stays the reference's own module and the owner of every
 parameter; its tiny MLPs (mapping network, texture mapper, encoder) run as they are.
 

@@ -1,4 +1,4 @@
-"""Regulariser heads of the generator on the sm_100a point evaluator.
+"""Regulariser heads of the generator on the sm_90a point evaluator.
 
 /root/reference/models/generator.py:520-585: on (nstrata-1)^3 stratified points per image the
 first decoder output d(x) and its spatial gradient feed the eikonal, distance, total-variation

@@ -3,7 +3,7 @@ row tiles of each image: ``render_row_sharded``), one all-gather.
 
 The reference scales with nn.DataParallel: scatter on the batch dimension,
 replicate the module, gather the outputs on GPU 0 (run.py:636-644).  The render
-path has no cross-image arithmetic (SURVEY.md section 8e), so the B200 version
+path has no cross-image arithmetic (SURVEY.md section 8e), so the H100 version
 is: every rank renders its own contiguous slice of the batch with the fused
 kernels and the output tiles are all-gathered so every rank holds the full
 batch (``gather=True``); inversion needs no gradient collective because latents

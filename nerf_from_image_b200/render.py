@@ -72,7 +72,7 @@ def enable_fused_heads(target_model, enabled=True):
 
 
 def enable_fused_synthesis(target_model, enabled=True):
-    """Makes ``render`` produce ``target_model``'s tri-planes with the sm_100a synthesis
+    """Makes ``render`` produce ``target_model``'s tri-planes with the sm_90a synthesis
     kernels (generator.FusedGeneratorFront) for the calls inside their envelope: under
     ``torch.no_grad()`` and without regulariser outputs.  Every other call keeps running the
     reference module's own forward (it needs autograd through the synthesis network)."""
@@ -210,7 +210,7 @@ def render(target_model,
     front = _FRONTS.get(id(target_model))
     hfront = _HEAD_FRONTS.get(id(target_model))
     if front is not None and front.supports(requests, extra_model_inputs):
-        # plane producer on sm_100a too (generator.FusedGeneratorFront; no_grad calls only)
+        # plane producer on sm_90a too (generator.FusedGeneratorFront; no_grad calls only)
         model_outputs = front(viewdirs, model_input, requests, extra_model_inputs)
     elif hfront is not None and hfront.supports(requests, extra_model_inputs):
         # regulariser heads on the fused point evaluator (generator.HeadsGeneratorFront)

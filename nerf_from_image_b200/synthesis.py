@@ -1,16 +1,16 @@
-"""The tri-plane producer on sm_100a: ``SynthesisNetwork.forward`` behind the C ABI.
+"""The tri-plane producer on sm_90a: ``SynthesisNetwork.forward`` behind the C ABI.
 
 ``FusedSynthesis(net)`` wraps the reference's UNMODIFIED ``models.stylegan.SynthesisNetwork``
 (/root/reference/models/stylegan.py:438-490; it stays the owner of every parameter) and runs its
-forward pass with the tcgen05 implicit-GEMM kernels of ``csrc/nfi_synth.cu`` through
+forward pass with the wgmma implicit-GEMM kernels of ``csrc/nfi_synth.cu`` through
 ``nfi_synthesis_forward`` (include/nfi_synth.h).  The call mirrors the module's:
 
     planes_cl = FusedSynthesis(net)(ws, noise_mode='random')     # [B,3,R,R,32] channel-last
 
 i.e. what ``Generator.forward`` obtains at models/generator.py:475-477 as
 ``synthesis_network(w_synthesis, **block_kwargs).view(B,3,32,R,R)``, but already in the layout
-``fused_render(..., planes_layout='channel_last')`` gathers from -- the 0.5 ms / 1.6 GB
-re-layout pass between the two disappears.
+``fused_render(..., planes_layout='channel_last')`` gathers from -- the 1.6 GB re-layout pass
+between the two disappears.
 
 Noise (stylegan.py:332-343): the per-layer ``torch.randn([B,1,res,res]) * noise_strength`` draws
 are made HERE, in the module's layer order and from the same generator, so a seeded run consumes

@@ -1,8 +1,8 @@
 """Run the UNMODIFIED reference hot path -- TEST / BASELINE INFRASTRUCTURE.
 
-/root/reference is mounted read-only in the build container and does not exist
-on the GPU box; there the same files are found, unmodified, under the git-ignored
-``baseline/_ref/`` (staged by ``tools/stage_reference.py`` from ``__graft_entry__.build()``).
+The reference's files are found, unmodified, under the git-ignored ``oracle/_ref/``
+(installed by ``oracle/stage_reference.py`` from ``__graft_entry__.build()`` where a reference
+checkout exists) or under ``$NFI_REFERENCE_ROOT``.
 Everything here is optional: ``available()`` says whether the reference can be
 imported; callers are ``tests/`` (oracle pinning, golden generation, the on-GPU
 ``render()`` drop-in tests) and ``bench.py``'s reference legs (``--impl reference``,
@@ -23,15 +23,14 @@ import warnings
 import torch
 import torch.nn.functional as F
 
-_STAGED = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
-                       'baseline', '_ref')
+_STAGED = os.path.join(os.path.dirname(os.path.abspath(__file__)), '_ref')
 
 
 def _find_root():
-    for cand in (os.environ.get('NFI_REFERENCE_ROOT'), '/root/reference', _STAGED):
+    for cand in (os.environ.get('NFI_REFERENCE_ROOT'), _STAGED):
         if cand and os.path.isfile(os.path.join(cand, 'run.py')):
             return cand
-    return '/root/reference'
+    return _STAGED
 
 
 REFERENCE_ROOT = _find_root()

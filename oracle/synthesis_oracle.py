@@ -3,12 +3,12 @@
 The StyleGAN2 synthesis network that ``Generator.forward`` runs to produce the tri-planes
 (/root/reference/models/generator.py:475-477 -> models/stylegan.py:438-490), restated as plain
 functions over a flat parameter dict so that it can be compared stage by stage with the
-sm_100a kernels of ``nerf_from_image_b200/csrc/nfi_synth.cu`` (SURVEY.md section 8f, N1).
+sm_90a kernels of ``nerf_from_image_b200/csrc/nfi_synth.cu`` (SURVEY.md section 8f, N1).
 Only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s reference legs import it.
 
 Pinned to the reference: ``tests/test_synthesis_oracle.py`` runs the UNMODIFIED
 ``models.stylegan.SynthesisNetwork`` (imported from /root/reference or the staged
-``baseline/_ref``) on the same weights and latents and compares every block; the fixtures under
+``oracle/_ref``) on the same weights and latents and compares every block; the fixtures under
 ``tests/golden/synth/`` were produced by the reference (``tests/golden/make_golden_synth.py``).
 
 Per layer (models/stylegan.py:114-145 ``conv_modulated2d``, :293-356 ``SynthesisLayer``):

@@ -1,11 +1,10 @@
 """Golden vectors of the tri-plane producer, made by the UNMODIFIED reference
-``models.stylegan.SynthesisNetwork`` (/root/reference/models/stylegan.py:438-490) in this
-container:  python tests/golden/make_golden_synth.py
+``models.stylegan.SynthesisNetwork`` (models/stylegan.py:438-490 of the reference checkout that
+oracle/reference_lift.py finds):  python tests/golden/make_golden_synth.py
 
-Small networks (32^2 planes, <= 64 channels, w_dim 128) so that the parameters themselves fit
-in the fixture: the GPU box has no /root/reference, and the kernels are checked there against
-these files (tests/test_synthesis_gpu.py) as well as, where the staged copy exists, against the
-reference module at full size.
+Small networks (8^2 planes, <= 64 channels, w_dim 128) so that the parameters themselves
+fit in the fixture (each file stays under 1 MB): the kernels are checked against these files
+(tests/test_synthesis_gpu.py) wherever the reference is not installed.
 """
 import os
 import sys
@@ -20,8 +19,8 @@ from oracle import synthesis_oracle as SO  # noqa: E402
 
 CASES = {
     # name: (seed, img_resolution, channel_base, channel_max, batch, noise_mode)
-    'synth_c64_const': (11, 32, 2048, 64, 2, 'const'),
-    'synth_mixed_nonoise': (12, 32, 1024, 64, 3, None),
+    'synth_c64_const': (11, 8, 2048, 64, 2, 'const'),
+    'synth_mixed_nonoise': (12, 8, 256, 64, 3, None),
 }
 
 

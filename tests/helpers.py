@@ -1,4 +1,6 @@
 """Shared helpers for the parity tests (oracle side and CUDA side)."""
+import os
+
 import torch
 
 from fixtures import synthetic
@@ -80,3 +82,33 @@ def run_cuda(scene, cams, H, W, S, noise_t, noise_u, use_sdf=True, fine_sampling
 
 def rel_l2(a, b):
     return ((a - b).norm() / b.norm().clamp_min(1e-12)).item()
+
+
+REFERENCE_GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'reference')
+
+
+def _detached(x):
+    if torch.is_tensor(x):
+        return x.detach().clone()
+    if isinstance(x, dict):
+        return {k: _detached(v) for k, v in x.items()}
+    if isinstance(x, (list, tuple)):
+        return type(x)(_detached(v) for v in x)
+    return x
+
+
+def reference_output(request, fn, part=''):
+    """What the reference computes for this test case (``fn`` calls it).  Where the reference is
+    installed (oracle/_ref) it runs live -- and with NFI_RECORD_REFERENCE=1 its output is stored
+    as tests/golden/reference/<test id>.pt -- elsewhere the stored output stands in for it, so
+    that the comparison with the original project runs on every machine."""
+    from oracle import reference_lift as RL
+    name = request.node.name.replace('[', '.').replace(']', '') + part
+    path = os.path.join(REFERENCE_GOLDEN, name + '.pt')
+    if RL.available():
+        out = fn()
+        if os.environ.get('NFI_RECORD_REFERENCE') == '1':
+            os.makedirs(REFERENCE_GOLDEN, exist_ok=True)
+            torch.save(_detached(out), path)
+        return out
+    return torch.load(path, weights_only=True)

@@ -29,7 +29,7 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(lib, name), name
     assert lib.nfi_abi_version() == _lib.ABI_VERSION
     assert ('#define NFI_ABI_VERSION %d' % _lib.ABI_VERSION) in open(HEADER).read()
-    assert b'sm_100a' in lib.nfi_build_info()
+    assert b'sm_90a' in lib.nfi_build_info()
 
 
 def test_struct_layout_matches_header():
@@ -86,7 +86,7 @@ def test_header_is_plain_c_and_links(tmp_path):
     res = subprocess.run([exe], capture_output=True, text=True)
     assert res.returncode == 0, (res.returncode, res.stdout, res.stderr)
     out = res.stdout
-    assert 'abi %d' % _lib.ABI_VERSION in out and 'sm_100a' in out
+    assert 'abi %d' % _lib.ABI_VERSION in out and 'sm_90a' in out
     sizes = re.search(r'sizeof params (\d+) grads (\d+) sample (\d+)', out).groups()
     assert [int(x) for x in sizes] == [ctypes.sizeof(_lib.RenderParams),
                                        ctypes.sizeof(_lib.RenderGrads),

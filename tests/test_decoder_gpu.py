@@ -1,4 +1,4 @@
-"""tcgen05 decoder tile (TriplanarDecoder.net) vs torch fp32 and vs the SIMT path."""
+"""Tensor-core (wgmma) decoder tile (TriplanarDecoder.net) vs torch fp32 and vs the SIMT path."""
 import ctypes
 
 import pytest

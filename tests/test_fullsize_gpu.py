@@ -1,7 +1,7 @@
 """Parity at the BENCHMARKED geometry and of the modes every training / evaluation render
 uses -- the gaps VERDICT round 1 listed (weak #1, #2; ADVICE medium #1, low #1).
 
-* backward of the tcgen05 kernel AND of the fp32 SIMT kernel at BASELINE config-2 geometry
+* backward of the tensor-core kernel AND of the fp32 SIMT kernel at bench config-2 geometry
   (one image, 128x128 rays, 64 + 64 samples, 256^2 planes: 64 tiles on a persistent grid, i.e.
   the multi-wave regime the small tests never reach) and the config-3 orthographic variant,
   against the oracle's autograd run in eager fp32 on the same GPU (TF32 off, run.py:59-60);
@@ -42,7 +42,7 @@ def test_backward_at_benchmark_geometry(cuda_lib, case, mode, wgrad):
     B, H, W, S = 1, 128, 128, 64
     scene, cams = Hh.make_case(case, batch=B, plane_res=256, device='cuda')
     nt, nu = synthetic.make_noise(51, B, H, W, S, device='cuda')
-    # mode 4 (tcgen05; frozen decoder = the inversion setting, or with wgrad the GAN G-step:
+    # mode 4 (tensor cores; frozen decoder = the inversion setting, or with wgrad the GAN G-step:
     # render_backward_pipe + render_wgrad_pipe) / mode 1 (SIMT, decoder weights too)
     names = ['planes', 'palette', 'beta', 'alpha'] + (['w1', 'b1', 'w2', 'b2'] if wgrad else [])
     cam_names = [k for k in ('c2w', 'focal', 'bbox', 'center') if cams[k] is not None]
@@ -50,7 +50,7 @@ def test_backward_at_benchmark_geometry(cuda_lib, case, mode, wgrad):
 
     # Ground truth = the oracle in float64.  (Its float32 run -- what the reference's autograd
     # computes -- is itself 2.3e-3 away from that on the plane gradient of the orthographic
-    # case: tools/grad_diag.py, profiles/r2_grad_diag.txt; it is only used for the image.)
+    # case: tools/grad_diag.py; it is only used for the image.)
     dbl = lambda d: {k: (v.double() if torch.is_tensor(v) else v) for k, v in d.items()}
     sc, cm = _leaves(dbl(scene), dbl(cams), names, cam_names)
     ref = Hh.run_oracle(sc, cm, H, W, S, nt.double(), nu.double())
@@ -64,10 +64,9 @@ def test_backward_at_benchmark_geometry(cuda_lib, case, mode, wgrad):
     assert Hh.rel_l2(rgb.detach(), ref_rgb) < 2e-4
     loss = (rgb * wr).sum() + (mask * wm).sum()
     got = torch.autograd.grad(loss, [sc2[n] for n in names] + [cm2[n] for n in cam_names])
-    # fp32 SIMT / 3xTF32 + MUFU tensor-core backward (measured r2: 3e-5 / 1.2e-4 .. 2.8e-4 on the
-    # plane gradient).  beta is ONE scalar: a sum over every sample of terms whose sign flips
-    # across the surface, so the per-sample 1e-4 shows up amplified by the cancellation
-    # (2e-3 on the bbox case; the fp32 reference autograd itself is at 1.3e-4 there).
+    # fp32 SIMT / 3xTF32 + MUFU tensor-core backward.  beta is ONE scalar: a sum over every sample
+    # of terms whose sign flips across the surface, so a per-sample 1e-4 shows up amplified by the
+    # cancellation.
     for n, a, b in zip(names + cam_names, got, gref):
         err = Hh.rel_l2(a.double(), b)
         tol = 2e-4 if mode == 1 else (5e-3 if n == 'beta' else 1e-3)
@@ -99,7 +98,7 @@ def test_force_no_cam_grad_on_cuda(cuda_lib, mode):
     # (the reference detaches the coarse points, the depths and the directions, run.py:210-214,
     # but builds the FINE points from the attached origins, run.py:286-288, so its autograd
     # still sends a fine-pass-only gradient to the camera position; the fused path cuts the
-    # cameras completely -- DESIGN.md section 6.  The field gradients are unaffected.)
+    # cameras completely.  The field gradients are unaffected.)
     for n, a, b in zip(names, g, gr):
         assert Hh.rel_l2(a, b) < 2e-3, n
 
@@ -186,7 +185,7 @@ def test_channel_last_planes_are_used_as_they_are(cuda_lib):
 def test_generator_step_backward_in_one_sweep(cuda_lib, case, A, kw):
     """The GAN generator step (run.py:1007-1044): gradients to the planes, the palette, beta /
     alpha AND the decoder weights, cameras are data -- render_wgrad_pipe<PLANES>, the whole
-    backward in one tcgen05 sweep -- against the oracle's autograd in float64; every head variant
+    backward in one tensor-core sweep -- against the oracle's autograd in float64; every head variant
     (palettes of 15 / 10 / 3 entries, direct colours, density model, no fine pass, white
     background, orthographic cameras)."""
     torch.backends.cuda.matmul.allow_tf32 = False

@@ -1,4 +1,4 @@
-"""The sm_100a SDF point evaluator (csrc/nfi_heads.cu through nfi_sdf_points_forward / _backward)
+"""The sm_90a SDF point evaluator (csrc/nfi_heads.cu through nfi_sdf_points_forward / _backward)
 and the regulariser heads built on it (nerf_from_image_b200/heads.py) against the oracle
 (oracle/heads_oracle.py, pinned to the reference Generator's own heads): values, first-order
 gradients, and the gradients of the eikonal term -- a double backward in the reference, one

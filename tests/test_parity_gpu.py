@@ -16,7 +16,7 @@ TOL = 2e-4
 
 @pytest.fixture(autouse=True, params=[1, 2, 4], ids=['simt', 'tc', 'pipe'])
 def mlp_mode(request):
-    """Every test below runs with the fp32 SIMT MLP and with the tcgen05
+    """Every test below runs with the fp32 SIMT MLP and with the wgmma
     3xTF32 MLP (S = 16 keeps the fine pass inside the tensor-core kernel's
     S % 16 == 0 envelope; other S fall back under NFI_MLP_AUTO)."""
     Hh.MLP_MODE = request.param
@@ -188,7 +188,7 @@ def test_backward_matches_oracle_autograd(cuda_lib, case):
 def test_backward_frozen_decoder_matches_oracle_autograd(cuda_lib, case):
     """The inversion setting (run.py:628-629: decoder frozen): gradients to the planes,
     palette, beta / alpha and cameras only.  Under the tensor-core mlp modes this is
-    render_backward_pipe (tcgen05, 3xTF32 for all four GEMMs); under 'simt' the fp32 kernel."""
+    render_backward_pipe (wgmma, 3xTF32 for all four GEMMs); under 'simt' the fp32 kernel."""
     B, H, W, S = 2, 12, 20, 16
     scene, cams = Hh.make_case(case, batch=B)
     nt, nu = _noise(29, B, H, W, S)

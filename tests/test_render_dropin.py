@@ -2,7 +2,7 @@
 and ``ParallelModel`` called exactly as run.py calls the reference's, with the reference's own
 UNMODIFIED ``Generator`` as ``target_model``.
 
-Runs on CPU where /root/reference is mounted.  Everything ``render`` does on the host is
+Runs on CPU where the reference is installed (oracle/_ref).  Everything ``render`` does on the host is
 exercised for real -- the generator front-end call, lifting planes / palette / decoder weights
 out of the ``sampler`` closure (``extract_field``, no-copy plane join), the two random draws in
 the reference's order, flag and extra-output handling -- and only the CUDA core
@@ -20,7 +20,7 @@ from oracle import reference_lift as RL
 from oracle import render_oracle as O
 from tests import helpers as Hh
 
-pytestmark = pytest.mark.skipif(not RL.available(), reason='/root/reference not mounted')
+pytestmark = pytest.mark.skipif(not RL.available(), reason='reference not installed (oracle/_ref)')
 
 H, W, S = 10, 14, 8
 
@@ -215,7 +215,7 @@ def test_parallel_model_forward(monkeypatch):
 
 
 def test_front_end_latent_handling_matches_the_generator(monkeypatch):
-    """generator.resolve_ws / resolve_palette (the host logic of both sm_100a front-ends) feed
+    """generator.resolve_ws / resolve_palette (the host logic of both sm_90a front-ends) feed
     the synthesis network and the palette exactly what Generator.forward feeds them
     (models/generator.py:423-468), for z, a single broadcast w and a complete w."""
     from nerf_from_image_b200 import generator as G

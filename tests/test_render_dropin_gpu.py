@@ -3,9 +3,9 @@
 seeded) on CUDA, against the UNMODIFIED reference ``render`` (run.py:176-350, lifted by AST)
 running eagerly in fp32 on the same GPU from the same seed.
 
-/root/reference does not exist on the GPU box: the reference files are staged, unmodified,
-into the git-ignored ``baseline/_ref/`` by ``tools/stage_reference.py`` (run from
-``__graft_entry__.build()``); without them these tests skip and say so.
+The reference files are installed, unmodified, into the git-ignored ``oracle/_ref/`` by
+``oracle/stage_reference.py`` (run from ``__graft_entry__.build()`` where a reference checkout
+exists); without them these tests skip and say so: they need the reference's model classes.
 
 What this pins that the CPU seam test (tests/test_render_dropin.py, CUDA core stood in for
 by the oracle) cannot: closure introspection on CUDA tensors, the no-copy plane join, the
@@ -21,7 +21,7 @@ from oracle import reference_lift as RL
 
 pytestmark = [pytest.mark.gpu,
               pytest.mark.skipif(not RL.available(),
-                                 reason='reference files not staged (tools/stage_reference.py)')]
+                                 reason='reference not installed (oracle/stage_reference.py)')]
 
 H = W = 32
 S = 16
@@ -113,7 +113,7 @@ def test_render_with_viewdir_equals_the_reference_on_cuda(cuda_lib, kw):
 
 
 def test_viewdir_with_the_fused_front_ends(cuda_lib):
-    """--use_viewdir together with enable_fused_synthesis (planes from the tcgen05 synthesis
+    """--use_viewdir together with enable_fused_synthesis (planes from the wgmma synthesis
     kernels, mapper trunk by the reference module) and enable_fused_heads (regulariser outputs)."""
     R, g, cams, ws, ref_render = _setup('p3d_car', use_viewdir=True)
     a = (g, H, W, cams['c2w'], cams['focal'], cams['center'], cams['bbox'], ws, S)
@@ -179,8 +179,8 @@ def test_parallel_model_on_cuda(cuda_lib):
 
 @pytest.mark.parametrize('input_kind', ['ws', 'z', 'w1'])
 def test_render_with_the_fused_plane_producer(cuda_lib, input_kind):
-    """w (or z) -> image entirely on the sm_100a kernels: ``enable_fused_synthesis`` routes the
-    no_grad calls through generator.FusedGeneratorFront (synthesis network on tcgen05, planes
+    """w (or z) -> image entirely on the sm_90a kernels: ``enable_fused_synthesis`` routes the
+    no_grad calls through generator.FusedGeneratorFront (synthesis network on wgmma, planes
     channel-last into the render kernels); the reference render, eager fp32, is the yardstick."""
     R, g, cams, ws, ref_render = _setup('p3d_car')
     model_input = {'ws': ws, 'z': torch.randn(ws.shape[0], 512, device='cuda'),

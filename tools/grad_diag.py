@@ -29,7 +29,7 @@ for case in (sys.argv[1:] or ['p3d_plain', 'cub_ortho', 'p3d_bbox']):
             r = Hh.run_oracle(sc, cm, H, W, S, cast(nt), cast(nu))
             rgb, mask = r['rgb'], r['mask']
         else:
-            if tag == 'tc':  # frozen decoder -> tcgen05 backward
+            if tag == 'tc':  # frozen decoder -> tensor-core backward
                 for k in ('w1', 'b1', 'w2', 'b2'):
                     sc[k] = sc[k].detach()
             rgb, _, mask, _ = Hh.run_cuda(sc, cm, H, W, S, nt, nu, mlp_mode=4 if tag == 'tc' else 1)

@@ -2,7 +2,7 @@
 # Recompiles only the named translation units (pipe render field synth heads viewdir) and relinks.
 # usage: bash tools/rebuild.sh pipe [render ...]
 cd "$(dirname "$0")/../nerf_from_image_b200/csrc" || exit 1
-FLAGS="-O3 -std=c++17 --fmad=false -lineinfo -gencode arch=compute_100a,code=sm_100a -Xcompiler -fPIC -Xcompiler -fvisibility=hidden -I../../include"
+FLAGS="-O3 -std=c++17 --fmad=false -lineinfo -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC -Xcompiler -fvisibility=hidden -I../../include"
 pids=()
 for tu in "$@"; do
   extra=""
@@ -11,5 +11,5 @@ for tu in "$@"; do
   pids+=($!)
 done
 for p in "${pids[@]}"; do wait $p; done
-nvcc -shared -cudart static -gencode arch=compute_100a,code=sm_100a -Xcompiler -fPIC -o libnfi_render.so \
+nvcc -shared -cudart static -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC -o libnfi_render.so \
   nfi_render.o nfi_pipe.o nfi_field.o nfi_synth.o nfi_heads.o nfi_viewdir.o && ls -la libnfi_render.so

@@ -1,5 +1,5 @@
 """Times the plane producer at BASELINE config-2 size (B images, 256^2 x 96 planes, 512-channel
-StyleGAN2 synthesis): the sm_100a kernels (FusedSynthesis) and, where the reference files are
+StyleGAN2 synthesis): the sm_90a kernels (FusedSynthesis) and, where the reference files are
 staged, the reference module in PyTorch eager fp32 (TF32 off, run.py:59-60) on the same GPU.
 Usage: python tools/time_synthesis.py [batch] [steps]"""
 import sys
@@ -12,7 +12,7 @@ torch.backends.cudnn.allow_tf32 = False
 B = int(sys.argv[1]) if len(sys.argv) > 1 else 32
 K = int(sys.argv[2]) if len(sys.argv) > 2 else 5
 if not RL.available():
-    raise SystemExit('reference files not staged (tools/stage_reference.py)')
+    raise SystemExit('reference not installed (oracle/stage_reference.py)')
 RL._import_reference()
 from models import stylegan
 torch.manual_seed(1234)

@@ -1,4 +1,4 @@
-"""Times the tcgen05 backward kernels of the GAN generator step at config-2 geometry: backward()
+"""Times the tensor-core backward kernels of the GAN generator step at config-2 geometry: backward()
 with only the decoder weights requiring grad (render_wgrad_pipe alone), only planes + palette
 (render_backward_pipe alone), both in ONE sweep (render_wgrad_pipe<PLANES>, the default) and both
 as two sweeps (debug bit 0x2000 of mlp_mode).  Usage: python tools/time_wgrad.py [batch]"""

@@ -1,4 +1,4 @@
-"""Decoder-weight gradients of the tcgen05 path (render_backward_pipe + render_wgrad_pipe) against
+"""Decoder-weight gradients of the tensor-core path (render_backward_pipe + render_wgrad_pipe) against
 the fp32 SIMT kernel on the same inputs: per-tensor relative L2 and a few entries.
 Usage: python tools/wgrad_check.py [B H W S R]"""
 import sys, torch
