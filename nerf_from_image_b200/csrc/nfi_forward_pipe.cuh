@@ -7,19 +7,23 @@
 // role only ever does its own kind of work:
 //
 //   persistent CTA (one per SM), one 16x8-pixel tile (128 rays) in flight:
-//     warpgroup 0   ACTIVATION  issues both decoder layers (wgmma, accumulators in its
-//                   registers, one 64-row half of the tile after the other): D1 -> softplus ->
-//                   H_hi / H_lo register A fragments -> D2 -> D2 slot in shared memory
+//     warpgroup 0   ACTIVATION  loads the stage's features as register A fragments, splits
+//                   them into TF32 hi / lo and issues both decoder layers (wgmma, accumulators
+//                   in its registers, one 64-row half of the tile after the other): D1 ->
+//                   softplus -> H_hi / H_lo register A fragments -> D2 -> D2 slot in shared memory
 //     warpgroup 1   SHADING     thread = ray: D2 -> density / colour -> coarse
 //                   weights or sorted merge + compositing (latency-bound chains);
 //                   the two groups put two independent instruction streams on
 //                   every SM sub-partition
 //     warpgroups 2+ P PRODUCER sets of 4 warps; set q gathers the steps n = q (mod P)
-//                   into A stage n mod (P+1) (A_hi/A_lo, 32 KB, SWIZZLE_128B)
+//                   into A stage n mod (P+1) (fp32 features, 16 KB, SWIZZLE_128B)
 //
 //   stage   : producers --full[q]--> activation --a_free[q]--> producers
-//             (a stage is released as soon as layer 1 has READ it; the
-//             hidden activations never come back to shared memory)
+//             (a stage is released as soon as the activation group has loaded its
+//             fragments, before any tensor work; the hidden activations never come
+//             back to shared memory)
+//   L1      : the stages are kept small because every byte of shared memory is taken from
+//             the L1 that serves the plane gather (run_fwd sets the carve-out)
 //   D2 slot : three [128 x 20] fp32 slots: activation --d2_full--> shading --slot_free-->
 //             activation
 //   softplus: ln2 * (max(x', 0) + lg2(1 + 2^-|x'|)) with x' = x log2 e: two MUFU ops (ex2, lg2)
@@ -103,7 +107,7 @@ __device__ __forceinline__ TileCoord tile_coord(int tile, int tiles_x, int tiles
 
 constexpr int kPipeSlots = 3;
 constexpr int kPipeStageBytes = 32768;
-constexpr int kFwdStageBytes = 32768;
+constexpr int kFwdStageBytes = 16384;  // fp32 features of 128 points (the TF32 split is done in registers)
 constexpr int kD2Ld = 20;  // floats per row of a D2 slot (80-byte rows: row reads are conflict-free)
 constexpr int kD2SlotBytes = kThreads * kD2Ld * 4;
 
@@ -127,7 +131,8 @@ struct PipeCfg {
   // setmaxnreg moves registers inside the CTA's launch allocation (threads x launch regs):
   //   P = 3: 640 x 96 = 61440 = 128 x (136 + 80) + 384 x 88 (12 texel loads in flight per
   //   producer warp: 48 data registers + 64-bit addresses + taps; the activation group holds a
-  //   64 x 64 accumulator block and its hi / lo split).
+  //   64 x 64 accumulator block and its hi / lo split, plus the 16 feature values of the second
+  //   64-row half).
   static constexpr int kActRegs = 136;
   static constexpr int kShadeRegs = 80;
   static constexpr int kProducerRegs = 88;
@@ -139,10 +144,28 @@ constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kLn2 = 0.6931471805599453f;
 constexpr float kPadLogit = -1e30f;
 
+// Second half of the decoder for one 64-row block, issued by the whole warpgroup: softplus on the
+// layer-1 accumulator registers, layer 2 with H as register A fragments (24 wgmma), D2 rows to `d2`.
+__device__ __forceinline__ void decoder_layer2(const float (&d)[32], uint64_t w2_hi, uint64_t w2_lo,
+                                               const float* __restrict__ b1, float* d2, int warp,
+                                               int lane) {
+  uint32_t hi[8][4], lo[8][4];
+  tc::softplus_frag<true>(d, b1, lane & 3, hi, lo);
+  float o[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) o[i] = 0.f;
+  tc::wgmma_fence();
+  tc::layer2_mb(o, hi, lo, w2_hi, w2_lo);
+  tc::wgmma_commit();
+  tc::wgmma_wait<0>();
+  tc::reg_fence(o);
+  tc::store_frag_rows(o, d2, kD2Ld, warp, lane);
+}
+
 // The decoder of one 128-point step, issued by the whole (activation) warpgroup: per 64-row
-// half, layer 1 from the A stage (3xTF32, 12 wgmma), softplus on the accumulator registers,
-// layer 2 with H as register A fragments (24 wgmma).  `on_stage_read` runs once layer 1 of both
-// halves has completed (the stage may be refilled); D2 goes to `d2` ([128][kD2Ld]).
+// half, layer 1 from a TF32 hi / lo A stage in shared memory (3xTF32, 12 wgmma), then
+// decoder_layer2.  `on_stage_read` runs once layer 1 of both halves has completed (the stage may
+// be refilled); D2 goes to `d2` ([128][kD2Ld]).
 template <typename F>
 __device__ __forceinline__ void decoder_step(uint64_t dsc_a, uint64_t w1_hi, uint64_t w1_lo,
                                              uint64_t w2_hi, uint64_t w2_lo,
@@ -159,17 +182,43 @@ __device__ __forceinline__ void decoder_step(uint64_t dsc_a, uint64_t w1_hi, uin
     tc::wgmma_wait<0>();
     tc::reg_fence(d);
     if (mb == 1) on_stage_read();
-    uint32_t hi[8][4], lo[8][4];
-    tc::softplus_frag<true>(d, b1, lane & 3, hi, lo);
-    float o[8];
+    decoder_layer2(d, w2_hi, w2_lo, b1, d2 + 64 * mb * kD2Ld, warp, lane);
+  }
+}
+
+// The same decoder from an fp32 feature stage ([128 x 32], SWIZZLE_128B): the warpgroup loads the
+// A fragments of both halves, `on_stage_read` runs (the stage may be refilled before any tensor
+// work on it), and each half is split into TF32 hi / lo in registers exactly as the producers of
+// a hi / lo stage would split it, so layer 1 sees the same operands as decoder_step.
+template <typename F>
+__device__ __forceinline__ void decoder_step_fp32(const unsigned char* stage, uint64_t w1_hi,
+                                                  uint64_t w1_lo, uint64_t w2_hi, uint64_t w2_lo,
+                                                  const float* __restrict__ b1, float* d2, int warp,
+                                                  int lane, F&& on_stage_read) {
+  float fa[4][4], fb[4][4];  // the features of the current half, of the second half
+  tc::load_afrag_sw128(fa, stage, 0, warp, lane);
+  tc::load_afrag_sw128(fb, stage, 64, warp, lane);
+  on_stage_read();
+#pragma unroll 1
+  for (int mb = 0; mb < 2; ++mb) {
+    uint32_t a_hi[4][4], a_lo[4][4];
 #pragma unroll
-    for (int i = 0; i < 8; ++i) o[i] = 0.f;
+    for (int kb = 0; kb < 4; ++kb)
+#pragma unroll
+      for (int s = 0; s < 4; ++s) tc::put_split(a_hi, a_lo, kb, s, fa[kb][s]);
+    float d[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) d[i] = 0.f;
     tc::wgmma_fence();
-    tc::layer2_mb(o, hi, lo, w2_hi, w2_lo);
+    tc::layer1_mb_rs(d, a_hi, a_lo, w1_hi, w1_lo);
     tc::wgmma_commit();
     tc::wgmma_wait<0>();
-    tc::reg_fence(o);
-    tc::store_frag_rows(o, d2 + 64 * mb * kD2Ld, kD2Ld, warp, lane);
+    tc::reg_fence(d);
+    decoder_layer2(d, w2_hi, w2_lo, b1, d2 + 64 * mb * kD2Ld, warp, lane);
+#pragma unroll
+    for (int kb = 0; kb < 4; ++kb)
+#pragma unroll
+      for (int s = 0; s < 4; ++s) fa[kb][s] = fb[kb][s];
   }
 }
 
@@ -461,7 +510,7 @@ render_forward_pipe(const nfi_render_params p, const unsigned char* __restrict__
   uint64_t* bars = reinterpret_cast<uint64_t*>(base + Cfg::kSmBars);
   constexpr int NS = Cfg::kStages;
   uint64_t* full = bars;                         // [NS] stage gathered            (4 warps)
-  uint64_t* a_free = full + NS;                  // [NS] stage read by layer 1     (4 warps)
+  uint64_t* a_free = full + NS;                  // [NS] stage loaded into registers (4 warps)
   uint64_t* d2_full = a_free + NS;               // [3]  D2 slot written           (4 warps)
   uint64_t* slot_free = d2_full + kPipeSlots;    // [3]  D2 read                   (4 warps)
   uint64_t* cw_ready = slot_free + kPipeSlots;   //      coarse weights of the tile written (4 warps)
@@ -627,9 +676,9 @@ render_forward_pipe(const nfi_render_params p, const unsigned char* __restrict__
             tp.o[2] &= 0x7FFu;
           }
           if (!dbg_skip_gather)
-            gather_to_tiles_lean(planes_b, R, tp, stage, stage + 16384, 32 * wig, lane);
+            gather_to_tiles_lean<TileStore::kFp32>(planes_b, R, tp, stage, nullptr, 32 * wig, lane);
           NFI_T(2)
-          tc::fence_async_smem();
+          // the stage is read with generic loads only (no async-proxy fence)
           __syncwarp();
           if (lane == 0) mbar_arrive(&full[st]);
           NFI_T(3)
@@ -648,7 +697,6 @@ render_forward_pipe(const nfi_render_params p, const unsigned char* __restrict__
     const uint64_t dsc_w1_lo = tc::gmma_desc_sw128(base_s + kWiW1Lo);
     const uint64_t dsc_w2_hi = tc::gmma_desc_sw128(base_s + kWiW2Hi);
     const uint64_t dsc_w2_lo = tc::gmma_desc_sw128(base_s + kWiW2Lo);
-    const uint64_t dsc_a0 = tc::gmma_desc_sw128(base_s + Cfg::kSmA);
     uint32_t st = 0, u = 0, sl = 0, v = 0;
     // the next ring position: stage + D2 slot -> decoder -> d2_full, a_free
     auto activate = [&]() {
@@ -659,11 +707,11 @@ render_forward_pipe(const nfi_render_params p, const unsigned char* __restrict__
       NFI_T(0)
       float* d2 = d2s + sl * (kThreads * kD2Ld);
       if (!dbg_skip_consumer) {
-        decoder_step(dsc_a0 + (uint64_t)st * (kFwdStageBytes >> 4), dsc_w1_hi, dsc_w1_lo, dsc_w2_hi,
-                     dsc_w2_lo, b1s, d2, wig, lane, [&]() {
-                       __syncwarp();
-                       if (lane == 0) mbar_arrive(&a_free[st]);
-                     });
+        decoder_step_fp32(base + Cfg::kSmA + st * kFwdStageBytes, dsc_w1_hi, dsc_w1_lo, dsc_w2_hi,
+                          dsc_w2_lo, b1s, d2, wig, lane, [&]() {
+                            __syncwarp();
+                            if (lane == 0) mbar_arrive(&a_free[st]);
+                          });
       } else {
         __syncwarp();
         if (lane == 0) mbar_arrive(&a_free[st]);

@@ -357,11 +357,17 @@ __device__ __forceinline__ float4 ldg_nc_volatile_next(const float4* p) {  // th
                : "l"(p));
   return r;
 }
-// BF16: the features as a bf16 hi/lo PAIR in two [128 rows][32 bf16] SWIZZLE_64B tiles (64-byte
-// rows) instead of the TF32 pair in two SWIZZLE_128B tiles: half the bytes, and a layout that is
-// both the K-major A operand of a kind::f16 layer-1 MMA and -- rows = K -- an MN-major B operand
-// (nfi_wgrad_pipe.cuh).
-template <bool BF16 = false>
+// How gather_to_tiles_lean stores the features of a point (a row of the tile):
+//   kTf32Pair  a TF32 hi/lo PAIR in two [128 rows][32 fp32] SWIZZLE_128B tiles, the shared-memory
+//              A operands of a 3xTF32 layer 1;
+//   kBf16Pair  a bf16 hi/lo PAIR in two [128 rows][32 bf16] SWIZZLE_64B tiles (64-byte rows): half
+//              the bytes, and a layout that is both the K-major A operand of a bf16 layer-1 MMA and
+//              -- rows = K -- an MN-major B operand (nfi_wgrad_pipe.cuh);
+//   kFp32      the fp32 features once, in one SWIZZLE_128B tile laid out like the kTf32Pair hi tile
+//              (`a_lo` unused): the consumer loads its A fragments and splits them in registers
+//              (nfi_forward_pipe.cuh).
+enum class TileStore { kTf32Pair, kBf16Pair, kFp32 };
+template <TileStore MODE = TileStore::kTf32Pair>
 __device__ __forceinline__ void gather_to_tiles_lean(const unsigned char* __restrict__ planes_b,
                                                      int R, const ByteTaps& tp,
                                                      unsigned char* a_hi, unsigned char* a_lo,
@@ -400,7 +406,9 @@ __device__ __forceinline__ void gather_to_tiles_lean(const unsigned char* __rest
     }
     const float third = 0.33333334f;
     const float4 f = make_float4(lo.x * third, lo.y * third, hi.x * third, hi.y * third);
-    if constexpr (BF16) {
+    if constexpr (MODE == TileStore::kFp32) {
+      *reinterpret_cast<float4*>(a_hi + tc::sw128_offset(row0 + src, k)) = f;
+    } else if constexpr (MODE == TileStore::kBf16Pair) {
       uint2 h, l;
       asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(h.x) : "f"(f.y), "f"(f.x));
       asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(h.y) : "f"(f.w), "f"(f.z));

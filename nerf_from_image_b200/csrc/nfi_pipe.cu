@@ -23,12 +23,26 @@ namespace {
     }                                                                                \
   } while (0)
 
+// The forward's plane gather runs out of L1, and on Hopper L1 gets what the shared-memory carve-out
+// leaves of 256 KiB.  The carve-out comes in steps (..., 100, 132, 164, 196, 228 KiB); with the
+// 1 KiB the driver reserves per CTA the forward fits the 132 KiB step, which leaves 124 KiB of L1.
+// A kernel that grows past it takes the 164 KiB step and loses a quarter of that L1.
+constexpr int kSmemPerSm = 228 * 1024, kSmemReservedPerCta = 1024;
+static_assert(PipeCfg<3>::kSmBytes + kSmemReservedPerCta <= 132 * 1024,
+              "render_forward_pipe no longer fits the 132 KiB carve-out step");
+// the smallest carve-out (percent of kSmemPerSm) that holds the kernel: the driver rounds it up
+// to the next step
+constexpr int kFwdCarveoutPct =
+    ((PipeCfg<3>::kSmBytes + kSmemReservedPerCta) * 100 + kSmemPerSm - 1) / kSmemPerSm;
+
 template <int NP, int EX, bool FINE, bool DBG, int NSLOT>
 int run_fwd(const nfi_render_params& p, const unsigned char* wimg, float* scratch, unsigned grid,
             cudaStream_t st, char* err, size_t err_len) {
   auto k = render_forward_pipe<NP, EX, FINE, 3, DBG, NSLOT>;
   NFI_PCUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  PipeCfg<3>::kSmBytes));
+  NFI_PCUDA(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                 kFwdCarveoutPct));
   k<<<grid, PipeCfg<3>::kThreadsTotal, PipeCfg<3>::kSmBytes, st>>>(p, wimg, scratch);
   NFI_PCUDA(cudaGetLastError());
   return 0;

@@ -315,6 +315,35 @@ __device__ __forceinline__ void layer1_mb(float (&d)[32], uint64_t a_hi, uint64_
 #pragma unroll
   for (int ks = 0; ks < 4; ++ks) wgmma_tf32_ss_n64(d, a_hi + 2 * ks, w_hi + 2 * ks, 1);
 }
+// The same 12 products in the same order with A as register fragments (natural K order: k-block
+// kb holds channels 8kb + t at a0 / a1 and 8kb + t + 4 at a2 / a3).
+__device__ __forceinline__ void layer1_mb_rs(float (&d)[32], const uint32_t (&a_hi)[4][4],
+                                             const uint32_t (&a_lo)[4][4], uint64_t w_hi,
+                                             uint64_t w_lo) {
+  wgmma_tf32_rs_n64(d, a_lo[0], w_hi, 0);
+#pragma unroll
+  for (int ks = 1; ks < 4; ++ks) wgmma_tf32_rs_n64(d, a_lo[ks], w_hi + 2 * ks, 1);
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) wgmma_tf32_rs_n64(d, a_hi[ks], w_lo + 2 * ks, 1);
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) wgmma_tf32_rs_n64(d, a_hi[ks], w_hi + 2 * ks, 1);
+}
+// A fragments of the 64-row block at `row0` of an fp32 [rows x 32] SWIZZLE_128B tile, in the order
+// layer1_mb_rs takes them.  The 8 rows a warp reads at once sit in 8 different 16-byte chunks of
+// their 128-byte rows, so each of the 16 loads is free of bank conflicts.
+__device__ __forceinline__ void load_afrag_sw128(float (&f)[4][4], const unsigned char* tile,
+                                                 int row0, int warp, int lane) {
+  const int g = lane >> 2, t = lane & 3;
+  const int r = row0 + 16 * warp + g;
+#pragma unroll
+  for (int kb = 0; kb < 4; ++kb) {
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      const int row = r + 8 * (s & 1), chunk = 2 * kb + (s >> 1);
+      f[kb][s] = *reinterpret_cast<const float*>(tile + sw128_offset(row, chunk) + 4 * t);
+    }
+  }
+}
 // Layer 2, D[64 x 16] = H W2^T with H as register fragments (hi / lo, 8 k-blocks): 24 wgmma.
 // W2 hi / lo: [16 x 64] as two [16 x 32] SWIZZLE_128B K-blocks of 2048 bytes.
 __device__ __forceinline__ void layer2_mb(float (&o)[8], const uint32_t (&hhi)[8][4],

@@ -217,7 +217,7 @@ render_wgrad_pipe(const nfi_render_params p, const nfi_render_grads g,
         const uint32_t st = m % NS, u = m / NS;
         unsigned char* const stage = base + Cfg::kSmA + st * Cfg::kStageBytes;
         NFI_STEP_WAIT(&a_free[st], (u & 1) ^ 1);
-        gather_to_tiles_lean<true>(planes_b, R, tp, stage, stage + 8192, 32 * wig, lane);
+        gather_to_tiles_lean<TileStore::kBf16Pair>(planes_b, R, tp, stage, stage + 8192, 32 * wig, lane);
         tc::fence_async_smem();
         __syncwarp();
         if (lane == 0) mbar_arrive(&full[st]);
