@@ -20,8 +20,15 @@
  * prologue (style scaling) folded into the producing layer's epilogue, epilogue (demodulation,
  * noise, bias, gain, leaky-relu, next layer's style, hi/lo split) fused.  Conventions as in nfi_render.h:
  * device pointers, fp32, stream as void*, 0 = success, text via nfi_last_error().
- * Forward only: callers that differentiate through the synthesis network (inversion, GAN
- * training) keep the reference module, which this entry point never falls back to.
+ * Backward to the latents (the inversion setting: every network parameter frozen):
+ * nfi_synthesis_forward_saved runs the same forward -- the same planes, bit for bit -- and also
+ * keeps each layer's pre-activation u in the workspace; nfi_synthesis_backward then turns the
+ * planes' gradient into the gradient of ws.  Its data-gradient GEMMs run on the same TMA + wgmma
+ * kernel with the weights re-laid-out [tap][Cin][Cout]; the up layer's adjoint is the FIR's
+ * (a correlation with the same symmetric taps) split into the four parity phases of the
+ * (2R+1)^2 raw gradient, then nine stride-1 taps over them.  Gradients to the weights, biases,
+ * affines, noise and b4.const are not computed (the GAN generator step keeps the reference
+ * module, which these entry points never fall back to).
  */
 #ifndef NFI_SYNTH_H_
 #define NFI_SYNTH_H_
@@ -67,6 +74,23 @@ typedef struct nfi_synth_params {
 
 NFI_API size_t nfi_synthesis_workspace_bytes(const nfi_synth_params *params);
 NFI_API int nfi_synthesis_forward(const nfi_synth_params *params, void *stream);
+
+/* Upstream gradient in, latent gradient out. */
+typedef struct nfi_synth_grads {
+  const float *g_planes; /* [B,3,R,R,32] channel-last dL/dplanes (nfi_render_backward's grad_planes
+                            for channel-last planes) */
+  float *g_ws;           /* [B,num_ws,w_dim] ACCUMULATED (+=) like nfi_render_grads */
+} nfi_synth_grads;
+
+/* Workspace of a saved forward and the backward that reads it: the forward's buffers, every
+   layer's pre-activation (fp32, channel-last) and the backward's scratch. */
+NFI_API size_t nfi_synthesis_saved_workspace_bytes(const nfi_synth_params *params);
+/* nfi_synthesis_forward, plus the tensors the backward reads, left in params->workspace
+   (>= nfi_synthesis_saved_workspace_bytes). */
+NFI_API int nfi_synthesis_forward_saved(const nfi_synth_params *params, void *stream);
+/* The same params (same ws, weights, noise) and the workspace as the saved forward left it. */
+NFI_API int nfi_synthesis_backward(const nfi_synth_params *params, const nfi_synth_grads *grads,
+                                   void *stream);
 
 #ifdef __cplusplus
 }

@@ -103,6 +103,11 @@ class SynthParams(ctypes.Structure):
     ]
 
 
+class SynthGrads(ctypes.Structure):
+    """struct nfi_synth_grads."""
+    _fields_ = [('g_planes', ctypes.c_void_p), ('g_ws', ctypes.c_void_p)]
+
+
 class SdfPointsParams(ctypes.Structure):
     """struct nfi_sdf_points_params (include/nfi_heads.h)."""
     _fields_ = [('batch', ctypes.c_int32), ('plane_res', ctypes.c_int32),
@@ -149,6 +154,10 @@ EXPORTS = {
                                                ctypes.POINTER(SdfPointsGrads), ctypes.c_void_p]),
     'nfi_synthesis_workspace_bytes': (ctypes.c_size_t, [ctypes.POINTER(SynthParams)]),
     'nfi_synthesis_forward': (ctypes.c_int, [ctypes.POINTER(SynthParams), ctypes.c_void_p]),
+    'nfi_synthesis_saved_workspace_bytes': (ctypes.c_size_t, [ctypes.POINTER(SynthParams)]),
+    'nfi_synthesis_forward_saved': (ctypes.c_int, [ctypes.POINTER(SynthParams), ctypes.c_void_p]),
+    'nfi_synthesis_backward': (ctypes.c_int, [ctypes.POINTER(SynthParams),
+                                              ctypes.POINTER(SynthGrads), ctypes.c_void_p]),
     'nfi_pose_to_matrix': (ctypes.c_int, [
         ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32,
         ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),

@@ -657,6 +657,24 @@ int nfi_synthesis_forward(const nfi_synth_params* params, void* stream) {
   return nfi::synth::forward(*params, (cudaStream_t)stream, g_err, sizeof(g_err));
 }
 
+size_t nfi_synthesis_saved_workspace_bytes(const nfi_synth_params* params) {
+  if (params == nullptr) return 0;
+  return nfi::synth::saved_workspace_bytes(*params);
+}
+
+int nfi_synthesis_forward_saved(const nfi_synth_params* params, void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  if (params->batch <= 0) return fail("empty batch");
+  return nfi::synth::forward_saved(*params, (cudaStream_t)stream, g_err, sizeof(g_err));
+}
+
+int nfi_synthesis_backward(const nfi_synth_params* params, const nfi_synth_grads* grads, void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  if (grads == nullptr) return fail("grads is NULL");
+  if (params->batch <= 0) return fail("empty batch");
+  return nfi::synth::backward(*params, *grads, (cudaStream_t)stream, g_err, sizeof(g_err));
+}
+
 int nfi_render_forward_host(const nfi_render_params* hp, int32_t device) {
   // Host buffers in, host buffers out.  The batch is cut into chunks of images
   // (images are independent: SURVEY.md section 8e) and pipelined over two

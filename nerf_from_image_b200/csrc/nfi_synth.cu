@@ -71,6 +71,7 @@ struct ActEpilogue {   // shared by conv_tc_kernel (stride-1 layers) and fir_act
   const float* style_b;  // second consumer or nullptr
   __nv_bfloat16* b_hi;
   __nv_bfloat16* b_lo;
+  float* u_out;          // [B,H,W,N] pre-activation u for the backward, or nullptr (plain forward)
 };
 
 struct ConvArgs {
@@ -84,6 +85,7 @@ struct ConvArgs {
   int ph_tile0[kMaxPhases + 1];                    // first m-tile of the phase (per image count)
   int ph_oy[kMaxPhases], ph_ox[kMaxPhases];        // RAW: output offset of the phase
   int tap_dy[kMaxTaps], tap_dx[kMaxTaps], tap_w[kMaxTaps];
+  int tap_img[kMaxTaps];        // image offset of the tap's A box (backward phase maps; else 0)
   int mode;
   // RAW
   float* out_raw;
@@ -179,9 +181,12 @@ __device__ __forceinline__ void act_store2(const ActEpilogue& e, int img, size_t
                                            float2 acc, float noise) {
   const float2 d = __ldg(reinterpret_cast<const float2*>(e.dcoef + (size_t)img * N + n));
   const float2 b = __ldg(reinterpret_cast<const float2*>(e.bias + n));
-  float2 v;
-  v.x = lrelu(((acc.x * d.x + noise) + b.x) * e.gain);
-  v.y = lrelu(((acc.y * d.y + noise) + b.y) * e.gain);
+  float2 u, v;
+  u.x = ((acc.x * d.x + noise) + b.x) * e.gain;
+  u.y = ((acc.y * d.y + noise) + b.y) * e.gain;
+  if (e.u_out != nullptr) *reinterpret_cast<float2*>(e.u_out + pos * N + n) = u;
+  v.x = lrelu(u.x);
+  v.y = lrelu(u.y);
   const float2 one = make_float2(1.f, 1.f);
   if (e.a_hi != nullptr) {
     const float2 s = e.style_a ? __ldg(reinterpret_cast<const float2*>(e.style_a + (size_t)img * N + n)) : one;
@@ -197,11 +202,16 @@ __device__ __forceinline__ void act_store4(const ActEpilogue& e, int img, size_t
                                            float4 acc, float noise) {
   const float4 d = __ldg(reinterpret_cast<const float4*>(e.dcoef + (size_t)img * N + n));
   const float4 b = __ldg(reinterpret_cast<const float4*>(e.bias + n));
-  float4 v;
-  v.x = lrelu(((acc.x * d.x + noise) + b.x) * e.gain);
-  v.y = lrelu(((acc.y * d.y + noise) + b.y) * e.gain);
-  v.z = lrelu(((acc.z * d.z + noise) + b.z) * e.gain);
-  v.w = lrelu(((acc.w * d.w + noise) + b.w) * e.gain);
+  float4 u, v;
+  u.x = ((acc.x * d.x + noise) + b.x) * e.gain;
+  u.y = ((acc.y * d.y + noise) + b.y) * e.gain;
+  u.z = ((acc.z * d.z + noise) + b.z) * e.gain;
+  u.w = ((acc.w * d.w + noise) + b.w) * e.gain;
+  if (e.u_out != nullptr) *reinterpret_cast<float4*>(e.u_out + pos * N + n) = u;
+  v.x = lrelu(u.x);
+  v.y = lrelu(u.y);
+  v.z = lrelu(u.z);
+  v.w = lrelu(u.w);
   const float4 one = make_float4(1.f, 1.f, 1.f, 1.f);
   if (e.a_hi != nullptr) {
     const float4 s = e.style_a ? __ldg(reinterpret_cast<const float4*>(e.style_a + (size_t)img * N + n)) : one;
@@ -405,12 +415,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
         const int tap0 = a.ph_tap0[t.phase];
         for (int tp = 0; tp < a.ph_taps[t.phase]; ++tp) {
           const int dy = a.tap_dy[tap0 + tp], dx = a.tap_dx[tap0 + tp], tw = a.tap_w[tap0 + tp];
+          const int im = t.img + a.tap_img[tap0 + tp];
           for (int kb = 0; kb < kblocks; ++kb) {
             tc::mbar_wait(&empty[st], ph ^ 1);
             unsigned char* s = smem + st * stage_bytes;
             tc::mbar_expect_tx(&full[st], (uint32_t)stage_bytes);
-            tma_load_4d(s, &tmAh, kb * kKBlock, x0 + dx, y0 + dy, t.img, &full[st]);
-            tma_load_4d(s + kATile, &tmAl, kb * kKBlock, x0 + dx, y0 + dy, t.img, &full[st]);
+            tma_load_4d(s, &tmAh, kb * kKBlock, x0 + dx, y0 + dy, im, &full[st]);
+            tma_load_4d(s + kATile, &tmAl, kb * kKBlock, x0 + dx, y0 + dy, im, &full[st]);
             tma_load_3d(s + 2 * kATile, &tmWh, kb * kKBlock, n0, tw, &full[st]);
             tma_load_3d(s + 2 * kATile + w_tile, &tmWl, kb * kKBlock, n0, tw, &full[st]);
             if (++st == kStages) { st = 0; ph ^= 1; }
@@ -548,6 +559,236 @@ __global__ void const_input_kernel(const float* __restrict__ cst, const float* _
   }
 }
 
+// ------------------------------------------------------------------ backward to the latents
+// The data gradients dx~ = conv^T(dacc, W) run on conv_tc_kernel (RAW mode) with the weights
+// re-laid-out below; everything between two GEMMs of a layer is ONE full-resolution pass
+// (act_backward_kernel), plus the FIR adjoint for the up layers.
+
+// weight [Cout,Cin,K,K] -> [K*K][Cin][Cout] hi / lo: the B operand of the data-gradient GEMM
+// (reduction over Cout).  The stride-1 layer's tap flip lives in the tap table, not here.
+__global__ void prep_weights_t_kernel(const float* __restrict__ w, int cout, int cin, int taps,
+                                      __nv_bfloat16* __restrict__ w_hi,
+                                      __nv_bfloat16* __restrict__ w_lo) {
+  const size_t total = (size_t)cout * cin;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (size_t)gridDim.x * blockDim.x) {
+    const size_t ci = i / cout, o = i - ci * cout;   // output index (ci, o): o fastest
+    for (int t = 0; t < taps; ++t)
+      split_bf16(w[(o * cin + ci) * taps + t], w_hi[(size_t)t * total + i], w_lo[(size_t)t * total + i]);
+  }
+}
+
+struct ActBackward {
+  const float* u;       // [B,HW,C] saved pre-activation of the layer
+  const float* noise;   // [B,HW] or nullptr
+  const float* bias;    // [C]
+  const float* dcoef;   // [B,C]
+  float gain;           // sqrt(2)
+  // up to two consumers of v = lrelu(u): the gradient of their STYLED input (dx~), their style s,
+  // and ds[b,c] += sum_pos dx~ v (the data half of their style gradient)
+  const float* dx_a; const float* s_a; float* ds_a;
+  const float* dx_b; const float* s_b; float* ds_b;
+  float* dd;            // [B,C] += sum_pos g (acc d),  g = dv lrelu'(u) gain
+  __nv_bfloat16* dacc_hi;  // dacc = g d as a pair (input of the next data-gradient GEMM) ...
+  __nv_bfloat16* dacc_lo;
+  float* dacc;             // ... or fp32 (input of the FIR adjoint)
+};
+
+__device__ __forceinline__ float lrelu_grad(float u) { return u > 0.f ? 1.f : 0.2f; }
+
+// One pass over a layer's output: dv = dx~_a s_a + dx~_b s_b, then dacc = dv lrelu'(u) gain d, and
+// the per-(b, channel) sums ds_a, ds_b, dd.  Block (chunk, b): 4 channels per thread, 256 / (C/4)
+// positions in parallel; the sums are reduced in shared memory, then one atomic per block.
+__global__ void __launch_bounds__(256)
+act_backward_kernel(ActBackward e, int HW, int C, int chunk) {
+  __shared__ float4 red[3][256];
+  const int cg = C >> 2, ppar = 256 / cg, tid = threadIdx.x;
+  const int p = tid / cg, c4 = tid - p * cg;
+  const int b = blockIdx.y;
+  const bool active = p < ppar;
+  const float inv_gain = 1.f / e.gain;
+  float4 sa = make_float4(0.f, 0.f, 0.f, 0.f), sb = sa, sd = sa;
+  if (active) {
+    const float4 d = *reinterpret_cast<const float4*>(e.dcoef + (size_t)b * C + 4 * c4);
+    const float4 bi = *reinterpret_cast<const float4*>(e.bias + 4 * c4);
+    const float4 one = make_float4(1.f, 1.f, 1.f, 1.f);
+    const float4 s_a = e.s_a ? *reinterpret_cast<const float4*>(e.s_a + (size_t)b * C + 4 * c4) : one;
+    const float4 s_b = e.s_b ? *reinterpret_cast<const float4*>(e.s_b + (size_t)b * C + 4 * c4) : one;
+    const int end = min(HW, (blockIdx.x + 1) * chunk);
+    for (int pos = blockIdx.x * chunk + p; pos < end; pos += ppar) {
+      const size_t row = (size_t)b * HW + pos, idx = row * C + 4 * c4;
+      const float4 u = __ldg(reinterpret_cast<const float4*>(e.u + idx));
+      const float nz = e.noise ? __ldg(e.noise + row) : 0.f;
+      float4 dv = make_float4(0.f, 0.f, 0.f, 0.f);
+#define NFI_CONSUMER(dx, s, acc)                                                    \
+  if (dx != nullptr) {                                                              \
+    const float4 x = __ldg(reinterpret_cast<const float4*>(dx + idx));              \
+    acc.x = fmaf(x.x, lrelu(u.x), acc.x); acc.y = fmaf(x.y, lrelu(u.y), acc.y);     \
+    acc.z = fmaf(x.z, lrelu(u.z), acc.z); acc.w = fmaf(x.w, lrelu(u.w), acc.w);     \
+    dv.x = fmaf(x.x, s.x, dv.x); dv.y = fmaf(x.y, s.y, dv.y);                       \
+    dv.z = fmaf(x.z, s.z, dv.z); dv.w = fmaf(x.w, s.w, dv.w);                       \
+  }
+      NFI_CONSUMER(e.dx_a, s_a, sa)
+      NFI_CONSUMER(e.dx_b, s_b, sb)
+#undef NFI_CONSUMER
+      float4 g, out;
+#define NFI_G(cmp)                                                                   \
+  g.cmp = dv.cmp * lrelu_grad(u.cmp) * e.gain;                                       \
+  sd.cmp = fmaf(g.cmp, u.cmp * inv_gain - nz - bi.cmp, sd.cmp);  /* acc d = u/gain - noise - bias */ \
+  out.cmp = g.cmp * d.cmp;
+      NFI_G(x) NFI_G(y) NFI_G(z) NFI_G(w)
+#undef NFI_G
+      if (e.dacc_hi != nullptr) store_split4(e.dacc_hi, e.dacc_lo, idx, out, one);
+      if (e.dacc != nullptr) *reinterpret_cast<float4*>(e.dacc + idx) = out;
+    }
+  }
+  red[0][tid] = sa;
+  red[1][tid] = sb;
+  red[2][tid] = sd;
+  __syncthreads();
+  if (tid < cg) {
+    float* dst[3] = {e.ds_a, e.ds_b, e.dd};
+#pragma unroll
+    for (int q = 0; q < 3; ++q) {
+      if (dst[q] == nullptr) continue;
+      float4 s = red[q][tid];
+      for (int k = 1; k < ppar; ++k) {
+        const float4 t = red[q][k * cg + tid];
+        s.x += t.x; s.y += t.y; s.z += t.z; s.w += t.w;
+      }
+      float* o = dst[q] + (size_t)b * C + 4 * tid;
+      atomicAdd(o + 0, s.x);
+      atomicAdd(o + 1, s.y);
+      atomicAdd(o + 2, s.z);
+      atomicAdd(o + 3, s.w);
+    }
+  }
+}
+
+// Adjoint of the up layer's 4x4 FIR (symmetric, so a correlation with the same taps), written as
+// the four parity phases of the (2H+1)^2 raw gradient: phase (py,px) at image offset (2py+px)*B of
+// a [4B, H+1, W+1, C] pair, position (a,b) = raw (2a+py, 2b+px); entries past the raw extent are 0.
+__global__ void fir_adjoint_kernel(const float* __restrict__ dacc, int B, int OH, int OW, int C,
+                                   __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo) {
+  const int PH = OH / 2 + 1, PW = OW / 2 + 1, groups = C >> 2;
+  const size_t total = (size_t)4 * B * PH * PW * groups;
+  const float kf[4] = {0.25f, 0.75f, 0.75f, 0.25f};
+  const float4 one = make_float4(1.f, 1.f, 1.f, 1.f);
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (size_t)gridDim.x * blockDim.x) {
+    const int g = (int)(i % groups);
+    size_t r = i / groups;
+    const int bx = (int)(r % PW); r /= PW;
+    const int ay = (int)(r % PH); r /= PH;
+    const int img = (int)(r % B);
+    const int phase = (int)(r / B);
+    const int ry = 2 * ay + (phase >> 1), rx = 2 * bx + (phase & 1);
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (ry <= OH && rx <= OW) {
+#pragma unroll
+      for (int ka = 0; ka < 4; ++ka) {
+        const int y = ry - ka + 1;
+        if (y < 0 || y >= OH) continue;
+#pragma unroll
+        for (int kb = 0; kb < 4; ++kb) {
+          const int x = rx - kb + 1;
+          if (x < 0 || x >= OW) continue;
+          const float w = kf[ka] * kf[kb];
+          const float4 t = __ldg(reinterpret_cast<const float4*>(dacc + (((size_t)img * OH + y) * OW + x) * C) + g);
+          acc.x = fmaf(w, t.x, acc.x); acc.y = fmaf(w, t.y, acc.y);
+          acc.z = fmaf(w, t.z, acc.z); acc.w = fmaf(w, t.w, acc.w);
+        }
+      }
+    }
+    store_split4(hi, lo, i * 4, acc, one);
+  }
+}
+
+// d(planes) [B,3,R,R,32] -> d(image) [B,R,R,96] (channel nn = plane * 32 + c), fp32 and as a pair
+__global__ void planes_grad_kernel(const float* __restrict__ gp, int B, int R, float* __restrict__ out,
+                                   __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo) {
+  const size_t total = (size_t)B * R * R * 96;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (size_t)gridDim.x * blockDim.x) {
+    const int nn = (int)(i % 96);
+    const size_t pix = i / 96, img = pix / ((size_t)R * R), yx = pix - img * R * R;
+    const float v = gp[((img * 3 + nn / 32) * R * R + yx) * 32 + (nn & 31)];
+    out[i] = v;
+    split_bf16(v, hi[i], lo[i]);
+  }
+}
+
+// Adjoint of upsample_img (stylegan.py:71-75) per axis: din[i] = 3/4 (dout[2i] + dout[2i+1]) +
+// 1/4 (dout[2i-1] + dout[2i+2]); [B,2h,2w,C] -> [B,h,w,C], fp32 and as a pair
+__global__ void upsample_adjoint_kernel(const float* __restrict__ dout, int B, int h, int w, int C,
+                                        float* __restrict__ out, __nv_bfloat16* __restrict__ hi,
+                                        __nv_bfloat16* __restrict__ lo) {
+  const size_t total = (size_t)B * h * w * C;
+  const float kf[4] = {0.25f, 0.75f, 0.75f, 0.25f};
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (size_t)gridDim.x * blockDim.x) {
+    const int c = (int)(i % C);
+    size_t r = i / C;
+    const int x = (int)(r % w); r /= w;
+    const int y = (int)(r % h);
+    const int img = (int)(r / h);
+    float acc = 0.f;
+    for (int a = 0; a < 4; ++a) {
+      const int Y = 2 * y - 1 + a;
+      if (Y < 0 || Y >= 2 * h) continue;
+      for (int bb = 0; bb < 4; ++bb) {
+        const int X = 2 * x - 1 + bb;
+        if (X < 0 || X >= 2 * w) continue;
+        acc = fmaf(kf[a] * kf[bb], dout[(((size_t)img * 2 * h + Y) * 2 * w + X) * C + c], acc);
+      }
+    }
+    out[i] = acc;
+    split_bf16(acc, hi[i], lo[i]);
+  }
+}
+
+// The demodulation chain: d = rsqrt(sum_o' wsq s^2 + 1e-8) gives dd/ds_i = -d^3 wsq[o,i] s_i, and
+// dd_true = dd_part / d (act_backward_kernel sums g (acc d)), so
+// ds[b,i] -= s_i sum_o dd_part[b,o] d[b,o]^2 wsq[o,i]; one warp per (b, i)
+__global__ void dcoef_backward_kernel(const float* __restrict__ wsq, const float* __restrict__ s,
+                                      const float* __restrict__ dd, const float* __restrict__ d,
+                                      int cout, int cin, int B, float* __restrict__ ds) {
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (warp >= B * cin) return;
+  const int b = warp / cin, i = warp % cin;
+  float acc = 0.f;
+  for (int o = lane; o < cout; o += 32) {
+    const float dv = d[(size_t)b * cout + o];
+    acc = fmaf(dd[(size_t)b * cout + o] * dv * dv, wsq[(size_t)o * cin + i], acc);
+  }
+#pragma unroll
+  for (int k = 16; k > 0; k >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, k);
+  if (lane == 0) ds[warp] -= s[warp] * acc;
+}
+
+// block 0's conv1 reads b4.const * style: ds[b,c] += sum_p dx~[b,p,c] const[c,p]
+__global__ void const_ds_kernel(const float* __restrict__ dx, const float* __restrict__ cst, int B,
+                                int C, float* __restrict__ ds) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B * C) return;
+  const int b = i / C, c = i % C;
+  float acc = 0.f;
+  for (int p = 0; p < 16; ++p) acc = fmaf(dx[((size_t)b * 16 + p) * C + c], cst[c * 16 + p], acc);
+  ds[i] += acc;
+}
+
+// The transpose of styles_kernel: g_ws[b,row,k] += gain / sqrt(w_dim) sum_c ds[b,c] A[c,k]
+__global__ void styles_backward_kernel(const float* __restrict__ ds, const float* __restrict__ aw,
+                                       int cin, int w_dim, int B, float scale, float* __restrict__ g_ws,
+                                       int ws_stride) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B * w_dim) return;
+  const int b = i / w_dim, k = i % w_dim;
+  float acc = 0.f;
+  for (int c = 0; c < cin; ++c) acc = fmaf(ds[(size_t)b * cin + c], aw[(size_t)c * w_dim + k], acc);
+  g_ws[(size_t)b * ws_stride + k] += scale * acc;
+}
+
 // ------------------------------------------------------------------ host side
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
                                   const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
@@ -618,9 +859,9 @@ static int sm_count() {
   return n;
 }
 
-// One convolution launch.  `in` [B,H,W,C] pair, weights [taps9][N][C] pair.
+// One convolution launch.  `in` [map_B (default B),H,W,C] pair, weights [taps9][N][C] pair.
 static int launch_conv(ConvArgs& a, Pair in, Pair wt, int w_taps, cudaStream_t st, char* err,
-                       size_t err_len) {
+                       size_t err_len, int map_B = 0) {
   if (encode_fn() == nullptr) {
     snprintf(err, err_len, "cuTensorMapEncodeTiled is not available from this driver");
     return 1;
@@ -642,7 +883,8 @@ static int launch_conv(ConvArgs& a, Pair in, Pair wt, int w_taps, cudaStream_t s
   a.ph_tile0[a.n_phases] = m_tiles;
   const int n_tiles = m_tiles * a.B * a.n_tiles_n;
   CUtensorMap tAh, tAl, tWh, tWl;
-  if (!make_act_map(&tAh, in.hi, a.B, a.H, a.W, a.C) || !make_act_map(&tAl, in.lo, a.B, a.H, a.W, a.C) ||
+  if (map_B == 0) map_B = a.B;
+  if (!make_act_map(&tAh, in.hi, map_B, a.H, a.W, a.C) || !make_act_map(&tAl, in.lo, map_B, a.H, a.W, a.C) ||
       !make_w_map(&tWh, wt.hi, w_taps, a.N, a.C, a.BN) || !make_w_map(&tWl, wt.lo, w_taps, a.N, a.C, a.BN)) {
     snprintf(err, err_len, "cuTensorMapEncodeTiled failed (B %d H %d W %d C %d N %d)", a.B, a.H, a.W,
              a.C, a.N);
@@ -738,8 +980,25 @@ static int check_params(const nfi_synth_params& P, char* err, size_t err_len) {
   return 0;
 }
 
-// Runs (or, with base == nullptr, only sizes) the whole network.
-static int run(const nfi_synth_params& P, Bump& ws, cudaStream_t st, bool dry, char* err, size_t err_len) {
+// What the backward reads of a saved forward: pointers into the workspace, recovered by walking the
+// same (deterministic) bump allocation again without launching anything.
+struct Saved {
+  float* style0[NFI_SYNTH_MAX_BLOCKS];
+  float* style1[NFI_SYNTH_MAX_BLOCKS];
+  float* style_rgb[NFI_SYNTH_MAX_BLOCKS];
+  float* dco0[NFI_SYNTH_MAX_BLOCKS];
+  float* dco1[NFI_SYNTH_MAX_BLOCKS];
+  float* wsq0[NFI_SYNTH_MAX_BLOCKS];
+  float* wsq1[NFI_SYNTH_MAX_BLOCKS];
+  float* u0[NFI_SYNTH_MAX_BLOCKS];  // pre-activations [B,res,res,cout] (save mode)
+  float* u1[NFI_SYNTH_MAX_BLOCKS];
+  int row0[NFI_SYNTH_MAX_BLOCKS], row1[NFI_SYNTH_MAX_BLOCKS], row_rgb[NFI_SYNTH_MAX_BLOCKS];
+};
+
+// Runs (or, with dry, only lays out) the whole network.  With `sv`, the forward also stores every
+// layer's pre-activation u (the save mode) and `sv` receives the pointers the backward reads.
+static int run(const nfi_synth_params& P, Bump& ws, cudaStream_t st, bool dry, char* err, size_t err_len,
+               Saved* sv = nullptr) {
   const int B = P.batch, nb = P.num_blocks, D = P.w_dim;
   const float sqrt2 = 1.4142135623730951f;
   auto blocks = [](size_t n, int per) { return (unsigned)((n + per - 1) / per); };
@@ -762,9 +1021,10 @@ static int run(const nfi_synth_params& P, Bump& ws, cudaStream_t st, bool dry, c
             P.ws + (size_t)widx * D, P.num_ws * D, D, L.affine_w, L.affine_b, c, B, gain, s);
       return s;
     };
+    float* wsq = nullptr;
     auto weights = [&](const nfi_synth_layer& L, int co, int ci, int taps, float* s, Pair& w) -> float* {
       w = ws.pair((size_t)taps * co * ci);
-      float* wsq = taps > 1 ? ws.take((size_t)co * ci) : nullptr;
+      wsq = taps > 1 ? ws.take((size_t)co * ci) : nullptr;
       float* d = taps > 1 ? ws.take((size_t)B * co) : nullptr;
       if (!dry) {
         prep_weights_kernel<<<blocks((size_t)co * ci, 256), 256, 0, st>>>(L.weight, co, ci, taps, w.hi,
@@ -777,13 +1037,26 @@ static int run(const nfi_synth_params& P, Bump& ws, cudaStream_t st, bool dry, c
     if (i) {
       style0[i] = style(P.conv0[i], cin, w_idx, 1.f);
       dco0[i] = weights(P.conv0[i], cout, cin, 9, style0[i], w0[i]);
+      if (sv) { sv->wsq0[i] = wsq; sv->row0[i] = w_idx; }
     }
     style1[i] = style(P.conv1[i], cout, w_idx + n_conv - 1, 1.f);
     dco1[i] = weights(P.conv1[i], cout, cout, 9, style1[i], w1[i]);
+    if (sv) { sv->wsq1[i] = wsq; sv->row1[i] = w_idx + n_conv - 1; }
     // OutputLayer: styles * 1/sqrt(cin * 1 * 1), no demodulation (stylegan.py:369,372-376)
     style_rgb[i] = style(P.torgb[i], cout, w_idx + n_conv, 1.f / sqrtf((float)cout));
     weights(P.torgb[i], P.img_channels, cout, 1, nullptr, wrgb[i]);
+    if (sv) sv->row_rgb[i] = w_idx + n_conv;
     w_idx += n_conv;
+  }
+
+  if (sv) {
+    for (int i = 0; i < nb; ++i) {
+      sv->style0[i] = style0[i]; sv->style1[i] = style1[i]; sv->style_rgb[i] = style_rgb[i];
+      sv->dco0[i] = dco0[i]; sv->dco1[i] = dco1[i];
+      const size_t n = (size_t)B * (4 << i) * (4 << i) * P.channels[i];
+      sv->u0[i] = i ? ws.take(n) : nullptr;
+      sv->u1[i] = ws.take(n);
+    }
   }
 
   // ---- the blocks ----
@@ -817,6 +1090,7 @@ static int run(const nfi_synth_params& P, Bump& ws, cudaStream_t st, bool dry, c
         memset(&e, 0, sizeof(e));
         e.dcoef = dco0[i]; e.noise = P.conv0[i].noise; e.bias = P.conv0[i].bias; e.gain = sqrt2;
         e.style_a = style1[i]; e.a_hi = y.hi; e.a_lo = y.lo;
+        e.u_out = sv ? sv->u0[i] : nullptr;
         const size_t total = (size_t)B * (res / 2) * (res / 2) * (cout / 4);
         unsigned grid = blocks(total, 256);
         if (grid > (unsigned)sm_count() * 16u) grid = (unsigned)sm_count() * 16u;
@@ -839,6 +1113,7 @@ static int run(const nfi_synth_params& P, Bump& ws, cudaStream_t st, bool dry, c
       a.act.gain = sqrt2;
       a.act.style_a = style_rgb[i]; a.act.a_hi = xr.hi; a.act.a_lo = xr.lo;
       if (!last) { a.act.style_b = style0[i + 1]; a.act.b_hi = xn.hi; a.act.b_lo = xn.lo; }
+      a.act.u_out = sv ? sv->u1[i] : nullptr;
       const int rc = launch_conv(a, x, w1[i], 9, st, err, err_len);
       if (rc) return rc;
     }
@@ -886,6 +1161,256 @@ int forward(const nfi_synth_params& P, cudaStream_t st, char* err, size_t err_le
       (reinterpret_cast<uintptr_t>(P.workspace) + 1023) & ~(uintptr_t)1023);
   Bump b{base, 0, P.workspace_bytes};
   return run(P, b, st, false, err, err_len);
+}
+
+// ---- backward ----
+// Walks the blocks from the last to the first.  Scratch reused across blocks (stream order keeps the
+// reuse safe): bufA holds g_rgb, then dx~ of conv1, then the raw-gradient phases of conv0; bufB the
+// dacc of conv1 (pair), then of conv0 (fp32); bufC dx~ of conv0 until the previous block's conv1
+// has consumed it.
+static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, const Saved& sv, Bump& ws,
+                        cudaStream_t st, bool dry, char* err, size_t err_len) {
+  const int B = P.batch, nb = P.num_blocks, D = P.w_dim, R = P.img_resolution, NI = P.img_channels;
+  const float sqrt2 = 1.4142135623730951f;
+  auto blocks = [](size_t n, int per) { return (unsigned)((n + per - 1) / per); };
+  auto flat_grid = [&](size_t n) {
+    unsigned g = blocks(n, 256);
+    return g > (unsigned)sm_count() * 16u ? (unsigned)sm_count() * 16u : g;
+  };
+  int cmax = 0;
+  for (int i = 0; i < nb; ++i) cmax = P.channels[i] > cmax ? P.channels[i] : cmax;
+  const size_t full = (size_t)B * R * R * cmax;
+  const size_t phases = (size_t)4 * B * (R / 2 + 1) * (R / 2 + 1) * cmax;
+  float* bufA = ws.take(full > phases ? full : phases);
+  float* bufB = ws.take(full);
+  float* bufC = ws.take((size_t)B * (R / 2) * (R / 2) * cmax);
+  float* dimg[2] = {ws.take((size_t)B * R * R * NI), ws.take((size_t)B * R * R * NI)};
+  Pair dimg_p = ws.pair((size_t)B * R * R * NI);
+  // per-(b, channel) sums, zeroed once
+  float *ds0[NFI_SYNTH_MAX_BLOCKS], *ds1[NFI_SYNTH_MAX_BLOCKS], *dsr[NFI_SYNTH_MAX_BLOCKS];
+  float *dd0[NFI_SYNTH_MAX_BLOCKS], *dd1[NFI_SYNTH_MAX_BLOCKS];
+  size_t small = 0;
+  for (int i = 0; i < nb; ++i) small += (size_t)B * (4 * P.channels[i] + (i ? P.channels[i - 1] : 0));
+  float* sums = ws.take(small);
+  {
+    float* q = sums;
+    for (int i = 0; i < nb; ++i) {
+      const int c = P.channels[i], ci = i ? P.channels[i - 1] : 0;
+      ds0[i] = q; q += (size_t)B * ci;
+      ds1[i] = q; q += (size_t)B * c;
+      dsr[i] = q; q += (size_t)B * c;
+      dd0[i] = q; q += (size_t)B * c;
+      dd1[i] = q; q += (size_t)B * c;
+    }
+  }
+  Pair wt0[NFI_SYNTH_MAX_BLOCKS], wt1[NFI_SYNTH_MAX_BLOCKS], wtr[NFI_SYNTH_MAX_BLOCKS];
+  for (int i = 0; i < nb; ++i) {
+    const int c = P.channels[i], ci = i ? P.channels[i - 1] : 0;
+    if (i) wt0[i] = ws.pair((size_t)9 * c * ci);
+    wt1[i] = ws.pair((size_t)9 * c * c);
+    wtr[i] = ws.pair((size_t)NI * c);
+  }
+  if (dry) return 0;
+
+  NFI_SCUDA(cudaMemsetAsync(sums, 0, small * sizeof(float), st));
+  for (int i = 0; i < nb; ++i) {
+    const int c = P.channels[i], ci = i ? P.channels[i - 1] : 0;
+    if (i)
+      prep_weights_t_kernel<<<blocks((size_t)c * ci, 256), 256, 0, st>>>(P.conv0[i].weight, c, ci, 9,
+                                                                         wt0[i].hi, wt0[i].lo);
+    prep_weights_t_kernel<<<blocks((size_t)c * c, 256), 256, 0, st>>>(P.conv1[i].weight, c, c, 9,
+                                                                       wt1[i].hi, wt1[i].lo);
+    prep_weights_t_kernel<<<blocks((size_t)NI * c, 256), 256, 0, st>>>(P.torgb[i].weight, NI, c, 1,
+                                                                       wtr[i].hi, wtr[i].lo);
+  }
+  planes_grad_kernel<<<flat_grid((size_t)B * R * R * NI), 256, 0, st>>>(G.g_planes, B, R, dimg[0],
+                                                                        dimg_p.hi, dimg_p.lo);
+  NFI_SCUDA(cudaGetLastError());
+
+  auto act_backward = [&](ActBackward& e, int HW, int C) -> int {
+    if (C % 4 != 0 || C / 4 > 256) {
+      snprintf(err, err_len, "synthesis backward: %d channels unsupported", C);
+      return 1;
+    }
+    const int chunk = 1024;
+    dim3 grid((unsigned)((HW + chunk - 1) / chunk), (unsigned)B);
+    act_backward_kernel<<<grid, 256, 0, st>>>(e, HW, C, chunk);
+    NFI_SCUDA(cudaGetLastError());
+    return 0;
+  };
+  auto to_ws = [&](const float* ds, const nfi_synth_layer& L, int cin, int row, float gain) {
+    styles_backward_kernel<<<blocks((size_t)B * D, 256), 256, 0, st>>>(
+        ds, L.affine_w, cin, D, B, gain / sqrtf((float)D), G.g_ws + (size_t)row * D, P.num_ws * D);
+  };
+  auto stride1_taps = [](ConvArgs& a, int H, int W) {  // the adjoint of conv3x3_phases: taps flipped
+    conv3x3_phases(a, H, W);
+    for (int t = 0; t < 9; ++t) {
+      a.tap_dy[t] = -a.tap_dy[t];
+      a.tap_dx[t] = -a.tap_dx[t];
+    }
+  };
+
+  int cur = 0;  // dimg[cur] is the gradient of block i's running image
+  for (int i = nb - 1; i >= 0; --i) {
+    const int res = 4 << i, c = P.channels[i], ci = i ? P.channels[i - 1] : 0, HW = res * res;
+    const bool last = (i == nb - 1);
+    // ToRGB: g = dimg Wrgb^T  [B,res,res,c] -> bufA
+    {
+      ConvArgs a;
+      memset(&a, 0, sizeof(a));
+      a.B = B; a.C = NI; a.N = c; a.H = res; a.W = res;
+      a.n_phases = 1; a.ph_taps[0] = 1; a.ph_DH[0] = res; a.ph_DW[0] = res;
+      a.mode = kModeRaw;
+      a.out_raw = bufA; a.out_H = res; a.out_W = res; a.out_stride = 1;
+      const int rc = launch_conv(a, dimg_p, wtr[i], 1, st, err, err_len);
+      if (rc) return rc;
+    }
+    if (i) {  // the running image's gradient one block down (the GEMM above has read dimg_p)
+      const int h = res / 2;
+      upsample_adjoint_kernel<<<flat_grid((size_t)B * h * h * NI), 256, 0, st>>>(
+          dimg[cur], B, h, h, NI, dimg[cur ^ 1], dimg_p.hi, dimg_p.lo);
+      NFI_SCUDA(cudaGetLastError());
+      cur ^= 1;
+    }
+    // conv1: consumers ToRGB (style_rgb) and, below the last block, conv0 of block i+1 (bufC)
+    {
+      ActBackward e;
+      memset(&e, 0, sizeof(e));
+      e.u = sv.u1[i]; e.noise = P.conv1[i].noise; e.bias = P.conv1[i].bias; e.dcoef = sv.dco1[i];
+      e.gain = sqrt2;
+      e.dx_a = bufA; e.s_a = sv.style_rgb[i]; e.ds_a = dsr[i];
+      if (!last) { e.dx_b = bufC; e.s_b = sv.style0[i + 1]; e.ds_b = ds0[i + 1]; }
+      e.dd = dd1[i];
+      Pair pb = {reinterpret_cast<__nv_bfloat16*>(bufB),
+                 reinterpret_cast<__nv_bfloat16*>(bufB) + (size_t)B * HW * c};
+      e.dacc_hi = pb.hi; e.dacc_lo = pb.lo;
+      if (int rc = act_backward(e, HW, c)) return rc;
+      to_ws(dsr[i], P.torgb[i], c, sv.row_rgb[i], 1.f / sqrtf((float)c));
+      if (!last) {
+        const int cn = P.channels[i + 1];
+        dcoef_backward_kernel<<<blocks((size_t)B * c * 32, 256), 256, 0, st>>>(
+            sv.wsq0[i + 1], sv.style0[i + 1], dd0[i + 1], sv.dco0[i + 1], cn, c, B, ds0[i + 1]);
+        to_ws(ds0[i + 1], P.conv0[i + 1], c, sv.row0[i + 1], 1.f);
+      }
+      // dx~ of conv1 = conv^T(dacc, W1) -> bufA
+      ConvArgs a;
+      memset(&a, 0, sizeof(a));
+      a.B = B; a.C = c; a.N = c; a.H = res; a.W = res;
+      stride1_taps(a, res, res);
+      a.mode = kModeRaw;
+      a.out_raw = bufA; a.out_H = res; a.out_W = res; a.out_stride = 1;
+      const int rc = launch_conv(a, pb, wt1[i], 9, st, err, err_len);
+      if (rc) return rc;
+    }
+    if (i == 0) {
+      const_ds_kernel<<<blocks((size_t)B * c, 256), 256, 0, st>>>(bufA, P.const_input, B, c, ds1[0]);
+      dcoef_backward_kernel<<<blocks((size_t)B * c * 32, 256), 256, 0, st>>>(
+          sv.wsq1[0], sv.style1[0], dd1[0], sv.dco1[0], c, c, B, ds1[0]);
+      to_ws(ds1[0], P.conv1[0], c, sv.row1[0], 1.f);
+      NFI_SCUDA(cudaGetLastError());
+      break;
+    }
+    // conv0 (up): its one consumer is conv1 -> dacc fp32 in bufB, ds1 and dd0
+    {
+      ActBackward e;
+      memset(&e, 0, sizeof(e));
+      e.u = sv.u0[i]; e.noise = P.conv0[i].noise; e.bias = P.conv0[i].bias; e.dcoef = sv.dco0[i];
+      e.gain = sqrt2;
+      e.dx_a = bufA; e.s_a = sv.style1[i]; e.ds_a = ds1[i];
+      e.dd = dd0[i];
+      e.dacc = bufB;
+      if (int rc = act_backward(e, HW, c)) return rc;
+      dcoef_backward_kernel<<<blocks((size_t)B * c * 32, 256), 256, 0, st>>>(
+          sv.wsq1[i], sv.style1[i], dd1[i], sv.dco1[i], c, c, B, ds1[i]);
+      to_ws(ds1[i], P.conv1[i], c, sv.row1[i], 1.f);
+    }
+    // FIR adjoint -> the four parity phases of the raw gradient (pair in bufA), then the
+    // stride-2 correlation with W0 as 9 stride-1 taps over them -> dx~ of conv0 in bufC
+    {
+      const int h = res / 2;
+      Pair ph = {reinterpret_cast<__nv_bfloat16*>(bufA),
+                 reinterpret_cast<__nv_bfloat16*>(bufA) + (size_t)4 * B * (h + 1) * (h + 1) * c};
+      fir_adjoint_kernel<<<flat_grid((size_t)4 * B * (h + 1) * (h + 1) * (c / 4)), 256, 0, st>>>(
+          bufB, B, res, res, c, ph.hi, ph.lo);
+      NFI_SCUDA(cudaGetLastError());
+      ConvArgs a;
+      memset(&a, 0, sizeof(a));
+      a.B = B; a.C = c; a.N = ci; a.H = h + 1; a.W = h + 1;
+      a.n_phases = 1; a.ph_taps[0] = 9; a.ph_DH[0] = h; a.ph_DW[0] = h;
+      for (int ky = 0; ky < 3; ++ky)
+        for (int kx = 0; kx < 3; ++kx) {
+          const int t = ky * 3 + kx;
+          a.tap_dy[t] = ky / 2;
+          a.tap_dx[t] = kx / 2;
+          a.tap_w[t] = t;
+          a.tap_img[t] = ((ky & 1) * 2 + (kx & 1)) * B;
+        }
+      a.mode = kModeRaw;
+      a.out_raw = bufC; a.out_H = h; a.out_W = h; a.out_stride = 1;
+      const int rc = launch_conv(a, ph, wt0[i], 9, st, err, err_len, 4 * B);
+      if (rc) return rc;
+    }
+  }
+  NFI_SCUDA(cudaGetLastError());
+  return 0;
+}
+
+static int saved_layout(const nfi_synth_params& P, Bump& b, Saved& sv, char* err, size_t err_len) {
+  return run(P, b, nullptr, true, err, err_len, &sv);
+}
+
+size_t saved_workspace_bytes(const nfi_synth_params& P) {
+  char err[256];
+  if (check_params(P, err, sizeof(err))) return 0;
+  Bump b{nullptr, 0, 0};
+  Saved sv;
+  memset(&sv, 0, sizeof(sv));
+  saved_layout(P, b, sv, err, sizeof(err));
+  nfi_synth_grads g = {nullptr, nullptr};
+  run_backward(P, g, sv, b, nullptr, true, err, sizeof(err));
+  return b.off + 1024;
+}
+
+static int check_saved(const nfi_synth_params& P, char* err, size_t err_len) {
+  const int rc = check_params(P, err, err_len);
+  if (rc) return rc;
+  if (P.ws == nullptr || P.const_input == nullptr || P.planes == nullptr || P.workspace == nullptr) {
+    snprintf(err, err_len, "synthesis: ws, const_input, planes and workspace must be set");
+    return 1;
+  }
+  const size_t need = saved_workspace_bytes(P);
+  if (P.workspace_bytes < need) {
+    snprintf(err, err_len, "synthesis: saved workspace too small (%zu < %zu bytes)", P.workspace_bytes,
+             need);
+    return 1;
+  }
+  return 0;
+}
+
+int forward_saved(const nfi_synth_params& P, cudaStream_t st, char* err, size_t err_len) {
+  if (const int rc = check_saved(P, err, err_len)) return rc;
+  unsigned char* base = reinterpret_cast<unsigned char*>(
+      (reinterpret_cast<uintptr_t>(P.workspace) + 1023) & ~(uintptr_t)1023);
+  Bump b{base, 0, P.workspace_bytes};
+  Saved sv;
+  memset(&sv, 0, sizeof(sv));
+  return run(P, b, st, false, err, err_len, &sv);
+}
+
+int backward(const nfi_synth_params& P, const nfi_synth_grads& G, cudaStream_t st, char* err,
+             size_t err_len) {
+  if (const int rc = check_saved(P, err, err_len)) return rc;
+  if (G.g_planes == nullptr || G.g_ws == nullptr) {
+    snprintf(err, err_len, "synthesis backward: g_planes and g_ws must be set");
+    return 1;
+  }
+  unsigned char* base = reinterpret_cast<unsigned char*>(
+      (reinterpret_cast<uintptr_t>(P.workspace) + 1023) & ~(uintptr_t)1023);
+  Bump b{base, 0, P.workspace_bytes};
+  Saved sv;
+  memset(&sv, 0, sizeof(sv));
+  if (const int rc = saved_layout(P, b, sv, err, err_len)) return rc;
+  return run_backward(P, G, sv, b, st, false, err, err_len);
 }
 
 }  // namespace synth

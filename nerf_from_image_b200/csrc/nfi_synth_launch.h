@@ -10,5 +10,9 @@ namespace nfi {
 namespace synth {
 size_t workspace_bytes(const nfi_synth_params& p);
 int forward(const nfi_synth_params& p, cudaStream_t st, char* err, size_t err_len);
+size_t saved_workspace_bytes(const nfi_synth_params& p);
+int forward_saved(const nfi_synth_params& p, cudaStream_t st, char* err, size_t err_len);
+int backward(const nfi_synth_params& p, const nfi_synth_grads& g, cudaStream_t st, char* err,
+             size_t err_len);
 }  // namespace synth
 }  // namespace nfi

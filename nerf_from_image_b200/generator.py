@@ -15,6 +15,12 @@ Envelope: requests within {'sampler', 'attention_values'} under ``torch.no_grad(
 renders, encoder-training targets, visualisation).  The regulariser heads and every call that
 differentiates through the synthesis network are the reference module's; ``render`` picks this
 front-end only when a call is inside the envelope (``render.enable_fused_synthesis``).
+
+``FusedInversionFront(G)`` is the same front-end for grad-enabled calls with a frozen synthesis
+network -- the inversion loop, which differentiates the render to the latents (and the pose):
+the planes come from ``FusedSynthesis.forward_differentiable``, whose backward carries dL/dplanes
+to ws on the sm_90a kernels.  Mapping network, texture mapper and the ``expand`` of [B,1,512]
+latents stay torch autograd.  ``render`` picks it with ``render.enable_fused_inversion``.
 """
 import torch
 
@@ -97,16 +103,19 @@ class FusedGeneratorFront:
                         for k in model_inputs))
 
     def __call__(self, viewdir, c, request_model_outputs=['sampler'], model_inputs={}):
-        g = self.g
         if not self.supports(request_model_outputs, model_inputs):
             raise _lib.NfiError('FusedGeneratorFront: outside its envelope (no_grad, outputs '
                                 'within %r)' % (SUPPORTED_OUTPUTS,))
+        return self._outputs(viewdir, c, request_model_outputs, model_inputs, self.synthesis)
+
+    def _outputs(self, viewdir, c, request_model_outputs, model_inputs, synthesis):
+        g = self.g
         ws, batch = resolve_ws(g, c)
         attention_values, w_synthesis = resolve_palette(g, ws, request_model_outputs, model_inputs)
         view = view_conditioning(g, viewdir) if (g.use_viewdir and viewdir is not None) else {}
         # ---- planes (generator.py:471-477), channel-last
         noise_mode = 'const' if model_inputs.get('freeze_noise') else 'random'
-        planes_cl = self.synthesis(w_synthesis, noise_mode=noise_mode)
+        planes_cl = synthesis(w_synthesis, noise_mode=noise_mode)
         assert planes_cl.shape[0] == batch
         w1, b1, w2, b2 = decoder_weights(g)
         out = {}
@@ -118,6 +127,25 @@ class FusedGeneratorFront:
             w1=w1, b1=b1, w2=w2, b2=b2,
             beta=getattr(g, 'beta', None), alpha=getattr(g, 'alpha', None), **view)
         return out
+
+
+class FusedInversionFront(FusedGeneratorFront):
+    """Grad-enabled calls, synthesis network frozen, requests within SUPPORTED_OUTPUTS."""
+
+    def supports(self, request_model_outputs, model_inputs):
+        return (torch.is_grad_enabled()
+                and not any(p.requires_grad for p in self.g.synthesis_network.parameters())
+                and all(o in SUPPORTED_OUTPUTS for o in request_model_outputs)
+                and all(k in ('freeze_noise', 'attention_values', 'attention_values_bias')
+                        for k in model_inputs))
+
+    def __call__(self, viewdir, c, request_model_outputs=['sampler'], model_inputs={}):
+        if not self.supports(request_model_outputs, model_inputs):
+            raise _lib.NfiError('FusedInversionFront: outside its envelope (grad enabled, '
+                                'synthesis network frozen, outputs within %r)'
+                                % (SUPPORTED_OUTPUTS,))
+        return self._outputs(viewdir, c, request_model_outputs, model_inputs,
+                             self.synthesis.forward_differentiable)
 
 
 class HeadsGeneratorFront:

@@ -56,6 +56,7 @@ def configure(new_args, new_dataset_config, samples_per_ray=None):
 
 
 _FRONTS = {}
+_INV_FRONTS = {}
 _HEAD_FRONTS = {}
 
 
@@ -81,6 +82,20 @@ def enable_fused_synthesis(target_model, enabled=True):
         _FRONTS[id(target_model)] = FusedGeneratorFront(target_model)
     else:
         _FRONTS.pop(id(target_model), None)
+
+
+def enable_fused_inversion(target_model, enabled=True):
+    """Makes ``render`` produce ``target_model``'s tri-planes with the sm_90a synthesis kernels
+    for grad-enabled calls too, when the synthesis network is frozen (the inversion loop:
+    gradients to the latents and the pose, generator.FusedInversionFront); the planes' gradient
+    goes back to ws through the fused synthesis backward.  A call with a trainable synthesis
+    parameter, or with regulariser outputs, keeps running the reference module.  Calls under
+    ``torch.no_grad()`` are ``enable_fused_synthesis``'s."""
+    from .generator import FusedInversionFront
+    if enabled:
+        _INV_FRONTS[id(target_model)] = FusedInversionFront(target_model)
+    else:
+        _INV_FRONTS.pop(id(target_model), None)
 
 
 def _closure_vars(fn):
@@ -208,10 +223,14 @@ def render(target_model,
 
     requests = ['sampler'] + list(extra_model_outputs)
     front = _FRONTS.get(id(target_model))
+    ifront = _INV_FRONTS.get(id(target_model))
     hfront = _HEAD_FRONTS.get(id(target_model))
     if front is not None and front.supports(requests, extra_model_inputs):
         # plane producer on sm_90a too (generator.FusedGeneratorFront; no_grad calls only)
         model_outputs = front(viewdirs, model_input, requests, extra_model_inputs)
+    elif ifront is not None and ifront.supports(requests, extra_model_inputs):
+        # ... and its backward to the latents (generator.FusedInversionFront; frozen synthesis)
+        model_outputs = ifront(viewdirs, model_input, requests, extra_model_inputs)
     elif hfront is not None and hfront.supports(requests, extra_model_inputs):
         # regulariser heads on the fused point evaluator (generator.HeadsGeneratorFront)
         model_outputs = hfront(viewdirs, model_input, requests, extra_model_inputs)

@@ -16,9 +16,17 @@ Noise (stylegan.py:332-343): the per-layer ``torch.randn([B,1,res,res]) * noise_
 are made HERE, in the module's layer order and from the same generator, so a seeded run consumes
 the RNG like the reference; ``noise_mode='const'`` uses the registered ``noise_const`` buffers.
 
-Forward only (evaluation renders, encoder-training targets, ``no_grad`` generator passes); a call
-that needs gradients raises -- the inversion / GAN loops keep differentiating through the
-reference module.  There is no CPU path and no fallback.
+``__call__`` is forward only (evaluation renders, encoder-training targets, ``no_grad``
+generator passes); a call that needs gradients raises.  The inversion setting -- every network
+parameter frozen, gradients to the latents -- has its own entry:
+
+    planes_cl = FusedSynthesis(net).forward_differentiable(ws, noise_mode='random')
+
+which runs ``nfi_synthesis_forward_saved`` (the same planes, bit for bit, plus each layer's
+pre-activation kept in the workspace) and, in backward, ``nfi_synthesis_backward`` to ws.
+Gradients to the weights, biases, affines, noise or ``b4.const`` are not offered: a network with
+a trainable parameter raises (the GAN loop keeps the reference module).  There is no CPU path
+and no fallback.
 """
 import ctypes
 import math
@@ -57,7 +65,7 @@ class FusedSynthesis:
         ns = lambda **kw: type('ns', (), kw)()
         net = ns(img_resolution=meta['img_resolution'], img_channels=meta['img_channels'],
                  w_dim=meta['w_dim'], block_resolutions=list(meta['resolutions']),
-                 parameters=lambda: [])
+                 parameters=staticmethod(lambda: []))
         for r in meta['resolutions']:
             pre = 'b%d' % r
             blk = ns()
@@ -106,6 +114,26 @@ class FusedSynthesis:
         if not ws.is_cuda:
             raise _lib.NfiError('the fused synthesis network only runs on CUDA tensors '
                                 '(there is no CPU path)')
+        return self._run(ws, noise_mode, saved=False)[0]
+
+    def forward_differentiable(self, ws, noise_mode='random'):
+        """Channel-last planes [B,3,R,R,32] differentiable with respect to ``ws`` (every network
+        parameter frozen).  The noise draws are the same draws, in the same order, as
+        ``__call__``'s; the saved workspace lives until the backward has run."""
+        assert noise_mode in ['random', 'const']
+        if any(p.requires_grad for p in self.net.parameters()):
+            raise _lib.NfiError(
+                'FusedSynthesis.forward_differentiable differentiates to the latents only: every '
+                'network parameter must be frozen (requires_grad_(False)); weight, bias and affine '
+                'gradients are the reference module\'s')
+        if not ws.is_cuda:
+            raise _lib.NfiError('the fused synthesis network only runs on CUDA tensors '
+                                '(there is no CPU path)')
+        return _SynthesisFunction.apply(ws, self, noise_mode)
+
+    def _run(self, ws, noise_mode, saved):
+        """-> (planes, (P, keep, work)) -- P, keep and work stay valid for a backward."""
+        net = self.net
         lib = _lib.load()
         dev = ws.device
         B = ws.shape[0]
@@ -143,17 +171,51 @@ class FusedSynthesis:
             R = net.img_resolution
             planes = torch.empty(B, 3, R, R, 32, device=dev, dtype=torch.float32)
             P.planes = _ptr(planes)
-            need = lib.nfi_synthesis_workspace_bytes(ctypes.byref(P))
+            sizer = lib.nfi_synthesis_saved_workspace_bytes if saved else \
+                lib.nfi_synthesis_workspace_bytes
+            need = sizer(ctypes.byref(P))
             if need == 0:
                 raise _lib.NfiError('unsupported synthesis configuration (channels must be '
                                     'multiples of 32, resolution a power of two >= 8)')
             work = torch.empty(need, dtype=torch.uint8, device=dev)
             P.workspace, P.workspace_bytes = _ptr(work), need
             stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            _lib.check(lib.nfi_synthesis_forward(ctypes.byref(P), stream))
+            fwd = lib.nfi_synthesis_forward_saved if saved else lib.nfi_synthesis_forward
+            _lib.check(fwd(ctypes.byref(P), stream))
             # the launches are stream-ordered; `keep` / `work` may be released by the caching
             # allocator afterwards only for reuse on this same stream
+        return planes, (P, keep, work)
+
+
+class _SynthesisFunction(torch.autograd.Function):
+    """ws -> planes (channel-last) with nfi_synthesis_backward as the backward."""
+
+    @staticmethod
+    def forward(ctx, ws, fs, noise_mode):
+        planes, state = fs._run(ws, noise_mode, saved=True)
+        ctx.state, ctx.ws_dtype = state, ws.dtype
         return planes
+
+    @staticmethod
+    def backward(ctx, g_planes):
+        if ctx.state is None:
+            raise _lib.NfiError('the fused synthesis backward ran twice on one forward '
+                                '(retain_graph is not supported: the workspace is released)')
+        if torch.is_grad_enabled():
+            raise _lib.NfiError('the fused synthesis backward is not differentiable (create_graph, '
+                                'e.g. the path-length regulariser): use the reference module')
+        P, keep, work = ctx.state
+        ctx.state = None          # the workspace and fp32 copies go once this returns
+        dev = g_planes.device
+        g_planes = g_planes.to(torch.float32).contiguous()
+        ws32 = keep[0]
+        g_ws = torch.zeros_like(ws32)
+        G = _lib.SynthGrads(g_planes=g_planes.data_ptr(), g_ws=g_ws.data_ptr())
+        with torch.cuda.device(dev):
+            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            _lib.check(_lib.load().nfi_synthesis_backward(ctypes.byref(P), ctypes.byref(G), stream))
+        del P, keep, work
+        return g_ws.to(ctx.ws_dtype), None, None
 
 
 def planes_channel_first(planes_cl):
