@@ -500,10 +500,16 @@ render_wgrad_pipe(const nfi_render_params p, const nfi_render_grads g,
         if constexpr (PLANES) mbar_arrive(d4_full);
       }
     };
+    // PLANES: the one producer set gathers a tile's first step only after it has scattered the
+    // previous tile's last one, which needs that step's act_bwd.  The look-ahead therefore stops at
+    // a tile boundary (else a CTA with a second tile waits on itself) and resumes after act_bwd.
     if (total_steps > 0) act_fwd(0);
     for (uint32_t m = 0; m < total_steps; ++m) {
-      if (m + 1 < total_steps) act_fwd(m + 1);
+      const bool next = m + 1 < total_steps;
+      const bool ahead = next && !(PLANES && (m + 1) % (uint32_t)n_total == 0);
+      if (ahead) act_fwd(m + 1);
       act_bwd(m);
+      if (next && !ahead) act_fwd(m + 1);
     }
   } else {
     // ================================ SHADING (forward and reverse) ================================

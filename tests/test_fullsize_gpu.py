@@ -2,8 +2,9 @@
 uses -- the gaps VERDICT round 1 listed (weak #1, #2; ADVICE medium #1, low #1).
 
 * backward of the tensor-core kernel AND of the fp32 SIMT kernel at bench config-2 geometry
-  (one image, 128x128 rays, 64 + 64 samples, 256^2 planes: 64 tiles on a persistent grid, i.e.
-  the multi-wave regime the small tests never reach) and the config-3 orthographic variant,
+  (one image, 128x128 rays, 64 + 64 samples, 256^2 planes: 128 tiles of 16x8 rays, one wave on
+  the 132 SMs of an H100 SXM, so no CTA owns a second tile; tests/test_multiwave_gpu.py covers
+  the multi-wave regime) and the config-3 orthographic variant,
   against the oracle's autograd run in eager fp32 on the same GPU (TF32 off, run.py:59-60);
 * ``cam_grad=False`` (the reference's ``force_no_cam_grad``: every D-step, evaluation and
   encoder-training render, run.py:1121-1124,1250,1639) on the CUDA path;
