@@ -26,9 +26,15 @@
  * planes' gradient into the gradient of ws.  Its data-gradient GEMMs run on the same TMA + wgmma
  * kernel with the weights re-laid-out [tap][Cin][Cout]; the up layer's adjoint is the FIR's
  * (a correlation with the same symmetric taps) split into the four parity phases of the
- * (2R+1)^2 raw gradient, then nine stride-1 taps over them.  Gradients to the weights, biases,
- * affines, noise and b4.const are not computed (the GAN generator step keeps the reference
- * module, which these entry points never fall back to).
+ * (2R+1)^2 raw gradient, then nine stride-1 taps over them.
+ * Backward to the parameters (the GAN generator step): nfi_synthesis_backward_params runs the same
+ * launches and adds the weight-gradient GEMMs (wgrad_tc_kernel: dL/dconv-output against the
+ * layer's input, both position-major bf16 pairs, contracted over positions in bounded tensor-core
+ * chains, split over CTAs and reduced in fp32 in a fixed order) and the small reductions for
+ * biases, noise, affines and b4.const.  The weight gradients are the same from run to run; the
+ * bias sums (one fp32 atomic per block of 1024 positions and image) and the noise sums (shared-
+ * memory fp32 atomics over channel groups) are not, in their last bits; g_ws is as reproducible
+ * as nfi_synthesis_backward's (the same launches).
  */
 #ifndef NFI_SYNTH_H_
 #define NFI_SYNTH_H_
@@ -91,6 +97,34 @@ NFI_API int nfi_synthesis_forward_saved(const nfi_synth_params *params, void *st
 /* The same params (same ws, weights, noise) and the workspace as the saved forward left it. */
 NFI_API int nfi_synthesis_backward(const nfi_synth_params *params, const nfi_synth_grads *grads,
                                    void *stream);
+
+/* Backward to the parameters (the GAN generator step).  Every pointer is ACCUMULATED (+=) like
+   g_ws, has the shape of the nfi_synth_layer field it differentiates, and may be NULL (that
+   gradient is not formed). */
+typedef struct nfi_synth_layer_grads {
+  float *g_weight;   /* [cout, cin, k, k] */
+  float *g_affine_w; /* [cin, w_dim] */
+  float *g_affine_b; /* [cin] */
+  float *g_bias;     /* [cout] */
+  float *g_noise;    /* [B, res, res]: gradient of the noise tensor the layer was handed (the value
+                        after the multiplication by noise_strength); ignored where noise is NULL */
+} nfi_synth_layer_grads;
+
+typedef struct nfi_synth_param_grads {
+  nfi_synth_layer_grads conv0[NFI_SYNTH_MAX_BLOCKS]; /* conv0[0] unused */
+  nfi_synth_layer_grads conv1[NFI_SYNTH_MAX_BLOCKS];
+  nfi_synth_layer_grads torgb[NFI_SYNTH_MAX_BLOCKS]; /* g_noise unused */
+  float *g_const;                                    /* [channels[0], 4, 4] b4.const */
+} nfi_synth_param_grads;
+
+/* Workspace of a saved forward whose backward also forms the parameter gradients
+   (>= nfi_synthesis_saved_workspace_bytes; nfi_synthesis_forward_saved accepts it). */
+NFI_API size_t nfi_synthesis_param_workspace_bytes(const nfi_synth_params *params);
+/* nfi_synthesis_backward (the same g_ws, bit for bit) plus the parameter gradients; the workspace
+   is a saved forward's of >= nfi_synthesis_param_workspace_bytes. */
+NFI_API int nfi_synthesis_backward_params(const nfi_synth_params *params,
+                                          const nfi_synth_grads *grads,
+                                          const nfi_synth_param_grads *param_grads, void *stream);
 
 #ifdef __cplusplus
 }

@@ -108,6 +108,20 @@ class SynthGrads(ctypes.Structure):
     _fields_ = [('g_planes', ctypes.c_void_p), ('g_ws', ctypes.c_void_p)]
 
 
+class SynthLayerGrads(ctypes.Structure):
+    """struct nfi_synth_layer_grads."""
+    _fields_ = [(n, ctypes.c_void_p) for n in ('g_weight', 'g_affine_w', 'g_affine_b', 'g_bias',
+                                               'g_noise')]
+
+
+class SynthParamGrads(ctypes.Structure):
+    """struct nfi_synth_param_grads."""
+    _fields_ = [
+        ('conv0', SynthLayerGrads * SYNTH_MAX_BLOCKS), ('conv1', SynthLayerGrads * SYNTH_MAX_BLOCKS),
+        ('torgb', SynthLayerGrads * SYNTH_MAX_BLOCKS), ('g_const', ctypes.c_void_p),
+    ]
+
+
 class SdfPointsParams(ctypes.Structure):
     """struct nfi_sdf_points_params (include/nfi_heads.h)."""
     _fields_ = [('batch', ctypes.c_int32), ('plane_res', ctypes.c_int32),
@@ -158,6 +172,11 @@ EXPORTS = {
     'nfi_synthesis_forward_saved': (ctypes.c_int, [ctypes.POINTER(SynthParams), ctypes.c_void_p]),
     'nfi_synthesis_backward': (ctypes.c_int, [ctypes.POINTER(SynthParams),
                                               ctypes.POINTER(SynthGrads), ctypes.c_void_p]),
+    'nfi_synthesis_param_workspace_bytes': (ctypes.c_size_t, [ctypes.POINTER(SynthParams)]),
+    'nfi_synthesis_backward_params': (ctypes.c_int, [ctypes.POINTER(SynthParams),
+                                                     ctypes.POINTER(SynthGrads),
+                                                     ctypes.POINTER(SynthParamGrads),
+                                                     ctypes.c_void_p]),
     'nfi_pose_to_matrix': (ctypes.c_int, [
         ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32,
         ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),

@@ -675,6 +675,21 @@ int nfi_synthesis_backward(const nfi_synth_params* params, const nfi_synth_grads
   return nfi::synth::backward(*params, *grads, (cudaStream_t)stream, g_err, sizeof(g_err));
 }
 
+size_t nfi_synthesis_param_workspace_bytes(const nfi_synth_params* params) {
+  if (params == nullptr) return 0;
+  return nfi::synth::param_workspace_bytes(*params);
+}
+
+int nfi_synthesis_backward_params(const nfi_synth_params* params, const nfi_synth_grads* grads,
+                                  const nfi_synth_param_grads* param_grads, void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  if (grads == nullptr) return fail("grads is NULL");
+  if (param_grads == nullptr) return fail("param_grads is NULL");
+  if (params->batch <= 0) return fail("empty batch");
+  return nfi::synth::backward_params(*params, *grads, *param_grads, (cudaStream_t)stream, g_err,
+                                     sizeof(g_err));
+}
+
 int nfi_render_forward_host(const nfi_render_params* hp, int32_t device) {
   // Host buffers in, host buffers out.  The batch is cut into chunks of images
   // (images are independent: SURVEY.md section 8e) and pipelined over two

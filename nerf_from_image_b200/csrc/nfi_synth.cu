@@ -592,16 +592,31 @@ struct ActBackward {
   __nv_bfloat16* dacc_hi;  // dacc = g d as a pair (input of the next data-gradient GEMM) ...
   __nv_bfloat16* dacc_lo;
   float* dacc;             // ... or fp32 (input of the FIR adjoint)
+  // parameter backward only (act_backward_kernel<true>): += sum_{b,pos} g and += sum_c g
+  float* g_bias;           // [C]
+  float* g_noise;          // [B,HW] (with noise)
 };
 
 __device__ __forceinline__ float lrelu_grad(float u) { return u > 0.f ? 1.f : 0.2f; }
 
+constexpr int kActChunk = 1024;  // positions per block of act_backward_kernel
+
 // One pass over a layer's output: dv = dx~_a s_a + dx~_b s_b, then dacc = dv lrelu'(u) gain d, and
 // the per-(b, channel) sums ds_a, ds_b, dd.  Block (chunk, b): 4 channels per thread, 256 / (C/4)
 // positions in parallel; the sums are reduced in shared memory, then one atomic per block.
+// kParams adds the bias sum of g (a fourth per-block reduction) and the noise gradient sum_c g per
+// position (shared atomics over the block's chunk, then one plain += per position: each position
+// belongs to one block); every other value is computed as without it.
+template <bool kParams>
 __global__ void __launch_bounds__(256)
 act_backward_kernel(ActBackward e, int HW, int C, int chunk) {
-  __shared__ float4 red[3][256];
+  __shared__ float4 red[kParams ? 4 : 3][256];
+  __shared__ float nsum[kParams ? kActChunk : 1];
+  if constexpr (kParams) {
+    for (int i = threadIdx.x; i < kActChunk; i += 256) nsum[i] = 0.f;
+    __syncthreads();
+  }
+  float4 sg = make_float4(0.f, 0.f, 0.f, 0.f);
   const int cg = C >> 2, ppar = 256 / cg, tid = threadIdx.x;
   const int p = tid / cg, c4 = tid - p * cg;
   const int b = blockIdx.y;
@@ -640,12 +655,34 @@ act_backward_kernel(ActBackward e, int HW, int C, int chunk) {
 #undef NFI_G
       if (e.dacc_hi != nullptr) store_split4(e.dacc_hi, e.dacc_lo, idx, out, one);
       if (e.dacc != nullptr) *reinterpret_cast<float4*>(e.dacc + idx) = out;
+      if constexpr (kParams) {
+        sg.x += g.x; sg.y += g.y; sg.z += g.z; sg.w += g.w;
+        if (e.g_noise != nullptr) atomicAdd(&nsum[pos - blockIdx.x * chunk], (g.x + g.y) + (g.z + g.w));
+      }
     }
   }
   red[0][tid] = sa;
   red[1][tid] = sb;
   red[2][tid] = sd;
+  if constexpr (kParams) red[3][tid] = sg;
   __syncthreads();
+  if constexpr (kParams) {
+    if (e.g_noise != nullptr) {
+      const int p0 = blockIdx.x * chunk, n = min(HW, p0 + chunk) - p0;
+      for (int i = tid; i < n; i += 256) e.g_noise[(size_t)b * HW + p0 + i] += nsum[i];
+    }
+    if (e.g_bias != nullptr && tid < cg) {
+      float4 s = red[3][tid];
+      for (int k = 1; k < ppar; ++k) {
+        const float4 t = red[3][k * cg + tid];
+        s.x += t.x; s.y += t.y; s.z += t.z; s.w += t.w;
+      }
+      atomicAdd(e.g_bias + 4 * tid + 0, s.x);
+      atomicAdd(e.g_bias + 4 * tid + 1, s.y);
+      atomicAdd(e.g_bias + 4 * tid + 2, s.z);
+      atomicAdd(e.g_bias + 4 * tid + 3, s.w);
+    }
+  }
   if (tid < cg) {
     float* dst[3] = {e.ds_a, e.ds_b, e.dd};
 #pragma unroll
@@ -789,6 +826,254 @@ __global__ void styles_backward_kernel(const float* __restrict__ ds, const float
   g_ws[(size_t)b * ws_stride + k] += scale * acc;
 }
 
+// ------------------------------------------------------------------ backward to the parameters
+// dW[co,ci,tap] = sum_{b,p} G_b[p + a_off(tap), co] X_b[p + x_off(tap), ci]: G is the gradient of
+// the conv output before demodulation (dacc, the up layer's four raw-gradient phases, or dimg for
+// ToRGB) and X the layer's styled input x~, both position-major [B,H,W,C] bf16 pairs.  A k-tile is
+// 16 x 4 positions: one [64 ch x 64 positions] TMA box per operand (128-byte rows, SWIZZLE_128B),
+// which is the MN-major wgmma operand as it lands (K = positions; out-of-range rows / columns /
+// channels arrive as zeros = the 3x3 padding).  A work item is (Cout tile, Cin tile, tap, K range);
+// it runs its K range as chains of kWgChain k-tiles (A_lo X_hi + A_hi X_lo + A_hi X_hi, fp32
+// accumulate in registers), adds each chain into an fp32 total in registers, and stores the total
+// to its own slice of a partials buffer; wgrad_reduce_kernel sums the slices in a fixed order.
+//
+// wgrad_tc_kernel (persistent, 160 threads, two CTAs per SM):
+//   warps 0-3   consumer warpgroup: D[64 co x 64 ci], 12 wgmma (bf16, M64 N64 K16) per k-tile
+//   warp 4      TMA producer: 4 boxes per k-tile (G_hi, G_lo, X_hi, X_lo, 8 KB each), 3-stage ring
+constexpr int kWgTileH = 4, kWgTileW = 16;
+constexpr int kWgBox = 64 * 128;
+constexpr int kWgStage = 4 * kWgBox;
+constexpr int kWgStages = 3;
+constexpr int kWgThreads = 160;
+constexpr int kWgChain = 8;          // k-tiles (512 positions) per tensor-core accumulation chain
+constexpr int kWgItems = 1024;       // the K split aims at this many work items (device-independent)
+constexpr int kWgMinSplit = 16;      // k-tiles per work item at least
+
+struct WgradArgs {
+  int kt_y, kt_x, kt_img, kt_total;    // k-tiles per column / row of the domain, per image, all
+  int taps;
+  int a_dy[kMaxTaps], a_dx[kMaxTaps], a_img[kMaxTaps];  // G box offset of the tap
+  int x_dy[kMaxTaps], x_dx[kMaxTaps];                   // X box offset of the tap
+  int cout, cin, n_co, n_ci;           // channels and 64-channel tiles
+  int n_split, split_len;              // K ranges of split_len k-tiles
+  int chain;                           // k-tiles per chain
+  float* part;                         // [n_split][taps][cout][cin]
+};
+
+__global__ void __launch_bounds__(kWgThreads, 2)
+wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_constant__ CUtensorMap tmGl,
+                const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUtensorMap tmXl,
+                const __grid_constant__ WgradArgs a, int n_items) {
+  extern __shared__ __align__(1024) unsigned char smem[];
+  const int tid = threadIdx.x;
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + kWgStages * kWgStage);
+  uint64_t* empty = full + kWgStages;
+  if (tid == 0) {
+    if (tc::smem_u32(smem) & 1023u) __trap();
+    for (int i = 0; i < kWgStages; ++i) {
+      tc::mbar_init(&full[i], 1);
+      tc::mbar_init(&empty[i], 4);
+    }
+    tc::fence_mbar_init();
+    prefetch_tmap(&tmGh);
+    prefetch_tmap(&tmGl);
+    prefetch_tmap(&tmXh);
+    prefetch_tmap(&tmXl);
+  }
+  __syncthreads();
+  // item = ((split * taps + tap) * n_co + co) * n_ci + ci: concurrent CTAs share a K range (L2)
+  auto decode = [&](int item, int& ci, int& co, int& tap, int& k0, int& k1) {
+    ci = item % a.n_ci;
+    int r = item / a.n_ci;
+    co = r % a.n_co;
+    r /= a.n_co;
+    tap = r % a.taps;
+    const int split = r / a.taps;
+    k0 = split * a.split_len;
+    k1 = min(a.kt_total, k0 + a.split_len);
+  };
+
+  if (__shfl_sync(0xffffffffu, tid >> 7, 0) != 0) {
+    // ================================ TMA PRODUCER ================================
+    if (elect_one()) {
+      uint32_t st = 0, ph = 0;
+      for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+        int ci, co, tap, k0, k1;
+        decode(item, ci, co, tap, k0, k1);
+        for (int kt = k0; kt < k1; ++kt) {
+          const int img = kt / a.kt_img, r = kt - img * a.kt_img;
+          const int ty = r / a.kt_x, tx = r - ty * a.kt_x;
+          const int y0 = ty * kWgTileH, x0 = tx * kWgTileW;
+          tc::mbar_wait(&empty[st], ph ^ 1);
+          unsigned char* s = smem + st * kWgStage;
+          tc::mbar_expect_tx(&full[st], (uint32_t)kWgStage);
+          tma_load_4d(s, &tmGh, co * 64, x0 + a.a_dx[tap], y0 + a.a_dy[tap], img + a.a_img[tap], &full[st]);
+          tma_load_4d(s + kWgBox, &tmGl, co * 64, x0 + a.a_dx[tap], y0 + a.a_dy[tap], img + a.a_img[tap],
+                      &full[st]);
+          tma_load_4d(s + 2 * kWgBox, &tmXh, ci * 64, x0 + a.x_dx[tap], y0 + a.x_dy[tap], img, &full[st]);
+          tma_load_4d(s + 3 * kWgBox, &tmXl, ci * 64, x0 + a.x_dx[tap], y0 + a.x_dy[tap], img, &full[st]);
+          if (++st == kWgStages) { st = 0; ph ^= 1; }
+        }
+      }
+    }
+    return;
+  }
+  // ================================ CONSUMER WARPGROUP ================================
+  const int lane = tid & 31, warp = tid >> 5;
+  const int g4 = lane >> 2, t = lane & 3;
+  const uint32_t smem_s = tc::smem_u32(smem);
+  uint32_t st = 0, ph = 0;
+  for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+    int ci, co, tap, k0, k1;
+    decode(item, ci, co, tap, k0, k1);
+    float tot[32], acc[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) tot[i] = 0.f;
+    for (int c0 = k0; c0 < k1; c0 += a.chain) {
+      const int c1 = min(k1, c0 + a.chain);
+#pragma unroll
+      for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+      tc::wgmma_fence();
+      uint32_t prev_st = 0;
+      for (int k = c0; k < c1; ++k) {
+        tc::mbar_wait(&full[st], ph);
+        const uint32_t sb = smem_s + st * kWgStage;
+        // small terms first; a K step of 16 positions = 16 rows of 128 B = 2048 B (two 8-row groups)
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks)
+          tc::wgmma_bf16_ss_n64<1, 1>(acc, tc::gmma_desc(sb + kWgBox + 2048 * ks, tc::kSw128, 16, 1024),
+                                      tc::gmma_desc(sb + 2 * kWgBox + 2048 * ks, tc::kSw128, 16, 1024), 1);
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks)
+          tc::wgmma_bf16_ss_n64<1, 1>(acc, tc::gmma_desc(sb + 2048 * ks, tc::kSw128, 16, 1024),
+                                      tc::gmma_desc(sb + 3 * kWgBox + 2048 * ks, tc::kSw128, 16, 1024), 1);
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks)
+          tc::wgmma_bf16_ss_n64<1, 1>(acc, tc::gmma_desc(sb + 2048 * ks, tc::kSw128, 16, 1024),
+                                      tc::gmma_desc(sb + 2 * kWgBox + 2048 * ks, tc::kSw128, 16, 1024), 1);
+        tc::wgmma_commit();
+        // the previous stage's products are complete once at most this one's are in flight
+        tc::wgmma_wait<1>();
+        if (k > c0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty[prev_st]);
+        }
+        prev_st = st;
+        if (++st == kWgStages) { st = 0; ph ^= 1; }
+      }
+      tc::wgmma_wait<0>();
+      tc::reg_fence(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[prev_st]);
+#pragma unroll
+      for (int i = 0; i < 32; ++i) tot[i] += acc[i];
+    }
+    // rows co*64 + 16 warp + g4 (+8), columns ci*64 + 8j + 2t (+1)
+    const int split = k0 / a.split_len;
+    float* dst = a.part + ((size_t)split * a.taps + tap) * a.cout * a.cin;
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+      const int o = co * 64 + 16 * warp + g4 + 8 * half;
+      if (o >= a.cout) continue;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int i = ci * 64 + 8 * j + 2 * t;
+        if (i < a.cin) dst[(size_t)o * a.cin + i] = tot[4 * j + 2 * half];
+        if (i + 1 < a.cin) dst[(size_t)o * a.cin + i + 1] = tot[4 * j + 2 * half + 1];
+      }
+    }
+  }
+}
+
+// g_weight[co,ci,tap] += sum_split part[split][tap][co][ci] (split order fixed) and, for the
+// modulated 3x3 layers, the demodulation term: d = rsqrt(sum_ci s^2 sum_taps W^2 + 1e-8) gives
+// dd/dW[co,ci,tap] = -d^3 s_ci^2 W, and dd_true = dd_part / d (act_backward_kernel sums g (acc d)),
+// so dW -= W sum_b dd_part[b,co] d[b,co]^2 s[b,ci]^2.  One thread per (co, ci).
+__global__ void wgrad_reduce_kernel(const float* __restrict__ part, int n_split, int taps, int cout,
+                                    int cin, const float* __restrict__ w, const float* __restrict__ dd,
+                                    const float* __restrict__ d, const float* __restrict__ s, int B,
+                                    float* __restrict__ g_w) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x, n = (size_t)cout * cin;
+  if (i >= n) return;
+  const int o = (int)(i / cin), c = (int)(i % cin);
+  float dem = 0.f;
+  if (dd != nullptr)
+    for (int b = 0; b < B; ++b) {
+      const float dv = d[(size_t)b * cout + o], sv = s[(size_t)b * cin + c];
+      dem = fmaf(dd[(size_t)b * cout + o] * dv * dv, sv * sv, dem);
+    }
+  for (int tp = 0; tp < taps; ++tp) {
+    float acc = 0.f;
+    for (int sp = 0; sp < n_split; ++sp) acc += part[((size_t)sp * taps + tp) * n + i];
+    g_w[i * taps + tp] += acc - w[i * taps + tp] * dem;
+  }
+}
+
+// x~ = lrelu(u) s as a pair: the same arithmetic as act_store4, so the same bits the forward fed
+// the layer's GEMM
+__global__ void restyle_kernel(const float* __restrict__ u, const float* __restrict__ s, int B, int HW,
+                               int C, __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo) {
+  const int groups = C >> 2;
+  const size_t total = (size_t)B * HW * groups;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (size_t)gridDim.x * blockDim.x) {
+    const int g = (int)(i % groups);
+    const int img = (int)(i / ((size_t)HW * groups));
+    float4 v = __ldg(reinterpret_cast<const float4*>(u) + i);
+    v.x = lrelu(v.x); v.y = lrelu(v.y); v.z = lrelu(v.z); v.w = lrelu(v.w);
+    const float4 sv = __ldg(reinterpret_cast<const float4*>(s + (size_t)img * C) + g);
+    store_split4(hi, lo, i * 4, v, sv);
+  }
+}
+
+// out[c] += sum over rows of x[row, c] (ToRGB bias: sum_{b,p} dimg).  Block: a chunk of rows,
+// 256 / C rows in parallel, reduced in shared memory, one atomic per column per block.
+__global__ void __launch_bounds__(256)
+colsum_kernel(const float* __restrict__ x, size_t rows, int C, int chunk, float* __restrict__ out) {
+  __shared__ float red[256];
+  const int par = 256 / C, tid = threadIdx.x, r0 = tid / C, c = tid - r0 * C;
+  float acc = 0.f;
+  if (r0 < par) {
+    const size_t end = min(rows, (size_t)(blockIdx.x + 1) * chunk);
+    for (size_t r = (size_t)blockIdx.x * chunk + r0; r < end; r += par) acc += x[r * C + c];
+  }
+  red[tid] = acc;
+  __syncthreads();
+  if (tid < C) {
+    for (int k = 1; k < par; ++k) acc += red[k * C + tid];
+    atomicAdd(out + tid, acc);
+  }
+}
+
+// The affine's gradients from the style gradient ds [B,cin] (styles_kernel's transpose in the
+// other operand): g_aw[c,k] += scale sum_b ds[b,c] ws[b,row,k], g_ab[c] += gain sum_b ds[b,c]
+__global__ void affine_backward_kernel(const float* __restrict__ ds, const float* __restrict__ ws,
+                                       int ws_stride, int B, int cin, int w_dim, float scale, float gain,
+                                       float* __restrict__ g_aw, float* __restrict__ g_ab) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= cin * w_dim) return;
+  const int c = i / w_dim, k = i % w_dim;
+  float acc = 0.f, sb = 0.f;
+  for (int b = 0; b < B; ++b) {
+    const float v = ds[(size_t)b * cin + c];
+    acc = fmaf(v, ws[(size_t)b * ws_stride + k], acc);
+    sb += v;
+  }
+  if (g_aw != nullptr) g_aw[i] += scale * acc;
+  if (g_ab != nullptr && k == 0) g_ab[c] += gain * sb;
+}
+
+// b4.const: x~[b,p,c] = const[c,p] s[b,c], so g_const[c,p] += sum_b dx~[b,p,c] s[b,c]
+__global__ void const_grad_kernel(const float* __restrict__ dx, const float* __restrict__ s, int B, int C,
+                                  float* __restrict__ g_const) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= C * 16) return;
+  const int c = i / 16, p = i % 16;
+  float acc = 0.f;
+  for (int b = 0; b < B; ++b) acc = fmaf(dx[((size_t)b * 16 + p) * C + c], s[(size_t)b * C + c], acc);
+  g_const[i] += acc;
+}
+
 // ------------------------------------------------------------------ host side
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
                                   const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
@@ -807,11 +1092,12 @@ static EncodeTiledFn encode_fn() {
   return fn;
 }
 
-// activation tensor [B,H,W,C] bf16 -> boxes of [1, 16, 16, 64]
-static bool make_act_map(CUtensorMap* tm, const __nv_bfloat16* base, int B, int H, int W, int C) {
+// activation tensor [B,H,W,C] bf16 -> boxes of [1, box_h, 16, 64]
+static bool make_act_map(CUtensorMap* tm, const __nv_bfloat16* base, int B, int H, int W, int C,
+                         int box_h = kTileH) {
   const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
   const cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-  const cuuint32_t box[4] = {kKBlock, kTileW, kTileH, 1};
+  const cuuint32_t box[4] = {kKBlock, kTileW, (cuuint32_t)box_h, 1};
   const cuuint32_t es[4] = {1, 1, 1, 1};
   return encode_fn()(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<__nv_bfloat16*>(base), dims, strides,
                      box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
@@ -895,6 +1181,51 @@ static int launch_conv(ConvArgs& a, Pair in, Pair wt, int w_taps, cudaStream_t s
   NFI_SCUDA(cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   const int grid = n_tiles < sm_count() ? n_tiles : sm_count();
   conv_tc_kernel<<<grid, kConvThreads, smem, st>>>(tAh, tAl, tWh, tWl, a, n_tiles);
+  NFI_SCUDA(cudaGetLastError());
+  return 0;
+}
+
+// The K split of one weight-gradient GEMM over a DH x DW position domain of B images: fills the
+// k-tile counts and split; returns the number of work items.
+static int plan_wgrad(WgradArgs& a, int B, int DH, int DW) {
+  a.kt_y = (DH + kWgTileH - 1) / kWgTileH;
+  a.kt_x = (DW + kWgTileW - 1) / kWgTileW;
+  a.kt_img = a.kt_y * a.kt_x;
+  a.kt_total = B * a.kt_img;
+  a.n_co = (a.cout + 63) / 64;
+  a.n_ci = (a.cin + 63) / 64;
+  a.chain = kWgChain;
+  const int base = a.n_co * a.n_ci * a.taps;
+  int n_split = (kWgItems + base - 1) / base;
+  const int max_split = (a.kt_total + kWgMinSplit - 1) / kWgMinSplit;
+  if (n_split > max_split) n_split = max_split;
+  if (n_split < 1) n_split = 1;
+  a.split_len = (a.kt_total + n_split - 1) / n_split;
+  a.n_split = (a.kt_total + a.split_len - 1) / a.split_len;
+  return base * a.n_split;
+}
+
+// One weight-gradient GEMM (plan_wgrad'ed `a`): G [gB,gH,gW,cout] and X [B,xH,xW,cin] pairs.
+static int launch_wgrad(WgradArgs& a, Pair g, int gB, int gH, int gW, Pair x, int B, int xH, int xW,
+                        cudaStream_t st, char* err, size_t err_len) {
+  if (encode_fn() == nullptr) {
+    snprintf(err, err_len, "cuTensorMapEncodeTiled is not available from this driver");
+    return 1;
+  }
+  const int n_items = a.n_co * a.n_ci * a.taps * a.n_split;
+  CUtensorMap tGh, tGl, tXh, tXl;
+  if (!make_act_map(&tGh, g.hi, gB, gH, gW, a.cout, kWgTileH) ||
+      !make_act_map(&tGl, g.lo, gB, gH, gW, a.cout, kWgTileH) ||
+      !make_act_map(&tXh, x.hi, B, xH, xW, a.cin, kWgTileH) ||
+      !make_act_map(&tXl, x.lo, B, xH, xW, a.cin, kWgTileH)) {
+    snprintf(err, err_len, "cuTensorMapEncodeTiled failed (weight gradient, Cout %d Cin %d)", a.cout,
+             a.cin);
+    return 1;
+  }
+  const int smem = kWgStages * kWgStage + 128;
+  NFI_SCUDA(cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  const int grid = n_items < 2 * sm_count() ? n_items : 2 * sm_count();
+  wgrad_tc_kernel<<<grid, kWgThreads, smem, st>>>(tGh, tGl, tXh, tXl, a, n_items);
   NFI_SCUDA(cudaGetLastError());
   return 0;
 }
@@ -1168,8 +1499,14 @@ int forward(const nfi_synth_params& P, cudaStream_t st, char* err, size_t err_le
 // reuse safe): bufA holds g_rgb, then dx~ of conv1, then the raw-gradient phases of conv0; bufB the
 // dacc of conv1 (pair), then of conv0 (fp32); bufC dx~ of conv0 until the previous block's conv1
 // has consumed it.
+// With `PG` (the parameter backward) the same launches run, act_backward_kernel<true> in place of
+// <false>, and each layer's weight GEMM runs while its gradient operand is still in scratch: ToRGB
+// on dimg before the running image's adjoint overwrites it, conv1 on its dacc pair, conv0 on the
+// raw-gradient phases.  Its extra buffers (the rebuilt layer input x~ and the GEMM partials) come
+// after the plain backward's, which keep their places.
 static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, const Saved& sv, Bump& ws,
-                        cudaStream_t st, bool dry, char* err, size_t err_len) {
+                        cudaStream_t st, bool dry, char* err, size_t err_len,
+                        const nfi_synth_param_grads* PG = nullptr) {
   const int B = P.batch, nb = P.num_blocks, D = P.w_dim, R = P.img_resolution, NI = P.img_channels;
   const float sqrt2 = 1.4142135623730951f;
   auto blocks = [](size_t n, int per) { return (unsigned)((n + per - 1) / per); };
@@ -1210,6 +1547,31 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
     wt1[i] = ws.pair((size_t)9 * c * c);
     wtr[i] = ws.pair((size_t)NI * c);
   }
+  Pair xt = {nullptr, nullptr};  // the layer input x~ of the current weight GEMM
+  float* part = nullptr;         // its partials
+  auto wgrad_args = [](int cout, int cin, int taps) {
+    WgradArgs a;
+    memset(&a, 0, sizeof(a));
+    a.cout = cout; a.cin = cin; a.taps = taps;
+    return a;
+  };
+  if (PG) {
+    xt = ws.pair(full);
+    size_t pmax = 0;
+    auto need = [&](int cout, int cin, int taps, int D_) {
+      WgradArgs a = wgrad_args(cout, cin, taps);
+      plan_wgrad(a, B, D_, D_);
+      const size_t n = (size_t)a.n_split * taps * cout * cin;
+      pmax = n > pmax ? n : pmax;
+    };
+    for (int i = 0; i < nb; ++i) {
+      const int res = 4 << i, c = P.channels[i];
+      need(NI, c, 1, res);
+      need(c, c, 9, res);
+      if (i) need(c, P.channels[i - 1], 9, res / 2);
+    }
+    part = ws.take(pmax);
+  }
   if (dry) return 0;
 
   NFI_SCUDA(cudaMemsetAsync(sums, 0, small * sizeof(float), st));
@@ -1232,15 +1594,39 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
       snprintf(err, err_len, "synthesis backward: %d channels unsupported", C);
       return 1;
     }
-    const int chunk = 1024;
+    const int chunk = kActChunk;
     dim3 grid((unsigned)((HW + chunk - 1) / chunk), (unsigned)B);
-    act_backward_kernel<<<grid, 256, 0, st>>>(e, HW, C, chunk);
+    if (PG)
+      act_backward_kernel<true><<<grid, 256, 0, st>>>(e, HW, C, chunk);
+    else
+      act_backward_kernel<false><<<grid, 256, 0, st>>>(e, HW, C, chunk);
     NFI_SCUDA(cudaGetLastError());
     return 0;
   };
   auto to_ws = [&](const float* ds, const nfi_synth_layer& L, int cin, int row, float gain) {
     styles_backward_kernel<<<blocks((size_t)B * D, 256), 256, 0, st>>>(
         ds, L.affine_w, cin, D, B, gain / sqrtf((float)D), G.g_ws + (size_t)row * D, P.num_ws * D);
+  };
+  // ---- parameter backward (PG only) ----
+  auto affine = [&](const float* ds, const nfi_synth_layer_grads& L, int cin, int row, float gain) {
+    if (L.g_affine_w == nullptr && L.g_affine_b == nullptr) return;
+    affine_backward_kernel<<<blocks((size_t)cin * D, 256), 256, 0, st>>>(
+        ds, P.ws + (size_t)row * D, P.num_ws * D, B, cin, D, gain / sqrtf((float)D), gain, L.g_affine_w,
+        L.g_affine_b);
+  };
+  auto restyle = [&](const float* u, const float* s, int HW, int C) {
+    restyle_kernel<<<flat_grid((size_t)B * HW * C / 4), 256, 0, st>>>(u, s, B, HW, C, xt.hi, xt.lo);
+  };
+  // plan, GEMM into the partials, then the fixed-order sum (+ demodulation term where dd is set)
+  auto wgrad = [&](WgradArgs& a, Pair g, int gB, int gH, int D_, const float* w, const float* dd,
+                   const float* d, const float* s, float* g_w) -> int {
+    plan_wgrad(a, B, D_, D_);
+    a.part = part;
+    if (const int rc = launch_wgrad(a, g, gB, gH, gH, xt, B, D_, D_, st, err, err_len)) return rc;
+    wgrad_reduce_kernel<<<blocks((size_t)a.cout * a.cin, 256), 256, 0, st>>>(
+        part, a.n_split, a.taps, a.cout, a.cin, w, dd, d, s, B, g_w);
+    NFI_SCUDA(cudaGetLastError());
+    return 0;
   };
   auto stride1_taps = [](ConvArgs& a, int H, int W) {  // the adjoint of conv3x3_phases: taps flipped
     conv3x3_phases(a, H, W);
@@ -1265,6 +1651,19 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
       const int rc = launch_conv(a, dimg_p, wtr[i], 1, st, err, err_len);
       if (rc) return rc;
     }
+    if (PG) {  // ToRGB bias and weight: sum dimg, and dimg against x~ = lrelu(u1) s_rgb
+      const nfi_synth_layer_grads& L = PG->torgb[i];
+      if (L.g_bias != nullptr) {
+        const size_t rows = (size_t)B * HW;
+        colsum_kernel<<<blocks(rows, kActChunk), 256, 0, st>>>(dimg[cur], rows, NI, kActChunk, L.g_bias);
+      }
+      if (L.g_weight != nullptr) {
+        restyle(sv.u1[i], sv.style_rgb[i], HW, c);
+        WgradArgs a = wgrad_args(NI, c, 1);
+        if (int rc = wgrad(a, dimg_p, B, res, res, P.torgb[i].weight, nullptr, nullptr, nullptr, L.g_weight))
+          return rc;
+      }
+    }
     if (i) {  // the running image's gradient one block down (the GEMM above has read dimg_p)
       const int h = res / 2;
       upsample_adjoint_kernel<<<flat_grid((size_t)B * h * h * NI), 256, 0, st>>>(
@@ -1284,13 +1683,19 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
       Pair pb = {reinterpret_cast<__nv_bfloat16*>(bufB),
                  reinterpret_cast<__nv_bfloat16*>(bufB) + (size_t)B * HW * c};
       e.dacc_hi = pb.hi; e.dacc_lo = pb.lo;
+      if (PG) {
+        e.g_bias = PG->conv1[i].g_bias;
+        e.g_noise = P.conv1[i].noise ? PG->conv1[i].g_noise : nullptr;
+      }
       if (int rc = act_backward(e, HW, c)) return rc;
       to_ws(dsr[i], P.torgb[i], c, sv.row_rgb[i], 1.f / sqrtf((float)c));
+      if (PG) affine(dsr[i], PG->torgb[i], c, sv.row_rgb[i], 1.f / sqrtf((float)c));
       if (!last) {
         const int cn = P.channels[i + 1];
         dcoef_backward_kernel<<<blocks((size_t)B * c * 32, 256), 256, 0, st>>>(
             sv.wsq0[i + 1], sv.style0[i + 1], dd0[i + 1], sv.dco0[i + 1], cn, c, B, ds0[i + 1]);
         to_ws(ds0[i + 1], P.conv0[i + 1], c, sv.row0[i + 1], 1.f);
+        if (PG) affine(ds0[i + 1], PG->conv0[i + 1], c, sv.row0[i + 1], 1.f);
       }
       // dx~ of conv1 = conv^T(dacc, W1) -> bufA
       ConvArgs a;
@@ -1301,12 +1706,30 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
       a.out_raw = bufA; a.out_H = res; a.out_W = res; a.out_stride = 1;
       const int rc = launch_conv(a, pb, wt1[i], 9, st, err, err_len);
       if (rc) return rc;
+      if (PG && PG->conv1[i].g_weight != nullptr) {  // dacc against x~ = lrelu(u0) s1 (const s1)
+        if (i)
+          restyle(sv.u0[i], sv.style1[i], HW, c);
+        else
+          const_input_kernel<<<blocks((size_t)B * 16 * c, 256), 256, 0, st>>>(P.const_input, sv.style1[0],
+                                                                             B, c, xt.hi, xt.lo);
+        WgradArgs w = wgrad_args(c, c, 9);
+        for (int t = 0; t < 9; ++t) {
+          w.x_dy[t] = t / 3 - 1;
+          w.x_dx[t] = t % 3 - 1;
+        }
+        if (int rc2 = wgrad(w, pb, B, res, res, P.conv1[i].weight, dd1[i], sv.dco1[i], sv.style1[i],
+                            PG->conv1[i].g_weight))
+          return rc2;
+      }
     }
     if (i == 0) {
       const_ds_kernel<<<blocks((size_t)B * c, 256), 256, 0, st>>>(bufA, P.const_input, B, c, ds1[0]);
+      if (PG && PG->g_const != nullptr)
+        const_grad_kernel<<<blocks((size_t)c * 16, 256), 256, 0, st>>>(bufA, sv.style1[0], B, c, PG->g_const);
       dcoef_backward_kernel<<<blocks((size_t)B * c * 32, 256), 256, 0, st>>>(
           sv.wsq1[0], sv.style1[0], dd1[0], sv.dco1[0], c, c, B, ds1[0]);
       to_ws(ds1[0], P.conv1[0], c, sv.row1[0], 1.f);
+      if (PG) affine(ds1[0], PG->conv1[0], c, sv.row1[0], 1.f);
       NFI_SCUDA(cudaGetLastError());
       break;
     }
@@ -1319,10 +1742,15 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
       e.dx_a = bufA; e.s_a = sv.style1[i]; e.ds_a = ds1[i];
       e.dd = dd0[i];
       e.dacc = bufB;
+      if (PG) {
+        e.g_bias = PG->conv0[i].g_bias;
+        e.g_noise = P.conv0[i].noise ? PG->conv0[i].g_noise : nullptr;
+      }
       if (int rc = act_backward(e, HW, c)) return rc;
       dcoef_backward_kernel<<<blocks((size_t)B * c * 32, 256), 256, 0, st>>>(
           sv.wsq1[i], sv.style1[i], dd1[i], sv.dco1[i], c, c, B, ds1[i]);
       to_ws(ds1[i], P.conv1[i], c, sv.row1[i], 1.f);
+      if (PG) affine(ds1[i], PG->conv1[i], c, sv.row1[i], 1.f);
     }
     // FIR adjoint -> the four parity phases of the raw gradient (pair in bufA), then the
     // stride-2 correlation with W0 as 9 stride-1 taps over them -> dx~ of conv0 in bufC
@@ -1333,6 +1761,22 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
       fir_adjoint_kernel<<<flat_grid((size_t)4 * B * (h + 1) * (h + 1) * (c / 4)), 256, 0, st>>>(
           bufB, B, res, res, c, ph.hi, ph.lo);
       NFI_SCUDA(cudaGetLastError());
+      if (PG && PG->conv0[i].g_weight != nullptr) {
+        // raw gradient at (2i+ky, 2j+kx) = phase (ky%2, kx%2) at (i + ky/2, j + kx/2), against
+        // x~ = lrelu(u1 of block i-1) s0 on the low-resolution grid
+        restyle(sv.u1[i - 1], sv.style0[i], h * h, ci);
+        WgradArgs w = wgrad_args(c, ci, 9);
+        for (int ky = 0; ky < 3; ++ky)
+          for (int kx = 0; kx < 3; ++kx) {
+            const int t = ky * 3 + kx;
+            w.a_dy[t] = ky / 2;
+            w.a_dx[t] = kx / 2;
+            w.a_img[t] = ((ky & 1) * 2 + (kx & 1)) * B;
+          }
+        if (int rc = wgrad(w, ph, 4 * B, h + 1, h, P.conv0[i].weight, dd0[i], sv.dco0[i], sv.style0[i],
+                           PG->conv0[i].g_weight))
+          return rc;
+      }
       ConvArgs a;
       memset(&a, 0, sizeof(a));
       a.B = B; a.C = c; a.N = ci; a.H = h + 1; a.W = h + 1;
@@ -1411,6 +1855,42 @@ int backward(const nfi_synth_params& P, const nfi_synth_grads& G, cudaStream_t s
   memset(&sv, 0, sizeof(sv));
   if (const int rc = saved_layout(P, b, sv, err, err_len)) return rc;
   return run_backward(P, G, sv, b, st, false, err, err_len);
+}
+
+size_t param_workspace_bytes(const nfi_synth_params& P) {
+  char err[256];
+  if (check_params(P, err, sizeof(err))) return 0;
+  Bump b{nullptr, 0, 0};
+  Saved sv;
+  memset(&sv, 0, sizeof(sv));
+  saved_layout(P, b, sv, err, sizeof(err));
+  nfi_synth_grads g = {nullptr, nullptr};
+  nfi_synth_param_grads pg;
+  memset(&pg, 0, sizeof(pg));
+  run_backward(P, g, sv, b, nullptr, true, err, sizeof(err), &pg);
+  return b.off + 1024;
+}
+
+int backward_params(const nfi_synth_params& P, const nfi_synth_grads& G, const nfi_synth_param_grads& PG,
+                    cudaStream_t st, char* err, size_t err_len) {
+  if (const int rc = check_saved(P, err, err_len)) return rc;
+  if (G.g_planes == nullptr || G.g_ws == nullptr) {
+    snprintf(err, err_len, "synthesis backward: g_planes and g_ws must be set");
+    return 1;
+  }
+  const size_t need = param_workspace_bytes(P);
+  if (P.workspace_bytes < need) {
+    snprintf(err, err_len, "synthesis parameter backward: workspace too small (%zu < %zu bytes)",
+             P.workspace_bytes, need);
+    return 1;
+  }
+  unsigned char* base = reinterpret_cast<unsigned char*>(
+      (reinterpret_cast<uintptr_t>(P.workspace) + 1023) & ~(uintptr_t)1023);
+  Bump b{base, 0, P.workspace_bytes};
+  Saved sv;
+  memset(&sv, 0, sizeof(sv));
+  if (const int rc = saved_layout(P, b, sv, err, err_len)) return rc;
+  return run_backward(P, G, sv, b, st, false, err, err_len, &PG);
 }
 
 }  // namespace synth

@@ -21,6 +21,12 @@ network -- the inversion loop, which differentiates the render to the latents (a
 the planes come from ``FusedSynthesis.forward_differentiable``, whose backward carries dL/dplanes
 to ws on the sm_90a kernels.  Mapping network, texture mapper and the ``expand`` of [B,1,512]
 latents stay torch autograd.  ``render`` picks it with ``render.enable_fused_inversion``.
+
+``GeneratorStepFront(G)`` is ``HeadsGeneratorFront``'s body (regulariser heads on the fused point
+evaluator) for grad-enabled calls with a trainable synthesis network -- the GAN generator step and
+the SDF pre-training step -- with the planes from ``FusedSynthesis.forward_trainable``.
+``render`` (and ``ParallelModel``'s ``pretrain_sdf`` branch) pick it with
+``render.enable_fused_generator_step``.
 """
 import torch
 
@@ -158,8 +164,16 @@ class HeadsGeneratorFront:
     the same order as the reference: synthesis noise, path-length noise, stratified points,
     total-variation perturbation."""
 
+    layout = 'channel_first'   # of the planes _planes returns
+
     def __init__(self, generator):
         self.g = generator
+
+    def _planes(self, w_synthesis, batch, model_inputs):
+        """The plane producer: the reference module, [B,3,32,R,R] channel-first."""
+        block_kwargs = {'noise_mode': 'const'} if model_inputs.get('freeze_noise') else {}
+        planes = self.g.synthesis_network(w_synthesis, **block_kwargs)
+        return planes.view(batch, 3, 32, planes.shape[-2], planes.shape[-1])
 
     @staticmethod
     def supports(request_model_outputs, model_inputs):
@@ -178,9 +192,7 @@ class HeadsGeneratorFront:
             assert torch.is_grad_enabled()
             ws = ws.contiguous().requires_grad_()
         attention_values, w_synthesis = resolve_palette(g, ws, request_model_outputs, model_inputs)
-        block_kwargs = {'noise_mode': 'const'} if model_inputs.get('freeze_noise') else {}
-        planes = g.synthesis_network(w_synthesis, **block_kwargs)
-        planes = planes.view(batch, 3, 32, planes.shape[-2], planes.shape[-1])
+        planes = self._planes(w_synthesis, batch, model_inputs)
         out = {}
         if 'attention_values' in request_model_outputs:
             assert g.attention_values > 0
@@ -195,10 +207,48 @@ class HeadsGeneratorFront:
         w1, b1, w2, b2 = decoder_weights(g)
         out.update(regulariser_heads(planes, w1, b1, w2, b2, getattr(g, 'beta', None),
                                      g.scene_range, request_model_outputs, use_sdf=g.use_sdf,
-                                     training=g.training))
+                                     training=g.training, layout=self.layout))
         if 'sampler' in request_model_outputs:
-            out['triplane'] = dict(planes=planes, planes_layout='channel_first',
+            out['triplane'] = dict(planes=planes, planes_layout=self.layout,
                                    palette=attention_values, w1=w1, b1=b1, w2=w2, b2=b2,
                                    beta=getattr(g, 'beta', None), alpha=getattr(g, 'alpha', None),
                                    **view)
         return out
+
+
+class GeneratorStepFront(HeadsGeneratorFront):
+    """The GAN generator step and the SDF pre-training step with the plane producer on sm_90a:
+    ``HeadsGeneratorFront``'s body with the planes from ``FusedSynthesis.forward_trainable``
+    (channel-last; the heads and the render read that layout), whose backward carries dL/dplanes
+    to ws and to every synthesis parameter.  Envelope: grad enabled, a synthesis parameter
+    requires grad, requests within SUPPORTED_OUTPUTS + HEAD_OUTPUTS ('path_length' is a double
+    backward through the synthesis network: it keeps the reference module).  It does not overlap
+    ``FusedGeneratorFront`` (no_grad) or ``FusedInversionFront`` (frozen synthesis).  Same random
+    draws in the same order as the reference: synthesis noise, stratified points, total-variation
+    perturbation.  ``render`` picks it with ``render.enable_fused_generator_step``."""
+
+    layout = 'channel_last'
+
+    def __init__(self, generator):
+        super().__init__(generator)
+        self.synthesis = FusedSynthesis(generator.synthesis_network)
+
+    def _planes(self, w_synthesis, batch, model_inputs):
+        noise_mode = 'const' if model_inputs.get('freeze_noise') else 'random'
+        planes_cl = self.synthesis.forward_trainable(w_synthesis, noise_mode=noise_mode)
+        assert planes_cl.shape[0] == batch
+        return planes_cl
+
+    def supports(self, request_model_outputs, model_inputs):
+        return (torch.is_grad_enabled()
+                and any(p.requires_grad for p in self.g.synthesis_network.parameters())
+                and all(o in SUPPORTED_OUTPUTS + HEAD_OUTPUTS for o in request_model_outputs)
+                and all(k in ('freeze_noise', 'attention_values', 'attention_values_bias')
+                        for k in model_inputs))
+
+    def __call__(self, viewdir, c, request_model_outputs=['sampler'], model_inputs={}):
+        if not self.supports(request_model_outputs, model_inputs):
+            raise _lib.NfiError('GeneratorStepFront: outside its envelope (grad enabled, a '
+                                'trainable synthesis network, outputs within %r)'
+                                % (SUPPORTED_OUTPUTS + HEAD_OUTPUTS,))
+        return super().__call__(viewdir, c, request_model_outputs, model_inputs)

@@ -58,6 +58,7 @@ def configure(new_args, new_dataset_config, samples_per_ray=None):
 _FRONTS = {}
 _INV_FRONTS = {}
 _HEAD_FRONTS = {}
+_GEN_FRONTS = {}
 
 
 def enable_fused_heads(target_model, enabled=True):
@@ -96,6 +97,20 @@ def enable_fused_inversion(target_model, enabled=True):
         _INV_FRONTS[id(target_model)] = FusedInversionFront(target_model)
     else:
         _INV_FRONTS.pop(id(target_model), None)
+
+
+def enable_fused_generator_step(target_model, enabled=True):
+    """Makes ``render`` (and ``ParallelModel``'s SDF pre-training branch) produce
+    ``target_model``'s tri-planes with the sm_90a synthesis kernels, forward and backward to ws and
+    to every synthesis parameter, for grad-enabled calls with a trainable synthesis network and
+    requests within SUPPORTED_OUTPUTS + HEAD_OUTPUTS (generator.GeneratorStepFront: the GAN
+    generator step, the dual discriminator's second call, SDF pre-training).  'path_length' and
+    calls outside that envelope route as before."""
+    from .generator import GeneratorStepFront
+    if enabled:
+        _GEN_FRONTS[id(target_model)] = GeneratorStepFront(target_model)
+    else:
+        _GEN_FRONTS.pop(id(target_model), None)
 
 
 def _closure_vars(fn):
@@ -224,6 +239,7 @@ def render(target_model,
     requests = ['sampler'] + list(extra_model_outputs)
     front = _FRONTS.get(id(target_model))
     ifront = _INV_FRONTS.get(id(target_model))
+    gfront = _GEN_FRONTS.get(id(target_model))
     hfront = _HEAD_FRONTS.get(id(target_model))
     if front is not None and front.supports(requests, extra_model_inputs):
         # plane producer on sm_90a too (generator.FusedGeneratorFront; no_grad calls only)
@@ -231,6 +247,9 @@ def render(target_model,
     elif ifront is not None and ifront.supports(requests, extra_model_inputs):
         # ... and its backward to the latents (generator.FusedInversionFront; frozen synthesis)
         model_outputs = ifront(viewdirs, model_input, requests, extra_model_inputs)
+    elif gfront is not None and gfront.supports(requests, extra_model_inputs):
+        # ... and to the synthesis parameters (generator.GeneratorStepFront; generator step)
+        model_outputs = gfront(viewdirs, model_input, requests, extra_model_inputs)
     elif hfront is not None and hfront.supports(requests, extra_model_inputs):
         # regulariser heads on the fused point evaluator (generator.HeadsGeneratorFront)
         model_outputs = hfront(viewdirs, model_input, requests, extra_model_inputs)
@@ -299,6 +318,9 @@ class ParallelModel(nn.Module):
         model_to_use = self.model_ema if use_ema else self.model
         if pretrain_sdf:
             req = ['sdf_distance_loss', 'sdf_eikonal_loss']
+            gfront = _GEN_FRONTS.get(id(model_to_use))
+            if gfront is not None and gfront.supports(req, {}):
+                return gfront(None, c, request_model_outputs=req)
             hfront = _HEAD_FRONTS.get(id(model_to_use))
             if hfront is not None:
                 return hfront(None, c, request_model_outputs=req)

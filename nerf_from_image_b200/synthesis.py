@@ -23,10 +23,13 @@ parameter frozen, gradients to the latents -- has its own entry:
     planes_cl = FusedSynthesis(net).forward_differentiable(ws, noise_mode='random')
 
 which runs ``nfi_synthesis_forward_saved`` (the same planes, bit for bit, plus each layer's
-pre-activation kept in the workspace) and, in backward, ``nfi_synthesis_backward`` to ws.
-Gradients to the weights, biases, affines, noise or ``b4.const`` are not offered: a network with
-a trainable parameter raises (the GAN loop keeps the reference module).  There is no CPU path
-and no fallback.
+pre-activation kept in the workspace) and, in backward, ``nfi_synthesis_backward`` to ws; a
+network with a trainable parameter raises there.  The generator step -- gradients to ws and to
+every parameter, noise strengths included -- has its own entry:
+
+    planes_cl = FusedSynthesis(net).forward_trainable(ws, noise_mode='random')
+
+backed by ``nfi_synthesis_backward_params``.  There is no CPU path and no fallback.
 """
 import ctypes
 import math
@@ -131,8 +134,44 @@ class FusedSynthesis:
                                 '(there is no CPU path)')
         return _SynthesisFunction.apply(ws, self, noise_mode)
 
-    def _run(self, ws, noise_mode, saved):
-        """-> (planes, (P, keep, work)) -- P, keep and work stay valid for a backward."""
+    def _layers(self):
+        """(kind, block index, layer) of every layer with parameters, in the C ABI's order."""
+        for i, blk in enumerate(self.blocks):
+            if i:
+                yield 'conv0', i, blk.conv0
+            yield 'conv1', i, blk.conv1
+            yield 'torgb', i, blk.torgb
+
+    def forward_trainable(self, ws, noise_mode='random'):
+        """Channel-last planes [B,3,R,R,32] differentiable with respect to ``ws`` and every
+        network parameter (weights, biases, affines, ``b4.const``) -- the GAN generator step.  The
+        per-layer noise tensors are formed here as ``raw * noise_strength`` (the same draws, in the
+        same order, as ``__call__``'s) and enter the autograd Function as inputs, so autograd
+        carries their gradient on to ``noise_strength``.  The backward runs
+        ``nfi_synthesis_backward_params``; it is not differentiable (no ``create_graph``, so no
+        path-length regulariser) and runs once per forward."""
+        assert noise_mode in ['random', 'const']
+        if not ws.is_cuda:
+            raise _lib.NfiError('the fused synthesis network only runs on CUDA tensors '
+                                '(there is no CPU path)')
+        B, dev = ws.shape[0], ws.device
+        noises = []   # per block (conv0, conv1), in the module's layer order like _run's draws
+        for i, blk in enumerate(self.blocks):
+            n0 = self._layer_noise(blk.conv0, B, noise_mode, dev) if i else None
+            noises.append((n0, self._layer_noise(blk.conv1, B, noise_mode, dev)))
+        params = []
+        for _, _, layer in self._layers():
+            params += [layer.weight, layer.affine.weight, layer.affine.bias, layer.bias]
+        params.append(self.blocks[0].const)
+        present = [(n0 is not None, n1 is not None) for n0, n1 in noises]
+        flat_noise = [n for pair in noises for n in pair if n is not None]
+        return _SynthesisTrainFunction.apply(ws, self, noise_mode, present, len(params),
+                                             *params, *flat_noise)
+
+    def _run(self, ws, noise_mode, saved, noises=None, trainable=False):
+        """-> (planes, (P, keep, work)) -- P, keep and work stay valid for a backward.  ``noises``:
+        per block (conv0, conv1) tensors drawn by the caller (else drawn here); ``trainable``
+        sizes the workspace for the parameter backward."""
         net = self.net
         lib = _lib.load()
         dev = ws.device
@@ -163,16 +202,24 @@ class FusedSynthesis:
                 P.channels[i] = blk.conv1.out_channels
                 if i == 0:
                     P.const_input = _ptr(f32(blk.const))
+                elif noises is not None:
+                    fill(P.conv0[i], blk.conv0, noises[i][0])
                 else:
                     fill(P.conv0[i], blk.conv0, self._layer_noise(blk.conv0, B, noise_mode, dev))
-                fill(P.conv1[i], blk.conv1, self._layer_noise(blk.conv1, B, noise_mode, dev))
+                if noises is not None:
+                    fill(P.conv1[i], blk.conv1, noises[i][1])
+                else:
+                    fill(P.conv1[i], blk.conv1, self._layer_noise(blk.conv1, B, noise_mode, dev))
                 fill(P.torgb[i], blk.torgb, None)
             P.ws = _ptr(ws)
             R = net.img_resolution
             planes = torch.empty(B, 3, R, R, 32, device=dev, dtype=torch.float32)
             P.planes = _ptr(planes)
-            sizer = lib.nfi_synthesis_saved_workspace_bytes if saved else \
-                lib.nfi_synthesis_workspace_bytes
+            if trainable:
+                sizer = lib.nfi_synthesis_param_workspace_bytes
+            else:
+                sizer = lib.nfi_synthesis_saved_workspace_bytes if saved else \
+                    lib.nfi_synthesis_workspace_bytes
             need = sizer(ctypes.byref(P))
             if need == 0:
                 raise _lib.NfiError('unsupported synthesis configuration (channels must be '
@@ -216,6 +263,63 @@ class _SynthesisFunction(torch.autograd.Function):
             _lib.check(_lib.load().nfi_synthesis_backward(ctypes.byref(P), ctypes.byref(G), stream))
         del P, keep, work
         return g_ws.to(ctx.ws_dtype), None, None
+
+
+class _SynthesisTrainFunction(torch.autograd.Function):
+    """(ws, every parameter, the per-layer noise tensors) -> planes (channel-last), with
+    nfi_synthesis_backward_params as the backward."""
+
+    @staticmethod
+    def forward(ctx, ws, fs, noise_mode, present, n_params, *tensors):
+        params, flat_noise = tensors[:n_params], list(tensors[n_params:])
+        noises = [(flat_noise.pop(0) if h0 else None, flat_noise.pop(0) if h1 else None)
+                  for h0, h1 in present]
+        planes, state = fs._run(ws, noise_mode, saved=True, noises=noises, trainable=True)
+        ctx.state, ctx.fs, ctx.present, ctx.ws_dtype = state, fs, present, ws.dtype
+        ctx.param_meta = [(p.shape, p.dtype) for p in params]
+        ctx.noise_meta = [(n.shape, n.dtype) for pair in noises for n in pair if n is not None]
+        return planes
+
+    @staticmethod
+    def backward(ctx, g_planes):
+        if ctx.state is None:
+            raise _lib.NfiError('the fused synthesis backward ran twice on one forward '
+                                '(retain_graph is not supported: the workspace is released)')
+        if torch.is_grad_enabled():
+            raise _lib.NfiError('the fused synthesis backward is not differentiable (create_graph, '
+                                'e.g. the path-length regulariser): use the reference module')
+        P, keep, work = ctx.state
+        ctx.state = None          # the workspace and fp32 copies go once this returns
+        dev = g_planes.device
+        g_planes = g_planes.to(torch.float32).contiguous()
+        ws32 = keep[0]
+        g_ws = torch.zeros_like(ws32)
+        G = _lib.SynthGrads(g_planes=g_planes.data_ptr(), g_ws=g_ws.data_ptr())
+        zeros = lambda shape: torch.zeros(shape, dtype=torch.float32, device=dev)
+        g_params = [zeros(shape) for shape, _ in ctx.param_meta]
+        g_noise = [zeros(shape) for shape, _ in ctx.noise_meta]
+        PG = _lib.SynthParamGrads()
+        k = 0
+        for kind, i, _ in ctx.fs._layers():
+            dst = getattr(PG, kind)[i]
+            dst.g_weight, dst.g_affine_w, dst.g_affine_b, dst.g_bias = (
+                _ptr(g) for g in g_params[k:k + 4])
+            k += 4
+        PG.g_const = _ptr(g_params[k])
+        it = iter(g_noise)
+        for i, (h0, h1) in enumerate(ctx.present):
+            if h0:
+                PG.conv0[i].g_noise = _ptr(next(it))
+            if h1:
+                PG.conv1[i].g_noise = _ptr(next(it))
+        with torch.cuda.device(dev):
+            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            _lib.check(_lib.load().nfi_synthesis_backward_params(
+                ctypes.byref(P), ctypes.byref(G), ctypes.byref(PG), stream))
+        del P, keep, work
+        out = [g.to(dt) for g, (_, dt) in zip(g_params, ctx.param_meta)]
+        out += [g.to(dt) for g, (_, dt) in zip(g_noise, ctx.noise_meta)]
+        return (g_ws.to(ctx.ws_dtype), None, None, None, None, *out)
 
 
 def planes_channel_first(planes_cl):
