@@ -126,6 +126,28 @@ NFI_API int nfi_synthesis_backward_params(const nfi_synth_params *params,
                                           const nfi_synth_grads *grads,
                                           const nfi_synth_param_grads *param_grads, void *stream);
 
+/* Path-length regulariser (the double backward of generator.py's path_length): with n = g_planes
+   the cotangent a first-order nfi_synthesis_backward turned into g_ws = J_ws^T n, and t = t_ws the
+   cotangent that arrives on that g_ws, nfi_synthesis_backward_hvp forms the gradient of
+   <t, J_ws^T n> with respect to ws (g_ws here, a Hessian-vector product), and, where param_grads
+   is not NULL, with respect to every parameter and noise tensor (the same fields as
+   nfi_synthesis_backward_params, ACCUMULATED).  It is the tangent of that backward along t: a
+   tangent forward pass, then the backward walk beside its tangent on the same GEMM kernels, the
+   product and its tangent stacked as 2B images.  params->workspace is a saved forward's and is only
+   read, so a later nfi_synthesis_backward_params on it is unaffected. */
+typedef struct nfi_synth_hvp {
+  const float *g_planes; /* [B,3,R,R,32] the cotangent n that g_ws was formed with */
+  const float *t_ws;     /* [B,num_ws,w_dim] cotangent of g_ws; rows the network does not read are ignored */
+  float *g_ws;           /* [B,num_ws,w_dim] ACCUMULATED */
+  void *scratch;         /* >= nfi_synthesis_hvp_scratch_bytes(params); separate from params->workspace */
+  size_t scratch_bytes;
+} nfi_synth_hvp;
+
+NFI_API size_t nfi_synthesis_hvp_scratch_bytes(const nfi_synth_params *params);
+NFI_API int nfi_synthesis_backward_hvp(const nfi_synth_params *params, const nfi_synth_hvp *hvp,
+                                       const nfi_synth_param_grads *param_grads /* may be NULL */,
+                                       void *stream);
+
 #ifdef __cplusplus
 }
 #endif

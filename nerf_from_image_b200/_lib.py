@@ -122,6 +122,12 @@ class SynthParamGrads(ctypes.Structure):
     ]
 
 
+class SynthHvp(ctypes.Structure):
+    """struct nfi_synth_hvp."""
+    _fields_ = [('g_planes', ctypes.c_void_p), ('t_ws', ctypes.c_void_p), ('g_ws', ctypes.c_void_p),
+                ('scratch', ctypes.c_void_p), ('scratch_bytes', ctypes.c_size_t)]
+
+
 class SdfPointsParams(ctypes.Structure):
     """struct nfi_sdf_points_params (include/nfi_heads.h)."""
     _fields_ = [('batch', ctypes.c_int32), ('plane_res', ctypes.c_int32),
@@ -177,6 +183,11 @@ EXPORTS = {
                                                      ctypes.POINTER(SynthGrads),
                                                      ctypes.POINTER(SynthParamGrads),
                                                      ctypes.c_void_p]),
+    'nfi_synthesis_hvp_scratch_bytes': (ctypes.c_size_t, [ctypes.POINTER(SynthParams)]),
+    'nfi_synthesis_backward_hvp': (ctypes.c_int, [ctypes.POINTER(SynthParams),
+                                                  ctypes.POINTER(SynthHvp),
+                                                  ctypes.POINTER(SynthParamGrads),
+                                                  ctypes.c_void_p]),
     'nfi_pose_to_matrix': (ctypes.c_int, [
         ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32,
         ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),

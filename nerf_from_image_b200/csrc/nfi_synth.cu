@@ -442,12 +442,40 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
   }
 }
 
+// The tangent of the ACT epilogue along ws (the path-length HVP's forward pass): with acc-dot the
+// conv of the tangent input, u-dot = gain (acc-dot d + acc d-dot), acc d = u / gain - noise - bias
+// recovered from the saved u (noise and bias do not depend on ws).
+struct TangentEpilogue {
+  const float* dcoef;  // [B,N] d
+  const float* ddot;   // [B,N] d-dot
+  const float* noise;  // [B,H,W] or nullptr
+  const float* bias;   // [N]
+  const float* u;      // [B,H,W,N] saved pre-activation
+  float gain;
+  float* u_dot;        // [B,H,W,N] out
+};
+__device__ __forceinline__ void act_store4(const TangentEpilogue& e, int img, size_t pos, int N, int n,
+                                           float4 acc, float noise) {
+  const float4 d = __ldg(reinterpret_cast<const float4*>(e.dcoef + (size_t)img * N + n));
+  const float4 dd = __ldg(reinterpret_cast<const float4*>(e.ddot + (size_t)img * N + n));
+  const float4 b = __ldg(reinterpret_cast<const float4*>(e.bias + n));
+  const float4 u = __ldg(reinterpret_cast<const float4*>(e.u + pos * N + n));
+  const float ig = 1.f / e.gain;
+  float4 o;
+  o.x = (acc.x * d.x + (u.x * ig - noise - b.x) * (dd.x / d.x)) * e.gain;
+  o.y = (acc.y * d.y + (u.y * ig - noise - b.y) * (dd.y / d.y)) * e.gain;
+  o.z = (acc.z * d.z + (u.z * ig - noise - b.z) * (dd.z / d.z)) * e.gain;
+  o.w = (acc.w * d.w + (u.w * ig - noise - b.w) * (dd.w / d.w)) * e.gain;
+  *reinterpret_cast<float4*>(e.u_dot + pos * N + n) = o;
+}
+
 // 4x4 FIR (outer([1,3,3,1]) / 16 = the reference's filter * gain 4, pad 1) over the (2H+1)x(2W+1)
-// transposed-conv result, then the ACT epilogue.  One thread per (2x2 output block, 4 channels):
-// the block needs a 5x5 window of the raw tensor (25 loads for 4 outputs instead of 16 each), rows
-// filtered first (separable), then columns.
+// transposed-conv result, then the ACT epilogue (or its tangent).  One thread per (2x2 output
+// block, 4 channels): the block needs a 5x5 window of the raw tensor (25 loads for 4 outputs
+// instead of 16 each), rows filtered first (separable), then columns.
+template <class Epilogue>
 __global__ void __launch_bounds__(256)
-fir_act_kernel(const float* __restrict__ raw, int B, int OH, int OW, int N, ActEpilogue e) {
+fir_act_kernel(const float* __restrict__ raw, int B, int OH, int OW, int N, Epilogue e) {
   const int RH = OH + 1, RW = OW + 1;
   const int groups = N >> 2, bh = OH >> 1, bw = OW >> 1;
   const size_t total = (size_t)B * bh * bw * groups;
@@ -516,7 +544,7 @@ __global__ void prep_weights_kernel(const float* __restrict__ w, int cout, int c
 }
 
 // styles[b,c] = (affine_w[c,:] . w[b,:] / sqrt(w_dim) + affine_b[c]) * gain   (stylegan.py:148-180,
-// 329,372); one warp per (b, c)
+// 329,372); one warp per (b, c).  affine_b NULL: the style's tangent along w (no bias term).
 __global__ void styles_kernel(const float* __restrict__ ws, int ws_stride, int w_dim,
                               const float* __restrict__ aw, const float* __restrict__ ab, int cin,
                               int B, float gain, float* __restrict__ out) {
@@ -529,7 +557,7 @@ __global__ void styles_kernel(const float* __restrict__ ws, int ws_stride, int w
   for (int k = lane; k < w_dim; k += 32) s = fmaf(row[k], wv[k], s);
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  if (lane == 0) out[warp] = (s * rsqrtf((float)w_dim) + ab[c]) * gain;
+  if (lane == 0) out[warp] = (s * rsqrtf((float)w_dim) + (ab ? ab[c] : 0.f)) * gain;
 }
 
 // dcoef[b,o] = rsqrt(sum_c wsq[o,c] s[b,c]^2 + 1e-8)  (stylegan.py:128); one warp per (b, o)
@@ -1074,6 +1102,248 @@ __global__ void const_grad_kernel(const float* __restrict__ dx, const float* __r
   g_const[i] += acc;
 }
 
+// ------------------------------------------------------------------ path-length HVP
+// The gradient of <t, J_ws^T n> with respect to ws and every parameter is the tangent, along
+// ws + eps t, of the backward with the planes cotangent n (symmetry of second derivatives).  Every
+// backward quantity q gets a tangent q-dot: a tangent forward pass first (s-dot, d-dot, and u-dot
+// per layer kept in fp32), then the backward walk recomputed beside its tangent; each GEMM is one
+// the backward already runs, on 2B stacked images where a product and its tangent share an operand.
+
+// d-dot[b,o] = -d^3 sum_c wsq[o,c] s s-dot (the tangent of dcoef_kernel); one warp per (b, o)
+__global__ void dcoef_tangent_kernel(const float* __restrict__ wsq, const float* __restrict__ s,
+                                     const float* __restrict__ sdot, const float* __restrict__ d, int cout,
+                                     int cin, int B, float* __restrict__ out) {
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (warp >= B * cout) return;
+  const int b = warp / cout, o = warp % cout;
+  float acc = 0.f;
+  for (int c = lane; c < cin; c += 32)
+    acc = fmaf(wsq[(size_t)o * cin + c], s[(size_t)b * cin + c] * sdot[(size_t)b * cin + c], acc);
+#pragma unroll
+  for (int k = 16; k > 0; k >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, k);
+  if (lane == 0) {
+    const float dv = d[warp];
+    out[warp] = -(dv * dv * dv) * acc;
+  }
+}
+
+// The tangent ACT pass of a stride-1 layer: acc-dot [B,HW,C] (the RAW conv of the tangent input)
+// -> u-dot, through the same epilogue as fir_act_kernel<TangentEpilogue>
+__global__ void tangent_act_kernel(const float* __restrict__ acc_dot, int B, int HW, int C, TangentEpilogue e) {
+  const int groups = C >> 2;
+  const size_t total = (size_t)B * HW * groups;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (size_t)gridDim.x * blockDim.x) {
+    const int g = (int)(i % groups);
+    const size_t pos = i / groups;
+    const float noise = e.noise ? __ldg(e.noise + pos) : 0.f;
+    act_store4(e, (int)(pos / HW), pos, C, 4 * g, __ldg(reinterpret_cast<const float4*>(acc_dot) + i), noise);
+  }
+}
+
+// x~-dot = lrelu'(u) u-dot s + lrelu(u) s-dot as a pair: the tangent of restyle_kernel
+__global__ void restyle_tangent_kernel(const float* __restrict__ u, const float* __restrict__ udot,
+                                       const float* __restrict__ s, const float* __restrict__ sdot, int B,
+                                       int HW, int C, __nv_bfloat16* __restrict__ hi,
+                                       __nv_bfloat16* __restrict__ lo) {
+  const int groups = C >> 2;
+  const size_t total = (size_t)B * HW * groups;
+  const float4 one = make_float4(1.f, 1.f, 1.f, 1.f);
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (size_t)gridDim.x * blockDim.x) {
+    const int g = (int)(i % groups);
+    const int img = (int)(i / ((size_t)HW * groups));
+    const float4 v = __ldg(reinterpret_cast<const float4*>(u) + i);
+    const float4 vd = __ldg(reinterpret_cast<const float4*>(udot) + i);
+    const float4 sv = __ldg(reinterpret_cast<const float4*>(s + (size_t)img * C) + g);
+    const float4 sd = __ldg(reinterpret_cast<const float4*>(sdot + (size_t)img * C) + g);
+    float4 x;
+    x.x = lrelu_grad(v.x) * vd.x * sv.x + lrelu(v.x) * sd.x;
+    x.y = lrelu_grad(v.y) * vd.y * sv.y + lrelu(v.y) * sd.y;
+    x.z = lrelu_grad(v.z) * vd.z * sv.z + lrelu(v.z) * sd.z;
+    x.w = lrelu_grad(v.w) * vd.w * sv.w + lrelu(v.w) * sd.w;
+    store_split4(hi, lo, i * 4, x, one);
+  }
+}
+
+struct ActBackwardTangent {
+  const float* u;       // [B,HW,C] saved pre-activation
+  const float* u_dot;   // [B,HW,C] its tangent
+  const float* noise;   // [B,HW] or nullptr
+  const float* bias;    // [C]
+  const float* dcoef;   // [B,C] d
+  const float* ddot;    // [B,C] d-dot
+  float gain;           // sqrt(2)
+  // up to two consumers of v: dx~ and its tangent (nullptr = 0), style and its tangent, and
+  // ds += sum_pos dx~ v, ds-dot += sum_pos dx~-dot v + dx~ v-dot
+  const float* dx_a; const float* dxt_a; const float* s_a; const float* st_a; float* ds_a; float* dst_a;
+  const float* dx_b; const float* dxt_b; const float* s_b; const float* st_b; float* ds_b; float* dst_b;
+  float* dd;            // [B,C] += sum_pos g (acc d)
+  float* ddt;           // [B,C] += sum_pos g-dot (acc d) + g u-dot / gain
+  // dacc = g d and dacc-dot = g-dot d + g d-dot, as pairs (stride-1 layers) or fp32 (up layers)
+  __nv_bfloat16* dacc_hi; __nv_bfloat16* dacc_lo; __nv_bfloat16* dacct_hi; __nv_bfloat16* dacct_lo;
+  float* dacc; float* dacct;
+  float* g_bias;        // [C] += sum_{b,pos} g-dot, or nullptr
+  float* g_noise;       // [B,HW] += sum_c g-dot, or nullptr
+};
+
+// act_backward_kernel<true> and its tangent in one pass (lrelu'' = 0): block (chunk, b), 4 channels
+// per thread, the seven per-channel sums reduced in shared memory, one atomic per block.
+__global__ void __launch_bounds__(256)
+act_backward_tangent_kernel(ActBackwardTangent e, int HW, int C, int chunk) {
+  __shared__ float4 red[7][256];
+  __shared__ float nsum[kActChunk];
+  for (int i = threadIdx.x; i < kActChunk; i += 256) nsum[i] = 0.f;
+  __syncthreads();
+  const int cg = C >> 2, ppar = 256 / cg, tid = threadIdx.x;
+  const int p = tid / cg, c4 = tid - p * cg;
+  const int b = blockIdx.y;
+  const bool active = p < ppar;
+  const float inv_gain = 1.f / e.gain;
+  float sum[7][4];  // ds_a, ds_b, dd, ds_a-dot, ds_b-dot, dd-dot, bias-dot
+#pragma unroll
+  for (int q = 0; q < 7; ++q)
+#pragma unroll
+    for (int k = 0; k < 4; ++k) sum[q][k] = 0.f;
+  if (active) {
+    auto ld = [](const float* ptr, size_t off, float dflt, float (&o)[4]) {
+      if (ptr == nullptr) {
+        o[0] = o[1] = o[2] = o[3] = dflt;
+        return;
+      }
+      const float4 t = __ldg(reinterpret_cast<const float4*>(ptr + off));
+      o[0] = t.x; o[1] = t.y; o[2] = t.z; o[3] = t.w;
+    };
+    const size_t bc = (size_t)b * C + 4 * c4;
+    float d[4], dd[4], bi[4], sa[4], sb[4], ta[4], tb[4];
+    ld(e.dcoef, bc, 0.f, d);
+    ld(e.ddot, bc, 0.f, dd);
+    ld(e.bias, 4 * c4, 0.f, bi);
+    ld(e.s_a, bc, 1.f, sa);
+    ld(e.s_b, bc, 1.f, sb);
+    ld(e.st_a, bc, 0.f, ta);
+    ld(e.st_b, bc, 0.f, tb);
+    const int end = min(HW, (blockIdx.x + 1) * chunk);
+    for (int pos = blockIdx.x * chunk + p; pos < end; pos += ppar) {
+      const size_t row = (size_t)b * HW + pos, idx = row * C + 4 * c4;
+      float u[4], ud[4], xa[4], xta[4], xb[4], xtb[4];
+      ld(e.u, idx, 0.f, u);
+      ld(e.u_dot, idx, 0.f, ud);
+      ld(e.dx_a, idx, 0.f, xa);
+      ld(e.dxt_a, idx, 0.f, xta);
+      ld(e.dx_b, idx, 0.f, xb);
+      ld(e.dxt_b, idx, 0.f, xtb);
+      const float nz = e.noise ? __ldg(e.noise + row) : 0.f;
+      float out[4], outt[4], gsum = 0.f;
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const float v = lrelu(u[k]), lg = lrelu_grad(u[k]), vd = lg * ud[k];
+        sum[0][k] = fmaf(xa[k], v, sum[0][k]);
+        sum[1][k] = fmaf(xb[k], v, sum[1][k]);
+        sum[3][k] += xta[k] * v + xa[k] * vd;
+        sum[4][k] += xtb[k] * v + xb[k] * vd;
+        const float dv = xa[k] * sa[k] + xb[k] * sb[k];
+        const float dvt = (xta[k] * sa[k] + xa[k] * ta[k]) + (xtb[k] * sb[k] + xb[k] * tb[k]);
+        const float g = dv * lg * e.gain, gt = dvt * lg * e.gain;
+        const float accd = u[k] * inv_gain - nz - bi[k];  // acc d = u/gain - noise - bias
+        sum[2][k] = fmaf(g, accd, sum[2][k]);
+        sum[5][k] += gt * accd + g * ud[k] * inv_gain;
+        sum[6][k] += gt;
+        gsum += gt;
+        out[k] = g * d[k];
+        outt[k] = gt * d[k] + g * dd[k];
+      }
+      const float4 o4 = make_float4(out[0], out[1], out[2], out[3]);
+      const float4 t4 = make_float4(outt[0], outt[1], outt[2], outt[3]);
+      const float4 one = make_float4(1.f, 1.f, 1.f, 1.f);
+      if (e.dacc_hi != nullptr) {
+        store_split4(e.dacc_hi, e.dacc_lo, idx, o4, one);
+        store_split4(e.dacct_hi, e.dacct_lo, idx, t4, one);
+      }
+      if (e.dacc != nullptr) {
+        *reinterpret_cast<float4*>(e.dacc + idx) = o4;
+        *reinterpret_cast<float4*>(e.dacct + idx) = t4;
+      }
+      if (e.g_noise != nullptr) atomicAdd(&nsum[pos - blockIdx.x * chunk], gsum);
+    }
+  }
+#pragma unroll
+  for (int q = 0; q < 7; ++q) red[q][tid] = make_float4(sum[q][0], sum[q][1], sum[q][2], sum[q][3]);
+  __syncthreads();
+  if (e.g_noise != nullptr) {
+    const int p0 = blockIdx.x * chunk, n = min(HW, p0 + chunk) - p0;
+    for (int i = tid; i < n; i += 256) e.g_noise[(size_t)b * HW + p0 + i] += nsum[i];
+  }
+  if (tid < cg) {
+    float* dst[7] = {e.ds_a, e.ds_b, e.dd, e.dst_a, e.dst_b, e.ddt, e.g_bias};
+#pragma unroll
+    for (int q = 0; q < 7; ++q) {
+      if (dst[q] == nullptr) continue;
+      float4 s = red[q][tid];
+      for (int k = 1; k < ppar; ++k) {
+        const float4 t = red[q][k * cg + tid];
+        s.x += t.x; s.y += t.y; s.z += t.z; s.w += t.w;
+      }
+      float* o = dst[q] + (q == 6 ? 0 : (size_t)b * C) + 4 * tid;
+      atomicAdd(o + 0, s.x);
+      atomicAdd(o + 1, s.y);
+      atomicAdd(o + 2, s.z);
+      atomicAdd(o + 3, s.w);
+    }
+  }
+}
+
+// dcoef_backward_kernel and its tangent: with P = sum_o dd d^2 wsq[o,i] and
+// Q = sum_o (dd-dot d^2 + 2 dd d d-dot) wsq[o,i]:  ds -= s P,  ds-dot -= s-dot P + s Q
+__global__ void dcoef_backward_tangent_kernel(const float* __restrict__ wsq, const float* __restrict__ s,
+                                              const float* __restrict__ sdot, const float* __restrict__ dd,
+                                              const float* __restrict__ ddt, const float* __restrict__ d,
+                                              const float* __restrict__ ddot, int cout, int cin, int B,
+                                              float* __restrict__ ds, float* __restrict__ dst) {
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (warp >= B * cin) return;
+  const int b = warp / cin, i = warp % cin;
+  float pa = 0.f, qa = 0.f;
+  for (int o = lane; o < cout; o += 32) {
+    const size_t bo = (size_t)b * cout + o;
+    const float dv = d[bo], w = wsq[(size_t)o * cin + i];
+    pa = fmaf(dd[bo] * dv * dv, w, pa);
+    qa = fmaf(ddt[bo] * dv * dv + 2.f * dd[bo] * dv * ddot[bo], w, qa);
+  }
+#pragma unroll
+  for (int k = 16; k > 0; k >>= 1) {
+    pa += __shfl_xor_sync(0xffffffffu, pa, k);
+    qa += __shfl_xor_sync(0xffffffffu, qa, k);
+  }
+  if (lane == 0) {
+    ds[warp] -= s[warp] * pa;
+    dst[warp] -= sdot[warp] * pa + s[warp] * qa;
+  }
+}
+
+// wgrad_reduce_kernel with the tangent of the demodulation term: g_w += sum_split part - W sum_b
+// [dd-dot d^2 s^2 + 2 dd d d-dot s^2 + 2 dd d^2 s s-dot]; one thread per (co, ci)
+__global__ void wgrad_reduce_tangent_kernel(const float* __restrict__ part, int n_split, int taps, int cout,
+                                            int cin, const float* __restrict__ w, const float* __restrict__ dd,
+                                            const float* __restrict__ ddt, const float* __restrict__ d,
+                                            const float* __restrict__ ddot, const float* __restrict__ s,
+                                            const float* __restrict__ sdot, int B, float* __restrict__ g_w) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x, n = (size_t)cout * cin;
+  if (i >= n) return;
+  const int o = (int)(i / cin), c = (int)(i % cin);
+  float dem = 0.f;
+  for (int b = 0; b < B; ++b) {
+    const size_t bo = (size_t)b * cout + o, bc = (size_t)b * cin + c;
+    const float dv = d[bo], sv = s[bc];
+    dem += (ddt[bo] * dv * dv + 2.f * dd[bo] * dv * ddot[bo]) * sv * sv + 2.f * dd[bo] * dv * dv * sv * sdot[bc];
+  }
+  for (int tp = 0; tp < taps; ++tp) {
+    float acc = 0.f;
+    for (int sp = 0; sp < n_split; ++sp) acc += part[((size_t)sp * taps + tp) * n + i];
+    g_w[i * taps + tp] += acc - w[i * taps + tp] * dem;
+  }
+}
+
 // ------------------------------------------------------------------ host side
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
                                   const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
@@ -1323,6 +1593,7 @@ struct Saved {
   float* wsq1[NFI_SYNTH_MAX_BLOCKS];
   float* u0[NFI_SYNTH_MAX_BLOCKS];  // pre-activations [B,res,res,cout] (save mode)
   float* u1[NFI_SYNTH_MAX_BLOCKS];
+  Pair w0[NFI_SYNTH_MAX_BLOCKS], w1[NFI_SYNTH_MAX_BLOCKS];  // [tap][Cout][Cin] pairs of the forward
   int row0[NFI_SYNTH_MAX_BLOCKS], row1[NFI_SYNTH_MAX_BLOCKS], row_rgb[NFI_SYNTH_MAX_BLOCKS];
 };
 
@@ -1384,6 +1655,8 @@ static int run(const nfi_synth_params& P, Bump& ws, cudaStream_t st, bool dry, c
     for (int i = 0; i < nb; ++i) {
       sv->style0[i] = style0[i]; sv->style1[i] = style1[i]; sv->style_rgb[i] = style_rgb[i];
       sv->dco0[i] = dco0[i]; sv->dco1[i] = dco1[i];
+      if (i) sv->w0[i] = w0[i];
+      sv->w1[i] = w1[i];
       const size_t n = (size_t)B * (4 << i) * (4 << i) * P.channels[i];
       sv->u0[i] = i ? ws.take(n) : nullptr;
       sv->u1[i] = ws.take(n);
@@ -1891,6 +2164,425 @@ int backward_params(const nfi_synth_params& P, const nfi_synth_grads& G, const n
   memset(&sv, 0, sizeof(sv));
   if (const int rc = saved_layout(P, b, sv, err, err_len)) return rc;
   return run_backward(P, G, sv, b, st, false, err, err_len, &PG);
+}
+
+
+// ---- path-length HVP (nfi_synthesis_backward_hvp) ----
+// Scratch of its own (the saved workspace is only read).  The tangent forward keeps s-dot, d-dot
+// and u-dot of every layer; the walk then runs run_backward's launches on 2B stacked images where
+// a quantity and its tangent meet the same operand: the data-gradient GEMMs on [dacc; dacc-dot]
+// against W^T, the weight GEMMs on [dacc; dacc-dot] against [x~-dot; x~] (one sum over 2B images
+// is the product rule's two terms).  Buffers as in run_backward, with room for 2B images.
+static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Saved& sv, Bump& ws,
+                   cudaStream_t st, bool dry, char* err, size_t err_len, const nfi_synth_param_grads* PG) {
+  const int B = P.batch, B2 = 2 * B, nb = P.num_blocks, D = P.w_dim, R = P.img_resolution,
+            NI = P.img_channels;
+  const float sqrt2 = 1.4142135623730951f;
+  auto blocks = [](size_t n, int per) { return (unsigned)((n + per - 1) / per); };
+  auto flat_grid = [&](size_t n) {
+    unsigned g = blocks(n, 256);
+    return g > (unsigned)sm_count() * 16u ? (unsigned)sm_count() * 16u : g;
+  };
+  int cmax = 0;
+  for (int i = 0; i < nb; ++i) cmax = P.channels[i] > cmax ? P.channels[i] : cmax;
+  const size_t full = (size_t)B * R * R * cmax;
+  const size_t phases = (size_t)8 * B * (R / 2 + 1) * (R / 2 + 1) * cmax;
+  float* bufA = ws.take(2 * full > phases ? 2 * full : phases);  // also the tangent conv's raw output
+  float* bufB = ws.take(2 * full);
+  float* bufC = ws.take((size_t)B2 * (R / 2) * (R / 2) * cmax);
+  float* dimg[2] = {ws.take((size_t)B * R * R * NI), ws.take((size_t)B * R * R * NI)};
+  Pair dimg_p = ws.pair((size_t)B * R * R * NI);
+  Pair xt = ws.pair(2 * full);  // [x~-dot; x~]: the tangent conv's input, the weight GEMMs' X
+  float *ud0[NFI_SYNTH_MAX_BLOCKS] = {nullptr}, *ud1[NFI_SYNTH_MAX_BLOCKS];
+  for (int i = 0; i < nb; ++i) {
+    const size_t n = (size_t)B * (4 << i) * (4 << i) * P.channels[i];
+    if (i) ud0[i] = ws.take(n);
+    ud1[i] = ws.take(n);
+  }
+  // per-(b, channel) sums and their tangents (zeroed once), style and dcoef tangents
+  float *ds0[2][NFI_SYNTH_MAX_BLOCKS], *ds1[2][NFI_SYNTH_MAX_BLOCKS], *dsr[2][NFI_SYNTH_MAX_BLOCKS];
+  float *dd0[2][NFI_SYNTH_MAX_BLOCKS], *dd1[2][NFI_SYNTH_MAX_BLOCKS];
+  float *sd0[NFI_SYNTH_MAX_BLOCKS], *sd1[NFI_SYNTH_MAX_BLOCKS], *sdr[NFI_SYNTH_MAX_BLOCKS];
+  float *ddot0[NFI_SYNTH_MAX_BLOCKS], *ddot1[NFI_SYNTH_MAX_BLOCKS];
+  size_t small = 0;
+  for (int i = 0; i < nb; ++i) small += (size_t)B * (4 * P.channels[i] + (i ? P.channels[i - 1] : 0));
+  float* sums = ws.take(2 * small);
+  {
+    float* q = sums;
+    for (int k = 0; k < 2; ++k)
+      for (int i = 0; i < nb; ++i) {
+        const int c = P.channels[i], ci = i ? P.channels[i - 1] : 0;
+        ds0[k][i] = q; q += (size_t)B * ci;
+        ds1[k][i] = q; q += (size_t)B * c;
+        dsr[k][i] = q; q += (size_t)B * c;
+        dd0[k][i] = q; q += (size_t)B * c;
+        dd1[k][i] = q; q += (size_t)B * c;
+      }
+  }
+  for (int i = 0; i < nb; ++i) {
+    const int c = P.channels[i], ci = i ? P.channels[i - 1] : 0;
+    sd0[i] = i ? ws.take((size_t)B * ci) : nullptr;
+    ddot0[i] = i ? ws.take((size_t)B * c) : nullptr;
+    sd1[i] = ws.take((size_t)B * c);
+    ddot1[i] = ws.take((size_t)B * c);
+    sdr[i] = ws.take((size_t)B * c);
+  }
+  Pair wt0[NFI_SYNTH_MAX_BLOCKS], wt1[NFI_SYNTH_MAX_BLOCKS], wtr[NFI_SYNTH_MAX_BLOCKS];
+  for (int i = 0; i < nb; ++i) {
+    const int c = P.channels[i], ci = i ? P.channels[i - 1] : 0;
+    if (i) wt0[i] = ws.pair((size_t)9 * c * ci);
+    wt1[i] = ws.pair((size_t)9 * c * c);
+    wtr[i] = ws.pair((size_t)NI * c);
+  }
+  auto wgrad_args = [](int cout, int cin, int taps) {
+    WgradArgs a;
+    memset(&a, 0, sizeof(a));
+    a.cout = cout; a.cin = cin; a.taps = taps;
+    return a;
+  };
+  float* part = nullptr;
+  if (PG) {
+    size_t pmax = 0;
+    auto need = [&](int cout, int cin, int taps, int D_, int nimg) {
+      WgradArgs a = wgrad_args(cout, cin, taps);
+      plan_wgrad(a, nimg, D_, D_);
+      const size_t n = (size_t)a.n_split * taps * cout * cin;
+      pmax = n > pmax ? n : pmax;
+    };
+    for (int i = 0; i < nb; ++i) {
+      const int res = 4 << i, c = P.channels[i];
+      need(NI, c, 1, res, B);
+      need(c, c, 9, res, B2);
+      if (i) need(c, P.channels[i - 1], 9, res / 2, B2);
+    }
+    part = ws.take(pmax);
+  }
+  if (dry) return 0;
+
+  NFI_SCUDA(cudaMemsetAsync(sums, 0, 2 * small * sizeof(float), st));
+  // ---- tangent forward ----
+  auto style_dot = [&](const nfi_synth_layer& L, int c, int row, float gain, float* out) {
+    styles_kernel<<<blocks((size_t)B * c * 32, 256), 256, 0, st>>>(H.t_ws + (size_t)row * D, P.num_ws * D, D,
+                                                                   L.affine_w, nullptr, c, B, gain, out);
+  };
+  auto restyle_dot = [&](const float* u, const float* ud, const float* s, const float* sdot, int HW, int C,
+                         Pair dst) {
+    restyle_tangent_kernel<<<flat_grid((size_t)B * HW * C / 4), 256, 0, st>>>(u, ud, s, sdot, B, HW, C, dst.hi,
+                                                                             dst.lo);
+  };
+  auto tangent_epi = [&](const nfi_synth_layer& L, const float* d, const float* ddot, const float* u,
+                         float* udot) {
+    TangentEpilogue e;
+    e.dcoef = d; e.ddot = ddot; e.noise = L.noise; e.bias = L.bias; e.u = u; e.gain = sqrt2; e.u_dot = udot;
+    return e;
+  };
+  for (int i = 0; i < nb; ++i) {
+    const int res = 4 << i, c = P.channels[i], ci = i ? P.channels[i - 1] : 0, HW = res * res;
+    if (i) {
+      style_dot(P.conv0[i], ci, sv.row0[i], 1.f, sd0[i]);
+      dcoef_tangent_kernel<<<blocks((size_t)B * c * 32, 256), 256, 0, st>>>(sv.wsq0[i], sv.style0[i], sd0[i],
+                                                                           sv.dco0[i], c, ci, B, ddot0[i]);
+    }
+    style_dot(P.conv1[i], c, sv.row1[i], 1.f, sd1[i]);
+    dcoef_tangent_kernel<<<blocks((size_t)B * c * 32, 256), 256, 0, st>>>(sv.wsq1[i], sv.style1[i], sd1[i],
+                                                                         sv.dco1[i], c, c, B, ddot1[i]);
+    style_dot(P.torgb[i], c, sv.row_rgb[i], 1.f / sqrtf((float)c), sdr[i]);
+    if (i) {  // conv0: x~-dot on the low-resolution grid, the four phase GEMMs, FIR + tangent epilogue
+      const int h = res / 2;
+      restyle_dot(sv.u1[i - 1], ud1[i - 1], sv.style0[i], sd0[i], h * h, ci, xt);
+      ConvArgs a;
+      memset(&a, 0, sizeof(a));
+      a.B = B; a.C = ci; a.N = c; a.H = h; a.W = h;
+      conv_up_phases(a, h, h);
+      a.mode = kModeRaw;
+      a.out_raw = bufA; a.out_H = res + 1; a.out_W = res + 1; a.out_stride = 2;
+      if (const int rc = launch_conv(a, xt, sv.w0[i], 9, st, err, err_len)) return rc;
+      const size_t total = (size_t)B * h * h * (c / 4);
+      fir_act_kernel<<<flat_grid(total), 256, 0, st>>>(bufA, B, res, res, c,
+                                                       tangent_epi(P.conv0[i], sv.dco0[i], ddot0[i], sv.u0[i], ud0[i]));
+      NFI_SCUDA(cudaGetLastError());
+      restyle_dot(sv.u0[i], ud0[i], sv.style1[i], sd1[i], HW, c, xt);
+    } else {  // b4.const does not depend on ws: x~-dot = const s-dot
+      const_input_kernel<<<blocks((size_t)B * 16 * c, 256), 256, 0, st>>>(P.const_input, sd1[0], B, c, xt.hi,
+                                                                         xt.lo);
+    }
+    ConvArgs a;
+    memset(&a, 0, sizeof(a));
+    a.B = B; a.C = c; a.N = c; a.H = res; a.W = res;
+    conv3x3_phases(a, res, res);
+    a.mode = kModeRaw;
+    a.out_raw = bufA; a.out_H = res; a.out_W = res; a.out_stride = 1;
+    if (const int rc = launch_conv(a, xt, sv.w1[i], 9, st, err, err_len)) return rc;
+    tangent_act_kernel<<<flat_grid((size_t)B * HW * c / 4), 256, 0, st>>>(
+        bufA, B, HW, c, tangent_epi(P.conv1[i], sv.dco1[i], ddot1[i], sv.u1[i], ud1[i]));
+    NFI_SCUDA(cudaGetLastError());
+  }
+
+  // ---- the backward and its tangent, last block first ----
+  for (int i = 0; i < nb; ++i) {
+    const int c = P.channels[i], ci = i ? P.channels[i - 1] : 0;
+    if (i)
+      prep_weights_t_kernel<<<blocks((size_t)c * ci, 256), 256, 0, st>>>(P.conv0[i].weight, c, ci, 9,
+                                                                         wt0[i].hi, wt0[i].lo);
+    prep_weights_t_kernel<<<blocks((size_t)c * c, 256), 256, 0, st>>>(P.conv1[i].weight, c, c, 9,
+                                                                       wt1[i].hi, wt1[i].lo);
+    prep_weights_t_kernel<<<blocks((size_t)NI * c, 256), 256, 0, st>>>(P.torgb[i].weight, NI, c, 1,
+                                                                       wtr[i].hi, wtr[i].lo);
+  }
+  planes_grad_kernel<<<flat_grid((size_t)B * R * R * NI), 256, 0, st>>>(H.g_planes, B, R, dimg[0],
+                                                                        dimg_p.hi, dimg_p.lo);
+  NFI_SCUDA(cudaGetLastError());
+
+  auto act_backward = [&](ActBackwardTangent& e, int HW, int C) -> int {
+    if (C % 4 != 0 || C / 4 > 256) {
+      snprintf(err, err_len, "synthesis HVP: %d channels unsupported", C);
+      return 1;
+    }
+    dim3 grid((unsigned)((HW + kActChunk - 1) / kActChunk), (unsigned)B);
+    act_backward_tangent_kernel<<<grid, 256, 0, st>>>(e, HW, C, kActChunk);
+    NFI_SCUDA(cudaGetLastError());
+    return 0;
+  };
+  // the ws gradient is the tangent's (the style gradient's tangent through styles_kernel's
+  // transpose); the affine weight's is (ds-dot)^T w + ds^T t, the affine bias's sum_b ds-dot
+  auto outputs = [&](const float* ds, const float* dst, const nfi_synth_layer& L, int cin, int row,
+                     float gain, const nfi_synth_layer_grads* LG) {
+    styles_backward_kernel<<<blocks((size_t)B * D, 256), 256, 0, st>>>(
+        dst, L.affine_w, cin, D, B, gain / sqrtf((float)D), H.g_ws + (size_t)row * D, P.num_ws * D);
+    if (LG == nullptr || (LG->g_affine_w == nullptr && LG->g_affine_b == nullptr)) return;
+    const float scale = gain / sqrtf((float)D);
+    affine_backward_kernel<<<blocks((size_t)cin * D, 256), 256, 0, st>>>(
+        dst, P.ws + (size_t)row * D, P.num_ws * D, B, cin, D, scale, gain, LG->g_affine_w, LG->g_affine_b);
+    if (LG->g_affine_w != nullptr)
+      affine_backward_kernel<<<blocks((size_t)cin * D, 256), 256, 0, st>>>(
+          ds, H.t_ws + (size_t)row * D, P.num_ws * D, B, cin, D, scale, gain, LG->g_affine_w, nullptr);
+  };
+  auto demod = [&](const float* wsq, const float* s, const float* sdot, float* const* dd, const float* d,
+                   const float* ddot, int cout, int cin, float* ds, float* dst) {
+    dcoef_backward_tangent_kernel<<<blocks((size_t)B * cin * 32, 256), 256, 0, st>>>(
+        wsq, s, sdot, dd[0], dd[1], d, ddot, cout, cin, B, ds, dst);
+  };
+  // a weight GEMM over nimg images (G pair [gB,gH,gH,cout], X = xt [nimg,D_,D_,cin]), then the
+  // fixed-order sum; with dd set, the tangent of the demodulation term
+  auto wgrad = [&](WgradArgs& a, Pair g, int gB, int gH, int D_, int nimg, const float* w, float* const* dd,
+                   const float* d, const float* ddot, const float* s, const float* sdot, float* g_w) -> int {
+    plan_wgrad(a, nimg, D_, D_);
+    a.part = part;
+    if (const int rc = launch_wgrad(a, g, gB, gH, gH, xt, nimg, D_, D_, st, err, err_len)) return rc;
+    if (dd == nullptr)
+      wgrad_reduce_kernel<<<blocks((size_t)a.cout * a.cin, 256), 256, 0, st>>>(
+          part, a.n_split, a.taps, a.cout, a.cin, w, nullptr, nullptr, nullptr, B, g_w);
+    else
+      wgrad_reduce_tangent_kernel<<<blocks((size_t)a.cout * a.cin, 256), 256, 0, st>>>(
+          part, a.n_split, a.taps, a.cout, a.cin, w, dd[0], dd[1], d, ddot, s, sdot, B, g_w);
+    NFI_SCUDA(cudaGetLastError());
+    return 0;
+  };
+
+  int cur = 0;
+  for (int i = nb - 1; i >= 0; --i) {
+    const int res = 4 << i, c = P.channels[i], ci = i ? P.channels[i - 1] : 0, HW = res * res;
+    const bool last = (i == nb - 1);
+    const size_t n1 = (size_t)B * HW * c;  // one half of a stacked full-resolution tensor
+    {  // ToRGB: dx~ = dimg Wrgb^T -> bufA (its tangent is 0: dimg does not depend on ws)
+      ConvArgs a;
+      memset(&a, 0, sizeof(a));
+      a.B = B; a.C = NI; a.N = c; a.H = res; a.W = res;
+      a.n_phases = 1; a.ph_taps[0] = 1; a.ph_DH[0] = res; a.ph_DW[0] = res;
+      a.mode = kModeRaw;
+      a.out_raw = bufA; a.out_H = res; a.out_W = res; a.out_stride = 1;
+      if (const int rc = launch_conv(a, dimg_p, wtr[i], 1, st, err, err_len)) return rc;
+    }
+    if (PG && PG->torgb[i].g_weight != nullptr) {  // dimg against x~-dot of ToRGB
+      restyle_dot(sv.u1[i], ud1[i], sv.style_rgb[i], sdr[i], HW, c, xt);
+      WgradArgs a = wgrad_args(NI, c, 1);
+      if (int rc = wgrad(a, dimg_p, B, res, res, B, P.torgb[i].weight, nullptr, nullptr, nullptr, nullptr,
+                         nullptr, PG->torgb[i].g_weight))
+        return rc;
+    }
+    if (i) {
+      const int h = res / 2;
+      upsample_adjoint_kernel<<<flat_grid((size_t)B * h * h * NI), 256, 0, st>>>(
+          dimg[cur], B, h, h, NI, dimg[cur ^ 1], dimg_p.hi, dimg_p.lo);
+      NFI_SCUDA(cudaGetLastError());
+      cur ^= 1;
+    }
+    // conv1: consumers ToRGB and conv0 of block i+1 ([dx~; dx~-dot] in bufC) -> [dacc; dacc-dot]
+    Pair pb = {reinterpret_cast<__nv_bfloat16*>(bufB), reinterpret_cast<__nv_bfloat16*>(bufB) + 2 * n1};
+    {
+      ActBackwardTangent e;
+      memset(&e, 0, sizeof(e));
+      e.u = sv.u1[i]; e.u_dot = ud1[i]; e.noise = P.conv1[i].noise; e.bias = P.conv1[i].bias;
+      e.dcoef = sv.dco1[i]; e.ddot = ddot1[i]; e.gain = sqrt2;
+      e.dx_a = bufA; e.s_a = sv.style_rgb[i]; e.st_a = sdr[i]; e.ds_a = dsr[0][i]; e.dst_a = dsr[1][i];
+      if (!last) {
+        e.dx_b = bufC; e.dxt_b = bufC + (size_t)B * HW * c;
+        e.s_b = sv.style0[i + 1]; e.st_b = sd0[i + 1]; e.ds_b = ds0[0][i + 1]; e.dst_b = ds0[1][i + 1];
+      }
+      e.dd = dd1[0][i]; e.ddt = dd1[1][i];
+      e.dacc_hi = pb.hi; e.dacc_lo = pb.lo; e.dacct_hi = pb.hi + n1; e.dacct_lo = pb.lo + n1;
+      if (PG) {
+        e.g_bias = PG->conv1[i].g_bias;
+        e.g_noise = P.conv1[i].noise ? PG->conv1[i].g_noise : nullptr;
+      }
+      if (int rc = act_backward(e, HW, c)) return rc;
+    }
+    outputs(dsr[0][i], dsr[1][i], P.torgb[i], c, sv.row_rgb[i], 1.f / sqrtf((float)c), PG ? &PG->torgb[i] : nullptr);
+    if (!last) {
+      const int cn = P.channels[i + 1];
+      float* dd[2] = {dd0[0][i + 1], dd0[1][i + 1]};
+      demod(sv.wsq0[i + 1], sv.style0[i + 1], sd0[i + 1], dd, sv.dco0[i + 1], ddot0[i + 1], cn, c,
+            ds0[0][i + 1], ds0[1][i + 1]);
+      outputs(ds0[0][i + 1], ds0[1][i + 1], P.conv0[i + 1], c, sv.row0[i + 1], 1.f,
+              PG ? &PG->conv0[i + 1] : nullptr);
+    }
+    {  // [dx~; dx~-dot] of conv1 = conv^T([dacc; dacc-dot], W1) -> bufA
+      ConvArgs a;
+      memset(&a, 0, sizeof(a));
+      a.B = B2; a.C = c; a.N = c; a.H = res; a.W = res;
+      conv3x3_phases(a, res, res);
+      for (int t = 0; t < 9; ++t) {
+        a.tap_dy[t] = -a.tap_dy[t];
+        a.tap_dx[t] = -a.tap_dx[t];
+      }
+      a.mode = kModeRaw;
+      a.out_raw = bufA; a.out_H = res; a.out_W = res; a.out_stride = 1;
+      if (const int rc = launch_conv(a, pb, wt1[i], 9, st, err, err_len)) return rc;
+    }
+    if (PG && PG->conv1[i].g_weight != nullptr) {  // [dacc; dacc-dot] against [x~-dot; x~]
+      if (i) {
+        restyle_dot(sv.u0[i], ud0[i], sv.style1[i], sd1[i], HW, c, xt);
+        restyle_kernel<<<flat_grid(n1 / 4), 256, 0, st>>>(sv.u0[i], sv.style1[i], B, HW, c, xt.hi + n1, xt.lo + n1);
+      } else {
+        const_input_kernel<<<blocks(n1, 256), 256, 0, st>>>(P.const_input, sd1[0], B, c, xt.hi, xt.lo);
+        const_input_kernel<<<blocks(n1, 256), 256, 0, st>>>(P.const_input, sv.style1[0], B, c, xt.hi + n1,
+                                                            xt.lo + n1);
+      }
+      WgradArgs w = wgrad_args(c, c, 9);
+      for (int t = 0; t < 9; ++t) {
+        w.x_dy[t] = t / 3 - 1;
+        w.x_dx[t] = t % 3 - 1;
+      }
+      float* dd[2] = {dd1[0][i], dd1[1][i]};
+      if (int rc = wgrad(w, pb, B2, res, res, B2, P.conv1[i].weight, dd, sv.dco1[i], ddot1[i], sv.style1[i],
+                         sd1[i], PG->conv1[i].g_weight))
+        return rc;
+    }
+    if (i == 0) {  // b4.const: x~ = const s
+      const float* dxt = bufA + n1;
+      const_ds_kernel<<<blocks((size_t)B * c, 256), 256, 0, st>>>(bufA, P.const_input, B, c, ds1[0][0]);
+      const_ds_kernel<<<blocks((size_t)B * c, 256), 256, 0, st>>>(dxt, P.const_input, B, c, ds1[1][0]);
+      if (PG && PG->g_const != nullptr) {  // sum_b dx~-dot s + dx~ s-dot
+        const_grad_kernel<<<blocks((size_t)c * 16, 256), 256, 0, st>>>(dxt, sv.style1[0], B, c, PG->g_const);
+        const_grad_kernel<<<blocks((size_t)c * 16, 256), 256, 0, st>>>(bufA, sd1[0], B, c, PG->g_const);
+      }
+      float* dd[2] = {dd1[0][0], dd1[1][0]};
+      demod(sv.wsq1[0], sv.style1[0], sd1[0], dd, sv.dco1[0], ddot1[0], c, c, ds1[0][0], ds1[1][0]);
+      outputs(ds1[0][0], ds1[1][0], P.conv1[0], c, sv.row1[0], 1.f, PG ? &PG->conv1[0] : nullptr);
+      NFI_SCUDA(cudaGetLastError());
+      break;
+    }
+    {  // conv0 (up): one consumer, conv1 -> [dacc; dacc-dot] fp32 in bufB
+      ActBackwardTangent e;
+      memset(&e, 0, sizeof(e));
+      e.u = sv.u0[i]; e.u_dot = ud0[i]; e.noise = P.conv0[i].noise; e.bias = P.conv0[i].bias;
+      e.dcoef = sv.dco0[i]; e.ddot = ddot0[i]; e.gain = sqrt2;
+      e.dx_a = bufA; e.dxt_a = bufA + n1;
+      e.s_a = sv.style1[i]; e.st_a = sd1[i]; e.ds_a = ds1[0][i]; e.dst_a = ds1[1][i];
+      e.dd = dd0[0][i]; e.ddt = dd0[1][i];
+      e.dacc = bufB; e.dacct = bufB + n1;
+      if (PG) {
+        e.g_bias = PG->conv0[i].g_bias;
+        e.g_noise = P.conv0[i].noise ? PG->conv0[i].g_noise : nullptr;
+      }
+      if (int rc = act_backward(e, HW, c)) return rc;
+      float* dd[2] = {dd1[0][i], dd1[1][i]};
+      demod(sv.wsq1[i], sv.style1[i], sd1[i], dd, sv.dco1[i], ddot1[i], c, c, ds1[0][i], ds1[1][i]);
+      outputs(ds1[0][i], ds1[1][i], P.conv1[i], c, sv.row1[i], 1.f, PG ? &PG->conv1[i] : nullptr);
+    }
+    {  // FIR adjoint over 2B images -> phases (pair in bufA), weight GEMM, then [dx~; dx~-dot] in bufC
+      const int h = res / 2;
+      const size_t nph = (size_t)4 * B2 * (h + 1) * (h + 1) * c;
+      Pair ph = {reinterpret_cast<__nv_bfloat16*>(bufA), reinterpret_cast<__nv_bfloat16*>(bufA) + nph};
+      fir_adjoint_kernel<<<flat_grid(nph / 4), 256, 0, st>>>(bufB, B2, res, res, c, ph.hi, ph.lo);
+      NFI_SCUDA(cudaGetLastError());
+      if (PG && PG->conv0[i].g_weight != nullptr) {
+        const size_t nl = (size_t)B * h * h * ci;
+        restyle_dot(sv.u1[i - 1], ud1[i - 1], sv.style0[i], sd0[i], h * h, ci, xt);
+        restyle_kernel<<<flat_grid(nl / 4), 256, 0, st>>>(sv.u1[i - 1], sv.style0[i], B, h * h, ci, xt.hi + nl,
+                                                          xt.lo + nl);
+        WgradArgs w = wgrad_args(c, ci, 9);
+        for (int ky = 0; ky < 3; ++ky)
+          for (int kx = 0; kx < 3; ++kx) {
+            const int t = ky * 3 + kx;
+            w.a_dy[t] = ky / 2;
+            w.a_dx[t] = kx / 2;
+            w.a_img[t] = ((ky & 1) * 2 + (kx & 1)) * B2;
+          }
+        float* dd[2] = {dd0[0][i], dd0[1][i]};
+        if (int rc = wgrad(w, ph, 4 * B2, h + 1, h, B2, P.conv0[i].weight, dd, sv.dco0[i], ddot0[i],
+                           sv.style0[i], sd0[i], PG->conv0[i].g_weight))
+          return rc;
+      }
+      ConvArgs a;
+      memset(&a, 0, sizeof(a));
+      a.B = B2; a.C = c; a.N = ci; a.H = h + 1; a.W = h + 1;
+      a.n_phases = 1; a.ph_taps[0] = 9; a.ph_DH[0] = h; a.ph_DW[0] = h;
+      for (int ky = 0; ky < 3; ++ky)
+        for (int kx = 0; kx < 3; ++kx) {
+          const int t = ky * 3 + kx;
+          a.tap_dy[t] = ky / 2;
+          a.tap_dx[t] = kx / 2;
+          a.tap_w[t] = t;
+          a.tap_img[t] = ((ky & 1) * 2 + (kx & 1)) * B2;
+        }
+      a.mode = kModeRaw;
+      a.out_raw = bufC; a.out_H = h; a.out_W = h; a.out_stride = 1;
+      if (const int rc = launch_conv(a, ph, wt0[i], 9, st, err, err_len, 4 * B2)) return rc;
+    }
+  }
+  NFI_SCUDA(cudaGetLastError());
+  return 0;
+}
+
+size_t hvp_scratch_bytes(const nfi_synth_params& P) {
+  char err[256];
+  if (check_params(P, err, sizeof(err))) return 0;
+  Bump b{nullptr, 0, 0};
+  Saved sv;
+  memset(&sv, 0, sizeof(sv));
+  saved_layout(P, b, sv, err, sizeof(err));
+  Bump h{nullptr, 0, 0};
+  nfi_synth_hvp hv;
+  memset(&hv, 0, sizeof(hv));
+  nfi_synth_param_grads pg;
+  memset(&pg, 0, sizeof(pg));
+  run_hvp(P, hv, sv, h, nullptr, true, err, sizeof(err), &pg);
+  return h.off + 1024;
+}
+
+int backward_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const nfi_synth_param_grads* PG,
+                 cudaStream_t st, char* err, size_t err_len) {
+  if (const int rc = check_saved(P, err, err_len)) return rc;
+  if (H.g_planes == nullptr || H.t_ws == nullptr || H.g_ws == nullptr || H.scratch == nullptr) {
+    snprintf(err, err_len, "synthesis HVP: g_planes, t_ws, g_ws and scratch must be set");
+    return 1;
+  }
+  const size_t need = hvp_scratch_bytes(P);
+  if (H.scratch_bytes < need) {
+    snprintf(err, err_len, "synthesis HVP: scratch too small (%zu < %zu bytes)", H.scratch_bytes, need);
+    return 1;
+  }
+  unsigned char* base = reinterpret_cast<unsigned char*>(
+      (reinterpret_cast<uintptr_t>(P.workspace) + 1023) & ~(uintptr_t)1023);
+  Bump b{base, 0, P.workspace_bytes};
+  Saved sv;
+  memset(&sv, 0, sizeof(sv));
+  if (const int rc = saved_layout(P, b, sv, err, err_len)) return rc;
+  unsigned char* sbase = reinterpret_cast<unsigned char*>(
+      (reinterpret_cast<uintptr_t>(H.scratch) + 1023) & ~(uintptr_t)1023);
+  Bump s{sbase, 0, H.scratch_bytes};
+  return run_hvp(P, H, sv, s, st, false, err, err_len, PG);
 }
 
 }  // namespace synth

@@ -17,5 +17,8 @@ int backward(const nfi_synth_params& p, const nfi_synth_grads& g, cudaStream_t s
 size_t param_workspace_bytes(const nfi_synth_params& p);
 int backward_params(const nfi_synth_params& p, const nfi_synth_grads& g,
                     const nfi_synth_param_grads& pg, cudaStream_t st, char* err, size_t err_len);
+size_t hvp_scratch_bytes(const nfi_synth_params& p);
+int backward_hvp(const nfi_synth_params& p, const nfi_synth_hvp& h, const nfi_synth_param_grads* pg,
+                 cudaStream_t st, char* err, size_t err_len);
 }  // namespace synth
 }  // namespace nfi

@@ -175,6 +175,17 @@ class HeadsGeneratorFront:
         planes = self.g.synthesis_network(w_synthesis, **block_kwargs)
         return planes.view(batch, 3, 32, planes.shape[-2], planes.shape[-1])
 
+    def _path_length(self, ws, planes, attention_values):
+        """generator.py:484-499: autograd through the reference module, create_graph."""
+        import math
+        g = self.g
+        pl_noise = torch.randn_like(planes) / math.sqrt(planes.shape[-2] * planes.shape[-1])
+        target = (planes * pl_noise).sum()
+        if g.attention_values > 0:
+            target = target + (attention_values * torch.randn_like(attention_values)).sum()
+        pl_grad, = torch.autograd.grad(target, inputs=ws, create_graph=True)
+        return pl_grad.square().sum(dim=-1).mean(dim=-1).sqrt()
+
     @staticmethod
     def supports(request_model_outputs, model_inputs):
         return (any(o in HEAD_OUTPUTS for o in request_model_outputs)
@@ -182,7 +193,6 @@ class HeadsGeneratorFront:
                         for o in request_model_outputs))
 
     def __call__(self, viewdir, c, request_model_outputs=['sampler'], model_inputs={}):
-        import math
         from .heads import regulariser_heads
         g = self.g
         # (the heads read the distance row of the decoder only: nothing view-dependent, 520-585)
@@ -198,12 +208,7 @@ class HeadsGeneratorFront:
             assert g.attention_values > 0
             out['attention_values'] = attention_values
         if 'path_length' in request_model_outputs:   # generator.py:484-499
-            pl_noise = torch.randn_like(planes) / math.sqrt(planes.shape[-2] * planes.shape[-1])
-            target = (planes * pl_noise).sum()
-            if g.attention_values > 0:
-                target = target + (attention_values * torch.randn_like(attention_values)).sum()
-            pl_grad, = torch.autograd.grad(target, inputs=ws, create_graph=True)
-            out['path_length'] = pl_grad.square().sum(dim=-1).mean(dim=-1).sqrt()
+            out['path_length'] = self._path_length(ws, planes, attention_values)
         w1, b1, w2, b2 = decoder_weights(g)
         out.update(regulariser_heads(planes, w1, b1, w2, b2, getattr(g, 'beta', None),
                                      g.scene_range, request_model_outputs, use_sdf=g.use_sdf,
@@ -252,3 +257,51 @@ class GeneratorStepFront(HeadsGeneratorFront):
                                 'trainable synthesis network, outputs within %r)'
                                 % (SUPPORTED_OUTPUTS + HEAD_OUTPUTS,))
         return super().__call__(viewdir, c, request_model_outputs, model_inputs)
+
+
+class PathLengthGeneratorStepFront(GeneratorStepFront):
+    """``GeneratorStepFront`` for the requests that also ask for 'path_length' -- the first
+    generator call of every G-step of the documented training recipe (run.py:970-986 with
+    --path_length_regularization).  The planes and the synthesis rows of the path-length gradient
+    come from ``FusedSynthesis.forward_trainable_with_path_length`` (its double backward is the
+    fused HVP); row 14 (the texture latent, read by the attention palette only) is autograd through
+    the texture mapper, create_graph, and ppl is formed as generator.py:498.  Same random draws in
+    the same order as the reference: synthesis noise, path-length noise, attention noise,
+    stratified points, total-variation perturbation.  ``render`` picks it with
+    ``render.enable_fused_path_length``."""
+
+    def _planes(self, w_synthesis, batch, model_inputs):
+        noise_mode = 'const' if model_inputs.get('freeze_noise') else 'random'
+        planes_cl, self._pl_grad = self.synthesis.forward_trainable_with_path_length(
+            w_synthesis, noise_mode=noise_mode)
+        assert planes_cl.shape[0] == batch
+        return planes_cl
+
+    def _path_length(self, ws, planes, attention_values):
+        g = self.g
+        pl_grad, self._pl_grad = self._pl_grad, None
+        if g.attention_values > 0:   # ws[:, 14] is w_tex; the synthesis reads ws[:, :14]
+            target = (attention_values * torch.randn_like(attention_values)).sum()
+            g_tex = None
+            if target.requires_grad:
+                g_tex, = torch.autograd.grad(target, inputs=ws, create_graph=True, allow_unused=True)
+            row = g_tex[:, 14:] if g_tex is not None else torch.zeros_like(ws[:, 14:])
+            pl_grad = torch.cat([pl_grad, row], dim=1)
+        return pl_grad.square().sum(dim=-1).mean(dim=-1).sqrt()
+
+    def supports(self, request_model_outputs, model_inputs):
+        return (torch.is_grad_enabled()
+                and 'path_length' in request_model_outputs
+                and any(p.requires_grad for p in self.g.synthesis_network.parameters())
+                and all(o in SUPPORTED_OUTPUTS + HEAD_OUTPUTS + ('path_length',)
+                        for o in request_model_outputs)
+                and all(k in ('freeze_noise', 'attention_values', 'attention_values_bias')
+                        for k in model_inputs))
+
+    def __call__(self, viewdir, c, request_model_outputs=['sampler'], model_inputs={}):
+        if not self.supports(request_model_outputs, model_inputs):
+            raise _lib.NfiError('PathLengthGeneratorStepFront: outside its envelope (grad '
+                                "enabled, a trainable synthesis network, 'path_length' requested, "
+                                'outputs within %r)' % (SUPPORTED_OUTPUTS + HEAD_OUTPUTS
+                                                        + ('path_length',),))
+        return HeadsGeneratorFront.__call__(self, viewdir, c, request_model_outputs, model_inputs)

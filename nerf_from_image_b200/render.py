@@ -59,6 +59,7 @@ _FRONTS = {}
 _INV_FRONTS = {}
 _HEAD_FRONTS = {}
 _GEN_FRONTS = {}
+_PL_FRONTS = {}
 
 
 def enable_fused_heads(target_model, enabled=True):
@@ -111,6 +112,20 @@ def enable_fused_generator_step(target_model, enabled=True):
         _GEN_FRONTS[id(target_model)] = GeneratorStepFront(target_model)
     else:
         _GEN_FRONTS.pop(id(target_model), None)
+
+
+def enable_fused_path_length(target_model, enabled=True):
+    """Makes ``render`` run ``target_model``'s generator calls that request 'path_length' (the
+    path-length regulariser, generator.py:484-499: the first G call of every generator step
+    with --path_length_regularization) on the sm_90a synthesis kernels, the regulariser's double
+    backward included (generator.PathLengthGeneratorStepFront).  It applies to grad-enabled calls
+    with a trainable synthesis network and requests within SUPPORTED_OUTPUTS + HEAD_OUTPUTS +
+    'path_length'; every other call routes as without it."""
+    from .generator import PathLengthGeneratorStepFront
+    if enabled:
+        _PL_FRONTS[id(target_model)] = PathLengthGeneratorStepFront(target_model)
+    else:
+        _PL_FRONTS.pop(id(target_model), None)
 
 
 def _closure_vars(fn):
@@ -241,7 +256,11 @@ def render(target_model,
     ifront = _INV_FRONTS.get(id(target_model))
     gfront = _GEN_FRONTS.get(id(target_model))
     hfront = _HEAD_FRONTS.get(id(target_model))
-    if front is not None and front.supports(requests, extra_model_inputs):
+    pfront = _PL_FRONTS.get(id(target_model)) if 'path_length' in requests else None
+    if pfront is not None and pfront.supports(requests, extra_model_inputs):
+        # ... with the path-length regulariser's double backward (PathLengthGeneratorStepFront)
+        model_outputs = pfront(viewdirs, model_input, requests, extra_model_inputs)
+    elif front is not None and front.supports(requests, extra_model_inputs):
         # plane producer on sm_90a too (generator.FusedGeneratorFront; no_grad calls only)
         model_outputs = front(viewdirs, model_input, requests, extra_model_inputs)
     elif ifront is not None and ifront.supports(requests, extra_model_inputs):

@@ -29,7 +29,12 @@ every parameter, noise strengths included -- has its own entry:
 
     planes_cl = FusedSynthesis(net).forward_trainable(ws, noise_mode='random')
 
-backed by ``nfi_synthesis_backward_params``.  There is no CPU path and no fallback.
+backed by ``nfi_synthesis_backward_params``.  The generator step with the path-length
+regulariser (generator.py:484-499) adds the first-order gradient to ws as a differentiable output:
+
+    planes_cl, pl_grad = FusedSynthesis(net).forward_trainable_with_path_length(ws)
+
+whose double backward is ``nfi_synthesis_backward_hvp``.  There is no CPU path and no fallback.
 """
 import ctypes
 import math
@@ -150,6 +155,30 @@ class FusedSynthesis:
         carries their gradient on to ``noise_strength``.  The backward runs
         ``nfi_synthesis_backward_params``; it is not differentiable (no ``create_graph``, so no
         path-length regulariser) and runs once per forward."""
+        present, params, flat_noise = self._trainable_inputs(ws, noise_mode)
+        return _SynthesisTrainFunction.apply(ws, self, noise_mode, present, len(params), None,
+                                             *params, *flat_noise)
+
+    def forward_trainable_with_path_length(self, ws, noise_mode='random'):
+        """``forward_trainable`` plus the path-length regulariser's gradient (generator.py:484-499):
+        -> (planes_cl, pl_grad), pl_grad [B,num_ws,w_dim] = d<planes, pl_noise>/dws with
+        ``pl_noise = randn(B,3,32,R,R) / R`` drawn right after the synthesis noise, as the
+        reference's ``randn_like(planes) / sqrt(R*R)`` on its channel-first view.  pl_grad is
+        differentiable (create_graph) with respect to ws, every parameter and the noise tensors: its
+        backward is ``nfi_synthesis_backward_hvp``.  Both outputs share the saved workspace, which
+        goes once both backwards have run; each runs once."""
+        present, params, flat_noise = self._trainable_inputs(ws, noise_mode)
+        B, R = ws.shape[0], self.net.img_resolution
+        pl_noise = (torch.randn(B, 3, 32, R, R, device=ws.device) / R).permute(0, 1, 3, 4, 2)
+        link = _SavedLink()
+        planes = _SynthesisTrainFunction.apply(ws, self, noise_mode, present, len(params), link,
+                                               *params, *flat_noise)
+        pl_grad = _PathLengthFunction.apply(pl_noise.contiguous(), link, ws, *params, *flat_noise)
+        return planes, pl_grad
+
+    def _trainable_inputs(self, ws, noise_mode):
+        """-> (present, params, flat_noise): the per-layer noise tensors drawn as ``__call__``
+        draws them, and every parameter in the C ABI's order."""
         assert noise_mode in ['random', 'const']
         if not ws.is_cuda:
             raise _lib.NfiError('the fused synthesis network only runs on CUDA tensors '
@@ -165,8 +194,29 @@ class FusedSynthesis:
         params.append(self.blocks[0].const)
         present = [(n0 is not None, n1 is not None) for n0, n1 in noises]
         flat_noise = [n for pair in noises for n in pair if n is not None]
-        return _SynthesisTrainFunction.apply(ws, self, noise_mode, present, len(params),
-                                             *params, *flat_noise)
+        return present, params, flat_noise
+
+    def _param_grads(self, present, param_meta, noise_meta, dev):
+        """Zeroed gradient buffers for every parameter and noise tensor, and the
+        nfi_synth_param_grads that points at them."""
+        zeros = lambda shape: torch.zeros(shape, dtype=torch.float32, device=dev)
+        g_params = [zeros(shape) for shape, _ in param_meta]
+        g_noise = [zeros(shape) for shape, _ in noise_meta]
+        PG = _lib.SynthParamGrads()
+        k = 0
+        for kind, i, _ in self._layers():
+            dst = getattr(PG, kind)[i]
+            dst.g_weight, dst.g_affine_w, dst.g_affine_b, dst.g_bias = (
+                _ptr(g) for g in g_params[k:k + 4])
+            k += 4
+        PG.g_const = _ptr(g_params[k])
+        it = iter(g_noise)
+        for i, (h0, h1) in enumerate(present):
+            if h0:
+                PG.conv0[i].g_noise = _ptr(next(it))
+            if h1:
+                PG.conv1[i].g_noise = _ptr(next(it))
+        return g_params, g_noise, PG
 
     def _run(self, ws, noise_mode, saved, noises=None, trainable=False):
         """-> (planes, (P, keep, work)) -- P, keep and work stay valid for a backward.  ``noises``:
@@ -270,12 +320,14 @@ class _SynthesisTrainFunction(torch.autograd.Function):
     nfi_synthesis_backward_params as the backward."""
 
     @staticmethod
-    def forward(ctx, ws, fs, noise_mode, present, n_params, *tensors):
+    def forward(ctx, ws, fs, noise_mode, present, n_params, link, *tensors):
         params, flat_noise = tensors[:n_params], list(tensors[n_params:])
         noises = [(flat_noise.pop(0) if h0 else None, flat_noise.pop(0) if h1 else None)
                   for h0, h1 in present]
         planes, state = fs._run(ws, noise_mode, saved=True, noises=noises, trainable=True)
         ctx.state, ctx.fs, ctx.present, ctx.ws_dtype = state, fs, present, ws.dtype
+        if link is not None:   # forward_trainable_with_path_length: _PathLengthFunction reads it
+            link.state, link.fs, link.present = state, fs, present
         ctx.param_meta = [(p.shape, p.dtype) for p in params]
         ctx.noise_meta = [(n.shape, n.dtype) for pair in noises for n in pair if n is not None]
         return planes
@@ -295,23 +347,7 @@ class _SynthesisTrainFunction(torch.autograd.Function):
         ws32 = keep[0]
         g_ws = torch.zeros_like(ws32)
         G = _lib.SynthGrads(g_planes=g_planes.data_ptr(), g_ws=g_ws.data_ptr())
-        zeros = lambda shape: torch.zeros(shape, dtype=torch.float32, device=dev)
-        g_params = [zeros(shape) for shape, _ in ctx.param_meta]
-        g_noise = [zeros(shape) for shape, _ in ctx.noise_meta]
-        PG = _lib.SynthParamGrads()
-        k = 0
-        for kind, i, _ in ctx.fs._layers():
-            dst = getattr(PG, kind)[i]
-            dst.g_weight, dst.g_affine_w, dst.g_affine_b, dst.g_bias = (
-                _ptr(g) for g in g_params[k:k + 4])
-            k += 4
-        PG.g_const = _ptr(g_params[k])
-        it = iter(g_noise)
-        for i, (h0, h1) in enumerate(ctx.present):
-            if h0:
-                PG.conv0[i].g_noise = _ptr(next(it))
-            if h1:
-                PG.conv1[i].g_noise = _ptr(next(it))
+        g_params, g_noise, PG = ctx.fs._param_grads(ctx.present, ctx.param_meta, ctx.noise_meta, dev)
         with torch.cuda.device(dev):
             stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
             _lib.check(_lib.load().nfi_synthesis_backward_params(
@@ -319,7 +355,67 @@ class _SynthesisTrainFunction(torch.autograd.Function):
         del P, keep, work
         out = [g.to(dt) for g, (_, dt) in zip(g_params, ctx.param_meta)]
         out += [g.to(dt) for g, (_, dt) in zip(g_noise, ctx.noise_meta)]
-        return (g_ws.to(ctx.ws_dtype), None, None, None, None, *out)
+        return (g_ws.to(ctx.ws_dtype), None, None, None, None, None, *out)
+
+
+class _SavedLink:
+    """The saved forward of a ``_SynthesisTrainFunction``, handed to the ``_PathLengthFunction``
+    built on it (its workspace lives while either still holds it)."""
+    state = fs = present = None
+
+
+class _PathLengthFunction(torch.autograd.Function):
+    """(pl_noise, ws, every parameter, the noise tensors) -> pl_grad = J_ws^T pl_noise: forward
+    ``nfi_synthesis_backward`` on the saved forward of ``link``, backward
+    ``nfi_synthesis_backward_hvp`` (the gradient of <t, pl_grad> with respect to ws, every
+    parameter and the noise tensors)."""
+
+    @staticmethod
+    def forward(ctx, pl_noise, link, ws, *tensors):
+        P, keep, work = link.state
+        ws32 = keep[0]
+        pl_grad = torch.zeros_like(ws32)
+        G = _lib.SynthGrads(g_planes=pl_noise.data_ptr(), g_ws=pl_grad.data_ptr())
+        dev = ws.device
+        with torch.cuda.device(dev):
+            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            _lib.check(_lib.load().nfi_synthesis_backward(ctypes.byref(P), ctypes.byref(G), stream))
+        ctx.state, ctx.fs, ctx.present, ctx.ws_dtype = link.state, link.fs, link.present, ws.dtype
+        ctx.pl_noise = pl_noise
+        n_params = 4 * sum(1 for _ in link.fs._layers()) + 1
+        ctx.param_meta = [(t.shape, t.dtype) for t in tensors[:n_params]]
+        ctx.noise_meta = [(t.shape, t.dtype) for t in tensors[n_params:]]
+        link.state = None
+        return pl_grad.to(ws.dtype)
+
+    @staticmethod
+    def backward(ctx, t_ws):
+        if ctx.state is None:
+            raise _lib.NfiError('the fused path-length backward ran twice on one forward '
+                                '(retain_graph is not supported: the workspace is released)')
+        if torch.is_grad_enabled():
+            raise _lib.NfiError('the fused path-length backward is not differentiable '
+                                '(create_graph)')
+        P, keep, work = ctx.state
+        ctx.state = None
+        dev = t_ws.device
+        lib = _lib.load()
+        t_ws = t_ws.to(torch.float32).contiguous()
+        g_ws = torch.zeros_like(keep[0])
+        g_params, g_noise, PG = ctx.fs._param_grads(ctx.present, ctx.param_meta, ctx.noise_meta, dev)
+        with torch.cuda.device(dev):
+            need = lib.nfi_synthesis_hvp_scratch_bytes(ctypes.byref(P))
+            scratch = torch.empty(need, dtype=torch.uint8, device=dev)
+            H = _lib.SynthHvp(g_planes=ctx.pl_noise.data_ptr(), t_ws=t_ws.data_ptr(),
+                              g_ws=g_ws.data_ptr(), scratch=scratch.data_ptr(), scratch_bytes=need)
+            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            _lib.check(lib.nfi_synthesis_backward_hvp(ctypes.byref(P), ctypes.byref(H),
+                                                      ctypes.byref(PG), stream))
+        del P, keep, work, scratch
+        ctx.pl_noise = None
+        out = [g.to(dt) for g, (_, dt) in zip(g_params, ctx.param_meta)]
+        out += [g.to(dt) for g, (_, dt) in zip(g_noise, ctx.noise_meta)]
+        return (None, None, g_ws.to(ctx.ws_dtype), *out)
 
 
 def planes_channel_first(planes_cl):
