@@ -97,6 +97,11 @@ NFI_API int nfi_synthesis_forward_saved(const nfi_synth_params *params, void *st
 /* The same params (same ws, weights, noise) and the workspace as the saved forward left it. */
 NFI_API int nfi_synthesis_backward(const nfi_synth_params *params, const nfi_synth_grads *grads,
                                    void *stream);
+/* Copies one layer's saved pre-activation u (fp32, [B,res,res,cout] channel-last, res = 4 << block)
+   out of a saved forward's workspace into `out`: which = 0 is conv0 (block >= 1), 1 is conv1.
+   For tests that compare the forward's leaky-ReLU branches with a reference. */
+NFI_API int nfi_synthesis_saved_preactivation(const nfi_synth_params *params, int32_t block,
+                                              int32_t which, float *out, void *stream);
 
 /* Backward to the parameters (the GAN generator step).  Every pointer is ACCUMULATED (+=) like
    g_ws, has the shape of the nfi_synth_layer field it differentiates, and may be NULL (that

@@ -178,6 +178,9 @@ EXPORTS = {
     'nfi_synthesis_forward_saved': (ctypes.c_int, [ctypes.POINTER(SynthParams), ctypes.c_void_p]),
     'nfi_synthesis_backward': (ctypes.c_int, [ctypes.POINTER(SynthParams),
                                               ctypes.POINTER(SynthGrads), ctypes.c_void_p]),
+    'nfi_synthesis_saved_preactivation': (ctypes.c_int, [ctypes.POINTER(SynthParams),
+                                                         ctypes.c_int32, ctypes.c_int32,
+                                                         ctypes.c_void_p, ctypes.c_void_p]),
     'nfi_synthesis_param_workspace_bytes': (ctypes.c_size_t, [ctypes.POINTER(SynthParams)]),
     'nfi_synthesis_backward_params': (ctypes.c_int, [ctypes.POINTER(SynthParams),
                                                      ctypes.POINTER(SynthGrads),

@@ -675,6 +675,14 @@ int nfi_synthesis_backward(const nfi_synth_params* params, const nfi_synth_grads
   return nfi::synth::backward(*params, *grads, (cudaStream_t)stream, g_err, sizeof(g_err));
 }
 
+int nfi_synthesis_saved_preactivation(const nfi_synth_params* params, int32_t block, int32_t which,
+                                      float* out, void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  if (params->batch <= 0) return fail("empty batch");
+  return nfi::synth::saved_preactivation(*params, block, which, out, (cudaStream_t)stream, g_err,
+                                         sizeof(g_err));
+}
+
 size_t nfi_synthesis_param_workspace_bytes(const nfi_synth_params* params) {
   if (params == nullptr) return 0;
   return nfi::synth::param_workspace_bytes(*params);

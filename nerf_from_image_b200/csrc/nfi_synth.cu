@@ -2130,6 +2130,30 @@ int backward(const nfi_synth_params& P, const nfi_synth_grads& G, cudaStream_t s
   return run_backward(P, G, sv, b, st, false, err, err_len);
 }
 
+int saved_preactivation(const nfi_synth_params& P, int block, int which, float* out, cudaStream_t st,
+                        char* err, size_t err_len) {
+  if (const int rc = check_saved(P, err, err_len)) return rc;
+  if (block < 0 || block >= P.num_blocks || (which != 0 && which != 1) || (which == 0 && block == 0)) {
+    snprintf(err, err_len, "synthesis pre-activation: no layer (block %d, which %d)", block, which);
+    return 1;
+  }
+  if (out == nullptr) {
+    snprintf(err, err_len, "synthesis pre-activation: out must be set");
+    return 1;
+  }
+  unsigned char* base = reinterpret_cast<unsigned char*>(
+      (reinterpret_cast<uintptr_t>(P.workspace) + 1023) & ~(uintptr_t)1023);
+  Bump b{base, 0, P.workspace_bytes};
+  Saved sv;
+  memset(&sv, 0, sizeof(sv));
+  if (const int rc = saved_layout(P, b, sv, err, err_len)) return rc;
+  const int res = 4 << block;
+  const size_t n = (size_t)P.batch * res * res * P.channels[block];
+  NFI_SCUDA(cudaMemcpyAsync(out, which ? sv.u1[block] : sv.u0[block], n * sizeof(float),
+                            cudaMemcpyDeviceToDevice, st));
+  return 0;
+}
+
 size_t param_workspace_bytes(const nfi_synth_params& P) {
   char err[256];
   if (check_params(P, err, sizeof(err))) return 0;

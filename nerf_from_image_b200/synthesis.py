@@ -418,6 +418,32 @@ class _PathLengthFunction(torch.autograd.Function):
         return (None, None, g_ws.to(ctx.ws_dtype), *out)
 
 
+def saved_preactivations(planes):
+    """Every layer's pre-activation u kept by the saved forward that produced ``planes`` (the
+    output of ``forward_differentiable`` / ``forward_trainable`` / the planes of
+    ``forward_trainable_with_path_length``, before its backward has run), as fp32 channel-last
+    [B,res,res,C] tensors in layer order: b4.conv1, b8.conv0, b8.conv1, ...  Tests read it to
+    compare the forward's leaky-ReLU branches with a reference."""
+    state = getattr(planes.grad_fn, 'state', None)
+    if state is None:
+        raise _lib.NfiError('no saved synthesis forward behind these planes (or its backward has '
+                            'already released the workspace)')
+    P, _, _ = state
+    lib = _lib.load()
+    B, dev = P.batch, planes.device
+    out = []
+    with torch.cuda.device(dev):
+        stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        for i in range(P.num_blocks):
+            res = 4 << i
+            for which in ((1,) if i == 0 else (0, 1)):
+                u = torch.empty(B, res, res, P.channels[i], device=dev, dtype=torch.float32)
+                _lib.check(lib.nfi_synthesis_saved_preactivation(ctypes.byref(P), i, which,
+                                                                 u.data_ptr(), stream))
+                out.append(u)
+    return out
+
+
 def planes_channel_first(planes_cl):
     """[B,3,R,R,32] -> the reference's [B,96,R,R] (tests, callers of the old layout)."""
     B, three, R, _, C = planes_cl.shape
