@@ -71,7 +71,8 @@ enum nfi_noise_mode {
 enum nfi_mlp_mode {
   NFI_MLP_AUTO = 0,
   NFI_MLP_FP32_SIMT = 1, /* fp32 FFMA on CUDA cores                      */
-  NFI_MLP_TC_3XTF32 = 2, /* wgmma tf32, hi/lo split (3 MMAs), lockstep tile groups */
+  NFI_MLP_TC_3XTF32 = 2, /* alias of NFI_MLP_TC_PIPE (the lockstep tensor-core kernel, whose
+                            tile groups gathered, decoded and shaded in turn, was retired) */
   NFI_MLP_TC_WARPSPEC = 3, /* alias of NFI_MLP_TC_PIPE (the first warp-specialised kernel, whose two
                               roles shared one ring stage per chain, was retired) */
   NFI_MLP_TC_PIPE = 4 /* same arithmetic, fully pipelined: A stages released at MMA completion,
@@ -221,8 +222,9 @@ NFI_API int nfi_render_forward(const nfi_render_params *params, void *stream);
 
 /* TriplanarDecoder.net on given features (models/generator.py:294-299,329-331):
  * features [N,32] -> [N,1+A] (density-or-distance first, colour logits after).
- * The tensor-core mode runs the same tiles / descriptors / epilogue as the
- * render kernel; `workspace` must hold 32 KiB (ignored in SIMT mode). */
+ * Any mode but NFI_MLP_FP32_SIMT runs a 3xTF32 wgmma decoder tile (four 128-point
+ * tiles per 512-thread CTA, weights split into TF32 hi / lo parts);
+ * `workspace` must hold 32 KiB (ignored in SIMT mode). */
 NFI_API int nfi_decoder_forward(const float *features, int64_t n_points, const float *w1,
                                 const float *b1, const float *w2, const float *b2,
                                 int32_t n_attention, float *out, int32_t mlp_mode,

@@ -4,7 +4,7 @@
 # the sampler seam and pose kernels (nfi_field.cu), the synthesis network (nfi_synth.cu), the
 # regulariser-head point evaluator (nfi_heads.cu), the view-direction-conditioned SIMT kernels
 # (nfi_viewdir.cu), and everything else (nfi_render.cu: C ABI,
-# re-layout, SIMT and lockstep kernels).  nfi_render.cu and nfi_viewdir.cu take
+# re-layout, SIMT kernels, stand-alone decoder).  nfi_render.cu and nfi_viewdir.cu take
 # --split-compile 0 (their many kernels are optimised in parallel).
 set -e
 cd "$(dirname "$0")"

@@ -406,7 +406,7 @@ struct FieldConst {
   int use_sdf;
 };
 
-template <int NOUT_PAD, bool FAST = false>
+template <int NOUT_PAD>
 __device__ __forceinline__ void field_head(const float (&out)[NOUT_PAD], const FieldConst& fc,
                                            const float* __restrict__ pal /*smem [A][3]*/,
                                            float keep /*1 - outside*/, float& sigma, float& cr,
@@ -414,7 +414,7 @@ __device__ __forceinline__ void field_head(const float (&out)[NOUT_PAD], const F
   const float d = out[0];
   if (fc.use_sdf) {
     const float nd = -d;
-    const float e = FAST ? __expf(-fabsf(nd) * fc.inv_beta) : expf(-fabsf(nd) * fc.inv_beta);
+    const float e = expf(-fabsf(nd) * fc.inv_beta);
     const float sg = (nd > 0.f) ? 1.f : ((nd < 0.f) ? -1.f : 0.f);
     const float cdf = 0.5f + 0.5f * sg * (1.f - e);
     sigma = fc.inv_alpha * (cdf * keep);
@@ -434,7 +434,7 @@ __device__ __forceinline__ void field_head(const float (&out)[NOUT_PAD], const F
       probs[a] = e;
       s += e;
     }
-    const float inv = FAST ? __fdividef(1.f, s) : 1.f / s;
+    const float inv = 1.f / s;
     cr = cg = cb = 0.f;
 #pragma unroll
     for (int a = 0; a < NOUT_PAD - 1; ++a) {

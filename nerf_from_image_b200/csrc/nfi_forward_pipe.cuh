@@ -1,7 +1,7 @@
 // Forward render kernel, pipelined tensor-core variant (NFI_MLP_TC_PIPE, the default).
 //
-// Same arithmetic as nfi_forward_tc.cuh (3xTF32 decoder on wgmma, thread = ray
-// for everything per-ray), but the per-step chain
+// A 3xTF32 decoder on wgmma (weight image and plane gather from nfi_forward_tc.cuh), thread =
+// ray for everything per-ray.  The per-step chain
 //     gather -> MMA1 -> softplus/split -> MMA2 -> density/colour/composite
 // is cut so that NO resource is held across more than one link of it, and every
 // role only ever does its own kind of work:
@@ -35,6 +35,7 @@
 #pragma once
 #include <type_traits>
 
+#include "nfi_forward.cuh"
 #include "nfi_forward_tc.cuh"
 
 namespace nfi {
@@ -54,24 +55,6 @@ __device__ __forceinline__ float ld_relaxed(const float* p) {
   float v;
   asm volatile("ld.relaxed.cta.global.f32 %0, [%1];" : "=f"(v) : "l"(p) : "memory");
   return v;
-}
-
-// Shell sort (gaps 23, 10, 4, 1) of a thread-private shared-memory column.
-__device__ __forceinline__ void column_sort(float* col, int n, int stride) {
-  const int gaps[4] = {23, 10, 4, 1};
-#pragma unroll 1
-  for (int gi = 0; gi < 4; ++gi) {
-    const int gap = gaps[gi];
-    for (int i = gap; i < n; ++i) {
-      const float v = col[i * stride];
-      int j = i - gap;
-      while (j >= 0 && col[j * stride] > v) {
-        col[(j + gap) * stride] = col[j * stride];
-        j -= gap;
-      }
-      col[(j + gap) * stride] = v;
-    }
-  }
 }
 
 __device__ __forceinline__ bool elect_one() {

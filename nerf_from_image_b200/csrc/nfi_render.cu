@@ -102,24 +102,37 @@ size_t num_tc_ctas(const nfi_render_params* p) {  // persistent grid: at most on
   return want < kMaxPersistentCtas ? want : kMaxPersistentCtas;
 }
 
-// Can the tensor-core kernel take this configuration?
+// the grid of a persistent pipelined launch: num_tc_ctas, and no more CTAs than this device's SMs
+int persistent_grid(const nfi_render_params& p, unsigned* grid) {
+  int dev = 0, sms = 0;
+  NFI_CUDA(cudaGetDevice(&dev));
+  NFI_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const size_t want = num_tc_ctas(&p);
+  *grid = (unsigned)(want < (size_t)sms ? want : (size_t)sms);
+  return 0;
+}
+
+// The modes that run the pipelined tensor-core kernels where they can take the configuration
+// (NFI_MLP_TC_3XTF32 and NFI_MLP_TC_WARPSPEC are aliases of NFI_MLP_TC_PIPE).
+bool tc_mode(int mode) {
+  return mode == NFI_MLP_AUTO || mode == NFI_MLP_TC_3XTF32 || mode == NFI_MLP_TC_WARPSPEC ||
+         mode == NFI_MLP_TC_PIPE;
+}
+
+// Can the pipelined tensor-core kernels take this configuration in this mode?
 bool tc_supported(const nfi_render_params* p) {
   if (p->view_features) return false;  // view-direction conditioning (CARLA): SIMT kernels
-  const int mode = p->mlp_mode & 0xff;
-  const bool pipe_mode = (mode == NFI_MLP_TC_PIPE || mode == NFI_MLP_AUTO || mode == NFI_MLP_TC_WARPSPEC);
+  if (!tc_mode(p->mlp_mode & 0xff)) return false;
   // surface normals: a second pipelined kernel after the render (nfi_normals_pipe.cuh), which
   // walks the merged samples and so needs the forward pass's fine depths; else the SIMT kernel
   if (p->compute_normals && !(p->mlp_mode & 0x1000) &&
-      !(pipe_mode && (!p->fine_sampling || p->z_fine != nullptr) && p->n_peers == 0))
+      !((!p->fine_sampling || p->z_fine != nullptr) && p->n_peers == 0))
     return false;
   // semantics: the pipelined kernel parks the coarse samples' probabilities; NOUT_PAD = 4 only
   // exists for palettes of <= 3 entries, kept on the SIMT kernel
-  if (p->extra_mode == NFI_EXTRA_SEMANTICS && !(pipe_mode && p->n_attention > 3)) return false;
-  const int smax = 64;  // lockstep kernel: per-ray columns in tile memory
-  if (pipe_mode)  // pipelined kernel: <= 4 samples per lane
-    return p->num_samples <= 128 && p->num_samples % 4 == 0;  // in the resampler, float4 jitter
-  if (p->fine_sampling && p->num_samples > smax) return false;
-  return true;
+  if (p->extra_mode == NFI_EXTRA_SEMANTICS && p->n_attention <= 3) return false;
+  // <= 4 samples per lane in the resampler, float4 jitter
+  return p->num_samples <= 128 && p->num_samples % 4 == 0;
 }
 
 bool wants_normals(const nfi_render_params* p) {
@@ -161,73 +174,15 @@ int launch_fwd_extra(const nfi_render_params& p, size_t smem, cudaStream_t st) {
   }
 }
 
-template <int NP, int EX>
-int launch_fwd_tc_fine(const nfi_render_params& p, const unsigned char* wimg, float* scratch,
-                       cudaStream_t st) {
-  const int mode = p.mlp_mode & 0xff;
-  if (mode == NFI_MLP_TC_PIPE || mode == NFI_MLP_AUTO || mode == NFI_MLP_TC_WARPSPEC) {
-    // persistent pipelined kernel (nfi_pipe.cu): one CTA per SM, tiles strided over the grid
-    int dev = 0, sms = 0;
-    NFI_CUDA(cudaGetDevice(&dev));
-    NFI_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    size_t grid = num_ctas(&p);
-    if (grid > (size_t)sms) grid = sms;
-    if (grid > kMaxPersistentCtas) grid = kMaxPersistentCtas;
-    return nfi::launch_pipe_forward(p, NP, wimg, scratch, (unsigned)grid, st, g_err,
-                                    sizeof(g_err));
-  }
-  if (p.n_peers > 0) return fail("peer outputs (n_peers > 0) need the pipelined kernel");
-  if constexpr (EX == 2) {
-    return fail("semantics output on tensor cores: pipelined kernel only");
-  } else {
-  {  // render_forward_tc: 4 tile groups per 512-thread CTA, one CTA per 2x2 tiles
-    const size_t tx = (p.width + nfi::kTileW - 1) / nfi::kTileW;
-    const size_t ty = (p.height + nfi::kTileH - 1) / nfi::kTileH;
-    const unsigned grid = (unsigned)(((tx + 1) / 2) * ((ty + 1) / 2) * (size_t)p.batch);
-    if (p.fine_sampling) {
-      auto k = nfi::render_forward_tc<NP, EX, true>;
-      NFI_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    nfi::kSmTcBytes));
-      k<<<grid, nfi::kTcThreads, nfi::kSmTcBytes, st>>>(p, wimg, scratch);
-    } else {
-      auto k = nfi::render_forward_tc<NP, EX, false>;
-      NFI_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    nfi::kSmTcBytes));
-      k<<<grid, nfi::kTcThreads, nfi::kSmTcBytes, st>>>(p, wimg, scratch);
-    }
-    NFI_CUDA(cudaGetLastError());
-    return 0;
-  }
-  }
-}
-
+// render_forward_pipe (nfi_pipe.cu): the weight image at the head of the workspace, the scratch
+// slabs behind it, tiles strided over the persistent grid
 int launch_fwd_tc(const nfi_render_params& p, int np, cudaStream_t st) {
   unsigned char* wimg = (unsigned char*)p.workspace;
-  float* scratch = (float*)(wimg + kWeightImageBytes);
-  const int nout = 1 + (p.n_attention > 0 ? p.n_attention : 3);
-  const int wmode = p.mlp_mode & 0xff;
-  const bool pipe = (wmode == NFI_MLP_TC_PIPE || wmode == NFI_MLP_AUTO || wmode == NFI_MLP_TC_WARPSPEC);
-  if (pipe) {
-    if (nfi::launch_pipe_weight_image(p, wimg, st)) return fail("weight image launch failed");
-  } else {
-    nfi::prep_weight_image<<<1, 256, 0, st>>>(p.w1, p.b1, p.w2, p.b2, nout, wimg, 1.f, 0.f, 1.f);
-  }
-  NFI_CUDA(cudaGetLastError());
-  const bool coords = p.extra_mode == NFI_EXTRA_COORDS;
-  const bool sem = p.extra_mode == NFI_EXTRA_SEMANTICS;  // pipelined kernel only (tc_supported)
-  switch (np) {
-    case 4:
-      return coords ? launch_fwd_tc_fine<4, 1>(p, wimg, scratch, st)
-                    : launch_fwd_tc_fine<4, 0>(p, wimg, scratch, st);
-    case 12:
-      if (sem) return launch_fwd_tc_fine<12, 2>(p, wimg, scratch, st);
-      return coords ? launch_fwd_tc_fine<12, 1>(p, wimg, scratch, st)
-                    : launch_fwd_tc_fine<12, 0>(p, wimg, scratch, st);
-    default:
-      if (sem) return launch_fwd_tc_fine<16, 2>(p, wimg, scratch, st);
-      return coords ? launch_fwd_tc_fine<16, 1>(p, wimg, scratch, st)
-                    : launch_fwd_tc_fine<16, 0>(p, wimg, scratch, st);
-  }
+  if (nfi::launch_pipe_weight_image(p, wimg, st)) return fail("weight image launch failed");
+  unsigned grid = 0;
+  if (int rc = persistent_grid(p, &grid)) return rc;
+  return nfi::launch_pipe_forward(p, np, wimg, (float*)(wimg + kWeightImageBytes), grid, st,
+                                  g_err, sizeof(g_err));
 }
 
 // SIMT reference decoder (one point per thread), for nfi_decoder_forward
@@ -356,18 +311,10 @@ size_t nfi_render_workspace_bytes(const nfi_render_params* p) {
   size_t fwd = 0;
   if (p->fine_sampling) {
     // scratch for the coarse samples, sized for the kernel that will run
-    const int mode = p->mlp_mode & 0xff;
-    const bool pipe_mode =
-        (mode == NFI_MLP_TC_PIPE || mode == NFI_MLP_AUTO || mode == NFI_MLP_TC_WARPSPEC);
-    if (pipe_mode && tc_supported(p)) {  // persistent: one slab per CTA (<= one per SM)
+    if (tc_supported(p)) {  // persistent: one slab per CTA (<= one per SM)
       fwd = num_tc_ctas(p) * nfi::pipe_scratch_bytes_per_cta(
                                  p->num_samples,
                                  p->extra_mode == NFI_EXTRA_SEMANTICS ? nout_pad_of(p) - 1 : 0);
-    } else if (mode == NFI_MLP_TC_3XTF32) {  // lockstep: one slab per tile group of every CTA
-      const size_t tx = (p->width + nfi::kTileW - 1) / nfi::kTileW;
-      const size_t ty = (p->height + nfi::kTileH - 1) / nfi::kTileH;
-      fwd = ((tx + 1) / 2) * ((ty + 1) / 2) * (size_t)p->batch * nfi::kGroups *
-            nfi::pipe_scratch_bytes_per_cta(p->num_samples, 0);
     } else {  // fp32 SIMT kernel: one slab per CTA (= tile)
       fwd = num_ctas(p) * nfi::fwd_scratch_floats_per_cta(p->num_samples, ne_store_of(p)) *
             sizeof(float);
@@ -416,13 +363,10 @@ int nfi_render_forward(const nfi_render_params* params, void* stream) {
   const int np = nout_pad_of(params);
   cudaStream_t st = (cudaStream_t)stream;
   const int mode = p.mlp_mode & 0xff;
-  if ((mode == NFI_MLP_TC_3XTF32 || mode == NFI_MLP_TC_WARPSPEC || mode == NFI_MLP_TC_PIPE) &&
-      !tc_supported(params))
-    return fail("tensor-core modes need S <= 128 and S % 4 == 0 (lockstep kernel: S <= 64) and "
-                "no semantics output; use NFI_MLP_AUTO");
-  const bool want_tc = mode == NFI_MLP_TC_3XTF32 || mode == NFI_MLP_TC_WARPSPEC ||
-                       mode == NFI_MLP_TC_PIPE ||
-                       (mode == NFI_MLP_AUTO && tc_supported(params));
+  const bool want_tc = tc_supported(params);
+  if (mode != NFI_MLP_AUTO && tc_mode(mode) && !want_tc)
+    return fail("tensor-core modes need S <= 128 and S % 4 == 0 and no semantics output; "
+                "use NFI_MLP_AUTO");
   if (want_tc || p.fine_sampling) {
     if (!p.workspace || p.workspace_bytes < nfi_render_workspace_bytes(params))
       return fail("workspace too small (see nfi_render_workspace_bytes)");
@@ -433,14 +377,11 @@ int nfi_render_forward(const nfi_render_params* params, void* stream) {
   if (want_tc) {
     if (int rc = launch_fwd_tc(p, np, st)) return rc;
     if (wants_normals(params)) {
-      int dev = 0, sms = 0;
-      NFI_CUDA(cudaGetDevice(&dev));
-      NFI_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-      size_t grid = num_ctas(&p);
-      if (grid > (size_t)sms) grid = sms;
+      unsigned grid = 0;
+      if (int rc = persistent_grid(p, &grid)) return rc;
       unsigned char* ws = (unsigned char*)p.workspace;
       const size_t off = (nfi_render_workspace_bytes(params) - 32768) & ~(size_t)255;
-      return nfi::launch_pipe_normals(p, np, ws, ws + off, (unsigned)grid, st, g_err, sizeof(g_err));
+      return nfi::launch_pipe_normals(p, np, ws, ws + off, grid, st, g_err, sizeof(g_err));
     }
     return 0;
   }
@@ -533,12 +474,8 @@ int nfi_render_backward(const nfi_render_params* params, const nfi_render_grads*
                                            p.workspace_bytes >= nfi::pipe_wgrad_workspace_bytes(
                                                                     (unsigned)kMaxPersistentCtas)));
   if (tc_ok) {
-    int dev = 0, sms = 0;
-    NFI_CUDA(cudaGetDevice(&dev));
-    NFI_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    size_t grid = num_ctas(&p);
-    if (grid > (size_t)sms) grid = sms;
-    if (grid > kMaxPersistentCtas) grid = kMaxPersistentCtas;  // (the wgrad workspace is sized for it)
+    unsigned grid = 0;  // <= kMaxPersistentCtas: the wgrad workspace is sized for that many CTAs
+    if (int rc = persistent_grid(p, &grid)) return rc;
     nfi_render_grads g1 = g;
     g1.grad_w1 = g1.grad_b1 = g1.grad_w2 = g1.grad_b2 = nullptr;
     const bool others = g1.grad_planes || g1.grad_palette || g1.grad_beta || g1.grad_alpha ||
@@ -549,12 +486,12 @@ int nfi_render_backward(const nfi_render_params* params, const nfi_render_grads*
     const bool one_sweep = wgrad && others && !g.grad_origins && !(p.mlp_mode & 0x2000);
     if ((others && !one_sweep) || !wgrad) {
       if (int rc = nfi::launch_pipe_backward(p, g1, nout_pad_of(params), (unsigned char*)p.workspace,
-                                             (unsigned)grid, st, g_err, sizeof(g_err)))
+                                             grid, st, g_err, sizeof(g_err)))
         return rc;
     }
     if (wgrad)
       return nfi::launch_pipe_wgrad(p, g, nout_pad_of(params), (unsigned char*)p.workspace,
-                                    (unsigned)grid, one_sweep, st, g_err, sizeof(g_err));
+                                    grid, one_sweep, st, g_err, sizeof(g_err));
     return 0;
   }
   return nfi::launch_backward(*params, *grads, st, g_err, sizeof(g_err));
@@ -769,7 +706,7 @@ int nfi_render_forward_host(const nfi_render_params* hp, int32_t device) {
     if (q) cudaMemcpyAsync(q, h, n * sizeof(float), cudaMemcpyHostToDevice, st);
     return q;
   };
-  // chunk = 8 images: 128 CTAs of the lockstep kernel, ~34 MB per image on the wire
+  // chunk = 8 images, ~34 MB per image on the wire
   const size_t CB = B < 8 ? B : 8;
   const size_t n_chunks = (B + CB - 1) / CB;
   const size_t plane_img = 3 * R * R * 32;

@@ -280,10 +280,6 @@ __host__ __device__ constexpr int kpos_of_hidden(int j) {
 // register of the same element: a0 = (g, t), a1 = (g + 8, t), a2 = (g, t + 4), a3 = (g + 8, t + 4)
 __host__ __device__ constexpr int afrag_slot(int e) { return ((e & 1) << 1) | (e >> 1); }
 
-__device__ __forceinline__ void prefetch_l1(const void* p) {
-  asm volatile("prefetch.global.L1 [%0];" ::"l"(p));
-}
-
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));

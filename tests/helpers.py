@@ -56,7 +56,7 @@ def run_oracle(scene, cams, H, W, S, noise_t, noise_u, **kw):
                            white_background=scene['white_background'], **kw)
 
 
-MLP_MODE = 0  # tests/test_parity_gpu.py switches this (0 auto, 1 SIMT, 2 tensor core)
+MLP_MODE = 0  # tests/test_parity_gpu.py switches this (0 auto, 1 SIMT, 2 / 4 tensor core)
 
 
 def run_cuda(scene, cams, H, W, S, noise_t, noise_u, use_sdf=True, fine_sampling=True,

@@ -16,9 +16,10 @@ TOL = 2e-4
 
 @pytest.fixture(autouse=True, params=[1, 2, 4], ids=['simt', 'tc', 'pipe'])
 def mlp_mode(request):
-    """Every test below runs with the fp32 SIMT MLP and with the wgmma
-    3xTF32 MLP (S = 16 keeps the fine pass inside the tensor-core kernel's
-    S % 16 == 0 envelope; other S fall back under NFI_MLP_AUTO)."""
+    """Every test below runs with the fp32 SIMT MLP, with NFI_MLP_TC_3XTF32 (an alias of the
+    pipelined kernels) and with the pipelined wgmma 3xTF32 MLP, NFI_MLP_TC_PIPE (S = 16 keeps
+    every render inside the tensor-core envelope S <= 128, S % 4 == 0; renders outside it fall
+    back under NFI_MLP_AUTO)."""
     Hh.MLP_MODE = request.param
     yield request.param
     Hh.MLP_MODE = 0
@@ -61,11 +62,9 @@ def test_forward_variants(cuda_lib, fine, A, use_sdf):
 
 
 @pytest.mark.parametrize('S', [32, 64, 128])
-def test_forward_and_backward_sample_counts(cuda_lib, S, mlp_mode):
+def test_forward_and_backward_sample_counts(cuda_lib, S):
     """BASELINE config 5 sweeps 32 -> 128 samples per ray: the pipelined kernels take
-    S <= 128 (2 or 4 resampling slots per lane), the older tensor-core kernels S <= 64."""
-    if mlp_mode == 2 and S > 64:
-        pytest.skip('lockstep / first warp-specialised kernel: S <= 64')
+    S <= 128 (2 or 4 resampling slots per lane)."""
     B, H, W = 1, 16, 24
     scene, cams = Hh.make_case('p3d_bbox', batch=B)
     nt, nu = _noise(37, B, H, W, S)
@@ -85,9 +84,7 @@ def test_forward_and_backward_sample_counts(cuda_lib, S, mlp_mode):
 
 
 @pytest.mark.parametrize('mode', ['coords', 'semantics'])
-def test_extra_outputs(cuda_lib, mode, mlp_mode):
-    if mode == 'semantics' and mlp_mode == 2:
-        pytest.skip('semantics output: SIMT and pipelined kernels only')
+def test_extra_outputs(cuda_lib, mode):
     B, H, W, S = 2, 16, 16, 16
     scene, cams = Hh.make_case('p3d_plain', batch=B)
     nt, nu = _noise(7, B, H, W, S)
@@ -259,6 +256,46 @@ def test_backward_extras_and_frozen_weights(cuda_lib):
         outs.append(torch.autograd.grad(loss, [sc['planes'], sc['palette'], cm['c2w']]))
     for a, b, n in zip(outs[1], outs[0], ['planes', 'palette', 'c2w']):
         assert Hh.rel_l2(a.cpu(), b) < 2e-3, n
+
+
+@pytest.mark.parametrize('mlp_mode', [2, 3], ids=['tc', 'warpspec'])  # (instead of the fixture)
+@pytest.mark.parametrize('case', ['fine_s128', 'semantics_a10', 'coarse_s160'])
+def test_tc_modes_are_aliases_of_pipe(cuda_lib, case, mlp_mode):
+    """NFI_MLP_TC_3XTF32 (2) and NFI_MLP_TC_WARPSPEC (3) run the pipelined kernels of
+    NFI_MLP_TC_PIPE (4): the same renders run (fine sampling at S = 128, semantics with 10 palette
+    entries) with the same outputs bit for bit and the same gradients, and the same renders are
+    refused (no fine sampling at S = 160: outside the pipelined kernels, left to NFI_MLP_AUTO)."""
+    from nerf_from_image_b200._lib import NfiError
+    fine, S, extra_mode = {'fine_s128': (True, 128, 0), 'semantics_a10': (True, 16, 2),
+                           'coarse_s160': (False, 160, 0)}[case]
+    B, H, W = 1, 16, 24
+    scene, cams = Hh.make_case('p3d_bbox', batch=B, attention_values=10)
+    nt, nu = _noise(47, B, H, W, S, fine=fine)
+    names = ['planes', 'w1', 'b1', 'w2', 'b2']
+
+    def run(mode):
+        sc, cm = Hh.to_device(scene, 'cuda'), Hh.to_device(cams, 'cuda')
+        for n in names:
+            sc[n] = sc[n].clone().requires_grad_()
+        cm['c2w'] = cm['c2w'].clone().requires_grad_()
+        outs = Hh.run_cuda(sc, cm, H, W, S, nt, nu, fine_sampling=fine, extra_mode=extra_mode,
+                           mlp_mode=mode)
+        rgb, depth, mask, extra = outs  # (extra: None without an extra output)
+        grads = _grads((rgb, mask), [sc[n] for n in names] + [cm['c2w']])
+        return [o.detach() for o in outs if o is not None], grads
+
+    if case == 'coarse_s160':
+        for mode in (mlp_mode, 4):
+            with pytest.raises(NfiError, match='NFI_MLP_AUTO'):
+                run(mode)
+        return
+    (outs, grads), (want_outs, want_grads) = run(mlp_mode), run(4)
+    for a, b in zip(outs, want_outs):  # rgb, depth, mask, extra
+        assert torch.equal(a, b)
+    # (the plane and decoder-weight gradients are sums of float atomics, in an order that varies
+    # from run to run)
+    for n, a, b in zip(names + ['c2w'], grads, want_grads):
+        assert Hh.rel_l2(a, b) < 1e-5, n
 
 
 def test_relayout_roundtrip(cuda_lib):
