@@ -129,20 +129,27 @@ __device__ __forceinline__ float linspace01(int k, int S) {
 
 // Bilinear taps of one plane, F.grid_sample(bilinear, border, align_corners=True)
 // (models/generator.py:312-326; ATen GridSamplerKernel: unnormalise, clip, floor).
+// The values are the same under both gradient rules below; only inx / iny differ.
+//   LOWER_FACE_IN = false: ATen's rule, the gradient flows strictly inside (0, R-1) -- the
+//     render, normals and sampler paths, whose reference fetch is F.grid_sample.
+//   LOWER_FACE_IN = true: the rule of the twice-differentiable fetch the regulariser heads'
+//     reference uses (lib/ops.py grid_sample2d), which clamps the tap INDICES instead of the
+//     coordinate, so the gradient also flows at texel coordinate 0 exactly: [0, R-1).
 struct Taps {
   int o00, o01, o10, o11;      // texel offsets (in texels) of nw, ne, sw, se
   float w00, w01, w10, w11;    // their weights
   float gx0, gx1, gy0, gy1;    // 1-d weights (west/east, north/south) for d/dcoord
-  bool inx, iny;               // coordinate strictly inside (0, R-1): grad flows
+  bool inx, iny;               // grad flows along x / y (see the rules above)
 };
 
+template <bool LOWER_FACE_IN = false>
 __device__ __forceinline__ Taps make_taps(float gx, float gy, int R) {
   Taps t;
   const float m = (float)(R - 1);
   float ix = ((gx + 1.f) / 2.f) * m;
   float iy = ((gy + 1.f) / 2.f) * m;
-  t.inx = (ix > 0.f) && (ix < m);
-  t.iny = (iy > 0.f) && (iy < m);
+  t.inx = (LOWER_FACE_IN ? ix >= 0.f : ix > 0.f) && (ix < m);
+  t.iny = (LOWER_FACE_IN ? iy >= 0.f : iy > 0.f) && (iy < m);
   ix = fminf(m, fmaxf(ix, 0.f));
   iy = fminf(m, fmaxf(iy, 0.f));
   const float fx = floorf(ix), fy = floorf(iy);
@@ -229,6 +236,8 @@ __device__ __forceinline__ void bilerp4_grad(const float4* plane, const Taps& t,
 // gather_features plus the derivatives of the features with respect to the three
 // normalised coordinates (rows of Grow: [3][32][kFRow]), up to the common factor
 // (R-1)/2 / 3 the caller applies.  Plane xy sees (x0, x1), xz (x0, x2), yz (x1, x2).
+// LOWER_FACE_IN selects make_taps' gradient rule.
+template <bool LOWER_FACE_IN = false>
 __device__ __forceinline__ void gather_features_grad(const float* __restrict__ planes_b, int R,
                                                      float x0, float x1, float x2, float* Frow,
                                                      float* Grow, int lane) {
@@ -242,9 +251,9 @@ __device__ __forceinline__ void gather_features_grad(const float* __restrict__ p
     const float c2 = __shfl_sync(kFull, x2, src);
     const float4* base = reinterpret_cast<const float4*>(planes_b) + k;
     float4 e0, e1, e2, ax, ay, bx, by, cx, cy;
-    bilerp4_grad(base, make_taps(c0, c1, R), e0, ax, ay);
-    bilerp4_grad(base + plane_stride / 4, make_taps(c0, c2, R), e1, bx, by);
-    bilerp4_grad(base + 2 * (plane_stride / 4), make_taps(c1, c2, R), e2, cx, cy);
+    bilerp4_grad(base, make_taps<LOWER_FACE_IN>(c0, c1, R), e0, ax, ay);
+    bilerp4_grad(base + plane_stride / 4, make_taps<LOWER_FACE_IN>(c0, c2, R), e1, bx, by);
+    bilerp4_grad(base + 2 * (plane_stride / 4), make_taps<LOWER_FACE_IN>(c1, c2, R), e2, cx, cy);
     float4 f;
     f.x = ((e0.x + e1.x) + e2.x) / 3.f;
     f.y = ((e0.y + e1.y) + e2.y) / 3.f;

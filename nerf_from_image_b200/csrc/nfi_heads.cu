@@ -4,7 +4,9 @@
 //   forward   d(x)  = b2_0 + sum_j W2_0j softplus(pre_j),   pre_j = b1_j + sum_c W1_jc F_c(x)
 //             g_k(x) = dd/dx_k = gamma sum_c t_c G_kc,       t_c = sum_j W1_jc v_j,  v_j = W2_0j sigmoid(pre_j)
 //             F = mean over the three planes of the bilinear fetch, G_k = dF/d(texel coordinate k)
-//             (gather_features_grad), gamma = (R-1)/2 / 3 / scene_range
+//             (gather_features_grad), gamma = (R-1)/2 / 3 / scene_range.  G follows the heads'
+//             reference fetch (lib/ops.py grid_sample2d), not F.grid_sample: it is nonzero on the
+//             lower faces (texel coordinate 0) and zero on the upper ones (make_taps<true>)
 //   backward  of BOTH outputs (the eikonal loss differentiates g: a double backward in the
 //             reference), with ghat = gamma * dL/dg:
 //               tbar_c = sum_k ghat_k G_kc            vbar_j = sum_c W1_jc tbar_c
@@ -164,7 +166,8 @@ sdf_points_fwd_kernel(const nfi_sdf_points_params p) {
   const size_t plane_img = (size_t)3 * p.plane_res * p.plane_res * kC;
   for (long long u = (long long)blockIdx.x * kWarps + warp; u < units; u += (long long)gridDim.x * kWarps) {
     const Unit q = load_unit(p, u, nb, lane);
-    gather_features_grad(p.planes + q.b * plane_img, p.plane_res, q.x0, q.x1, q.x2, Fw, Gw, lane);
+    gather_features_grad<true>(p.planes + q.b * plane_img, p.plane_res, q.x0, q.x1, q.x2, Fw, Gw,
+                               lane);
     float h[kHid];
     pre_activations(Fw + lane * kFRow, s, h);
     float d = b2_0;
@@ -225,7 +228,7 @@ sdf_points_bwd_kernel(const nfi_sdf_points_params p, const nfi_sdf_points_grads 
       gh2 = gamma * g.g_grad[q.row * 3 + 2];
     }
     const float* planes_b = p.planes + q.b * plane_img;
-    gather_features_grad(planes_b, p.plane_res, q.x0, q.x1, q.x2, Fw, Gw, lane);
+    gather_features_grad<true>(planes_b, p.plane_res, q.x0, q.x1, q.x2, Fw, Gw, lane);
     float h[kHid], vb[kHid];
     pre_activations(Fw + lane * kFRow, s, h);
     // tbar_c -> Tw row; vbar_j = sum_c W1_jc tbar_c
@@ -326,7 +329,7 @@ sdf_points_bwd_kernel(const nfi_sdf_points_params p, const nfi_sdf_points_grads 
         for (int pl = 0; pl < 3; ++pl) {
           const float ga = (pl == 2) ? c1 : c0, gb = (pl == 0) ? c1 : c2;
           const float ha = (pl == 2) ? a1 : a0, hb = (pl == 0) ? a1 : a2;  // ghat of the two axes
-          const Taps t = make_taps(ga, gb, p.plane_res);
+          const Taps t = make_taps<true>(ga, gb, p.plane_res);
           const float A = t.inx ? ha : 0.f, Bc = t.iny ? hb : 0.f;
           float* gp = gplanes_b + pl * plane_stride + 4 * kq;
           const float k00 = -t.gy0 * A - t.gx0 * Bc, k01 = t.gy0 * A - t.gx1 * Bc,
