@@ -156,8 +156,9 @@ typedef struct nfi_render_params {
    * second layer emits 1 + 32 values (w2 [33,64], b2 [33]) and every sample's colour logits are
    *     w3 . leaky_relu(view_features[ray] + decoder_features, 0.2) + b3
    * (ViewDirectionMapper.mapper_closure); view_features is the mapper's per-RAY trunk output
-   * (fc0 .. fc6 on the unit ray direction, computed by the caller once per ray).  fp32 SIMT
-   * kernels only. */
+   * (fc0 .. fc6 on the unit ray direction, computed by the caller once per ray).  Forward: the
+   * pipelined tensor-core kernel inside its envelope (the fp32 SIMT kernel outside it or with
+   * NFI_MLP_FP32_SIMT); backward: the fp32 SIMT kernel. */
   const float *view_features; /* [B,H,W,32] or NULL */
   const float *w3;            /* [A,32] ([3,32] when A == 0): EFFECTIVE weight of mapper.output */
   const float *b3;            /* [A] ([3]) */

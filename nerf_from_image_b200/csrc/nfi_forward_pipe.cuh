@@ -28,6 +28,8 @@
 //             activation
 //   softplus: ln2 * (max(x', 0) + lg2(1 + 2^-|x'|)) with x' = x log2 e: two MUFU ops (ex2, lg2)
 //             per hidden unit; log2(e) is folded into W1/b1 by prep_weight_image;
+//   view    : the VD instantiation (--use_viewdir) puts a third layer behind the decoder in the
+//             activation warpgroup (decoder_layers23_vd below); every other role is unchanged
 //   resample: the S uniforms of a ray are sorted by a bitonic network across the
 //             warp (2 per lane) and pushed through the inverse CDF with shuffle
 //             binary searches: one warp-pass per ray instead of a serial per-thread
@@ -99,13 +101,19 @@ __host__ __device__ inline size_t pipe_scratch_floats(int S, int nes) {
   return tc_scratch_floats_per_group(S) + (size_t)S * kThreads * nes;
 }
 
-template <int P>
+// view features of a tile plus b2[1..32], in the layer-2 accumulator's fragment order (VD only)
+constexpr int kViewTileBytes = kThreads * NFI_VIEW_FEATURES * 4;
+
+// VD: the view-direction-conditioned instantiation (a larger weight image, nfi_layout.h, and the
+// tile's view features); the offsets of the plain kernel do not depend on it.
+template <int P, bool VD = false>
 struct PipeCfg {
   static constexpr int kThreadsTotal = 256 + 128 * P;
   static constexpr int kStages = P + 1;  // one spare: a set never waits for its own MMA
-  static constexpr int kSmA = 25600;
+  static constexpr int kSmA = VD ? 41984 : 25600;
   static constexpr int kSmD2 = kSmA + kStages * kFwdStageBytes;
-  static constexpr int kSmPal = kSmD2 + kPipeSlots * kD2SlotBytes;
+  static constexpr int kSmView = kSmD2 + kPipeSlots * kD2SlotBytes;
+  static constexpr int kSmPal = kSmView + (VD ? kViewTileBytes : 0);
   static constexpr int kSmFrac = kSmPal + 48 * 4;  // s / S for s < 128 (one IEEE division each)
   static constexpr int kSmBars = kSmFrac + 128 * 4;
   // full[P+1], a_free[P+1], d2_full[3], slot_free[3], cw_ready, zf_ready, weights
@@ -198,6 +206,122 @@ __device__ __forceinline__ void decoder_step_fp32(const unsigned char* stage, ui
     tc::wgmma_wait<0>();
     tc::reg_fence(d);
     decoder_layer2(d, w2_hi, w2_lo, b1, d2 + 64 * mb * kD2Ld, warp, lane);
+#pragma unroll
+    for (int kb = 0; kb < 4; ++kb)
+#pragma unroll
+      for (int s = 0; s < 4; ++s) fa[kb][s] = fb[kb][s];
+  }
+}
+
+// ------------------------------------------------------------------ view-direction conditioning
+// (--use_viewdir, models/generator.py:189-253,662-663): layer 2 emits the distance and 32
+// features, and the colour logits are W3 . leaky_relu(view_features[ray] + features, 0.2) + b3.
+// A step's row is a ray, so the view features are constant per row for the whole tile: the
+// activation warpgroup keeps them (with b2[1..32] added) in shared memory in the order of its own
+// layer-2 accumulator fragment -- float4 (mb, j) of thread gt holds rows g / g + 8 of 64-row block
+// mb, columns 8j + 2t, 8j + 2t + 1 -- written and read by the same thread, so no barrier guards it.
+__device__ __forceinline__ void fill_view_tile(const nfi_render_params& p, const TileCoord& tcd,
+                                               const float* __restrict__ b2f, float4* vt, int wig,
+                                               int lane) {
+  const int g = lane >> 2, t = lane & 3;
+#pragma unroll
+  for (int mb = 0; mb < 2; ++mb) {
+    const float* src[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = 64 * mb + 16 * wig + g + 8 * h;
+      int px, py;
+      tile_pixel(tcd.tile_x, tcd.tile_y, row >> 5, row & 31, px, py);
+      px = min(px, p.width - 1);  // rows outside the image: any finite value (masked later)
+      py = min(py, p.height - 1);
+      const size_t ray = ((size_t)tcd.b * p.height + py) * p.width + px;
+      src[h] = p.view_features + ray * NFI_VIEW_FEATURES + 2 * t;
+    }
+#pragma unroll
+    for (int j = 0; j < NFI_VIEW_FEATURES / 8; ++j) {
+      const float2 a = __ldg(reinterpret_cast<const float2*>(src[0] + 8 * j));
+      const float2 c = __ldg(reinterpret_cast<const float2*>(src[1] + 8 * j));
+      const float2 bb = *reinterpret_cast<const float2*>(b2f + 8 * j + 2 * t);
+      vt[(mb * 4 + j) * kThreads] = make_float4(a.x + bb.x, a.y + bb.y, c.x + bb.x, c.y + bb.y);
+    }
+  }
+}
+
+// Second half of the view-conditioned decoder for one 64-row block: softplus, layer 2 with N = 40
+// (24 wgmma), leaky ReLU of features + view features on the accumulator registers, which become
+// the register A fragments of layer 3 (12 wgmma), and the D2 row [distance, logits] to `d2`.
+// Both accumulators start from zero and the fp32 terms (view features, biases, the distance) are
+// added on the CUDA cores, as the plain kernel adds b2: the tensor core only sums products.
+__device__ __forceinline__ void decoder_layers23_vd(const float (&d)[32], uint64_t w2_hi,
+                                                    uint64_t w2_lo, uint64_t w3_hi, uint64_t w3_lo,
+                                                    const float* __restrict__ b1, const float4* vt,
+                                                    float* d2, int warp, int lane) {
+  uint32_t hi[8][4], lo[8][4];
+  tc::softplus_frag<true>(d, b1, lane & 3, hi, lo);
+  float o[20];
+#pragma unroll
+  for (int i = 0; i < 20; ++i) o[i] = 0.f;
+  tc::wgmma_fence();
+  tc::layer2_vd_mb(o, hi, lo, w2_hi, w2_lo);
+  tc::wgmma_commit();
+  tc::wgmma_wait<0>();
+  tc::reg_fence(o);
+  uint32_t yhi[4][4], ylo[4][4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float4 v = vt[j * kThreads];
+    const float ve[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const float z = o[4 * j + e] + ve[e];
+      tc::put_split(yhi, ylo, j, tc::afrag_slot(e), z > 0.f ? z : z * 0.2f);
+    }
+  }
+  float q[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) q[i] = 0.f;
+  tc::wgmma_fence();
+  tc::layer3_vd_mb(q, yhi, ylo, w3_hi, w3_lo);
+  tc::wgmma_commit();
+  tc::wgmma_wait<0>();
+  tc::reg_fence(q);
+  // column 0 of layer 3 has zero weights; the thread that owns it (t = 0) also owns column 32
+  // of layer 2, the distance, for the same two rows
+  if ((lane & 3) == 0) {
+    q[0] = o[16];
+    q[2] = o[18];
+  }
+  tc::store_frag_rows(q, d2, kD2Ld, warp, lane);
+}
+
+// decoder_step_fp32 with the view-conditioned layers 2 and 3; `vt` = this thread's view tile
+template <typename F>
+__device__ __forceinline__ void decoder_step_vd(const unsigned char* stage, uint64_t w1_hi,
+                                                uint64_t w1_lo, uint64_t w2_hi, uint64_t w2_lo,
+                                                uint64_t w3_hi, uint64_t w3_lo,
+                                                const float* __restrict__ b1, const float4* vt,
+                                                float* d2, int warp, int lane, F&& on_stage_read) {
+  float fa[4][4], fb[4][4];
+  tc::load_afrag_sw128(fa, stage, 0, warp, lane);
+  tc::load_afrag_sw128(fb, stage, 64, warp, lane);
+  on_stage_read();
+#pragma unroll 1
+  for (int mb = 0; mb < 2; ++mb) {
+    uint32_t a_hi[4][4], a_lo[4][4];
+#pragma unroll
+    for (int kb = 0; kb < 4; ++kb)
+#pragma unroll
+      for (int s = 0; s < 4; ++s) tc::put_split(a_hi, a_lo, kb, s, fa[kb][s]);
+    float d[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) d[i] = 0.f;
+    tc::wgmma_fence();
+    tc::layer1_mb_rs(d, a_hi, a_lo, w1_hi, w1_lo);
+    tc::wgmma_commit();
+    tc::wgmma_wait<0>();
+    tc::reg_fence(d);
+    decoder_layers23_vd(d, w2_hi, w2_lo, w3_hi, w3_lo, b1, vt + mb * 4 * kThreads,
+                        d2 + 64 * mb * kD2Ld, warp, lane);
 #pragma unroll
     for (int kb = 0; kb < 4; ++kb)
 #pragma unroll
@@ -467,11 +591,15 @@ __device__ __forceinline__ void resample_rows_impl(const ResampleArgs& a, int fi
     cur = nxt;
   }
 }
-template <int NOUT_PAD, int EXTRA, bool FINE, int P, bool DBG, int NSLOT = 2>
+template <int NOUT_PAD, int EXTRA, bool FINE, int P, bool DBG, int NSLOT = 2, bool VD = false>
 __global__ void __launch_bounds__(PipeCfg<P>::kThreadsTotal, 1)
 render_forward_pipe(const nfi_render_params p, const unsigned char* __restrict__ wimg,
                     float* __restrict__ scratch) {
-  using Cfg = PipeCfg<P>;
+  using Cfg = PipeCfg<P, VD>;
+  static_assert(!(VD && DBG), "the phase timers are not instantiated for the view-conditioned kernel");
+  // VD: the image of nfi_layout.h; its `head` is what the shading group adds to a D2 row
+  constexpr int kImgBytes = VD ? kVdBytes : kWiBytes;
+  constexpr int kImgB1 = VD ? kVdB1 : kWiB1, kImgB2 = VD ? kVdHead : kWiB2;
   // extras composited with the weights: 3 world coordinates (EXTRA 1, recomputed from the
   // depth) or the NA attention probabilities (EXTRA 2, parked in scratch for the coarse samples)
   constexpr int NA_ = NOUT_PAD - 1;
@@ -500,8 +628,8 @@ render_forward_pipe(const nfi_render_params p, const unsigned char* __restrict__
   uint64_t* zf_ready = cw_ready + 1;             //      fine depths of the tile written (every resampling warp)
   uint64_t* wbar = zf_ready + 1;                 //      weight image landed
   float* d2s = reinterpret_cast<float*>(base + Cfg::kSmD2);  // [3][128][kD2Ld]
-  const float* b1s = reinterpret_cast<const float*>(base + kWiB1);
-  const float* b2s = reinterpret_cast<const float*>(base + kWiB2);
+  const float* b1s = reinterpret_cast<const float*>(base + kImgB1);
+  const float* b2s = reinterpret_cast<const float*>(base + kImgB2);
   float* pal = reinterpret_cast<float*>(base + Cfg::kSmPal);
   float* frac = reinterpret_cast<float*>(base + Cfg::kSmFrac);
   if (tid < 128) frac[tid] = (float)tid / (float)S;
@@ -525,8 +653,8 @@ render_forward_pipe(const nfi_render_params p, const unsigned char* __restrict__
   }
   __syncthreads();
   if (tid == 0) {
-    tc::mbar_expect_tx(wbar, kWiBytes);
-    tc::tma_bulk_g2s(base, wimg, kWiBytes, wbar);
+    tc::mbar_expect_tx(wbar, kImgBytes);
+    tc::tma_bulk_g2s(base, wimg, kImgBytes, wbar);
   }
   tc::mbar_wait(wbar, 0);
 
@@ -678,8 +806,9 @@ render_forward_pipe(const nfi_render_params p, const unsigned char* __restrict__
     const uint32_t base_s = tc::smem_u32(base);
     const uint64_t dsc_w1_hi = tc::gmma_desc_sw128(base_s + kWiW1Hi);
     const uint64_t dsc_w1_lo = tc::gmma_desc_sw128(base_s + kWiW1Lo);
-    const uint64_t dsc_w2_hi = tc::gmma_desc_sw128(base_s + kWiW2Hi);
-    const uint64_t dsc_w2_lo = tc::gmma_desc_sw128(base_s + kWiW2Lo);
+    const uint64_t dsc_w2_hi = tc::gmma_desc_sw128(base_s + (VD ? kVdW2Hi : kWiW2Hi));
+    const uint64_t dsc_w2_lo = tc::gmma_desc_sw128(base_s + (VD ? kVdW2Lo : kWiW2Lo));
+    const float4* vt = reinterpret_cast<const float4*>(base + Cfg::kSmView) + gt;  // (VD only)
     uint32_t st = 0, u = 0, sl = 0, v = 0;
     // the next ring position: stage + D2 slot -> decoder -> d2_full, a_free
     auto activate = [&]() {
@@ -689,7 +818,14 @@ render_forward_pipe(const nfi_render_params p, const unsigned char* __restrict__
       NFI_STEP_WAIT(&slot_free[sl], (v & 1) ^ 1);
       NFI_T(0)
       float* d2 = d2s + sl * (kThreads * kD2Ld);
-      if (!dbg_skip_consumer) {
+      if constexpr (VD) {
+        decoder_step_vd(base + Cfg::kSmA + st * kFwdStageBytes, dsc_w1_hi, dsc_w1_lo, dsc_w2_hi,
+                        dsc_w2_lo, tc::gmma_desc_sw128(base_s + kVdW3Hi),
+                        tc::gmma_desc_sw128(base_s + kVdW3Lo), b1s, vt, d2, wig, lane, [&]() {
+                          __syncwarp();
+                          if (lane == 0) mbar_arrive(&a_free[st]);
+                        });
+      } else if (!dbg_skip_consumer) {
         decoder_step_fp32(base + Cfg::kSmA + st * kFwdStageBytes, dsc_w1_hi, dsc_w1_lo, dsc_w2_hi,
                           dsc_w2_lo, b1s, d2, wig, lane, [&]() {
                             __syncwarp();
@@ -708,6 +844,10 @@ render_forward_pipe(const nfi_render_params p, const unsigned char* __restrict__
     };
     uint32_t tile_it = 0;
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tile_it) {
+      if constexpr (VD)
+        fill_view_tile(p, tile_coord(tile, tiles_x, tiles_y),
+                       reinterpret_cast<const float*>(base + kVdB2f),
+                       reinterpret_cast<float4*>(base + Cfg::kSmView) + gt, wig, lane);
       for (int s = 0; s < S; ++s) activate();
       if (FINE) {
         // second half of this warp's rows is resampled here, the first half by the

@@ -1,0 +1,121 @@
+// Operand layouts of the tensor-core kernels as plain index arithmetic, compilable by a host
+// C++ compiler without the CUDA toolkit (tests/c/vd_image_check.cpp runs them on the CPU):
+// the SWIZZLE_128B tile offset, the K permutation of a register A fragment, and the weight image
+// of the view-direction-conditioned forward kernel (render_forward_pipe<..., VD = true>).
+#pragma once
+#include <stdint.h>
+#include <string.h>
+
+#ifdef __CUDACC__
+#define NFI_HD __host__ __device__ __forceinline__
+#else
+#define NFI_HD inline
+#endif
+
+namespace nfi {
+namespace tc {
+
+// byte offset of (row, 16-byte chunk) inside a [rows x 128 B] SWIZZLE_128B tile
+NFI_HD uint32_t sw128_offset(int row, int chunk) {
+  return (uint32_t)((row >> 3) * 1024 + (row & 7) * 128 + ((chunk ^ (row & 7)) << 4));
+}
+
+// K position, inside its block of 8, at which a register A fragment holds hidden unit j (see
+// nfi_tc.cuh): units 2t and 2t + 1 of the block sit at positions t and t + 4
+NFI_HD constexpr int kpos_of_hidden(int j) {
+  return (j & ~7) | ((j & 1) ? 4 + ((j >> 1) & 3) : ((j >> 1) & 3));
+}
+// accumulator register e of a column block (rows g / g + 8, columns 2t / 2t + 1) -> A-fragment
+// register of the same element: a0 = (g, t), a1 = (g + 8, t), a2 = (g, t + 4), a3 = (g + 8, t + 4)
+NFI_HD constexpr int afrag_slot(int e) { return ((e & 1) << 1) | (e >> 1); }
+
+}  // namespace tc
+
+// ---------------------------------------------------------------------------
+// Weight image of the view-direction-conditioned decoder (models/generator.py:189-253,662-663):
+//   layer 1   W1 [64 x 32], b1                       as in the plain image (nfi_forward_tc.cuh)
+//   layer 2   W2 [33 x 64]: row 0 = distance, rows 1..32 = features.  Stored as a [40 x 64] B
+//             operand whose output column c < 32 is feature c (w2 row c + 1) and column 32 the
+//             distance (w2 row 0); columns 33..39 are zero.  K positions in fragment order.
+//   layer 3   W3 [A or 3 x 32] as a [16 x 32] B operand: output column 0 has zero weights (the
+//             distance is moved there in registers), column 1 + a is w3 row a; K position of
+//             feature c = kpos_of_hidden(c), the layer-2 accumulator being layer 3's A fragment.
+//   biases    b1 [64]; b2f [32] = b2[1..32] (added to the features with the ray's view features);
+//             head [16] = what the shading warpgroup adds to a D2 row: b2[0], then b3, then the
+//             padding value of the unused logits.
+// `scale1` multiplies W1 / b1, `scale3` W3 / b3 (the colour logits), `pad` fills head[1 + A ..].
+// ---------------------------------------------------------------------------
+constexpr int kVdW2Cols = 40;                      // layer-2 output columns (N of the wgmma)
+constexpr int kVdW2KBlockBytes = kVdW2Cols * 128;  // one [40 x 32] SWIZZLE_128B K-block
+constexpr int kVdW1Hi = 0;                         // [64 x 32] SW128, 8 KB
+constexpr int kVdW1Lo = 8192;
+constexpr int kVdW2Hi = 16384;                     // two K-blocks, 10 KB
+constexpr int kVdW2Lo = kVdW2Hi + 2 * kVdW2KBlockBytes;
+constexpr int kVdW3Hi = kVdW2Lo + 2 * kVdW2KBlockBytes;  // [16 x 32] SW128, 2 KB
+constexpr int kVdW3Lo = kVdW3Hi + 2048;
+constexpr int kVdB1 = kVdW3Lo + 2048;              // 64 floats
+constexpr int kVdB2f = kVdB1 + 256;                // 32 floats
+constexpr int kVdHead = kVdB2f + 128;              // 16 floats
+constexpr int kVdBytes = kVdHead + 64;             // 41408
+static_assert(kVdW3Hi % 1024 == 0 && kVdBytes % 16 == 0, "SWIZZLE_128B atoms / bulk-copy size");
+
+// output column of layer 2 that holds row `row` of w2
+NFI_HD constexpr int vd_w2_col(int row) { return row == 0 ? 32 : row - 1; }
+// byte offset, inside a W2 hi / lo block, of (output column, hidden unit j)
+NFI_HD uint32_t vd_w2_offset(int col, int j) {
+  const int jp = tc::kpos_of_hidden(j);
+  return (uint32_t)((jp >> 5) * kVdW2KBlockBytes) + tc::sw128_offset(col, (jp & 31) >> 2) +
+         (uint32_t)(jp & 3) * 4u;
+}
+// byte offset, inside a W3 hi / lo block, of (output column, feature c)
+NFI_HD uint32_t vd_w3_offset(int col, int c) {
+  const int cp = tc::kpos_of_hidden(c);
+  return tc::sw128_offset(col, cp >> 2) + (uint32_t)(cp & 3) * 4u;
+}
+
+// x with the low 13 mantissa bits cleared: exactly representable in TF32
+NFI_HD float vd_tf32_hi(float x) {
+  uint32_t u;
+  memcpy(&u, &x, 4);
+  u &= 0xFFFFE000u;
+  memcpy(&x, &u, 4);
+  return x;
+}
+NFI_HD void vd_put_split(unsigned char* img, int hi_base, int lo_base, uint32_t off, float w) {
+  const float hi = vd_tf32_hi(w);
+  const float lo = w - hi;
+  memcpy(img + hi_base + off, &hi, 4);
+  memcpy(img + lo_base + off, &lo, 4);
+}
+
+// Worker `idx` of `n` fills its share of the image (a CUDA block's threads, or 0 of 1 on the host).
+NFI_HD void vd_weight_image_fill(const float* w1, const float* b1, const float* w2, const float* b2,
+                                 const float* w3, const float* b3, int n_attention,
+                                 unsigned char* img, float scale1, float scale3, float pad,
+                                 int idx, int n) {
+  const int nlogit = n_attention > 0 ? n_attention : 3;
+  for (int i = idx; i < 64 * 32; i += n) {
+    const int j = i / 32, k = i % 32;  // W1[j][k]
+    vd_put_split(img, kVdW1Hi, kVdW1Lo, tc::sw128_offset(j, k >> 2) + (uint32_t)(k & 3) * 4u,
+                 w1[i] * scale1);
+  }
+  for (int i = idx; i < kVdW2Cols * 64; i += n) {
+    const int col = i / 64, j = i % 64;
+    const float w = col < 32 ? w2[(col + 1) * 64 + j] : (col == 32 ? w2[j] : 0.f);
+    vd_put_split(img, kVdW2Hi, kVdW2Lo, vd_w2_offset(col, j), w);
+  }
+  for (int i = idx; i < 16 * 32; i += n) {
+    const int col = i / 32, c = i % 32;
+    const float w = (col >= 1 && col <= nlogit) ? w3[(col - 1) * 32 + c] * scale3 : 0.f;
+    vd_put_split(img, kVdW3Hi, kVdW3Lo, vd_w3_offset(col, c), w);
+  }
+  float* b1i = reinterpret_cast<float*>(img + kVdB1);
+  float* b2f = reinterpret_cast<float*>(img + kVdB2f);
+  float* head = reinterpret_cast<float*>(img + kVdHead);
+  for (int i = idx; i < 64; i += n) b1i[i] = b1[i] * scale1;
+  for (int i = idx; i < 32; i += n) b2f[i] = b2[1 + i];
+  for (int i = idx; i < 16; i += n)
+    head[i] = i == 0 ? b2[0] : (i <= nlogit ? b3[i - 1] * scale3 : pad);
+}
+
+}  // namespace nfi

@@ -35,4 +35,11 @@ int launch_pipe_normals(const nfi_render_params& p, int nout_pad, const unsigned
 // layer 2, padded logits at -1e30)
 int launch_pipe_weight_image(const nfi_render_params& p, unsigned char* wimg, cudaStream_t st);
 size_t pipe_scratch_bytes_per_cta(int num_samples, int nes);
+// The view-direction-conditioned render (params.view_features / w3 / b3, w2 of 33 rows) on
+// render_forward_pipe<..., VD = true> (nfi_pipe_vd.cu): its weight image (nfi_layout.h, up to
+// 64 KiB at `wimg`) and the launch, `scratch` and `grid` as for launch_pipe_forward.
+int launch_pipe_weight_image_vd(const nfi_render_params& p, unsigned char* wimg, cudaStream_t st);
+int launch_pipe_forward_vd(const nfi_render_params& p, int nout_pad, const unsigned char* wimg,
+                           float* scratch, unsigned grid, cudaStream_t st, char* err,
+                           size_t err_len);
 }  // namespace nfi

@@ -92,6 +92,13 @@ size_t num_ctas(const nfi_render_params* p) {
 }
 
 constexpr size_t kWeightImageBytes = 32768;  // workspace header (nfi::kWiBytes rounded up)
+constexpr size_t kViewWeightImageBytes = 65536;  // ... of a view-conditioned render (nfi::kVdBytes)
+static_assert(nfi::kWiBytes <= kWeightImageBytes && nfi::kVdBytes <= kViewWeightImageBytes,
+              "weight image larger than the workspace header");
+// the workspace header of this render: every user of the workspace starts behind it
+size_t header_bytes(const nfi_render_params* p) {
+  return p->view_features ? kViewWeightImageBytes : kWeightImageBytes;
+}
 constexpr size_t kBackwardWorkspaceBytes = 65536;  // forward + backward weight images
 
 constexpr size_t kMaxPersistentCtas = 160;  // >= SM count of any sm_90 part (H100 SXM: 132)
@@ -121,7 +128,6 @@ bool tc_mode(int mode) {
 
 // Can the pipelined tensor-core kernels take this configuration in this mode?
 bool tc_supported(const nfi_render_params* p) {
-  if (p->view_features) return false;  // view-direction conditioning (CARLA): SIMT kernels
   if (!tc_mode(p->mlp_mode & 0xff)) return false;
   // surface normals: a second pipelined kernel after the render (nfi_normals_pipe.cuh), which
   // walks the merged samples and so needs the forward pass's fine depths; else the SIMT kernel
@@ -175,14 +181,18 @@ int launch_fwd_extra(const nfi_render_params& p, size_t smem, cudaStream_t st) {
 }
 
 // render_forward_pipe (nfi_pipe.cu): the weight image at the head of the workspace, the scratch
-// slabs behind it, tiles strided over the persistent grid
+// slabs behind it, tiles strided over the persistent grid.  A view-conditioned render takes the
+// VD instantiation and its weight image (nfi_pipe_vd.cu).
 int launch_fwd_tc(const nfi_render_params& p, int np, cudaStream_t st) {
   unsigned char* wimg = (unsigned char*)p.workspace;
-  if (nfi::launch_pipe_weight_image(p, wimg, st)) return fail("weight image launch failed");
+  const bool vd = p.view_features != nullptr;
+  if (vd ? nfi::launch_pipe_weight_image_vd(p, wimg, st) : nfi::launch_pipe_weight_image(p, wimg, st))
+    return fail("weight image launch failed");
   unsigned grid = 0;
   if (int rc = persistent_grid(p, &grid)) return rc;
-  return nfi::launch_pipe_forward(p, np, wimg, (float*)(wimg + kWeightImageBytes), grid, st,
-                                  g_err, sizeof(g_err));
+  float* scratch = (float*)(wimg + header_bytes(&p));
+  if (vd) return nfi::launch_pipe_forward_vd(p, np, wimg, scratch, grid, st, g_err, sizeof(g_err));
+  return nfi::launch_pipe_forward(p, np, wimg, scratch, grid, st, g_err, sizeof(g_err));
 }
 
 // SIMT reference decoder (one point per thread), for nfi_decoder_forward
@@ -321,7 +331,7 @@ size_t nfi_render_workspace_bytes(const nfi_render_params* p) {
     }
   }
   // (+ the backward weight image of the normals kernel, behind the scratch)
-  return kWeightImageBytes + fwd + 256 + (wants_normals(p) && tc_supported(p) ? 32768 : 0);
+  return header_bytes(p) + fwd + 256 + (wants_normals(p) && tc_supported(p) ? 32768 : 0);
 }
 
 int nfi_planes_to_channel_last(const float* xy, const float* xz, const float* yz,
@@ -380,6 +390,11 @@ int nfi_render_forward(const nfi_render_params* params, void* stream) {
       unsigned grid = 0;
       if (int rc = persistent_grid(p, &grid)) return rc;
       unsigned char* ws = (unsigned char*)p.workspace;
+      // render_normals_pipe reads the plain image, of which it needs layer 1 and the distance
+      // row: row 0 of w2 with or without a view.  The view render is done with its own image
+      // (stream order), so the plain one takes its place at the head of the workspace.
+      if (p.view_features && nfi::launch_pipe_weight_image(p, ws, st))
+        return fail("weight image launch failed");
       const size_t off = (nfi_render_workspace_bytes(params) - 32768) & ~(size_t)255;
       return nfi::launch_pipe_normals(p, np, ws, ws + off, grid, st, g_err, sizeof(g_err));
     }
@@ -388,7 +403,7 @@ int nfi_render_forward(const nfi_render_params* params, void* stream) {
   if (p.n_peers > 0) return fail("peer outputs (n_peers > 0) need the pipelined kernel");
   if (p.view_features) {
     nfi_render_params pv = p;  // SIMT scratch starts after the weight-image header
-    if (pv.workspace) pv.workspace = (unsigned char*)pv.workspace + kWeightImageBytes;
+    if (pv.workspace) pv.workspace = (unsigned char*)pv.workspace + header_bytes(params);
     return nfi::launch_forward_viewdir(pv, np, wants_normals(params), st, g_err, sizeof(g_err));
   }
   const size_t smem =

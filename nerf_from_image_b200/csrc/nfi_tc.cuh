@@ -19,6 +19,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "nfi_layout.h"  // sw128_offset, kpos_of_hidden, afrag_slot
+
 namespace nfi {
 namespace tc {
 
@@ -172,6 +174,17 @@ __device__ __forceinline__ void wgmma_tf32_rs_n32(float (&d)[16], const uint32_t
       : "memory");
 }
 
+__device__ __forceinline__ void wgmma_tf32_rs_n40(float (&d)[20], const uint32_t (&a)[4], uint64_t b,
+                                                   int acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %25, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n40k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19}, {%20, %21, %22, %23}, %24, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc)
+      : "memory");
+}
+
 __device__ __forceinline__ void wgmma_tf32_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t b,
                                                    int acc) {
   asm volatile(
@@ -249,11 +262,6 @@ __device__ __forceinline__ void wgmma_bf16_ss_n128(float (&d)[64], uint64_t a, u
       : "memory");
 }
 
-// byte offset of (row, 16-byte chunk) inside a [rows x 128 B] SWIZZLE_128B tile
-__host__ __device__ __forceinline__ uint32_t sw128_offset(int row, int chunk) {
-  return (uint32_t)((row >> 3) * 1024 + (row & 7) * 128 + ((chunk ^ (row & 7)) << 4));
-}
-
 // byte offset of (row, 16-byte chunk) inside a [rows x 64 B] SWIZZLE_64B tile (chunk 0..3) and a
 // [rows x 32 B] SWIZZLE_32B tile (chunk 0..1): address bits [4,6) / [4,5) XOR bits [7,9) / [7,8)
 __device__ __forceinline__ uint32_t sw64_offset(int row, int chunk) {
@@ -270,15 +278,6 @@ __host__ __device__ __forceinline__ float tf32_hi(float x) {
   return x;
 #endif
 }
-
-// K position, inside its block of 8, at which a register A fragment holds hidden unit j (see the
-// header): units 2t and 2t + 1 of the block sit at positions t and t + 4
-__host__ __device__ constexpr int kpos_of_hidden(int j) {
-  return (j & ~7) | ((j & 1) ? 4 + ((j >> 1) & 3) : ((j >> 1) & 3));
-}
-// accumulator register e of a column block (rows g / g + 8, columns 2t / 2t + 1) -> A-fragment
-// register of the same element: a0 = (g, t), a1 = (g + 8, t), a2 = (g, t + 4), a3 = (g + 8, t + 4)
-__host__ __device__ constexpr int afrag_slot(int e) { return ((e & 1) << 1) | (e >> 1); }
 
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
@@ -354,6 +353,34 @@ __device__ __forceinline__ void layer2_mb(float (&o)[8], const uint32_t (&hhi)[8
 #pragma unroll
   for (int ks = 0; ks < 8; ++ks)
     wgmma_tf32_rs_n16(o, hhi[ks], w2_hi + (ks >> 2) * 128 + (ks & 3) * 2, 1);
+}
+
+// The view-conditioned decoder's layer 2, D[64 x 40] = H W2'^T (32 features, the distance, 7 zero
+// columns): the 24 products of layer2_mb on [40 x 32] K-blocks (nfi_layout.h).
+__device__ __forceinline__ void layer2_vd_mb(float (&o)[20], const uint32_t (&hhi)[8][4],
+                                             const uint32_t (&hlo)[8][4], uint64_t w2_hi,
+                                             uint64_t w2_lo) {
+  constexpr int kb = kVdW2KBlockBytes >> 4;
+#pragma unroll
+  for (int ks = 0; ks < 8; ++ks)
+    wgmma_tf32_rs_n40(o, hlo[ks], w2_hi + (ks >> 2) * kb + (ks & 3) * 2, ks != 0);
+#pragma unroll
+  for (int ks = 0; ks < 8; ++ks)
+    wgmma_tf32_rs_n40(o, hhi[ks], w2_lo + (ks >> 2) * kb + (ks & 3) * 2, 1);
+#pragma unroll
+  for (int ks = 0; ks < 8; ++ks)
+    wgmma_tf32_rs_n40(o, hhi[ks], w2_hi + (ks >> 2) * kb + (ks & 3) * 2, 1);
+}
+// Its layer 3, D[64 x 16] = Y W3'^T with the 32 activated features as register fragments: 12 wgmma.
+__device__ __forceinline__ void layer3_vd_mb(float (&q)[8], const uint32_t (&yhi)[4][4],
+                                             const uint32_t (&ylo)[4][4], uint64_t w3_hi,
+                                             uint64_t w3_lo) {
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) wgmma_tf32_rs_n16(q, ylo[ks], w3_hi + 2 * ks, ks != 0);
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) wgmma_tf32_rs_n16(q, yhi[ks], w3_lo + 2 * ks, 1);
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) wgmma_tf32_rs_n16(q, yhi[ks], w3_hi + 2 * ks, 1);
 }
 
 // split v into TF32 hi / remainder and place both at A-fragment register `slot` of k-block kb

@@ -399,7 +399,8 @@ def fused_render(planes, w1, b1, w2, b2, palette, beta, alpha, c2w, focal,
     ``peers``: list of (rgb, depth, mask) device ADDRESSES of this rank's slices in the other
     ranks' buffers; the kernel stores its tiles there too (parallel.PeerExchange).
     ``view``: (view_features [B,H,W,32], w3 [A,32], b3 [A]) switches on the view-direction
-    conditioning of the CARLA models (--use_viewdir; fp32 SIMT kernels).
+    conditioning of the CARLA models (--use_viewdir; the forward on the pipelined tensor-core
+    kernel where it can take the configuration, the backward on the fp32 SIMT kernel).
     ``rows``: (row_offset, full_height) renders rows [row_offset, row_offset + height) of images
     full_height rows tall; every per-ray tensor (noise, outputs) then has ``height`` rows.
 
