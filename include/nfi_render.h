@@ -158,7 +158,8 @@ typedef struct nfi_render_params {
    * (ViewDirectionMapper.mapper_closure); view_features is the mapper's per-RAY trunk output
    * (fc0 .. fc6 on the unit ray direction, computed by the caller once per ray).  Forward: the
    * pipelined tensor-core kernel inside its envelope (the fp32 SIMT kernel outside it or with
-   * NFI_MLP_FP32_SIMT); backward: the fp32 SIMT kernel. */
+   * NFI_MLP_FP32_SIMT); backward: the pipelined tensor-core kernel with a frozen decoder and mapper
+ * output inside its envelope (nfi_render_backward), the fp32 SIMT kernel otherwise. */
   const float *view_features; /* [B,H,W,32] or NULL */
   const float *w3;            /* [A,32] ([3,32] when A == 0): EFFECTIVE weight of mapper.output */
   const float *b3;            /* [A] ([3]) */
@@ -237,8 +238,13 @@ NFI_API int nfi_decoder_forward(const float *features, int64_t n_points, const f
  * b1 / w2 / b2) come from render_wgrad_pipe (MN-major bf16-pair GEMMs on wgmma), which needs
  * params->workspace >= NFI_BACKWARD_WORKSPACE_BYTES: without pose gradients (the GAN generator
  * step) it is the WHOLE backward in one sweep, with them it runs beside render_backward_pipe.
+ * A view-conditioned render (params->view_features) takes the same envelope on its own
+ * instantiation of render_backward_pipe when no grad_w1 / b1 / w2 / b2 / w3 / b3 is requested (the
+ * inversion step: decoder and mapper frozen) and params->workspace holds
+ * NFI_VIEW_BACKWARD_WORKSPACE_BYTES (its two weight images); grad_view_features may be NULL.
  * Everything outside that envelope: the fp32 SIMT kernel. */
 #define NFI_BACKWARD_WORKSPACE_BYTES (65536 + 160 * 32768)
+#define NFI_VIEW_BACKWARD_WORKSPACE_BYTES 98304
 NFI_API int nfi_render_backward(const nfi_render_params *params, const nfi_render_grads *grads,
                         void *stream);
 

@@ -19,6 +19,7 @@ c_float_p = ctypes.POINTER(ctypes.c_float)
 ABI_VERSION = 5  # NFI_ABI_VERSION of include/nfi_render.h
 MAX_PEERS = 7
 BACKWARD_WORKSPACE_BYTES = 65536 + 160 * 32768  # NFI_BACKWARD_WORKSPACE_BYTES
+VIEW_BACKWARD_WORKSPACE_BYTES = 98304  # NFI_VIEW_BACKWARD_WORKSPACE_BYTES
 
 EXTRA_NONE, EXTRA_COORDS, EXTRA_SEMANTICS = 0, 1, 2
 NOISE_DETERMINISTIC, NOISE_EXPLICIT, NOISE_PHILOX = 0, 1, 2

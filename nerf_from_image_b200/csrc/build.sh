@@ -1,7 +1,8 @@
 #!/bin/bash
 # Builds libnfi_render.so in-tree for sm_90a (cross-compiles without a GPU).
 # Seven translation units compiled in parallel: the pipelined tensor-core kernels (nfi_pipe.cu),
-# the view-direction-conditioned instantiations of the pipelined forward kernel (nfi_pipe_vd.cu),
+# the view-direction-conditioned instantiations of the pipelined forward and backward kernels
+# (nfi_pipe_vd.cu),
 # the sampler seam and pose kernels (nfi_field.cu), the synthesis network (nfi_synth.cu), the
 # regulariser-head point evaluator (nfi_heads.cu), the view-direction-conditioned SIMT kernels
 # (nfi_viewdir.cu), and everything else (nfi_render.cu: C ABI,

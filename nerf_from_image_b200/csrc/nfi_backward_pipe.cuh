@@ -41,14 +41,22 @@ constexpr int kWbW1tHi = 16384;  // [32 rows = channel c][64 k = hidden j] as tw
 constexpr int kWbW1tLo = 24576;  //   (K positions in register-fragment order: tc::kpos_of_hidden)
 constexpr int kWbBytes = 32768;
 
-template <int P>
+// VD: the view-conditioned instantiation.  Its two weight images (nfi_layout.h) are larger, so its
+// stages hold fp32 features (split into TF32 hi / lo in registers, as the forward kernel does)
+// instead of hi / lo pairs, and it keeps the tile's view features and the rays' view-gradient sums
+// (both in the activation warpgroup's fragment order) behind the D4 slots.  The offsets of the
+// plain kernel do not depend on it.
+template <int P, bool VD = false>
 struct BwdCfg {
   static constexpr int kThreadsTotal = 256 + 128 * P;
-  static constexpr int kSmWb = 25600;                      // backward weight image
-  static constexpr int kSmA = kSmWb + kWbBytes;            // 58368 = 57 * 1024
-  static constexpr int kSmD2 = kSmA + kBwdStages * kPipeStageBytes;  // D2 / dOut slots
+  static constexpr int kSmWb = VD ? 41984 : 25600;         // backward weight image
+  static constexpr int kSmA = kSmWb + (VD ? 41984 : kWbBytes);  // 58368 = 57 * 1024 (plain)
+  static constexpr int kStageBytes = VD ? kFwdStageBytes : kPipeStageBytes;
+  static constexpr int kSmD2 = kSmA + kBwdStages * kStageBytes;      // D2 / dOut slots
   static constexpr int kSmD4 = kSmD2 + kBwdSlots * kD2SlotBytes;     // D4 slots
-  static constexpr int kSmStage = kSmD4 + kBwdSlots * kD4SlotBytes;  // per-warp coord-grad staging
+  static constexpr int kSmView = kSmD4 + kBwdSlots * kD4SlotBytes;   // VD: view tile, then sums
+  static constexpr int kSmVg = kSmView + (VD ? kViewTileBytes : 0);
+  static constexpr int kSmStage = kSmVg + (VD ? kViewTileBytes : 0);  // per-warp coord-grad staging
   static constexpr int kStageWarp = 32 * 4 * 4;                      // [32][4] coord grads
   static constexpr int kSmPal = kSmStage + P * 4 * kStageWarp;
   static constexpr int kSmFrac = kSmPal + 48 * 4;
@@ -107,6 +115,28 @@ __device__ __forceinline__ void mma3_mb(float (&d3)[32], const uint32_t (&hi)[2]
   tc::wgmma_tf32_rs_n64(d3, hi[1], b_lo + 2, 1);
   tc::wgmma_tf32_rs_n64(d3, hi[0], b_hi, 1);
   tc::wgmma_tf32_rs_n64(d3, hi[1], b_hi + 2, 1);
+}
+// VD: dG = dOut W3 (K = 16 outputs, N = 32 features), the same six products as mma3_mb
+__device__ __forceinline__ void mma_dg_mb(float (&dg)[16], const uint32_t (&hi)[2][4],
+                                          const uint32_t (&lo)[2][4], uint64_t b_hi, uint64_t b_lo) {
+  tc::wgmma_tf32_rs_n32(dg, lo[0], b_hi, 0);
+  tc::wgmma_tf32_rs_n32(dg, lo[1], b_hi + 2, 1);
+  tc::wgmma_tf32_rs_n32(dg, hi[0], b_lo, 1);
+  tc::wgmma_tf32_rs_n32(dg, hi[1], b_lo + 2, 1);
+  tc::wgmma_tf32_rs_n32(dg, hi[0], b_hi, 1);
+  tc::wgmma_tf32_rs_n32(dg, hi[1], b_hi + 2, 1);
+}
+// VD: D3 += dF W2[1..32] (K = 32 features, N = 64), dF as register fragments; D3 arrives holding
+// the distance row's part
+__device__ __forceinline__ void mma3_vd_mb(float (&d3)[32], const uint32_t (&hi)[4][4],
+                                           const uint32_t (&lo)[4][4], uint64_t b_hi,
+                                           uint64_t b_lo) {
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) tc::wgmma_tf32_rs_n64(d3, lo[ks], b_hi + 2 * ks, 1);
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) tc::wgmma_tf32_rs_n64(d3, hi[ks], b_lo + 2 * ks, 1);
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) tc::wgmma_tf32_rs_n64(d3, hi[ks], b_hi + 2 * ks, 1);
 }
 // D4 = dpre_lo*B_hi + dpre_hi*B_lo + dpre_hi*B_hi   (K = 64: two k-blocks of 4 k-steps)
 __device__ __forceinline__ void mma4_mb(float (&d4)[16], const uint32_t (&hi)[8][4],
@@ -201,11 +231,17 @@ struct MergeWalk {
   }
 };
 
-template <int NOUT_PAD, int EXTRA, bool CAM, int P>
+// VD: the view-conditioned decoder.  `wimg` holds its forward image (nfi_layout.h) at 0 and its
+// backward image at kVdBwdImageOffset.
+template <int NOUT_PAD, int EXTRA, bool CAM, int P, bool VD = false>
 __global__ void __launch_bounds__(BwdCfg<P>::kThreadsTotal, 1)
 render_backward_pipe(const nfi_render_params p, const nfi_render_grads g,
                      const unsigned char* __restrict__ wimg) {
-  using Cfg = BwdCfg<P>;
+  using Cfg = BwdCfg<P, VD>;
+  constexpr int kImgBytes = VD ? kVdBytes : kWiBytes;
+  constexpr int kImgB1 = VD ? kVdB1 : kWiB1, kImgB2 = VD ? kVdHead : kWiB2;
+  constexpr int kBwdImgOff = VD ? kVdBwdImageOffset : 32768;
+  constexpr int kBwdImgBytes = VD ? kVbBytes : kWbBytes;
   constexpr int NA = NOUT_PAD - 1;
   constexpr int NS = kBwdStages;
   extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -229,8 +265,8 @@ render_backward_pipe(const nfi_render_params p, const nfi_render_grads g,
   uint64_t* wbar = slot_free + kBwdSlots;       // [2] weight images landed
   float* d2s = reinterpret_cast<float*>(base + Cfg::kSmD2);  // [2][128][kD2Ld]
   float* d4s = reinterpret_cast<float*>(base + Cfg::kSmD4);  // [2][128][kD4Ld]
-  const float* b1s = reinterpret_cast<const float*>(base + kWiB1);
-  const float* b2s = reinterpret_cast<const float*>(base + kWiB2);
+  const float* b1s = reinterpret_cast<const float*>(base + kImgB1);
+  const float* b2s = reinterpret_cast<const float*>(base + kImgB2);
   float* pal = reinterpret_cast<float*>(base + Cfg::kSmPal);
   float* frac = reinterpret_cast<float*>(base + Cfg::kSmFrac);
   if (tid < 128) frac[tid] = (float)tid / (float)S;
@@ -253,10 +289,10 @@ render_backward_pipe(const nfi_render_params p, const nfi_render_grads g,
   }
   __syncthreads();
   if (tid == 0) {
-    tc::mbar_expect_tx(&wbar[0], kWiBytes);
-    tc::tma_bulk_g2s(base, wimg, kWiBytes, &wbar[0]);
-    tc::mbar_expect_tx(&wbar[1], kWbBytes);
-    tc::tma_bulk_g2s(base + Cfg::kSmWb, wimg + 32768, kWbBytes, &wbar[1]);
+    tc::mbar_expect_tx(&wbar[0], kImgBytes);
+    tc::tma_bulk_g2s(base, wimg, kImgBytes, &wbar[0]);
+    tc::mbar_expect_tx(&wbar[1], kBwdImgBytes);
+    tc::tma_bulk_g2s(base + Cfg::kSmWb, wimg + kBwdImgOff, kBwdImgBytes, &wbar[1]);
   }
   tc::mbar_wait(&wbar[0], 0);
   tc::mbar_wait(&wbar[1], 0);
@@ -303,10 +339,14 @@ render_backward_pipe(const nfi_render_params p, const nfi_render_grads g,
       auto gather_step = [&](int i, const ByteTaps& tp) {
         const uint32_t m = n0 + (uint32_t)i;
         const uint32_t st = m % NS, u = m / NS;
-        unsigned char* const stage = base + Cfg::kSmA + st * kPipeStageBytes;
+        unsigned char* const stage = base + Cfg::kSmA + st * Cfg::kStageBytes;
         NFI_STEP_WAIT(&a_free[st], (u & 1) ^ 1);
-        gather_to_tiles_lean(planes_b, R, tp, stage, stage + 16384, 32 * wig, lane);
-        tc::fence_async_smem();
+        if constexpr (VD) {  // fp32 stage, read with generic loads only
+          gather_to_tiles_lean<TileStore::kFp32>(planes_b, R, tp, stage, nullptr, 32 * wig, lane);
+        } else {
+          gather_to_tiles_lean(planes_b, R, tp, stage, stage + 16384, 32 * wig, lane);
+          tc::fence_async_smem();
+        }
         __syncwarp();
         if (lane == 0) mbar_arrive(&full[st]);
       };
@@ -467,6 +507,190 @@ render_backward_pipe(const nfi_render_params p, const nfi_render_grads g,
     // ================================ ACTIVATION: the four GEMMs ================================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(Cfg::kActRegs));
     const uint32_t base_s = tc::smem_u32(base);
+    if constexpr (VD) {
+    // Per step: fwd = the forward kernel's view-conditioned decoder (decoder_step_vd) from the
+    // fp32 stage, which stays resident, keeping the leaky ReLU's branches (one bit per element,
+    // 32 per thread); bwd, per 64-row half: D1 again from the stage, dG = dOut W3 (column 0 of W3
+    // is zero: the distance's gradient does not leak in), dF = dG * (1 or 0.2) by the kept
+    // branches, added to the ray's view-gradient sum, D3 = dF W2[1..32] + dDist W2[0], then dpre
+    // and D4 as the plain kernel.
+    const uint64_t w1_hi = tc::gmma_desc_sw128(base_s + kVdW1Hi);
+    const uint64_t w1_lo = tc::gmma_desc_sw128(base_s + kVdW1Lo);
+    const uint64_t w2_hi = tc::gmma_desc_sw128(base_s + kVdW2Hi);
+    const uint64_t w2_lo = tc::gmma_desc_sw128(base_s + kVdW2Lo);
+    const uint64_t w3_hi = tc::gmma_desc_sw128(base_s + kVdW3Hi);
+    const uint64_t w3_lo = tc::gmma_desc_sw128(base_s + kVdW3Lo);
+    const uint64_t g3_hi = tc::gmma_desc_sw128(base_s + Cfg::kSmWb + kVbW3Hi);
+    const uint64_t g3_lo = tc::gmma_desc_sw128(base_s + Cfg::kSmWb + kVbW3Lo);
+    const uint64_t b3_hi = tc::gmma_desc_sw128(base_s + Cfg::kSmWb + kVbW2tHi);
+    const uint64_t b3_lo = tc::gmma_desc_sw128(base_s + Cfg::kSmWb + kVbW2tLo);
+    const uint64_t b4_hi = tc::gmma_desc_sw128(base_s + Cfg::kSmWb + kVbW1tHi);
+    const uint64_t b4_lo = tc::gmma_desc_sw128(base_s + Cfg::kSmWb + kVbW1tLo);
+    const float* w2d = reinterpret_cast<const float*>(base + Cfg::kSmWb + kVbW2d);
+    const float* b2f = reinterpret_cast<const float*>(base + kVdB2f);
+    float4* vt = reinterpret_cast<float4*>(base + Cfg::kSmView) + gt;  // view tile (+ b2[1..32])
+    float4* vg = reinterpret_cast<float4*>(base + Cfg::kSmVg) + gt;    // view-gradient sums
+    const bool vgrad = g.grad_view_features != nullptr;
+    const int t = lane & 3, gq = lane >> 2;
+    auto clear_sums = [&]() {
+      if (vgrad)
+#pragma unroll
+        for (int i = 0; i < 8; ++i) vg[i * kThreads] = make_float4(0.f, 0.f, 0.f, 0.f);
+    };
+    // the tile's sums -> grad_view_features (overwritten; rows outside the image skipped: they
+    // carry the edge ray's view features but not its gradient)
+    auto flush_sums = [&](int tile) {
+      if (!vgrad) return;
+      const TileCoord tcd = tile_coord(tile, tiles_x, tiles_y);
+#pragma unroll
+      for (int mb = 0; mb < 2; ++mb) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = 64 * mb + 16 * wig + gq + 8 * h;
+          int px, py;
+          tile_pixel(tcd.tile_x, tcd.tile_y, row >> 5, row & 31, px, py);
+          if (px >= p.width || py >= p.height) continue;
+          const size_t ray = ((size_t)tcd.b * p.height + py) * p.width + px;
+          float* dst = g.grad_view_features + ray * NFI_VIEW_FEATURES + 2 * t;
+#pragma unroll
+          for (int j = 0; j < NFI_VIEW_FEATURES / 8; ++j) {
+            const float4 s = vg[(mb * 4 + j) * kThreads];
+            *reinterpret_cast<float2*>(dst + 8 * j) = h ? make_float2(s.z, s.w) : make_float2(s.x, s.y);
+          }
+        }
+      }
+    };
+    auto act_fwd = [&](uint32_t m) -> uint32_t {
+      const uint32_t st = m % NS, u = m / NS, sl = m % kBwdSlots;
+      NFI_STEP_WAIT(&full[st], u & 1);
+      const uint32_t neg =
+          decoder_step_vd(base + Cfg::kSmA + st * Cfg::kStageBytes, w1_hi, w1_lo, w2_hi, w2_lo,
+                          w3_hi, w3_lo, b1s, vt, d2s + sl * (kThreads * kD2Ld), wig, lane, []() {});
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&d2_full[sl]);
+      return neg;
+    };
+    auto act_bwd = [&](uint32_t m, uint32_t neg) {
+      const uint32_t st = m % NS, sl = m % kBwdSlots, v = m / kBwdSlots;
+      const unsigned char* stage = base + Cfg::kSmA + st * Cfg::kStageBytes;
+      const float* dout = d2s + sl * (kThreads * kD2Ld);
+      float* d4 = d4s + sl * (kThreads * kD4Ld);
+      NFI_STEP_WAIT(&dout_ready[sl], v & 1);
+      NFI_STEP_WAIT(&slot_free[sl], (v & 1) ^ 1);  // D4 of step m - 2 scattered
+#pragma unroll 1
+      for (int mb = 0; mb < 2; ++mb) {
+        uint32_t a_hi[4][4], a_lo[4][4];
+        {
+          float fa[4][4];
+          tc::load_afrag_sw128(fa, stage, 64 * mb, wig, lane);
+#pragma unroll
+          for (int kb = 0; kb < 4; ++kb)
+#pragma unroll
+            for (int s = 0; s < 4; ++s) tc::put_split(a_hi, a_lo, kb, s, fa[kb][s]);
+        }
+        if (mb == 1) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&a_free[st]);
+        }
+        const float* drows = dout + 64 * mb * kD2Ld;
+        float d[32], dg[16];
+        zero(d);
+        zero(dg);
+        uint32_t ohi[2][4], olo[2][4];
+        load_dout_frags(drows, wig, lane, ohi, olo);
+        tc::wgmma_fence();
+        tc::layer1_mb_rs(d, a_hi, a_lo, w1_hi, w1_lo);
+        mma_dg_mb(dg, ohi, olo, g3_hi, g3_lo);
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::reg_fence(d);
+        tc::reg_fence(dg);
+        // dF by the forward's branches, into the view-gradient sums and the A fragments of D3
+        const uint32_t nb = neg >> (16 * mb);
+        uint32_t fhi[4][4], flo[4][4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          float df[4];
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            df[e] = ((nb >> (4 * j + e)) & 1u) ? dg[4 * j + e] * 0.2f : dg[4 * j + e];
+            tc::put_split(fhi, flo, j, tc::afrag_slot(e), df[e]);
+          }
+          if (vgrad) {
+            float4 s = vg[(mb * 4 + j) * kThreads];
+            s.x += df[0];
+            s.y += df[1];
+            s.z += df[2];
+            s.w += df[3];
+            vg[(mb * 4 + j) * kThreads] = s;
+          }
+        }
+        // D3 starts from the distance row's part, dDist (column 0 of dOut) x w2 row 0
+        float d3[32];
+        {
+          const float dd0 = drows[(16 * wig + gq) * kD2Ld], dd1 = drows[(16 * wig + gq + 8) * kD2Ld];
+#pragma unroll
+          for (int jb = 0; jb < 8; ++jb) {
+            const float2 w = *reinterpret_cast<const float2*>(w2d + 8 * jb + 2 * t);
+            d3[4 * jb + 0] = dd0 * w.x;
+            d3[4 * jb + 1] = dd0 * w.y;
+            d3[4 * jb + 2] = dd1 * w.x;
+            d3[4 * jb + 3] = dd1 * w.y;
+          }
+        }
+        tc::wgmma_fence();
+        mma3_vd_mb(d3, fhi, flo, b3_hi, b3_lo);
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::reg_fence(d3);
+        uint32_t phi[8][4], plo[8][4];
+#pragma unroll
+        for (int kb = 0; kb < 8; ++kb) {
+          const float2 bb = *reinterpret_cast<const float2*>(b1s + 8 * kb + 2 * t);
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const float h = tc::softplus_mufu<true>(d[4 * kb + e] + ((e & 1) ? bb.y : bb.x));
+            const float sg = 1.f - tc::ex2_approx(-h * kLog2e);
+            tc::put_split(phi, plo, kb, tc::afrag_slot(e), d3[4 * kb + e] * sg);
+          }
+        }
+        float d4v[16];
+        zero(d4v);
+        tc::wgmma_fence();
+        mma4_mb(d4v, phi, plo, b4_hi, b4_lo);
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::reg_fence(d4v);
+        tc::store_frag_rows(d4v, d4 + 64 * mb * kD4Ld, kD4Ld, wig, lane);
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&d4_full[sl]);
+    };
+    // step m belongs to the CTA's tile m / n_total: its view tile is filled before the tile's
+    // first fwd, its sums written after the tile's last bwd (the fwd of the next tile's first
+    // step comes in between and only reads the view tile)
+    clear_sums();
+    uint32_t neg_cur = 0, neg_nxt = 0;
+    if (total_steps > 0) {
+      fill_view_tile(p, tile_coord(blockIdx.x, tiles_x, tiles_y), b2f, vt, wig, lane);
+      neg_cur = act_fwd(0);
+    }
+    for (uint32_t m = 0; m < total_steps; ++m) {
+      const int tile = (int)blockIdx.x + (int)(m / (uint32_t)n_total) * (int)gridDim.x;
+      const bool last = (m + 1) % (uint32_t)n_total == 0;
+      if (m + 1 < total_steps) {
+        if (last)
+          fill_view_tile(p, tile_coord(tile + (int)gridDim.x, tiles_x, tiles_y), b2f, vt, wig, lane);
+        neg_nxt = act_fwd(m + 1);
+      }
+      act_bwd(m, neg_cur);
+      neg_cur = neg_nxt;
+      if (last) {
+        flush_sums(tile);
+        clear_sums();
+      }
+    }
+    } else {
     const uint64_t w1_hi = tc::gmma_desc_sw128(base_s + kWiW1Hi);
     const uint64_t w1_lo = tc::gmma_desc_sw128(base_s + kWiW1Lo);
     const uint64_t w2_hi = tc::gmma_desc_sw128(base_s + kWiW2Hi);
@@ -540,6 +764,7 @@ render_backward_pipe(const nfi_render_params p, const nfi_render_grads g,
     for (uint32_t m = 0; m < total_steps; ++m) {
       if (m + 1 < total_steps) act_fwd(m + 1);
       act_bwd(m);
+    }
     }
   } else {
     // ================================ SHADING (forward and reverse) ================================

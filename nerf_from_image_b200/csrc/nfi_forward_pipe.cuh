@@ -252,10 +252,13 @@ __device__ __forceinline__ void fill_view_tile(const nfi_render_params& p, const
 // the register A fragments of layer 3 (12 wgmma), and the D2 row [distance, logits] to `d2`.
 // Both accumulators start from zero and the fp32 terms (view features, biases, the distance) are
 // added on the CUDA cores, as the plain kernel adds b2: the tensor core only sums products.
-__device__ __forceinline__ void decoder_layers23_vd(const float (&d)[32], uint64_t w2_hi,
-                                                    uint64_t w2_lo, uint64_t w3_hi, uint64_t w3_lo,
-                                                    const float* __restrict__ b1, const float4* vt,
-                                                    float* d2, int warp, int lane) {
+// Returns the leaky ReLU's branches: bit 4j + e set where element 4j + e of the accumulator took
+// the 0.2 slope (the backward kernel replays them; the forward ignores the value).
+__device__ __forceinline__ uint32_t decoder_layers23_vd(const float (&d)[32], uint64_t w2_hi,
+                                                        uint64_t w2_lo, uint64_t w3_hi,
+                                                        uint64_t w3_lo, const float* __restrict__ b1,
+                                                        const float4* vt, float* d2, int warp,
+                                                        int lane) {
   uint32_t hi[8][4], lo[8][4];
   tc::softplus_frag<true>(d, b1, lane & 3, hi, lo);
   float o[20];
@@ -267,6 +270,7 @@ __device__ __forceinline__ void decoder_layers23_vd(const float (&d)[32], uint64
   tc::wgmma_wait<0>();
   tc::reg_fence(o);
   uint32_t yhi[4][4], ylo[4][4];
+  uint32_t neg = 0;
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     const float4 v = vt[j * kThreads];
@@ -275,6 +279,7 @@ __device__ __forceinline__ void decoder_layers23_vd(const float (&d)[32], uint64
     for (int e = 0; e < 4; ++e) {
       const float z = o[4 * j + e] + ve[e];
       tc::put_split(yhi, ylo, j, tc::afrag_slot(e), z > 0.f ? z : z * 0.2f);
+      neg |= (z > 0.f ? 0u : 1u) << (4 * j + e);
     }
   }
   float q[8];
@@ -292,11 +297,13 @@ __device__ __forceinline__ void decoder_layers23_vd(const float (&d)[32], uint64
     q[2] = o[18];
   }
   tc::store_frag_rows(q, d2, kD2Ld, warp, lane);
+  return neg;
 }
 
-// decoder_step_fp32 with the view-conditioned layers 2 and 3; `vt` = this thread's view tile
+// decoder_step_fp32 with the view-conditioned layers 2 and 3; `vt` = this thread's view tile.
+// Returns the leaky ReLU branches of both halves (decoder_layers23_vd; half mb at bit 16 mb).
 template <typename F>
-__device__ __forceinline__ void decoder_step_vd(const unsigned char* stage, uint64_t w1_hi,
+__device__ __forceinline__ uint32_t decoder_step_vd(const unsigned char* stage, uint64_t w1_hi,
                                                 uint64_t w1_lo, uint64_t w2_hi, uint64_t w2_lo,
                                                 uint64_t w3_hi, uint64_t w3_lo,
                                                 const float* __restrict__ b1, const float4* vt,
@@ -305,6 +312,7 @@ __device__ __forceinline__ void decoder_step_vd(const unsigned char* stage, uint
   tc::load_afrag_sw128(fa, stage, 0, warp, lane);
   tc::load_afrag_sw128(fb, stage, 64, warp, lane);
   on_stage_read();
+  uint32_t neg = 0;
 #pragma unroll 1
   for (int mb = 0; mb < 2; ++mb) {
     uint32_t a_hi[4][4], a_lo[4][4];
@@ -320,13 +328,15 @@ __device__ __forceinline__ void decoder_step_vd(const unsigned char* stage, uint
     tc::wgmma_commit();
     tc::wgmma_wait<0>();
     tc::reg_fence(d);
-    decoder_layers23_vd(d, w2_hi, w2_lo, w3_hi, w3_lo, b1, vt + mb * 4 * kThreads,
-                        d2 + 64 * mb * kD2Ld, warp, lane);
+    neg |= decoder_layers23_vd(d, w2_hi, w2_lo, w3_hi, w3_lo, b1, vt + mb * 4 * kThreads,
+                               d2 + 64 * mb * kD2Ld, warp, lane)
+           << (16 * mb);
 #pragma unroll
     for (int kb = 0; kb < 4; ++kb)
 #pragma unroll
       for (int s = 0; s < 4; ++s) fa[kb][s] = fb[kb][s];
   }
+  return neg;
 }
 
 __device__ __forceinline__ float ldcg(const float* p) {

@@ -1,7 +1,8 @@
 // Operand layouts of the tensor-core kernels as plain index arithmetic, compilable by a host
 // C++ compiler without the CUDA toolkit (tests/c/vd_image_check.cpp runs them on the CPU):
-// the SWIZZLE_128B tile offset, the K permutation of a register A fragment, and the weight image
-// of the view-direction-conditioned forward kernel (render_forward_pipe<..., VD = true>).
+// the SWIZZLE_128B tile offset, the K permutation of a register A fragment, and the weight images
+// of the view-direction-conditioned kernels (render_forward_pipe / render_backward_pipe<...,
+// VD = true>; tests/c/vd_bwd_image_check.cpp runs the backward one).
 #pragma once
 #include <stdint.h>
 #include <string.h>
@@ -116,6 +117,74 @@ NFI_HD void vd_weight_image_fill(const float* w1, const float* b1, const float* 
   for (int i = idx; i < 32; i += n) b2f[i] = b2[1 + i];
   for (int i = idx; i < 16; i += n)
     head[i] = i == 0 ? b2[0] : (i <= nlogit ? b3[i - 1] * scale3 : pad);
+}
+
+// ---------------------------------------------------------------------------
+// Backward weight image of the view-conditioned decoder (render_backward_pipe<..., VD = true>),
+// loaded beside the forward image above.  All weights in natural units (no log2 e): the shading
+// warpgroup's dOut is the derivative with respect to the natural-units outputs.
+//   W1^T / 3  [32 rows = channel c][64 K = hidden j] as two [32 x 32] K-blocks (4 KB each), K
+//             positions in fragment order: D4 = dpre (W1 / 3), dpre a register A fragment
+//   W2f^T     [64 rows = hidden j][32 K = feature c], K in fragment order: D3 = dF W2[1..32],
+//             dF (the layer-3 reverse accumulator) a register A fragment
+//   W3^T      [32 rows = feature c][32 K = output o, 16 used]: dG = dOut W3, dOut loaded from
+//             shared memory in natural K order; K position 0 (the distance) has zero weights,
+//             K position 1 + a is w3 row a
+//   w2d       w2 row 0 (the distance row) in fp32: its part of D3, dDist w2d, is added on the
+//             CUDA cores
+// Each operand block is a multiple of 1 KB (SWIZZLE_128B atoms); hi / lo TF32 parts.
+// ---------------------------------------------------------------------------
+constexpr int kVbW1tHi = 0;
+constexpr int kVbW1tLo = 8192;
+constexpr int kVbW2tHi = 16384;  // [64 x 32] SW128, 8 KB
+constexpr int kVbW2tLo = 24576;
+constexpr int kVbW3Hi = 32768;   // [32 x 32] SW128, 4 KB
+constexpr int kVbW3Lo = 36864;
+constexpr int kVbW2d = 40960;    // 64 floats
+constexpr int kVbBytes = kVbW2d + 256;  // 41216
+static_assert(kVbBytes % 16 == 0, "bulk-copy size");
+// the backward's workspace: forward image in [0, 48 KiB), backward image in [48 KiB, 96 KiB)
+// (NFI_VIEW_BACKWARD_WORKSPACE_BYTES)
+constexpr int kVdBwdImageOffset = 49152;
+constexpr int kVdBackwardWorkspaceBytes = 2 * kVdBwdImageOffset;
+static_assert(kVdBytes <= kVdBwdImageOffset && kVbBytes <= kVdBwdImageOffset,
+              "a weight image overflows its workspace slot");
+
+// byte offset, inside a W1^T / 3 hi / lo block, of (channel c, hidden unit j)
+NFI_HD uint32_t vb_w1t_offset(int c, int j) {
+  const int jp = tc::kpos_of_hidden(j);
+  return (uint32_t)((jp >> 5) * 4096) + tc::sw128_offset(c, (jp & 31) >> 2) +
+         (uint32_t)(jp & 3) * 4u;
+}
+// byte offset, inside a W2f^T hi / lo block, of (hidden unit j, feature c)
+NFI_HD uint32_t vb_w2t_offset(int j, int c) {
+  const int cp = tc::kpos_of_hidden(c);
+  return tc::sw128_offset(j, cp >> 2) + (uint32_t)(cp & 3) * 4u;
+}
+// byte offset, inside a W3^T hi / lo block, of (feature c, output o)
+NFI_HD uint32_t vb_w3t_offset(int c, int o) {
+  return tc::sw128_offset(c, o >> 2) + (uint32_t)(o & 3) * 4u;
+}
+
+// Worker `idx` of `n` fills its share of the backward image (w2 [33 x 64], w3 [A or 3 x 32]).
+NFI_HD void vd_bwd_weight_image_fill(const float* w1, const float* w2, const float* w3,
+                                     int n_attention, unsigned char* img, int idx, int n) {
+  const int nlogit = n_attention > 0 ? n_attention : 3;
+  for (int i = idx; i < 32 * 64; i += n) {
+    const int c = i / 64, j = i % 64;
+    vd_put_split(img, kVbW1tHi, kVbW1tLo, vb_w1t_offset(c, j), w1[j * 32 + c] * (1.f / 3.f));
+  }
+  for (int i = idx; i < 64 * 32; i += n) {
+    const int j = i / 32, c = i % 32;
+    vd_put_split(img, kVbW2tHi, kVbW2tLo, vb_w2t_offset(j, c), w2[(c + 1) * 64 + j]);
+  }
+  for (int i = idx; i < 32 * 32; i += n) {
+    const int c = i / 32, o = i % 32;
+    const float w = (o >= 1 && o <= nlogit) ? w3[(o - 1) * 32 + c] : 0.f;
+    vd_put_split(img, kVbW3Hi, kVbW3Lo, vb_w3t_offset(c, o), w);
+  }
+  float* w2d = reinterpret_cast<float*>(img + kVbW2d);
+  for (int i = idx; i < 64; i += n) w2d[i] = w2[i];
 }
 
 }  // namespace nfi

@@ -42,4 +42,10 @@ int launch_pipe_weight_image_vd(const nfi_render_params& p, unsigned char* wimg,
 int launch_pipe_forward_vd(const nfi_render_params& p, int nout_pad, const unsigned char* wimg,
                            float* scratch, unsigned grid, cudaStream_t st, char* err,
                            size_t err_len);
+// Its backward with a frozen decoder and mapper output (no grad_w1 .. grad_b3):
+// render_backward_pipe<..., VD = true> and both weight images (kVdBackwardWorkspaceBytes at
+// `wimg`, nfi_layout.h).
+int launch_pipe_backward_vd(const nfi_render_params& p, const nfi_render_grads& g, int nout_pad,
+                            unsigned char* wimg, unsigned grid, cudaStream_t st, char* err,
+                            size_t err_len);
 }  // namespace nfi

@@ -471,17 +471,27 @@ int nfi_render_backward(const nfi_render_params* params, const nfi_render_grads*
   // setting, run.py:628-629), no semantics output, S within the pipelined kernels' envelope,
   // and a workspace for the two weight images.  Everything else: render_backward_simt.
   const int mode = p.mlp_mode & 0xff;
-  if (p.view_features)
+  const bool wgrad = g.grad_w1 || g.grad_b1 || g.grad_w2 || g.grad_b2;
+  const bool tc_env_any = mode != NFI_MLP_FP32_SIMT && p.extra_mode != NFI_EXTRA_SEMANTICS &&
+                          p.num_samples <= 128 && p.num_samples % 4 == 0 &&
+                          p.workspace != nullptr && (!p.fine_sampling || p.z_fine != nullptr) &&
+                          g.out_rgb && g.out_mask && (!g.g_extra || g.out_extra) &&
+                          ((g.grad_origins == nullptr) == (g.grad_dirs == nullptr));
+  if (p.view_features) {
+    // the inversion step of a view-conditioned model (decoder and mapper frozen):
+    // render_backward_pipe<..., VD> (nfi_pipe_vd.cu); its GAN step stays on the SIMT kernel
+    if (tc_env_any && !wgrad && !g.grad_w3 && !g.grad_b3 &&
+        p.workspace_bytes >= (size_t)NFI_VIEW_BACKWARD_WORKSPACE_BYTES) {
+      unsigned grid = 0;
+      if (int rc = persistent_grid(p, &grid)) return rc;
+      return nfi::launch_pipe_backward_vd(p, g, nout_pad_of(params), (unsigned char*)p.workspace,
+                                          grid, st, g_err, sizeof(g_err));
+    }
     return nfi::launch_backward_viewdir(p, g, nout_pad_of(params), st, g_err, sizeof(g_err));
+  }
   if (g.grad_view_features || g.grad_w3 || g.grad_b3)
     return fail("grad_view_features / grad_w3 / grad_b3 need params->view_features");
-  const bool wgrad = g.grad_w1 || g.grad_b1 || g.grad_w2 || g.grad_b2;
-  const bool tc_env = mode != NFI_MLP_FP32_SIMT && p.extra_mode != NFI_EXTRA_SEMANTICS &&
-                      p.num_samples <= 128 && p.num_samples % 4 == 0 && p.workspace != nullptr &&
-                      p.workspace_bytes >= kBackwardWorkspaceBytes &&
-                      (!p.fine_sampling || p.z_fine != nullptr) && g.out_rgb && g.out_mask &&
-                      (!g.g_extra || g.out_extra) &&
-                      ((g.grad_origins == nullptr) == (g.grad_dirs == nullptr));
+  const bool tc_env = tc_env_any && p.workspace_bytes >= kBackwardWorkspaceBytes;
   // decoder-weight gradients (the GAN generator step, run.py:1044) on the tensor cores too: a second
   // kernel (render_wgrad_pipe) beside render_backward_pipe, which then sees a frozen decoder.
   // An upstream gradient of the coords output stays on the SIMT kernel.

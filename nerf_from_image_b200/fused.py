@@ -343,9 +343,13 @@ class FusedTriplaneRender(torch.autograd.Function):
             if DEBUG_RAY is not None and DEBUG_BUF is not None:
                 p.normals, p.noise_seed = _ptr(DEBUG_BUF), int(DEBUG_RAY)
                 p.mlp_mode = cfg.mlp_mode | 0x4000
-            # the tensor-core backward keeps its two weight images here (64 KiB), the
+            # the tensor-core backward keeps its two weight images here (64 KiB; 96 KiB for a
+            # view-conditioned decoder, whose weight gradients stay on the SIMT kernel), the
             # weight-gradient kernel one accumulator row buffer per CTA behind them
-            ws_bytes = _lib.BACKWARD_WORKSPACE_BYTES if (n_w1 or n_b1 or n_w2 or n_b2) else 65536
+            if vd:
+                ws_bytes = _lib.VIEW_BACKWARD_WORKSPACE_BYTES
+            else:
+                ws_bytes = _lib.BACKWARD_WORKSPACE_BYTES if (n_w1 or n_b1 or n_w2 or n_b2) else 65536
             ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
             p.workspace, p.workspace_bytes = _ptr(ws), ws_bytes
             _lib.check(lib.nfi_render_backward(ctypes.byref(p), ctypes.byref(g), stream))
@@ -399,8 +403,9 @@ def fused_render(planes, w1, b1, w2, b2, palette, beta, alpha, c2w, focal,
     ``peers``: list of (rgb, depth, mask) device ADDRESSES of this rank's slices in the other
     ranks' buffers; the kernel stores its tiles there too (parallel.PeerExchange).
     ``view``: (view_features [B,H,W,32], w3 [A,32], b3 [A]) switches on the view-direction
-    conditioning of the CARLA models (--use_viewdir; the forward on the pipelined tensor-core
-    kernel where it can take the configuration, the backward on the fp32 SIMT kernel).
+    conditioning of the CARLA models (--use_viewdir; the forward, and the backward with frozen
+    decoder and mapper output, on the pipelined tensor-core kernels where they can take the
+    configuration, the GAN step's decoder / mapper-output gradients on the fp32 SIMT kernel).
     ``rows``: (row_offset, full_height) renders rows [row_offset, row_offset + height) of images
     full_height rows tall; every per-ray tensor (noise, outputs) then has ``height`` rows.
 
