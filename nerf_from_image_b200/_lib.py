@@ -18,6 +18,7 @@ LIB_PATH = os.environ.get('NFI_LIB_PATH') or os.path.join(_HERE, 'csrc', 'libnfi
 c_float_p = ctypes.POINTER(ctypes.c_float)
 ABI_VERSION = 5  # NFI_ABI_VERSION of include/nfi_render.h
 MAX_PEERS = 7
+BACKWARD_IMAGES_BYTES = 65536  # the two weight images of a frozen-decoder backward (nfi_layout.h)
 BACKWARD_WORKSPACE_BYTES = 65536 + 160 * 32768  # NFI_BACKWARD_WORKSPACE_BYTES
 VIEW_BACKWARD_WORKSPACE_BYTES = 98304  # NFI_VIEW_BACKWARD_WORKSPACE_BYTES
 

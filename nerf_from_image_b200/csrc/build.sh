@@ -1,12 +1,12 @@
 #!/bin/bash
 # Builds libnfi_render.so in-tree for sm_90a (cross-compiles without a GPU).
-# Seven translation units compiled in parallel: the pipelined tensor-core kernels (nfi_pipe.cu),
-# the view-direction-conditioned instantiations of the pipelined forward and backward kernels
-# (nfi_pipe_vd.cu),
-# the sampler seam and pose kernels (nfi_field.cu), the synthesis network (nfi_synth.cu), the
-# regulariser-head point evaluator (nfi_heads.cu), the view-direction-conditioned SIMT kernels
-# (nfi_viewdir.cu), and everything else (nfi_render.cu: C ABI,
-# re-layout, SIMT kernels, stand-alone decoder).  nfi_render.cu and nfi_viewdir.cu take
+# Seven translation units compiled in parallel: the pipelined tensor-core kernels (nfi_pipe.cu) and
+# their view-direction-conditioned instantiations (nfi_pipe_vd.cu), both on the launchers of
+# nfi_pipe_ladder.cuh; the sampler seam and pose kernels (nfi_field.cu), the synthesis network
+# (nfi_synth.cu), the regulariser-head point evaluator (nfi_heads.cu), the view-direction-
+# conditioned instantiations of the SIMT launchers (nfi_viewdir.cu), and everything else
+# (nfi_render.cu: C ABI and routing, re-layout, plain SIMT kernels, stand-alone decoder).  Each
+# kernel is compiled only in the unit that launches it.  nfi_render.cu and nfi_viewdir.cu take
 # --split-compile 0 (their many kernels are optimised in parallel).
 set -e
 cd "$(dirname "$0")"

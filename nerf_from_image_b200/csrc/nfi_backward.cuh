@@ -25,7 +25,7 @@
 //            chains them to tform_cam2world / focal with tiny torch ops).
 #pragma once
 #include "nfi_common.cuh"
-#include "nfi_forward.cuh"  // kViewMlpPad
+#include "nfi_forward.cuh"  // kViewMlpPad, num_tiles
 
 namespace nfi {
 
@@ -646,49 +646,37 @@ render_backward_simt(const nfi_render_params p, const nfi_render_grads g) {
   }
 }
 
-inline int launch_backward(const nfi_render_params& p, const nfi_render_grads& g,
-                           cudaStream_t st, char* err, size_t err_len) {
-  if (p.fine_sampling && p.z_fine == nullptr) {
-    snprintf(err, err_len, "backward needs the z_fine buffer the forward pass filled");
-    return 1;
-  }
-  if (!g.out_rgb || !g.out_mask) {
-    snprintf(err, err_len, "backward needs the forward outputs (out_rgb, out_mask)");
-    return 1;
-  }
-  if (g.g_extra && !g.out_extra) {
-    snprintf(err, err_len, "g_extra given without out_extra");
-    return 1;
-  }
-  if ((g.grad_origins == nullptr) != (g.grad_dirs == nullptr)) {
-    snprintf(err, err_len, "grad_origins and grad_dirs must be given together");
-    return 1;
-  }
-  const int nout = 1 + (p.n_attention > 0 ? p.n_attention : 3);
-  const int np = nout <= 4 ? 4 : (nout <= 12 ? 12 : 16);
-  const bool wgrad = g.grad_w1 || g.grad_b1 || g.grad_w2 || g.grad_b2;
-  const size_t smem = bwd_smem_floats(np, wgrad) * sizeof(float);
-  const size_t tx = (p.width + kTileW - 1) / kTileW, ty = (p.height + kTileH - 1) / kTileH;
-  const unsigned grid = (unsigned)(tx * ty * (size_t)p.batch);
-  cudaError_t e = cudaSuccess;
-#define NFI_LAUNCH_BWD(NP, WG)                                                              \
-  do {                                                                                      \
-    e = cudaFuncSetAttribute(render_backward_simt<NP, WG>,                                  \
-                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);       \
-    if (e == cudaSuccess) {                                                                 \
-      render_backward_simt<NP, WG><<<grid, kThreads, smem, st>>>(p, g);                     \
-      e = cudaGetLastError();                                                               \
-    }                                                                                       \
-  } while (0)
-  if (np == 4) { if (wgrad) NFI_LAUNCH_BWD(4, true); else NFI_LAUNCH_BWD(4, false); }
-  else if (np == 12) { if (wgrad) NFI_LAUNCH_BWD(12, true); else NFI_LAUNCH_BWD(12, false); }
-  else { if (wgrad) NFI_LAUNCH_BWD(16, true); else NFI_LAUNCH_BWD(16, false); }
-#undef NFI_LAUNCH_BWD
-  if (e != cudaSuccess) {
-    snprintf(err, err_len, "backward launch failed: %s", cudaGetErrorString(e));
-    return 2;
-  }
+namespace simt {
+
+template <int NP, bool WG, bool VD>
+int launch_bwd(const nfi_render_params& p, const nfi_render_grads& g, cudaStream_t st, char* err,
+               size_t err_len) {
+  const size_t smem = bwd_smem_floats(NP, WG, VD) * sizeof(float);
+  auto k = render_backward_simt<NP, WG, VD>;
+  NFI_LAUNCH_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k<<<(unsigned)num_tiles(p), kThreads, smem, st>>>(p, g);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
   return 0;
 }
+
+}  // namespace simt
+
+// render_backward_simt, for arguments nfi_render_backward has checked.  nfi_render.cu instantiates
+// it for VD = false, nfi_viewdir.cu for VD = true.
+template <bool VD>
+int launch_backward_simt(const nfi_render_params& p, const nfi_render_grads& g, cudaStream_t st,
+                         char* err, size_t err_len) {
+  const bool wg = g.grad_w1 || g.grad_b1 || g.grad_w2 || g.grad_b2 || g.grad_w3 || g.grad_b3;
+  switch (nout_pad_of(p.n_attention)) {
+    case 4: return wg ? simt::launch_bwd<4, true, VD>(p, g, st, err, err_len)
+                      : simt::launch_bwd<4, false, VD>(p, g, st, err, err_len);
+    case 12: return wg ? simt::launch_bwd<12, true, VD>(p, g, st, err, err_len)
+                       : simt::launch_bwd<12, false, VD>(p, g, st, err, err_len);
+    default: return wg ? simt::launch_bwd<16, true, VD>(p, g, st, err, err_len)
+                       : simt::launch_bwd<16, false, VD>(p, g, st, err, err_len);
+  }
+}
+extern template int launch_backward_simt<true>(const nfi_render_params&, const nfi_render_grads&,
+                                               cudaStream_t, char*, size_t);
 
 }  // namespace nfi

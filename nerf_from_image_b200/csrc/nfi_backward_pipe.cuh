@@ -26,6 +26,7 @@
 // row of D2 and writes its row of dOut in its place) and D4 ([128 x 36] fp32).
 // Decoder-weight gradients (GAN generator step) are NOT produced here (nfi_wgrad_pipe.cuh).
 #pragma once
+#include "nfi_backward.cuh"  // red_add_v4, warp_sum
 #include "nfi_forward_pipe.cuh"
 
 namespace nfi {
@@ -40,6 +41,7 @@ constexpr int kWbW2tLo = 8192;
 constexpr int kWbW1tHi = 16384;  // [32 rows = channel c][64 k = hidden j] as two [32 x 32] k-blocks
 constexpr int kWbW1tLo = 24576;  //   (K positions in register-fragment order: tc::kpos_of_hidden)
 constexpr int kWbBytes = 32768;
+static_assert(kWbBytes == kBwdImageBytes, "backward weight image and its workspace slot");
 
 // VD: the view-conditioned instantiation.  Its two weight images (nfi_layout.h) are larger, so its
 // stages hold fp32 features (split into TF32 hi / lo in registers, as the forward kernel does)
@@ -69,28 +71,6 @@ struct BwdCfg {
   static constexpr int kActRegs = 144;
   static constexpr int kShadeRegs = 112;
 };
-
-// W2^T (padded to K = 32) and W1^T / 3, split into TF32 hi/lo, K-major SWIZZLE_128B.
-static __global__ void prep_weight_image_bwd(const float* __restrict__ w1, const float* __restrict__ w2,
-                                      int nout, unsigned char* __restrict__ img) {
-  for (int i = threadIdx.x; i < kHid * 32; i += blockDim.x) {
-    const int j = i / 32, o = i % 32;  // B3[j][o] = W2[o][j]
-    const float w = (o < nout) ? w2[o * kHid + j] : 0.f;
-    const float hi = tc::tf32_hi(w);
-    const uint32_t off = tc::sw128_offset(j, o >> 2) + (o & 3) * 4;
-    *reinterpret_cast<float*>(img + kWbW2tHi + off) = hi;
-    *reinterpret_cast<float*>(img + kWbW2tLo + off) = w - hi;
-  }
-  for (int i = threadIdx.x; i < kC * kHid; i += blockDim.x) {
-    const int c = i / kHid, j = i % kHid;  // B4[c][j] = W1[j][c] / 3 (features = mean of 3 planes)
-    const float w = w1[j * kC + c] * (1.f / 3.f);
-    const float hi = tc::tf32_hi(w);
-    const int jp = tc::kpos_of_hidden(j);
-    const uint32_t off = (jp >> 5) * 4096 + tc::sw128_offset(c, (jp & 31) >> 2) + (jp & 3) * 4;
-    *reinterpret_cast<float*>(img + kWbW1tHi + off) = hi;
-    *reinterpret_cast<float*>(img + kWbW1tLo + off) = w - hi;
-  }
-}
 
 // dOut rows of one 64-row block (row-major slot, kD2Ld floats per row) as TF32 hi / lo register
 // A fragments of the two k-blocks of K = 16
@@ -240,7 +220,7 @@ render_backward_pipe(const nfi_render_params p, const nfi_render_grads g,
   using Cfg = BwdCfg<P, VD>;
   constexpr int kImgBytes = VD ? kVdBytes : kWiBytes;
   constexpr int kImgB1 = VD ? kVdB1 : kWiB1, kImgB2 = VD ? kVdHead : kWiB2;
-  constexpr int kBwdImgOff = VD ? kVdBwdImageOffset : 32768;
+  constexpr int kBwdImgOff = VD ? kVdBwdImageOffset : kBwdImageOffset;
   constexpr int kBwdImgBytes = VD ? kVbBytes : kWbBytes;
   constexpr int NA = NOUT_PAD - 1;
   constexpr int NS = kBwdStages;

@@ -15,15 +15,6 @@
 namespace nfi {
 namespace {
 
-#define NFI_FCUDA(expr)                                                              \
-  do {                                                                               \
-    cudaError_t e__ = (expr);                                                        \
-    if (e__ != cudaSuccess) {                                                        \
-      snprintf(err, err_len, "%s failed: %s", #expr, cudaGetErrorString(e__));       \
-      return 2;                                                                      \
-    }                                                                                \
-  } while (0)
-
 // One thread = one point; a warp fetches its 32 points' features cooperatively.  blockIdx.y is
 // the image, blockIdx.x the 128-point chunk.  `p` carries the field (planes, decoder, palette,
 // beta/alpha, scene_range): the same struct the render kernels read, so load_weights_smem and
@@ -124,10 +115,10 @@ int run_sampler(const nfi_render_params& p, const nfi_sample_params& io, cudaStr
                 char* err, size_t err_len) {
   const size_t smem = fwd_smem_floats(NP, 0, false, NORM) * sizeof(float);
   auto k = sample_field_simt<NP, NORM>;
-  NFI_FCUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  NFI_LAUNCH_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const dim3 grid((unsigned)((io.n_points + kThreads - 1) / kThreads), (unsigned)io.batch);
   k<<<grid, kThreads, smem, st>>>(p, io);
-  NFI_FCUDA(cudaGetLastError());
+  NFI_LAUNCH_CHECK(cudaGetLastError());
   return 0;
 }
 
@@ -318,7 +309,7 @@ int launch_pose_to_matrix(const float* z0, const float* t2, const float* s, cons
                           char* err, size_t err_len) {
   pose_to_matrix_kernel<<<(batch + 63) / 64, 64, 0, st>>>(z0, t2, s, q, flipped, batch, c2w,
                                                           focal);
-  NFI_FCUDA(cudaGetLastError());
+  NFI_LAUNCH_CHECK(cudaGetLastError());
   return 0;
 }
 
@@ -328,7 +319,7 @@ int launch_pose_to_matrix_backward(const float* z0, const float* t2, const float
                                    float* g_q, cudaStream_t st, char* err, size_t err_len) {
   pose_to_matrix_bwd_kernel<<<(batch + 63) / 64, 64, 0, st>>>(z0, t2, s, q, flipped, batch, g_c2w,
                                                               g_focal, g_z0, g_t2, g_s, g_q);
-  NFI_FCUDA(cudaGetLastError());
+  NFI_LAUNCH_CHECK(cudaGetLastError());
   return 0;
 }
 

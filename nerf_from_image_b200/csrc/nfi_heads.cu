@@ -368,15 +368,6 @@ sdf_points_bwd_kernel(const nfi_sdf_points_params p, const nfi_sdf_points_grads 
   }
 }
 
-#define NFI_HCUDA(expr)                                                              \
-  do {                                                                               \
-    cudaError_t e__ = (expr);                                                        \
-    if (e__ != cudaSuccess) {                                                        \
-      snprintf(err, err_len, "%s failed: %s", #expr, cudaGetErrorString(e__));       \
-      return 2;                                                                      \
-    }                                                                                \
-  } while (0)
-
 static unsigned grid_for(const nfi_sdf_points_params& p) {
   const long long units = ((p.n_points + 31) / 32) * p.batch;
   long long ctas = (units + kWarps - 1) / kWarps;
@@ -386,20 +377,20 @@ static unsigned grid_for(const nfi_sdf_points_params& p) {
 
 int launch_forward(const nfi_sdf_points_params& p, cudaStream_t st, char* err, size_t err_len) {
   const size_t smem = smem_floats(false) * sizeof(float);
-  NFI_HCUDA(cudaFuncSetAttribute(sdf_points_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  NFI_LAUNCH_CHECK(cudaFuncSetAttribute(sdf_points_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  (int)smem));
   sdf_points_fwd_kernel<<<grid_for(p), kThreads, smem, st>>>(p);
-  NFI_HCUDA(cudaGetLastError());
+  NFI_LAUNCH_CHECK(cudaGetLastError());
   return 0;
 }
 
 int launch_backward(const nfi_sdf_points_params& p, const nfi_sdf_points_grads& g, cudaStream_t st,
                     char* err, size_t err_len) {
   const size_t smem = smem_floats(true) * sizeof(float);
-  NFI_HCUDA(cudaFuncSetAttribute(sdf_points_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  NFI_LAUNCH_CHECK(cudaFuncSetAttribute(sdf_points_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  (int)smem));
   sdf_points_bwd_kernel<<<grid_for(p), kThreads, smem, st>>>(p, g);
-  NFI_HCUDA(cudaGetLastError());
+  NFI_LAUNCH_CHECK(cudaGetLastError());
   return 0;
 }
 

@@ -32,6 +32,30 @@ NFI_HD constexpr int afrag_slot(int e) { return ((e & 1) << 1) | (e >> 1); }
 
 }  // namespace tc
 
+// decoder outputs: the distance and A colour logits (three when A = 0), padded for the kernels
+constexpr int nout_of(int n_attention) { return 1 + (n_attention > 0 ? n_attention : 3); }
+constexpr int nout_pad_of(int n_attention) {
+  return nout_of(n_attention) <= 4 ? 4 : (nout_of(n_attention) <= 12 ? 12 : 16);
+}
+
+// ---------------------------------------------------------------------------
+// Workspace of the render kernels (bytes from params.workspace).
+//   forward   [0, kFwdImageSlot): the weight image (kVdFwdImageSlot with a view), then the
+//             scratch slabs of the coarse samples, then, when render_normals_pipe runs, its
+//             backward weight image (kBwdImageBytes; nfi_render.cu computes the offsets)
+//   backward  the forward image at 0, the backward image at kBwdImageOffset, then from
+//             kWgAccOffset render_wgrad_pipe's accumulator rows, one per CTA of at most
+//             kMaxPersistentCtas (NFI_BACKWARD_WORKSPACE_BYTES); with a view both images take
+//             48 KiB slots (kVdBwdImageOffset below, NFI_VIEW_BACKWARD_WORKSPACE_BYTES)
+// ---------------------------------------------------------------------------
+constexpr int kFwdImageSlot = 32768;    // nfi::kWiBytes rounded up
+constexpr int kVdFwdImageSlot = 65536;  // kVdBytes rounded up
+constexpr int kBwdImageOffset = 32768;
+constexpr int kBwdImageBytes = 32768;   // nfi::kWbBytes
+constexpr int kWgAccOffset = kBwdImageOffset + kBwdImageBytes;
+constexpr size_t kWgAccBytesPerCta = 128 * 64 * sizeof(float);
+constexpr size_t kMaxPersistentCtas = 160;  // >= SM count of any sm_90 part (H100 SXM: 132)
+
 // ---------------------------------------------------------------------------
 // Weight image of the view-direction-conditioned decoder (models/generator.py:189-253,662-663):
 //   layer 1   W1 [64 x 32], b1                       as in the plain image (nfi_forward_tc.cuh)
@@ -59,6 +83,7 @@ constexpr int kVdB2f = kVdB1 + 256;                // 32 floats
 constexpr int kVdHead = kVdB2f + 128;              // 16 floats
 constexpr int kVdBytes = kVdHead + 64;             // 41408
 static_assert(kVdW3Hi % 1024 == 0 && kVdBytes % 16 == 0, "SWIZZLE_128B atoms / bulk-copy size");
+static_assert(kVdBytes <= kVdFwdImageSlot, "weight image larger than the workspace header");
 
 // output column of layer 2 that holds row `row` of w2
 NFI_HD constexpr int vd_w2_col(int row) { return row == 0 ? 32 : row - 1; }

@@ -1,195 +1,121 @@
 // Translation unit of the pipelined tensor-core kernels: forward (nfi_forward_pipe.cuh),
 // backward (nfi_backward_pipe.cuh), surface normals (nfi_normals_pipe.cuh) and decoder-weight
-// gradients (nfi_wgrad_pipe.cuh).
-#include <cuda_runtime.h>
-#include <stdio.h>
-
-#include "nfi_backward.cuh"
-#include "nfi_backward_pipe.cuh"
-#include "nfi_forward_pipe.cuh"
+// gradients (nfi_wgrad_pipe.cuh), with the plain decoder's weight images.
 #include "nfi_normals_pipe.cuh"
-#include "nfi_pipe_launch.h"
+#include "nfi_pipe_ladder.cuh"
+#include "nfi_weight_image.cuh"
 #include "nfi_wgrad_pipe.cuh"
 
 namespace nfi {
-namespace {
 
-#define NFI_PCUDA(expr)                                                              \
-  do {                                                                               \
-    cudaError_t e__ = (expr);                                                        \
-    if (e__ != cudaSuccess) {                                                        \
-      snprintf(err, err_len, "%s failed: %s", #expr, cudaGetErrorString(e__));       \
-      return 2;                                                                      \
-    }                                                                                \
-  } while (0)
-
-// The forward's plane gather runs out of L1, and on Hopper L1 gets what the shared-memory carve-out
-// leaves of 256 KiB.  The carve-out comes in steps (..., 100, 132, 164, 196, 228 KiB); with the
-// 1 KiB the driver reserves per CTA the forward fits the 132 KiB step, which leaves 124 KiB of L1.
-// A kernel that grows past it takes the 164 KiB step and loses a quarter of that L1.
-constexpr int kSmemPerSm = 228 * 1024, kSmemReservedPerCta = 1024;
+// The plain forward fits the 132 KiB carve-out step, which leaves 124 KiB of L1.  A kernel that
+// grows past it takes the 164 KiB step and loses a quarter of that L1.
 static_assert(PipeCfg<3>::kSmBytes + kSmemReservedPerCta <= 132 * 1024,
               "render_forward_pipe no longer fits the 132 KiB carve-out step");
-// the smallest carve-out (percent of kSmemPerSm) that holds the kernel: the driver rounds it up
-// to the next step
-constexpr int kFwdCarveoutPct =
-    ((PipeCfg<3>::kSmBytes + kSmemReservedPerCta) * 100 + kSmemPerSm - 1) / kSmemPerSm;
 
-template <int NP, int EX, bool FINE, bool DBG, int NSLOT>
-int run_fwd(const nfi_render_params& p, const unsigned char* wimg, float* scratch, unsigned grid,
-            cudaStream_t st, char* err, size_t err_len) {
-  auto k = render_forward_pipe<NP, EX, FINE, 3, DBG, NSLOT>;
-  NFI_PCUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 PipeCfg<3>::kSmBytes));
-  NFI_PCUDA(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                 kFwdCarveoutPct));
-  k<<<grid, PipeCfg<3>::kThreadsTotal, PipeCfg<3>::kSmBytes, st>>>(p, wimg, scratch);
-  NFI_PCUDA(cudaGetLastError());
+// W2^T (padded to K = 32) and W1^T / 3, split into TF32 hi/lo, K-major SWIZZLE_128B.
+static __global__ void prep_weight_image_bwd(const float* __restrict__ w1, const float* __restrict__ w2,
+                                      int nout, unsigned char* __restrict__ img) {
+  for (int i = threadIdx.x; i < kHid * 32; i += blockDim.x) {
+    const int j = i / 32, o = i % 32;  // B3[j][o] = W2[o][j]
+    const float w = (o < nout) ? w2[o * kHid + j] : 0.f;
+    const float hi = tc::tf32_hi(w);
+    const uint32_t off = tc::sw128_offset(j, o >> 2) + (o & 3) * 4;
+    *reinterpret_cast<float*>(img + kWbW2tHi + off) = hi;
+    *reinterpret_cast<float*>(img + kWbW2tLo + off) = w - hi;
+  }
+  for (int i = threadIdx.x; i < kC * kHid; i += blockDim.x) {
+    const int c = i / kHid, j = i % kHid;  // B4[c][j] = W1[j][c] / 3 (features = mean of 3 planes)
+    const float w = w1[j * kC + c] * (1.f / 3.f);
+    const float hi = tc::tf32_hi(w);
+    const int jp = tc::kpos_of_hidden(j);
+    const uint32_t off = (jp >> 5) * 4096 + tc::sw128_offset(c, (jp & 31) >> 2) + (jp & 3) * 4;
+    *reinterpret_cast<float*>(img + kWbW1tHi + off) = hi;
+    *reinterpret_cast<float*>(img + kWbW1tLo + off) = w - hi;
+  }
+}
+
+// log2 e goes into layer 1 and the colour rows of layer 2; padded logits at -1e30
+template <>
+int prep_weight_images<false>(const nfi_render_params& p, unsigned char* wimg, bool bwd,
+                              cudaStream_t st, char* err, size_t err_len) {
+  const int nout = nout_of(p.n_attention);
+  const bool att = p.n_attention > 0;
+  prep_weight_image<<<1, 256, 0, st>>>(p.w1, p.b1, p.w2, p.b2, nout, wimg, kLog2e,
+                                       att ? kPadLogit : 0.f, att ? kLog2e : 1.f);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  if (bwd) {
+    prep_weight_image_bwd<<<1, 256, 0, st>>>(p.w1, p.w2, nout, wimg + kBwdImageOffset);
+    NFI_LAUNCH_CHECK(cudaGetLastError());
+  }
   return 0;
 }
 
-template <int NP, int EX>
-int fwd_np_ex(const nfi_render_params& p, const unsigned char* wimg, float* scratch, unsigned grid,
-              cudaStream_t st, char* err, size_t err_len) {
-  if constexpr (NP == 12 && EX == 0) {
-    if ((p.mlp_mode & 0x1000) && p.fine_sampling)  // phase-timer build (tools/phase_times_pipe.py)
-      return run_fwd<NP, EX, true, true, 2>(p, wimg, scratch, grid, st, err, err_len);
-  }
-  if (p.fine_sampling && p.num_samples > 64)  // 4 resampling slots per lane (S <= 128)
-    return run_fwd<NP, EX, true, false, 4>(p, wimg, scratch, grid, st, err, err_len);
-  if (p.fine_sampling) return run_fwd<NP, EX, true, false, 2>(p, wimg, scratch, grid, st, err, err_len);
-  return run_fwd<NP, EX, false, false, 2>(p, wimg, scratch, grid, st, err, err_len);
-}
+template int launch_pipe_forward<false>(const nfi_render_params&, unsigned char*, float*, unsigned, cudaStream_t, char*, size_t);
+template int launch_pipe_backward<false>(const nfi_render_params&, const nfi_render_grads&, unsigned char*, unsigned, cudaStream_t,
+                                         char*, size_t);
 
-template <int NP>
-int fwd_np(const nfi_render_params& p, const unsigned char* wimg, float* scratch, unsigned grid,
-           cudaStream_t st, char* err, size_t err_len) {
-  if (p.extra_mode == NFI_EXTRA_COORDS)
-    return fwd_np_ex<NP, 1>(p, wimg, scratch, grid, st, err, err_len);
-  if constexpr (NP > 4) {
-    if (p.extra_mode == NFI_EXTRA_SEMANTICS)
-      return fwd_np_ex<NP, 2>(p, wimg, scratch, grid, st, err, err_len);
-  }
-  return fwd_np_ex<NP, 0>(p, wimg, scratch, grid, st, err, err_len);
-}
-
-template <int NP, int EX, bool CAM>
-int run_bwd(const nfi_render_params& p, const nfi_render_grads& g, const unsigned char* wimg,
-            unsigned grid, cudaStream_t st, char* err, size_t err_len) {
-  using Cfg = BwdCfg<2>;
-  auto k = render_backward_pipe<NP, EX, CAM, 2>;
-  NFI_PCUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmBytes));
-  k<<<grid, Cfg::kThreadsTotal, Cfg::kSmBytes, st>>>(p, g, wimg);
-  NFI_PCUDA(cudaGetLastError());
-  return 0;
-}
-
-template <int NP>
-int bwd_np(const nfi_render_params& p, const nfi_render_grads& g, const unsigned char* wimg,
-           unsigned grid, cudaStream_t st, char* err, size_t err_len) {
-  const bool cam = g.grad_origins != nullptr;
-  const bool coords = p.extra_mode == NFI_EXTRA_COORDS && g.g_extra != nullptr;
-  if (coords)
-    return cam ? run_bwd<NP, 1, true>(p, g, wimg, grid, st, err, err_len)
-               : run_bwd<NP, 1, false>(p, g, wimg, grid, st, err, err_len);
-  return cam ? run_bwd<NP, 0, true>(p, g, wimg, grid, st, err, err_len)
-             : run_bwd<NP, 0, false>(p, g, wimg, grid, st, err, err_len);
-}
+namespace {
 
 template <int NP, bool PLANES>
-int run_wgrad(const nfi_render_params& p, const nfi_render_grads& g, const unsigned char* wimg,
+int run_wgrad(const nfi_render_params& p, const nfi_render_grads& g, unsigned char* wimg,
               unsigned grid, cudaStream_t st, char* err, size_t err_len) {
   using Cfg = WgCfgT<PLANES>;
   auto k = render_wgrad_pipe<NP, PLANES>;
-  NFI_PCUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmBytes));
-  k<<<grid, Cfg::kThreadsTotal, Cfg::kSmBytes, st>>>(
-      p, g, wimg, reinterpret_cast<float*>(const_cast<unsigned char*>(wimg) + 65536));
-  NFI_PCUDA(cudaGetLastError());
+  NFI_LAUNCH_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        Cfg::kSmBytes));
+  k<<<grid, Cfg::kThreadsTotal, Cfg::kSmBytes, st>>>(p, g, wimg,
+                                                     reinterpret_cast<float*>(wimg + kWgAccOffset));
+  NFI_LAUNCH_CHECK(cudaGetLastError());
   return 0;
 }
 
-}  // namespace
+template <bool PLANES>
+int wgrad_np(const nfi_render_params& p, const nfi_render_grads& g, unsigned char* wimg,
+             unsigned grid, cudaStream_t st, char* err, size_t err_len) {
+  switch (nout_pad_of(p.n_attention)) {
+    case 4: return run_wgrad<4, PLANES>(p, g, wimg, grid, st, err, err_len);
+    case 12: return run_wgrad<12, PLANES>(p, g, wimg, grid, st, err, err_len);
+    default: return run_wgrad<16, PLANES>(p, g, wimg, grid, st, err, err_len);
+  }
+}
 
-size_t pipe_wgrad_workspace_bytes(unsigned grid) { return 65536 + (size_t)grid * kWgAccBytesPerCta; }
+}  // namespace
 
 size_t pipe_scratch_bytes_per_cta(int num_samples, int nes) {
   return pipe_scratch_floats(num_samples, nes) * sizeof(float);
 }
 
-int launch_pipe_weight_image(const nfi_render_params& p, unsigned char* wimg, cudaStream_t st) {
-  const int nout = 1 + (p.n_attention > 0 ? p.n_attention : 3);
-  prep_weight_image<<<1, 256, 0, st>>>(p.w1, p.b1, p.w2, p.b2, nout, wimg, kLog2e,
-                                       p.n_attention > 0 ? kPadLogit : 0.f,
-                                       p.n_attention > 0 ? kLog2e : 1.f);
-  return cudaGetLastError() == cudaSuccess ? 0 : 2;
+int launch_pipe_wgrad(const nfi_render_params& p, const nfi_render_grads& g, unsigned char* wimg,
+                      unsigned grid, bool planes, cudaStream_t st, char* err, size_t err_len) {
+  if (int rc = prep_weight_images<false>(p, wimg, true, st, err, err_len)) return rc;
+  return planes ? wgrad_np<true>(p, g, wimg, grid, st, err, err_len)
+                : wgrad_np<false>(p, g, wimg, grid, st, err, err_len);
 }
 
-int launch_pipe_forward(const nfi_render_params& p, int nout_pad, const unsigned char* wimg,
-                        float* scratch, unsigned grid, cudaStream_t st, char* err,
-                        size_t err_len) {
-  if (nout_pad == 4) return fwd_np<4>(p, wimg, scratch, grid, st, err, err_len);
-  if (nout_pad == 12) return fwd_np<12>(p, wimg, scratch, grid, st, err, err_len);
-  return fwd_np<16>(p, wimg, scratch, grid, st, err, err_len);
-}
-
-int launch_pipe_backward(const nfi_render_params& p, const nfi_render_grads& g, int nout_pad,
-                         unsigned char* wimg, unsigned grid, cudaStream_t st, char* err,
-                         size_t err_len) {
-  const int nout = 1 + (p.n_attention > 0 ? p.n_attention : 3);
-  if (launch_pipe_weight_image(p, wimg, st)) {
-    snprintf(err, err_len, "weight image launch failed");
-    return 2;
-  }
-  prep_weight_image_bwd<<<1, 256, 0, st>>>(p.w1, p.w2, nout, wimg + 32768);
-  NFI_PCUDA(cudaGetLastError());
-  if (nout_pad == 4) return bwd_np<4>(p, g, wimg, grid, st, err, err_len);
-  if (nout_pad == 12) return bwd_np<12>(p, g, wimg, grid, st, err, err_len);
-  return bwd_np<16>(p, g, wimg, grid, st, err, err_len);
-}
-
-// decoder-weight gradients on the tensor cores (nfi_wgrad_pipe.cuh): both weight images +
-// render_wgrad_pipe
-int launch_pipe_wgrad(const nfi_render_params& p, const nfi_render_grads& g, int nout_pad,
-                      unsigned char* wimg, unsigned grid, bool planes, cudaStream_t st, char* err,
-                      size_t err_len) {
-  const int nout = 1 + (p.n_attention > 0 ? p.n_attention : 3);
-  if (launch_pipe_weight_image(p, wimg, st)) {
-    snprintf(err, err_len, "weight image launch failed");
-    return 2;
-  }
-  prep_weight_image_bwd<<<1, 256, 0, st>>>(p.w1, p.w2, nout, wimg + 32768);
-  NFI_PCUDA(cudaGetLastError());
-  if (planes) {
-    if (nout_pad == 4) return run_wgrad<4, true>(p, g, wimg, grid, st, err, err_len);
-    if (nout_pad == 12) return run_wgrad<12, true>(p, g, wimg, grid, st, err, err_len);
-    return run_wgrad<16, true>(p, g, wimg, grid, st, err, err_len);
-  }
-  if (nout_pad == 4) return run_wgrad<4, false>(p, g, wimg, grid, st, err, err_len);
-  if (nout_pad == 12) return run_wgrad<12, false>(p, g, wimg, grid, st, err, err_len);
-  return run_wgrad<16, false>(p, g, wimg, grid, st, err, err_len);
-}
-
-// surface normals after render_forward_pipe (nfi_normals_pipe.cuh): `wimg` = the forward weight
-// image of that launch, `wimg_bwd` = 32 KiB for the backward image (W1^T / 3 is what is used)
-int launch_pipe_normals(const nfi_render_params& p, int nout_pad, const unsigned char* wimg,
-                        unsigned char* wimg_bwd, unsigned grid, cudaStream_t st, char* err,
-                        size_t err_len) {
-  const int nout = 1 + (p.n_attention > 0 ? p.n_attention : 3);
-  prep_weight_image_bwd<<<1, 256, 0, st>>>(p.w1, p.w2, nout, wimg_bwd);
-  NFI_PCUDA(cudaGetLastError());
-  NFI_PCUDA(cudaMemsetAsync(p.normals, 0,
-                            (size_t)p.batch * p.height * p.width * 3 * sizeof(float), st));
+int launch_pipe_normals(const nfi_render_params& p, unsigned char* wimg, unsigned char* wimg_bwd,
+                        unsigned grid, cudaStream_t st, char* err, size_t err_len) {
+  // render_normals_pipe needs layer 1 and the distance row of the plain image: row 0 of w2 with
+  // or without a view.  A view render is done with its own image (stream order), so the plain
+  // one takes its place.
+  if (p.view_features)
+    if (int rc = prep_weight_images<false>(p, wimg, false, st, err, err_len)) return rc;
+  prep_weight_image_bwd<<<1, 256, 0, st>>>(p.w1, p.w2, nout_of(p.n_attention), wimg_bwd);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_LAUNCH_CHECK(cudaMemsetAsync(p.normals, 0,
+                                   (size_t)p.batch * p.height * p.width * 3 * sizeof(float), st));
   using Cfg = BwdCfg<2>;
   constexpr int smem = Cfg::kSmBytes + (kBwdSlots * 128 + kHid) * (int)sizeof(float);
 #define NFI_NRM(NP)                                                                          \
   do {                                                                                       \
     auto k = render_normals_pipe<NP, 2>;                                                     \
-    NFI_PCUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));   \
+    NFI_LAUNCH_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); \
     k<<<grid, Cfg::kThreadsTotal, smem, st>>>(p, wimg, wimg_bwd);                            \
   } while (0)
-  if (nout_pad == 4) NFI_NRM(4); else if (nout_pad == 12) NFI_NRM(12); else NFI_NRM(16);
+  const int np = nout_pad_of(p.n_attention);
+  if (np == 4) NFI_NRM(4); else if (np == 12) NFI_NRM(12); else NFI_NRM(16);
 #undef NFI_NRM
-  NFI_PCUDA(cudaGetLastError());
+  NFI_LAUNCH_CHECK(cudaGetLastError());
   return 0;
 }
 

@@ -8,12 +8,11 @@
 #include <string.h>
 
 #include "nfi_backward.cuh"
-#include "nfi_forward.cuh"
-#include "nfi_forward_tc.cuh"
+#include "nfi_weight_image.cuh"
 #include "nfi_field_launch.h"
 #include "nfi_pipe_launch.h"
-#include "nfi_viewdir_launch.h"
 #include "nfi_render.h"
+#include "nfi_route.h"
 #include "nfi_heads.h"
 #include "nfi_heads_launch.h"
 #include "nfi_synth.h"
@@ -40,11 +39,6 @@ int fail(const char* fmt, const char* detail = "") {
       return 2;                                                             \
     }                                                                       \
   } while (0)
-
-int nout_pad_of(const nfi_render_params* p) {
-  const int nout = 1 + (p->n_attention > 0 ? p->n_attention : 3);
-  return nout <= 4 ? 4 : (nout <= 12 ? 12 : 16);
-}
 
 int check_params(const nfi_render_params* p) {
   if (p == nullptr) return fail("params is NULL");
@@ -77,7 +71,7 @@ int check_params(const nfi_render_params* p) {
     return fail("compute_semantics needs attention_values > 0");  // run.py:232
   if (p->extra_mode < 0 || p->extra_mode > 2) return fail("unknown extra_mode");
   if (p->extra_mode != NFI_EXTRA_NONE && !p->extra) return fail("extra output buffer missing");
-  if (p->compute_normals && !(p->mlp_mode & 0x1000)) {  // (0x1000: p->normals is a debug buffer)
+  if (nfi::wants_normals(*p)) {
     if (!p->use_sdf) return fail("compute_normals needs use_sdf");  // run.py:229
     if (!p->normals) return fail("normals output buffer missing");
   }
@@ -85,114 +79,53 @@ int check_params(const nfi_render_params* p) {
   return 0;
 }
 
-size_t num_ctas(const nfi_render_params* p) {
-  const size_t tx = (p->width + nfi::kTileW - 1) / nfi::kTileW;
-  const size_t ty = (p->height + nfi::kTileH - 1) / nfi::kTileH;
-  return tx * ty * (size_t)p->batch;
+// the SM count of the current device
+int sm_count(int* sms) {
+  int dev = 0;
+  NFI_CUDA(cudaGetDevice(&dev));
+  NFI_CUDA(cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev));
+  return 0;
 }
 
-constexpr size_t kWeightImageBytes = 32768;  // workspace header (nfi::kWiBytes rounded up)
-constexpr size_t kViewWeightImageBytes = 65536;  // ... of a view-conditioned render (nfi::kVdBytes)
-static_assert(nfi::kWiBytes <= kWeightImageBytes && nfi::kVdBytes <= kViewWeightImageBytes,
-              "weight image larger than the workspace header");
-// the workspace header of this render: every user of the workspace starts behind it
-size_t header_bytes(const nfi_render_params* p) {
-  return p->view_features ? kViewWeightImageBytes : kWeightImageBytes;
-}
-constexpr size_t kBackwardWorkspaceBytes = 65536;  // forward + backward weight images
-
-constexpr size_t kMaxPersistentCtas = 160;  // >= SM count of any sm_90 part (H100 SXM: 132)
-
-// persistent pipelined kernels (nfi_pipe.cu): one CTA per SM, one scratch slab per CTA
-size_t num_tc_ctas(const nfi_render_params* p) {  // persistent grid: at most one CTA per SM
-  const size_t want = num_ctas(p);
-  return want < kMaxPersistentCtas ? want : kMaxPersistentCtas;
+// persistent pipelined kernels (nfi_pipe.cu): one CTA per SM, one scratch slab per CTA, at most
+// kMaxPersistentCtas (the workspace sizes assume no more)
+size_t num_tc_ctas(const nfi_render_params& p) {
+  const size_t want = nfi::num_tiles(p);
+  return want < nfi::kMaxPersistentCtas ? want : nfi::kMaxPersistentCtas;
 }
 
 // the grid of a persistent pipelined launch: num_tc_ctas, and no more CTAs than this device's SMs
 int persistent_grid(const nfi_render_params& p, unsigned* grid) {
-  int dev = 0, sms = 0;
-  NFI_CUDA(cudaGetDevice(&dev));
-  NFI_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const size_t want = num_tc_ctas(&p);
+  int sms = 0;
+  if (int rc = sm_count(&sms)) return rc;
+  const size_t want = num_tc_ctas(p);
   *grid = (unsigned)(want < (size_t)sms ? want : (size_t)sms);
   return 0;
 }
 
-// The modes that run the pipelined tensor-core kernels where they can take the configuration
-// (NFI_MLP_TC_3XTF32 and NFI_MLP_TC_WARPSPEC are aliases of NFI_MLP_TC_PIPE).
-bool tc_mode(int mode) {
-  return mode == NFI_MLP_AUTO || mode == NFI_MLP_TC_3XTF32 || mode == NFI_MLP_TC_WARPSPEC ||
-         mode == NFI_MLP_TC_PIPE;
-}
+bool is_pipe(nfi::Route r) { return r == nfi::Route::kPipe || r == nfi::Route::kPipeVd; }
 
-// Can the pipelined tensor-core kernels take this configuration in this mode?
-bool tc_supported(const nfi_render_params* p) {
-  if (!tc_mode(p->mlp_mode & 0xff)) return false;
-  // surface normals: a second pipelined kernel after the render (nfi_normals_pipe.cuh), which
-  // walks the merged samples and so needs the forward pass's fine depths; else the SIMT kernel
-  if (p->compute_normals && !(p->mlp_mode & 0x1000) &&
-      !((!p->fine_sampling || p->z_fine != nullptr) && p->n_peers == 0))
-    return false;
-  // semantics: the pipelined kernel parks the coarse samples' probabilities; NOUT_PAD = 4 only
-  // exists for palettes of <= 3 entries, kept on the SIMT kernel
-  if (p->extra_mode == NFI_EXTRA_SEMANTICS && p->n_attention <= 3) return false;
-  // <= 4 samples per lane in the resampler, float4 jitter
-  return p->num_samples <= 128 && p->num_samples % 4 == 0;
-}
-
-bool wants_normals(const nfi_render_params* p) {
-  return p->compute_normals && !(p->mlp_mode & 0x1000);
-}
-
-int ne_store_of(const nfi_render_params* p) {
-  return (p->extra_mode == NFI_EXTRA_SEMANTICS ? nout_pad_of(p) - 1 : 0) +
-         (wants_normals(p) ? 3 : 0);
-}
-
-template <typename K>
-int launch(K kernel, const nfi_render_params& p, size_t smem_bytes, cudaStream_t st) {
-  if (smem_bytes > 227 * 1024)
-    return fail("depth_samples_per_ray too large for the shared-memory columns");
-  NFI_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)smem_bytes));
-  kernel<<<(unsigned)num_ctas(&p), nfi::kThreads, smem_bytes, st>>>(p);
-  NFI_CUDA(cudaGetLastError());
-  return 0;
-}
-
-template <int NP, int EX>
-int launch_fwd_fine(const nfi_render_params& p, size_t smem, cudaStream_t st) {
-  if (wants_normals(&p)) {
-    if (p.fine_sampling) return launch(nfi::render_forward_simt<NP, EX, true, true>, p, smem, st);
-    return launch(nfi::render_forward_simt<NP, EX, false, true>, p, smem, st);
+// Byte offsets in the forward's workspace (nfi_layout.h): the scratch slabs behind the weight
+// image, the backward image of the normals kernel behind the scratch, and the total size.
+struct FwdWorkspace {
+  size_t scratch, normals_image, total;
+};
+FwdWorkspace fwd_workspace(const nfi_render_params& p, const nfi::Plan& r) {
+  const int nes = p.extra_mode == NFI_EXTRA_SEMANTICS ? nfi::nout_pad_of(p.n_attention) - 1 : 0;
+  size_t slabs = 0;
+  if (p.fine_sampling) {  // the coarse samples, one slab per CTA of the kernel that will run
+    if (is_pipe(r.route))
+      slabs = num_tc_ctas(p) * nfi::pipe_scratch_bytes_per_cta(p.num_samples, nes);
+    else  // the SIMT kernel parks the normals as three more extras
+      slabs = nfi::num_tiles(p) * sizeof(float) *
+              nfi::fwd_scratch_floats_per_cta(p.num_samples, nes + (nfi::wants_normals(p) ? 3 : 0));
   }
-  if (p.fine_sampling) return launch(nfi::render_forward_simt<NP, EX, true>, p, smem, st);
-  return launch(nfi::render_forward_simt<NP, EX, false>, p, smem, st);
-}
-
-template <int NP>
-int launch_fwd_extra(const nfi_render_params& p, size_t smem, cudaStream_t st) {
-  switch (p.extra_mode) {
-    case NFI_EXTRA_COORDS: return launch_fwd_fine<NP, 1>(p, smem, st);
-    case NFI_EXTRA_SEMANTICS: return launch_fwd_fine<NP, 2>(p, smem, st);
-    default: return launch_fwd_fine<NP, 0>(p, smem, st);
-  }
-}
-
-// render_forward_pipe (nfi_pipe.cu): the weight image at the head of the workspace, the scratch
-// slabs behind it, tiles strided over the persistent grid.  A view-conditioned render takes the
-// VD instantiation and its weight image (nfi_pipe_vd.cu).
-int launch_fwd_tc(const nfi_render_params& p, int np, cudaStream_t st) {
-  unsigned char* wimg = (unsigned char*)p.workspace;
-  const bool vd = p.view_features != nullptr;
-  if (vd ? nfi::launch_pipe_weight_image_vd(p, wimg, st) : nfi::launch_pipe_weight_image(p, wimg, st))
-    return fail("weight image launch failed");
-  unsigned grid = 0;
-  if (int rc = persistent_grid(p, &grid)) return rc;
-  float* scratch = (float*)(wimg + header_bytes(&p));
-  if (vd) return nfi::launch_pipe_forward_vd(p, np, wimg, scratch, grid, st, g_err, sizeof(g_err));
-  return nfi::launch_pipe_forward(p, np, wimg, scratch, grid, st, g_err, sizeof(g_err));
+  FwdWorkspace w;
+  w.scratch = p.view_features ? nfi::kVdFwdImageSlot : nfi::kFwdImageSlot;
+  const size_t end = w.scratch + slabs + 256;
+  w.normals_image = end & ~(size_t)255;
+  w.total = end + (r.normals_pipe ? nfi::kBwdImageBytes : 0);
+  return w;
 }
 
 // SIMT reference decoder (one point per thread), for nfi_decoder_forward
@@ -318,20 +251,7 @@ const char* nfi_last_error(void) { return g_err; }
 
 size_t nfi_render_workspace_bytes(const nfi_render_params* p) {
   if (p == nullptr) return 0;
-  size_t fwd = 0;
-  if (p->fine_sampling) {
-    // scratch for the coarse samples, sized for the kernel that will run
-    if (tc_supported(p)) {  // persistent: one slab per CTA (<= one per SM)
-      fwd = num_tc_ctas(p) * nfi::pipe_scratch_bytes_per_cta(
-                                 p->num_samples,
-                                 p->extra_mode == NFI_EXTRA_SEMANTICS ? nout_pad_of(p) - 1 : 0);
-    } else {  // fp32 SIMT kernel: one slab per CTA (= tile)
-      fwd = num_ctas(p) * nfi::fwd_scratch_floats_per_cta(p->num_samples, ne_store_of(p)) *
-            sizeof(float);
-    }
-  }
-  // (+ the backward weight image of the normals kernel, behind the scratch)
-  return header_bytes(p) + fwd + 256 + (wants_normals(p) && tc_supported(p) ? 32768 : 0);
+  return fwd_workspace(*p, nfi::route_forward(*p)).total;
 }
 
 int nfi_planes_to_channel_last(const float* xy, const float* xz, const float* yz,
@@ -370,52 +290,31 @@ int nfi_fill_uniform(float* dst, int64_t n, uint64_t seed, uint32_t stream_id, i
 int nfi_render_forward(const nfi_render_params* params, void* stream) {
   if (int rc = check_params(params)) return rc;
   const nfi_render_params& p = *params;
-  const int np = nout_pad_of(params);
   cudaStream_t st = (cudaStream_t)stream;
-  const int mode = p.mlp_mode & 0xff;
-  const bool want_tc = tc_supported(params);
-  if (mode != NFI_MLP_AUTO && tc_mode(mode) && !want_tc)
-    return fail("tensor-core modes need S <= 128 and S % 4 == 0 and no semantics output; "
-                "use NFI_MLP_AUTO");
-  if (want_tc || p.fine_sampling) {
-    if (!p.workspace || p.workspace_bytes < nfi_render_workspace_bytes(params))
-      return fail("workspace too small (see nfi_render_workspace_bytes)");
-  }
   if (p.n_peers < 0 || p.n_peers > NFI_MAX_PEERS) return fail("n_peers out of range");
   for (int q = 0; q < p.n_peers; ++q)
     if (!p.peer_rgb[q] || !p.peer_depth[q] || !p.peer_mask[q]) return fail("peer output pointer is NULL");
-  if (want_tc) {
-    if (int rc = launch_fwd_tc(p, np, st)) return rc;
-    if (wants_normals(params)) {
-      unsigned grid = 0;
-      if (int rc = persistent_grid(p, &grid)) return rc;
-      unsigned char* ws = (unsigned char*)p.workspace;
-      // render_normals_pipe reads the plain image, of which it needs layer 1 and the distance
-      // row: row 0 of w2 with or without a view.  The view render is done with its own image
-      // (stream order), so the plain one takes its place at the head of the workspace.
-      if (p.view_features && nfi::launch_pipe_weight_image(p, ws, st))
-        return fail("weight image launch failed");
-      const size_t off = (nfi_render_workspace_bytes(params) - 32768) & ~(size_t)255;
-      return nfi::launch_pipe_normals(p, np, ws, ws + off, grid, st, g_err, sizeof(g_err));
-    }
-    return 0;
+  const nfi::Plan r = nfi::route_forward(p);
+  if (r.route == nfi::Route::kRefused) return fail(r.refusal);
+  const FwdWorkspace ws = fwd_workspace(p, r);
+  if ((is_pipe(r.route) || p.fine_sampling) && (!p.workspace || p.workspace_bytes < ws.total))
+    return fail("workspace too small (see nfi_render_workspace_bytes)");
+  unsigned char* wsp = (unsigned char*)p.workspace;
+  if (!is_pipe(r.route)) {
+    nfi_render_params ps = p;  // SIMT scratch starts after the weight-image header
+    if (ps.workspace) ps.workspace = wsp + ws.scratch;
+    if (r.route == nfi::Route::kSimtVd)
+      return nfi::launch_forward_simt<true>(ps, nfi::wants_normals(p), st, g_err, sizeof(g_err));
+    return nfi::launch_forward_simt<false>(ps, nfi::wants_normals(p), st, g_err, sizeof(g_err));
   }
-  if (p.n_peers > 0) return fail("peer outputs (n_peers > 0) need the pipelined kernel");
-  if (p.view_features) {
-    nfi_render_params pv = p;  // SIMT scratch starts after the weight-image header
-    if (pv.workspace) pv.workspace = (unsigned char*)pv.workspace + header_bytes(params);
-    return nfi::launch_forward_viewdir(pv, np, wants_normals(params), st, g_err, sizeof(g_err));
-  }
-  const size_t smem =
-      nfi::fwd_smem_floats(np, p.num_samples, p.fine_sampling != 0, wants_normals(params)) *
-      sizeof(float);
-  nfi_render_params ps = p;  // SIMT scratch starts after the weight-image header
-  if (ps.workspace) ps.workspace = (unsigned char*)ps.workspace + kWeightImageBytes;
-  switch (np) {
-    case 4: return launch_fwd_extra<4>(ps, smem, st);
-    case 12: return launch_fwd_extra<12>(ps, smem, st);
-    default: return launch_fwd_extra<16>(ps, smem, st);
-  }
+  unsigned grid = 0;
+  if (int rc = persistent_grid(p, &grid)) return rc;
+  float* scratch = (float*)(wsp + ws.scratch);
+  const int rc = r.route == nfi::Route::kPipeVd
+                     ? nfi::launch_pipe_forward<true>(p, wsp, scratch, grid, st, g_err, sizeof(g_err))
+                     : nfi::launch_pipe_forward<false>(p, wsp, scratch, grid, st, g_err, sizeof(g_err));
+  if (rc || !r.normals_pipe) return rc;
+  return nfi::launch_pipe_normals(p, wsp, wsp + ws.normals_image, grid, st, g_err, sizeof(g_err));
 }
 
 int nfi_decoder_forward(const float* features, int64_t n_points, const float* w1, const float* b1,
@@ -424,8 +323,7 @@ int nfi_decoder_forward(const float* features, int64_t n_points, const float* w1
   if (!features || !w1 || !b1 || !w2 || !b2 || !out || n_points <= 0)
     return fail("bad decoder arguments");
   if (n_attention < 0 || n_attention > NFI_MAX_ATTENTION) return fail("attention_values out of range");
-  const int nout = 1 + (n_attention > 0 ? n_attention : 3);
-  const int np = nout <= 4 ? 4 : (nout <= 12 ? 12 : 16);
+  const int nout = nfi::nout_of(n_attention), np = nfi::nout_pad_of(n_attention);
   cudaStream_t st = (cudaStream_t)stream;
   if (mlp_mode == NFI_MLP_FP32_SIMT) {
     const unsigned grid = (unsigned)((n_points + 127) / 128);
@@ -440,9 +338,8 @@ int nfi_decoder_forward(const float* features, int64_t n_points, const float* w1
   nfi::prep_weight_image<<<1, 256, 0, st>>>(w1, b1, w2, b2, nout, wimg, 1.f, 0.f, 1.f);
   NFI_CUDA(cudaGetLastError());
   const long long tiles = (n_points + 127) / 128;
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  int sms = 0;
+  if (int rc = sm_count(&sms)) return rc;
   const unsigned grid = (unsigned)((tiles + nfi::kGroups - 1) / nfi::kGroups < sms
                                        ? (tiles + nfi::kGroups - 1) / nfi::kGroups
                                        : sms);
@@ -466,60 +363,34 @@ int nfi_render_backward(const nfi_render_params* params, const nfi_render_grads*
   if (grads == nullptr || grads->g_rgb == nullptr) return fail("grads->g_rgb missing");
   const nfi_render_params& p = *params;
   const nfi_render_grads& g = *grads;
+  if (p.fine_sampling && p.z_fine == nullptr)
+    return fail("backward needs the z_fine buffer the forward pass filled");
+  if (!g.out_rgb || !g.out_mask) return fail("backward needs the forward outputs (out_rgb, out_mask)");
+  if (g.g_extra && !g.out_extra) return fail("g_extra given without out_extra");
+  if ((g.grad_origins == nullptr) != (g.grad_dirs == nullptr))
+    return fail("grad_origins and grad_dirs must be given together");
   cudaStream_t st = (cudaStream_t)stream;
-  // Tensor-core backward (nfi_backward_pipe.cuh): frozen decoder weights (the inversion
-  // setting, run.py:628-629), no semantics output, S within the pipelined kernels' envelope,
-  // and a workspace for the two weight images.  Everything else: render_backward_simt.
-  const int mode = p.mlp_mode & 0xff;
-  const bool wgrad = g.grad_w1 || g.grad_b1 || g.grad_w2 || g.grad_b2;
-  const bool tc_env_any = mode != NFI_MLP_FP32_SIMT && p.extra_mode != NFI_EXTRA_SEMANTICS &&
-                          p.num_samples <= 128 && p.num_samples % 4 == 0 &&
-                          p.workspace != nullptr && (!p.fine_sampling || p.z_fine != nullptr) &&
-                          g.out_rgb && g.out_mask && (!g.g_extra || g.out_extra) &&
-                          ((g.grad_origins == nullptr) == (g.grad_dirs == nullptr));
-  if (p.view_features) {
-    // the inversion step of a view-conditioned model (decoder and mapper frozen):
-    // render_backward_pipe<..., VD> (nfi_pipe_vd.cu); its GAN step stays on the SIMT kernel
-    if (tc_env_any && !wgrad && !g.grad_w3 && !g.grad_b3 &&
-        p.workspace_bytes >= (size_t)NFI_VIEW_BACKWARD_WORKSPACE_BYTES) {
-      unsigned grid = 0;
-      if (int rc = persistent_grid(p, &grid)) return rc;
-      return nfi::launch_pipe_backward_vd(p, g, nout_pad_of(params), (unsigned char*)p.workspace,
-                                          grid, st, g_err, sizeof(g_err));
-    }
-    return nfi::launch_backward_viewdir(p, g, nout_pad_of(params), st, g_err, sizeof(g_err));
+  const nfi::Plan r = nfi::route_backward(p, g);
+  switch (r.route) {
+    case nfi::Route::kRefused: return fail(r.refusal);
+    case nfi::Route::kSimt: return nfi::launch_backward_simt<false>(p, g, st, g_err, sizeof(g_err));
+    case nfi::Route::kSimtVd: return nfi::launch_backward_simt<true>(p, g, st, g_err, sizeof(g_err));
+    default: break;
   }
-  if (g.grad_view_features || g.grad_w3 || g.grad_b3)
-    return fail("grad_view_features / grad_w3 / grad_b3 need params->view_features");
-  const bool tc_env = tc_env_any && p.workspace_bytes >= kBackwardWorkspaceBytes;
-  // decoder-weight gradients (the GAN generator step, run.py:1044) on the tensor cores too: a second
-  // kernel (render_wgrad_pipe) beside render_backward_pipe, which then sees a frozen decoder.
-  // An upstream gradient of the coords output stays on the SIMT kernel.
-  const bool tc_ok = tc_env && (!wgrad || (!g.g_extra &&
-                                           p.workspace_bytes >= nfi::pipe_wgrad_workspace_bytes(
-                                                                    (unsigned)kMaxPersistentCtas)));
-  if (tc_ok) {
-    unsigned grid = 0;  // <= kMaxPersistentCtas: the wgrad workspace is sized for that many CTAs
-    if (int rc = persistent_grid(p, &grid)) return rc;
-    nfi_render_grads g1 = g;
+  unsigned char* ws = (unsigned char*)p.workspace;
+  unsigned grid = 0;  // <= kMaxPersistentCtas: the accumulator rows are sized for that many CTAs
+  if (int rc = persistent_grid(p, &grid)) return rc;
+  if (r.route == nfi::Route::kPipeVd)
+    return nfi::launch_pipe_backward<true>(p, g, ws, grid, st, g_err, sizeof(g_err));
+  if (r.route == nfi::Route::kPipe || r.route == nfi::Route::kPipeAndWgrad) {
+    nfi_render_grads g1 = g;  // the decoder gradients are render_wgrad_pipe's
     g1.grad_w1 = g1.grad_b1 = g1.grad_w2 = g1.grad_b2 = nullptr;
-    const bool others = g1.grad_planes || g1.grad_palette || g1.grad_beta || g1.grad_alpha ||
-                        g1.grad_origins;
-    // The generator step (decoder gradients, cameras are data): ONE sweep, render_wgrad_pipe with
-    // the plane scatter folded in.  With a pose gradient too: render_backward_pipe beside it.
-    // (mlp_mode bit 0x2000: timing experiments, tools/time_wgrad.py -- two sweeps anyway)
-    const bool one_sweep = wgrad && others && !g.grad_origins && !(p.mlp_mode & 0x2000);
-    if ((others && !one_sweep) || !wgrad) {
-      if (int rc = nfi::launch_pipe_backward(p, g1, nout_pad_of(params), (unsigned char*)p.workspace,
-                                             grid, st, g_err, sizeof(g_err)))
-        return rc;
-    }
-    if (wgrad)
-      return nfi::launch_pipe_wgrad(p, g, nout_pad_of(params), (unsigned char*)p.workspace,
-                                    grid, one_sweep, st, g_err, sizeof(g_err));
-    return 0;
+    if (int rc = nfi::launch_pipe_backward<false>(p, g1, ws, grid, st, g_err, sizeof(g_err)))
+      return rc;
+    if (r.route == nfi::Route::kPipe) return 0;
   }
-  return nfi::launch_backward(*params, *grads, st, g_err, sizeof(g_err));
+  return nfi::launch_pipe_wgrad(p, g, ws, grid, r.route == nfi::Route::kWgradOneSweep, st, g_err,
+                                sizeof(g_err));
 }
 
 int nfi_sample_field(const nfi_sample_params* sp, void* stream) {
@@ -556,8 +427,8 @@ int nfi_sample_field(const nfi_sample_params* sp, void* stream) {
   p.palette = sp->palette;
   p.beta = sp->beta;
   p.alpha = sp->alpha;
-  return nfi::launch_sample_field(p, *sp, nout_pad_of(&p), (cudaStream_t)stream, g_err,
-                                  sizeof(g_err));
+  return nfi::launch_sample_field(p, *sp, nfi::nout_pad_of(p.n_attention), (cudaStream_t)stream,
+                                  g_err, sizeof(g_err));
 }
 
 int nfi_pose_to_matrix(const float* z0, const float* t2, const float* s, const float* q,
@@ -714,7 +585,7 @@ int nfi_render_forward_host(const nfi_render_params* hp, int32_t device) {
   nfi_render_params d = *hp;
   const size_t B = hp->batch, H = hp->height, W = hp->width, S = hp->num_samples;
   const size_t R = hp->plane_res, A = hp->n_attention;
-  const size_t nout = 1 + (A > 0 ? A : 3);
+  const size_t nout = nfi::nout_of(hp->n_attention);
   const size_t rays_img = H * W, n_rays = B * rays_img;
   void* to_free[40];
   int n_free = 0;

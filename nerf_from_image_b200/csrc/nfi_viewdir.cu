@@ -1,116 +1,11 @@
-// Translation unit of the view-direction-conditioned render (--use_viewdir, the CARLA models:
-// run.py:216-217, models/generator.py:189-253,376-377,662-663): render_forward_simt /
-// render_backward_simt with VD = true.  The decoder's second layer emits 1 + 32 values and every
-// sample's colour logits are w3 . leaky_relu(view_features[ray] + features, 0.2) + b3, where
-// view_features is the ViewDirectionMapper trunk evaluated once per ray by the caller.
-#include <cuda_runtime.h>
-#include <stdio.h>
-
+// Translation unit of the view-direction-conditioned SIMT render (--use_viewdir, the CARLA
+// models: run.py:216-217, models/generator.py:189-253,376-377,662-663): the launchers of
+// render_forward_simt / render_backward_simt instantiated with VD = true, a unit of its own that
+// build.sh compiles in parallel with the others.
 #include "nfi_backward.cuh"
-#include "nfi_forward.cuh"
-#include "nfi_viewdir_launch.h"
 
 namespace nfi {
-namespace {
-
-#define NFI_VCUDA(expr)                                                              \
-  do {                                                                               \
-    cudaError_t e__ = (expr);                                                        \
-    if (e__ != cudaSuccess) {                                                        \
-      snprintf(err, err_len, "%s failed: %s", #expr, cudaGetErrorString(e__));       \
-      return 2;                                                                      \
-    }                                                                                \
-  } while (0)
-
-unsigned tiles_of(const nfi_render_params& p) {
-  const size_t tx = (p.width + kTileW - 1) / kTileW, ty = (p.height + kTileH - 1) / kTileH;
-  return (unsigned)(tx * ty * (size_t)p.batch);
-}
-
-template <typename K>
-int launch_fwd(K kernel, const nfi_render_params& p, size_t smem, cudaStream_t st, char* err,
-               size_t err_len) {
-  if (smem > 227 * 1024) {
-    snprintf(err, err_len, "depth_samples_per_ray too large for the shared-memory columns");
-    return 1;
-  }
-  NFI_VCUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  kernel<<<tiles_of(p), kThreads, smem, st>>>(p);
-  NFI_VCUDA(cudaGetLastError());
-  return 0;
-}
-
-template <int NP, int EX>
-int fwd_fine(const nfi_render_params& p, bool normals, size_t smem, cudaStream_t st, char* err,
-             size_t err_len) {
-  if (normals) {
-    if (p.fine_sampling)
-      return launch_fwd(render_forward_simt<NP, EX, true, true, true>, p, smem, st, err, err_len);
-    return launch_fwd(render_forward_simt<NP, EX, false, true, true>, p, smem, st, err, err_len);
-  }
-  if (p.fine_sampling)
-    return launch_fwd(render_forward_simt<NP, EX, true, false, true>, p, smem, st, err, err_len);
-  return launch_fwd(render_forward_simt<NP, EX, false, false, true>, p, smem, st, err, err_len);
-}
-
-template <int NP>
-int fwd_extra(const nfi_render_params& p, bool normals, size_t smem, cudaStream_t st, char* err,
-              size_t err_len) {
-  switch (p.extra_mode) {
-    case NFI_EXTRA_COORDS: return fwd_fine<NP, 1>(p, normals, smem, st, err, err_len);
-    case NFI_EXTRA_SEMANTICS: return fwd_fine<NP, 2>(p, normals, smem, st, err, err_len);
-    default: return fwd_fine<NP, 0>(p, normals, smem, st, err, err_len);
-  }
-}
-
-template <int NP, bool WG>
-int bwd(const nfi_render_params& p, const nfi_render_grads& g, cudaStream_t st, char* err,
-        size_t err_len) {
-  const size_t smem = bwd_smem_floats(NP, WG, true) * sizeof(float);
-  auto k = render_backward_simt<NP, WG, true>;
-  NFI_VCUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k<<<tiles_of(p), kThreads, smem, st>>>(p, g);
-  NFI_VCUDA(cudaGetLastError());
-  return 0;
-}
-
-}  // namespace
-
-int launch_forward_viewdir(const nfi_render_params& p, int np, bool normals, cudaStream_t st,
-                           char* err, size_t err_len) {
-  const size_t smem =
-      fwd_smem_floats(np, p.num_samples, p.fine_sampling != 0, normals, true) * sizeof(float);
-  switch (np) {
-    case 4: return fwd_extra<4>(p, normals, smem, st, err, err_len);
-    case 12: return fwd_extra<12>(p, normals, smem, st, err, err_len);
-    default: return fwd_extra<16>(p, normals, smem, st, err, err_len);
-  }
-}
-
-int launch_backward_viewdir(const nfi_render_params& p, const nfi_render_grads& g, int np,
-                            cudaStream_t st, char* err, size_t err_len) {
-  if (p.fine_sampling && p.z_fine == nullptr) {
-    snprintf(err, err_len, "backward needs the z_fine buffer the forward pass filled");
-    return 1;
-  }
-  if (!g.out_rgb || !g.out_mask) {
-    snprintf(err, err_len, "backward needs the forward outputs (out_rgb, out_mask)");
-    return 1;
-  }
-  if (g.g_extra && !g.out_extra) {
-    snprintf(err, err_len, "g_extra given without out_extra");
-    return 1;
-  }
-  if ((g.grad_origins == nullptr) != (g.grad_dirs == nullptr)) {
-    snprintf(err, err_len, "grad_origins and grad_dirs must be given together");
-    return 1;
-  }
-  const bool wgrad = g.grad_w1 || g.grad_b1 || g.grad_w2 || g.grad_b2 || g.grad_w3 || g.grad_b3;
-  switch (np) {
-    case 4: return wgrad ? bwd<4, true>(p, g, st, err, err_len) : bwd<4, false>(p, g, st, err, err_len);
-    case 12: return wgrad ? bwd<12, true>(p, g, st, err, err_len) : bwd<12, false>(p, g, st, err, err_len);
-    default: return wgrad ? bwd<16, true>(p, g, st, err, err_len) : bwd<16, false>(p, g, st, err, err_len);
-  }
-}
-
+template int launch_forward_simt<true>(const nfi_render_params&, bool, cudaStream_t, char*, size_t);
+template int launch_backward_simt<true>(const nfi_render_params&, const nfi_render_grads&,
+                                        cudaStream_t, char*, size_t);
 }  // namespace nfi

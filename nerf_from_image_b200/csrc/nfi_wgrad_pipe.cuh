@@ -47,7 +47,6 @@ constexpr int kWgStages = 3;
 // round-to-nearest, to a per-CTA row buffer in global memory (L2-resident, single writer per
 // element) and the next chain starts from zero.
 constexpr int kWgFlush = 16;
-constexpr size_t kWgAccBytesPerCta = 128 * 64 * sizeof(float);
 
 // PLANES: the kernel also forms dL/d(texel features) (MMA4) and scatters it into the plane
 // gradient, and accumulates the palette / beta / alpha gradients -- i.e. it is the WHOLE backward
@@ -162,7 +161,7 @@ render_wgrad_pipe(const nfi_render_params p, const nfi_render_grads g,
     tc::mbar_expect_tx(&wbar[0], kWiBytes);
     tc::tma_bulk_g2s(base, wimg, kWiBytes, &wbar[0]);
     tc::mbar_expect_tx(&wbar[1], Cfg::kWbBytes);
-    tc::tma_bulk_g2s(base + Cfg::kSmWb, wimg + 32768, Cfg::kWbBytes, &wbar[1]);  // W2^T (| W1^T / 3)
+    tc::tma_bulk_g2s(base + Cfg::kSmWb, wimg + kBwdImageOffset, Cfg::kWbBytes, &wbar[1]);  // W2^T (| W1^T / 3)
   }
   tc::mbar_wait(&wbar[0], 0);
   tc::mbar_wait(&wbar[1], 0);

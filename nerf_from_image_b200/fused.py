@@ -349,7 +349,8 @@ class FusedTriplaneRender(torch.autograd.Function):
             if vd:
                 ws_bytes = _lib.VIEW_BACKWARD_WORKSPACE_BYTES
             else:
-                ws_bytes = _lib.BACKWARD_WORKSPACE_BYTES if (n_w1 or n_b1 or n_w2 or n_b2) else 65536
+                ws_bytes = (_lib.BACKWARD_WORKSPACE_BYTES if (n_w1 or n_b1 or n_w2 or n_b2)
+                            else _lib.BACKWARD_IMAGES_BYTES)
             ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
             p.workspace, p.workspace_bytes = _ptr(ws), ws_bytes
             _lib.check(lib.nfi_render_backward(ctypes.byref(p), ctypes.byref(g), stream))
