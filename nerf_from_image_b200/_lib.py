@@ -1,4 +1,5 @@
-"""ctypes binding of libnfi_render.so (the C ABI declared in include/nfi_render.h).
+"""ctypes binding of libnfi_render.so (the C ABI declared in include/nfi_render.h and the headers
+next to it).
 
 The library is built in-tree by ``nerf_from_image_b200/csrc/build.sh`` (or
 ``__graft_entry__.build()``).  There is no fallback: if the shared object is
@@ -143,8 +144,24 @@ class SdfPointsGrads(ctypes.Structure):
         'g_d', 'g_grad', 'grad_planes', 'grad_w1', 'grad_b1', 'grad_w2_row0', 'grad_b2_0')]
 
 
-# every symbol include/*.h declare (tests/test_abi.py checks the
-# header against this table and the table against the built library)
+LPIPS_CONVS, LPIPS_TAPS = 13, 5
+
+
+class LpipsParams(ctypes.Structure):
+    """struct nfi_lpips_params (include/nfi_lpips.h)."""
+    _fields_ = [
+        ('n', ctypes.c_int32), ('height', ctypes.c_int32), ('width', ctypes.c_int32),
+        ('save', ctypes.c_int32), ('in0', ctypes.c_void_p), ('in1', ctypes.c_void_p),
+        ('conv_w', ctypes.c_void_p * LPIPS_CONVS), ('conv_b', ctypes.c_void_p * LPIPS_CONVS),
+        ('lin_w', ctypes.c_void_p * LPIPS_TAPS), ('shift', ctypes.c_void_p),
+        ('scale', ctypes.c_void_p), ('out', ctypes.c_void_p), ('workspace', ctypes.c_void_p),
+        ('workspace_bytes', ctypes.c_size_t),
+    ]
+
+
+# every symbol include/nfi_render.h, nfi_synth.h and nfi_heads.h declare (tests/test_abi.py checks
+# those headers against this table and the table against the built library); LPIPS_EXPORTS below
+# holds the symbols of include/nfi_lpips.h (tests/test_lpips_abi.py)
 EXPORTS = {
     'nfi_abi_version': (ctypes.c_int, []),
     'nfi_build_info': (ctypes.c_char_p, []),
@@ -202,6 +219,15 @@ EXPORTS = {
         ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
 }
 
+LPIPS_EXPORTS = {
+    'nfi_lpips_workspace_bytes': (ctypes.c_size_t, [ctypes.POINTER(LpipsParams)]),
+    'nfi_lpips_forward': (ctypes.c_int, [ctypes.POINTER(LpipsParams), ctypes.c_void_p]),
+    'nfi_lpips_backward': (ctypes.c_int, [ctypes.POINTER(LpipsParams), ctypes.c_void_p,
+                                          ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    'nfi_lpips_saved_preactivation': (ctypes.c_int, [ctypes.POINTER(LpipsParams), ctypes.c_int32,
+                                                     ctypes.c_void_p, ctypes.c_void_p]),
+}
+
 _lib = None
 _lock = threading.Lock()
 
@@ -241,7 +267,7 @@ def load():
                 # memory corruption, not an error
                 raise NfiError('%s has ABI version %d, this binding needs %d: rebuild it '
                                '(nerf_from_image_b200/csrc/build.sh)' % (LIB_PATH, got, ABI_VERSION))
-            for name, (restype, argtypes) in EXPORTS.items():
+            for name, (restype, argtypes) in list(EXPORTS.items()) + list(LPIPS_EXPORTS.items()):
                 fn = getattr(lib, name, None)
                 if fn is None and os.environ.get('NFI_LIB_PATH'):
                     continue  # an older build under test lacks the newer entry points

@@ -15,6 +15,8 @@
 #include "nfi_route.h"
 #include "nfi_heads.h"
 #include "nfi_heads_launch.h"
+#include "nfi_lpips.h"
+#include "nfi_lpips_launch.h"
 #include "nfi_synth.h"
 #include "nfi_synth_launch.h"
 
@@ -477,6 +479,28 @@ int nfi_sdf_points_backward(const nfi_sdf_points_params* params, const nfi_sdf_p
   if (grads->grad_w1 && (!grads->grad_b1 || !grads->grad_w2_row0 || !grads->grad_b2_0))
     return fail("decoder gradients come as a set: grad_w1, grad_b1, grad_w2_row0, grad_b2_0");
   return nfi::heads::launch_backward(*params, *grads, (cudaStream_t)stream, g_err, sizeof(g_err));
+}
+
+size_t nfi_lpips_workspace_bytes(const nfi_lpips_params* params) {
+  if (params == nullptr) return 0;
+  return nfi::lpips::workspace_bytes(*params);
+}
+
+int nfi_lpips_forward(const nfi_lpips_params* params, void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  return nfi::lpips::forward(*params, (cudaStream_t)stream, g_err, sizeof(g_err));
+}
+
+int nfi_lpips_backward(const nfi_lpips_params* params, const float* g_dist, float* grad_in0, float* grad_in1,
+                       void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  return nfi::lpips::backward(*params, g_dist, grad_in0, grad_in1, (cudaStream_t)stream, g_err,
+                              sizeof(g_err));
+}
+
+int nfi_lpips_saved_preactivation(const nfi_lpips_params* params, int32_t layer, float* out, void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  return nfi::lpips::saved_preactivation(*params, layer, out, (cudaStream_t)stream, g_err, sizeof(g_err));
 }
 
 size_t nfi_synthesis_workspace_bytes(const nfi_synth_params* params) {

@@ -61,10 +61,11 @@ constexpr int kSkipDim = 10, kSkipRow4 = 25;
 constexpr int kSkipBytes = kSkipDim * kSkipDim * kSkipRow4 * 16;
 
 struct ActEpilogue {   // shared by conv_tc_kernel (stride-1 layers) and fir_act_kernel (up layers)
-  const float* dcoef;  // [B,N]
+  const float* dcoef;  // [B,N] or nullptr (1: no demodulation, the LPIPS network's plain convs)
   const float* noise;  // [B,H,W] or nullptr
   const float* bias;   // [N]
   float gain;          // sqrt(2)
+  float slope;         // negative slope of the activation: 0.2 (leaky ReLU), 0 (ReLU)
   const float* style_a;  // [B,N] style of consumer a (or nullptr: plain value)
   __nv_bfloat16* a_hi;   // [B,H,W,N]
   __nv_bfloat16* a_lo;
@@ -165,6 +166,7 @@ __device__ __forceinline__ void store_split4(__nv_bfloat16* hi, __nv_bfloat16* l
   *reinterpret_cast<uint2*>(lo + idx) = *reinterpret_cast<const uint2*>(l);
 }
 __device__ __forceinline__ float lrelu(float x) { return x > 0.f ? x : 0.2f * x; }
+__device__ __forceinline__ float lrelu(float x, float slope) { return x > 0.f ? x : slope * x; }
 
 // value -> (value * style) as a bf16 hi / lo pair, 2 channels (4 bytes per tensor) at a time
 __device__ __forceinline__ void store_split2(__nv_bfloat16* hi, __nv_bfloat16* lo, size_t idx,
@@ -179,14 +181,15 @@ __device__ __forceinline__ void store_split2(__nv_bfloat16* hi, __nv_bfloat16* l
 // fragments hold channel pairs).
 __device__ __forceinline__ void act_store2(const ActEpilogue& e, int img, size_t pos, int N, int n,
                                            float2 acc, float noise) {
-  const float2 d = __ldg(reinterpret_cast<const float2*>(e.dcoef + (size_t)img * N + n));
+  const float2 d = e.dcoef ? __ldg(reinterpret_cast<const float2*>(e.dcoef + (size_t)img * N + n))
+                          : make_float2(1.f, 1.f);
   const float2 b = __ldg(reinterpret_cast<const float2*>(e.bias + n));
   float2 u, v;
   u.x = ((acc.x * d.x + noise) + b.x) * e.gain;
   u.y = ((acc.y * d.y + noise) + b.y) * e.gain;
   if (e.u_out != nullptr) *reinterpret_cast<float2*>(e.u_out + pos * N + n) = u;
-  v.x = lrelu(u.x);
-  v.y = lrelu(u.y);
+  v.x = lrelu(u.x, e.slope);
+  v.y = lrelu(u.y, e.slope);
   const float2 one = make_float2(1.f, 1.f);
   if (e.a_hi != nullptr) {
     const float2 s = e.style_a ? __ldg(reinterpret_cast<const float2*>(e.style_a + (size_t)img * N + n)) : one;
@@ -200,7 +203,8 @@ __device__ __forceinline__ void act_store2(const ActEpilogue& e, int img, size_t
 // The ACT epilogue on 4 consecutive channels n..n+3 of position `pos` (= (img*H + y)*W + x).
 __device__ __forceinline__ void act_store4(const ActEpilogue& e, int img, size_t pos, int N, int n,
                                            float4 acc, float noise) {
-  const float4 d = __ldg(reinterpret_cast<const float4*>(e.dcoef + (size_t)img * N + n));
+  const float4 d = e.dcoef ? __ldg(reinterpret_cast<const float4*>(e.dcoef + (size_t)img * N + n))
+                          : make_float4(1.f, 1.f, 1.f, 1.f);
   const float4 b = __ldg(reinterpret_cast<const float4*>(e.bias + n));
   float4 u, v;
   u.x = ((acc.x * d.x + noise) + b.x) * e.gain;
@@ -208,10 +212,10 @@ __device__ __forceinline__ void act_store4(const ActEpilogue& e, int img, size_t
   u.z = ((acc.z * d.z + noise) + b.z) * e.gain;
   u.w = ((acc.w * d.w + noise) + b.w) * e.gain;
   if (e.u_out != nullptr) *reinterpret_cast<float4*>(e.u_out + pos * N + n) = u;
-  v.x = lrelu(u.x);
-  v.y = lrelu(u.y);
-  v.z = lrelu(u.z);
-  v.w = lrelu(u.w);
+  v.x = lrelu(u.x, e.slope);
+  v.y = lrelu(u.y, e.slope);
+  v.z = lrelu(u.z, e.slope);
+  v.w = lrelu(u.w, e.slope);
   const float4 one = make_float4(1.f, 1.f, 1.f, 1.f);
   if (e.a_hi != nullptr) {
     const float4 s = e.style_a ? __ldg(reinterpret_cast<const float4*>(e.style_a + (size_t)img * N + n)) : one;
@@ -1693,6 +1697,7 @@ static int run(const nfi_synth_params& P, Bump& ws, cudaStream_t st, bool dry, c
         ActEpilogue e;
         memset(&e, 0, sizeof(e));
         e.dcoef = dco0[i]; e.noise = P.conv0[i].noise; e.bias = P.conv0[i].bias; e.gain = sqrt2;
+        e.slope = 0.2f;
         e.style_a = style1[i]; e.a_hi = y.hi; e.a_lo = y.lo;
         e.u_out = sv ? sv->u0[i] : nullptr;
         const size_t total = (size_t)B * (res / 2) * (res / 2) * (cout / 4);
@@ -1715,6 +1720,7 @@ static int run(const nfi_synth_params& P, Bump& ws, cudaStream_t st, bool dry, c
       a.mode = kModeAct;
       a.act.dcoef = dco1[i]; a.act.noise = P.conv1[i].noise; a.act.bias = P.conv1[i].bias;
       a.act.gain = sqrt2;
+      a.act.slope = 0.2f;
       a.act.style_a = style_rgb[i]; a.act.a_hi = xr.hi; a.act.a_lo = xr.lo;
       if (!last) { a.act.style_b = style0[i + 1]; a.act.b_hi = xn.hi; a.act.b_lo = xn.lo; }
       a.act.u_out = sv ? sv->u1[i] : nullptr;
@@ -2607,6 +2613,41 @@ int backward_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const nfi_sy
       (reinterpret_cast<uintptr_t>(H.scratch) + 1023) & ~(uintptr_t)1023);
   Bump s{sbase, 0, H.scratch_bytes};
   return run_hvp(P, H, sv, s, st, false, err, err_len, PG);
+}
+
+// ---- the narrow entries of nfi_synth_launch.h ----
+int conv3x3(const Conv3x3& c, cudaStream_t st, char* err, size_t err_len) {
+  ConvArgs a;
+  memset(&a, 0, sizeof(a));
+  a.B = c.B; a.C = c.C; a.N = c.N; a.H = c.H; a.W = c.W;
+  conv3x3_phases(a, c.H, c.W);
+  if (c.adjoint) {
+    for (int t = 0; t < 9; ++t) {  // the adjoint of a cross-correlation: taps flipped
+      a.tap_dy[t] = -a.tap_dy[t];
+      a.tap_dx[t] = -a.tap_dx[t];
+    }
+    a.mode = kModeRaw;
+    a.out_raw = c.raw_out; a.out_H = c.H; a.out_W = c.W; a.out_stride = 1;
+  } else {
+    a.mode = kModeAct;
+    a.act.bias = c.bias; a.act.gain = 1.f; a.act.slope = 0.f;
+    a.act.a_hi = c.out_hi; a.act.a_lo = c.out_lo;
+    a.act.u_out = c.u_out;
+  }
+  const Pair in = {const_cast<__nv_bfloat16*>(c.in_hi), const_cast<__nv_bfloat16*>(c.in_lo)};
+  const Pair wt = {const_cast<__nv_bfloat16*>(c.w_hi), const_cast<__nv_bfloat16*>(c.w_lo)};
+  return launch_conv(a, in, wt, 9, st, err, err_len);
+}
+
+int prep_weights3x3(const float* w, int cout, int cin, int transposed, __nv_bfloat16* hi,
+                    __nv_bfloat16* lo, cudaStream_t st, char* err, size_t err_len) {
+  const unsigned grid = (unsigned)(((size_t)cout * cin + 255) / 256);
+  if (transposed)
+    prep_weights_t_kernel<<<grid, 256, 0, st>>>(w, cout, cin, 9, hi, lo);
+  else
+    prep_weights_kernel<<<grid, 256, 0, st>>>(w, cout, cin, 9, hi, lo, nullptr);
+  NFI_SCUDA(cudaGetLastError());
+  return 0;
 }
 
 }  // namespace synth
