@@ -1419,6 +1419,13 @@ static int sm_count() {
   return n;
 }
 
+static unsigned blocks(size_t n, int per) { return (unsigned)((n + per - 1) / per); }
+// The grid of a grid-stride kernel over n items: one thread each, at most 16 blocks of 256 per SM
+static unsigned flat_grid(size_t n) {
+  const unsigned g = blocks(n, 256), cap = (unsigned)sm_count() * 16u;
+  return g > cap ? cap : g;
+}
+
 // One convolution launch.  `in` [map_B (default B),H,W,C] pair, weights [taps9][N][C] pair.
 static int launch_conv(ConvArgs& a, Pair in, Pair wt, int w_taps, cudaStream_t st, char* err,
                        size_t err_len, int map_B = 0) {
@@ -1504,32 +1511,47 @@ static int launch_wgrad(WgradArgs& a, Pair g, int gB, int gH, int gW, Pair x, in
   return 0;
 }
 
-static void conv3x3_phases(ConvArgs& a, int H, int W) {  // stride 1, pad 1 (cross-correlation)
+// ---- conv descriptors: one per GEMM shape the network runs on conv_tc_kernel, with its phases,
+// taps, mode and output extents; the caller sets the epilogue's pointers ----
+static ConvArgs conv_args(int B, int C, int N, int H, int W, int mode) {
+  ConvArgs a;
+  memset(&a, 0, sizeof(a));
+  a.B = B; a.C = C; a.N = N; a.H = H; a.W = W;
+  a.mode = mode;
+  return a;
+}
+// The stride-1 3x3 conv (pad 1, cross-correlation) of [B,H,W,C] into N channels; RAW writes
+// [B,H,W,N].  `adjoint` flips the taps: conv^T, the data gradient against prep_weights_t_kernel's W.
+static ConvArgs conv3x3_args(int B, int C, int N, int H, int W, int mode, bool adjoint = false) {
+  ConvArgs a = conv_args(B, C, N, H, W, mode);
   a.n_phases = 1;
   a.ph_taps[0] = 9;
-  a.ph_tap0[0] = 0;
   a.ph_DH[0] = H;
   a.ph_DW[0] = W;
-  a.ph_oy[0] = a.ph_ox[0] = 0;
+  const int sign = adjoint ? -1 : 1;
   for (int ky = 0; ky < 3; ++ky)
     for (int kx = 0; kx < 3; ++kx) {
       const int t = ky * 3 + kx;
-      a.tap_dy[t] = ky - 1;
-      a.tap_dx[t] = kx - 1;
+      a.tap_dy[t] = sign * (ky - 1);
+      a.tap_dx[t] = sign * (kx - 1);
       a.tap_w[t] = t;
     }
+  if (mode == kModeRaw) { a.out_H = H; a.out_W = W; a.out_stride = 1; }
+  return a;
 }
-// conv_transpose2d(stride 2): out[2i+ky, 2j+kx] += x[i,j] W[ky,kx].  Output parity (py,px) takes the
-// taps with ky = py (mod 2), kx = px (mod 2); position (a,b) of the phase reads x[a - ky/2, b - kx/2].
-static void conv_up_phases(ConvArgs& a, int H, int W) {
+// conv_transpose2d(stride 2) of [B,h,h,C] into the (2h+1)^2 raw result (RAW; fir_act_kernel filters
+// it): out[2i+ky, 2j+kx] += x[i,j] W[ky,kx].  Output parity (py,px) takes the taps with
+// ky = py (mod 2), kx = px (mod 2); position (a,b) of the phase reads x[a - ky/2, b - kx/2].
+static ConvArgs conv_up_args(int B, int C, int N, int h) {
+  ConvArgs a = conv_args(B, C, N, h, h, kModeRaw);
   a.n_phases = 4;
   int t = 0;
   for (int py = 0; py < 2; ++py)
     for (int px = 0; px < 2; ++px) {
       const int p = py * 2 + px;
       a.ph_tap0[p] = t;
-      a.ph_DH[p] = py ? H : H + 1;
-      a.ph_DW[p] = px ? W : W + 1;
+      a.ph_DH[p] = py ? h : h + 1;
+      a.ph_DW[p] = px ? h : h + 1;
       a.ph_oy[p] = py;
       a.ph_ox[p] = px;
       for (int ky = py; ky < 3; ky += 2)
@@ -1541,6 +1563,75 @@ static void conv_up_phases(ConvArgs& a, int H, int W) {
         }
       a.ph_taps[p] = t - a.ph_tap0[p];
     }
+  a.out_H = a.out_W = 2 * h + 1;
+  a.out_stride = 2;
+  return a;
+}
+// The adjoint of conv_up_args: the stride-2 correlation with W0 as 9 stride-1 taps over the four
+// parity phases of the raw gradient, phase (py,px) at image offset (2py+px) nimg of a
+// [4 nimg, h+1, h+1, C] pair (fir_adjoint_kernel; nimg = B, or 2B with the tangent stacked): tap
+// (ky,kx) reads phase (ky%2, kx%2) at offset (ky/2, kx/2).  RAW into [nimg,h,h,N]; the caller's
+// activation map spans all 4 nimg images.
+static ConvArgs conv_up_adjoint_args(int nimg, int C, int N, int h) {
+  ConvArgs a = conv_args(nimg, C, N, h + 1, h + 1, kModeRaw);
+  a.n_phases = 1;
+  a.ph_taps[0] = 9;
+  a.ph_DH[0] = h;
+  a.ph_DW[0] = h;
+  for (int ky = 0; ky < 3; ++ky)
+    for (int kx = 0; kx < 3; ++kx) {
+      const int t = ky * 3 + kx;
+      a.tap_dy[t] = ky / 2;
+      a.tap_dx[t] = kx / 2;
+      a.tap_w[t] = t;
+      a.tap_img[t] = ((ky & 1) * 2 + (kx & 1)) * nimg;
+    }
+  a.out_H = h; a.out_W = h; a.out_stride = 1;
+  return a;
+}
+// ToRGB, the 1x1 conv at resolution res: forward (kModeRgb) from the layer's [B,res,res,C] input
+// into the N = 96 image channels, or its adjoint (kModeRaw) from the image gradient into
+// [B,res,res,N]
+static ConvArgs torgb_args(int B, int C, int N, int res, int mode) {
+  ConvArgs a = conv_args(B, C, N, res, res, mode);
+  a.n_phases = 1;
+  a.ph_taps[0] = 1;
+  a.ph_DH[0] = res;
+  a.ph_DW[0] = res;
+  if (mode == kModeRaw) { a.out_H = res; a.out_W = res; a.out_stride = 1; }
+  return a;
+}
+
+// ---- tap tables of the weight GEMMs (plan_wgrad fills the rest) ----
+static WgradArgs wgrad_args(int cout, int cin, int taps) {
+  WgradArgs a;
+  memset(&a, 0, sizeof(a));
+  a.cout = cout; a.cin = cin; a.taps = taps;
+  return a;
+}
+// ToRGB: dimg against the layer's input at the same position
+static WgradArgs torgb_wgrad(int cout, int cin) { return wgrad_args(cout, cin, 1); }
+// conv1 (stride 1): dacc at p against x~ at p + (ky - 1, kx - 1)
+static WgradArgs conv1_wgrad(int c) {
+  WgradArgs a = wgrad_args(c, c, 9);
+  for (int t = 0; t < 9; ++t) {
+    a.x_dy[t] = t / 3 - 1;
+    a.x_dx[t] = t % 3 - 1;
+  }
+  return a;
+}
+// conv0 (up): the raw gradient at (2i+ky, 2j+kx) is phase (ky%2, kx%2) at (i + ky/2, j + kx/2), the
+// phases stacked as in conv_up_adjoint_args over nimg images each, against x~ at (i, j)
+static WgradArgs conv0_wgrad(int cout, int cin, int nimg) {
+  WgradArgs a = wgrad_args(cout, cin, 9);
+  for (int ky = 0; ky < 3; ++ky)
+    for (int kx = 0; kx < 3; ++kx) {
+      const int t = ky * 3 + kx;
+      a.a_dy[t] = ky / 2;
+      a.a_dx[t] = kx / 2;
+      a.a_img[t] = ((ky & 1) * 2 + (kx & 1)) * nimg;
+    }
+  return a;
 }
 
 struct Bump {
@@ -1559,6 +1650,13 @@ struct Bump {
     return p;
   }
 };
+
+// A Bump over a caller's buffer from its first 1024-byte boundary (the sizers add the 1024 bytes)
+static Bump aligned_bump(void* p, size_t bytes) {
+  unsigned char* base =
+      reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(p) + 1023) & ~(uintptr_t)1023);
+  return Bump{base, 0, bytes};
+}
 
 static int check_params(const nfi_synth_params& P, char* err, size_t err_len) {
   const int R = P.img_resolution;
@@ -1607,7 +1705,6 @@ static int run(const nfi_synth_params& P, Bump& ws, cudaStream_t st, bool dry, c
                Saved* sv = nullptr) {
   const int B = P.batch, nb = P.num_blocks, D = P.w_dim;
   const float sqrt2 = 1.4142135623730951f;
-  auto blocks = [](size_t n, int per) { return (unsigned)((n + per - 1) / per); };
 
   // ---- per-layer styles, demodulation coefficients, re-laid-out weights ----
   float* style0[NFI_SYNTH_MAX_BLOCKS] = {nullptr};
@@ -1686,12 +1783,8 @@ static int run(const nfi_synth_params& P, Bump& ws, cudaStream_t st, bool dry, c
       float* raw = ws.take((size_t)B * (res + 1) * (res + 1) * cout);
       Pair y = ws.pair((size_t)B * res * res * cout);
       if (!dry) {
-        ConvArgs a;
-        memset(&a, 0, sizeof(a));
-        a.B = B; a.C = cin; a.N = cout; a.H = hin; a.W = hin;
-        conv_up_phases(a, hin, hin);
-        a.mode = kModeRaw;
-        a.out_raw = raw; a.out_H = res + 1; a.out_W = res + 1; a.out_stride = 2;
+        ConvArgs a = conv_up_args(B, cin, cout, hin);
+        a.out_raw = raw;
         const int rc = launch_conv(a, x, w0[i], 9, st, err, err_len);
         if (rc) return rc;
         ActEpilogue e;
@@ -1701,9 +1794,7 @@ static int run(const nfi_synth_params& P, Bump& ws, cudaStream_t st, bool dry, c
         e.style_a = style1[i]; e.a_hi = y.hi; e.a_lo = y.lo;
         e.u_out = sv ? sv->u0[i] : nullptr;
         const size_t total = (size_t)B * (res / 2) * (res / 2) * (cout / 4);
-        unsigned grid = blocks(total, 256);
-        if (grid > (unsigned)sm_count() * 16u) grid = (unsigned)sm_count() * 16u;
-        fir_act_kernel<<<grid, 256, 0, st>>>(raw, B, res, res, cout, e);
+        fir_act_kernel<<<flat_grid(total), 256, 0, st>>>(raw, B, res, res, cout, e);
         NFI_SCUDA(cudaGetLastError());
       }
       x = y;
@@ -1713,11 +1804,7 @@ static int run(const nfi_synth_params& P, Bump& ws, cudaStream_t st, bool dry, c
     if (!last) xn = ws.pair((size_t)B * res * res * cout);
     Pair xr = ws.pair((size_t)B * res * res * cout);
     if (!dry) {
-      ConvArgs a;
-      memset(&a, 0, sizeof(a));
-      a.B = B; a.C = cout; a.N = cout; a.H = res; a.W = res;
-      conv3x3_phases(a, res, res);
-      a.mode = kModeAct;
+      ConvArgs a = conv3x3_args(B, cout, cout, res, res, kModeAct);
       a.act.dcoef = dco1[i]; a.act.noise = P.conv1[i].noise; a.act.bias = P.conv1[i].bias;
       a.act.gain = sqrt2;
       a.act.slope = 0.2f;
@@ -1730,12 +1817,7 @@ static int run(const nfi_synth_params& P, Bump& ws, cudaStream_t st, bool dry, c
     // ToRGB (1x1, K = cout) + bias + upsampled running image
     float* img = last ? nullptr : ws.take((size_t)B * res * res * P.img_channels);
     if (!dry) {
-      ConvArgs a;
-      memset(&a, 0, sizeof(a));
-      a.B = B; a.C = cout; a.N = P.img_channels; a.H = res; a.W = res;
-      a.n_phases = 1; a.ph_taps[0] = 1; a.ph_tap0[0] = 0; a.ph_DH[0] = res; a.ph_DW[0] = res;
-      a.tap_dy[0] = a.tap_dx[0] = a.tap_w[0] = 0;
-      a.mode = kModeRgb;
+      ConvArgs a = torgb_args(B, cout, P.img_channels, res, kModeRgb);
       a.act.bias = P.torgb[i].bias;
       a.skip = img_prev; a.img = img; a.planes = last ? P.planes : nullptr;
       const int rc = launch_conv(a, xr, wrgb[i], 1, st, err, err_len);
@@ -1747,12 +1829,19 @@ static int run(const nfi_synth_params& P, Bump& ws, cudaStream_t st, bool dry, c
   return 0;
 }
 
-size_t workspace_bytes(const nfi_synth_params& P) {
-  Bump b{nullptr, 0, 0};
+// A sizer: 0 for params check_params refuses, else what `layout` takes from a dry Bump plus the
+// 1024 bytes an entry may lose aligning the caller's pointer
+template <class Layout>
+static size_t sized(const nfi_synth_params& P, Layout layout) {
   char err[256];
   if (check_params(P, err, sizeof(err))) return 0;
-  run(P, b, nullptr, true, err, sizeof(err));
+  Bump b{nullptr, 0, 0};
+  layout(b, err, sizeof(err));
   return b.off + 1024;
+}
+
+size_t workspace_bytes(const nfi_synth_params& P) {
+  return sized(P, [&](Bump& b, char* err, size_t err_len) { run(P, b, nullptr, true, err, err_len); });
 }
 
 int forward(const nfi_synth_params& P, cudaStream_t st, char* err, size_t err_len) {
@@ -1767,106 +1856,126 @@ int forward(const nfi_synth_params& P, cudaStream_t st, char* err, size_t err_le
     snprintf(err, err_len, "synthesis: workspace too small (%zu < %zu bytes)", P.workspace_bytes, need);
     return 1;
   }
-  unsigned char* base = reinterpret_cast<unsigned char*>(
-      (reinterpret_cast<uintptr_t>(P.workspace) + 1023) & ~(uintptr_t)1023);
-  Bump b{base, 0, P.workspace_bytes};
+  Bump b = aligned_bump(P.workspace, P.workspace_bytes);
   return run(P, b, st, false, err, err_len);
 }
 
 // ---- backward ----
-// Walks the blocks from the last to the first.  Scratch reused across blocks (stream order keeps the
-// reuse safe): bufA holds g_rgb, then dx~ of conv1, then the raw-gradient phases of conv0; bufB the
-// dacc of conv1 (pair), then of conv0 (fp32); bufC dx~ of conv0 until the previous block's conv1
-// has consumed it.
-// With `PG` (the parameter backward) the same launches run, act_backward_kernel<true> in place of
-// <false>, and each layer's weight GEMM runs while its gradient operand is still in scratch: ToRGB
-// on dimg before the running image's adjoint overwrites it, conv1 on its dacc pair, conv0 on the
-// raw-gradient phases.  Its extra buffers (the rebuilt layer input x~ and the GEMM partials) come
-// after the plain backward's, which keep their places.
-static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, const Saved& sv, Bump& ws,
-                        cudaStream_t st, bool dry, char* err, size_t err_len,
-                        const nfi_synth_param_grads* PG = nullptr) {
-  const int B = P.batch, nb = P.num_blocks, D = P.w_dim, R = P.img_resolution, NI = P.img_channels;
-  const float sqrt2 = 1.4142135623730951f;
-  auto blocks = [](size_t n, int per) { return (unsigned)((n + per - 1) / per); };
-  auto flat_grid = [&](size_t n) {
-    unsigned g = blocks(n, 256);
-    return g > (unsigned)sm_count() * 16u ? (unsigned)sm_count() * 16u : g;
-  };
+// The scratch of the backward walk (run_backward) and of its tangent (run_hvp), for `copies` stacked
+// copies of every quantity the walk derives from ws: 1, or 2 for [q; q-dot] on 2B images.  Reused
+// across blocks (stream order keeps the reuse safe): bufA holds g_rgb, then dx~ of conv1, then the
+// raw-gradient phases of conv0; bufB the dacc of conv1 (pair), then of conv0 (fp32); bufC dx~ of
+// conv0 until the previous block's conv1 has consumed it.
+struct BackwardScratch {
+  float *bufA, *bufB, *bufC;
+  float* dimg[2];  // the running image's gradient, alternately per block (one copy: not from ws)
+  Pair dimg_p;
+  float* sums;     // the per-(b, channel) sums of every copy, zeroed once
+  size_t n_sums;
+  float *ds0[2][NFI_SYNTH_MAX_BLOCKS], *ds1[2][NFI_SYNTH_MAX_BLOCKS], *dsr[2][NFI_SYNTH_MAX_BLOCKS];
+  float *dd0[2][NFI_SYNTH_MAX_BLOCKS], *dd1[2][NFI_SYNTH_MAX_BLOCKS];  // [copy][block]
+  Pair wt0[NFI_SYNTH_MAX_BLOCKS], wt1[NFI_SYNTH_MAX_BLOCKS], wtr[NFI_SYNTH_MAX_BLOCKS];  // W^T pairs
+  Pair xt;         // the layer input x~ of the current weight GEMM, `copies` deep (or none)
+  float* part;     // the weight GEMMs' partials (or none)
+};
+
+// Takes the scratch from `ws`; x~ with `take_xt`, the partials with `plan_parts`.  The optional
+// buffers come last, so the ones every walk uses keep their places.
+static BackwardScratch backward_scratch(const nfi_synth_params& P, Bump& ws, int copies, bool take_xt,
+                                        bool plan_parts) {
+  const int B = P.batch, nb = P.num_blocks, R = P.img_resolution, NI = P.img_channels;
+  BackwardScratch s;
+  memset(&s, 0, sizeof(s));
   int cmax = 0;
   for (int i = 0; i < nb; ++i) cmax = P.channels[i] > cmax ? P.channels[i] : cmax;
-  const size_t full = (size_t)B * R * R * cmax;
-  const size_t phases = (size_t)4 * B * (R / 2 + 1) * (R / 2 + 1) * cmax;
-  float* bufA = ws.take(full > phases ? full : phases);
-  float* bufB = ws.take(full);
-  float* bufC = ws.take((size_t)B * (R / 2) * (R / 2) * cmax);
-  float* dimg[2] = {ws.take((size_t)B * R * R * NI), ws.take((size_t)B * R * R * NI)};
-  Pair dimg_p = ws.pair((size_t)B * R * R * NI);
-  // per-(b, channel) sums, zeroed once
-  float *ds0[NFI_SYNTH_MAX_BLOCKS], *ds1[NFI_SYNTH_MAX_BLOCKS], *dsr[NFI_SYNTH_MAX_BLOCKS];
-  float *dd0[NFI_SYNTH_MAX_BLOCKS], *dd1[NFI_SYNTH_MAX_BLOCKS];
+  const size_t full = (size_t)copies * B * R * R * cmax;
+  const size_t phases = (size_t)4 * copies * B * (R / 2 + 1) * (R / 2 + 1) * cmax;
+  s.bufA = ws.take(full > phases ? full : phases);  // (the HVP: also the tangent conv's raw output)
+  s.bufB = ws.take(full);
+  s.bufC = ws.take((size_t)copies * B * (R / 2) * (R / 2) * cmax);
+  s.dimg[0] = ws.take((size_t)B * R * R * NI);
+  s.dimg[1] = ws.take((size_t)B * R * R * NI);
+  s.dimg_p = ws.pair((size_t)B * R * R * NI);
   size_t small = 0;
   for (int i = 0; i < nb; ++i) small += (size_t)B * (4 * P.channels[i] + (i ? P.channels[i - 1] : 0));
-  float* sums = ws.take(small);
-  {
-    float* q = sums;
+  s.n_sums = copies * small;
+  s.sums = ws.take(s.n_sums);
+  float* q = s.sums;
+  for (int k = 0; k < copies; ++k)
     for (int i = 0; i < nb; ++i) {
       const int c = P.channels[i], ci = i ? P.channels[i - 1] : 0;
-      ds0[i] = q; q += (size_t)B * ci;
-      ds1[i] = q; q += (size_t)B * c;
-      dsr[i] = q; q += (size_t)B * c;
-      dd0[i] = q; q += (size_t)B * c;
-      dd1[i] = q; q += (size_t)B * c;
+      s.ds0[k][i] = q; q += (size_t)B * ci;
+      s.ds1[k][i] = q; q += (size_t)B * c;
+      s.dsr[k][i] = q; q += (size_t)B * c;
+      s.dd0[k][i] = q; q += (size_t)B * c;
+      s.dd1[k][i] = q; q += (size_t)B * c;
     }
-  }
-  Pair wt0[NFI_SYNTH_MAX_BLOCKS], wt1[NFI_SYNTH_MAX_BLOCKS], wtr[NFI_SYNTH_MAX_BLOCKS];
   for (int i = 0; i < nb; ++i) {
     const int c = P.channels[i], ci = i ? P.channels[i - 1] : 0;
-    if (i) wt0[i] = ws.pair((size_t)9 * c * ci);
-    wt1[i] = ws.pair((size_t)9 * c * c);
-    wtr[i] = ws.pair((size_t)NI * c);
+    if (i) s.wt0[i] = ws.pair((size_t)9 * c * ci);
+    s.wt1[i] = ws.pair((size_t)9 * c * c);
+    s.wtr[i] = ws.pair((size_t)NI * c);
   }
-  Pair xt = {nullptr, nullptr};  // the layer input x~ of the current weight GEMM
-  float* part = nullptr;         // its partials
-  auto wgrad_args = [](int cout, int cin, int taps) {
-    WgradArgs a;
-    memset(&a, 0, sizeof(a));
-    a.cout = cout; a.cin = cin; a.taps = taps;
-    return a;
-  };
-  if (PG) {
-    xt = ws.pair(full);
+  if (take_xt) s.xt = ws.pair(full);
+  if (plan_parts) {  // the largest GEMM's; ToRGB's runs on one copy (dimg does not depend on ws)
     size_t pmax = 0;
-    auto need = [&](int cout, int cin, int taps, int D_) {
-      WgradArgs a = wgrad_args(cout, cin, taps);
-      plan_wgrad(a, B, D_, D_);
-      const size_t n = (size_t)a.n_split * taps * cout * cin;
+    auto need = [&](WgradArgs a, int nimg, int D_) {
+      plan_wgrad(a, nimg, D_, D_);
+      const size_t n = (size_t)a.n_split * a.taps * a.cout * a.cin;
       pmax = n > pmax ? n : pmax;
     };
     for (int i = 0; i < nb; ++i) {
       const int res = 4 << i, c = P.channels[i];
-      need(NI, c, 1, res);
-      need(c, c, 9, res);
-      if (i) need(c, P.channels[i - 1], 9, res / 2);
+      need(torgb_wgrad(NI, c), B, res);
+      need(conv1_wgrad(c), copies * B, res);
+      if (i) need(conv0_wgrad(c, P.channels[i - 1], copies * B), copies * B, res / 2);
     }
-    part = ws.take(pmax);
+    s.part = ws.take(pmax);
   }
-  if (dry) return 0;
+  return s;
+}
 
-  NFI_SCUDA(cudaMemsetAsync(sums, 0, small * sizeof(float), st));
-  for (int i = 0; i < nb; ++i) {
+// The walk's operands that do not depend on it: every layer's W^T pair, and the planes' gradient
+// as the last block's image gradient dimg[0] (fp32 and pair)
+static int prep_backward(const nfi_synth_params& P, const float* g_planes, const BackwardScratch& s,
+                         cudaStream_t st, char* err, size_t err_len) {
+  const int B = P.batch, R = P.img_resolution, NI = P.img_channels;
+  for (int i = 0; i < P.num_blocks; ++i) {
     const int c = P.channels[i], ci = i ? P.channels[i - 1] : 0;
     if (i)
       prep_weights_t_kernel<<<blocks((size_t)c * ci, 256), 256, 0, st>>>(P.conv0[i].weight, c, ci, 9,
-                                                                         wt0[i].hi, wt0[i].lo);
+                                                                         s.wt0[i].hi, s.wt0[i].lo);
     prep_weights_t_kernel<<<blocks((size_t)c * c, 256), 256, 0, st>>>(P.conv1[i].weight, c, c, 9,
-                                                                       wt1[i].hi, wt1[i].lo);
+                                                                       s.wt1[i].hi, s.wt1[i].lo);
     prep_weights_t_kernel<<<blocks((size_t)NI * c, 256), 256, 0, st>>>(P.torgb[i].weight, NI, c, 1,
-                                                                       wtr[i].hi, wtr[i].lo);
+                                                                       s.wtr[i].hi, s.wtr[i].lo);
   }
-  planes_grad_kernel<<<flat_grid((size_t)B * R * R * NI), 256, 0, st>>>(G.g_planes, B, R, dimg[0],
-                                                                        dimg_p.hi, dimg_p.lo);
+  planes_grad_kernel<<<flat_grid((size_t)B * R * R * NI), 256, 0, st>>>(g_planes, B, R, s.dimg[0],
+                                                                        s.dimg_p.hi, s.dimg_p.lo);
   NFI_SCUDA(cudaGetLastError());
+  return 0;
+}
+
+// Walks the blocks from the last to the first.
+// With `PG` (the parameter backward) the same launches run, act_backward_kernel<true> in place of
+// <false>, and each layer's weight GEMM runs while its gradient operand is still in scratch: ToRGB
+// on dimg before the running image's adjoint overwrites it, conv1 on its dacc pair, conv0 on the
+// raw-gradient phases.  It also takes the rebuilt layer input x~ and the GEMM partials.
+static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, const Saved& sv, Bump& ws,
+                        cudaStream_t st, bool dry, char* err, size_t err_len,
+                        const nfi_synth_param_grads* PG = nullptr) {
+  const int B = P.batch, nb = P.num_blocks, D = P.w_dim, NI = P.img_channels;
+  const float sqrt2 = 1.4142135623730951f;
+  const BackwardScratch s = backward_scratch(P, ws, 1, PG != nullptr, PG != nullptr);
+  if (dry) return 0;
+  float *const bufA = s.bufA, *const bufB = s.bufB, *const bufC = s.bufC, *const part = s.part;
+  const auto& dimg = s.dimg;
+  const auto &wt0 = s.wt0, &wt1 = s.wt1, &wtr = s.wtr;
+  const auto &ds0 = s.ds0[0], &ds1 = s.ds1[0], &dsr = s.dsr[0], &dd0 = s.dd0[0], &dd1 = s.dd1[0];
+  const Pair dimg_p = s.dimg_p, xt = s.xt;
+
+  NFI_SCUDA(cudaMemsetAsync(s.sums, 0, s.n_sums * sizeof(float), st));
+  if (const int rc = prep_backward(P, G.g_planes, s, st, err, err_len)) return rc;
 
   auto act_backward = [&](ActBackward& e, int HW, int C) -> int {
     if (C % 4 != 0 || C / 4 > 256) {
@@ -1907,13 +2016,6 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
     NFI_SCUDA(cudaGetLastError());
     return 0;
   };
-  auto stride1_taps = [](ConvArgs& a, int H, int W) {  // the adjoint of conv3x3_phases: taps flipped
-    conv3x3_phases(a, H, W);
-    for (int t = 0; t < 9; ++t) {
-      a.tap_dy[t] = -a.tap_dy[t];
-      a.tap_dx[t] = -a.tap_dx[t];
-    }
-  };
 
   int cur = 0;  // dimg[cur] is the gradient of block i's running image
   for (int i = nb - 1; i >= 0; --i) {
@@ -1921,12 +2023,8 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
     const bool last = (i == nb - 1);
     // ToRGB: g = dimg Wrgb^T  [B,res,res,c] -> bufA
     {
-      ConvArgs a;
-      memset(&a, 0, sizeof(a));
-      a.B = B; a.C = NI; a.N = c; a.H = res; a.W = res;
-      a.n_phases = 1; a.ph_taps[0] = 1; a.ph_DH[0] = res; a.ph_DW[0] = res;
-      a.mode = kModeRaw;
-      a.out_raw = bufA; a.out_H = res; a.out_W = res; a.out_stride = 1;
+      ConvArgs a = torgb_args(B, NI, c, res, kModeRaw);
+      a.out_raw = bufA;
       const int rc = launch_conv(a, dimg_p, wtr[i], 1, st, err, err_len);
       if (rc) return rc;
     }
@@ -1938,7 +2036,7 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
       }
       if (L.g_weight != nullptr) {
         restyle(sv.u1[i], sv.style_rgb[i], HW, c);
-        WgradArgs a = wgrad_args(NI, c, 1);
+        WgradArgs a = torgb_wgrad(NI, c);
         if (int rc = wgrad(a, dimg_p, B, res, res, P.torgb[i].weight, nullptr, nullptr, nullptr, L.g_weight))
           return rc;
       }
@@ -1977,12 +2075,8 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
         if (PG) affine(ds0[i + 1], PG->conv0[i + 1], c, sv.row0[i + 1], 1.f);
       }
       // dx~ of conv1 = conv^T(dacc, W1) -> bufA
-      ConvArgs a;
-      memset(&a, 0, sizeof(a));
-      a.B = B; a.C = c; a.N = c; a.H = res; a.W = res;
-      stride1_taps(a, res, res);
-      a.mode = kModeRaw;
-      a.out_raw = bufA; a.out_H = res; a.out_W = res; a.out_stride = 1;
+      ConvArgs a = conv3x3_args(B, c, c, res, res, kModeRaw, true);
+      a.out_raw = bufA;
       const int rc = launch_conv(a, pb, wt1[i], 9, st, err, err_len);
       if (rc) return rc;
       if (PG && PG->conv1[i].g_weight != nullptr) {  // dacc against x~ = lrelu(u0) s1 (const s1)
@@ -1991,11 +2085,7 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
         else
           const_input_kernel<<<blocks((size_t)B * 16 * c, 256), 256, 0, st>>>(P.const_input, sv.style1[0],
                                                                              B, c, xt.hi, xt.lo);
-        WgradArgs w = wgrad_args(c, c, 9);
-        for (int t = 0; t < 9; ++t) {
-          w.x_dy[t] = t / 3 - 1;
-          w.x_dx[t] = t % 3 - 1;
-        }
+        WgradArgs w = conv1_wgrad(c);
         if (int rc2 = wgrad(w, pb, B, res, res, P.conv1[i].weight, dd1[i], sv.dco1[i], sv.style1[i],
                             PG->conv1[i].g_weight))
           return rc2;
@@ -2044,32 +2134,13 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
         // raw gradient at (2i+ky, 2j+kx) = phase (ky%2, kx%2) at (i + ky/2, j + kx/2), against
         // x~ = lrelu(u1 of block i-1) s0 on the low-resolution grid
         restyle(sv.u1[i - 1], sv.style0[i], h * h, ci);
-        WgradArgs w = wgrad_args(c, ci, 9);
-        for (int ky = 0; ky < 3; ++ky)
-          for (int kx = 0; kx < 3; ++kx) {
-            const int t = ky * 3 + kx;
-            w.a_dy[t] = ky / 2;
-            w.a_dx[t] = kx / 2;
-            w.a_img[t] = ((ky & 1) * 2 + (kx & 1)) * B;
-          }
+        WgradArgs w = conv0_wgrad(c, ci, B);
         if (int rc = wgrad(w, ph, 4 * B, h + 1, h, P.conv0[i].weight, dd0[i], sv.dco0[i], sv.style0[i],
                            PG->conv0[i].g_weight))
           return rc;
       }
-      ConvArgs a;
-      memset(&a, 0, sizeof(a));
-      a.B = B; a.C = c; a.N = ci; a.H = h + 1; a.W = h + 1;
-      a.n_phases = 1; a.ph_taps[0] = 9; a.ph_DH[0] = h; a.ph_DW[0] = h;
-      for (int ky = 0; ky < 3; ++ky)
-        for (int kx = 0; kx < 3; ++kx) {
-          const int t = ky * 3 + kx;
-          a.tap_dy[t] = ky / 2;
-          a.tap_dx[t] = kx / 2;
-          a.tap_w[t] = t;
-          a.tap_img[t] = ((ky & 1) * 2 + (kx & 1)) * B;
-        }
-      a.mode = kModeRaw;
-      a.out_raw = bufC; a.out_H = h; a.out_W = h; a.out_stride = 1;
+      ConvArgs a = conv_up_adjoint_args(B, c, ci, h);
+      a.out_raw = bufC;
       const int rc = launch_conv(a, ph, wt0[i], 9, st, err, err_len, 4 * B);
       if (rc) return rc;
     }
@@ -2082,16 +2153,20 @@ static int saved_layout(const nfi_synth_params& P, Bump& b, Saved& sv, char* err
   return run(P, b, nullptr, true, err, err_len, &sv);
 }
 
-size_t saved_workspace_bytes(const nfi_synth_params& P) {
-  char err[256];
-  if (check_params(P, err, sizeof(err))) return 0;
-  Bump b{nullptr, 0, 0};
-  Saved sv;
-  memset(&sv, 0, sizeof(sv));
-  saved_layout(P, b, sv, err, sizeof(err));
-  nfi_synth_grads g = {nullptr, nullptr};
-  run_backward(P, g, sv, b, nullptr, true, err, sizeof(err));
-  return b.off + 1024;
+// The saved forward and, after it, the backward's scratch (with PG, the parameter backward's)
+static size_t backward_bytes(const nfi_synth_params& P, const nfi_synth_param_grads* PG) {
+  return sized(P, [&](Bump& b, char* err, size_t err_len) {
+    Saved sv{};
+    saved_layout(P, b, sv, err, err_len);
+    run_backward(P, nfi_synth_grads{}, sv, b, nullptr, true, err, err_len, PG);
+  });
+}
+
+size_t saved_workspace_bytes(const nfi_synth_params& P) { return backward_bytes(P, nullptr); }
+
+size_t param_workspace_bytes(const nfi_synth_params& P) {
+  const nfi_synth_param_grads pg{};
+  return backward_bytes(P, &pg);
 }
 
 static int check_saved(const nfi_synth_params& P, char* err, size_t err_len) {
@@ -2110,35 +2185,51 @@ static int check_saved(const nfi_synth_params& P, char* err, size_t err_len) {
   return 0;
 }
 
-int forward_saved(const nfi_synth_params& P, cudaStream_t st, char* err, size_t err_len) {
+// The prologue of every entry that uses the saved workspace: the checks (the params and the saved
+// workspace's size; g_planes and g_ws where G is given; the parameter backward's larger workspace
+// with `param_ws`), then the Bump over the aligned workspace and, where `sv` is given, the saved
+// forward's pointers, which leave the Bump past the saved forward.
+static int open_saved(const nfi_synth_params& P, const nfi_synth_grads* G, bool param_ws, Bump& b,
+                      Saved* sv, char* err, size_t err_len) {
   if (const int rc = check_saved(P, err, err_len)) return rc;
-  unsigned char* base = reinterpret_cast<unsigned char*>(
-      (reinterpret_cast<uintptr_t>(P.workspace) + 1023) & ~(uintptr_t)1023);
-  Bump b{base, 0, P.workspace_bytes};
-  Saved sv;
-  memset(&sv, 0, sizeof(sv));
+  if (G != nullptr && (G->g_planes == nullptr || G->g_ws == nullptr)) {
+    snprintf(err, err_len, "synthesis backward: g_planes and g_ws must be set");
+    return 1;
+  }
+  if (param_ws) {
+    const size_t need = param_workspace_bytes(P);
+    if (P.workspace_bytes < need) {
+      snprintf(err, err_len, "synthesis parameter backward: workspace too small (%zu < %zu bytes)",
+               P.workspace_bytes, need);
+      return 1;
+    }
+  }
+  b = aligned_bump(P.workspace, P.workspace_bytes);
+  if (sv == nullptr) return 0;
+  *sv = Saved{};
+  return saved_layout(P, b, *sv, err, err_len);
+}
+
+int forward_saved(const nfi_synth_params& P, cudaStream_t st, char* err, size_t err_len) {
+  Bump b;
+  if (const int rc = open_saved(P, nullptr, false, b, nullptr, err, err_len)) return rc;
+  Saved sv{};
   return run(P, b, st, false, err, err_len, &sv);
 }
 
 int backward(const nfi_synth_params& P, const nfi_synth_grads& G, cudaStream_t st, char* err,
              size_t err_len) {
-  if (const int rc = check_saved(P, err, err_len)) return rc;
-  if (G.g_planes == nullptr || G.g_ws == nullptr) {
-    snprintf(err, err_len, "synthesis backward: g_planes and g_ws must be set");
-    return 1;
-  }
-  unsigned char* base = reinterpret_cast<unsigned char*>(
-      (reinterpret_cast<uintptr_t>(P.workspace) + 1023) & ~(uintptr_t)1023);
-  Bump b{base, 0, P.workspace_bytes};
+  Bump b;
   Saved sv;
-  memset(&sv, 0, sizeof(sv));
-  if (const int rc = saved_layout(P, b, sv, err, err_len)) return rc;
+  if (const int rc = open_saved(P, &G, false, b, &sv, err, err_len)) return rc;
   return run_backward(P, G, sv, b, st, false, err, err_len);
 }
 
 int saved_preactivation(const nfi_synth_params& P, int block, int which, float* out, cudaStream_t st,
                         char* err, size_t err_len) {
-  if (const int rc = check_saved(P, err, err_len)) return rc;
+  Bump b;
+  Saved sv;
+  if (const int rc = open_saved(P, nullptr, false, b, &sv, err, err_len)) return rc;
   if (block < 0 || block >= P.num_blocks || (which != 0 && which != 1) || (which == 0 && block == 0)) {
     snprintf(err, err_len, "synthesis pre-activation: no layer (block %d, which %d)", block, which);
     return 1;
@@ -2147,12 +2238,6 @@ int saved_preactivation(const nfi_synth_params& P, int block, int which, float* 
     snprintf(err, err_len, "synthesis pre-activation: out must be set");
     return 1;
   }
-  unsigned char* base = reinterpret_cast<unsigned char*>(
-      (reinterpret_cast<uintptr_t>(P.workspace) + 1023) & ~(uintptr_t)1023);
-  Bump b{base, 0, P.workspace_bytes};
-  Saved sv;
-  memset(&sv, 0, sizeof(sv));
-  if (const int rc = saved_layout(P, b, sv, err, err_len)) return rc;
   const int res = 4 << block;
   const size_t n = (size_t)P.batch * res * res * P.channels[block];
   NFI_SCUDA(cudaMemcpyAsync(out, which ? sv.u1[block] : sv.u0[block], n * sizeof(float),
@@ -2160,39 +2245,11 @@ int saved_preactivation(const nfi_synth_params& P, int block, int which, float* 
   return 0;
 }
 
-size_t param_workspace_bytes(const nfi_synth_params& P) {
-  char err[256];
-  if (check_params(P, err, sizeof(err))) return 0;
-  Bump b{nullptr, 0, 0};
-  Saved sv;
-  memset(&sv, 0, sizeof(sv));
-  saved_layout(P, b, sv, err, sizeof(err));
-  nfi_synth_grads g = {nullptr, nullptr};
-  nfi_synth_param_grads pg;
-  memset(&pg, 0, sizeof(pg));
-  run_backward(P, g, sv, b, nullptr, true, err, sizeof(err), &pg);
-  return b.off + 1024;
-}
-
 int backward_params(const nfi_synth_params& P, const nfi_synth_grads& G, const nfi_synth_param_grads& PG,
                     cudaStream_t st, char* err, size_t err_len) {
-  if (const int rc = check_saved(P, err, err_len)) return rc;
-  if (G.g_planes == nullptr || G.g_ws == nullptr) {
-    snprintf(err, err_len, "synthesis backward: g_planes and g_ws must be set");
-    return 1;
-  }
-  const size_t need = param_workspace_bytes(P);
-  if (P.workspace_bytes < need) {
-    snprintf(err, err_len, "synthesis parameter backward: workspace too small (%zu < %zu bytes)",
-             P.workspace_bytes, need);
-    return 1;
-  }
-  unsigned char* base = reinterpret_cast<unsigned char*>(
-      (reinterpret_cast<uintptr_t>(P.workspace) + 1023) & ~(uintptr_t)1023);
-  Bump b{base, 0, P.workspace_bytes};
+  Bump b;
   Saved sv;
-  memset(&sv, 0, sizeof(sv));
-  if (const int rc = saved_layout(P, b, sv, err, err_len)) return rc;
+  if (const int rc = open_saved(P, &G, true, b, &sv, err, err_len)) return rc;
   return run_backward(P, G, sv, b, st, false, err, err_len, &PG);
 }
 
@@ -2205,50 +2262,19 @@ int backward_params(const nfi_synth_params& P, const nfi_synth_grads& G, const n
 // is the product rule's two terms).  Buffers as in run_backward, with room for 2B images.
 static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Saved& sv, Bump& ws,
                    cudaStream_t st, bool dry, char* err, size_t err_len, const nfi_synth_param_grads* PG) {
-  const int B = P.batch, B2 = 2 * B, nb = P.num_blocks, D = P.w_dim, R = P.img_resolution,
-            NI = P.img_channels;
+  const int B = P.batch, B2 = 2 * B, nb = P.num_blocks, D = P.w_dim, NI = P.img_channels;
   const float sqrt2 = 1.4142135623730951f;
-  auto blocks = [](size_t n, int per) { return (unsigned)((n + per - 1) / per); };
-  auto flat_grid = [&](size_t n) {
-    unsigned g = blocks(n, 256);
-    return g > (unsigned)sm_count() * 16u ? (unsigned)sm_count() * 16u : g;
-  };
-  int cmax = 0;
-  for (int i = 0; i < nb; ++i) cmax = P.channels[i] > cmax ? P.channels[i] : cmax;
-  const size_t full = (size_t)B * R * R * cmax;
-  const size_t phases = (size_t)8 * B * (R / 2 + 1) * (R / 2 + 1) * cmax;
-  float* bufA = ws.take(2 * full > phases ? 2 * full : phases);  // also the tangent conv's raw output
-  float* bufB = ws.take(2 * full);
-  float* bufC = ws.take((size_t)B2 * (R / 2) * (R / 2) * cmax);
-  float* dimg[2] = {ws.take((size_t)B * R * R * NI), ws.take((size_t)B * R * R * NI)};
-  Pair dimg_p = ws.pair((size_t)B * R * R * NI);
-  Pair xt = ws.pair(2 * full);  // [x~-dot; x~]: the tangent conv's input, the weight GEMMs' X
+  // xt is [x~-dot; x~]: the tangent conv's input, the weight GEMMs' X
+  const BackwardScratch s = backward_scratch(P, ws, 2, true, PG != nullptr);
+  // u-dot of every layer, and the style and dcoef tangents
   float *ud0[NFI_SYNTH_MAX_BLOCKS] = {nullptr}, *ud1[NFI_SYNTH_MAX_BLOCKS];
   for (int i = 0; i < nb; ++i) {
     const size_t n = (size_t)B * (4 << i) * (4 << i) * P.channels[i];
     if (i) ud0[i] = ws.take(n);
     ud1[i] = ws.take(n);
   }
-  // per-(b, channel) sums and their tangents (zeroed once), style and dcoef tangents
-  float *ds0[2][NFI_SYNTH_MAX_BLOCKS], *ds1[2][NFI_SYNTH_MAX_BLOCKS], *dsr[2][NFI_SYNTH_MAX_BLOCKS];
-  float *dd0[2][NFI_SYNTH_MAX_BLOCKS], *dd1[2][NFI_SYNTH_MAX_BLOCKS];
   float *sd0[NFI_SYNTH_MAX_BLOCKS], *sd1[NFI_SYNTH_MAX_BLOCKS], *sdr[NFI_SYNTH_MAX_BLOCKS];
   float *ddot0[NFI_SYNTH_MAX_BLOCKS], *ddot1[NFI_SYNTH_MAX_BLOCKS];
-  size_t small = 0;
-  for (int i = 0; i < nb; ++i) small += (size_t)B * (4 * P.channels[i] + (i ? P.channels[i - 1] : 0));
-  float* sums = ws.take(2 * small);
-  {
-    float* q = sums;
-    for (int k = 0; k < 2; ++k)
-      for (int i = 0; i < nb; ++i) {
-        const int c = P.channels[i], ci = i ? P.channels[i - 1] : 0;
-        ds0[k][i] = q; q += (size_t)B * ci;
-        ds1[k][i] = q; q += (size_t)B * c;
-        dsr[k][i] = q; q += (size_t)B * c;
-        dd0[k][i] = q; q += (size_t)B * c;
-        dd1[k][i] = q; q += (size_t)B * c;
-      }
-  }
   for (int i = 0; i < nb; ++i) {
     const int c = P.channels[i], ci = i ? P.channels[i - 1] : 0;
     sd0[i] = i ? ws.take((size_t)B * ci) : nullptr;
@@ -2257,39 +2283,14 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
     ddot1[i] = ws.take((size_t)B * c);
     sdr[i] = ws.take((size_t)B * c);
   }
-  Pair wt0[NFI_SYNTH_MAX_BLOCKS], wt1[NFI_SYNTH_MAX_BLOCKS], wtr[NFI_SYNTH_MAX_BLOCKS];
-  for (int i = 0; i < nb; ++i) {
-    const int c = P.channels[i], ci = i ? P.channels[i - 1] : 0;
-    if (i) wt0[i] = ws.pair((size_t)9 * c * ci);
-    wt1[i] = ws.pair((size_t)9 * c * c);
-    wtr[i] = ws.pair((size_t)NI * c);
-  }
-  auto wgrad_args = [](int cout, int cin, int taps) {
-    WgradArgs a;
-    memset(&a, 0, sizeof(a));
-    a.cout = cout; a.cin = cin; a.taps = taps;
-    return a;
-  };
-  float* part = nullptr;
-  if (PG) {
-    size_t pmax = 0;
-    auto need = [&](int cout, int cin, int taps, int D_, int nimg) {
-      WgradArgs a = wgrad_args(cout, cin, taps);
-      plan_wgrad(a, nimg, D_, D_);
-      const size_t n = (size_t)a.n_split * taps * cout * cin;
-      pmax = n > pmax ? n : pmax;
-    };
-    for (int i = 0; i < nb; ++i) {
-      const int res = 4 << i, c = P.channels[i];
-      need(NI, c, 1, res, B);
-      need(c, c, 9, res, B2);
-      if (i) need(c, P.channels[i - 1], 9, res / 2, B2);
-    }
-    part = ws.take(pmax);
-  }
   if (dry) return 0;
+  float *const bufA = s.bufA, *const bufB = s.bufB, *const bufC = s.bufC, *const part = s.part;
+  const auto& dimg = s.dimg;
+  const auto &wt0 = s.wt0, &wt1 = s.wt1, &wtr = s.wtr;
+  const auto &ds0 = s.ds0, &ds1 = s.ds1, &dsr = s.dsr, &dd0 = s.dd0, &dd1 = s.dd1;  // [0]: q, [1]: q-dot
+  const Pair dimg_p = s.dimg_p, xt = s.xt;
 
-  NFI_SCUDA(cudaMemsetAsync(sums, 0, 2 * small * sizeof(float), st));
+  NFI_SCUDA(cudaMemsetAsync(s.sums, 0, s.n_sums * sizeof(float), st));
   // ---- tangent forward ----
   auto style_dot = [&](const nfi_synth_layer& L, int c, int row, float gain, float* out) {
     styles_kernel<<<blocks((size_t)B * c * 32, 256), 256, 0, st>>>(H.t_ws + (size_t)row * D, P.num_ws * D, D,
@@ -2320,12 +2321,8 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
     if (i) {  // conv0: x~-dot on the low-resolution grid, the four phase GEMMs, FIR + tangent epilogue
       const int h = res / 2;
       restyle_dot(sv.u1[i - 1], ud1[i - 1], sv.style0[i], sd0[i], h * h, ci, xt);
-      ConvArgs a;
-      memset(&a, 0, sizeof(a));
-      a.B = B; a.C = ci; a.N = c; a.H = h; a.W = h;
-      conv_up_phases(a, h, h);
-      a.mode = kModeRaw;
-      a.out_raw = bufA; a.out_H = res + 1; a.out_W = res + 1; a.out_stride = 2;
+      ConvArgs a = conv_up_args(B, ci, c, h);
+      a.out_raw = bufA;
       if (const int rc = launch_conv(a, xt, sv.w0[i], 9, st, err, err_len)) return rc;
       const size_t total = (size_t)B * h * h * (c / 4);
       fir_act_kernel<<<flat_grid(total), 256, 0, st>>>(bufA, B, res, res, c,
@@ -2336,12 +2333,8 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
       const_input_kernel<<<blocks((size_t)B * 16 * c, 256), 256, 0, st>>>(P.const_input, sd1[0], B, c, xt.hi,
                                                                          xt.lo);
     }
-    ConvArgs a;
-    memset(&a, 0, sizeof(a));
-    a.B = B; a.C = c; a.N = c; a.H = res; a.W = res;
-    conv3x3_phases(a, res, res);
-    a.mode = kModeRaw;
-    a.out_raw = bufA; a.out_H = res; a.out_W = res; a.out_stride = 1;
+    ConvArgs a = conv3x3_args(B, c, c, res, res, kModeRaw);
+    a.out_raw = bufA;
     if (const int rc = launch_conv(a, xt, sv.w1[i], 9, st, err, err_len)) return rc;
     tangent_act_kernel<<<flat_grid((size_t)B * HW * c / 4), 256, 0, st>>>(
         bufA, B, HW, c, tangent_epi(P.conv1[i], sv.dco1[i], ddot1[i], sv.u1[i], ud1[i]));
@@ -2349,19 +2342,7 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
   }
 
   // ---- the backward and its tangent, last block first ----
-  for (int i = 0; i < nb; ++i) {
-    const int c = P.channels[i], ci = i ? P.channels[i - 1] : 0;
-    if (i)
-      prep_weights_t_kernel<<<blocks((size_t)c * ci, 256), 256, 0, st>>>(P.conv0[i].weight, c, ci, 9,
-                                                                         wt0[i].hi, wt0[i].lo);
-    prep_weights_t_kernel<<<blocks((size_t)c * c, 256), 256, 0, st>>>(P.conv1[i].weight, c, c, 9,
-                                                                       wt1[i].hi, wt1[i].lo);
-    prep_weights_t_kernel<<<blocks((size_t)NI * c, 256), 256, 0, st>>>(P.torgb[i].weight, NI, c, 1,
-                                                                       wtr[i].hi, wtr[i].lo);
-  }
-  planes_grad_kernel<<<flat_grid((size_t)B * R * R * NI), 256, 0, st>>>(H.g_planes, B, R, dimg[0],
-                                                                        dimg_p.hi, dimg_p.lo);
-  NFI_SCUDA(cudaGetLastError());
+  if (const int rc = prep_backward(P, H.g_planes, s, st, err, err_len)) return rc;
 
   auto act_backward = [&](ActBackwardTangent& e, int HW, int C) -> int {
     if (C % 4 != 0 || C / 4 > 256) {
@@ -2415,17 +2396,13 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
     const bool last = (i == nb - 1);
     const size_t n1 = (size_t)B * HW * c;  // one half of a stacked full-resolution tensor
     {  // ToRGB: dx~ = dimg Wrgb^T -> bufA (its tangent is 0: dimg does not depend on ws)
-      ConvArgs a;
-      memset(&a, 0, sizeof(a));
-      a.B = B; a.C = NI; a.N = c; a.H = res; a.W = res;
-      a.n_phases = 1; a.ph_taps[0] = 1; a.ph_DH[0] = res; a.ph_DW[0] = res;
-      a.mode = kModeRaw;
-      a.out_raw = bufA; a.out_H = res; a.out_W = res; a.out_stride = 1;
+      ConvArgs a = torgb_args(B, NI, c, res, kModeRaw);
+      a.out_raw = bufA;
       if (const int rc = launch_conv(a, dimg_p, wtr[i], 1, st, err, err_len)) return rc;
     }
     if (PG && PG->torgb[i].g_weight != nullptr) {  // dimg against x~-dot of ToRGB
       restyle_dot(sv.u1[i], ud1[i], sv.style_rgb[i], sdr[i], HW, c, xt);
-      WgradArgs a = wgrad_args(NI, c, 1);
+      WgradArgs a = torgb_wgrad(NI, c);
       if (int rc = wgrad(a, dimg_p, B, res, res, B, P.torgb[i].weight, nullptr, nullptr, nullptr, nullptr,
                          nullptr, PG->torgb[i].g_weight))
         return rc;
@@ -2467,16 +2444,8 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
               PG ? &PG->conv0[i + 1] : nullptr);
     }
     {  // [dx~; dx~-dot] of conv1 = conv^T([dacc; dacc-dot], W1) -> bufA
-      ConvArgs a;
-      memset(&a, 0, sizeof(a));
-      a.B = B2; a.C = c; a.N = c; a.H = res; a.W = res;
-      conv3x3_phases(a, res, res);
-      for (int t = 0; t < 9; ++t) {
-        a.tap_dy[t] = -a.tap_dy[t];
-        a.tap_dx[t] = -a.tap_dx[t];
-      }
-      a.mode = kModeRaw;
-      a.out_raw = bufA; a.out_H = res; a.out_W = res; a.out_stride = 1;
+      ConvArgs a = conv3x3_args(B2, c, c, res, res, kModeRaw, true);
+      a.out_raw = bufA;
       if (const int rc = launch_conv(a, pb, wt1[i], 9, st, err, err_len)) return rc;
     }
     if (PG && PG->conv1[i].g_weight != nullptr) {  // [dacc; dacc-dot] against [x~-dot; x~]
@@ -2488,11 +2457,7 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
         const_input_kernel<<<blocks(n1, 256), 256, 0, st>>>(P.const_input, sv.style1[0], B, c, xt.hi + n1,
                                                             xt.lo + n1);
       }
-      WgradArgs w = wgrad_args(c, c, 9);
-      for (int t = 0; t < 9; ++t) {
-        w.x_dy[t] = t / 3 - 1;
-        w.x_dx[t] = t % 3 - 1;
-      }
+      WgradArgs w = conv1_wgrad(c);
       float* dd[2] = {dd1[0][i], dd1[1][i]};
       if (int rc = wgrad(w, pb, B2, res, res, B2, P.conv1[i].weight, dd, sv.dco1[i], ddot1[i], sv.style1[i],
                          sd1[i], PG->conv1[i].g_weight))
@@ -2541,33 +2506,14 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
         restyle_dot(sv.u1[i - 1], ud1[i - 1], sv.style0[i], sd0[i], h * h, ci, xt);
         restyle_kernel<<<flat_grid(nl / 4), 256, 0, st>>>(sv.u1[i - 1], sv.style0[i], B, h * h, ci, xt.hi + nl,
                                                           xt.lo + nl);
-        WgradArgs w = wgrad_args(c, ci, 9);
-        for (int ky = 0; ky < 3; ++ky)
-          for (int kx = 0; kx < 3; ++kx) {
-            const int t = ky * 3 + kx;
-            w.a_dy[t] = ky / 2;
-            w.a_dx[t] = kx / 2;
-            w.a_img[t] = ((ky & 1) * 2 + (kx & 1)) * B2;
-          }
+        WgradArgs w = conv0_wgrad(c, ci, B2);
         float* dd[2] = {dd0[0][i], dd0[1][i]};
         if (int rc = wgrad(w, ph, 4 * B2, h + 1, h, B2, P.conv0[i].weight, dd, sv.dco0[i], ddot0[i],
                            sv.style0[i], sd0[i], PG->conv0[i].g_weight))
           return rc;
       }
-      ConvArgs a;
-      memset(&a, 0, sizeof(a));
-      a.B = B2; a.C = c; a.N = ci; a.H = h + 1; a.W = h + 1;
-      a.n_phases = 1; a.ph_taps[0] = 9; a.ph_DH[0] = h; a.ph_DW[0] = h;
-      for (int ky = 0; ky < 3; ++ky)
-        for (int kx = 0; kx < 3; ++kx) {
-          const int t = ky * 3 + kx;
-          a.tap_dy[t] = ky / 2;
-          a.tap_dx[t] = kx / 2;
-          a.tap_w[t] = t;
-          a.tap_img[t] = ((ky & 1) * 2 + (kx & 1)) * B2;
-        }
-      a.mode = kModeRaw;
-      a.out_raw = bufC; a.out_H = h; a.out_W = h; a.out_stride = 1;
+      ConvArgs a = conv_up_adjoint_args(B2, c, ci, h);
+      a.out_raw = bufC;
       if (const int rc = launch_conv(a, ph, wt0[i], 9, st, err, err_len, 4 * B2)) return rc;
     }
   }
@@ -2576,24 +2522,18 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
 }
 
 size_t hvp_scratch_bytes(const nfi_synth_params& P) {
-  char err[256];
-  if (check_params(P, err, sizeof(err))) return 0;
-  Bump b{nullptr, 0, 0};
-  Saved sv;
-  memset(&sv, 0, sizeof(sv));
-  saved_layout(P, b, sv, err, sizeof(err));
-  Bump h{nullptr, 0, 0};
-  nfi_synth_hvp hv;
-  memset(&hv, 0, sizeof(hv));
-  nfi_synth_param_grads pg;
-  memset(&pg, 0, sizeof(pg));
-  run_hvp(P, hv, sv, h, nullptr, true, err, sizeof(err), &pg);
-  return h.off + 1024;
+  return sized(P, [&](Bump& b, char* err, size_t err_len) {
+    const Saved sv{};  // (the dry walk reads no saved pointer)
+    const nfi_synth_param_grads pg{};
+    run_hvp(P, nfi_synth_hvp{}, sv, b, nullptr, true, err, err_len, &pg);
+  });
 }
 
 int backward_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const nfi_synth_param_grads* PG,
                  cudaStream_t st, char* err, size_t err_len) {
-  if (const int rc = check_saved(P, err, err_len)) return rc;
+  Bump b;
+  Saved sv;
+  if (const int rc = open_saved(P, nullptr, false, b, &sv, err, err_len)) return rc;
   if (H.g_planes == nullptr || H.t_ws == nullptr || H.g_ws == nullptr || H.scratch == nullptr) {
     snprintf(err, err_len, "synthesis HVP: g_planes, t_ws, g_ws and scratch must be set");
     return 1;
@@ -2603,33 +2543,16 @@ int backward_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const nfi_sy
     snprintf(err, err_len, "synthesis HVP: scratch too small (%zu < %zu bytes)", H.scratch_bytes, need);
     return 1;
   }
-  unsigned char* base = reinterpret_cast<unsigned char*>(
-      (reinterpret_cast<uintptr_t>(P.workspace) + 1023) & ~(uintptr_t)1023);
-  Bump b{base, 0, P.workspace_bytes};
-  Saved sv;
-  memset(&sv, 0, sizeof(sv));
-  if (const int rc = saved_layout(P, b, sv, err, err_len)) return rc;
-  unsigned char* sbase = reinterpret_cast<unsigned char*>(
-      (reinterpret_cast<uintptr_t>(H.scratch) + 1023) & ~(uintptr_t)1023);
-  Bump s{sbase, 0, H.scratch_bytes};
+  Bump s = aligned_bump(H.scratch, H.scratch_bytes);
   return run_hvp(P, H, sv, s, st, false, err, err_len, PG);
 }
 
 // ---- the narrow entries of nfi_synth_launch.h ----
 int conv3x3(const Conv3x3& c, cudaStream_t st, char* err, size_t err_len) {
-  ConvArgs a;
-  memset(&a, 0, sizeof(a));
-  a.B = c.B; a.C = c.C; a.N = c.N; a.H = c.H; a.W = c.W;
-  conv3x3_phases(a, c.H, c.W);
+  ConvArgs a = conv3x3_args(c.B, c.C, c.N, c.H, c.W, c.adjoint ? kModeRaw : kModeAct, c.adjoint != 0);
   if (c.adjoint) {
-    for (int t = 0; t < 9; ++t) {  // the adjoint of a cross-correlation: taps flipped
-      a.tap_dy[t] = -a.tap_dy[t];
-      a.tap_dx[t] = -a.tap_dx[t];
-    }
-    a.mode = kModeRaw;
-    a.out_raw = c.raw_out; a.out_H = c.H; a.out_W = c.W; a.out_stride = 1;
+    a.out_raw = c.raw_out;
   } else {
-    a.mode = kModeAct;
     a.act.bias = c.bias; a.act.gain = 1.f; a.act.slope = 0.f;
     a.act.a_hi = c.out_hi; a.act.a_lo = c.out_lo;
     a.act.u_out = c.u_out;
@@ -2641,7 +2564,7 @@ int conv3x3(const Conv3x3& c, cudaStream_t st, char* err, size_t err_len) {
 
 int prep_weights3x3(const float* w, int cout, int cin, int transposed, __nv_bfloat16* hi,
                     __nv_bfloat16* lo, cudaStream_t st, char* err, size_t err_len) {
-  const unsigned grid = (unsigned)(((size_t)cout * cin + 255) / 256);
+  const unsigned grid = blocks((size_t)cout * cin, 256);
   if (transposed)
     prep_weights_t_kernel<<<grid, 256, 0, st>>>(w, cout, cin, 9, hi, lo);
   else
