@@ -159,9 +159,32 @@ class LpipsParams(ctypes.Structure):
     ]
 
 
+ENCODER_MAPS = 4
+
+
+class EncoderParams(ctypes.Structure):
+    """struct nfi_encoder_params (include/nfi_encoder.h)."""
+    _fields_ = [
+        ('batch', ctypes.c_int32), ('height', ctypes.c_int32), ('width', ctypes.c_int32),
+        ('channels', ctypes.c_int32), ('pose_regressor', ctypes.c_int32),
+        ('latent_regressor', ctypes.c_int32), ('save', ctypes.c_int32),
+    ] + [(n, ctypes.c_void_p) for n in (
+        'features', 'features_latent', 'post0_w', 'post0_b', 'post2_w', 'post2_b', 'post4_w',
+        'post4_b', 'wpre_w', 'wpre_b', 'maps', 'pooled', 'workspace')] + [
+        ('workspace_bytes', ctypes.c_size_t)]
+
+
+class EncoderGrads(ctypes.Structure):
+    """struct nfi_encoder_grads."""
+    _fields_ = [(n, ctypes.c_void_p) for n in (
+        'g_features', 'g_features_latent', 'g_post0_w', 'g_post0_b', 'g_post2_w', 'g_post2_b',
+        'g_post4_w', 'g_post4_b', 'g_wpre_w', 'g_wpre_b')]
+
+
 # every symbol include/nfi_render.h, nfi_synth.h and nfi_heads.h declare (tests/test_abi.py checks
-# those headers against this table and the table against the built library); LPIPS_EXPORTS below
-# holds the symbols of include/nfi_lpips.h (tests/test_lpips_abi.py)
+# those headers against this table and the table against the built library); LPIPS_EXPORTS and
+# ENCODER_EXPORTS below hold the symbols of include/nfi_lpips.h (tests/test_lpips_abi.py) and
+# include/nfi_encoder.h (tests/test_encoder_abi.py)
 EXPORTS = {
     'nfi_abi_version': (ctypes.c_int, []),
     'nfi_build_info': (ctypes.c_char_p, []),
@@ -228,6 +251,16 @@ LPIPS_EXPORTS = {
                                                      ctypes.c_void_p, ctypes.c_void_p]),
 }
 
+ENCODER_EXPORTS = {
+    'nfi_encoder_workspace_bytes': (ctypes.c_size_t, [ctypes.POINTER(EncoderParams)]),
+    'nfi_encoder_forward': (ctypes.c_int, [ctypes.POINTER(EncoderParams), ctypes.c_void_p]),
+    'nfi_encoder_backward': (ctypes.c_int, [ctypes.POINTER(EncoderParams), ctypes.c_void_p,
+                                            ctypes.c_void_p, ctypes.POINTER(EncoderGrads),
+                                            ctypes.c_void_p]),
+    'nfi_encoder_saved_activation': (ctypes.c_int, [ctypes.POINTER(EncoderParams), ctypes.c_int32,
+                                                    ctypes.c_void_p, ctypes.c_void_p]),
+}
+
 _lib = None
 _lock = threading.Lock()
 
@@ -267,7 +300,8 @@ def load():
                 # memory corruption, not an error
                 raise NfiError('%s has ABI version %d, this binding needs %d: rebuild it '
                                '(nerf_from_image_b200/csrc/build.sh)' % (LIB_PATH, got, ABI_VERSION))
-            for name, (restype, argtypes) in list(EXPORTS.items()) + list(LPIPS_EXPORTS.items()):
+            for name, (restype, argtypes) in (list(EXPORTS.items()) + list(LPIPS_EXPORTS.items())
+                                       + list(ENCODER_EXPORTS.items())):
                 fn = getattr(lib, name, None)
                 if fn is None and os.environ.get('NFI_LIB_PATH'):
                     continue  # an older build under test lacks the newer entry points

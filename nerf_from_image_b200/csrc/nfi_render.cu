@@ -15,6 +15,8 @@
 #include "nfi_route.h"
 #include "nfi_heads.h"
 #include "nfi_heads_launch.h"
+#include "nfi_encoder.h"
+#include "nfi_encoder_launch.h"
 #include "nfi_lpips.h"
 #include "nfi_lpips_launch.h"
 #include "nfi_synth.h"
@@ -501,6 +503,27 @@ int nfi_lpips_backward(const nfi_lpips_params* params, const float* g_dist, floa
 int nfi_lpips_saved_preactivation(const nfi_lpips_params* params, int32_t layer, float* out, void* stream) {
   if (params == nullptr) return fail("params is NULL");
   return nfi::lpips::saved_preactivation(*params, layer, out, (cudaStream_t)stream, g_err, sizeof(g_err));
+}
+
+size_t nfi_encoder_workspace_bytes(const nfi_encoder_params* params) {
+  if (params == nullptr) return 0;
+  return nfi::encoder::workspace_bytes(*params);
+}
+
+int nfi_encoder_forward(const nfi_encoder_params* params, void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  return nfi::encoder::forward(*params, (cudaStream_t)stream, g_err, sizeof(g_err));
+}
+
+int nfi_encoder_backward(const nfi_encoder_params* params, const float* g_maps, const float* g_pooled,
+                         const nfi_encoder_grads* grads, void* stream) {
+  if (params == nullptr || grads == nullptr) return fail("params / grads is NULL");
+  return nfi::encoder::backward(*params, g_maps, g_pooled, *grads, (cudaStream_t)stream, g_err, sizeof(g_err));
+}
+
+int nfi_encoder_saved_activation(const nfi_encoder_params* params, int32_t layer, float* out, void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  return nfi::encoder::saved_activation(*params, layer, out, (cudaStream_t)stream, g_err, sizeof(g_err));
 }
 
 size_t nfi_synthesis_workspace_bytes(const nfi_synth_params* params) {

@@ -1486,17 +1486,19 @@ static int plan_wgrad(WgradArgs& a, int B, int DH, int DW) {
   return base * a.n_split;
 }
 
-// One weight-gradient GEMM (plan_wgrad'ed `a`): G [gB,gH,gW,cout] and X [B,xH,xW,cin] pairs.
+// One weight-gradient GEMM (plan_wgrad'ed `a`): G [gB,gH,gW,g_channels (default cout)] and
+// X [B,xH,xW,cin] pairs.
 static int launch_wgrad(WgradArgs& a, Pair g, int gB, int gH, int gW, Pair x, int B, int xH, int xW,
-                        cudaStream_t st, char* err, size_t err_len) {
+                        cudaStream_t st, char* err, size_t err_len, int g_channels = 0) {
   if (encode_fn() == nullptr) {
     snprintf(err, err_len, "cuTensorMapEncodeTiled is not available from this driver");
     return 1;
   }
   const int n_items = a.n_co * a.n_ci * a.taps * a.n_split;
+  if (g_channels == 0) g_channels = a.cout;
   CUtensorMap tGh, tGl, tXh, tXl;
-  if (!make_act_map(&tGh, g.hi, gB, gH, gW, a.cout, kWgTileH) ||
-      !make_act_map(&tGl, g.lo, gB, gH, gW, a.cout, kWgTileH) ||
+  if (!make_act_map(&tGh, g.hi, gB, gH, gW, g_channels, kWgTileH) ||
+      !make_act_map(&tGl, g.lo, gB, gH, gW, g_channels, kWgTileH) ||
       !make_act_map(&tXh, x.hi, B, xH, xW, a.cin, kWgTileH) ||
       !make_act_map(&tXl, x.lo, B, xH, xW, a.cin, kWgTileH)) {
     snprintf(err, err_len, "cuTensorMapEncodeTiled failed (weight gradient, Cout %d Cin %d)", a.cout,
@@ -1611,15 +1613,17 @@ static WgradArgs wgrad_args(int cout, int cin, int taps) {
 }
 // ToRGB: dimg against the layer's input at the same position
 static WgradArgs torgb_wgrad(int cout, int cin) { return wgrad_args(cout, cin, 1); }
-// conv1 (stride 1): dacc at p against x~ at p + (ky - 1, kx - 1)
-static WgradArgs conv1_wgrad(int c) {
-  WgradArgs a = wgrad_args(c, c, 9);
+// A stride-1 3x3 conv: the output gradient at p against the input at p + (ky - 1, kx - 1)
+static WgradArgs conv3x3_wgrad(int cout, int cin) {
+  WgradArgs a = wgrad_args(cout, cin, 9);
   for (int t = 0; t < 9; ++t) {
     a.x_dy[t] = t / 3 - 1;
     a.x_dx[t] = t % 3 - 1;
   }
   return a;
 }
+// conv1 (stride 1): dacc against x~
+static WgradArgs conv1_wgrad(int c) { return conv3x3_wgrad(c, c); }
 // conv0 (up): the raw gradient at (2i+ky, 2j+kx) is phase (ky%2, kx%2) at (i + ky/2, j + kx/2), the
 // phases stacked as in conv_up_adjoint_args over nimg images each, against x~ at (i, j)
 static WgradArgs conv0_wgrad(int cout, int cin, int nimg) {
@@ -2569,6 +2573,31 @@ int prep_weights3x3(const float* w, int cout, int cin, int transposed, __nv_bflo
     prep_weights_t_kernel<<<grid, 256, 0, st>>>(w, cout, cin, 9, hi, lo);
   else
     prep_weights_kernel<<<grid, 256, 0, st>>>(w, cout, cin, 9, hi, lo, nullptr);
+  NFI_SCUDA(cudaGetLastError());
+  return 0;
+}
+
+size_t wgrad3x3_partial_floats(int B, int H, int W, int cout, int cin) {
+  WgradArgs a = conv3x3_wgrad(cout, cin);
+  plan_wgrad(a, B, H, W);
+  return (size_t)a.n_split * a.taps * cout * cin;
+}
+
+int wgrad3x3(const Wgrad3x3& c, cudaStream_t st, char* err, size_t err_len) {
+  if (c.g_channels < c.cout || c.g_channels % 8 != 0 || c.cin % 8 != 0) {
+    snprintf(err, err_len, "conv weight gradient: unsupported channel counts (G %d for Cout %d, Cin %d)",
+             c.g_channels, c.cout, c.cin);
+    return 1;
+  }
+  WgradArgs a = conv3x3_wgrad(c.cout, c.cin);
+  plan_wgrad(a, c.B, c.H, c.W);
+  a.part = c.partials;
+  const Pair g = {const_cast<__nv_bfloat16*>(c.g_hi), const_cast<__nv_bfloat16*>(c.g_lo)};
+  const Pair x = {const_cast<__nv_bfloat16*>(c.x_hi), const_cast<__nv_bfloat16*>(c.x_lo)};
+  if (const int rc = launch_wgrad(a, g, c.B, c.H, c.W, x, c.B, c.H, c.W, st, err, err_len, c.g_channels))
+    return rc;
+  wgrad_reduce_kernel<<<blocks((size_t)a.cout * a.cin, 256), 256, 0, st>>>(
+      c.partials, a.n_split, a.taps, a.cout, a.cin, c.w, nullptr, nullptr, nullptr, c.B, c.g_w);
   NFI_SCUDA(cudaGetLastError());
   return 0;
 }

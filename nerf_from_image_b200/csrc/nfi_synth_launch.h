@@ -47,5 +47,25 @@ int conv3x3(const Conv3x3& c, cudaStream_t st, char* err, size_t err_len);
 // weight [Cout,Cin,3,3] -> [9][Cout][Cin] (transposed 0) or [9][Cin][Cout] (transposed 1) pair
 int prep_weights3x3(const float* w, int cout, int cin, int transposed, __nv_bfloat16* hi,
                     __nv_bfloat16* lo, cudaStream_t st, char* err, size_t err_len);
+
+// The weight gradient of such a conv on wgrad_tc_kernel (the encoder heads, nfi_encoder.cu):
+//   g_w[co,ci,ky,kx] += sum_{b,y,x} G[b,y,x,co] X[b,y+ky-1,x+kx-1,ci]
+// G [B,H,W,g_channels] (the gradient of the conv output; channels >= cout are not read into g_w, so
+// a narrow Cout can be zero-padded to the 16-byte TMA row pitch) and X [B,H,W,cin] are bf16 pairs.
+// The K split's partial sums go to `partials` (wgrad3x3_partial_floats) and are reduced in a fixed
+// order: two calls on the same inputs give the same bits.  `w` is the layer's weight (the shared
+// reduction reads it; with no demodulation term it does not change the result).
+struct Wgrad3x3 {
+  int B, H, W, cout, cin, g_channels;
+  const __nv_bfloat16* g_hi;
+  const __nv_bfloat16* g_lo;
+  const __nv_bfloat16* x_hi;
+  const __nv_bfloat16* x_lo;
+  const float* w;
+  float* partials;
+  float* g_w;
+};
+size_t wgrad3x3_partial_floats(int B, int H, int W, int cout, int cin);
+int wgrad3x3(const Wgrad3x3& c, cudaStream_t st, char* err, size_t err_len);
 }  // namespace synth
 }  // namespace nfi
