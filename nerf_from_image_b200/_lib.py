@@ -315,3 +315,41 @@ def load():
 def check(rc):
     if rc != 0:
         raise NfiError(load().nfi_last_error().decode() or 'nfi error %d' % rc)
+
+
+def ptr(t):
+    """A tensor's device address for the C ABI; None (NULL) for None."""
+    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
+
+
+def stream(dev):
+    """The current CUDA stream of ``dev`` for the C ABI."""
+    import torch
+    return ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+
+
+def take_saved(ctx, what, hint=''):
+    """The state an autograd forward kept in ``ctx.state`` for its backward, handed over once: the
+    workspace it holds is released when the backward returns.  ``what`` names the backward in the
+    refusals; ``hint`` ends the one for ``create_graph``."""
+    import torch
+    if ctx.state is None:
+        raise NfiError('the fused %s backward ran twice on one forward (retain_graph is not '
+                       'supported: the workspace is released)' % what)
+    if torch.is_grad_enabled():
+        raise NfiError('the fused %s backward is not differentiable (create_graph)%s'
+                       % (what, ': ' + hint if hint else ''))
+    state, ctx.state = ctx.state, None
+    return state
+
+
+def find_saved(out, what):
+    """The state kept by the fused forward behind ``out`` (the first node with one on the walk down
+    ``grad_fn``'s first inputs), before its backward has run."""
+    fn = out.grad_fn
+    while fn is not None and getattr(fn, 'state', None) is None:
+        fn = fn.next_functions[0][0] if fn.next_functions else None
+    if fn is None:
+        raise NfiError('no saved %s forward behind this output (or its backward has already '
+                       'released the workspace)' % what)
+    return fn.state

@@ -1,43 +1,43 @@
 #!/bin/bash
-# Builds libnfi_render.so in-tree for sm_90a (cross-compiles without a GPU).
-# Nine translation units compiled in parallel: the pipelined tensor-core kernels (nfi_pipe.cu) and
-# their view-direction-conditioned instantiations (nfi_pipe_vd.cu), both on the launchers of
-# nfi_pipe_ladder.cuh; the sampler seam and pose kernels (nfi_field.cu), the synthesis network
-# (nfi_synth.cu), the LPIPS-VGG loss and the encoder's regression heads on the synthesis network's
-# conv kernels (nfi_lpips.cu, nfi_encoder.cu), the regulariser-head point evaluator (nfi_heads.cu),
-# the view-direction-conditioned instantiations of the SIMT launchers (nfi_viewdir.cu), and everything else
-# (nfi_render.cu: C ABI and routing, re-layout, plain SIMT kernels, stand-alone decoder).  Each
-# kernel is compiled only in the unit that launches it.  nfi_render.cu and nfi_viewdir.cu take
+# Builds libnfi_render.so in-tree for sm_90a (cross-compiles without a GPU).  Every nfi_*.cu here is
+# one translation unit; they compile in parallel and the library links them all.  Each kernel is
+# compiled only in the unit that launches it.  nfi_render.cu and nfi_viewdir.cu take
 # --split-compile 0 (their many kernels are optimised in parallel).
+#
+#   build.sh [unit ...] [-nvcc-flag ...]
+# With unit names (synth for nfi_synth.cu, ...) only those units are recompiled before the link;
+# arguments that start with '-' go to every compile.  NFI_VARIANT=<name> compiles the named units
+# to nfi_<unit>_<name>.o instead and links them with the other units' regular objects into
+# libnfi_render_<name>.so (tools/build_variant.sh).  NFI_PTXAS_V=1 adds the register / spill report.
 set -e
 cd "$(dirname "$0")"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
 FLAGS="-O3 -std=c++17 --fmad=false -lineinfo -gencode arch=compute_90a,code=sm_90a \
   -Xcompiler -fPIC -Xcompiler -fvisibility=hidden -I../../include ${NFI_PTXAS_V:+-Xptxas -v}"
-$NVCC $FLAGS -c -o nfi_pipe.o nfi_pipe.cu "$@" &
-pipe_pid=$!
-$NVCC $FLAGS -c -o nfi_pipe_vd.o nfi_pipe_vd.cu "$@" &
-pipe_vd_pid=$!
-$NVCC $FLAGS -c -o nfi_field.o nfi_field.cu "$@" &
-field_pid=$!
-$NVCC $FLAGS -c -o nfi_synth.o nfi_synth.cu "$@" &
-synth_pid=$!
-$NVCC $FLAGS -c -o nfi_heads.o nfi_heads.cu "$@" &
-heads_pid=$!
-$NVCC $FLAGS -c -o nfi_lpips.o nfi_lpips.cu "$@" &
-lpips_pid=$!
-$NVCC $FLAGS -c -o nfi_encoder.o nfi_encoder.cu "$@" &
-encoder_pid=$!
-$NVCC $FLAGS --split-compile 0 -c -o nfi_viewdir.o nfi_viewdir.cu "$@" &
-viewdir_pid=$!
-$NVCC $FLAGS --split-compile 0 -c -o nfi_render.o nfi_render.cu "$@"
-wait $pipe_pid
-wait $pipe_vd_pid
-wait $field_pid
-wait $synth_pid
-wait $heads_pid
-wait $lpips_pid
-wait $encoder_pid
-wait $viewdir_pid
+all=()
+for f in nfi_*.cu; do u=${f#nfi_}; all+=("${u%.cu}"); done
+units=() flags=()
+for a in "$@"; do
+  case $a in
+    -*) flags+=("$a") ;;
+    *) [ -f "nfi_$a.cu" ] || { echo "build.sh: no unit nfi_$a.cu" >&2; exit 1; }; units+=("$a") ;;
+  esac
+done
+[ ${#units[@]} -gt 0 ] || units=("${all[@]}")
+obj() {  # the object of unit $1 that this build links
+  case " ${units[*]} " in *" $1 "*) echo "nfi_$1${NFI_VARIANT:+_$NFI_VARIANT}.o" ;; *) echo "nfi_$1.o" ;; esac
+}
+pids=()
+for u in "${units[@]}"; do
+  split=()
+  case $u in render|viewdir) split=(--split-compile 0) ;; esac
+  $NVCC $FLAGS "${split[@]}" -c -o "$(obj "$u")" "nfi_$u.cu" "${flags[@]}" &
+  pids+=($!)
+done
+failed=0
+for p in "${pids[@]}"; do wait "$p" || failed=1; done
+[ $failed = 0 ]
+objs=()
+for u in "${all[@]}"; do objs+=("$(obj "$u")"); done
 $NVCC -shared -cudart static -gencode arch=compute_90a,code=sm_90a \
-  -Xcompiler -fPIC -o libnfi_render.so nfi_render.o nfi_pipe.o nfi_pipe_vd.o nfi_field.o nfi_synth.o nfi_lpips.o nfi_encoder.o nfi_heads.o nfi_viewdir.o
+  -Xcompiler -fPIC -o "libnfi_render${NFI_VARIANT:+_$NFI_VARIANT}.so" "${objs[@]}"

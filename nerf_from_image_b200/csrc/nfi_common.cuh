@@ -11,18 +11,8 @@
 #include <stdio.h>
 #include <math.h>
 
+#include "nfi_check.h"
 #include "nfi_render.h"
-
-// A CUDA runtime call in a launcher, which reports into (err, err_len): on failure the call and
-// the CUDA error go there and the launcher returns 2.
-#define NFI_LAUNCH_CHECK(expr)                                                       \
-  do {                                                                               \
-    cudaError_t e__ = (expr);                                                        \
-    if (e__ != cudaSuccess) {                                                        \
-      snprintf(err, err_len, "%s failed: %s", #expr, cudaGetErrorString(e__));       \
-      return 2;                                                                      \
-    }                                                                                \
-  } while (0)
 
 namespace nfi {
 

@@ -19,7 +19,7 @@
 //                          adjoint g_pooled / (h w) relu'(ul) -> pair.  Each writes per-chunk
 //                          partial sums of its gradient; bias_reduce_kernel adds them to the bias
 //                          gradient in chunk order
-//   conv_tc_kernel RAW     the data gradients with the flipped tap table (conv3x3, adjoint = 1)
+//   conv_tc_kernel RAW     the data gradients with the flipped tap table (nfi::synth::conv3x3_adjoint)
 //   wgrad_tc_kernel        the weight gradients (nfi::synth::wgrad3x3): G against the saved input
 //   upsample_adjoint_kernel each source texel gathers the destination pixels whose bilinear footprint
 //                          covers it (clamped borders included), times relu' of the upsample; at
@@ -33,6 +33,7 @@
 
 #include "nfi_encoder.h"
 #include "nfi_encoder_launch.h"
+#include "nfi_pair.cuh"
 #include "nfi_synth_launch.h"
 
 namespace nfi {
@@ -44,12 +45,6 @@ constexpr int kMaps = NFI_ENCODER_MAPS;
 constexpr int kMapsN = 32;    // post[4]'s Cout on conv_tc_kernel (its narrowest N)
 constexpr int kMapsG = 64;    // g_maps' channels as a pair (one 64-channel K block, 128-byte rows)
 constexpr int kRows = 256;    // positions per partial bias sum
-
-__device__ __forceinline__ void split_bf16(float t, __nv_bfloat16& hi, __nv_bfloat16& lo) {
-  hi = __float2bfloat16_rn(t);
-  lo = __float2bfloat16_rn(t - __bfloat162float(hi));
-}
-__device__ __forceinline__ float relu(float x) { return x > 0.f ? x : 0.f; }
 
 // PyTorch's upsample_bilinear2d source index for align_corners=False with a given scale factor
 // (area_pixel_compute_source_index with scale 1 / factor): the two taps and their weights
@@ -241,37 +236,6 @@ unpack_kernel(const __nv_bfloat16* __restrict__ hi, const __nv_bfloat16* __restr
 }
 
 // ---------------------------------------------------------------- host side
-#define NFI_ECUDA(expr)                                                              \
-  do {                                                                               \
-    cudaError_t e__ = (expr);                                                        \
-    if (e__ != cudaSuccess) {                                                        \
-      snprintf(err, err_len, "%s failed: %s", #expr, cudaGetErrorString(e__));       \
-      return 2;                                                                      \
-    }                                                                                \
-  } while (0)
-
-struct Pair {
-  __nv_bfloat16* hi;
-  __nv_bfloat16* lo;
-};
-
-struct Bump {
-  unsigned char* base;
-  size_t off;
-  float* take(size_t floats) {
-    const size_t bytes = (floats * sizeof(float) + 1023) & ~(size_t)1023;
-    float* p = base ? reinterpret_cast<float*>(base + off) : nullptr;
-    off += bytes;
-    return p;
-  }
-  Pair pair(size_t elems) {
-    Pair p;
-    p.hi = reinterpret_cast<__nv_bfloat16*>(take((elems + 1) / 2));
-    p.lo = reinterpret_cast<__nv_bfloat16*>(take((elems + 1) / 2));
-    return p;
-  }
-};
-
 // The workspace: a deterministic walk, so the backward finds what a saved forward left.
 struct Layout {
   float* fcl;          // [B,h,w,C] a backbone output channel-last (also the backward's gather out)
@@ -371,56 +335,20 @@ static int check(const nfi_encoder_params& P, char* err, size_t err_len) {
   return 0;
 }
 
-static unsigned flat_grid(size_t n) {
-  size_t g = (n + 255) / 256;
-  return (unsigned)(g > 132 * 32 ? 132 * 32 : g);
-}
-
 // [B][R][Cc] -> [B][Cc][R]
 static void transpose(const float* src, int B, int R, int Cc, float* dst, bool accumulate, cudaStream_t st) {
   transpose_kernel<<<dim3((unsigned)((Cc + 31) / 32), (unsigned)((R + 31) / 32), (unsigned)B), dim3(32, 8), 0,
                      st>>>(src, R, Cc, dst, accumulate ? 1 : 0);
 }
 
-static int conv(int B, int H, int W, int C, int N, Pair in, Pair wt, const float* bias, float* u_out, Pair out,
-                cudaStream_t st, char* err, size_t err_len) {
-  synth::Conv3x3 c;
-  memset(&c, 0, sizeof(c));
-  c.B = B; c.H = H; c.W = W; c.C = C; c.N = N;
-  c.in_hi = in.hi; c.in_lo = in.lo;
-  c.w_hi = wt.hi; c.w_lo = wt.lo;
-  c.bias = bias; c.u_out = u_out;
-  c.out_hi = out.hi; c.out_lo = out.lo;
-  return synth::conv3x3(c, st, err, err_len);
-}
-static int conv_adjoint(int B, int H, int W, int C, int N, Pair in, Pair wt, float* raw, cudaStream_t st,
-                        char* err, size_t err_len) {
-  synth::Conv3x3 c;
-  memset(&c, 0, sizeof(c));
-  c.B = B; c.H = H; c.W = W; c.C = C; c.N = N;
-  c.in_hi = in.hi; c.in_lo = in.lo;
-  c.w_hi = wt.hi; c.w_lo = wt.lo;
-  c.adjoint = 1;
-  c.raw_out = raw;
-  return synth::conv3x3(c, st, err, err_len);
-}
-static int wgrad(int B, int H, int W, int cout, int cin, int gc, Pair g, Pair x, const float* w, float* part,
-                 float* g_w, cudaStream_t st, char* err, size_t err_len) {
-  if (g_w == nullptr) return 0;
-  synth::Wgrad3x3 c;
-  c.B = B; c.H = H; c.W = W; c.cout = cout; c.cin = cin; c.g_channels = gc;
-  c.g_hi = g.hi; c.g_lo = g.lo; c.x_hi = x.hi; c.x_lo = x.lo;
-  c.w = w; c.partials = part; c.g_w = g_w;
-  return synth::wgrad3x3(c, st, err, err_len);
-}
 // the pair of a gradient with relu' applied, and its sum over positions into g_b (if set)
 static int act_backward(ActBackward a, float* g_b, cudaStream_t st, char* err, size_t err_len) {
   const int n = (int)chunks((size_t)a.M);
   act_backward_kernel<<<n, 256, 0, st>>>(a);
-  NFI_ECUDA(cudaGetLastError());
+  NFI_LAUNCH_CHECK(cudaGetLastError());
   if (g_b != nullptr) {
     bias_reduce_kernel<<<(a.C + 255) / 256, 256, 0, st>>>(a.partial, n, a.C, g_b);
-    NFI_ECUDA(cudaGetLastError());
+    NFI_LAUNCH_CHECK(cudaGetLastError());
   }
   return 0;
 }
@@ -430,7 +358,7 @@ static int act_backward(ActBackward a, float* g_b, cudaStream_t st, char* err, s
 size_t workspace_bytes(const nfi_encoder_params& P) {
   char err[160];
   if (check(P, err, sizeof(err))) return 0;
-  Bump b{nullptr, 0};
+  Bump b{nullptr, 0, 0};
   Layout L;
   layout(P, b, L);
   return b.off + 1024;
@@ -457,9 +385,7 @@ static int setup(const nfi_encoder_params& P, Layout& L, char* err, size_t err_l
     snprintf(err, err_len, "encoder: workspace too small (%zu < %zu bytes)", P.workspace_bytes, need);
     return 1;
   }
-  Bump b{reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(P.workspace) + 1023) &
-                                          ~(uintptr_t)1023),
-         0};
+  Bump b = aligned_bump(P.workspace, P.workspace_bytes);
   layout(P, b, L);
   return 0;
 }
@@ -471,30 +397,31 @@ int forward(const nfi_encoder_params& P, cudaStream_t st, char* err, size_t err_
   const size_t M = (size_t)B * H * W, Ml = (size_t)B * h * w;
   const Pair none = {nullptr, nullptr};
   if (P.pose_regressor) {
-    NFI_ECUDA(cudaMemsetAsync(L.w4p, 0, (size_t)kMapsG * C * 9 * sizeof(float), st));
-    NFI_ECUDA(cudaMemsetAsync(L.b4p, 0, kMapsG * sizeof(float), st));
-    NFI_ECUDA(cudaMemcpyAsync(L.w4p, P.post4_w, (size_t)kMaps * C * 9 * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    NFI_ECUDA(cudaMemcpyAsync(L.b4p, P.post4_b, kMaps * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    NFI_LAUNCH_CHECK(cudaMemsetAsync(L.w4p, 0, (size_t)kMapsG * C * 9 * sizeof(float), st));
+    NFI_LAUNCH_CHECK(cudaMemsetAsync(L.b4p, 0, kMapsG * sizeof(float), st));
+    NFI_LAUNCH_CHECK(
+        cudaMemcpyAsync(L.w4p, P.post4_w, (size_t)kMaps * C * 9 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    NFI_LAUNCH_CHECK(cudaMemcpyAsync(L.b4p, P.post4_b, kMaps * sizeof(float), cudaMemcpyDeviceToDevice, st));
     if (int rc = synth::prep_weights3x3(P.post0_w, C, C, 0, L.w0.hi, L.w0.lo, st, err, err_len)) return rc;
     if (int rc = synth::prep_weights3x3(P.post2_w, C, C, 0, L.w2.hi, L.w2.lo, st, err, err_len)) return rc;
     if (int rc = synth::prep_weights3x3(L.w4p, kMapsN, C, 0, L.w4.hi, L.w4.lo, st, err, err_len)) return rc;
     transpose(P.features, B, C, h * w, L.fcl, false, st);
     upsample_relu_kernel<<<flat_grid(M * C / 4), 256, 0, st>>>(L.fcl, B, h, w, C, kScale, L.x0.hi, L.x0.lo);
-    NFI_ECUDA(cudaGetLastError());
-    if (int rc = conv(B, H, W, C, C, L.x0, L.w0, P.post0_b, nullptr, L.a1, st, err, err_len)) return rc;
-    if (int rc = conv(B, H, W, C, C, L.a1, L.w2, P.post2_b, nullptr, L.a2, st, err, err_len)) return rc;
-    if (int rc = conv(B, H, W, C, kMapsN, L.a2, L.w4, L.b4p, L.u4, none, st, err, err_len)) return rc;
+    NFI_LAUNCH_CHECK(cudaGetLastError());
+    if (int rc = synth::conv3x3(B, H, W, C, C, L.x0, L.w0, P.post0_b, nullptr, L.a1, st, err, err_len)) return rc;
+    if (int rc = synth::conv3x3(B, H, W, C, C, L.a1, L.w2, P.post2_b, nullptr, L.a2, st, err, err_len)) return rc;
+    if (int rc = synth::conv3x3(B, H, W, C, kMapsN, L.a2, L.w4, L.b4p, L.u4, none, st, err, err_len)) return rc;
     maps_kernel<<<flat_grid(M), 256, 0, st>>>(L.u4, M, P.maps);
-    NFI_ECUDA(cudaGetLastError());
+    NFI_LAUNCH_CHECK(cudaGetLastError());
   }
   if (P.latent_regressor) {
     if (int rc = synth::prep_weights3x3(P.wpre_w, C, C, 0, L.wl.hi, L.wl.lo, st, err, err_len)) return rc;
     transpose(P.features_latent, B, C, h * w, L.fcl, false, st);
     upsample_relu_kernel<<<flat_grid(Ml * C / 4), 256, 0, st>>>(L.fcl, B, h, w, C, 1, L.xl.hi, L.xl.lo);
-    NFI_ECUDA(cudaGetLastError());
-    if (int rc = conv(B, h, w, C, C, L.xl, L.wl, P.wpre_b, L.ul, none, st, err, err_len)) return rc;
+    NFI_LAUNCH_CHECK(cudaGetLastError());
+    if (int rc = synth::conv3x3(B, h, w, C, C, L.xl, L.wl, P.wpre_b, L.ul, none, st, err, err_len)) return rc;
     mean_pool_kernel<<<dim3((unsigned)(C / 64), (unsigned)B), 256, 0, st>>>(L.ul, h * w, C, P.pooled);
-    NFI_ECUDA(cudaGetLastError());
+    NFI_LAUNCH_CHECK(cudaGetLastError());
   }
   return 0;
 }
@@ -523,31 +450,34 @@ int backward(const nfi_encoder_params& P, const float* g_maps, const float* g_po
     // post[4]: g_maps as the zero-padded pair
     a.C = kMaps; a.out_C = kMapsG; a.g = g_maps; a.hi = L.g4.hi; a.lo = L.g4.lo;
     if (int rc = act_backward(a, G.g_post4_b, st, err, err_len)) return rc;
-    if (int rc = wgrad(B, H, W, kMaps, C, kMapsG, L.g4, L.a2, P.post4_w, L.part, G.g_post4_w, st, err, err_len))
+    if (int rc = synth::wgrad3x3(B, H, W, kMaps, C, kMapsG, L.g4, L.a2, P.post4_w, L.part, G.g_post4_w, st, err,
+                                 err_len))
       return rc;
     const bool below2 = G.g_post2_w || G.g_post2_b || G.g_post0_w || G.g_post0_b || G.g_features;
     const bool below0 = G.g_post0_w || G.g_post0_b || G.g_features;
     if (below2) {
-      if (int rc = conv_adjoint(B, H, W, kMapsG, C, L.g4, L.t4, L.d, st, err, err_len)) return rc;
+      if (int rc = synth::conv3x3_adjoint(B, H, W, kMapsG, C, L.g4, L.t4, L.d, st, err, err_len)) return rc;
       // post[2]
       a.C = C; a.out_C = C; a.g = L.d; a.mask_hi = L.a2.hi; a.hi = L.g.hi; a.lo = L.g.lo;
       if (int rc = act_backward(a, G.g_post2_b, st, err, err_len)) return rc;
-      if (int rc = wgrad(B, H, W, C, C, C, L.g, L.a1, P.post2_w, L.part, G.g_post2_w, st, err, err_len)) return rc;
+      if (int rc = synth::wgrad3x3(B, H, W, C, C, C, L.g, L.a1, P.post2_w, L.part, G.g_post2_w, st, err, err_len))
+        return rc;
     }
     if (below0) {
-      if (int rc = conv_adjoint(B, H, W, C, C, L.g, L.t2, L.d, st, err, err_len)) return rc;
+      if (int rc = synth::conv3x3_adjoint(B, H, W, C, C, L.g, L.t2, L.d, st, err, err_len)) return rc;
       // post[0]
       a.mask_hi = L.a1.hi;
       if (int rc = act_backward(a, G.g_post0_b, st, err, err_len)) return rc;
-      if (int rc = wgrad(B, H, W, C, C, C, L.g, L.x0, P.post0_w, L.part, G.g_post0_w, st, err, err_len)) return rc;
+      if (int rc = synth::wgrad3x3(B, H, W, C, C, C, L.g, L.x0, P.post0_w, L.part, G.g_post0_w, st, err, err_len))
+        return rc;
     }
     if (G.g_features) {
-      if (int rc = conv_adjoint(B, H, W, C, C, L.g, L.t0, L.d, st, err, err_len)) return rc;
+      if (int rc = synth::conv3x3_adjoint(B, H, W, C, C, L.g, L.t0, L.d, st, err, err_len)) return rc;
       upsample_adjoint_kernel<<<flat_grid((size_t)Ml * C / 4), 256, 0, st>>>(L.d, L.x0.hi, B, h, w, C, kScale,
                                                                              L.fcl);
-      NFI_ECUDA(cudaGetLastError());
+      NFI_LAUNCH_CHECK(cudaGetLastError());
       transpose(L.fcl, B, h * w, C, G.g_features, true, st);
-      NFI_ECUDA(cudaGetLastError());
+      NFI_LAUNCH_CHECK(cudaGetLastError());
     }
   }
   if (P.latent_regressor) {
@@ -558,13 +488,14 @@ int backward(const nfi_encoder_params& P, const float* g_maps, const float* g_po
     a.g_img = g_pooled; a.per_img = h * w; a.g_scale = 1.f / (float)(h * w);
     a.mask_u = L.ul; a.hi = L.g.hi; a.lo = L.g.lo;
     if (int rc = act_backward(a, G.g_wpre_b, st, err, err_len)) return rc;
-    if (int rc = wgrad(B, h, w, C, C, C, L.g, L.xl, P.wpre_w, L.part, G.g_wpre_w, st, err, err_len)) return rc;
+    if (int rc = synth::wgrad3x3(B, h, w, C, C, C, L.g, L.xl, P.wpre_w, L.part, G.g_wpre_w, st, err, err_len))
+      return rc;
     if (G.g_features_latent) {
-      if (int rc = conv_adjoint(B, h, w, C, C, L.g, L.tl, L.d, st, err, err_len)) return rc;
+      if (int rc = synth::conv3x3_adjoint(B, h, w, C, C, L.g, L.tl, L.d, st, err, err_len)) return rc;
       upsample_adjoint_kernel<<<flat_grid((size_t)Ml * C / 4), 256, 0, st>>>(L.d, L.xl.hi, B, h, w, C, 1, L.fcl);
-      NFI_ECUDA(cudaGetLastError());
+      NFI_LAUNCH_CHECK(cudaGetLastError());
       transpose(L.fcl, B, h * w, C, G.g_features_latent, true, st);
-      NFI_ECUDA(cudaGetLastError());
+      NFI_LAUNCH_CHECK(cudaGetLastError());
     }
   }
   return 0;
@@ -587,7 +518,7 @@ int saved_activation(const nfi_encoder_params& P, int layer, float* out, cudaStr
     unpack_kernel<<<flat_grid(count), 256, 0, st>>>(nullptr, nullptr, L.ul, count, out);
   else
     unpack_kernel<<<flat_grid(count), 256, 0, st>>>(src[layer].hi, src[layer].lo, nullptr, count, out);
-  NFI_ECUDA(cudaGetLastError());
+  NFI_LAUNCH_CHECK(cudaGetLastError());
   return 0;
 }
 

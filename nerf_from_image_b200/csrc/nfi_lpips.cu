@@ -32,6 +32,7 @@
 
 #include "nfi_lpips.h"
 #include "nfi_lpips_launch.h"
+#include "nfi_pair.cuh"
 #include "nfi_synth_launch.h"
 
 namespace nfi {
@@ -48,11 +49,6 @@ constexpr float kEps = 1e-10f;    // normalize_tensor
 
 inline bool pooled_after(int l) { return kTapOf[l] >= 0 && l < kConvs - 1; }
 
-__device__ __forceinline__ void split_bf16(float t, __nv_bfloat16& hi, __nv_bfloat16& lo) {
-  hi = __float2bfloat16_rn(t);
-  lo = __float2bfloat16_rn(t - __bfloat162float(hi));
-}
-__device__ __forceinline__ float relu(float x) { return x > 0.f ? x : 0.f; }
 __device__ __forceinline__ float warp_sum(float v) {  // butterfly: every lane holds the same bits
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -338,7 +334,6 @@ conv11_backward_kernel(const float* __restrict__ g, const float* __restrict__ u,
           for (int ci = 0; ci < 3; ++ci) acc[ci] = fmaf(gu[j], wt[(4 * c4 + j) * 3 + ci], acc[ci]);
       }
     }
-#pragma unroll
     float* dst = img < (size_t)N ? grad_in0 + img * 3 * HW : grad_in1 + (img - N) * 3 * HW;
 #pragma unroll
     for (int ci = 0; ci < 3; ++ci) dst[ci * HW + (size_t)y * W + x] += acc[ci] / scale[ci];
@@ -346,37 +341,6 @@ conv11_backward_kernel(const float* __restrict__ g, const float* __restrict__ u,
 }
 
 // ---------------------------------------------------------------- host side
-#define NFI_LCUDA(expr)                                                              \
-  do {                                                                               \
-    cudaError_t e__ = (expr);                                                        \
-    if (e__ != cudaSuccess) {                                                        \
-      snprintf(err, err_len, "%s failed: %s", #expr, cudaGetErrorString(e__));       \
-      return 2;                                                                      \
-    }                                                                                \
-  } while (0)
-
-struct Pair {
-  __nv_bfloat16* hi;
-  __nv_bfloat16* lo;
-};
-
-struct Bump {
-  unsigned char* base;
-  size_t off;
-  float* take(size_t floats) {
-    const size_t bytes = (floats * sizeof(float) + 1023) & ~(size_t)1023;
-    float* p = base ? reinterpret_cast<float*>(base + off) : nullptr;
-    off += bytes;
-    return p;
-  }
-  Pair pair(size_t elems) {
-    Pair p;
-    p.hi = reinterpret_cast<__nv_bfloat16*>(take((elems + 1) / 2));
-    p.lo = reinterpret_cast<__nv_bfloat16*>(take((elems + 1) / 2));
-    return p;
-  }
-};
-
 // The workspace: a deterministic walk, so the backward finds what a saved forward left.
 struct Layout {
   Pair wf[kConvs];   // forward weights [9][Cout][Cin] (layers 1..12)
@@ -437,11 +401,6 @@ static int check(const nfi_lpips_params& P, char* err, size_t err_len) {
   return 0;
 }
 
-static unsigned flat_grid(size_t n) {
-  size_t g = (n + 255) / 256;
-  return (unsigned)(g > 132 * 32 ? 132 * 32 : g);
-}
-
 template <int KC>
 static void head_forward(const float* u, int N, int hw, const float* lin, float* partial, int n_chunks,
                          cudaStream_t st) {
@@ -459,7 +418,7 @@ static void tap_backward(const TapBackward& a, cudaStream_t st) {
 size_t workspace_bytes(const nfi_lpips_params& P) {
   char err[128];
   if (check(P, err, sizeof(err))) return 0;
-  Bump b{nullptr, 0};
+  Bump b{nullptr, 0, 0};
   Layout L;
   layout(P, b, L);
   return b.off + 1024;
@@ -486,9 +445,7 @@ static int setup(const nfi_lpips_params& P, Layout& L, char* err, size_t err_len
     snprintf(err, err_len, "lpips: workspace too small (%zu < %zu bytes)", P.workspace_bytes, need);
     return 1;
   }
-  Bump b{reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(P.workspace) + 1023) &
-                                          ~(uintptr_t)1023),
-         0};
+  Bump b = aligned_bump(P.workspace, P.workspace_bytes);
   layout(P, b, L);
   return 0;
 }
@@ -503,19 +460,15 @@ int forward(const nfi_lpips_params& P, cudaStream_t st, char* err, size_t err_le
       return rc;
   conv11_forward_kernel<<<flat_grid((size_t)B2 * H * W * 8), 256, 0, st>>>(
       P.in0, P.in1, N, H, W, P.conv_w[0], P.conv_b[0], P.shift, P.scale, L.u[0], L.act[0].hi, L.act[0].lo);
-  NFI_LCUDA(cudaGetLastError());
+  NFI_LAUNCH_CHECK(cudaGetLastError());
   int cur = 0;
   for (int l = 1; l < kConvs; ++l) {
     const int h = H >> kLevel[l], w = W >> kLevel[l], t = kTapOf[l];
     const bool writes_pair = t < 0;  // a tap's relu(u) is read from u (head, pool)
-    synth::Conv3x3 c;
-    memset(&c, 0, sizeof(c));
-    c.B = B2; c.H = h; c.W = w; c.C = kCin[l]; c.N = kCout[l];
-    c.in_hi = L.act[cur].hi; c.in_lo = L.act[cur].lo;
-    c.w_hi = L.wf[l].hi; c.w_lo = L.wf[l].lo;
-    c.bias = P.conv_b[l]; c.u_out = L.u[l];
-    if (writes_pair) { c.out_hi = L.act[cur ^ 1].hi; c.out_lo = L.act[cur ^ 1].lo; }
-    if (const int rc = synth::conv3x3(c, st, err, err_len)) return rc;
+    const Pair out = writes_pair ? L.act[cur ^ 1] : Pair{nullptr, nullptr};
+    if (const int rc = synth::conv3x3(B2, h, w, kCin[l], kCout[l], L.act[cur], L.wf[l], P.conv_b[l], L.u[l], out,
+                                      st, err, err_len))
+      return rc;
     if (t >= 0) {
       float* part = L.partial + L.taps.off[t];
       const int hw = h * w, nc = L.taps.n_chunks[t];
@@ -525,17 +478,17 @@ int forward(const nfi_lpips_params& P, cudaStream_t st, char* err, size_t err_le
         case 256: head_forward<8>(L.u[l], N, hw, P.lin_w[t], part, nc, st); break;
         default: head_forward<16>(L.u[l], N, hw, P.lin_w[t], part, nc, st); break;
       }
-      NFI_LCUDA(cudaGetLastError());
+      NFI_LAUNCH_CHECK(cudaGetLastError());
       if (pooled_after(l)) {
         pool_kernel<<<flat_grid((size_t)B2 * (h / 2) * (w / 2) * (kCout[l] / 4)), 256, 0, st>>>(
             L.u[l], B2, h, w, kCout[l], L.act[cur ^ 1].hi, L.act[cur ^ 1].lo);
-        NFI_LCUDA(cudaGetLastError());
+        NFI_LAUNCH_CHECK(cudaGetLastError());
       }
     }
     cur ^= 1;
   }
   head_sum_kernel<<<(N + 255) / 256, 256, 0, st>>>(L.partial, L.taps, N, P.out);
-  NFI_LCUDA(cudaGetLastError());
+  NFI_LAUNCH_CHECK(cudaGetLastError());
   return 0;
 }
 
@@ -573,21 +526,16 @@ int backward(const nfi_lpips_params& P, const float* g_dist, float* grad_in0, fl
       case 256: tap_backward<8>(a, st); break;
       default: tap_backward<16>(a, st); break;
     }
-    NFI_LCUDA(cudaGetLastError());
-    synth::Conv3x3 c;
-    memset(&c, 0, sizeof(c));
-    c.B = B; c.H = h; c.W = w; c.C = kCout[l]; c.N = kCin[l];
-    c.in_hi = L.dacc.hi; c.in_lo = L.dacc.lo;
-    c.w_hi = L.wt[l].hi; c.w_lo = L.wt[l].lo;
-    c.adjoint = 1;
-    c.raw_out = L.g[cur];
-    if (const int rc = synth::conv3x3(c, st, err, err_len)) return rc;
+    NFI_LAUNCH_CHECK(cudaGetLastError());
+    if (const int rc = synth::conv3x3_adjoint(B, h, w, kCout[l], kCin[l], L.dacc, L.wt[l], L.g[cur], st, err,
+                                              err_len))
+      return rc;
     gin = L.g[cur];
     cur ^= 1;
   }
   conv11_backward_kernel<<<flat_grid((size_t)B * H * W), 256, 0, st>>>(gin, L.u[0], N, B, H, W, P.conv_w[0],
                                                                       P.scale, grad_in0, grad_in1);
-  NFI_LCUDA(cudaGetLastError());
+  NFI_LAUNCH_CHECK(cudaGetLastError());
   return 0;
 }
 
@@ -600,7 +548,7 @@ int saved_preactivation(const nfi_lpips_params& P, int layer, float* out, cudaSt
   Layout L;
   if (const int rc = setup(P, L, err, err_len)) return rc;
   const size_t n = (size_t)2 * P.n * ((size_t)P.height * P.width >> (2 * kLevel[layer])) * kCout[layer];
-  NFI_LCUDA(cudaMemcpyAsync(out, L.u[layer], n * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  NFI_LAUNCH_CHECK(cudaMemcpyAsync(out, L.u[layer], n * sizeof(float), cudaMemcpyDeviceToDevice, st));
   return 0;
 }
 

@@ -38,6 +38,7 @@
 #include <stdio.h>
 #include <string.h>
 
+#include "nfi_pair.cuh"
 #include "nfi_synth.h"
 #include "nfi_synth_launch.h"
 #include "nfi_tc.cuh"
@@ -149,11 +150,6 @@ __device__ __forceinline__ TileCoord decode_tile(const ConvArgs& a, int tile) {
   return t;
 }
 
-// t = hi + lo with hi = bf16(t), lo = bf16(t - hi)
-__device__ __forceinline__ void split_bf16(float t, __nv_bfloat16& hi, __nv_bfloat16& lo) {
-  hi = __float2bfloat16_rn(t);
-  lo = __float2bfloat16_rn(t - __bfloat162float(hi));
-}
 // value -> (value * style) as a bf16 hi / lo pair, 4 channels (8 bytes per tensor) at a time
 __device__ __forceinline__ void store_split4(__nv_bfloat16* hi, __nv_bfloat16* lo, size_t idx,
                                              float4 v, float4 s) {
@@ -1395,37 +1391,6 @@ static int pick_bn(int N) {
   return 0;
 }
 
-struct Pair {
-  __nv_bfloat16* hi;
-  __nv_bfloat16* lo;
-};
-
-#define NFI_SCUDA(expr)                                                              \
-  do {                                                                               \
-    cudaError_t e__ = (expr);                                                        \
-    if (e__ != cudaSuccess) {                                                        \
-      snprintf(err, err_len, "%s failed: %s", #expr, cudaGetErrorString(e__));       \
-      return 2;                                                                      \
-    }                                                                                \
-  } while (0)
-
-static int sm_count() {
-  static int n = []() {
-    int dev = 0, v = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    return v;
-  }();
-  return n;
-}
-
-static unsigned blocks(size_t n, int per) { return (unsigned)((n + per - 1) / per); }
-// The grid of a grid-stride kernel over n items: one thread each, at most 16 blocks of 256 per SM
-static unsigned flat_grid(size_t n) {
-  const unsigned g = blocks(n, 256), cap = (unsigned)sm_count() * 16u;
-  return g > cap ? cap : g;
-}
-
 // One convolution launch.  `in` [map_B (default B),H,W,C] pair, weights [taps9][N][C] pair.
 static int launch_conv(ConvArgs& a, Pair in, Pair wt, int w_taps, cudaStream_t st, char* err,
                        size_t err_len, int map_B = 0) {
@@ -1459,10 +1424,10 @@ static int launch_conv(ConvArgs& a, Pair in, Pair wt, int w_taps, cudaStream_t s
   }
   const int smem = kStages * (2 * kATile + 2 * a.BN * 128) + 128 +
                    ((a.mode == kModeRgb && a.skip != nullptr) ? kSkipBytes : 0);
-  NFI_SCUDA(cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  NFI_LAUNCH_CHECK(cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   const int grid = n_tiles < sm_count() ? n_tiles : sm_count();
   conv_tc_kernel<<<grid, kConvThreads, smem, st>>>(tAh, tAl, tWh, tWl, a, n_tiles);
-  NFI_SCUDA(cudaGetLastError());
+  NFI_LAUNCH_CHECK(cudaGetLastError());
   return 0;
 }
 
@@ -1506,10 +1471,10 @@ static int launch_wgrad(WgradArgs& a, Pair g, int gB, int gH, int gW, Pair x, in
     return 1;
   }
   const int smem = kWgStages * kWgStage + 128;
-  NFI_SCUDA(cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  NFI_LAUNCH_CHECK(cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   const int grid = n_items < 2 * sm_count() ? n_items : 2 * sm_count();
   wgrad_tc_kernel<<<grid, kWgThreads, smem, st>>>(tGh, tGl, tXh, tXl, a, n_items);
-  NFI_SCUDA(cudaGetLastError());
+  NFI_LAUNCH_CHECK(cudaGetLastError());
   return 0;
 }
 
@@ -1636,30 +1601,6 @@ static WgradArgs conv0_wgrad(int cout, int cin, int nimg) {
       a.a_img[t] = ((ky & 1) * 2 + (kx & 1)) * nimg;
     }
   return a;
-}
-
-struct Bump {
-  unsigned char* base;
-  size_t off, cap;
-  float* take(size_t floats) {
-    const size_t bytes = (floats * sizeof(float) + 1023) & ~(size_t)1023;
-    float* p = base ? reinterpret_cast<float*>(base + off) : nullptr;
-    off += bytes;
-    return p;
-  }
-  Pair pair(size_t elems) {  // two bf16 tensors of `elems` elements
-    Pair p;
-    p.hi = reinterpret_cast<__nv_bfloat16*>(take((elems + 1) / 2));
-    p.lo = reinterpret_cast<__nv_bfloat16*>(take((elems + 1) / 2));
-    return p;
-  }
-};
-
-// A Bump over a caller's buffer from its first 1024-byte boundary (the sizers add the 1024 bytes)
-static Bump aligned_bump(void* p, size_t bytes) {
-  unsigned char* base =
-      reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(p) + 1023) & ~(uintptr_t)1023);
-  return Bump{base, 0, bytes};
 }
 
 static int check_params(const nfi_synth_params& P, char* err, size_t err_len) {
@@ -1799,7 +1740,7 @@ static int run(const nfi_synth_params& P, Bump& ws, cudaStream_t st, bool dry, c
         e.u_out = sv ? sv->u0[i] : nullptr;
         const size_t total = (size_t)B * (res / 2) * (res / 2) * (cout / 4);
         fir_act_kernel<<<flat_grid(total), 256, 0, st>>>(raw, B, res, res, cout, e);
-        NFI_SCUDA(cudaGetLastError());
+        NFI_LAUNCH_CHECK(cudaGetLastError());
       }
       x = y;
     }
@@ -1956,7 +1897,7 @@ static int prep_backward(const nfi_synth_params& P, const float* g_planes, const
   }
   planes_grad_kernel<<<flat_grid((size_t)B * R * R * NI), 256, 0, st>>>(g_planes, B, R, s.dimg[0],
                                                                         s.dimg_p.hi, s.dimg_p.lo);
-  NFI_SCUDA(cudaGetLastError());
+  NFI_LAUNCH_CHECK(cudaGetLastError());
   return 0;
 }
 
@@ -1978,7 +1919,7 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
   const auto &ds0 = s.ds0[0], &ds1 = s.ds1[0], &dsr = s.dsr[0], &dd0 = s.dd0[0], &dd1 = s.dd1[0];
   const Pair dimg_p = s.dimg_p, xt = s.xt;
 
-  NFI_SCUDA(cudaMemsetAsync(s.sums, 0, s.n_sums * sizeof(float), st));
+  NFI_LAUNCH_CHECK(cudaMemsetAsync(s.sums, 0, s.n_sums * sizeof(float), st));
   if (const int rc = prep_backward(P, G.g_planes, s, st, err, err_len)) return rc;
 
   auto act_backward = [&](ActBackward& e, int HW, int C) -> int {
@@ -1992,7 +1933,7 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
       act_backward_kernel<true><<<grid, 256, 0, st>>>(e, HW, C, chunk);
     else
       act_backward_kernel<false><<<grid, 256, 0, st>>>(e, HW, C, chunk);
-    NFI_SCUDA(cudaGetLastError());
+    NFI_LAUNCH_CHECK(cudaGetLastError());
     return 0;
   };
   auto to_ws = [&](const float* ds, const nfi_synth_layer& L, int cin, int row, float gain) {
@@ -2017,7 +1958,7 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
     if (const int rc = launch_wgrad(a, g, gB, gH, gH, xt, B, D_, D_, st, err, err_len)) return rc;
     wgrad_reduce_kernel<<<blocks((size_t)a.cout * a.cin, 256), 256, 0, st>>>(
         part, a.n_split, a.taps, a.cout, a.cin, w, dd, d, s, B, g_w);
-    NFI_SCUDA(cudaGetLastError());
+    NFI_LAUNCH_CHECK(cudaGetLastError());
     return 0;
   };
 
@@ -2049,7 +1990,7 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
       const int h = res / 2;
       upsample_adjoint_kernel<<<flat_grid((size_t)B * h * h * NI), 256, 0, st>>>(
           dimg[cur], B, h, h, NI, dimg[cur ^ 1], dimg_p.hi, dimg_p.lo);
-      NFI_SCUDA(cudaGetLastError());
+      NFI_LAUNCH_CHECK(cudaGetLastError());
       cur ^= 1;
     }
     // conv1: consumers ToRGB (style_rgb) and, below the last block, conv0 of block i+1 (bufC)
@@ -2103,7 +2044,7 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
           sv.wsq1[0], sv.style1[0], dd1[0], sv.dco1[0], c, c, B, ds1[0]);
       to_ws(ds1[0], P.conv1[0], c, sv.row1[0], 1.f);
       if (PG) affine(ds1[0], PG->conv1[0], c, sv.row1[0], 1.f);
-      NFI_SCUDA(cudaGetLastError());
+      NFI_LAUNCH_CHECK(cudaGetLastError());
       break;
     }
     // conv0 (up): its one consumer is conv1 -> dacc fp32 in bufB, ds1 and dd0
@@ -2133,7 +2074,7 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
                  reinterpret_cast<__nv_bfloat16*>(bufA) + (size_t)4 * B * (h + 1) * (h + 1) * c};
       fir_adjoint_kernel<<<flat_grid((size_t)4 * B * (h + 1) * (h + 1) * (c / 4)), 256, 0, st>>>(
           bufB, B, res, res, c, ph.hi, ph.lo);
-      NFI_SCUDA(cudaGetLastError());
+      NFI_LAUNCH_CHECK(cudaGetLastError());
       if (PG && PG->conv0[i].g_weight != nullptr) {
         // raw gradient at (2i+ky, 2j+kx) = phase (ky%2, kx%2) at (i + ky/2, j + kx/2), against
         // x~ = lrelu(u1 of block i-1) s0 on the low-resolution grid
@@ -2149,7 +2090,7 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
       if (rc) return rc;
     }
   }
-  NFI_SCUDA(cudaGetLastError());
+  NFI_LAUNCH_CHECK(cudaGetLastError());
   return 0;
 }
 
@@ -2244,7 +2185,7 @@ int saved_preactivation(const nfi_synth_params& P, int block, int which, float* 
   }
   const int res = 4 << block;
   const size_t n = (size_t)P.batch * res * res * P.channels[block];
-  NFI_SCUDA(cudaMemcpyAsync(out, which ? sv.u1[block] : sv.u0[block], n * sizeof(float),
+  NFI_LAUNCH_CHECK(cudaMemcpyAsync(out, which ? sv.u1[block] : sv.u0[block], n * sizeof(float),
                             cudaMemcpyDeviceToDevice, st));
   return 0;
 }
@@ -2294,7 +2235,7 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
   const auto &ds0 = s.ds0, &ds1 = s.ds1, &dsr = s.dsr, &dd0 = s.dd0, &dd1 = s.dd1;  // [0]: q, [1]: q-dot
   const Pair dimg_p = s.dimg_p, xt = s.xt;
 
-  NFI_SCUDA(cudaMemsetAsync(s.sums, 0, s.n_sums * sizeof(float), st));
+  NFI_LAUNCH_CHECK(cudaMemsetAsync(s.sums, 0, s.n_sums * sizeof(float), st));
   // ---- tangent forward ----
   auto style_dot = [&](const nfi_synth_layer& L, int c, int row, float gain, float* out) {
     styles_kernel<<<blocks((size_t)B * c * 32, 256), 256, 0, st>>>(H.t_ws + (size_t)row * D, P.num_ws * D, D,
@@ -2331,7 +2272,7 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
       const size_t total = (size_t)B * h * h * (c / 4);
       fir_act_kernel<<<flat_grid(total), 256, 0, st>>>(bufA, B, res, res, c,
                                                        tangent_epi(P.conv0[i], sv.dco0[i], ddot0[i], sv.u0[i], ud0[i]));
-      NFI_SCUDA(cudaGetLastError());
+      NFI_LAUNCH_CHECK(cudaGetLastError());
       restyle_dot(sv.u0[i], ud0[i], sv.style1[i], sd1[i], HW, c, xt);
     } else {  // b4.const does not depend on ws: x~-dot = const s-dot
       const_input_kernel<<<blocks((size_t)B * 16 * c, 256), 256, 0, st>>>(P.const_input, sd1[0], B, c, xt.hi,
@@ -2342,7 +2283,7 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
     if (const int rc = launch_conv(a, xt, sv.w1[i], 9, st, err, err_len)) return rc;
     tangent_act_kernel<<<flat_grid((size_t)B * HW * c / 4), 256, 0, st>>>(
         bufA, B, HW, c, tangent_epi(P.conv1[i], sv.dco1[i], ddot1[i], sv.u1[i], ud1[i]));
-    NFI_SCUDA(cudaGetLastError());
+    NFI_LAUNCH_CHECK(cudaGetLastError());
   }
 
   // ---- the backward and its tangent, last block first ----
@@ -2355,7 +2296,7 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
     }
     dim3 grid((unsigned)((HW + kActChunk - 1) / kActChunk), (unsigned)B);
     act_backward_tangent_kernel<<<grid, 256, 0, st>>>(e, HW, C, kActChunk);
-    NFI_SCUDA(cudaGetLastError());
+    NFI_LAUNCH_CHECK(cudaGetLastError());
     return 0;
   };
   // the ws gradient is the tangent's (the style gradient's tangent through styles_kernel's
@@ -2390,7 +2331,7 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
     else
       wgrad_reduce_tangent_kernel<<<blocks((size_t)a.cout * a.cin, 256), 256, 0, st>>>(
           part, a.n_split, a.taps, a.cout, a.cin, w, dd[0], dd[1], d, ddot, s, sdot, B, g_w);
-    NFI_SCUDA(cudaGetLastError());
+    NFI_LAUNCH_CHECK(cudaGetLastError());
     return 0;
   };
 
@@ -2415,7 +2356,7 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
       const int h = res / 2;
       upsample_adjoint_kernel<<<flat_grid((size_t)B * h * h * NI), 256, 0, st>>>(
           dimg[cur], B, h, h, NI, dimg[cur ^ 1], dimg_p.hi, dimg_p.lo);
-      NFI_SCUDA(cudaGetLastError());
+      NFI_LAUNCH_CHECK(cudaGetLastError());
       cur ^= 1;
     }
     // conv1: consumers ToRGB and conv0 of block i+1 ([dx~; dx~-dot] in bufC) -> [dacc; dacc-dot]
@@ -2478,7 +2419,7 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
       float* dd[2] = {dd1[0][0], dd1[1][0]};
       demod(sv.wsq1[0], sv.style1[0], sd1[0], dd, sv.dco1[0], ddot1[0], c, c, ds1[0][0], ds1[1][0]);
       outputs(ds1[0][0], ds1[1][0], P.conv1[0], c, sv.row1[0], 1.f, PG ? &PG->conv1[0] : nullptr);
-      NFI_SCUDA(cudaGetLastError());
+      NFI_LAUNCH_CHECK(cudaGetLastError());
       break;
     }
     {  // conv0 (up): one consumer, conv1 -> [dacc; dacc-dot] fp32 in bufB
@@ -2504,7 +2445,7 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
       const size_t nph = (size_t)4 * B2 * (h + 1) * (h + 1) * c;
       Pair ph = {reinterpret_cast<__nv_bfloat16*>(bufA), reinterpret_cast<__nv_bfloat16*>(bufA) + nph};
       fir_adjoint_kernel<<<flat_grid(nph / 4), 256, 0, st>>>(bufB, B2, res, res, c, ph.hi, ph.lo);
-      NFI_SCUDA(cudaGetLastError());
+      NFI_LAUNCH_CHECK(cudaGetLastError());
       if (PG && PG->conv0[i].g_weight != nullptr) {
         const size_t nl = (size_t)B * h * h * ci;
         restyle_dot(sv.u1[i - 1], ud1[i - 1], sv.style0[i], sd0[i], h * h, ci, xt);
@@ -2521,7 +2462,7 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
       if (const int rc = launch_conv(a, ph, wt0[i], 9, st, err, err_len, 4 * B2)) return rc;
     }
   }
-  NFI_SCUDA(cudaGetLastError());
+  NFI_LAUNCH_CHECK(cudaGetLastError());
   return 0;
 }
 
@@ -2552,18 +2493,20 @@ int backward_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const nfi_sy
 }
 
 // ---- the narrow entries of nfi_synth_launch.h ----
-int conv3x3(const Conv3x3& c, cudaStream_t st, char* err, size_t err_len) {
-  ConvArgs a = conv3x3_args(c.B, c.C, c.N, c.H, c.W, c.adjoint ? kModeRaw : kModeAct, c.adjoint != 0);
-  if (c.adjoint) {
-    a.out_raw = c.raw_out;
-  } else {
-    a.act.bias = c.bias; a.act.gain = 1.f; a.act.slope = 0.f;
-    a.act.a_hi = c.out_hi; a.act.a_lo = c.out_lo;
-    a.act.u_out = c.u_out;
-  }
-  const Pair in = {const_cast<__nv_bfloat16*>(c.in_hi), const_cast<__nv_bfloat16*>(c.in_lo)};
-  const Pair wt = {const_cast<__nv_bfloat16*>(c.w_hi), const_cast<__nv_bfloat16*>(c.w_lo)};
-  return launch_conv(a, in, wt, 9, st, err, err_len);
+int conv3x3(int B, int H, int W, int C, int N, Pair in, Pair w, const float* bias, float* u_out, Pair out,
+            cudaStream_t st, char* err, size_t err_len) {
+  ConvArgs a = conv3x3_args(B, C, N, H, W, kModeAct);
+  a.act.bias = bias; a.act.gain = 1.f; a.act.slope = 0.f;
+  a.act.a_hi = out.hi; a.act.a_lo = out.lo;
+  a.act.u_out = u_out;
+  return launch_conv(a, in, w, 9, st, err, err_len);
+}
+
+int conv3x3_adjoint(int B, int H, int W, int C, int N, Pair in, Pair w, float* raw_out, cudaStream_t st,
+                    char* err, size_t err_len) {
+  ConvArgs a = conv3x3_args(B, C, N, H, W, kModeRaw, true);
+  a.out_raw = raw_out;
+  return launch_conv(a, in, w, 9, st, err, err_len);
 }
 
 int prep_weights3x3(const float* w, int cout, int cin, int transposed, __nv_bfloat16* hi,
@@ -2573,7 +2516,7 @@ int prep_weights3x3(const float* w, int cout, int cin, int transposed, __nv_bflo
     prep_weights_t_kernel<<<grid, 256, 0, st>>>(w, cout, cin, 9, hi, lo);
   else
     prep_weights_kernel<<<grid, 256, 0, st>>>(w, cout, cin, 9, hi, lo, nullptr);
-  NFI_SCUDA(cudaGetLastError());
+  NFI_LAUNCH_CHECK(cudaGetLastError());
   return 0;
 }
 
@@ -2583,22 +2526,21 @@ size_t wgrad3x3_partial_floats(int B, int H, int W, int cout, int cin) {
   return (size_t)a.n_split * a.taps * cout * cin;
 }
 
-int wgrad3x3(const Wgrad3x3& c, cudaStream_t st, char* err, size_t err_len) {
-  if (c.g_channels < c.cout || c.g_channels % 8 != 0 || c.cin % 8 != 0) {
+int wgrad3x3(int B, int H, int W, int cout, int cin, int g_channels, Pair g, Pair x, const float* w,
+             float* partials, float* g_w, cudaStream_t st, char* err, size_t err_len) {
+  if (g_w == nullptr) return 0;
+  if (g_channels < cout || g_channels % 8 != 0 || cin % 8 != 0) {
     snprintf(err, err_len, "conv weight gradient: unsupported channel counts (G %d for Cout %d, Cin %d)",
-             c.g_channels, c.cout, c.cin);
+             g_channels, cout, cin);
     return 1;
   }
-  WgradArgs a = conv3x3_wgrad(c.cout, c.cin);
-  plan_wgrad(a, c.B, c.H, c.W);
-  a.part = c.partials;
-  const Pair g = {const_cast<__nv_bfloat16*>(c.g_hi), const_cast<__nv_bfloat16*>(c.g_lo)};
-  const Pair x = {const_cast<__nv_bfloat16*>(c.x_hi), const_cast<__nv_bfloat16*>(c.x_lo)};
-  if (const int rc = launch_wgrad(a, g, c.B, c.H, c.W, x, c.B, c.H, c.W, st, err, err_len, c.g_channels))
-    return rc;
+  WgradArgs a = conv3x3_wgrad(cout, cin);
+  plan_wgrad(a, B, H, W);
+  a.part = partials;
+  if (const int rc = launch_wgrad(a, g, B, H, W, x, B, H, W, st, err, err_len, g_channels)) return rc;
   wgrad_reduce_kernel<<<blocks((size_t)a.cout * a.cin, 256), 256, 0, st>>>(
-      c.partials, a.n_split, a.taps, a.cout, a.cin, c.w, nullptr, nullptr, nullptr, c.B, c.g_w);
-  NFI_SCUDA(cudaGetLastError());
+      partials, a.n_split, a.taps, a.cout, a.cin, w, nullptr, nullptr, nullptr, B, g_w);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
   return 0;
 }
 

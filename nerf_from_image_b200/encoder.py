@@ -40,10 +40,6 @@ MAPS = _lib.ENCODER_MAPS
 SCALE = 4   # SegFormer's output is 1/4 of the image (encoder.py:75-80)
 
 
-def _ptr(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-
 def _conv_ok(m, cin, cout):
     return (isinstance(m, nn.Conv2d) and type(m).forward is nn.Conv2d.forward
             and m.in_channels == cin and m.out_channels == cout
@@ -136,17 +132,17 @@ class _HeadsFunction(torch.autograd.Function):
             p = _lib.EncoderParams()
             p.batch, p.height, p.width, p.channels = B, h, w, C
             p.pose_regressor, p.latent_regressor, p.save = int(pose), int(latent), save
-            p.features, p.features_latent = _ptr(fc), _ptr(flc)
+            p.features, p.features_latent = _lib.ptr(fc), _lib.ptr(flc)
             (p.post0_w, p.post0_b, p.post2_w, p.post2_b, p.post4_w, p.post4_b, p.wpre_w,
-             p.wpre_b) = [_ptr(t) for t in wc]
-            p.maps, p.pooled = (_ptr(maps) if pose else None), (_ptr(pooled) if latent else None)
+             p.wpre_b) = [_lib.ptr(t) for t in wc]
+            p.maps, p.pooled = (_lib.ptr(maps) if pose else None), (_lib.ptr(pooled) if latent else None)
             nbytes = lib.nfi_encoder_workspace_bytes(ctypes.byref(p))
             if nbytes == 0:
                 raise _lib.NfiError('fused encoder: sizes outside the kernels\' envelope (B %d, features '
                                     '%d x %d, %d channels)' % (B, h, w, C))
             work = torch.empty(nbytes, dtype=torch.uint8, device=dev)
             p.workspace, p.workspace_bytes = work.data_ptr(), nbytes
-            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            stream = _lib.stream(dev)
             _lib.check(lib.nfi_encoder_forward(ctypes.byref(p), stream))
         # the backward reads the workspace and the tensors behind p's pointers
         ctx.state = (p, work, fc, flc, wc) if save else None
@@ -155,13 +151,7 @@ class _HeadsFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_maps, g_pooled):
-        if ctx.state is None:
-            raise _lib.NfiError('the fused encoder backward ran twice on one forward (retain_graph is '
-                                'not supported: the workspace is released)')
-        if torch.is_grad_enabled():
-            raise _lib.NfiError('the fused encoder backward is not differentiable (create_graph)')
-        p, work, fc, flc, wc = ctx.state
-        ctx.state = None
+        p, work, fc, flc, wc = _lib.take_saved(ctx, 'encoder')
         needs = ctx.needs_input_grad
         dev = work.device
         with torch.cuda.device(dev):
@@ -169,15 +159,14 @@ class _HeadsFunction(torch.autograd.Function):
             gfl = torch.zeros_like(flc) if (needs[1] and not ctx.shared) else None
             gw = [torch.zeros_like(t) if (t is not None and needs[4 + i]) else None for i, t in enumerate(wc)]
             g = _lib.EncoderGrads()
-            g.g_features = _ptr(gf)
-            g.g_features_latent = _ptr(gf) if ctx.shared else _ptr(gfl)
+            g.g_features = _lib.ptr(gf)
+            g.g_features_latent = _lib.ptr(gf) if ctx.shared else _lib.ptr(gfl)
             (g.g_post0_w, g.g_post0_b, g.g_post2_w, g.g_post2_b, g.g_post4_w, g.g_post4_b, g.g_wpre_w,
-             g.g_wpre_b) = [_ptr(t) for t in gw]
+             g.g_wpre_b) = [_lib.ptr(t) for t in gw]
             gm = g_maps.to(torch.float32).contiguous() if p.pose_regressor else None
             gp = g_pooled.to(torch.float32).contiguous() if p.latent_regressor else None
-            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            _lib.check(_lib.load().nfi_encoder_backward(ctypes.byref(p), _ptr(gm), _ptr(gp), ctypes.byref(g),
-                                                        stream))
+            _lib.check(_lib.load().nfi_encoder_backward(ctypes.byref(p), _lib.ptr(gm), _lib.ptr(gp),
+                                                        ctypes.byref(g), _lib.stream(dev)))
         del p, work
         return (gf, gfl, None, None, *gw)
 
@@ -187,14 +176,8 @@ def saved_activations(out):
     a call that requires grad, before its backward has run), fp32 channel-last: a dict of
     'x0', 'a1', 'a2' [B,4h,4w,512] (pose head) and 'xl', 'al' [B,h,w,512] (latent head).  Where a
     value is positive the backward takes the ReLU's pass branch; tests read the branches from them."""
-    fn = out.grad_fn
-    while fn is not None and getattr(fn, 'state', None) is None:
-        fn = fn.next_functions[0][0] if fn.next_functions else None
-    if fn is None:
-        raise _lib.NfiError('no saved encoder forward behind this output (or its backward has already '
-                            'released the workspace)')
-    p = fn.state[0]
-    dev = fn.state[1].device
+    p, work = _lib.find_saved(out, 'encoder')[:2]
+    dev = work.device
     lib = _lib.load()
     B, h, w, C = p.batch, p.height, p.width, p.channels
     names = []
@@ -204,10 +187,10 @@ def saved_activations(out):
         names += [(3, 'xl', 1), (4, 'al', 1)]
     res = {}
     with torch.cuda.device(dev):
-        stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        stream = _lib.stream(dev)
         for layer, name, s in names:
             t = torch.empty(B, s * h, s * w, C, device=dev)
-            _lib.check(lib.nfi_encoder_saved_activation(ctypes.byref(p), layer, _ptr(t), stream))
+            _lib.check(lib.nfi_encoder_saved_activation(ctypes.byref(p), layer, _lib.ptr(t), stream))
             res[name] = t
     return res
 

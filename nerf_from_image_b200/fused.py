@@ -38,10 +38,6 @@ DEBUG_BUF = None
 DEBUG_RAY = None
 
 
-def _ptr(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-
 def _f32c(t, name):
     if t is None:
         return None
@@ -58,12 +54,12 @@ def planes_to_channel_last(planes):
     planes = _f32c(planes, 'planes')
     out = torch.empty(B, 3, R, R, C, device=planes.device, dtype=torch.float32)
     lib = _lib.load()
-    stream = ctypes.c_void_p(torch.cuda.current_stream(planes.device).cuda_stream)
+    stream = _lib.stream(planes.device)
     base = planes.data_ptr()
     step = C * R * R * 4
     _lib.check(lib.nfi_planes_to_channel_last(
         ctypes.c_void_p(base), ctypes.c_void_p(base + step),
-        ctypes.c_void_p(base + 2 * step), 3 * C * R * R, B, R, _ptr(out), stream))
+        ctypes.c_void_p(base + 2 * step), 3 * C * R * R, B, R, _lib.ptr(out), stream))
     return out
 
 
@@ -71,8 +67,8 @@ def planes_from_channel_last(planes_cl):
     B, three, R, R2, C = planes_cl.shape
     out = torch.empty(B, 3, C, R, R, device=planes_cl.device, dtype=torch.float32)
     lib = _lib.load()
-    stream = ctypes.c_void_p(torch.cuda.current_stream(planes_cl.device).cuda_stream)
-    _lib.check(lib.nfi_planes_from_channel_last(_ptr(planes_cl), B, R, _ptr(out), stream))
+    stream = _lib.stream(planes_cl.device)
+    _lib.check(lib.nfi_planes_from_channel_last(_lib.ptr(planes_cl), B, R, _lib.ptr(out), stream))
     return out
 
 
@@ -92,12 +88,12 @@ def _make_params(cfg, planes_cl, w1, b1, w2, b2, palette, beta, alpha, c2w,
     p.extra_mode = extra_mode
     p.compute_normals = 0
     p.mlp_mode = cfg.mlp_mode
-    p.planes, p.w1, p.b1, p.w2, p.b2 = (_ptr(planes_cl), _ptr(w1), _ptr(b1),
-                                        _ptr(w2), _ptr(b2))
-    p.palette, p.beta, p.alpha = _ptr(palette), _ptr(beta), _ptr(alpha)
-    p.c2w, p.focal, p.center, p.bbox = _ptr(c2w), _ptr(focal), _ptr(center), _ptr(bbox)
-    p.noise_t, p.noise_u = _ptr(noise_t), _ptr(noise_u)
-    p.view_features, p.w3, p.b3 = _ptr(view_feat), _ptr(w3), _ptr(b3)
+    p.planes, p.w1, p.b1, p.w2, p.b2 = (_lib.ptr(planes_cl), _lib.ptr(w1), _lib.ptr(b1),
+                                        _lib.ptr(w2), _lib.ptr(b2))
+    p.palette, p.beta, p.alpha = _lib.ptr(palette), _lib.ptr(beta), _lib.ptr(alpha)
+    p.c2w, p.focal, p.center, p.bbox = _lib.ptr(c2w), _lib.ptr(focal), _lib.ptr(center), _lib.ptr(bbox)
+    p.noise_t, p.noise_u = _lib.ptr(noise_t), _lib.ptr(noise_u)
+    p.view_features, p.w3, p.b3 = _lib.ptr(view_feat), _lib.ptr(w3), _lib.ptr(b3)
     if rows is not None:
         p.row_offset, p.full_height = int(rows[0]), int(rows[1])
     return p
@@ -171,7 +167,7 @@ class FusedTriplaneRender(torch.autograd.Function):
         lib = _lib.load()
         dev = planes.device
         with torch.cuda.device(dev):
-            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            stream = _lib.stream(dev)
             # [B,3,R,R,32] as synthesis.FusedSynthesis emits it: no re-layout pass
             planes_cl = (_f32c(planes.detach(), 'planes') if channel_last
                          else planes_to_channel_last(planes.detach()))
@@ -225,12 +221,13 @@ class FusedTriplaneRender(torch.autograd.Function):
                              t['focal'], t['center'], t['bbox'], height, width,
                              S, t['noise_t'], t['noise_u'], extra_mode,
                              t['view_feat'], t['w3'], t['b3'], rows)
-            p.rgb, p.depth, p.mask, p.extra = _ptr(rgb), _ptr(depth), _ptr(mask), _ptr(extra)
-            p.z_fine = _ptr(z_fine)
+            p.rgb, p.depth, p.mask = _lib.ptr(rgb), _lib.ptr(depth), _lib.ptr(mask)
+            p.extra = _lib.ptr(extra)
+            p.z_fine = _lib.ptr(z_fine)
             if normals is not None:
-                p.compute_normals, p.normals = 1, _ptr(normals)
+                p.compute_normals, p.normals = 1, _lib.ptr(normals)
             if DEBUG_BUF is not None:
-                p.normals = _ptr(DEBUG_BUF)
+                p.normals = _lib.ptr(DEBUG_BUF)
             if peers:
                 # raw device addresses of this rank's [rgb, depth, mask] slices inside each peer's
                 # buffers (parallel.PeerExchange): the kernel stores its tiles there as well
@@ -249,7 +246,7 @@ class FusedTriplaneRender(torch.autograd.Function):
                     p.peer_done = int(peers['done'])
             ws_bytes = lib.nfi_render_workspace_bytes(ctypes.byref(p))
             ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-            p.workspace, p.workspace_bytes = _ptr(ws), ws_bytes
+            p.workspace, p.workspace_bytes = _lib.ptr(ws), ws_bytes
             if KERNEL_EVENTS is not None:
                 e0 = torch.cuda.Event(enable_timing=True)
                 e1 = torch.cuda.Event(enable_timing=True)
@@ -300,17 +297,17 @@ class FusedTriplaneRender(torch.autograd.Function):
         rgb, mask, extra = saved['out_rgb'], saved['out_mask'], saved.get('out_extra')
         A = cfg.attention_values
         with torch.cuda.device(dev):
-            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            stream = _lib.stream(dev)
             z = lambda ref: torch.zeros_like(ref)
             g = _lib.RenderGrads()
             g_rgb = _f32c(g_rgb, 'grad rgb') if g_rgb is not None else torch.zeros_like(rgb)
-            g.g_rgb = _ptr(g_rgb)
+            g.g_rgb = _lib.ptr(g_rgb)
             g_mask = _f32c(g_mask, 'grad mask') if g_mask is not None else None
-            g.g_mask = _ptr(g_mask)
+            g.g_mask = _lib.ptr(g_mask)
             if extra is not None and g_extra is not None and g_extra.numel() > 0:
                 g_extra = _f32c(g_extra, 'grad extra')
-                g.g_extra, g.out_extra = _ptr(g_extra), _ptr(extra)
-            g.out_rgb, g.out_mask = _ptr(rgb), _ptr(mask)
+                g.g_extra, g.out_extra = _lib.ptr(g_extra), _lib.ptr(extra)
+            g.out_rgb, g.out_mask = _lib.ptr(rgb), _lib.ptr(mask)
             gp_cl = z(planes_cl) if n_planes else None
             gw1 = z(t['w1']) if n_w1 else None
             gb1 = z(t['b1']) if n_b1 else None
@@ -326,22 +323,22 @@ class FusedTriplaneRender(torch.autograd.Function):
             gvf = z(t['view_feat']) if (vd and n_vf) else None
             gw3 = z(t['w3']) if (vd and n_w3) else None
             gb3 = z(t['b3']) if (vd and n_b3) else None
-            g.grad_view_features, g.grad_w3, g.grad_b3 = _ptr(gvf), _ptr(gw3), _ptr(gb3)
+            g.grad_view_features, g.grad_w3, g.grad_b3 = _lib.ptr(gvf), _lib.ptr(gw3), _lib.ptr(gb3)
             (g.grad_planes, g.grad_w1, g.grad_b1, g.grad_w2, g.grad_b2,
              g.grad_palette, g.grad_beta, g.grad_alpha, g.grad_origins,
-             g.grad_dirs) = (_ptr(gp_cl), _ptr(gw1), _ptr(gb1), _ptr(gw2),
-                             _ptr(gb2), _ptr(gpal), _ptr(gbeta), _ptr(galpha),
-                             _ptr(go), _ptr(gd))
+             g.grad_dirs) = (_lib.ptr(gp_cl), _lib.ptr(gw1), _lib.ptr(gb1), _lib.ptr(gw2),
+                             _lib.ptr(gb2), _lib.ptr(gpal), _lib.ptr(gbeta), _lib.ptr(galpha),
+                             _lib.ptr(go), _lib.ptr(gd))
             p = _make_params(cfg, planes_cl, t['w1'], t['b1'], t['w2'], t['b2'],
                              t['palette'], t['beta'], t['alpha'], t['c2w'],
                              t['focal'], t['center'], t['bbox'], height, width,
                              S, t['noise_t'], t['noise_u'], ctx.extra_mode,
                              t['view_feat'], t['w3'], t['b3'], ctx.rows)
-            p.rgb, p.depth, p.mask = _ptr(rgb), _ptr(mask), _ptr(mask)  # unused
-            p.extra = _ptr(extra)
-            p.z_fine = _ptr(z_fine)
+            p.rgb, p.depth, p.mask = _lib.ptr(rgb), _lib.ptr(mask), _lib.ptr(mask)  # unused
+            p.extra = _lib.ptr(extra)
+            p.z_fine = _lib.ptr(z_fine)
             if DEBUG_RAY is not None and DEBUG_BUF is not None:
-                p.normals, p.noise_seed = _ptr(DEBUG_BUF), int(DEBUG_RAY)
+                p.normals, p.noise_seed = _lib.ptr(DEBUG_BUF), int(DEBUG_RAY)
                 p.mlp_mode = cfg.mlp_mode | 0x4000
             # the tensor-core backward keeps its two weight images here (64 KiB; 96 KiB for a
             # view-conditioned decoder, whose weight gradients stay on the SIMT kernel), the
@@ -352,7 +349,7 @@ class FusedTriplaneRender(torch.autograd.Function):
                 ws_bytes = (_lib.BACKWARD_WORKSPACE_BYTES if (n_w1 or n_b1 or n_w2 or n_b2)
                             else _lib.BACKWARD_IMAGES_BYTES)
             ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-            p.workspace, p.workspace_bytes = _ptr(ws), ws_bytes
+            p.workspace, p.workspace_bytes = _lib.ptr(ws), ws_bytes
             _lib.check(lib.nfi_render_backward(ctypes.byref(p), ctypes.byref(g), stream))
             gplanes = None
             if n_planes:  # gradient in the layout the planes came in

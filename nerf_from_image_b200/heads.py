@@ -22,10 +22,6 @@ from . import _lib
 from .fused import planes_from_channel_last, planes_to_channel_last
 
 
-def _ptr(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-
 class SdfPoints(torch.autograd.Function):
     """(planes, w1 [64,32], b1 [64], w2 [1+A,64], b2 [1+A], points [B,N,3] world units) ->
     (d [B,N] first decoder output, g [B,N,3] = d d / d point).  Differentiable in planes and the
@@ -47,8 +43,8 @@ class SdfPoints(torch.autograd.Function):
             d = torch.empty(B, N, device=dev)
             g = torch.empty(B, N, 3, device=dev) if want_grad else None
             p = SdfPoints._params(planes_cl, w1c, b1c, w2c, b2c, pts, scene_range)
-            p.d, p.grad = _ptr(d), _ptr(g)
-            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            p.d, p.grad = _lib.ptr(d), _lib.ptr(g)
+            stream = _lib.stream(dev)
             _lib.check(lib.nfi_sdf_points_forward(ctypes.byref(p), stream))
         ctx.scene_range, ctx.layout = float(scene_range), layout
         ctx.save_for_backward(planes_cl, w1c, b1c, w2c, b2c, pts)
@@ -62,8 +58,8 @@ class SdfPoints(torch.autograd.Function):
         p = _lib.SdfPointsParams()
         p.batch, p.plane_res = planes_cl.shape[0], planes_cl.shape[2]
         p.scene_range, p.n_points = float(scene_range), pts.shape[1]
-        p.planes, p.w1, p.b1, p.w2, p.b2, p.points = (_ptr(planes_cl), _ptr(w1), _ptr(b1), _ptr(w2),
-                                                       _ptr(b2), _ptr(pts))
+        p.planes, p.w1, p.b1, p.w2, p.b2, p.points = (_lib.ptr(planes_cl), _lib.ptr(w1), _lib.ptr(b1),
+                                                       _lib.ptr(w2), _lib.ptr(b2), _lib.ptr(pts))
         return p
 
     @staticmethod
@@ -79,16 +75,16 @@ class SdfPoints(torch.autograd.Function):
             g_g = g_g.to(torch.float32).contiguous() if (g_g is not None and g_g.numel() > 0) else None
             if g_d is None and g_g is None:
                 return (None,) * 9
-            g.g_d, g.g_grad = _ptr(g_d), _ptr(g_g)
+            g.g_d, g.g_grad = _lib.ptr(g_d), _lib.ptr(g_g)
             gp = torch.zeros_like(planes_cl) if n_planes else None
             wgrad = n_w1 or n_b1 or n_w2 or n_b2
             gw1 = torch.zeros_like(w1) if wgrad else None
             gb1 = torch.zeros_like(b1) if wgrad else None
             gw2 = torch.zeros_like(w2) if wgrad else None     # only row 0 receives a gradient
             gb2 = torch.zeros_like(b2) if wgrad else None
-            g.grad_planes, g.grad_w1, g.grad_b1 = _ptr(gp), _ptr(gw1), _ptr(gb1)
-            g.grad_w2_row0, g.grad_b2_0 = _ptr(gw2), _ptr(gb2)
-            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            g.grad_planes, g.grad_w1, g.grad_b1 = _lib.ptr(gp), _lib.ptr(gw1), _lib.ptr(gb1)
+            g.grad_w2_row0, g.grad_b2_0 = _lib.ptr(gw2), _lib.ptr(gb2)
+            stream = _lib.stream(dev)
             _lib.check(lib.nfi_sdf_points_backward(ctypes.byref(p), ctypes.byref(g), stream))
             if n_planes and ctx.layout != 'channel_last':
                 gp = planes_from_channel_last(gp)

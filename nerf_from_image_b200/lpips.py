@@ -30,10 +30,6 @@ CONV_CHANNELS = ((3, 64), (64, 64), (64, 128), (128, 128), (128, 256), (256, 256
 TAP_CHANNELS = (64, 128, 256, 512, 512)
 
 
-def _ptr(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-
 def extract_weights(lpips_loss):
     """(shift [3], scale [3], [13 conv weights], [13 conv biases], [5 lin weights [C]]) of a module
     laid out as the reference's ``LPIPSLoss``: ``.lpips.scaling_layer.shift / .scale``, the Conv2d
@@ -107,8 +103,8 @@ def _params(m, in0, in1, out, save):
     ws = m.weights()
     p = _lib.LpipsParams()
     p.n, p.height, p.width, p.save = in0.shape[0], in0.shape[2], in0.shape[3], save
-    p.in0, p.in1, p.out = _ptr(in0), _ptr(in1), _ptr(out)
-    p.shift, p.scale = _ptr(ws[0]), _ptr(ws[1])
+    p.in0, p.in1, p.out = _lib.ptr(in0), _lib.ptr(in1), _lib.ptr(out)
+    p.shift, p.scale = _lib.ptr(ws[0]), _lib.ptr(ws[1])
     n = len(CONV_CHANNELS)
     for i in range(n):
         p.conv_w[i] = ws[2 + i].data_ptr()
@@ -150,7 +146,7 @@ class _LpipsFunction(torch.autograd.Function):
                 _lib.check(1)
             work = torch.empty(nbytes, dtype=torch.uint8, device=dev)
             p.workspace, p.workspace_bytes = work.data_ptr(), nbytes
-            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            stream = _lib.stream(dev)
             _lib.check(lib.nfi_lpips_forward(ctypes.byref(p), stream))
         # the backward reads the workspace and the tensors behind p's pointers
         ctx.state = (p, a, b, work, ws) if save else None
@@ -159,21 +155,14 @@ class _LpipsFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_out):
-        if ctx.state is None:
-            raise _lib.NfiError('the fused LPIPS backward ran twice on one forward (retain_graph is '
-                                'not supported: the workspace is released)')
-        if torch.is_grad_enabled():
-            raise _lib.NfiError('the fused LPIPS backward is not differentiable (create_graph)')
-        p, a, b, work, ws = ctx.state
-        ctx.state = None
+        p, a, b, work, ws = _lib.take_saved(ctx, 'LPIPS')
         dev = a.device
         with torch.cuda.device(dev):
             g = g_out.to(torch.float32).contiguous()
             grad0 = torch.zeros_like(a)
             grad1 = torch.zeros_like(b) if p.save == 2 else None
-            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            _lib.check(_lib.load().nfi_lpips_backward(ctypes.byref(p), _ptr(g), _ptr(grad0), _ptr(grad1),
-                                                      stream))
+            _lib.check(_lib.load().nfi_lpips_backward(ctypes.byref(p), _lib.ptr(g), _lib.ptr(grad0),
+                                                      _lib.ptr(grad1), _lib.stream(dev)))
         del p, a, b, work, ws
         n0, n1 = ctx.needs_input_grad[:2]
         return (grad0.to(ctx.in0_dtype) if n0 else None,
@@ -185,23 +174,17 @@ def saved_preactivations(dist):
     that requires grad, before its backward has run), as fp32 [2N,C,h,w] tensors (in0's images
     first) in layer order conv1_1 .. conv5_3.  Tests read the kernel's ReLU and pool branches from
     them."""
-    fn = dist.grad_fn
-    while fn is not None and getattr(fn, 'state', None) is None:
-        fn = fn.next_functions[0][0] if fn.next_functions else None
-    if fn is None:
-        raise _lib.NfiError('no saved LPIPS forward behind this distance (or its backward has '
-                            'already released the workspace)')
-    p = fn.state[0]
+    p, a = _lib.find_saved(dist, 'LPIPS')[:2]
     lib = _lib.load()
-    dev = fn.state[1].device
+    dev = a.device
     out = []
     with torch.cuda.device(dev):
-        stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        stream = _lib.stream(dev)
         level = 0
         for i, (_, cout) in enumerate(CONV_CHANNELS):
             if i in (2, 4, 7, 10):
                 level += 1
             u = torch.empty(2 * p.n, p.height >> level, p.width >> level, cout, device=dev)
-            _lib.check(lib.nfi_lpips_saved_preactivation(ctypes.byref(p), i, _ptr(u), stream))
+            _lib.check(lib.nfi_lpips_saved_preactivation(ctypes.byref(p), i, _lib.ptr(u), stream))
             out.append(u.permute(0, 3, 1, 2))
     return out

@@ -9,15 +9,9 @@ the vector-Jacobian product are one launch each (``nfi_pose_to_matrix``,
 ``nfi_pose_to_matrix_backward``), and the result feeds ``render`` directly.
 """
 
-import ctypes
-
 import torch
 
 from . import _lib
-
-
-def _ptr(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
 
 
 def _prep(t, name, shape_tail):
@@ -43,10 +37,10 @@ class PoseToMatrix(torch.autograd.Function):
         focal = torch.empty(B, device=q_.device, dtype=torch.float32) if z0_ is not None else None
         lib = _lib.load()
         with torch.cuda.device(q_.device):
-            stream = torch.cuda.current_stream().cuda_stream
-            _lib.check(lib.nfi_pose_to_matrix(_ptr(z0_), _ptr(t2_), _ptr(s_), _ptr(q_),
-                                              int(bool(camera_flipped)), B, _ptr(mat),
-                                              _ptr(focal), ctypes.c_void_p(stream)))
+            stream = _lib.stream(q_.device)
+            _lib.check(lib.nfi_pose_to_matrix(_lib.ptr(z0_), _lib.ptr(t2_), _lib.ptr(s_), _lib.ptr(q_),
+                                              int(bool(camera_flipped)), B, _lib.ptr(mat),
+                                              _lib.ptr(focal), stream))
         ctx.save_for_backward(*(t for t in (z0_, t2_, s_, q_) if t is not None))
         ctx.persp = z0_ is not None
         ctx.flipped = int(bool(camera_flipped))
@@ -67,11 +61,11 @@ class PoseToMatrix(torch.autograd.Function):
         g_t2, g_s, g_q = torch.empty_like(t2), torch.empty_like(s), torch.empty_like(q)
         lib = _lib.load()
         with torch.cuda.device(q.device):
-            stream = torch.cuda.current_stream().cuda_stream
+            stream = _lib.stream(q.device)
             _lib.check(lib.nfi_pose_to_matrix_backward(
-                _ptr(z0), _ptr(t2), _ptr(s), _ptr(q), ctx.flipped, B, _ptr(g_mat),
-                _ptr(g_focal), _ptr(g_z0), _ptr(g_t2), _ptr(g_s), _ptr(g_q),
-                ctypes.c_void_p(stream)))
+                _lib.ptr(z0), _lib.ptr(t2), _lib.ptr(s), _lib.ptr(q), ctx.flipped, B, _lib.ptr(g_mat),
+                _lib.ptr(g_focal), _lib.ptr(g_z0), _lib.ptr(g_t2), _lib.ptr(g_s), _lib.ptr(g_q),
+                stream))
         return g_z0, g_t2, g_s, g_q, None
 
 

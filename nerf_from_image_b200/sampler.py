@@ -27,10 +27,6 @@ from .fused import planes_to_channel_last
 OUTPUT_NAMES = ('sdf_distance', 'sigma', 'rgb', 'normals', 'semantics', 'coords')
 
 
-def _ptr(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-
 def _f32c(t, name):
     if t is None:
         return None
@@ -135,13 +131,12 @@ class FusedSampler:
             for k, t in (('planes', self.planes_cl), ('w1', self.w1), ('b1', self.b1),
                          ('w2', self.w2), ('b2', self.b2), ('palette', self.palette),
                          ('beta', self.beta), ('alpha', self.alpha), ('points', pts)):
-                setattr(sp, k, _ptr(t))
+                setattr(sp, k, _lib.ptr(t))
             for k, t in bufs.items():
-                setattr(sp, k, _ptr(t))
+                setattr(sp, k, _lib.ptr(t))
             lib = _lib.load()
             with torch.cuda.device(dev):
-                stream = torch.cuda.current_stream().cuda_stream
-                _lib.check(lib.nfi_sample_field(ctypes.byref(sp), ctypes.c_void_p(stream)))
+                _lib.check(lib.nfi_sample_field(ctypes.byref(sp), _lib.stream(dev)))
         for k, t in bufs.items():
             if t is not None:
                 out[k] = t

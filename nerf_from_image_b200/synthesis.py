@@ -44,10 +44,6 @@ import torch
 from . import _lib
 
 
-def _ptr(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-
 class _Layer:
     """Attribute view of one layer of a flat parameter dict (``from_params``)."""
 
@@ -207,15 +203,15 @@ class FusedSynthesis:
         for kind, i, _ in self._layers():
             dst = getattr(PG, kind)[i]
             dst.g_weight, dst.g_affine_w, dst.g_affine_b, dst.g_bias = (
-                _ptr(g) for g in g_params[k:k + 4])
+                _lib.ptr(g) for g in g_params[k:k + 4])
             k += 4
-        PG.g_const = _ptr(g_params[k])
+        PG.g_const = _lib.ptr(g_params[k])
         it = iter(g_noise)
         for i, (h0, h1) in enumerate(present):
             if h0:
-                PG.conv0[i].g_noise = _ptr(next(it))
+                PG.conv0[i].g_noise = _lib.ptr(next(it))
             if h1:
-                PG.conv1[i].g_noise = _ptr(next(it))
+                PG.conv1[i].g_noise = _lib.ptr(next(it))
         return g_params, g_noise, PG
 
     def _run(self, ws, noise_mode, saved, noises=None, trainable=False):
@@ -241,17 +237,17 @@ class FusedSynthesis:
             return t
 
         def fill(dst, layer, noise):
-            dst.weight = _ptr(f32(layer.weight))
-            dst.affine_w = _ptr(f32(layer.affine.weight))
-            dst.affine_b = _ptr(f32(layer.affine.bias))
-            dst.bias = _ptr(f32(layer.bias))
-            dst.noise = _ptr(f32(noise)) if noise is not None else None
+            dst.weight = _lib.ptr(f32(layer.weight))
+            dst.affine_w = _lib.ptr(f32(layer.affine.weight))
+            dst.affine_b = _lib.ptr(f32(layer.affine.bias))
+            dst.bias = _lib.ptr(f32(layer.bias))
+            dst.noise = _lib.ptr(f32(noise)) if noise is not None else None
 
         with torch.cuda.device(dev):
             for i, blk in enumerate(self.blocks):
                 P.channels[i] = blk.conv1.out_channels
                 if i == 0:
-                    P.const_input = _ptr(f32(blk.const))
+                    P.const_input = _lib.ptr(f32(blk.const))
                 elif noises is not None:
                     fill(P.conv0[i], blk.conv0, noises[i][0])
                 else:
@@ -261,10 +257,10 @@ class FusedSynthesis:
                 else:
                     fill(P.conv1[i], blk.conv1, self._layer_noise(blk.conv1, B, noise_mode, dev))
                 fill(P.torgb[i], blk.torgb, None)
-            P.ws = _ptr(ws)
+            P.ws = _lib.ptr(ws)
             R = net.img_resolution
             planes = torch.empty(B, 3, R, R, 32, device=dev, dtype=torch.float32)
-            P.planes = _ptr(planes)
+            P.planes = _lib.ptr(planes)
             if trainable:
                 sizer = lib.nfi_synthesis_param_workspace_bytes
             else:
@@ -275,8 +271,8 @@ class FusedSynthesis:
                 raise _lib.NfiError('unsupported synthesis configuration (channels must be '
                                     'multiples of 32, resolution a power of two >= 8)')
             work = torch.empty(need, dtype=torch.uint8, device=dev)
-            P.workspace, P.workspace_bytes = _ptr(work), need
-            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            P.workspace, P.workspace_bytes = _lib.ptr(work), need
+            stream = _lib.stream(dev)
             fwd = lib.nfi_synthesis_forward_saved if saved else lib.nfi_synthesis_forward
             _lib.check(fwd(ctypes.byref(P), stream))
             # the launches are stream-ordered; `keep` / `work` may be released by the caching
@@ -295,21 +291,15 @@ class _SynthesisFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_planes):
-        if ctx.state is None:
-            raise _lib.NfiError('the fused synthesis backward ran twice on one forward '
-                                '(retain_graph is not supported: the workspace is released)')
-        if torch.is_grad_enabled():
-            raise _lib.NfiError('the fused synthesis backward is not differentiable (create_graph, '
-                                'e.g. the path-length regulariser): use the reference module')
-        P, keep, work = ctx.state
-        ctx.state = None          # the workspace and fp32 copies go once this returns
+        # the workspace and fp32 copies go once this returns
+        P, keep, work = _lib.take_saved(ctx, 'synthesis', hint='use the reference module')
         dev = g_planes.device
         g_planes = g_planes.to(torch.float32).contiguous()
         ws32 = keep[0]
         g_ws = torch.zeros_like(ws32)
         G = _lib.SynthGrads(g_planes=g_planes.data_ptr(), g_ws=g_ws.data_ptr())
         with torch.cuda.device(dev):
-            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            stream = _lib.stream(dev)
             _lib.check(_lib.load().nfi_synthesis_backward(ctypes.byref(P), ctypes.byref(G), stream))
         del P, keep, work
         return g_ws.to(ctx.ws_dtype), None, None
@@ -334,14 +324,8 @@ class _SynthesisTrainFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_planes):
-        if ctx.state is None:
-            raise _lib.NfiError('the fused synthesis backward ran twice on one forward '
-                                '(retain_graph is not supported: the workspace is released)')
-        if torch.is_grad_enabled():
-            raise _lib.NfiError('the fused synthesis backward is not differentiable (create_graph, '
-                                'e.g. the path-length regulariser): use the reference module')
-        P, keep, work = ctx.state
-        ctx.state = None          # the workspace and fp32 copies go once this returns
+        # the workspace and fp32 copies go once this returns
+        P, keep, work = _lib.take_saved(ctx, 'synthesis', hint='use the reference module')
         dev = g_planes.device
         g_planes = g_planes.to(torch.float32).contiguous()
         ws32 = keep[0]
@@ -349,7 +333,7 @@ class _SynthesisTrainFunction(torch.autograd.Function):
         G = _lib.SynthGrads(g_planes=g_planes.data_ptr(), g_ws=g_ws.data_ptr())
         g_params, g_noise, PG = ctx.fs._param_grads(ctx.present, ctx.param_meta, ctx.noise_meta, dev)
         with torch.cuda.device(dev):
-            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            stream = _lib.stream(dev)
             _lib.check(_lib.load().nfi_synthesis_backward_params(
                 ctypes.byref(P), ctypes.byref(G), ctypes.byref(PG), stream))
         del P, keep, work
@@ -378,7 +362,7 @@ class _PathLengthFunction(torch.autograd.Function):
         G = _lib.SynthGrads(g_planes=pl_noise.data_ptr(), g_ws=pl_grad.data_ptr())
         dev = ws.device
         with torch.cuda.device(dev):
-            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            stream = _lib.stream(dev)
             _lib.check(_lib.load().nfi_synthesis_backward(ctypes.byref(P), ctypes.byref(G), stream))
         ctx.state, ctx.fs, ctx.present, ctx.ws_dtype = link.state, link.fs, link.present, ws.dtype
         ctx.pl_noise = pl_noise
@@ -390,14 +374,7 @@ class _PathLengthFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, t_ws):
-        if ctx.state is None:
-            raise _lib.NfiError('the fused path-length backward ran twice on one forward '
-                                '(retain_graph is not supported: the workspace is released)')
-        if torch.is_grad_enabled():
-            raise _lib.NfiError('the fused path-length backward is not differentiable '
-                                '(create_graph)')
-        P, keep, work = ctx.state
-        ctx.state = None
+        P, keep, work = _lib.take_saved(ctx, 'path-length')
         dev = t_ws.device
         lib = _lib.load()
         t_ws = t_ws.to(torch.float32).contiguous()
@@ -408,7 +385,7 @@ class _PathLengthFunction(torch.autograd.Function):
             scratch = torch.empty(need, dtype=torch.uint8, device=dev)
             H = _lib.SynthHvp(g_planes=ctx.pl_noise.data_ptr(), t_ws=t_ws.data_ptr(),
                               g_ws=g_ws.data_ptr(), scratch=scratch.data_ptr(), scratch_bytes=need)
-            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            stream = _lib.stream(dev)
             _lib.check(lib.nfi_synthesis_backward_hvp(ctypes.byref(P), ctypes.byref(H),
                                                       ctypes.byref(PG), stream))
         del P, keep, work, scratch
@@ -424,16 +401,12 @@ def saved_preactivations(planes):
     ``forward_trainable_with_path_length``, before its backward has run), as fp32 channel-last
     [B,res,res,C] tensors in layer order: b4.conv1, b8.conv0, b8.conv1, ...  Tests read it to
     compare the forward's leaky-ReLU branches with a reference."""
-    state = getattr(planes.grad_fn, 'state', None)
-    if state is None:
-        raise _lib.NfiError('no saved synthesis forward behind these planes (or its backward has '
-                            'already released the workspace)')
-    P, _, _ = state
+    P, _, _ = _lib.find_saved(planes, 'synthesis')
     lib = _lib.load()
     B, dev = P.batch, planes.device
     out = []
     with torch.cuda.device(dev):
-        stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        stream = _lib.stream(dev)
         for i in range(P.num_blocks):
             res = 4 << i
             for which in ((1,) if i == 0 else (0, 1)):

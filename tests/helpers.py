@@ -1,5 +1,6 @@
-"""Shared helpers for the parity tests (oracle side and CUDA side)."""
+"""Shared helpers for the parity tests (oracle side and CUDA side) and the C-header checks."""
 import os
+import re
 
 import torch
 
@@ -112,3 +113,15 @@ def reference_output(request, fn, part=''):
             torch.save(_detached(out), path)
         return out
     return torch.load(path, weights_only=True)
+
+
+def header_functions(src):
+    """The functions C header source ``src`` declares with NFI_API."""
+    return re.findall(r'NFI_API\s+[\w\s\*]+?\b(nfi_\w+)\s*\(', src)
+
+
+def struct_fields(src, name):
+    """The field names of ``typedef struct name {...} name;`` in C header source ``src``, in order."""
+    body = re.search(r'typedef struct %s \{(.*?)\} %s;' % (name, name), src, re.S).group(1)
+    body = re.sub(r'/\*.*?\*/', '', body, flags=re.S)
+    return [re.search(r'(\w+)\s*(?:\[\w+\])?$', d.strip()).group(1) for d in body.split(';') if d.strip()]

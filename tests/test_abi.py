@@ -5,6 +5,7 @@ import os
 import re
 
 from nerf_from_image_b200 import _lib
+from tests import helpers as Hh
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HEADER = os.path.join(ROOT, 'include', 'nfi_render.h')
@@ -13,8 +14,7 @@ HEADS_HEADER = os.path.join(ROOT, 'include', 'nfi_heads.h')
 
 
 def header_functions():
-    src = open(HEADER).read() + open(SYNTH_HEADER).read() + open(HEADS_HEADER).read()
-    return re.findall(r'NFI_API\s+[\w\s\*]+?\b(nfi_\w+)\s*\(', src)
+    return Hh.header_functions(open(HEADER).read() + open(SYNTH_HEADER).read() + open(HEADS_HEADER).read())
 
 
 def test_header_and_binding_agree():
@@ -42,11 +42,7 @@ def test_struct_layout_matches_header():
                        ('nfi_synth_params', _lib.SynthParams),
                        ('nfi_sdf_points_params', _lib.SdfPointsParams),
                        ('nfi_sdf_points_grads', _lib.SdfPointsGrads)):
-        body = re.search(r'typedef struct %s \{(.*?)\} %s;' % (cname, cname), src, re.S).group(1)
-        body = re.sub(r'/\*.*?\*/', '', body, flags=re.S)
-        fields = [re.search(r'(\w+)\s*(?:\[\w+\])?$', d.strip()).group(1)
-                  for d in body.split(';') if d.strip()]
-        assert fields == [f[0] for f in cls._fields_], cname
+        assert Hh.struct_fields(src, cname) == [f[0] for f in cls._fields_], cname
 
 
 def test_errors_are_reported_without_a_gpu():
@@ -59,7 +55,6 @@ def test_errors_are_reported_without_a_gpu():
 
 def test_no_cpu_fallback():
     import pytest
-    from tests import helpers as Hh
     scene, cams = Hh.make_case('p3d_plain', batch=1, plane_res=8)
     with pytest.raises(_lib.NfiError):
         Hh.run_cuda(scene, cams, 8, 8, 8, None, None, device='cpu')

@@ -2,9 +2,11 @@
 _lib.EncoderGrads) and the built library, without a GPU."""
 import ctypes
 import os
-import re
+
+import pytest
 
 from nerf_from_image_b200 import _lib
+from tests import helpers as Hh
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HEADER = os.path.join(ROOT, 'include', 'nfi_encoder.h')
@@ -14,14 +16,8 @@ def _src():
     return open(HEADER).read()
 
 
-def _fields(src, name):
-    body = re.search(r'typedef struct %s \{(.*?)\} %s;' % (name, name), src, re.S).group(1)
-    body = re.sub(r'/\*.*?\*/', '', body, flags=re.S)
-    return [re.search(r'(\w+)\s*(?:\[\w+\])?$', d.strip()).group(1) for d in body.split(';') if d.strip()]
-
-
 def test_header_and_table_agree():
-    names = re.findall(r'NFI_API\s+[\w\s\*]+?\b(nfi_\w+)\s*\(', _src())
+    names = Hh.header_functions(_src())
     assert len(names) == 4
     assert sorted(names) == sorted(_lib.ENCODER_EXPORTS)
     assert not set(names) & (set(_lib.EXPORTS) | set(_lib.LPIPS_EXPORTS))
@@ -37,8 +33,8 @@ def test_library_exports_the_encoder_symbols():
 def test_struct_layouts_match_the_header():
     src = _src()
     assert '#define NFI_ENCODER_MAPS %d' % _lib.ENCODER_MAPS in src
-    assert _fields(src, 'nfi_encoder_params') == [f[0] for f in _lib.EncoderParams._fields_]
-    assert _fields(src, 'nfi_encoder_grads') == [f[0] for f in _lib.EncoderGrads._fields_]
+    assert Hh.struct_fields(src, 'nfi_encoder_params') == [f[0] for f in _lib.EncoderParams._fields_]
+    assert Hh.struct_fields(src, 'nfi_encoder_grads') == [f[0] for f in _lib.EncoderGrads._fields_]
 
 
 def _params(b=2, h=8, w=8, c=512, pose=1, latent=1, save=1):
@@ -69,3 +65,21 @@ def test_workspace_sizes_and_refusals_without_a_gpu():
     assert lib.nfi_encoder_backward(ctypes.byref(_params()), None, None, None, None) != 0
     assert lib.nfi_encoder_saved_activation(ctypes.byref(_params()), 5, None, None) != 0
     assert lib.nfi_encoder_saved_activation(ctypes.byref(_params(latent=0)), 3, ctypes.c_void_p(16), None) != 0
+
+
+# Exact workspace totals at the encoder-training feature size (32 x 32 x 512, 128^2 images): the
+# forward, the backward and saved_activation walk one layout, so a buffer lost, taken twice or
+# resized changes a total.  (B, pose head, latent head, save) -> bytes.
+WORKSPACE_TOTALS = {
+    (2, 1, 0, 0): 163252224, (2, 1, 0, 1): 412157952, (2, 0, 1, 0): 22021120,
+    (2, 0, 1, 1): 58737664, (2, 1, 1, 0): 181078016, (2, 1, 1, 1): 439420928,
+    (32, 1, 0, 0): 2302347264, (32, 1, 0, 1): 5700913152, (32, 0, 1, 0): 210764800,
+    (32, 0, 1, 1): 373556224, (32, 1, 1, 0): 2446002176, (32, 1, 1, 1): 5854005248,
+}
+
+
+@pytest.mark.parametrize('b, pose, latent, save', sorted(WORKSPACE_TOTALS))
+def test_workspace_keeps_its_totals(b, pose, latent, save):
+    lib = _lib.load()
+    p = _params(b=b, h=32, w=32, pose=pose, latent=latent, save=save)
+    assert lib.nfi_encoder_workspace_bytes(ctypes.byref(p)) == WORKSPACE_TOTALS[(b, pose, latent, save)]

@@ -2,9 +2,11 @@
 library, without a GPU.  (The other headers and _lib.EXPORTS are checked by tests/test_abi.py.)"""
 import ctypes
 import os
-import re
+
+import pytest
 
 from nerf_from_image_b200 import _lib
+from tests import helpers as Hh
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HEADER = os.path.join(ROOT, 'include', 'nfi_lpips.h')
@@ -15,7 +17,7 @@ def _src():
 
 
 def test_header_and_table_agree():
-    names = re.findall(r'NFI_API\s+[\w\s\*]+?\b(nfi_\w+)\s*\(', _src())
+    names = Hh.header_functions(_src())
     assert len(names) == 4
     assert sorted(names) == sorted(_lib.LPIPS_EXPORTS)
     assert not set(names) & set(_lib.EXPORTS)
@@ -32,10 +34,7 @@ def test_struct_layout_matches_the_header():
     src = _src()
     assert '#define NFI_LPIPS_CONVS %d' % _lib.LPIPS_CONVS in src
     assert '#define NFI_LPIPS_TAPS %d' % _lib.LPIPS_TAPS in src
-    body = re.search(r'typedef struct nfi_lpips_params \{(.*?)\} nfi_lpips_params;', src, re.S).group(1)
-    body = re.sub(r'/\*.*?\*/', '', body, flags=re.S)
-    fields = [re.search(r'(\w+)\s*(?:\[\w+\])?$', d.strip()).group(1) for d in body.split(';') if d.strip()]
-    assert fields == [f[0] for f in _lib.LpipsParams._fields_]
+    assert Hh.struct_fields(src, 'nfi_lpips_params') == [f[0] for f in _lib.LpipsParams._fields_]
 
 
 def _params(n=2, h=32, w=32, save=1):
@@ -66,3 +65,20 @@ def test_workspace_sizes_and_refusals_without_a_gpu():
     assert lib.nfi_lpips_workspace_bytes(ctypes.byref(_params(save=2))) > saved
     assert lib.nfi_lpips_workspace_bytes(ctypes.byref(_params(save=3))) == 0
     assert lib.nfi_lpips_saved_preactivation(ctypes.byref(_params()), 13, None, None) != 0
+
+
+# Exact workspace totals: the forward, the backward and saved_preactivation walk one layout, so a
+# buffer lost, taken twice or resized changes a total.  (N, H = W, save) -> bytes.
+WORKSPACE_TOTALS = {
+    (1, 16, 0): 59361280, (1, 16, 1): 118683648, (1, 16, 2): 118880256,
+    (1, 128, 0): 92392448, (1, 128, 1): 182422528, (1, 128, 2): 195005440,
+    (256, 16, 0): 193061888, (256, 16, 1): 376677376, (256, 16, 2): 427009024,
+    (256, 128, 0): 8649119744, (256, 128, 1): 16693909504, (256, 128, 2): 19915134976,
+}
+
+
+@pytest.mark.parametrize('n, hw, save', sorted(WORKSPACE_TOTALS))
+def test_workspace_keeps_its_totals(n, hw, save):
+    lib = _lib.load()
+    got = lib.nfi_lpips_workspace_bytes(ctypes.byref(_params(n=n, h=hw, w=hw, save=save)))
+    assert got == WORKSPACE_TOTALS[(n, hw, save)]

@@ -4,12 +4,12 @@ oracle.synthesis_oracle, and the C ABI of the parameter backward (struct mirror,
 paths, workspace sizing)."""
 import ctypes
 import os
-import re
 
 import pytest
 import torch
 
 from oracle import synthesis_oracle as SO
+from tests import helpers as Hh
 from tests import synthesis_param_backward_oracle as SP
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -63,13 +63,9 @@ def test_torgb_decomposition_equals_autograd():
 def test_param_grads_struct_mirrors_the_header():
     from nerf_from_image_b200 import _lib
     src = open(os.path.join(ROOT, 'include', 'nfi_synth.h')).read()
-    src = re.sub(r'/\*.*?\*/', '', src, flags=re.S)
     for cname, cls in (('nfi_synth_layer_grads', _lib.SynthLayerGrads),
                        ('nfi_synth_param_grads', _lib.SynthParamGrads)):
-        body = re.search(r'typedef struct %s \{(.*?)\} %s;' % (cname, cname), src, re.S).group(1)
-        fields = [re.search(r'(\w+)\s*(?:\[\w+\])?$', d.strip()).group(1)
-                  for d in body.split(';') if d.strip()]
-        assert fields == [f[0] for f in cls._fields_], cname
+        assert Hh.struct_fields(src, cname) == [f[0] for f in cls._fields_], cname
     ptr = ctypes.sizeof(ctypes.c_void_p)
     assert ctypes.sizeof(_lib.SynthLayerGrads) == 5 * ptr
     assert ctypes.sizeof(_lib.SynthParamGrads) == (3 * _lib.SYNTH_MAX_BLOCKS * 5 + 1) * ptr
