@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define NFI_ABI_VERSION 5
+#define NFI_ABI_VERSION 6
 
 #if defined(__GNUC__)
 #define NFI_API __attribute__((visibility("default")))

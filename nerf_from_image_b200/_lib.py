@@ -17,7 +17,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get('NFI_LIB_PATH') or os.path.join(_HERE, 'csrc', 'libnfi_render.so')
 
 c_float_p = ctypes.POINTER(ctypes.c_float)
-ABI_VERSION = 5  # NFI_ABI_VERSION of include/nfi_render.h
+ABI_VERSION = 6  # NFI_ABI_VERSION of include/nfi_render.h
 MAX_PEERS = 7
 BACKWARD_IMAGES_BYTES = 65536  # the two weight images of a frozen-decoder backward (nfi_layout.h)
 BACKWARD_WORKSPACE_BYTES = 65536 + 160 * 32768  # NFI_BACKWARD_WORKSPACE_BYTES
@@ -181,10 +181,34 @@ class EncoderGrads(ctypes.Structure):
         'g_post4_w', 'g_post4_b', 'g_wpre_w', 'g_wpre_b')]
 
 
+DISC_MAX_BLOCKS = 6
+
+
+class DiscParams(ctypes.Structure):
+    """struct nfi_disc_params (include/nfi_disc.h)."""
+    _fields_ = [(n, ctypes.c_int32) for n in (
+        'batch', 'resolution', 'img_channels', 'cmap_dim', 'save')] + [
+        (n, ctypes.c_void_p) for n in ('img', 'cmap', 'fromrgb_w', 'fromrgb_b')] + [
+        (n, ctypes.c_void_p * DISC_MAX_BLOCKS) for n in (
+            'conv0_w', 'conv0_b', 'conv1_w', 'conv1_b', 'skip_w')] + [
+        (n, ctypes.c_void_p) for n in (
+            'b4_conv_w', 'b4_conv_b', 'fc_w', 'fc_b', 'out_w', 'out_b', 'logits', 'workspace')] + [
+        ('workspace_bytes', ctypes.c_size_t)]
+
+
+class DiscGrads(ctypes.Structure):
+    """struct nfi_disc_grads."""
+    _fields_ = [(n, ctypes.c_void_p) for n in ('fromrgb_w', 'fromrgb_b')] + [
+        (n, ctypes.c_void_p * DISC_MAX_BLOCKS) for n in (
+            'conv0_w', 'conv0_b', 'conv1_w', 'conv1_b', 'skip_w')] + [
+        (n, ctypes.c_void_p) for n in ('b4_conv_w', 'b4_conv_b', 'fc_w', 'fc_b', 'out_w', 'out_b')]
+
+
 # every symbol include/nfi_render.h, nfi_synth.h and nfi_heads.h declare (tests/test_abi.py checks
 # those headers against this table and the table against the built library); LPIPS_EXPORTS and
 # ENCODER_EXPORTS below hold the symbols of include/nfi_lpips.h (tests/test_lpips_abi.py) and
-# include/nfi_encoder.h (tests/test_encoder_abi.py)
+# include/nfi_encoder.h (tests/test_encoder_abi.py), DISC_EXPORTS those of include/nfi_disc.h
+# (tests/test_disc_abi.py)
 EXPORTS = {
     'nfi_abi_version': (ctypes.c_int, []),
     'nfi_build_info': (ctypes.c_char_p, []),
@@ -261,6 +285,15 @@ ENCODER_EXPORTS = {
                                                     ctypes.c_void_p, ctypes.c_void_p]),
 }
 
+DISC_EXPORTS = {
+    'nfi_disc_workspace_bytes': (ctypes.c_size_t, [ctypes.POINTER(DiscParams)]),
+    'nfi_disc_forward': (ctypes.c_int, [ctypes.POINTER(DiscParams), ctypes.c_void_p]),
+    'nfi_disc_backward': (ctypes.c_int, [ctypes.POINTER(DiscParams), ctypes.c_void_p, ctypes.c_void_p,
+                                         ctypes.c_void_p, ctypes.POINTER(DiscGrads), ctypes.c_void_p]),
+    'nfi_disc_saved_preactivation': (ctypes.c_int, [ctypes.POINTER(DiscParams), ctypes.c_int32,
+                                                    ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p]),
+}
+
 _lib = None
 _lock = threading.Lock()
 
@@ -301,7 +334,7 @@ def load():
                 raise NfiError('%s has ABI version %d, this binding needs %d: rebuild it '
                                '(nerf_from_image_b200/csrc/build.sh)' % (LIB_PATH, got, ABI_VERSION))
             for name, (restype, argtypes) in (list(EXPORTS.items()) + list(LPIPS_EXPORTS.items())
-                                       + list(ENCODER_EXPORTS.items())):
+                                       + list(ENCODER_EXPORTS.items()) + list(DISC_EXPORTS.items())):
                 fn = getattr(lib, name, None)
                 if fn is None and os.environ.get('NFI_LIB_PATH'):
                     continue  # an older build under test lacks the newer entry points

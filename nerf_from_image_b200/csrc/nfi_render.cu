@@ -15,6 +15,8 @@
 #include "nfi_route.h"
 #include "nfi_heads.h"
 #include "nfi_heads_launch.h"
+#include "nfi_disc.h"
+#include "nfi_disc_launch.h"
 #include "nfi_encoder.h"
 #include "nfi_encoder_launch.h"
 #include "nfi_lpips.h"
@@ -524,6 +526,29 @@ int nfi_encoder_backward(const nfi_encoder_params* params, const float* g_maps, 
 int nfi_encoder_saved_activation(const nfi_encoder_params* params, int32_t layer, float* out, void* stream) {
   if (params == nullptr) return fail("params is NULL");
   return nfi::encoder::saved_activation(*params, layer, out, (cudaStream_t)stream, g_err, sizeof(g_err));
+}
+
+size_t nfi_disc_workspace_bytes(const nfi_disc_params* params) {
+  if (params == nullptr) return 0;
+  return nfi::disc::workspace_bytes(*params);
+}
+
+int nfi_disc_forward(const nfi_disc_params* params, void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  return nfi::disc::forward(*params, (cudaStream_t)stream, g_err, sizeof(g_err));
+}
+
+int nfi_disc_backward(const nfi_disc_params* params, const float* g_logits, float* grad_img, float* grad_cmap,
+                      const nfi_disc_grads* grads, void* stream) {
+  if (params == nullptr || grads == nullptr) return fail("params / grads is NULL");
+  return nfi::disc::backward(*params, g_logits, grad_img, grad_cmap, *grads, (cudaStream_t)stream, g_err,
+                             sizeof(g_err));
+}
+
+int nfi_disc_saved_preactivation(const nfi_disc_params* params, int32_t block, int32_t which, float* out,
+                                 void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  return nfi::disc::saved_preactivation(*params, block, which, out, (cudaStream_t)stream, g_err, sizeof(g_err));
 }
 
 size_t nfi_synthesis_workspace_bytes(const nfi_synth_params* params) {

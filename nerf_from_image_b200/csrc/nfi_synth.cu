@@ -2544,5 +2544,72 @@ int wgrad3x3(int B, int H, int W, int cout, int cin, int g_channels, Pair g, Pai
   return 0;
 }
 
+int conv3x3_act(int B, int H, int W, int C, int N, Pair in, Pair w, const float* bias, float gain, float slope,
+                Pair out, cudaStream_t st, char* err, size_t err_len) {
+  ConvArgs a = conv3x3_args(B, C, N, H, W, kModeAct);
+  a.act.bias = bias; a.act.gain = gain; a.act.slope = slope;
+  a.act.a_hi = out.hi; a.act.a_lo = out.lo;
+  return launch_conv(a, in, w, 9, st, err, err_len);
+}
+
+int conv_down3x3(int B, int h, int C, int N, Pair phases, Pair w, float* raw_out, cudaStream_t st, char* err,
+                 size_t err_len) {
+  ConvArgs a = conv_up_adjoint_args(B, C, N, h);
+  a.out_raw = raw_out;
+  return launch_conv(a, phases, w, 9, st, err, err_len, 4 * B);
+}
+
+int conv_up3x3(int B, int h, int C, int N, Pair in, Pair w, float* raw_out, cudaStream_t st, char* err,
+               size_t err_len) {
+  ConvArgs a = conv_up_args(B, C, N, h);
+  a.out_raw = raw_out;
+  return launch_conv(a, in, w, 9, st, err, err_len);
+}
+
+int conv1x1(int B, int H, int C, int N, Pair in, Pair w, float* raw_out, cudaStream_t st, char* err,
+            size_t err_len) {
+  ConvArgs a = torgb_args(B, C, N, H, kModeRaw);
+  a.out_raw = raw_out;
+  return launch_conv(a, in, w, 1, st, err, err_len);
+}
+
+size_t wgrad_down3x3_partial_floats(int B, int h, int cin, int cout) {
+  WgradArgs a = conv0_wgrad(cin, cout, B);
+  plan_wgrad(a, B, h, h);
+  return (size_t)a.n_split * a.taps * cout * cin;
+}
+
+int wgrad_down3x3(int B, int h, int cin, int cout, Pair phases, Pair g, const float* w, float* partials,
+                  float* g_wt, cudaStream_t st, char* err, size_t err_len) {
+  if (g_wt == nullptr) return 0;
+  WgradArgs a = conv0_wgrad(cin, cout, B);
+  plan_wgrad(a, B, h, h);
+  a.part = partials;
+  if (const int rc = launch_wgrad(a, phases, 4 * B, h + 1, h + 1, g, B, h, h, st, err, err_len)) return rc;
+  wgrad_reduce_kernel<<<blocks((size_t)a.cout * a.cin, 256), 256, 0, st>>>(
+      partials, a.n_split, a.taps, a.cout, a.cin, w, nullptr, nullptr, nullptr, B, g_wt);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  return 0;
+}
+
+size_t wgrad1x1_partial_floats(int B, int H, int cout, int cin) {
+  WgradArgs a = torgb_wgrad(cout, cin);
+  plan_wgrad(a, B, H, H);
+  return (size_t)a.n_split * a.taps * cout * cin;
+}
+
+int wgrad1x1(int B, int H, int cout, int cin, Pair g, Pair x, const float* w, float* partials, float* g_w,
+             cudaStream_t st, char* err, size_t err_len) {
+  if (g_w == nullptr) return 0;
+  WgradArgs a = torgb_wgrad(cout, cin);
+  plan_wgrad(a, B, H, H);
+  a.part = partials;
+  if (const int rc = launch_wgrad(a, g, B, H, H, x, B, H, H, st, err, err_len)) return rc;
+  wgrad_reduce_kernel<<<blocks((size_t)a.cout * a.cin, 256), 256, 0, st>>>(
+      partials, a.n_split, a.taps, a.cout, a.cin, w, nullptr, nullptr, nullptr, B, g_w);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  return 0;
+}
+
 }  // namespace synth
 }  // namespace nfi

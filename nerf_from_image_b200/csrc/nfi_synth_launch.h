@@ -51,5 +51,32 @@ int prep_weights3x3(const float* w, int cout, int cin, int transposed, __nv_bflo
 size_t wgrad3x3_partial_floats(int B, int H, int W, int cout, int cin);
 int wgrad3x3(int B, int H, int W, int cout, int cin, int g_channels, Pair g, Pair x, const float* w,
              float* partials, float* g_w, cudaStream_t st, char* err, size_t err_len);
+
+// The discriminator's layers (nfi_disc.cu), on the same two kernels:
+//   conv3x3_act: conv3x3 with the ACT epilogue's gain and negative slope: lrelu(gain (conv + bias))
+//   conv_down3x3: the stride-2 3x3 correlation of a [B,2h+1,2h+1,C] image given as its four parity
+//            phases, phase (py,px) at image offset (2py+px) B of a [4B,h+1,h+1,C] pair; weights
+//            [9][N][C] (transposed 0) -> raw_out fp32 [B,h,h,N]
+//   conv_up3x3: its adjoint, the stride-2 transposed conv of [B,h,h,C] with weights [9][N][C]
+//            (transposed 1 of a [C,N,3,3] layer) -> raw_out fp32 [B,2h+1,2h+1,N]
+//   conv1x1: [B,H,H,C] against weights [1][N][C] -> raw_out fp32 [B,H,H,N]
+//   wgrad_down3x3: conv_down3x3's weight gradient, TRANSPOSED: g_wt[ci,co,ky,kx] += sum over
+//            (b,i,j) of phases(ky%2,kx%2)[b, i+ky/2, j+kx/2, ci] g[b,i,j,co]
+//   wgrad1x1: g_w[co,ci] += sum over positions of g[.,co] x[.,ci], both [B,H,H,.]
+// (`w` as for wgrad3x3: any buffer of the gradient's size; it does not change the result.)
+int conv3x3_act(int B, int H, int W, int C, int N, Pair in, Pair w, const float* bias, float gain, float slope,
+                Pair out, cudaStream_t st, char* err, size_t err_len);
+int conv_down3x3(int B, int h, int C, int N, Pair phases, Pair w, float* raw_out, cudaStream_t st, char* err,
+                 size_t err_len);
+int conv_up3x3(int B, int h, int C, int N, Pair in, Pair w, float* raw_out, cudaStream_t st, char* err,
+               size_t err_len);
+int conv1x1(int B, int H, int C, int N, Pair in, Pair w, float* raw_out, cudaStream_t st, char* err,
+            size_t err_len);
+size_t wgrad_down3x3_partial_floats(int B, int h, int cin, int cout);
+int wgrad_down3x3(int B, int h, int cin, int cout, Pair phases, Pair g, const float* w, float* partials,
+                  float* g_wt, cudaStream_t st, char* err, size_t err_len);
+size_t wgrad1x1_partial_floats(int B, int H, int cout, int cin);
+int wgrad1x1(int B, int H, int cout, int cin, Pair g, Pair x, const float* w, float* partials, float* g_w,
+             cudaStream_t st, char* err, size_t err_len);
 }  // namespace synth
 }  // namespace nfi
