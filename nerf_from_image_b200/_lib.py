@@ -204,6 +204,13 @@ class DiscGrads(ctypes.Structure):
         (n, ctypes.c_void_p) for n in ('b4_conv_w', 'b4_conv_b', 'fc_w', 'fc_b', 'out_w', 'out_b')]
 
 
+class DiscHvp(ctypes.Structure):
+    """struct nfi_disc_hvp (include/nfi_disc_r1.h)."""
+    _fields_ = [(n, ctypes.c_void_p) for n in ('g_logits', 't_img', 'scratch')] + [
+        ('scratch_bytes', ctypes.c_size_t)] + [
+        (n, ctypes.c_void_p) for n in ('grad_img', 'grad_cmap', 'grad_g_logits')]
+
+
 # every symbol include/nfi_render.h, nfi_synth.h and nfi_heads.h declare (tests/test_abi.py checks
 # those headers against this table and the table against the built library); LPIPS_EXPORTS and
 # ENCODER_EXPORTS below hold the symbols of include/nfi_lpips.h (tests/test_lpips_abi.py) and
@@ -294,6 +301,13 @@ DISC_EXPORTS = {
                                                     ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p]),
 }
 
+# include/nfi_disc_r1.h (tests/test_disc_r1_abi.py)
+DISC_R1_EXPORTS = {
+    'nfi_disc_r1_scratch_bytes': (ctypes.c_size_t, [ctypes.POINTER(DiscParams)]),
+    'nfi_disc_backward_hvp': (ctypes.c_int, [ctypes.POINTER(DiscParams), ctypes.POINTER(DiscHvp),
+                                             ctypes.POINTER(DiscGrads), ctypes.c_void_p]),
+}
+
 _lib = None
 _lock = threading.Lock()
 
@@ -334,7 +348,8 @@ def load():
                 raise NfiError('%s has ABI version %d, this binding needs %d: rebuild it '
                                '(nerf_from_image_b200/csrc/build.sh)' % (LIB_PATH, got, ABI_VERSION))
             for name, (restype, argtypes) in (list(EXPORTS.items()) + list(LPIPS_EXPORTS.items())
-                                       + list(ENCODER_EXPORTS.items()) + list(DISC_EXPORTS.items())):
+                                       + list(ENCODER_EXPORTS.items()) + list(DISC_EXPORTS.items())
+                                       + list(DISC_R1_EXPORTS.items())):
                 fn = getattr(lib, name, None)
                 if fn is None and os.environ.get('NFI_LIB_PATH'):
                     continue  # an older build under test lacks the newer entry points

@@ -993,5 +993,449 @@ int saved_preactivation(const nfi_disc_params& P, int block, int which, float* o
   return 0;
 }
 
+
+// ================================================================ R1: the double backward
+// (C ABI: include/nfi_disc_r1.h).  With L = sum_b g_logits[b] logits[b] and a tangent t of the
+// image, the pass returns the gradients of Phi = <t, dL/dimg>: the tangent of every first-order
+// gradient along img + eps t.  Three properties of the network keep it small:
+//   1. every layer but the minibatch std is piecewise linear in the image; on the saved forward's
+//      leaky-ReLU branches lrelu'' = 0, so a layer's tangent is its linear map times lrelu';
+//   2. above the minibatch std the first-order cotangents (g_out = g_logits cmap / sqrt N, g_hf,
+//      g_uf, g_a4, g_u4, g_xs and the std channel's g_sd) do not depend on the image: their
+//      tangents are zero.  So the epilogue's weight terms are g (x) a-dot only (xs-dot for the
+//      conv, a4-dot for fc, hf-dot for out), its three biases get exactly zero, and
+//      dPhi/dcmap = g_logits out-dot / sqrt N;
+//   3. the minibatch std is the one second-order kernel: with v = mean_k (x_k - mu)^2 over a group
+//      of 4 and s = sqrt(v + 1e-8) its backward is G_j / (16 * 512) (x_k - mu) / (4 s); its tangent
+//      along x4-dot seeds the blocks' reverse walk, where g-dot runs through the same linear maps
+//      as g.
+// Kernels:
+//   tangent forward from t, on the saved branches: fromrgb_tangent_kernel; conv0 RAW
+//   (nfi::synth::conv3x3, zero bias) then act_tangent_kernel; fir_phases_kernel and conv1
+//   (conv_down3x3); fir_down_kernel and the skip (conv1x1); block_out_tangent_kernel;
+//   mbstd_tangent_kernel; b4_conv_kernel / linear_kernel with a zero bias, then
+//   act_backward_kernel for the branches; logits_kernel (J_img t, the g_logits gradient).
+//   reverse walk: the epilogue's g as in the first-order backward, mbstd_backward_kernel (g) and
+//   mbstd_hvp_kernel (g-dot) into one stacked [g; g-dot] buffer of 2B images; per block the data
+//   GEMMs (conv_up3x3, conv3x3_adjoint, conv1x1) and fir_down_adjoint_kernel run once over the 2B
+//   images, the pointwise passes (out_backward_kernel, fir_up_act_kernel) per half with the
+//   g-dot half's bias partials; each weight's gradient sum g-dot (x) a + g (x) a-dot is two
+//   wgrad_* launches into one buffer and one finish.
+// Reads a save = 1 workspace only; everything it writes but the caller's outputs is the scratch.
+namespace {
+
+__device__ __forceinline__ float branch(const __nv_bfloat16* hi, size_t i) {
+  return __bfloat162float(hi[i]) > 0.f ? 1.f : kSlope;
+}
+
+// x-dot[b,p,c] = sqrt2 lrelu'(x) sum_ci (w[c,ci] g) t[b,ci,p] -> pair [B,R,R,C]
+__global__ void __launch_bounds__(256)
+fromrgb_tangent_kernel(const float* __restrict__ t, int B, int nc, int RR, int C, const float* __restrict__ w,
+                       float g, const __nv_bfloat16* __restrict__ xhi, __nv_bfloat16* __restrict__ hi,
+                       __nv_bfloat16* __restrict__ lo) {
+  const size_t total = (size_t)B * RR * C;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int c = (int)(i % C);
+    const size_t q = i / C;
+    const int p = (int)(q % RR);
+    const size_t b = q / RR;
+    float s = 0.f;
+    for (int ci = 0; ci < nc; ++ci) s += (__ldg(w + c * nc + ci) * g) * __ldg(t + (b * nc + ci) * RR + p);
+    split_bf16(s * kSqrt2 * branch(xhi, i), hi[i], lo[i]);
+  }
+}
+
+// a-dot = gain lrelu'(a) raw -> pair
+__global__ void __launch_bounds__(256)
+act_tangent_kernel(const float* __restrict__ raw, const __nv_bfloat16* __restrict__ ahi, size_t n, float gain,
+                   __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+    split_bf16(__ldg(raw + i) * gain * branch(ahi, i), hi[i], lo[i]);
+}
+
+// y-dot = lrelu'(u1) u1-dot + skip-dot -> pair and / or fp32
+__global__ void __launch_bounds__(256)
+block_out_tangent_kernel(const float* __restrict__ raw1, const float* __restrict__ skip,
+                         const float* __restrict__ u1, size_t n, __nv_bfloat16* __restrict__ hi,
+                         __nv_bfloat16* __restrict__ lo, float* __restrict__ y_out) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const float y = __ldg(skip + i) + __ldg(raw1 + i) * dlrelu(__ldg(u1 + i));
+    if (hi != nullptr) split_bf16(y, hi[i], lo[i]);
+    if (y_out != nullptr) y_out[i] = y;
+  }
+}
+
+// The minibatch std's tangent: sd-dot[j] = mean over (p, c) of sum_k (x_k - m)(x-dot_k - m-dot) / (4 s),
+// in mbstd_kernel's order; xs-dot [B,16,513] = x-dot and sd-dot.  One block per group.
+__global__ void __launch_bounds__(256)
+mbstd_tangent_kernel(const float* __restrict__ x, const float* __restrict__ dx, int B, float* __restrict__ dxs) {
+  __shared__ float part[256];
+  const int G = B / kGroup, j = blockIdx.x;
+  float s = 0.f;
+  for (int e = threadIdx.x; e < 16 * kC4; e += 256) {
+    float v[kGroup], dv[kGroup], m = 0.f, dm = 0.f;
+    for (int k = 0; k < kGroup; ++k) {
+      const size_t o = (size_t)(k * G + j) * 16 * kC4 + e;
+      v[k] = __ldg(x + o);
+      dv[k] = __ldg(dx + o);
+      m += v[k];
+      dm += dv[k];
+    }
+    m /= (float)kGroup;
+    dm /= (float)kGroup;
+    float var = 0.f, dvar = 0.f;
+    for (int k = 0; k < kGroup; ++k) {
+      var += (v[k] - m) * (v[k] - m);
+      dvar += (v[k] - m) * (dv[k] - dm);
+    }
+    s += dvar / ((float)kGroup * sqrtf(var / (float)kGroup + 1e-8f));
+    for (int k = 0; k < kGroup; ++k) dxs[((size_t)(k * G + j) * 16 + e / kC4) * kCat + e % kC4] = dv[k];
+  }
+  part[threadIdx.x] = s;
+  __syncthreads();
+  for (int w = 128; w > 0; w >>= 1) {
+    if (threadIdx.x < w) part[threadIdx.x] += part[threadIdx.x + w];
+    __syncthreads();
+  }
+  if (threadIdx.x < kGroup * 16) {
+    const int k = threadIdx.x / 16, p = threadIdx.x % 16;
+    dxs[((size_t)(k * G + j) * 16 + p) * kCat + kC4] = part[0] / (float)(16 * kC4);
+  }
+}
+
+// The tangent of mbstd_backward_kernel's g_x along x-dot (g_xs does not move): with G_j as there,
+// g-dot_x = G_j / (16 * 512 * 4) ((x-dot_k - m-dot) / s - (x_k - m) s-dot / s^2),
+// s-dot = sum_k (x_k - m)(x-dot_k - m-dot) / (4 s).  Thread per (group, e).
+__global__ void mbstd_hvp_kernel(const float* __restrict__ gxs, const float* __restrict__ x,
+                                 const float* __restrict__ dx, int B, float* __restrict__ dgx) {
+  const int G = B / kGroup;
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t)G * 16 * kC4) return;
+  const int e = (int)(i % (16 * kC4)), j = (int)(i / (16 * kC4));
+  float gs = 0.f;
+  for (int k = 0; k < kGroup; ++k)
+    for (int p = 0; p < 16; ++p) gs += __ldg(gxs + ((size_t)(k * G + j) * 16 + p) * kCat + kC4);
+  float v[kGroup], dv[kGroup], m = 0.f, dm = 0.f;
+  for (int k = 0; k < kGroup; ++k) {
+    const size_t o = (size_t)(k * G + j) * 16 * kC4 + e;
+    v[k] = __ldg(x + o);
+    dv[k] = __ldg(dx + o);
+    m += v[k];
+    dm += dv[k];
+  }
+  m /= (float)kGroup;
+  dm /= (float)kGroup;
+  float var = 0.f, dvar = 0.f;
+  for (int k = 0; k < kGroup; ++k) {
+    var += (v[k] - m) * (v[k] - m);
+    dvar += (v[k] - m) * (dv[k] - dm);
+  }
+  const float s = sqrtf(var / (float)kGroup + 1e-8f);
+  const float ds = dvar / ((float)kGroup * s);
+  const float c = gs / (float)(16 * kC4) / (float)kGroup;
+  for (int k = 0; k < kGroup; ++k)
+    dgx[(size_t)(k * G + j) * 16 * kC4 + e] = c * ((dv[k] - dm) / s - (v[k] - m) * ds / (s * s));
+}
+
+__global__ void accumulate_kernel(const float* __restrict__ src, int n, float* __restrict__ dst) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) dst[i] += src[i];
+}
+
+Pair shifted(Pair p, size_t n) { return Pair{p.hi + n, p.lo + n}; }
+
+// The scratch: the tangent forward's activations per block, the stacked [g; g-dot] buffers of the
+// reverse walk, the weights in both orientations and the partial sums.
+struct HvpLayout {
+  Pair dx[kMaxBlocks], da[kMaxBlocks], dph[kMaxBlocks], dd[kMaxBlocks];  // as Layout's x, a, ph, d
+  Pair w0, w1, ws, t0, t1, ts;
+  float* raw0;                   // [B,r,r,C] conv0's raw tangent
+  float* raw1;
+  float* raws;
+  float* zero;                   // [512] zero bias
+  float *dx4, *dxs, *du4, *junk, *da4, *dhf, *dout, *jt;
+  float* g4[4];                  // as Layout's g4
+  float *gA, *gB;                // [2B,r,r,C] stacked
+  float* gf;                     // [2B,r+1,r+1,C]
+  float* gd;                     // [2B,h,h,C]
+  Pair gy, gu;                   // [2B,h,h,C']
+  Pair g0;                       // [2B,r,r,C]
+  float* part;
+  float* wtmp;
+  float* bpart;
+};
+
+void hvp_layout(const nfi_disc_params& P, Bump& b, HvpLayout& L) {
+  memset(&L, 0, sizeof(L));
+  const size_t B = P.batch;
+  const int nb = n_blocks(P.resolution), N = P.cmap_dim ? P.cmap_dim : 1;
+  size_t big = 0, bigo = 0, bigf = 0, bigw = 0, part = 0, bp = 0;
+  for (int i = 0; i < nb; ++i) {
+    const BlockShape s = shape(P.resolution, i);
+    const size_t rr = (size_t)s.r * s.r, hh = (size_t)s.h * s.h;
+    L.dx[i] = b.pair(B * rr * s.C);
+    L.da[i] = b.pair(B * rr * s.C);
+    L.dph[i] = b.pair(4 * B * (s.h + 1) * (s.h + 1) * s.C);
+    L.dd[i] = b.pair(B * hh * s.C);
+    big = big > B * rr * s.C ? big : B * rr * s.C;
+    bigo = bigo > B * hh * s.Co ? bigo : B * hh * s.Co;
+    const size_t f = B * (s.r + 1) * (s.r + 1) * s.C;
+    bigf = bigf > f ? bigf : f;
+    const size_t w = (size_t)9 * s.C * (s.C > s.Co ? s.C : s.Co);
+    bigw = bigw > w ? bigw : w;
+    const size_t p0 = synth::wgrad3x3_partial_floats(P.batch, s.r, s.r, s.C, s.C);
+    const size_t p1 = synth::wgrad_down3x3_partial_floats(P.batch, s.h, s.C, s.Co);
+    const size_t p2 = synth::wgrad1x1_partial_floats(P.batch, s.h, s.Co, s.C);
+    part = part > p0 ? part : p0;
+    part = part > p1 ? part : p1;
+    part = part > p2 ? part : p2;
+    const size_t c0 = chunks(B * rr) * s.C * (i == 0 ? 1 + P.img_channels : 1);
+    const size_t c1 = chunks(B * hh) * s.Co;
+    bp = bp > c0 ? bp : c0;
+    bp = bp > c1 ? bp : c1;
+  }
+  L.w0 = b.pair(bigw);
+  L.w1 = b.pair(bigw);
+  L.ws = b.pair(bigw / 9);
+  L.t0 = b.pair(bigw);
+  L.t1 = b.pair(bigw);
+  L.ts = b.pair(bigw / 9);
+  L.raw0 = b.take(big);
+  L.raw1 = b.take(bigo);
+  L.raws = b.take(bigo);
+  L.zero = b.take(kC4);
+  L.dx4 = b.take(B * kFcIn);
+  L.dxs = b.take(B * 16 * kCat);
+  L.du4 = b.take(B * kFcIn);
+  L.junk = b.take(B * kFcIn);
+  L.da4 = b.take(B * kFcIn);
+  L.dhf = b.take(B * kC4);
+  L.dout = b.take(B * N);
+  L.jt = b.take(B);
+  L.g4[0] = b.take(B * N);
+  L.g4[1] = b.take(B * kC4);
+  L.g4[2] = b.take(B * kFcIn);
+  L.g4[3] = b.take(B * 16 * kCat);
+  L.gA = b.take(2 * big);
+  L.gB = b.take(2 * big);
+  L.gf = b.take(2 * bigf);
+  L.gd = b.take(2 * bigo);
+  L.gy = b.pair(2 * bigo);
+  L.gu = b.pair(2 * bigo);
+  L.g0 = b.pair(2 * big);
+  L.part = b.take(part);
+  L.wtmp = b.take(bigw);
+  L.bpart = b.take(bp);
+}
+
+// g_w += gain (sum g-dot (x) a + g (x) a-dot): the two weight GEMMs into one buffer, then one finish
+template <class Wgrad>
+int two_term(float* g_w, size_t n, Wgrad&& wgrad, int cout, int cin, int taps, float gain, int transposed,
+             float* wtmp, cudaStream_t st, char* err, size_t err_len) {
+  if (g_w == nullptr) return 0;
+  NFI_LAUNCH_CHECK(cudaMemsetAsync(wtmp, 0, n * sizeof(float), st));
+  if (int rc = wgrad(0)) return rc;
+  if (int rc = wgrad(1)) return rc;
+  return finish(wtmp, cout, cin, taps, gain, transposed, g_w, st, err, err_len);
+}
+
+}  // namespace
+
+size_t hvp_scratch_bytes(const nfi_disc_params& P) {
+  char err[160];
+  if (check(P, err, sizeof(err))) return 0;
+  Bump b{nullptr, 0, 0};
+  HvpLayout H;
+  hvp_layout(P, b, H);
+  return b.off + 1024;
+}
+
+int backward_hvp(const nfi_disc_params& P, const nfi_disc_hvp& V, const nfi_disc_grads& G, cudaStream_t st,
+                 char* err, size_t err_len) {
+  if (P.save != 1) {
+    snprintf(err, err_len, "discriminator HVP: needs the workspace of a forward with save = 1");
+    return 1;
+  }
+  if (!V.g_logits || !V.t_img || !V.scratch) {
+    snprintf(err, err_len, "discriminator HVP: g_logits, t_img and scratch must be set");
+    return 1;
+  }
+  Layout L;
+  if (const int rc = setup(P, L, err, err_len)) return rc;
+  const size_t need = hvp_scratch_bytes(P);
+  if (V.scratch_bytes < need) {
+    snprintf(err, err_len, "discriminator HVP: scratch too small (%zu < %zu bytes)", V.scratch_bytes, need);
+    return 1;
+  }
+  HvpLayout H;
+  Bump sb = aligned_bump(V.scratch, V.scratch_bytes);
+  hvp_layout(P, sb, H);
+  const int B = P.batch, R = P.resolution, nc = P.img_channels, nb = n_blocks(R);
+  const int N = P.cmap_dim ? P.cmap_dim : 1;
+  const int C = channels(R), RR = R * R;
+  const float grgb = 1.f / sqrtf((float)nc);
+  NFI_LAUNCH_CHECK(cudaMemsetAsync(H.zero, 0, kC4 * sizeof(float), st));
+  // ---- the tangent forward along t, on the saved branches
+  fromrgb_tangent_kernel<<<flat_grid((size_t)B * RR * C), 256, 0, st>>>(V.t_img, B, nc, RR, C, P.fromrgb_w, grgb,
+                                                                       L.x[0].hi, H.dx[0].hi, H.dx[0].lo);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  for (int i = 0; i < nb; ++i) {
+    const BlockShape s = shape(R, i);
+    const size_t rr = (size_t)B * s.r * s.r, hh = (size_t)B * s.h * s.h;
+    if (int rc = prep(P.conv0_w[i], s.C, s.C, 9, conv_gain(s.C, 3), 0, H.w0, st, err, err_len)) return rc;
+    if (int rc = prep(P.conv1_w[i], s.Co, s.C, 9, conv_gain(s.C, 3), 0, H.w1, st, err, err_len)) return rc;
+    if (int rc = prep(P.skip_w[i], s.Co, s.C, 1, conv_gain(s.C, 1) * kSkipGain, 0, H.ws, st, err, err_len))
+      return rc;
+    if (int rc = synth::conv3x3(B, s.r, s.r, s.C, s.C, H.dx[i], H.w0, H.zero, H.raw0, Pair{nullptr, nullptr}, st,
+                                err, err_len))
+      return rc;
+    act_tangent_kernel<<<flat_grid(rr * s.C), 256, 0, st>>>(H.raw0, L.a[i].hi, rr * s.C, kSqrt2, H.da[i].hi,
+                                                            H.da[i].lo);
+    NFI_LAUNCH_CHECK(cudaGetLastError());
+    fir_phases_kernel<<<flat_grid((size_t)4 * B * (s.h + 1) * (s.h + 1) * s.C), 256, 0, st>>>(
+        H.da[i].hi, H.da[i].lo, B, s.r, s.C, H.dph[i].hi, H.dph[i].lo);
+    NFI_LAUNCH_CHECK(cudaGetLastError());
+    if (int rc = synth::conv_down3x3(B, s.h, s.C, s.Co, H.dph[i], H.w1, H.raw1, st, err, err_len)) return rc;
+    fir_down_kernel<<<flat_grid(hh * s.C), 256, 0, st>>>(H.dx[i].hi, H.dx[i].lo, B, s.r, s.C, H.dd[i].hi,
+                                                         H.dd[i].lo);
+    NFI_LAUNCH_CHECK(cudaGetLastError());
+    if (int rc = synth::conv1x1(B, s.h, s.C, s.Co, H.dd[i], H.ws, H.raws, st, err, err_len)) return rc;
+    const bool last = i == nb - 1;
+    block_out_tangent_kernel<<<flat_grid(hh * s.Co), 256, 0, st>>>(
+        H.raw1, H.raws, L.u1[i], hh * s.Co, last ? nullptr : H.dx[i + 1].hi, last ? nullptr : H.dx[i + 1].lo,
+        last ? H.dx4 : nullptr);
+    NFI_LAUNCH_CHECK(cudaGetLastError());
+  }
+  mbstd_tangent_kernel<<<B / kGroup, 256, 0, st>>>(L.x4, H.dx4, B, H.dxs);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  b4_conv_kernel<<<dim3((unsigned)B, kC4 / 64), 256, 0, st>>>(H.dxs, L.wt4, H.zero, H.du4, H.junk);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  act_backward_kernel<<<flat_grid((size_t)B * kFcIn), 256, 0, st>>>(H.du4, L.u4, (size_t)B * kFcIn, 1.f, H.da4);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  const unsigned bgrid = blocks(B, kLinImg);
+  const float g_out_w = 1.f / sqrtf((float)kC4), g_fc_w = 1.f / sqrtf((float)kFcIn);
+  linear_kernel<<<dim3(kC4, bgrid), 256, 0, st>>>(H.da4, P.fc_w, g_fc_w, H.zero, B, kFcIn, kC4, 0, nullptr, H.dhf);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  act_backward_kernel<<<flat_grid((size_t)B * kC4), 256, 0, st>>>(H.dhf, L.uf, (size_t)B * kC4, kSqrt2, H.dhf);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  linear_kernel<<<dim3((unsigned)N, bgrid), 256, 0, st>>>(H.dhf, P.out_w, g_out_w, H.zero, B, kC4, N, 0, nullptr,
+                                                          H.dout);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  if (V.grad_g_logits) {
+    logits_kernel<<<blocks(B, 128), 128, 0, st>>>(H.dout, P.cmap, B, P.cmap_dim, H.jt);
+    NFI_LAUNCH_CHECK(cudaGetLastError());
+    accumulate_kernel<<<blocks(B, 128), 128, 0, st>>>(H.jt, B, V.grad_g_logits);
+    NFI_LAUNCH_CHECK(cudaGetLastError());
+  }
+  // ---- the epilogue: g as in the first-order backward; its g-dot is zero (property 2)
+  float *g_out = H.g4[0], *g_hf = H.g4[1], *g_a4 = H.g4[2], *g_xs = H.g4[3];
+  logits_backward_kernel<<<blocks((size_t)B * N, 256), 256, 0, st>>>(V.g_logits, L.out, P.cmap, B, P.cmap_dim,
+                                                                     g_out, nullptr);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  if (V.grad_cmap && P.cmap_dim) {  // g_logits out-dot / sqrt N (g_out's write here is discarded)
+    logits_backward_kernel<<<blocks((size_t)B * N, 256), 256, 0, st>>>(V.g_logits, H.dout, P.cmap, B, P.cmap_dim,
+                                                                       H.junk, V.grad_cmap);
+    NFI_LAUNCH_CHECK(cudaGetLastError());
+  }
+  linear_dw_kernel<<<blocks((size_t)N * kC4, 256), 256, 0, st>>>(g_out, H.dhf, g_out_w, B, kC4, N, G.out_w, nullptr);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  linear_dx_kernel<<<blocks((size_t)B * kC4, 256), 256, 0, st>>>(g_out, P.out_w, g_out_w, B, kC4, N, g_hf);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  act_backward_kernel<<<flat_grid((size_t)B * kC4), 256, 0, st>>>(g_hf, L.uf, (size_t)B * kC4, kSqrt2, g_hf);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  linear_dw_kernel<<<blocks((size_t)kC4 * kFcIn, 256), 256, 0, st>>>(g_hf, H.da4, g_fc_w, B, kFcIn, kC4, G.fc_w,
+                                                                     nullptr);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  linear_dx_kernel<<<blocks((size_t)B * kFcIn, 256), 256, 0, st>>>(g_hf, P.fc_w, g_fc_w, B, kFcIn, kC4, g_a4);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  act_backward_kernel<<<flat_grid((size_t)B * kFcIn), 256, 0, st>>>(g_a4, L.u4, (size_t)B * kFcIn, kSqrt2, g_a4);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  const float g4w = conv_gain(kCat, 3);
+  if (G.b4_conv_w) {
+    b4_conv_dw_kernel<<<blocks((size_t)kC4 * kCat * 9, 256), 256, 0, st>>>(g_a4, H.dxs, g4w, B, G.b4_conv_w,
+                                                                          nullptr);
+    NFI_LAUNCH_CHECK(cudaGetLastError());
+  }
+  b4_conv_dx_kernel<<<dim3(blocks(kCat, 256), (unsigned)B), 256, 0, st>>>(g_a4, P.b4_conv_w, g4w, g_xs);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  // [g; g-dot] of the last block's output, stacked over 2B images
+  float* gy = H.gA;
+  const size_t n4 = (size_t)B * kFcIn;
+  mbstd_backward_kernel<<<blocks((size_t)B / kGroup * kFcIn, 256), 256, 0, st>>>(g_xs, L.x4, B, gy);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  mbstd_hvp_kernel<<<blocks((size_t)B / kGroup * kFcIn, 256), 256, 0, st>>>(g_xs, L.x4, H.dx4, B, gy + n4);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  // ---- the blocks, last to first
+  for (int i = nb - 1; i >= 0; --i) {
+    const BlockShape s = shape(R, i);
+    const int M = B * s.h * s.h, Mr = B * s.r * s.r;
+    const size_t mo = (size_t)M * s.Co, mr = (size_t)Mr * s.C, mf = (size_t)B * (s.r + 1) * (s.r + 1) * s.C;
+    float* gx = gy == H.gA ? H.gB : H.gA;
+    for (int half = 0; half < 2; ++half) {
+      out_backward_kernel<<<(unsigned)chunks(M), 256, 0, st>>>(gy + half * mo, L.u1[i], M, s.Co, H.gy.hi + half * mo,
+                                                               H.gy.lo + half * mo, H.gu.hi + half * mo,
+                                                               H.gu.lo + half * mo, H.bpart);
+      NFI_LAUNCH_CHECK(cudaGetLastError());
+    }
+    if (int rc = bias_reduce(M, s.Co, H.bpart, G.conv1_b[i], st, err, err_len)) return rc;
+    const Pair gu = H.gu, dgu = shifted(H.gu, mo), gyp = H.gy, dgy = shifted(H.gy, mo);
+    if (int rc = two_term(G.conv1_w[i], (size_t)9 * s.C * s.Co, [&](int k) {
+          return synth::wgrad_down3x3(B, s.h, s.C, s.Co, k ? H.dph[i] : L.ph[i], k ? gu : dgu, P.conv1_w[i],
+                                      H.part, H.wtmp, st, err, err_len);
+        }, s.Co, s.C, 9, conv_gain(s.C, 3), 1, H.wtmp, st, err, err_len))
+      return rc;
+    if (int rc = two_term(G.skip_w[i], (size_t)s.C * s.Co, [&](int k) {
+          return synth::wgrad1x1(B, s.h, s.Co, s.C, k ? gyp : dgy, k ? H.dd[i] : L.d[i], P.skip_w[i], H.part,
+                                 H.wtmp, st, err, err_len);
+        }, s.Co, s.C, 1, conv_gain(s.C, 1) * kSkipGain, 0, H.wtmp, st, err, err_len))
+      return rc;
+    if (int rc = prep(P.conv1_w[i], s.Co, s.C, 9, conv_gain(s.C, 3), 1, H.t1, st, err, err_len)) return rc;
+    if (int rc = synth::conv_up3x3(2 * B, s.h, s.Co, s.C, H.gu, H.t1, H.gf, st, err, err_len)) return rc;
+    for (int half = 0; half < 2; ++half) {
+      fir_up_act_kernel<<<(unsigned)chunks(Mr), 256, 0, st>>>(H.gf + half * mf, L.a[i].hi, B, s.r, s.C,
+                                                              H.g0.hi + half * mr, H.g0.lo + half * mr, H.bpart);
+      NFI_LAUNCH_CHECK(cudaGetLastError());
+    }
+    if (int rc = bias_reduce(Mr, s.C, H.bpart, G.conv0_b[i], st, err, err_len)) return rc;
+    const Pair g0 = H.g0, dg0 = shifted(H.g0, mr);
+    if (int rc = two_term(G.conv0_w[i], (size_t)9 * s.C * s.C, [&](int k) {
+          return synth::wgrad3x3(B, s.r, s.r, s.C, s.C, s.C, k ? g0 : dg0, k ? H.dx[i] : L.x[i], P.conv0_w[i],
+                                 H.part, H.wtmp, st, err, err_len);
+        }, s.C, s.C, 9, conv_gain(s.C, 3), 0, H.wtmp, st, err, err_len))
+      return rc;
+    if (int rc = prep(P.conv0_w[i], s.C, s.C, 9, conv_gain(s.C, 3), 1, H.t0, st, err, err_len)) return rc;
+    if (int rc = synth::conv3x3_adjoint(2 * B, s.r, s.r, s.C, s.C, H.g0, H.t0, gx, st, err, err_len)) return rc;
+    if (int rc = prep(P.skip_w[i], s.Co, s.C, 1, conv_gain(s.C, 1) * kSkipGain, 1, H.ts, st, err, err_len))
+      return rc;
+    if (int rc = synth::conv1x1(2 * B, s.h, s.Co, s.C, H.gy, H.ts, H.gd, st, err, err_len)) return rc;
+    fir_down_adjoint_kernel<<<flat_grid((size_t)2 * mr), 256, 0, st>>>(H.gd, 2 * B, s.r, s.C, gx);
+    NFI_LAUNCH_CHECK(cudaGetLastError());
+    gy = gx;
+  }
+  // ---- fromrgb: gy holds [g; g-dot] of its output
+  const size_t m0 = (size_t)B * RR * C;
+  if (G.fromrgb_w || G.fromrgb_b) {
+    const int n = (int)chunks((size_t)B * RR);
+    fromrgb_backward_kernel<<<n, 256, 0, st>>>(gy + m0, L.x[0].hi, P.img, B, nc, RR, C, H.bpart);
+    NFI_LAUNCH_CHECK(cudaGetLastError());
+    fromrgb_reduce_kernel<<<blocks((size_t)C * (1 + nc), 256), 256, 0, st>>>(H.bpart, n, C, nc, grgb, G.fromrgb_w,
+                                                                             G.fromrgb_b);
+    NFI_LAUNCH_CHECK(cudaGetLastError());
+    if (G.fromrgb_w) {
+      fromrgb_backward_kernel<<<n, 256, 0, st>>>(gy, L.x[0].hi, V.t_img, B, nc, RR, C, H.bpart);
+      NFI_LAUNCH_CHECK(cudaGetLastError());
+      fromrgb_reduce_kernel<<<blocks((size_t)C * (1 + nc), 256), 256, 0, st>>>(H.bpart, n, C, nc, grgb,
+                                                                               G.fromrgb_w, nullptr);
+      NFI_LAUNCH_CHECK(cudaGetLastError());
+    }
+  }
+  if (V.grad_img) {
+    fromrgb_gimg_kernel<<<flat_grid((size_t)B * RR * 32), 256, 0, st>>>(gy + m0, L.x[0].hi, P.fromrgb_w, grgb, B, nc,
+                                                                        RR, C, V.grad_img);
+    NFI_LAUNCH_CHECK(cudaGetLastError());
+  }
+  return 0;
+}
+
 }  // namespace disc
 }  // namespace nfi

@@ -5,6 +5,7 @@
 #include <stddef.h>
 
 #include "nfi_disc.h"
+#include "nfi_disc_r1.h"
 
 namespace nfi {
 namespace disc {
@@ -14,5 +15,8 @@ int backward(const nfi_disc_params& p, const float* g_logits, float* grad_img, f
              const nfi_disc_grads& g, cudaStream_t st, char* err, size_t err_len);
 int saved_preactivation(const nfi_disc_params& p, int block, int which, float* out, cudaStream_t st, char* err,
                         size_t err_len);
+size_t hvp_scratch_bytes(const nfi_disc_params& p);
+int backward_hvp(const nfi_disc_params& p, const nfi_disc_hvp& h, const nfi_disc_grads& g, cudaStream_t st,
+                 char* err, size_t err_len);
 }  // namespace disc
 }  // namespace nfi

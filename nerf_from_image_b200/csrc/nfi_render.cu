@@ -551,6 +551,17 @@ int nfi_disc_saved_preactivation(const nfi_disc_params* params, int32_t block, i
   return nfi::disc::saved_preactivation(*params, block, which, out, (cudaStream_t)stream, g_err, sizeof(g_err));
 }
 
+size_t nfi_disc_r1_scratch_bytes(const nfi_disc_params* params) {
+  if (params == nullptr) return 0;
+  return nfi::disc::hvp_scratch_bytes(*params);
+}
+
+int nfi_disc_backward_hvp(const nfi_disc_params* params, const nfi_disc_hvp* hvp, const nfi_disc_grads* grads,
+                          void* stream) {
+  if (params == nullptr || hvp == nullptr || grads == nullptr) return fail("params / hvp / grads is NULL");
+  return nfi::disc::backward_hvp(*params, *hvp, *grads, (cudaStream_t)stream, g_err, sizeof(g_err));
+}
+
 size_t nfi_synthesis_workspace_bytes(const nfi_synth_params* params) {
   if (params == nullptr) return 0;
   return nfi::synth::workspace_bytes(*params);

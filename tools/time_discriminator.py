@@ -3,14 +3,17 @@ against the eager reference module with TF32 off, at B = 32, 128^2, nc = 4, cond
 
   (a) the generator step's call: D frozen, forward and backward to the image;
   (b) one discriminator step without R1: D(real) and D(fake), backward to every parameter;
-  (c) (b) with R1's real call (image gradient with create_graph), which runs the module in both arms;
+  (c) (b) with R1's real call (image gradient with create_graph), which runs the module in the fused
+      and eager arms; a third arm, fused_r1, runs it on the kernels too
+      (enable_fused_discriminator(D, r1=True): nfi_disc_backward_hvp for the penalty's backward);
   (d) a whole G/D iteration pair: the generator step through render() (fused synthesis, heads on,
       128^2, 64 + 64 samples) with D(rgb + alpha) in its loss, then a D step on real images and a
       no-grad render's fakes; with the fused D, the eager D, and no D at all (the generator step's
       loss without the discriminator term, no D step) -- the discriminator's share of the pair is
       1 - (no D) / (with D);
-  (e) (d) with R1 on that D step.
-With --profile, one fused call of (a) and of (b) under torch.profiler: CUDA time per kernel.
+  (e) (d) with R1 on that D step, with the fused_r1 arm as in (c).
+With --profile, one fused call of (a) and of (b), and one R1 call of the fused_r1 arm (its create_graph
+backward, the HVP and the plain backward), under torch.profiler: CUDA time per kernel.
 
 CUDA events around each step, the arms alternated, the median of the rounds; peak memory above
 what was allocated before the step ((a) - (c)).  One JSON line for (a) - (c), one for (d), (e).  Needs the reference discriminator staged
@@ -62,6 +65,7 @@ def main():
     B, R, nc = args.batch, args.resolution, 4
     eager = DC.seed_module(mods[0].Discriminator(R, nc, DC.DATASET_CONFIG, conditional_pose=True), 1).to(dev)
     fused = enable_fused_discriminator(copy.deepcopy(eager))
+    fused_r1 = enable_fused_discriminator(copy.deepcopy(eager), r1=True)
     pose, focal = (t.to(dev) for t in DC.poses(B, 2))
     real, fake = DC.image(B, nc, R, 3).to(dev), DC.image(B, nc, R, 4).to(dev)
     crit = lambda x, t: F.softplus(-x if t else x).mean()
@@ -83,16 +87,24 @@ def main():
         (crit(out, True) + 2.5 * pen).backward()
         crit(D(fake, 1, pose, None, focal), False).backward()
 
+    def r1_call(D):
+        D.requires_grad_(True)
+        x = real.clone().requires_grad_()
+        out = D(x, 1, pose, None, focal)
+        g, = torch.autograd.grad(out.sum(), x, create_graph=True)
+        (crit(out, True) + 2.5 * g.reshape(B, -1).square().sum(dim=1).mean()).backward()
+
     rows = {'a_g_call': g_call, 'b_d_step': lambda D: d_step(D, False), 'c_d_step_r1': lambda D: d_step(D, True)}
     res = {}
     for name, fn in rows.items():
-        times = {'fused': [], 'eager': []}
+        arms = (('fused', fused), ('eager', eager)) + ((('fused_r1', fused_r1),) if name == 'c_d_step_r1' else ())
+        times = {a: [] for a, _ in arms}
         peak = {}
-        for arm, D in (('fused', fused), ('eager', eager)):   # warm-up
+        for arm, D in arms:   # warm-up
             fn(D)
         torch.cuda.synchronize()
         for _ in range(args.rounds):
-            for arm, D in (('fused', fused), ('eager', eager)):
+            for arm, D in arms:
                 torch.cuda.synchronize()
                 base = torch.cuda.memory_allocated()
                 torch.cuda.reset_peak_memory_stats()
@@ -109,9 +121,11 @@ def main():
            'rows': res}
     if args.profile:
         out['kernels_ms'] = {name: _profile(lambda: fn(fused)) for name, fn in list(rows.items())[:2]}
+        out['kernels_ms']['r1_call'] = _profile(lambda: r1_call(fused_r1))
     print(json.dumps(out), flush=True)
     print(json.dumps({'gpu': _gpu_info(), 'batch': B, 'resolution': R, 'img_channels': nc,
-                      'rows': _iteration_pairs(fused, eager, real, pose, focal, B, max(3, args.rounds // 2))}))
+                      'rows': _iteration_pairs(fused, eager, fused_r1, real, pose, focal, B,
+                                               max(3, args.rounds // 2))}))
 
 
 def _profile(fn):
@@ -130,7 +144,7 @@ def _profile(fn):
     return dict(sorted(per.items(), key=lambda kv: -kv[1])[:25])
 
 
-def _iteration_pairs(fused, eager, real, pose, focal, B, rounds):
+def _iteration_pairs(fused, eager, fused_r1, real, pose, focal, B, rounds):
     """(d) and (e): G/D iteration pairs through render() with each arm's discriminator."""
     import types
     from fixtures import synthetic
@@ -182,7 +196,7 @@ def _iteration_pairs(fused, eager, real, pose, focal, B, rounds):
 
     res = {}
     for name, r1 in (('d_iteration_pair', False), ('e_iteration_pair_r1', True)):
-        arms = (('fused', fused), ('eager', eager), ('no_d', None))
+        arms = (('fused', fused), ('eager', eager)) + ((('fused_r1', fused_r1),) if r1 else ()) + (('no_d', None),)
         times = {a: [] for a, _ in arms}
         for _, D in arms:
             pair(D, r1)
@@ -196,7 +210,7 @@ def _iteration_pairs(fused, eager, real, pose, focal, B, rounds):
                 torch.cuda.synchronize()
                 times[a].append(e0.elapsed_time(e1))
         row = {a: {'median_ms': statistics.median(t), 'min_ms': min(t), 'max_ms': max(t)} for a, t in times.items()}
-        for a in ('fused', 'eager'):
+        for a in [a for a in row if a != 'no_d']:
             row[a]['d_share'] = 1 - row['no_d']['median_ms'] / row[a]['median_ms']
         res[name] = row
     return res
