@@ -14,26 +14,30 @@
 //   4x4, in fp32 on the CUDA cores: mbstd_kernel (concat -> [B,16,513]), b4_conv_kernel (-> u, a in
 //   flatten order [B,512*16]), linear_kernel (fc with lrelu sqrt2; out), logits_kernel
 //
-// Backward (every sum over positions or images in a fixed order; no atomics):
-//   4x4: logits_backward_kernel, linear_dx / linear_dw kernels, b4_conv_dx / _dw kernels,
-//   mbstd_backward_kernel -> g of the last block's output, fp32 [B,4,4,512]
-//   per block, from the last to the first:
+// Backward (every sum over positions or images in a fixed order; no atomics), one reverse walk that
+// the R1 double backward below also runs, over a stacked [g; g-dot]:
+//   epilogue_backward, 4x4: logits_backward_kernel, linear_dx / linear_dw kernels, b4_conv_dx / _dw
+//   kernels, mbstd_backward_kernel -> g of the last block's output, fp32 [B,4,4,512]
+//   reverse_walk, per block from the last to the first, over the walk's 1 or 2 copies of B images:
 //     out_backward_kernel  g_y -> pairs of g_y (the skip's output gradient) and g_u1 = g_y lrelu'(u1)
-//                          (conv1's), with per-chunk sums of g_u1 for the bias
+//                          (conv1's), with per-chunk sums of g_u1 for the bias; once per copy
 //     wgrad_tc_kernel      conv1 (transposed, against the phases), skip (against the downsampled x)
 //     conv_tc_kernel RAW   conv1's data gradient: the stride-2 transposed conv (conv_up3x3) ->
 //                          [B,r+1,r+1,C]; skip's (conv1x1 with transposed weights) -> [B,h,h,C]
-//     fir_up_act_kernel    the adjoint of filter2d^T, times sqrt2 lrelu'(conv0) -> pair, bias sums
+//     fir_up_act_kernel    the adjoint of filter2d^T, times sqrt2 lrelu'(conv0) -> pair, bias sums;
+//                          once per copy
 //     wgrad_tc_kernel      conv0;  conv_tc_kernel RAW: its data gradient (flipped taps) -> g_x
 //     fir_down_adjoint_kernel  g_x += downsample2d^T(skip's data gradient)
-//   fromrgb_backward_kernel / fromrgb_gimg_kernel: the 1x1 in fp32 (weight, bias, image gradients)
-// Weight gradients land in a scratch buffer and wgrad_finish_kernel adds gain x it (transposed for
-// conv1) to the caller's.
+//   then fromrgb_backward_kernel / fromrgb_gimg_kernel: the 1x1 in fp32 (weight, bias, image gradients)
+// Each weight gradient sums its terms (one here, two in R1) in a scratch buffer and
+// wgrad_finish_kernel adds gain x it (transposed for conv1) to the caller's.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdio.h>
 #include <string.h>
+
+#include <algorithm>
 
 #include "nfi_disc.h"
 #include "nfi_disc_launch.h"
@@ -60,6 +64,51 @@ __device__ __forceinline__ float lrelu(float x) { return x > 0.f ? x : kSlope * 
 __device__ __forceinline__ float dlrelu(float u) { return u > 0.f ? 1.f : kSlope; }
 __device__ __forceinline__ float pair_at(const __nv_bfloat16* hi, const __nv_bfloat16* lo, size_t i) {
   return __bfloat162float(hi[i]) + __bfloat162float(lo[i]);
+}
+// lrelu' on the branch a saved activation pair took (its hi half has the sign)
+__device__ __forceinline__ float branch(const __nv_bfloat16* hi, size_t i) {
+  return __bfloat162float(hi[i]) > 0.f ? 1.f : kSlope;
+}
+
+// Minibatch-std group j (images j + k B/4, k < 4) at element e of [16,512]: the values v, their
+// mean m, var = sum_k (v_k - m)^2 and s = sqrt(var / 4 + 1e-8); along a tangent dx also its values
+// dv, their mean dm and dvar = sum_k (v_k - m)(dv_k - dm).
+struct Group {
+  float v[kGroup], m, var, s;
+  float dv[kGroup], dm, dvar;
+};
+__device__ __forceinline__ Group group(const float* __restrict__ x, int G, int j, int e) {
+  Group q;
+  q.m = 0.f;
+  for (int k = 0; k < kGroup; ++k) {
+    q.v[k] = __ldg(x + (size_t)(k * G + j) * 16 * kC4 + e);
+    q.m += q.v[k];
+  }
+  q.m /= (float)kGroup;
+  q.var = 0.f;
+  for (int k = 0; k < kGroup; ++k) q.var += (q.v[k] - q.m) * (q.v[k] - q.m);
+  q.s = sqrtf(q.var / (float)kGroup + 1e-8f);
+  return q;
+}
+__device__ __forceinline__ Group group(const float* __restrict__ x, const float* __restrict__ dx, int G, int j,
+                                       int e) {
+  Group q = group(x, G, j, e);
+  q.dm = 0.f;
+  for (int k = 0; k < kGroup; ++k) {
+    q.dv[k] = __ldg(dx + (size_t)(k * G + j) * 16 * kC4 + e);
+    q.dm += q.dv[k];
+  }
+  q.dm /= (float)kGroup;
+  q.dvar = 0.f;
+  for (int k = 0; k < kGroup; ++k) q.dvar += (q.v[k] - q.m) * (q.dv[k] - q.dm);
+  return q;
+}
+// G_j: the std channel's gradient in g_xs [B,16,513], summed over group j's images and positions
+__device__ __forceinline__ float std_grad_sum(const float* __restrict__ gxs, int G, int j) {
+  float gs = 0.f;
+  for (int k = 0; k < kGroup; ++k)
+    for (int p = 0; p < 16; ++p) gs += __ldg(gxs + ((size_t)(k * G + j) * 16 + p) * kCat + kC4);
+  return gs;
 }
 
 int channels(int r) { return r >= 64 ? 32768 / r > 512 ? 512 : 32768 / r : 512; }
@@ -191,16 +240,9 @@ mbstd_kernel(const float* __restrict__ x, int B, float* __restrict__ xs, float* 
   const int G = B / kGroup, j = blockIdx.x;
   float s = 0.f;
   for (int e = threadIdx.x; e < 16 * kC4; e += 256) {
-    float v[kGroup], m = 0.f;
-    for (int k = 0; k < kGroup; ++k) {
-      v[k] = __ldg(x + (size_t)(k * G + j) * 16 * kC4 + e);
-      m += v[k];
-    }
-    m /= (float)kGroup;
-    float var = 0.f;
-    for (int k = 0; k < kGroup; ++k) var += (v[k] - m) * (v[k] - m);
-    s += sqrtf(var / (float)kGroup + 1e-8f);
-    for (int k = 0; k < kGroup; ++k) xs[((size_t)(k * G + j) * 16 + e / kC4) * kCat + e % kC4] = v[k];
+    const Group q = group(x, G, j, e);
+    s += q.s;
+    for (int k = 0; k < kGroup; ++k) xs[((size_t)(k * G + j) * 16 + e / kC4) * kCat + e % kC4] = q.v[k];
   }
   part[threadIdx.x] = s;
   __syncthreads();
@@ -405,22 +447,12 @@ __global__ void mbstd_backward_kernel(const float* __restrict__ gxs, const float
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (size_t)G * 16 * kC4) return;
   const int e = (int)(i % (16 * kC4)), j = (int)(i / (16 * kC4));
-  float gs = 0.f;
-  for (int k = 0; k < kGroup; ++k)
-    for (int p = 0; p < 16; ++p) gs += __ldg(gxs + ((size_t)(k * G + j) * 16 + p) * kCat + kC4);
-  float v[kGroup], m = 0.f;
-  for (int k = 0; k < kGroup; ++k) {
-    v[k] = __ldg(x + (size_t)(k * G + j) * 16 * kC4 + e);
-    m += v[k];
-  }
-  m /= (float)kGroup;
-  float var = 0.f;
-  for (int k = 0; k < kGroup; ++k) var += (v[k] - m) * (v[k] - m);
-  const float s = sqrtf(var / (float)kGroup + 1e-8f);
-  const float c = gs / (float)(16 * kC4) / ((float)kGroup * s);
+  const float gs = std_grad_sum(gxs, G, j);
+  const Group q = group(x, G, j, e);
+  const float c = gs / (float)(16 * kC4) / ((float)kGroup * q.s);
   for (int k = 0; k < kGroup; ++k) {
     const size_t b = (size_t)(k * G + j);
-    gx[b * 16 * kC4 + e] = __ldg(gxs + (b * 16 + e / kC4) * kCat + e % kC4) + c * (v[k] - m);
+    gx[b * 16 * kC4 + e] = __ldg(gxs + (b * 16 + e / kC4) * kCat + e % kC4) + c * (q.v[k] - q.m);
   }
 }
 
@@ -468,7 +500,7 @@ fir_up_act_kernel(const float* __restrict__ gf, const __nv_bfloat16* __restrict_
         acc += fir(u) * ar;
       }
       const size_t o = (size_t)q * C + c;
-      const float g = acc * kSqrt2 * (__bfloat162float(ahi[o]) > 0.f ? 1.f : kSlope);
+      const float g = acc * kSqrt2 * branch(ahi, o);
       split_bf16(g, hi[o], lo[o]);
       s += g;
     }
@@ -517,7 +549,7 @@ fromrgb_backward_kernel(const float* __restrict__ gx, const __nv_bfloat16* __res
     float s[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
     for (int q = r0; q < r1; ++q) {
       const size_t o = (size_t)q * C + c;
-      const float g = __ldg(gx + o) * kSqrt2 * (__bfloat162float(xhi[o]) > 0.f ? 1.f : kSlope);
+      const float g = __ldg(gx + o) * kSqrt2 * branch(xhi, o);
       const int b = q / RR, p = q % RR;
       s[0] += g;
       for (int ci = 0; ci < nc; ++ci) s[1 + ci] += g * __ldg(img + ((size_t)b * nc + ci) * RR + p);
@@ -552,7 +584,7 @@ fromrgb_gimg_kernel(const float* __restrict__ gx, const __nv_bfloat16* __restric
     float s[4] = {0.f, 0.f, 0.f, 0.f};
     for (int c = lane; c < C; c += 32) {
       const size_t o = q * C + c;
-      const float gu = __ldg(gx + o) * kSqrt2 * (__bfloat162float(xhi[o]) > 0.f ? 1.f : kSlope);
+      const float gu = __ldg(gx + o) * kSqrt2 * branch(xhi, o);
       for (int ci = 0; ci < nc; ++ci) s[ci] += (__ldg(w + c * nc + ci) * g) * gu;
     }
 #pragma unroll
@@ -604,6 +636,73 @@ static BlockShape shape(int R, int i) {
   return s;
 }
 
+static size_t chunks(size_t M) { return (M + kRows - 1) / kRows; }
+
+// The largest per-block sizes (floats or pair elements), which the buffers reused block by block take
+struct Sizes {
+  size_t big;   // [B,r,r,C]
+  size_t bigo;  // [B,h,h,C']
+  size_t bigf;  // [B,r+1,r+1,C]
+  size_t bigw;  // a 3x3 weight, 9 C max(C, C')
+  size_t part;  // weight-GEMM partials
+  size_t bp;    // partial sums of the bias and fromrgb reductions
+};
+
+static Sizes sizes(const nfi_disc_params& P) {
+  Sizes z = {};
+  const size_t B = P.batch;
+  for (int i = 0; i < n_blocks(P.resolution); ++i) {
+    const BlockShape s = shape(P.resolution, i);
+    const size_t rr = (size_t)s.r * s.r, hh = (size_t)s.h * s.h;
+    z.big = std::max(z.big, B * rr * s.C);
+    z.bigo = std::max(z.bigo, B * hh * s.Co);
+    z.bigf = std::max(z.bigf, B * (s.r + 1) * (s.r + 1) * s.C);
+    z.bigw = std::max(z.bigw, (size_t)9 * s.C * std::max(s.C, s.Co));
+    z.part = std::max({z.part, synth::wgrad3x3_partial_floats(P.batch, s.r, s.r, s.C, s.C),
+                       synth::wgrad_down3x3_partial_floats(P.batch, s.h, s.C, s.Co),
+                       synth::wgrad1x1_partial_floats(P.batch, s.h, s.Co, s.C)});
+    z.bp = std::max({z.bp, chunks(B * rr) * s.C * (i == 0 ? 1 + P.img_channels : 1), chunks(B * hh) * s.Co});
+  }
+  return z;
+}
+
+// The reverse walk's buffers, for `copies` stacked copies of the B images: the first-order backward
+// walks g (one copy), the HVP [g; g-dot] (two).
+struct Reverse {
+  Pair t0, t1, ts;       // transposed weights
+  float* gA;             // fp32 gradients, largest [copies B,r,r,C]
+  float* gB;
+  float* gf;             // [copies B,r+1,r+1,C]
+  float* gd;             // [copies B,h,h,C]
+  Pair gy, gu;           // [copies B,h,h,C'] pairs
+  Pair g0;               // [copies B,r,r,C] pair
+  float* part;           // weight-GEMM partials
+  float* wtmp;           // weight gradient before its gain
+  float* bpart;          // partial sums
+  float* g4[4];          // 4x4 epilogue gradients (g only): [B,N], [B,512], [B,8192], [B,16,513]
+};
+
+static void reverse_layout(const nfi_disc_params& P, const Sizes& z, int copies, Bump& b, Reverse& V) {
+  const size_t B = P.batch, n = copies, N = P.cmap_dim ? P.cmap_dim : 1;
+  V.t0 = b.pair(z.bigw);
+  V.t1 = b.pair(z.bigw);
+  V.ts = b.pair(z.bigw / 9);
+  V.gA = b.take(n * z.big);
+  V.gB = b.take(n * z.big);
+  V.gf = b.take(n * z.bigf);
+  V.gd = b.take(n * z.bigo);
+  V.gy = b.pair(n * z.bigo);
+  V.gu = b.pair(n * z.bigo);
+  V.g0 = b.pair(n * z.big);
+  V.part = b.take(z.part);
+  V.wtmp = b.take(z.bigw);
+  V.bpart = b.take(z.bp);
+  V.g4[0] = b.take(B * N);
+  V.g4[1] = b.take(B * kC4);
+  V.g4[2] = b.take(B * kFcIn);
+  V.g4[3] = b.take(B * 16 * kCat);
+}
+
 // The workspace: a deterministic walk, so the backward finds what a saved forward left.
 struct Layout {
   Pair x[kMaxBlocks];    // block input [B,r,r,C] (x[0]: fromrgb's output)
@@ -623,28 +722,14 @@ struct Layout {
   float* uf;             // [B,512]
   float* hf;
   float* out;            // [B,N]
-  // backward (save only)
-  Pair t0, t1, ts;       // transposed weights
-  float* gA;             // fp32 gradients, largest [B,r,r,C]
-  float* gB;
-  float* gf;             // [B,r+1,r+1,C]
-  float* gd;             // [B,h,h,C]
-  Pair gy, gu;           // [B,h,h,C'] pairs
-  Pair g0;               // [B,r,r,C] pair
-  float* part;           // weight-GEMM partials
-  float* wtmp;           // weight gradient before its gain
-  float* bpart;          // partial sums
-  float* g4[4];          // 4x4 epilogue gradients: [B,N], [B,512], [B,8192], [B,16,513]
+  Reverse rev;           // the first-order backward's (save only)
 };
-
-static size_t chunks(size_t M) { return (M + kRows - 1) / kRows; }
 
 static void layout(const nfi_disc_params& P, Bump& b, Layout& L) {
   memset(&L, 0, sizeof(L));
-  const size_t B = P.batch;
-  const int nb = n_blocks(P.resolution), N = P.cmap_dim ? P.cmap_dim : 1;
-  size_t big = 0, bigo = 0, bigf = 0, bigw = 0, part = 0, bp = 0;
-  for (int i = 0; i < nb; ++i) {
+  const Sizes z = sizes(P);
+  const size_t B = P.batch, N = P.cmap_dim ? P.cmap_dim : 1;
+  for (int i = 0; i < n_blocks(P.resolution); ++i) {
     const BlockShape s = shape(P.resolution, i);
     const size_t rr = (size_t)s.r * s.r, hh = (size_t)s.h * s.h;
     L.x[i] = b.pair(B * rr * s.C);
@@ -652,28 +737,12 @@ static void layout(const nfi_disc_params& P, Bump& b, Layout& L) {
     L.ph[i] = b.pair(4 * B * (s.h + 1) * (s.h + 1) * s.C);
     L.d[i] = b.pair(B * hh * s.C);
     L.u1[i] = b.take(B * hh * s.Co);
-    big = big > B * rr * s.C ? big : B * rr * s.C;
-    bigo = bigo > B * hh * s.Co ? bigo : B * hh * s.Co;
-    const size_t f = B * (s.r + 1) * (s.r + 1) * s.C;
-    bigf = bigf > f ? bigf : f;
-    const size_t w = (size_t)9 * s.C * (s.C > s.Co ? s.C : s.Co);
-    bigw = bigw > w ? bigw : w;
-    const size_t p0 = synth::wgrad3x3_partial_floats(P.batch, s.r, s.r, s.C, s.C);
-    const size_t p1 = synth::wgrad_down3x3_partial_floats(P.batch, s.h, s.C, s.Co);
-    const size_t p2 = synth::wgrad1x1_partial_floats(P.batch, s.h, s.Co, s.C);
-    part = part > p0 ? part : p0;
-    part = part > p1 ? part : p1;
-    part = part > p2 ? part : p2;
-    const size_t c0 = chunks(B * rr) * s.C * (i == 0 ? 1 + P.img_channels : 1);
-    const size_t c1 = chunks(B * hh) * s.Co;
-    bp = bp > c0 ? bp : c0;
-    bp = bp > c1 ? bp : c1;
   }
-  L.w0 = b.pair(bigw);
-  L.w1 = b.pair(bigw);
-  L.ws = b.pair(bigw / 9);
-  L.raw1 = b.take(bigo);
-  L.raws = b.take(bigo);
+  L.w0 = b.pair(z.bigw);
+  L.w1 = b.pair(z.bigw);
+  L.ws = b.pair(z.bigw / 9);
+  L.raw1 = b.take(z.bigo);
+  L.raws = b.take(z.bigo);
   L.x4 = b.take(B * kFcIn);
   L.xs = b.take(B * 16 * kCat);
   L.sd = b.take(B / kGroup);
@@ -683,25 +752,7 @@ static void layout(const nfi_disc_params& P, Bump& b, Layout& L) {
   L.uf = b.take(B * kC4);
   L.hf = b.take(B * kC4);
   L.out = b.take(B * N);
-  if (P.save) {
-    L.t0 = b.pair(bigw);
-    L.t1 = b.pair(bigw);
-    L.ts = b.pair(bigw / 9);
-    L.gA = b.take(big);
-    L.gB = b.take(big);
-    L.gf = b.take(bigf);
-    L.gd = b.take(bigo);
-    L.gy = b.pair(bigo);
-    L.gu = b.pair(bigo);
-    L.g0 = b.pair(big);
-    L.part = b.take(part);
-    L.wtmp = b.take(bigw);
-    L.bpart = b.take(bp);
-    L.g4[0] = b.take(B * N);
-    L.g4[1] = b.take(B * kC4);
-    L.g4[2] = b.take(B * kFcIn);
-    L.g4[3] = b.take(B * 16 * kCat);
-  }
+  if (P.save) reverse_layout(P, z, 1, b, L.rev);
 }
 
 static int check(const nfi_disc_params& P, char* err, size_t err_len) {
@@ -781,6 +832,142 @@ static int finish(const float* tmp, int cout, int cin, int taps, float gain, int
   return 0;
 }
 
+// g_w += gain (sum over terms k < n of wgrad(k)): the weight GEMMs into one buffer, then one finish
+template <class Wgrad>
+int wgrad_terms(float* g_w, size_t len, int n, Wgrad&& wgrad, int cout, int cin, int taps, float gain,
+                int transposed, float* wtmp, cudaStream_t st, char* err, size_t err_len) {
+  if (g_w == nullptr) return 0;
+  NFI_LAUNCH_CHECK(cudaMemsetAsync(wtmp, 0, len * sizeof(float), st));
+  for (int k = 0; k < n; ++k)
+    if (int rc = wgrad(k)) return rc;
+  return finish(wtmp, cout, cin, taps, gain, transposed, g_w, st, err, err_len);
+}
+
+Pair shifted(Pair p, size_t n) { return Pair{p.hi + n, p.lo + n}; }
+
+// The 4x4 epilogue's backward: g_logits -> g of the last block's output in V.gA [B,16,512].  The out,
+// fc and conv weight gradients pair g with hf, a4 and xs: the saved forward's, or in the HVP their
+// tangents, where the bias gradients are zero and not asked for.
+static int epilogue_backward(const nfi_disc_params& P, const Layout& L, const Reverse& V, const float* g_logits,
+                             const float* hf, const float* a4, const float* xs, float* gw_out, float* gw_fc,
+                             float* gw_b4, float* gb_out, float* gb_fc, float* gb_b4, float* grad_cmap,
+                             cudaStream_t st, char* err, size_t err_len) {
+  const int B = P.batch, N = P.cmap_dim ? P.cmap_dim : 1;
+  float *g_out = V.g4[0], *g_hf = V.g4[1], *g_a4 = V.g4[2], *g_xs = V.g4[3];
+  logits_backward_kernel<<<blocks((size_t)B * N, 256), 256, 0, st>>>(g_logits, L.out, P.cmap, B, P.cmap_dim,
+                                                                     g_out, grad_cmap);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  const float g_out_w = 1.f / sqrtf((float)kC4), g_fc_w = 1.f / sqrtf((float)kFcIn);
+  linear_dw_kernel<<<blocks((size_t)N * kC4, 256), 256, 0, st>>>(g_out, hf, g_out_w, B, kC4, N, gw_out, gb_out);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  linear_dx_kernel<<<blocks((size_t)B * kC4, 256), 256, 0, st>>>(g_out, P.out_w, g_out_w, B, kC4, N, g_hf);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  act_backward_kernel<<<flat_grid((size_t)B * kC4), 256, 0, st>>>(g_hf, L.uf, (size_t)B * kC4, kSqrt2, g_hf);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  linear_dw_kernel<<<blocks((size_t)kC4 * kFcIn, 256), 256, 0, st>>>(g_hf, a4, g_fc_w, B, kFcIn, kC4, gw_fc, gb_fc);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  linear_dx_kernel<<<blocks((size_t)B * kFcIn, 256), 256, 0, st>>>(g_hf, P.fc_w, g_fc_w, B, kFcIn, kC4, g_a4);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  act_backward_kernel<<<flat_grid((size_t)B * kFcIn), 256, 0, st>>>(g_a4, L.u4, (size_t)B * kFcIn, kSqrt2, g_a4);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  const float g4w = conv_gain(kCat, 3);
+  if (gw_b4 || gb_b4) {
+    b4_conv_dw_kernel<<<blocks((size_t)kC4 * kCat * 9, 256), 256, 0, st>>>(g_a4, xs, g4w, B, gw_b4, gb_b4);
+    NFI_LAUNCH_CHECK(cudaGetLastError());
+  }
+  b4_conv_dx_kernel<<<dim3(blocks(kCat, 256), (unsigned)B), 256, 0, st>>>(g_a4, P.b4_conv_w, g4w, g_xs);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  mbstd_backward_kernel<<<blocks((size_t)B / kGroup * kFcIn, 256), 256, 0, st>>>(g_xs, L.x4, B, V.gA);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  return 0;
+}
+
+// What the weight gradients pair the reverse walk's g with, per block and at fromrgb: the saved
+// forward's activations and image, or in the HVP their tangents.
+struct Acts {
+  const Pair *x, *ph, *d;
+  const float* img;
+};
+
+// The blocks' reverse walk, last to first, and fromrgb's, over `copies` stacked copies of the B
+// images, from g of the last block's output in V.gA.  Term k of a weight gradient pairs acts[k] with
+// gradient copy copies - 1 - k: the first order's one term is g (x) a, the HVP's two are g-dot (x) a
+// and g (x) a-dot.  A bias pairs with a constant, so its gradient, like the image's, takes the last
+// copy alone.  Below block 0 only what is asked for runs.
+static int reverse_walk(const nfi_disc_params& P, const Layout& L, const Reverse& V, int copies, const Acts* acts,
+                        float* grad_img, const nfi_disc_grads& G, cudaStream_t st, char* err, size_t err_len) {
+  const int B = P.batch, R = P.resolution, nc = P.img_channels, nb = n_blocks(R);
+  float* gy = V.gA;  // the gradient of the current block's output
+  for (int i = nb - 1; i >= 0; --i) {
+    const BlockShape s = shape(R, i);
+    const int M = B * s.h * s.h, Mr = B * s.r * s.r;
+    const size_t mo = (size_t)M * s.Co, mr = (size_t)Mr * s.C, mf = (size_t)B * (s.r + 1) * (s.r + 1) * s.C;
+    float* gx = gy == V.gA ? V.gB : V.gA;
+    const bool below = i > 0 || grad_img || G.fromrgb_w || G.fromrgb_b;
+    for (int c = 0; c < copies; ++c) {
+      out_backward_kernel<<<(unsigned)chunks(M), 256, 0, st>>>(gy + c * mo, L.u1[i], M, s.Co, V.gy.hi + c * mo,
+                                                               V.gy.lo + c * mo, V.gu.hi + c * mo, V.gu.lo + c * mo,
+                                                               V.bpart);
+      NFI_LAUNCH_CHECK(cudaGetLastError());
+    }
+    if (int rc = bias_reduce(M, s.Co, V.bpart, G.conv1_b[i], st, err, err_len)) return rc;
+    if (int rc = wgrad_terms(G.conv1_w[i], (size_t)9 * s.C * s.Co, copies, [&](int k) {
+          return synth::wgrad_down3x3(B, s.h, s.C, s.Co, acts[k].ph[i], shifted(V.gu, (copies - 1 - k) * mo),
+                                      P.conv1_w[i], V.part, V.wtmp, st, err, err_len);
+        }, s.Co, s.C, 9, conv_gain(s.C, 3), 1, V.wtmp, st, err, err_len))
+      return rc;
+    if (int rc = wgrad_terms(G.skip_w[i], (size_t)s.C * s.Co, copies, [&](int k) {
+          return synth::wgrad1x1(B, s.h, s.Co, s.C, shifted(V.gy, (copies - 1 - k) * mo), acts[k].d[i],
+                                 P.skip_w[i], V.part, V.wtmp, st, err, err_len);
+        }, s.Co, s.C, 1, conv_gain(s.C, 1) * kSkipGain, 0, V.wtmp, st, err, err_len))
+      return rc;
+    if (below || G.conv0_w[i] || G.conv0_b[i]) {
+      if (int rc = prep(P.conv1_w[i], s.Co, s.C, 9, conv_gain(s.C, 3), 1, V.t1, st, err, err_len)) return rc;
+      if (int rc = synth::conv_up3x3(copies * B, s.h, s.Co, s.C, V.gu, V.t1, V.gf, st, err, err_len)) return rc;
+      for (int c = 0; c < copies; ++c) {
+        fir_up_act_kernel<<<(unsigned)chunks(Mr), 256, 0, st>>>(V.gf + c * mf, L.a[i].hi, B, s.r, s.C,
+                                                                V.g0.hi + c * mr, V.g0.lo + c * mr, V.bpart);
+        NFI_LAUNCH_CHECK(cudaGetLastError());
+      }
+      if (int rc = bias_reduce(Mr, s.C, V.bpart, G.conv0_b[i], st, err, err_len)) return rc;
+      if (int rc = wgrad_terms(G.conv0_w[i], (size_t)9 * s.C * s.C, copies, [&](int k) {
+            return synth::wgrad3x3(B, s.r, s.r, s.C, s.C, s.C, shifted(V.g0, (copies - 1 - k) * mr), acts[k].x[i],
+                                   P.conv0_w[i], V.part, V.wtmp, st, err, err_len);
+          }, s.C, s.C, 9, conv_gain(s.C, 3), 0, V.wtmp, st, err, err_len))
+        return rc;
+    }
+    if (!below) break;
+    if (int rc = prep(P.conv0_w[i], s.C, s.C, 9, conv_gain(s.C, 3), 1, V.t0, st, err, err_len)) return rc;
+    if (int rc = synth::conv3x3_adjoint(copies * B, s.r, s.r, s.C, s.C, V.g0, V.t0, gx, st, err, err_len)) return rc;
+    if (int rc = prep(P.skip_w[i], s.Co, s.C, 1, conv_gain(s.C, 1) * kSkipGain, 1, V.ts, st, err, err_len))
+      return rc;
+    if (int rc = synth::conv1x1(copies * B, s.h, s.Co, s.C, V.gy, V.ts, V.gd, st, err, err_len)) return rc;
+    fir_down_adjoint_kernel<<<flat_grid(copies * mr), 256, 0, st>>>(V.gd, copies * B, s.r, s.C, gx);
+    NFI_LAUNCH_CHECK(cudaGetLastError());
+    gy = gx;
+  }
+  // ---- fromrgb: gy is now the gradient of its output
+  const int C = channels(R), RR = R * R, n = (int)chunks((size_t)B * RR);
+  const float grgb = 1.f / sqrtf((float)nc);
+  const size_t m0 = (size_t)B * RR * C;
+  for (int k = 0; k < copies; ++k) {
+    float* g_b = k == 0 ? G.fromrgb_b : nullptr;
+    if (!G.fromrgb_w && !g_b) continue;
+    fromrgb_backward_kernel<<<n, 256, 0, st>>>(gy + (copies - 1 - k) * m0, L.x[0].hi, acts[k].img, B, nc, RR, C,
+                                               V.bpart);
+    NFI_LAUNCH_CHECK(cudaGetLastError());
+    fromrgb_reduce_kernel<<<blocks((size_t)C * (1 + nc), 256), 256, 0, st>>>(V.bpart, n, C, nc, grgb, G.fromrgb_w,
+                                                                             g_b);
+    NFI_LAUNCH_CHECK(cudaGetLastError());
+  }
+  if (grad_img) {
+    fromrgb_gimg_kernel<<<flat_grid((size_t)B * RR * 32), 256, 0, st>>>(gy + (copies - 1) * m0, L.x[0].hi,
+                                                                        P.fromrgb_w, grgb, B, nc, RR, C, grad_img);
+    NFI_LAUNCH_CHECK(cudaGetLastError());
+  }
+  return 0;
+}
+
 }  // namespace
 
 size_t workspace_bytes(const nfi_disc_params& P) {
@@ -856,105 +1043,11 @@ int backward(const nfi_disc_params& P, const float* g_logits, float* grad_img, f
   }
   Layout L;
   if (const int rc = setup(P, L, err, err_len)) return rc;
-  const int B = P.batch, R = P.resolution, nc = P.img_channels, nb = n_blocks(R);
-  const int N = P.cmap_dim ? P.cmap_dim : 1;
-  // ---- the 4x4 epilogue
-  float *g_out = L.g4[0], *g_hf = L.g4[1], *g_a4 = L.g4[2], *g_xs = L.g4[3];
-  logits_backward_kernel<<<blocks((size_t)B * N, 256), 256, 0, st>>>(g_logits, L.out, P.cmap, B, P.cmap_dim,
-                                                                     g_out, grad_cmap);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  const float g_out_w = 1.f / sqrtf((float)kC4), g_fc_w = 1.f / sqrtf((float)kFcIn);
-  linear_dw_kernel<<<blocks((size_t)N * kC4, 256), 256, 0, st>>>(g_out, L.hf, g_out_w, B, kC4, N, G.out_w, G.out_b);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  linear_dx_kernel<<<blocks((size_t)B * kC4, 256), 256, 0, st>>>(g_out, P.out_w, g_out_w, B, kC4, N, g_hf);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  act_backward_kernel<<<flat_grid((size_t)B * kC4), 256, 0, st>>>(g_hf, L.uf, (size_t)B * kC4, kSqrt2, g_hf);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  linear_dw_kernel<<<blocks((size_t)kC4 * kFcIn, 256), 256, 0, st>>>(g_hf, L.a4, g_fc_w, B, kFcIn, kC4, G.fc_w,
-                                                                     G.fc_b);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  linear_dx_kernel<<<blocks((size_t)B * kFcIn, 256), 256, 0, st>>>(g_hf, P.fc_w, g_fc_w, B, kFcIn, kC4, g_a4);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  act_backward_kernel<<<flat_grid((size_t)B * kFcIn), 256, 0, st>>>(g_a4, L.u4, (size_t)B * kFcIn, kSqrt2, g_a4);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  const float g4w = conv_gain(kCat, 3);
-  if (G.b4_conv_w || G.b4_conv_b) {
-    b4_conv_dw_kernel<<<blocks((size_t)kC4 * kCat * 9, 256), 256, 0, st>>>(g_a4, L.xs, g4w, B, G.b4_conv_w,
-                                                                          G.b4_conv_b);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
-  }
-  b4_conv_dx_kernel<<<dim3(blocks(kCat, 256), (unsigned)B), 256, 0, st>>>(g_a4, P.b4_conv_w, g4w, g_xs);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  float* gy = L.gA;  // the gradient of the current block's output
-  mbstd_backward_kernel<<<blocks((size_t)B / kGroup * kFcIn, 256), 256, 0, st>>>(g_xs, L.x4, B, gy);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  // ---- the blocks, last to first
-  for (int i = nb - 1; i >= 0; --i) {
-    const BlockShape s = shape(R, i);
-    const int M = B * s.h * s.h, Mr = B * s.r * s.r;
-    float* gx = gy == L.gA ? L.gB : L.gA;
-    const bool below = i > 0 || grad_img || G.fromrgb_w || G.fromrgb_b;
-    out_backward_kernel<<<(unsigned)chunks(M), 256, 0, st>>>(gy, L.u1[i], M, s.Co, L.gy.hi, L.gy.lo, L.gu.hi,
-                                                             L.gu.lo, L.bpart);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
-    if (int rc = bias_reduce(M, s.Co, L.bpart, G.conv1_b[i], st, err, err_len)) return rc;
-    if (G.conv1_w[i]) {
-      NFI_LAUNCH_CHECK(cudaMemsetAsync(L.wtmp, 0, (size_t)9 * s.C * s.Co * sizeof(float), st));
-      if (int rc = synth::wgrad_down3x3(B, s.h, s.C, s.Co, L.ph[i], L.gu, P.conv1_w[i], L.part, L.wtmp, st, err,
-                                        err_len))
-        return rc;
-      if (int rc = finish(L.wtmp, s.Co, s.C, 9, conv_gain(s.C, 3), 1, G.conv1_w[i], st, err, err_len)) return rc;
-    }
-    if (G.skip_w[i]) {
-      NFI_LAUNCH_CHECK(cudaMemsetAsync(L.wtmp, 0, (size_t)s.C * s.Co * sizeof(float), st));
-      if (int rc = synth::wgrad1x1(B, s.h, s.Co, s.C, L.gy, L.d[i], P.skip_w[i], L.part, L.wtmp, st, err, err_len))
-        return rc;
-      if (int rc = finish(L.wtmp, s.Co, s.C, 1, conv_gain(s.C, 1) * kSkipGain, 0, G.skip_w[i], st, err, err_len))
-        return rc;
-    }
-    const bool need0 = below || G.conv0_w[i] || G.conv0_b[i];
-    if (need0) {
-      if (int rc = prep(P.conv1_w[i], s.Co, s.C, 9, conv_gain(s.C, 3), 1, L.t1, st, err, err_len)) return rc;
-      if (int rc = synth::conv_up3x3(B, s.h, s.Co, s.C, L.gu, L.t1, L.gf, st, err, err_len)) return rc;
-      fir_up_act_kernel<<<(unsigned)chunks(Mr), 256, 0, st>>>(L.gf, L.a[i].hi, B, s.r, s.C, L.g0.hi, L.g0.lo,
-                                                              L.bpart);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
-      if (int rc = bias_reduce(Mr, s.C, L.bpart, G.conv0_b[i], st, err, err_len)) return rc;
-      if (G.conv0_w[i]) {
-        NFI_LAUNCH_CHECK(cudaMemsetAsync(L.wtmp, 0, (size_t)9 * s.C * s.C * sizeof(float), st));
-        if (int rc = synth::wgrad3x3(B, s.r, s.r, s.C, s.C, s.C, L.g0, L.x[i], P.conv0_w[i], L.part, L.wtmp, st,
-                                     err, err_len))
-          return rc;
-        if (int rc = finish(L.wtmp, s.C, s.C, 9, conv_gain(s.C, 3), 0, G.conv0_w[i], st, err, err_len)) return rc;
-      }
-    }
-    if (!below) break;
-    if (int rc = prep(P.conv0_w[i], s.C, s.C, 9, conv_gain(s.C, 3), 1, L.t0, st, err, err_len)) return rc;
-    if (int rc = synth::conv3x3_adjoint(B, s.r, s.r, s.C, s.C, L.g0, L.t0, gx, st, err, err_len)) return rc;
-    if (int rc = prep(P.skip_w[i], s.Co, s.C, 1, conv_gain(s.C, 1) * kSkipGain, 1, L.ts, st, err, err_len))
-      return rc;
-    if (int rc = synth::conv1x1(B, s.h, s.Co, s.C, L.gy, L.ts, L.gd, st, err, err_len)) return rc;
-    fir_down_adjoint_kernel<<<flat_grid((size_t)Mr * s.C), 256, 0, st>>>(L.gd, B, s.r, s.C, gx);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
-    gy = gx;
-  }
-  // ---- fromrgb: gy is now the gradient of its output
-  const int C = channels(R), RR = R * R;
-  const float grgb = 1.f / sqrtf((float)nc);
-  if (G.fromrgb_w || G.fromrgb_b) {
-    const int n = (int)chunks((size_t)B * RR);
-    fromrgb_backward_kernel<<<n, 256, 0, st>>>(gy, L.x[0].hi, P.img, B, nc, RR, C, L.bpart);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
-    fromrgb_reduce_kernel<<<blocks((size_t)C * (1 + nc), 256), 256, 0, st>>>(L.bpart, n, C, nc, grgb, G.fromrgb_w,
-                                                                             G.fromrgb_b);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
-  }
-  if (grad_img) {
-    fromrgb_gimg_kernel<<<flat_grid((size_t)B * RR * 32), 256, 0, st>>>(gy, L.x[0].hi, P.fromrgb_w, grgb, B, nc, RR, C,
-                                                                   grad_img);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
-  }
-  return 0;
+  if (int rc = epilogue_backward(P, L, L.rev, g_logits, L.hf, L.a4, L.xs, G.out_w, G.fc_w, G.b4_conv_w, G.out_b,
+                                 G.fc_b, G.b4_conv_b, grad_cmap, st, err, err_len))
+    return rc;
+  const Acts saved = {L.x, L.ph, L.d, P.img};
+  return reverse_walk(P, L, L.rev, 1, &saved, grad_img, G, st, err, err_len);
 }
 
 int saved_preactivation(const nfi_disc_params& P, int block, int which, float* out, cudaStream_t st, char* err,
@@ -1015,18 +1108,15 @@ int saved_preactivation(const nfi_disc_params& P, int block, int which, float* o
 //   (conv_down3x3); fir_down_kernel and the skip (conv1x1); block_out_tangent_kernel;
 //   mbstd_tangent_kernel; b4_conv_kernel / linear_kernel with a zero bias, then
 //   act_backward_kernel for the branches; logits_kernel (J_img t, the g_logits gradient).
-//   reverse walk: the epilogue's g as in the first-order backward, mbstd_backward_kernel (g) and
-//   mbstd_hvp_kernel (g-dot) into one stacked [g; g-dot] buffer of 2B images; per block the data
-//   GEMMs (conv_up3x3, conv3x3_adjoint, conv1x1) and fir_down_adjoint_kernel run once over the 2B
-//   images, the pointwise passes (out_backward_kernel, fir_up_act_kernel) per half with the
-//   g-dot half's bias partials; each weight's gradient sum g-dot (x) a + g (x) a-dot is two
+//   dPhi/dcmap: logits_backward_kernel on out-dot.
+//   reverse walk: the first-order backward's, with two copies.  epilogue_backward (g, its weight
+//   terms against the tangents) ends in mbstd_backward_kernel (g), and mbstd_hvp_kernel (g-dot)
+//   fills the second half of the stacked [g; g-dot] buffer of 2B images.  reverse_walk runs the
+//   data GEMMs and fir_down_adjoint_kernel once over the 2B images, the pointwise passes per copy
+//   with the g-dot copy's bias partials, and each weight's gradient g-dot (x) a + g (x) a-dot as two
 //   wgrad_* launches into one buffer and one finish.
 // Reads a save = 1 workspace only; everything it writes but the caller's outputs is the scratch.
 namespace {
-
-__device__ __forceinline__ float branch(const __nv_bfloat16* hi, size_t i) {
-  return __bfloat162float(hi[i]) > 0.f ? 1.f : kSlope;
-}
 
 // x-dot[b,p,c] = sqrt2 lrelu'(x) sum_ci (w[c,ci] g) t[b,ci,p] -> pair [B,R,R,C]
 __global__ void __launch_bounds__(256)
@@ -1073,23 +1163,9 @@ mbstd_tangent_kernel(const float* __restrict__ x, const float* __restrict__ dx, 
   const int G = B / kGroup, j = blockIdx.x;
   float s = 0.f;
   for (int e = threadIdx.x; e < 16 * kC4; e += 256) {
-    float v[kGroup], dv[kGroup], m = 0.f, dm = 0.f;
-    for (int k = 0; k < kGroup; ++k) {
-      const size_t o = (size_t)(k * G + j) * 16 * kC4 + e;
-      v[k] = __ldg(x + o);
-      dv[k] = __ldg(dx + o);
-      m += v[k];
-      dm += dv[k];
-    }
-    m /= (float)kGroup;
-    dm /= (float)kGroup;
-    float var = 0.f, dvar = 0.f;
-    for (int k = 0; k < kGroup; ++k) {
-      var += (v[k] - m) * (v[k] - m);
-      dvar += (v[k] - m) * (dv[k] - dm);
-    }
-    s += dvar / ((float)kGroup * sqrtf(var / (float)kGroup + 1e-8f));
-    for (int k = 0; k < kGroup; ++k) dxs[((size_t)(k * G + j) * 16 + e / kC4) * kCat + e % kC4] = dv[k];
+    const Group q = group(x, dx, G, j, e);
+    s += q.dvar / ((float)kGroup * q.s);
+    for (int k = 0; k < kGroup; ++k) dxs[((size_t)(k * G + j) * 16 + e / kC4) * kCat + e % kC4] = q.dv[k];
   }
   part[threadIdx.x] = s;
   __syncthreads();
@@ -1112,29 +1188,12 @@ __global__ void mbstd_hvp_kernel(const float* __restrict__ gxs, const float* __r
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (size_t)G * 16 * kC4) return;
   const int e = (int)(i % (16 * kC4)), j = (int)(i / (16 * kC4));
-  float gs = 0.f;
-  for (int k = 0; k < kGroup; ++k)
-    for (int p = 0; p < 16; ++p) gs += __ldg(gxs + ((size_t)(k * G + j) * 16 + p) * kCat + kC4);
-  float v[kGroup], dv[kGroup], m = 0.f, dm = 0.f;
-  for (int k = 0; k < kGroup; ++k) {
-    const size_t o = (size_t)(k * G + j) * 16 * kC4 + e;
-    v[k] = __ldg(x + o);
-    dv[k] = __ldg(dx + o);
-    m += v[k];
-    dm += dv[k];
-  }
-  m /= (float)kGroup;
-  dm /= (float)kGroup;
-  float var = 0.f, dvar = 0.f;
-  for (int k = 0; k < kGroup; ++k) {
-    var += (v[k] - m) * (v[k] - m);
-    dvar += (v[k] - m) * (dv[k] - dm);
-  }
-  const float s = sqrtf(var / (float)kGroup + 1e-8f);
-  const float ds = dvar / ((float)kGroup * s);
+  const float gs = std_grad_sum(gxs, G, j);
+  const Group q = group(x, dx, G, j, e);
+  const float ds = q.dvar / ((float)kGroup * q.s);
   const float c = gs / (float)(16 * kC4) / (float)kGroup;
   for (int k = 0; k < kGroup; ++k)
-    dgx[(size_t)(k * G + j) * 16 * kC4 + e] = c * ((dv[k] - dm) / s - (v[k] - m) * ds / (s * s));
+    dgx[(size_t)(k * G + j) * 16 * kC4 + e] = c * ((q.dv[k] - q.dm) / q.s - (q.v[k] - q.m) * ds / (q.s * q.s));
 }
 
 __global__ void accumulate_kernel(const float* __restrict__ src, int n, float* __restrict__ dst) {
@@ -1142,67 +1201,37 @@ __global__ void accumulate_kernel(const float* __restrict__ src, int n, float* _
   if (i < n) dst[i] += src[i];
 }
 
-Pair shifted(Pair p, size_t n) { return Pair{p.hi + n, p.lo + n}; }
-
-// The scratch: the tangent forward's activations per block, the stacked [g; g-dot] buffers of the
-// reverse walk, the weights in both orientations and the partial sums.
+// The scratch: the tangent forward's activations per block, its weights, and the reverse walk's
+// buffers for the stacked [g; g-dot].
 struct HvpLayout {
   Pair dx[kMaxBlocks], da[kMaxBlocks], dph[kMaxBlocks], dd[kMaxBlocks];  // as Layout's x, a, ph, d
-  Pair w0, w1, ws, t0, t1, ts;
+  Pair w0, w1, ws;
   float* raw0;                   // [B,r,r,C] conv0's raw tangent
   float* raw1;
   float* raws;
   float* zero;                   // [512] zero bias
   float *dx4, *dxs, *du4, *junk, *da4, *dhf, *dout, *jt;
-  float* g4[4];                  // as Layout's g4
-  float *gA, *gB;                // [2B,r,r,C] stacked
-  float* gf;                     // [2B,r+1,r+1,C]
-  float* gd;                     // [2B,h,h,C]
-  Pair gy, gu;                   // [2B,h,h,C']
-  Pair g0;                       // [2B,r,r,C]
-  float* part;
-  float* wtmp;
-  float* bpart;
+  Reverse rev;
 };
 
 void hvp_layout(const nfi_disc_params& P, Bump& b, HvpLayout& L) {
   memset(&L, 0, sizeof(L));
-  const size_t B = P.batch;
-  const int nb = n_blocks(P.resolution), N = P.cmap_dim ? P.cmap_dim : 1;
-  size_t big = 0, bigo = 0, bigf = 0, bigw = 0, part = 0, bp = 0;
-  for (int i = 0; i < nb; ++i) {
+  const Sizes z = sizes(P);
+  const size_t B = P.batch, N = P.cmap_dim ? P.cmap_dim : 1;
+  for (int i = 0; i < n_blocks(P.resolution); ++i) {
     const BlockShape s = shape(P.resolution, i);
     const size_t rr = (size_t)s.r * s.r, hh = (size_t)s.h * s.h;
     L.dx[i] = b.pair(B * rr * s.C);
     L.da[i] = b.pair(B * rr * s.C);
     L.dph[i] = b.pair(4 * B * (s.h + 1) * (s.h + 1) * s.C);
     L.dd[i] = b.pair(B * hh * s.C);
-    big = big > B * rr * s.C ? big : B * rr * s.C;
-    bigo = bigo > B * hh * s.Co ? bigo : B * hh * s.Co;
-    const size_t f = B * (s.r + 1) * (s.r + 1) * s.C;
-    bigf = bigf > f ? bigf : f;
-    const size_t w = (size_t)9 * s.C * (s.C > s.Co ? s.C : s.Co);
-    bigw = bigw > w ? bigw : w;
-    const size_t p0 = synth::wgrad3x3_partial_floats(P.batch, s.r, s.r, s.C, s.C);
-    const size_t p1 = synth::wgrad_down3x3_partial_floats(P.batch, s.h, s.C, s.Co);
-    const size_t p2 = synth::wgrad1x1_partial_floats(P.batch, s.h, s.Co, s.C);
-    part = part > p0 ? part : p0;
-    part = part > p1 ? part : p1;
-    part = part > p2 ? part : p2;
-    const size_t c0 = chunks(B * rr) * s.C * (i == 0 ? 1 + P.img_channels : 1);
-    const size_t c1 = chunks(B * hh) * s.Co;
-    bp = bp > c0 ? bp : c0;
-    bp = bp > c1 ? bp : c1;
   }
-  L.w0 = b.pair(bigw);
-  L.w1 = b.pair(bigw);
-  L.ws = b.pair(bigw / 9);
-  L.t0 = b.pair(bigw);
-  L.t1 = b.pair(bigw);
-  L.ts = b.pair(bigw / 9);
-  L.raw0 = b.take(big);
-  L.raw1 = b.take(bigo);
-  L.raws = b.take(bigo);
+  L.w0 = b.pair(z.bigw);
+  L.w1 = b.pair(z.bigw);
+  L.ws = b.pair(z.bigw / 9);
+  L.raw0 = b.take(z.big);
+  L.raw1 = b.take(z.bigo);
+  L.raws = b.take(z.bigo);
   L.zero = b.take(kC4);
   L.dx4 = b.take(B * kFcIn);
   L.dxs = b.take(B * 16 * kCat);
@@ -1212,31 +1241,7 @@ void hvp_layout(const nfi_disc_params& P, Bump& b, HvpLayout& L) {
   L.dhf = b.take(B * kC4);
   L.dout = b.take(B * N);
   L.jt = b.take(B);
-  L.g4[0] = b.take(B * N);
-  L.g4[1] = b.take(B * kC4);
-  L.g4[2] = b.take(B * kFcIn);
-  L.g4[3] = b.take(B * 16 * kCat);
-  L.gA = b.take(2 * big);
-  L.gB = b.take(2 * big);
-  L.gf = b.take(2 * bigf);
-  L.gd = b.take(2 * bigo);
-  L.gy = b.pair(2 * bigo);
-  L.gu = b.pair(2 * bigo);
-  L.g0 = b.pair(2 * big);
-  L.part = b.take(part);
-  L.wtmp = b.take(bigw);
-  L.bpart = b.take(bp);
-}
-
-// g_w += gain (sum g-dot (x) a + g (x) a-dot): the two weight GEMMs into one buffer, then one finish
-template <class Wgrad>
-int two_term(float* g_w, size_t n, Wgrad&& wgrad, int cout, int cin, int taps, float gain, int transposed,
-             float* wtmp, cudaStream_t st, char* err, size_t err_len) {
-  if (g_w == nullptr) return 0;
-  NFI_LAUNCH_CHECK(cudaMemsetAsync(wtmp, 0, n * sizeof(float), st));
-  if (int rc = wgrad(0)) return rc;
-  if (int rc = wgrad(1)) return rc;
-  return finish(wtmp, cout, cin, taps, gain, transposed, g_w, st, err, err_len);
+  reverse_layout(P, z, 2, b, L.rev);
 }
 
 }  // namespace
@@ -1327,114 +1332,21 @@ int backward_hvp(const nfi_disc_params& P, const nfi_disc_hvp& V, const nfi_disc
     accumulate_kernel<<<blocks(B, 128), 128, 0, st>>>(H.jt, B, V.grad_g_logits);
     NFI_LAUNCH_CHECK(cudaGetLastError());
   }
-  // ---- the epilogue: g as in the first-order backward; its g-dot is zero (property 2)
-  float *g_out = H.g4[0], *g_hf = H.g4[1], *g_a4 = H.g4[2], *g_xs = H.g4[3];
-  logits_backward_kernel<<<blocks((size_t)B * N, 256), 256, 0, st>>>(V.g_logits, L.out, P.cmap, B, P.cmap_dim,
-                                                                     g_out, nullptr);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
   if (V.grad_cmap && P.cmap_dim) {  // g_logits out-dot / sqrt N (g_out's write here is discarded)
     logits_backward_kernel<<<blocks((size_t)B * N, 256), 256, 0, st>>>(V.g_logits, H.dout, P.cmap, B, P.cmap_dim,
                                                                        H.junk, V.grad_cmap);
     NFI_LAUNCH_CHECK(cudaGetLastError());
   }
-  linear_dw_kernel<<<blocks((size_t)N * kC4, 256), 256, 0, st>>>(g_out, H.dhf, g_out_w, B, kC4, N, G.out_w, nullptr);
+  // ---- the reverse walk: the epilogue's g as in the first-order backward (its g-dot is zero, property
+  // 2), the minibatch std's g-dot after it, then the blocks over the stacked [g; g-dot]
+  if (int rc = epilogue_backward(P, L, H.rev, V.g_logits, H.dhf, H.da4, H.dxs, G.out_w, G.fc_w, G.b4_conv_w,
+                                 nullptr, nullptr, nullptr, nullptr, st, err, err_len))
+    return rc;
+  mbstd_hvp_kernel<<<blocks((size_t)B / kGroup * kFcIn, 256), 256, 0, st>>>(H.rev.g4[3], L.x4, H.dx4, B,
+                                                                            H.rev.gA + (size_t)B * kFcIn);
   NFI_LAUNCH_CHECK(cudaGetLastError());
-  linear_dx_kernel<<<blocks((size_t)B * kC4, 256), 256, 0, st>>>(g_out, P.out_w, g_out_w, B, kC4, N, g_hf);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  act_backward_kernel<<<flat_grid((size_t)B * kC4), 256, 0, st>>>(g_hf, L.uf, (size_t)B * kC4, kSqrt2, g_hf);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  linear_dw_kernel<<<blocks((size_t)kC4 * kFcIn, 256), 256, 0, st>>>(g_hf, H.da4, g_fc_w, B, kFcIn, kC4, G.fc_w,
-                                                                     nullptr);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  linear_dx_kernel<<<blocks((size_t)B * kFcIn, 256), 256, 0, st>>>(g_hf, P.fc_w, g_fc_w, B, kFcIn, kC4, g_a4);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  act_backward_kernel<<<flat_grid((size_t)B * kFcIn), 256, 0, st>>>(g_a4, L.u4, (size_t)B * kFcIn, kSqrt2, g_a4);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  const float g4w = conv_gain(kCat, 3);
-  if (G.b4_conv_w) {
-    b4_conv_dw_kernel<<<blocks((size_t)kC4 * kCat * 9, 256), 256, 0, st>>>(g_a4, H.dxs, g4w, B, G.b4_conv_w,
-                                                                          nullptr);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
-  }
-  b4_conv_dx_kernel<<<dim3(blocks(kCat, 256), (unsigned)B), 256, 0, st>>>(g_a4, P.b4_conv_w, g4w, g_xs);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  // [g; g-dot] of the last block's output, stacked over 2B images
-  float* gy = H.gA;
-  const size_t n4 = (size_t)B * kFcIn;
-  mbstd_backward_kernel<<<blocks((size_t)B / kGroup * kFcIn, 256), 256, 0, st>>>(g_xs, L.x4, B, gy);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  mbstd_hvp_kernel<<<blocks((size_t)B / kGroup * kFcIn, 256), 256, 0, st>>>(g_xs, L.x4, H.dx4, B, gy + n4);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  // ---- the blocks, last to first
-  for (int i = nb - 1; i >= 0; --i) {
-    const BlockShape s = shape(R, i);
-    const int M = B * s.h * s.h, Mr = B * s.r * s.r;
-    const size_t mo = (size_t)M * s.Co, mr = (size_t)Mr * s.C, mf = (size_t)B * (s.r + 1) * (s.r + 1) * s.C;
-    float* gx = gy == H.gA ? H.gB : H.gA;
-    for (int half = 0; half < 2; ++half) {
-      out_backward_kernel<<<(unsigned)chunks(M), 256, 0, st>>>(gy + half * mo, L.u1[i], M, s.Co, H.gy.hi + half * mo,
-                                                               H.gy.lo + half * mo, H.gu.hi + half * mo,
-                                                               H.gu.lo + half * mo, H.bpart);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
-    }
-    if (int rc = bias_reduce(M, s.Co, H.bpart, G.conv1_b[i], st, err, err_len)) return rc;
-    const Pair gu = H.gu, dgu = shifted(H.gu, mo), gyp = H.gy, dgy = shifted(H.gy, mo);
-    if (int rc = two_term(G.conv1_w[i], (size_t)9 * s.C * s.Co, [&](int k) {
-          return synth::wgrad_down3x3(B, s.h, s.C, s.Co, k ? H.dph[i] : L.ph[i], k ? gu : dgu, P.conv1_w[i],
-                                      H.part, H.wtmp, st, err, err_len);
-        }, s.Co, s.C, 9, conv_gain(s.C, 3), 1, H.wtmp, st, err, err_len))
-      return rc;
-    if (int rc = two_term(G.skip_w[i], (size_t)s.C * s.Co, [&](int k) {
-          return synth::wgrad1x1(B, s.h, s.Co, s.C, k ? gyp : dgy, k ? H.dd[i] : L.d[i], P.skip_w[i], H.part,
-                                 H.wtmp, st, err, err_len);
-        }, s.Co, s.C, 1, conv_gain(s.C, 1) * kSkipGain, 0, H.wtmp, st, err, err_len))
-      return rc;
-    if (int rc = prep(P.conv1_w[i], s.Co, s.C, 9, conv_gain(s.C, 3), 1, H.t1, st, err, err_len)) return rc;
-    if (int rc = synth::conv_up3x3(2 * B, s.h, s.Co, s.C, H.gu, H.t1, H.gf, st, err, err_len)) return rc;
-    for (int half = 0; half < 2; ++half) {
-      fir_up_act_kernel<<<(unsigned)chunks(Mr), 256, 0, st>>>(H.gf + half * mf, L.a[i].hi, B, s.r, s.C,
-                                                              H.g0.hi + half * mr, H.g0.lo + half * mr, H.bpart);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
-    }
-    if (int rc = bias_reduce(Mr, s.C, H.bpart, G.conv0_b[i], st, err, err_len)) return rc;
-    const Pair g0 = H.g0, dg0 = shifted(H.g0, mr);
-    if (int rc = two_term(G.conv0_w[i], (size_t)9 * s.C * s.C, [&](int k) {
-          return synth::wgrad3x3(B, s.r, s.r, s.C, s.C, s.C, k ? g0 : dg0, k ? H.dx[i] : L.x[i], P.conv0_w[i],
-                                 H.part, H.wtmp, st, err, err_len);
-        }, s.C, s.C, 9, conv_gain(s.C, 3), 0, H.wtmp, st, err, err_len))
-      return rc;
-    if (int rc = prep(P.conv0_w[i], s.C, s.C, 9, conv_gain(s.C, 3), 1, H.t0, st, err, err_len)) return rc;
-    if (int rc = synth::conv3x3_adjoint(2 * B, s.r, s.r, s.C, s.C, H.g0, H.t0, gx, st, err, err_len)) return rc;
-    if (int rc = prep(P.skip_w[i], s.Co, s.C, 1, conv_gain(s.C, 1) * kSkipGain, 1, H.ts, st, err, err_len))
-      return rc;
-    if (int rc = synth::conv1x1(2 * B, s.h, s.Co, s.C, H.gy, H.ts, H.gd, st, err, err_len)) return rc;
-    fir_down_adjoint_kernel<<<flat_grid((size_t)2 * mr), 256, 0, st>>>(H.gd, 2 * B, s.r, s.C, gx);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
-    gy = gx;
-  }
-  // ---- fromrgb: gy holds [g; g-dot] of its output
-  const size_t m0 = (size_t)B * RR * C;
-  if (G.fromrgb_w || G.fromrgb_b) {
-    const int n = (int)chunks((size_t)B * RR);
-    fromrgb_backward_kernel<<<n, 256, 0, st>>>(gy + m0, L.x[0].hi, P.img, B, nc, RR, C, H.bpart);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
-    fromrgb_reduce_kernel<<<blocks((size_t)C * (1 + nc), 256), 256, 0, st>>>(H.bpart, n, C, nc, grgb, G.fromrgb_w,
-                                                                             G.fromrgb_b);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
-    if (G.fromrgb_w) {
-      fromrgb_backward_kernel<<<n, 256, 0, st>>>(gy, L.x[0].hi, V.t_img, B, nc, RR, C, H.bpart);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
-      fromrgb_reduce_kernel<<<blocks((size_t)C * (1 + nc), 256), 256, 0, st>>>(H.bpart, n, C, nc, grgb,
-                                                                               G.fromrgb_w, nullptr);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
-    }
-  }
-  if (V.grad_img) {
-    fromrgb_gimg_kernel<<<flat_grid((size_t)B * RR * 32), 256, 0, st>>>(gy + m0, L.x[0].hi, P.fromrgb_w, grgb, B, nc,
-                                                                        RR, C, V.grad_img);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
-  }
-  return 0;
+  const Acts acts[2] = {{L.x, L.ph, L.d, P.img}, {H.dx, H.dph, H.dd, V.t_img}};
+  return reverse_walk(P, L, H.rev, 2, acts, V.grad_img, G, st, err, err_len);
 }
 
 }  // namespace disc

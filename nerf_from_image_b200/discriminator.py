@@ -183,10 +183,7 @@ def _backward(state, g_logits, needs):
     p, work, ic, cc, wc, out = state
     dev = work.device
     with torch.cuda.device(dev):
-        gi = torch.zeros_like(ic) if needs[0] else None
-        gc = torch.zeros_like(cc) if (cc is not None and needs[1]) else None
-        gw = [torch.zeros_like(t) if needs[2 + i] else None for i, t in enumerate(wc)]
-        g = _params_grads(gw, p.resolution)
+        gi, gc, gw, g = _grad_outputs(state, needs)
         gl = g_logits.detach().to(torch.float32).reshape(-1).contiguous()
         _lib.check(_lib.load().nfi_disc_backward(ctypes.byref(p), _lib.ptr(gl), _lib.ptr(gi), _lib.ptr(gc),
                                                  ctypes.byref(g), _lib.stream(dev)))
@@ -303,18 +300,25 @@ def _hvp(state, g_logits, t_img, need_gl, needs):
         gl = g_logits.detach().to(torch.float32).reshape(-1).contiguous()
         t = t_img.detach().to(torch.float32).contiguous()
         g_gl = torch.zeros_like(gl) if need_gl else None
-        gi = torch.zeros_like(ic) if needs[0] else None
-        gc = torch.zeros_like(cc) if (cc is not None and needs[1]) else None
-        gw = [torch.zeros_like(w) if needs[2 + i] else None for i, w in enumerate(wc)]
+        gi, gc, gw, g = _grad_outputs(state, needs)
         nbytes = lib.nfi_disc_r1_scratch_bytes(ctypes.byref(p))
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         h = _lib.DiscHvp(g_logits=gl.data_ptr(), t_img=t.data_ptr(), scratch=scratch.data_ptr(),
                          scratch_bytes=nbytes, grad_img=_lib.ptr(gi), grad_cmap=_lib.ptr(gc),
                          grad_g_logits=_lib.ptr(g_gl))
-        g = _params_grads(gw, p.resolution)
         _lib.check(lib.nfi_disc_backward_hvp(ctypes.byref(p), ctypes.byref(h), ctypes.byref(g), _lib.stream(dev)))
         del scratch
     return ((g_gl.view_as(g_logits) if g_gl is not None else None), gi, gc, *gw)
+
+
+def _grad_outputs(state, needs):
+    """The zeroed ``+=`` outputs of a backward pass on ``state``'s forward: image, cmap and every
+    weight (None where ``needs``, one flag per input, says not), and the weights' ``DiscGrads``."""
+    p, work, ic, cc, wc, out = state
+    gi = torch.zeros_like(ic) if needs[0] else None
+    gc = torch.zeros_like(cc) if (cc is not None and needs[1]) else None
+    gw = [torch.zeros_like(t) if needs[2 + i] else None for i, t in enumerate(wc)]
+    return gi, gc, gw, _params_grads(gw, p.resolution)
 
 
 def _params_grads(gw, R):
