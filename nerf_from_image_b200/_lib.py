@@ -308,6 +308,26 @@ DISC_R1_EXPORTS = {
                                              ctypes.POINTER(DiscGrads), ctypes.c_void_p]),
 }
 
+SEGFORMER_STAGES, SEGFORMER_MAX_DEPTH, SEGFORMER_DECODER = 4, 64, 768
+
+
+class SegformerParams(ctypes.Structure):
+    """struct nfi_segformer_params (include/nfi_segformer.h)."""
+    _fields_ = [('batch', ctypes.c_int32), ('height', ctypes.c_int32), ('width', ctypes.c_int32),
+                ('depths', ctypes.c_int32 * SEGFORMER_STAGES), ('out_features', ctypes.c_int32),
+                ('save', ctypes.c_int32)] + [
+        (n, ctypes.c_void_p) for n in ('image', 'params', 'drop_scales', 'features', 'workspace')] + [
+        ('workspace_bytes', ctypes.c_size_t)]
+
+
+# include/nfi_segformer.h (tests/test_segformer_abi.py)
+SEGFORMER_EXPORTS = {
+    'nfi_segformer_workspace_bytes': (ctypes.c_size_t, [ctypes.POINTER(SegformerParams)]),
+    'nfi_segformer_forward': (ctypes.c_int, [ctypes.POINTER(SegformerParams), ctypes.c_void_p]),
+    'nfi_segformer_backward': (ctypes.c_int, [ctypes.POINTER(SegformerParams), ctypes.c_void_p,
+                                              ctypes.c_void_p, ctypes.c_void_p]),
+}
+
 _lib = None
 _lock = threading.Lock()
 
@@ -349,7 +369,8 @@ def load():
                                '(nerf_from_image_b200/csrc/build.sh)' % (LIB_PATH, got, ABI_VERSION))
             for name, (restype, argtypes) in (list(EXPORTS.items()) + list(LPIPS_EXPORTS.items())
                                        + list(ENCODER_EXPORTS.items()) + list(DISC_EXPORTS.items())
-                                       + list(DISC_R1_EXPORTS.items())):
+                                       + list(DISC_R1_EXPORTS.items())
+                                       + list(SEGFORMER_EXPORTS.items())):
                 fn = getattr(lib, name, None)
                 if fn is None and os.environ.get('NFI_LIB_PATH'):
                     continue  # an older build under test lacks the newer entry points

@@ -21,6 +21,8 @@
 #include "nfi_encoder_launch.h"
 #include "nfi_lpips.h"
 #include "nfi_lpips_launch.h"
+#include "nfi_segformer.h"
+#include "nfi_segformer_launch.h"
 #include "nfi_synth.h"
 #include "nfi_synth_launch.h"
 
@@ -526,6 +528,22 @@ int nfi_encoder_backward(const nfi_encoder_params* params, const float* g_maps, 
 int nfi_encoder_saved_activation(const nfi_encoder_params* params, int32_t layer, float* out, void* stream) {
   if (params == nullptr) return fail("params is NULL");
   return nfi::encoder::saved_activation(*params, layer, out, (cudaStream_t)stream, g_err, sizeof(g_err));
+}
+
+size_t nfi_segformer_workspace_bytes(const nfi_segformer_params* params) {
+  if (params == nullptr) return 0;
+  return nfi::segformer::workspace_bytes(*params);
+}
+
+int nfi_segformer_forward(const nfi_segformer_params* params, void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  return nfi::segformer::forward(*params, (cudaStream_t)stream, g_err, sizeof(g_err));
+}
+
+int nfi_segformer_backward(const nfi_segformer_params* params, const float* g_features, float* const* grads,
+                           void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  return nfi::segformer::backward(*params, g_features, grads, (cudaStream_t)stream, g_err, sizeof(g_err));
 }
 
 size_t nfi_disc_workspace_bytes(const nfi_disc_params* params) {

@@ -5,9 +5,10 @@
     rate from the shape arithmetic and its share of the bf16 dense bound for three products per
     GEMM (989 / 3 TFLOP/s);
 (b) one encoder step (SegFormer backbone, heads, criteria, backward, Adam) of the reference
-    BootstrapEncoder, fused against eager, and the backbone's own forward + backward;
+    BootstrapEncoder in three arms: the heads fused ('heads'), the backbone and the heads fused
+    ('full'), and eager; and the backbone's own forward + backward, eager and fused;
 (c) one whole iteration: (b) after the no-grad generator render with compute_coords=True (fused
-    synthesis and render);
+    synthesis and render), in the same three arms;
 (d) the peak memory of each arm.
 Arms alternate within each round (CUDA events, every shape warmed up first); the median of the
 rounds is printed.  The card's name, power limit and SM clock are read in the same call.  Needs the
@@ -69,6 +70,7 @@ def main():
     torch.backends.cuda.matmul.allow_tf32 = False
     torch.backends.cudnn.allow_tf32 = False
     from nerf_from_image_b200.encoder import enable_fused_encoder, heads
+    from nerf_from_image_b200.segformer import enable_fused_segformer
     from oracle import encoder_oracle as EO
     from tests.encoder_standin import StandInBootstrapEncoder, load_params, reference_encoder
 
@@ -110,11 +112,13 @@ def main():
     tc, tm = torch.randn(B, R, R, 3, generator=g).cuda(), (torch.rand(B, R, R, generator=g) > 0.5).float().cuda()
     tw = torch.randn(B, 1, LAT, generator=g).cuda()
     models = {}
-    for name in ('fused', 'eager'):
+    for name in ('heads', 'full', 'eager'):
         m = reference_encoder(LAT)
         m.load_state_dict(state)
-        if name == 'fused':
+        if name != 'eager':
             enable_fused_encoder(m)
+        if name == 'full':
+            enable_fused_segformer(m.backbone)
         model = nn.DataParallel(m.cuda(), [0])
         model.requires_grad_(True)
         model.train()
@@ -128,17 +132,18 @@ def main():
         loss.backward()
         opt.step()
 
-    backbone = models['eager'][0].module.backbone
     gfeat = torch.randn(B, 512, h, w, generator=g).cuda()
+    bb = {k: models[k][0].module.backbone for k in ('eager', 'full')}
 
-    def backbone_only():
-        backbone(img).backward(gfeat)
-
-    res = alternate({'fused': lambda: step('fused'), 'eager': lambda: step('eager'), 'backbone': backbone_only})
-    for k in ('fused', 'eager'):
+    res = alternate({'heads': lambda: step('heads'), 'full': lambda: step('full'), 'eager': lambda: step('eager'),
+                     'backbone eager': lambda: bb['eager'](img).backward(gfeat),
+                     'backbone fused': lambda: bb['full'](img).backward(gfeat)})
+    for k in ('backbone eager', 'backbone fused'):
+        print('(b) SegFormer-B5 forward + backward, B=%d %d^2, %-5s: %.1f ms, peak %.2f GB'
+              % (B, R, k.split()[1], *res[k]))
+    for k, what in (('heads', 'heads fused'), ('full', 'backbone + heads fused'), ('eager', 'eager')):
         ms, gb = res[k]
-        print('(b) encoder step, B=%d %d^2, %-5s: %.1f ms (backbone fwd + bwd %.1f ms = %.0f%%), peak %.2f GB'
-              % (B, R, k, ms, res['backbone'][0], 100 * res['backbone'][0] / ms, gb))
+        print('(b) encoder step, B=%d %d^2, %-22s: %.1f ms, peak %.2f GB' % (B, R, what, ms, gb))
 
     # (c) the whole iteration: the no-grad generator render with coords, then the encoder step
     from fixtures import synthetic
@@ -162,10 +167,11 @@ def main():
             x = out[0].clamp(-1, 1).permute(0, 3, 1, 2)
         step(name, x)
 
-    res = alternate({'fused': lambda: iteration('fused'), 'eager': lambda: iteration('eager')}, reps=2)
-    for k, (ms, gb) in res.items():
-        print('(c) train_coord_regressor iteration (render with coords + encoder step), B=%d %d^2, %-5s: '
-              '%.1f ms, peak %.2f GB' % (B, R, k, ms, gb))
+    res = alternate({k: (lambda k=k: iteration(k)) for k in ('heads', 'full', 'eager')}, reps=2)
+    for k, what in (('heads', 'heads fused'), ('full', 'backbone + heads fused'), ('eager', 'eager')):
+        ms, gb = res[k]
+        print('(c) train_coord_regressor iteration (render with coords + encoder step), B=%d %d^2, %-22s: '
+              '%.1f ms, peak %.2f GB' % (B, R, what, ms, gb))
 
 
 if __name__ == '__main__':
