@@ -422,3 +422,24 @@ def find_saved(out, what):
         raise NfiError('no saved %s forward behind this output (or its backward has already '
                        'released the workspace)' % what)
     return fn.state
+
+
+_FUSED_CLASSES = {}
+
+
+def switch_class(module, forward, enabled):
+    """Switches ``module`` to the class ``Fused<Base>``, its reference class ``Base`` with ``forward``
+    in place of ``Base.forward`` (``enabled=False`` switches it back to ``Base``); returns the module.
+    The class is made once per (``Base``, ``forward``); it keeps ``Base`` as ``_nfi_unfused_class``
+    and takes the ``__module__`` of ``forward``'s module."""
+    base = getattr(type(module), '_nfi_unfused_class', type(module))
+    if not enabled:
+        module.__class__ = base
+        return module
+    key = (base, forward)
+    if key not in _FUSED_CLASSES:
+        _FUSED_CLASSES[key] = type('Fused' + base.__name__, (base,),
+                                   {'forward': forward, '_nfi_unfused_class': base,
+                                    '__module__': forward.__module__})
+    module.__class__ = _FUSED_CLASSES[key]
+    return module

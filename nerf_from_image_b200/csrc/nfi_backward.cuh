@@ -37,12 +37,6 @@ __device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float 
                : "memory");
 }
 
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-  return v;
-}
-
 __host__ __device__ inline size_t bwd_smem_floats(int nout_pad, bool wgrad, bool viewdir = false) {
   const int nm = viewdir ? kViewMlpPad : nout_pad;
   size_t n = kC * kHid + kHid + kHid * nm + nm + 48;  // weights, palette

@@ -26,7 +26,7 @@
 // row of D2 and writes its row of dOut in its place) and D4 ([128 x 36] fp32).
 // Decoder-weight gradients (GAN generator step) are NOT produced here (nfi_wgrad_pipe.cuh).
 #pragma once
-#include "nfi_backward.cuh"  // red_add_v4, warp_sum
+#include "nfi_backward.cuh"  // red_add_v4
 #include "nfi_forward_pipe.cuh"
 
 namespace nfi {

@@ -30,7 +30,7 @@
 //     fir_down_adjoint_kernel  g_x += downsample2d^T(skip's data gradient)
 //   then fromrgb_backward_kernel / fromrgb_gimg_kernel: the 1x1 in fp32 (weight, bias, image gradients)
 // Each weight gradient sums its terms (one here, two in R1) in a scratch buffer and
-// wgrad_finish_kernel adds gain x it (transposed for conv1) to the caller's.
+// synth::wgrad_terms adds gain x it (transposed for conv1) to the caller's.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <math.h>
@@ -60,8 +60,6 @@ constexpr float kSqrt2 = 1.41421356237309505f;
 
 // [1,3,3,1] / 8 per axis: bilinear_filter() is its outer product, normalised to sum 1
 __device__ __forceinline__ float fir(int u) { return (u == 0 || u == 3) ? 0.125f : 0.375f; }
-__device__ __forceinline__ float lrelu(float x) { return x > 0.f ? x : kSlope * x; }
-__device__ __forceinline__ float dlrelu(float u) { return u > 0.f ? 1.f : kSlope; }
 __device__ __forceinline__ float pair_at(const __nv_bfloat16* hi, const __nv_bfloat16* lo, size_t i) {
   return __bfloat162float(hi[i]) + __bfloat162float(lo[i]);
 }
@@ -118,17 +116,6 @@ int n_blocks(int R) {
   return n;
 }
 
-// w [cout][cin][taps] * gain -> [taps][cout][cin] (transposed 0) or [taps][cin][cout] (1) pair
-__global__ void prep_kernel(const float* __restrict__ w, int cout, int cin, int taps, float gain, int transposed,
-                            __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo) {
-  const size_t n = (size_t)cout * cin;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const int o = (int)(i / cin), c = (int)(i % cin);
-    const size_t d = transposed ? (size_t)c * cout + o : i;
-    for (int t = 0; t < taps; ++t) split_bf16(w[i * taps + t] * gain, hi[t * n + d], lo[t * n + d]);
-  }
-}
-
 // the 4x4 conv's weights [512][513][9] * gain -> fp32 [513*9][512]
 __global__ void w4_kernel(const float* __restrict__ w, float gain, float* __restrict__ wt) {
   const size_t n = (size_t)kC4 * kCat * 9;
@@ -151,7 +138,7 @@ fromrgb_kernel(const float* __restrict__ img, int B, int nc, int RR, int C, cons
     const size_t b = q / RR;
     float s = 0.f;
     for (int ci = 0; ci < nc; ++ci) s += (__ldg(w + c * nc + ci) * g) * __ldg(img + (b * nc + ci) * RR + p);
-    split_bf16(lrelu((s + __ldg(bias + c)) * kSqrt2), hi[i], lo[i]);
+    split_bf16(lrelu((s + __ldg(bias + c)) * kSqrt2, kSlope), hi[i], lo[i]);
   }
 }
 
@@ -226,7 +213,7 @@ block_out_kernel(const float* __restrict__ raw1, const float* __restrict__ skip,
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     const float u = __ldg(raw1 + i) + __ldg(b1 + i % C);
     u_out[i] = u;
-    const float y = __ldg(skip + i) + lrelu(u);
+    const float y = __ldg(skip + i) + lrelu(u, kSlope);
     if (hi != nullptr) split_bf16(y, hi[i], lo[i]);
     if (y_out != nullptr) y_out[i] = y;
   }
@@ -283,7 +270,7 @@ b4_conv_kernel(const float* __restrict__ xs, const float* __restrict__ wt, const
     const float v = (acc[q] + __ldg(bias + co)) * kSqrt2;
     const size_t o = b * kFcIn + (size_t)co * 16 + p0 + q;
     u[o] = v;
-    a[o] = lrelu(v);
+    a[o] = lrelu(v, kSlope);
   }
 }
 
@@ -313,7 +300,7 @@ linear_kernel(const float* __restrict__ x, const float* __restrict__ W, float g,
     float v = part[threadIdx.x][0] + __ldg(bias + o);
     if (act) v *= kSqrt2;
     if (u != nullptr) u[(size_t)b * O + o] = v;
-    y[(size_t)b * O + o] = act ? lrelu(v) : v;
+    y[(size_t)b * O + o] = act ? lrelu(v, kSlope) : v;
   }
 }
 
@@ -351,7 +338,7 @@ __global__ void logits_backward_kernel(const float* __restrict__ g, const float*
 // g_u = g_y gain lrelu'(u); runs in place (gu == gy), so neither is __restrict__
 __global__ void act_backward_kernel(const float* gy, const float* __restrict__ u, size_t n, float gain, float* gu) {
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-    gu[i] = gy[i] * gain * dlrelu(u[i]);
+    gu[i] = gy[i] * gain * lrelu_grad(u[i], kSlope);
 }
 
 // g_x[b,k] = sum_o g_u[b,o] W[o,k] g
@@ -467,7 +454,7 @@ out_backward_kernel(const float* __restrict__ gy, const float* __restrict__ u1, 
     float s = 0.f;
     for (int r = r0; r < r1; ++r) {
       const size_t o = (size_t)r * C + c;
-      const float g = __ldg(gy + o), gu = g * dlrelu(__ldg(u1 + o));
+      const float g = __ldg(gy + o), gu = g * lrelu_grad(__ldg(u1 + o), kSlope);
       split_bf16(g, yhi[o], ylo[o]);
       split_bf16(gu, uhi[o], ulo[o]);
       s += gu;
@@ -597,24 +584,6 @@ fromrgb_gimg_kernel(const float* __restrict__ gx, const __nv_bfloat16* __restric
   }
 }
 
-__global__ void bias_reduce_kernel(const float* __restrict__ partial, int chunks, int C, float* __restrict__ g_b) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= C) return;
-  float s = 0.f;
-  for (int k = 0; k < chunks; ++k) s += partial[(size_t)k * C + c];
-  g_b[c] += s;
-}
-
-// g_w[co,ci,t] += gain tmp, with tmp [co][ci][taps] or (transposed) [ci][co][taps]
-__global__ void wgrad_finish_kernel(const float* __restrict__ tmp, int cout, int cin, int taps, float gain,
-                                    int transposed, float* __restrict__ g_w) {
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (size_t)cout * cin * taps) return;
-  const int t = (int)(i % taps), ci = (int)((i / taps) % cin), co = (int)(i / ((size_t)taps * cin));
-  const size_t s = transposed ? ((size_t)ci * cout + co) * taps + t : i;
-  g_w[i] += gain * tmp[s];
-}
-
 // a saved tensor as fp32: hi + lo of a pair, or a copy
 __global__ void __launch_bounds__(256)
 unpack_kernel(const __nv_bfloat16* __restrict__ hi, const __nv_bfloat16* __restrict__ lo,
@@ -635,8 +604,6 @@ static BlockShape shape(int R, int i) {
   s.Co = channels(s.h);
   return s;
 }
-
-static size_t chunks(size_t M) { return (M + kRows - 1) / kRows; }
 
 // The largest per-block sizes (floats or pair elements), which the buffers reused block by block take
 struct Sizes {
@@ -661,7 +628,8 @@ static Sizes sizes(const nfi_disc_params& P) {
     z.part = std::max({z.part, synth::wgrad3x3_partial_floats(P.batch, s.r, s.r, s.C, s.C),
                        synth::wgrad_down3x3_partial_floats(P.batch, s.h, s.C, s.Co),
                        synth::wgrad1x1_partial_floats(P.batch, s.h, s.Co, s.C)});
-    z.bp = std::max({z.bp, chunks(B * rr) * s.C * (i == 0 ? 1 + P.img_channels : 1), chunks(B * hh) * s.Co});
+    z.bp = std::max({z.bp, (size_t)blocks(B * rr, kRows) * s.C * (i == 0 ? 1 + P.img_channels : 1),
+                     (size_t)blocks(B * hh, kRows) * s.Co});
   }
   return z;
 }
@@ -806,42 +774,8 @@ static int setup(const nfi_disc_params& P, Layout& L, char* err, size_t err_len)
   return 0;
 }
 
-static int prep(const float* w, int cout, int cin, int taps, float gain, int transposed, Pair out,
-                cudaStream_t st, char* err, size_t err_len) {
-  prep_kernel<<<flat_grid((size_t)cout * cin), 256, 0, st>>>(w, cout, cin, taps, gain, transposed, out.hi,
-                                                               out.lo);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  return 0;
-}
-
 static float conv_gain(int cin, int k) { return 1.f / sqrtf((float)(cin * k * k)); }
 static const float kSkipGain = 0.70710678118654752f;  // sqrt2 / 2
-
-static int bias_reduce(int M, int C, float* part, float* g_b, cudaStream_t st, char* err, size_t err_len) {
-  if (g_b == nullptr) return 0;
-  bias_reduce_kernel<<<blocks(C, 256), 256, 0, st>>>(part, (int)chunks(M), C, g_b);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  return 0;
-}
-
-static int finish(const float* tmp, int cout, int cin, int taps, float gain, int transposed, float* g_w,
-                  cudaStream_t st, char* err, size_t err_len) {
-  wgrad_finish_kernel<<<blocks((size_t)cout * cin * taps, 256), 256, 0, st>>>(tmp, cout, cin, taps, gain,
-                                                                              transposed, g_w);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  return 0;
-}
-
-// g_w += gain (sum over terms k < n of wgrad(k)): the weight GEMMs into one buffer, then one finish
-template <class Wgrad>
-int wgrad_terms(float* g_w, size_t len, int n, Wgrad&& wgrad, int cout, int cin, int taps, float gain,
-                int transposed, float* wtmp, cudaStream_t st, char* err, size_t err_len) {
-  if (g_w == nullptr) return 0;
-  NFI_LAUNCH_CHECK(cudaMemsetAsync(wtmp, 0, len * sizeof(float), st));
-  for (int k = 0; k < n; ++k)
-    if (int rc = wgrad(k)) return rc;
-  return finish(wtmp, cout, cin, taps, gain, transposed, g_w, st, err, err_len);
-}
 
 Pair shifted(Pair p, size_t n) { return Pair{p.hi + n, p.lo + n}; }
 
@@ -905,41 +839,46 @@ static int reverse_walk(const nfi_disc_params& P, const Layout& L, const Reverse
     float* gx = gy == V.gA ? V.gB : V.gA;
     const bool below = i > 0 || grad_img || G.fromrgb_w || G.fromrgb_b;
     for (int c = 0; c < copies; ++c) {
-      out_backward_kernel<<<(unsigned)chunks(M), 256, 0, st>>>(gy + c * mo, L.u1[i], M, s.Co, V.gy.hi + c * mo,
-                                                               V.gy.lo + c * mo, V.gu.hi + c * mo, V.gu.lo + c * mo,
-                                                               V.bpart);
+      out_backward_kernel<<<blocks(M, kRows), 256, 0, st>>>(gy + c * mo, L.u1[i], M, s.Co, V.gy.hi + c * mo,
+                                                            V.gy.lo + c * mo, V.gu.hi + c * mo, V.gu.lo + c * mo,
+                                                            V.bpart);
       NFI_LAUNCH_CHECK(cudaGetLastError());
     }
-    if (int rc = bias_reduce(M, s.Co, V.bpart, G.conv1_b[i], st, err, err_len)) return rc;
-    if (int rc = wgrad_terms(G.conv1_w[i], (size_t)9 * s.C * s.Co, copies, [&](int k) {
-          return synth::wgrad_down3x3(B, s.h, s.C, s.Co, acts[k].ph[i], shifted(V.gu, (copies - 1 - k) * mo),
-                                      P.conv1_w[i], V.part, V.wtmp, st, err, err_len);
-        }, s.Co, s.C, 9, conv_gain(s.C, 3), 1, V.wtmp, st, err, err_len))
+    if (int rc = synth::bias_reduce(V.bpart, blocks(M, kRows), s.Co, G.conv1_b[i], st, err, err_len)) return rc;
+    if (int rc = synth::wgrad_terms(G.conv1_w[i], copies, [&](int k) {
+          return synth::wgrad_down3x3(B, s.h, s.C, s.Co, acts[k].ph[i], shifted(V.gu, (copies - 1 - k) * mo), V.part,
+                                      V.wtmp, st, err, err_len);
+        }, s.Co, s.C, 9, 9 * s.C, conv_gain(s.C, 3), synth::kCiCoTap, V.wtmp, st, err, err_len))
       return rc;
-    if (int rc = wgrad_terms(G.skip_w[i], (size_t)s.C * s.Co, copies, [&](int k) {
-          return synth::wgrad1x1(B, s.h, s.Co, s.C, shifted(V.gy, (copies - 1 - k) * mo), acts[k].d[i],
-                                 P.skip_w[i], V.part, V.wtmp, st, err, err_len);
-        }, s.Co, s.C, 1, conv_gain(s.C, 1) * kSkipGain, 0, V.wtmp, st, err, err_len))
+    if (int rc = synth::wgrad_terms(G.skip_w[i], copies, [&](int k) {
+          return synth::wgrad1x1(B, s.h, s.Co, s.C, shifted(V.gy, (copies - 1 - k) * mo), acts[k].d[i], V.part,
+                                 V.wtmp, st, err, err_len);
+        }, s.Co, s.C, 1, s.C, conv_gain(s.C, 1) * kSkipGain, synth::kCoCiTap, V.wtmp, st, err, err_len))
       return rc;
     if (below || G.conv0_w[i] || G.conv0_b[i]) {
-      if (int rc = prep(P.conv1_w[i], s.Co, s.C, 9, conv_gain(s.C, 3), 1, V.t1, st, err, err_len)) return rc;
+      if (int rc = synth::prep_weights(P.conv1_w[i], s.Co, s.C, 9, 9 * s.C, conv_gain(s.C, 3), synth::kTapCiCo, V.t1,
+                                       st, err, err_len))
+        return rc;
       if (int rc = synth::conv_up3x3(copies * B, s.h, s.Co, s.C, V.gu, V.t1, V.gf, st, err, err_len)) return rc;
       for (int c = 0; c < copies; ++c) {
-        fir_up_act_kernel<<<(unsigned)chunks(Mr), 256, 0, st>>>(V.gf + c * mf, L.a[i].hi, B, s.r, s.C,
-                                                                V.g0.hi + c * mr, V.g0.lo + c * mr, V.bpart);
+        fir_up_act_kernel<<<blocks(Mr, kRows), 256, 0, st>>>(V.gf + c * mf, L.a[i].hi, B, s.r, s.C,
+                                                             V.g0.hi + c * mr, V.g0.lo + c * mr, V.bpart);
         NFI_LAUNCH_CHECK(cudaGetLastError());
       }
-      if (int rc = bias_reduce(Mr, s.C, V.bpart, G.conv0_b[i], st, err, err_len)) return rc;
-      if (int rc = wgrad_terms(G.conv0_w[i], (size_t)9 * s.C * s.C, copies, [&](int k) {
+      if (int rc = synth::bias_reduce(V.bpart, blocks(Mr, kRows), s.C, G.conv0_b[i], st, err, err_len)) return rc;
+      if (int rc = synth::wgrad_terms(G.conv0_w[i], copies, [&](int k) {
             return synth::wgrad3x3(B, s.r, s.r, s.C, s.C, s.C, shifted(V.g0, (copies - 1 - k) * mr), acts[k].x[i],
-                                   P.conv0_w[i], V.part, V.wtmp, st, err, err_len);
-          }, s.C, s.C, 9, conv_gain(s.C, 3), 0, V.wtmp, st, err, err_len))
+                                   V.part, V.wtmp, st, err, err_len);
+          }, s.C, s.C, 9, 9 * s.C, conv_gain(s.C, 3), synth::kCoCiTap, V.wtmp, st, err, err_len))
         return rc;
     }
     if (!below) break;
-    if (int rc = prep(P.conv0_w[i], s.C, s.C, 9, conv_gain(s.C, 3), 1, V.t0, st, err, err_len)) return rc;
+    if (int rc = synth::prep_weights(P.conv0_w[i], s.C, s.C, 9, 9 * s.C, conv_gain(s.C, 3), synth::kTapCiCo, V.t0,
+                                     st, err, err_len))
+      return rc;
     if (int rc = synth::conv3x3_adjoint(copies * B, s.r, s.r, s.C, s.C, V.g0, V.t0, gx, st, err, err_len)) return rc;
-    if (int rc = prep(P.skip_w[i], s.Co, s.C, 1, conv_gain(s.C, 1) * kSkipGain, 1, V.ts, st, err, err_len))
+    if (int rc = synth::prep_weights(P.skip_w[i], s.Co, s.C, 1, s.C, conv_gain(s.C, 1) * kSkipGain, synth::kTapCiCo,
+                                     V.ts, st, err, err_len))
       return rc;
     if (int rc = synth::conv1x1(copies * B, s.h, s.Co, s.C, V.gy, V.ts, V.gd, st, err, err_len)) return rc;
     fir_down_adjoint_kernel<<<flat_grid(copies * mr), 256, 0, st>>>(V.gd, copies * B, s.r, s.C, gx);
@@ -947,7 +886,7 @@ static int reverse_walk(const nfi_disc_params& P, const Layout& L, const Reverse
     gy = gx;
   }
   // ---- fromrgb: gy is now the gradient of its output
-  const int C = channels(R), RR = R * R, n = (int)chunks((size_t)B * RR);
+  const int C = channels(R), RR = R * R, n = (int)blocks((size_t)B * RR, kRows);
   const float grgb = 1.f / sqrtf((float)nc);
   const size_t m0 = (size_t)B * RR * C;
   for (int k = 0; k < copies; ++k) {
@@ -993,9 +932,14 @@ int forward(const nfi_disc_params& P, cudaStream_t st, char* err, size_t err_len
   for (int i = 0; i < nb; ++i) {
     const BlockShape s = shape(R, i);
     const size_t hh = (size_t)B * s.h * s.h;
-    if (int rc = prep(P.conv0_w[i], s.C, s.C, 9, conv_gain(s.C, 3), 0, L.w0, st, err, err_len)) return rc;
-    if (int rc = prep(P.conv1_w[i], s.Co, s.C, 9, conv_gain(s.C, 3), 0, L.w1, st, err, err_len)) return rc;
-    if (int rc = prep(P.skip_w[i], s.Co, s.C, 1, conv_gain(s.C, 1) * kSkipGain, 0, L.ws, st, err, err_len))
+    if (int rc = synth::prep_weights(P.conv0_w[i], s.C, s.C, 9, 9 * s.C, conv_gain(s.C, 3), synth::kTapCoCi, L.w0,
+                                     st, err, err_len))
+      return rc;
+    if (int rc = synth::prep_weights(P.conv1_w[i], s.Co, s.C, 9, 9 * s.C, conv_gain(s.C, 3), synth::kTapCoCi, L.w1,
+                                     st, err, err_len))
+      return rc;
+    if (int rc = synth::prep_weights(P.skip_w[i], s.Co, s.C, 1, s.C, conv_gain(s.C, 1) * kSkipGain, synth::kTapCoCi,
+                                     L.ws, st, err, err_len))
       return rc;
     if (int rc = synth::conv3x3_act(B, s.r, s.r, s.C, s.C, L.x[i], L.w0, P.conv0_b[i], kSqrt2, kSlope, L.a[i], st,
                                     err, err_len))
@@ -1149,7 +1093,7 @@ block_out_tangent_kernel(const float* __restrict__ raw1, const float* __restrict
                          const float* __restrict__ u1, size_t n, __nv_bfloat16* __restrict__ hi,
                          __nv_bfloat16* __restrict__ lo, float* __restrict__ y_out) {
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const float y = __ldg(skip + i) + __ldg(raw1 + i) * dlrelu(__ldg(u1 + i));
+    const float y = __ldg(skip + i) + __ldg(raw1 + i) * lrelu_grad(__ldg(u1 + i), kSlope);
     if (hi != nullptr) split_bf16(y, hi[i], lo[i]);
     if (y_out != nullptr) y_out[i] = y;
   }
@@ -1287,9 +1231,14 @@ int backward_hvp(const nfi_disc_params& P, const nfi_disc_hvp& V, const nfi_disc
   for (int i = 0; i < nb; ++i) {
     const BlockShape s = shape(R, i);
     const size_t rr = (size_t)B * s.r * s.r, hh = (size_t)B * s.h * s.h;
-    if (int rc = prep(P.conv0_w[i], s.C, s.C, 9, conv_gain(s.C, 3), 0, H.w0, st, err, err_len)) return rc;
-    if (int rc = prep(P.conv1_w[i], s.Co, s.C, 9, conv_gain(s.C, 3), 0, H.w1, st, err, err_len)) return rc;
-    if (int rc = prep(P.skip_w[i], s.Co, s.C, 1, conv_gain(s.C, 1) * kSkipGain, 0, H.ws, st, err, err_len))
+    if (int rc = synth::prep_weights(P.conv0_w[i], s.C, s.C, 9, 9 * s.C, conv_gain(s.C, 3), synth::kTapCoCi, H.w0,
+                                     st, err, err_len))
+      return rc;
+    if (int rc = synth::prep_weights(P.conv1_w[i], s.Co, s.C, 9, 9 * s.C, conv_gain(s.C, 3), synth::kTapCoCi, H.w1,
+                                     st, err, err_len))
+      return rc;
+    if (int rc = synth::prep_weights(P.skip_w[i], s.Co, s.C, 1, s.C, conv_gain(s.C, 1) * kSkipGain, synth::kTapCoCi,
+                                     H.ws, st, err, err_len))
       return rc;
     if (int rc = synth::conv3x3(B, s.r, s.r, s.C, s.C, H.dx[i], H.w0, H.zero, H.raw0, Pair{nullptr, nullptr}, st,
                                 err, err_len))

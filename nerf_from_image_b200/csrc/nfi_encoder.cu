@@ -2,7 +2,7 @@
 // reference's models/encoder.py:70-103 from the backbone output(s) on.
 //
 // Forward, channel-last throughout (M = B 4h 4w image positions):
-//   transpose_kernel       features [B,C,h,w] -> fp32 [B,h,w,C]
+//   synth::transpose       features [B,C,h,w] -> fp32 [B,h,w,C]
 //   upsample_relu_kernel   relu(bilinear x4, align_corners=False, PyTorch's scale_factor index rule)
 //                          -> x0 pair [M,C], the A operand of the first conv; at scale 1 the same
 //                          kernel writes relu(features_latent) -> xl pair [B,h,w,C]
@@ -17,13 +17,13 @@
 //                          adjoint conv's input and the weight GEMM's G; between convs the RAW data
 //                          gradient times relu' (from the saved pair's sign) -> pair; the mean pool's
 //                          adjoint g_pooled / (h w) relu'(ul) -> pair.  Each writes per-chunk
-//                          partial sums of its gradient; bias_reduce_kernel adds them to the bias
+//                          partial sums of its gradient; synth::bias_reduce adds them to the bias
 //                          gradient in chunk order
 //   conv_tc_kernel RAW     the data gradients with the flipped tap table (nfi::synth::conv3x3_adjoint)
 //   wgrad_tc_kernel        the weight gradients (nfi::synth::wgrad3x3): G against the saved input
 //   upsample_adjoint_kernel each source texel gathers the destination pixels whose bilinear footprint
 //                          covers it (clamped borders included), times relu' of the upsample; at
-//                          scale 1 it is relu'(features_latent) times the gradient; transpose_kernel
+//                          scale 1 it is relu'(features_latent) times the gradient; synth::transpose
 //                          adds the result into g_features / g_features_latent ([B,C,h,w])
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -45,46 +45,6 @@ constexpr int kMaps = NFI_ENCODER_MAPS;
 constexpr int kMapsN = 32;    // post[4]'s Cout on conv_tc_kernel (its narrowest N)
 constexpr int kMapsG = 64;    // g_maps' channels as a pair (one 64-channel K block, 128-byte rows)
 constexpr int kRows = 256;    // positions per partial bias sum
-
-// PyTorch's upsample_bilinear2d source index for align_corners=False with a given scale factor
-// (area_pixel_compute_source_index with scale 1 / factor): the two taps and their weights
-__device__ __forceinline__ void src_index(int dst, float inv_s, int in, int& i0, int& i1, float& l0,
-                                          float& l1) {
-  float s = inv_s * ((float)dst + 0.5f) - 0.5f;
-  if (s < 0.f) s = 0.f;
-  i0 = (int)s;
-  i1 = i0 + (i0 < in - 1 ? 1 : 0);
-  l1 = s - (float)i0;
-  l0 = 1.f - l1;
-}
-// The weight with which destination index `dst` reads source index `src` (both taps may be `src`
-// at the clamped last row)
-__device__ __forceinline__ float src_weight(int dst, int src, float inv_s, int in) {
-  int i0, i1;
-  float l0, l1;
-  src_index(dst, inv_s, in, i0, i1, l0, l1);
-  return (i0 == src ? l0 : 0.f) + (i1 == src ? l1 : 0.f);
-}
-
-// src [B][R][Cc] -> dst [B][Cc][R] (dst += with `accumulate`): 32 x 32 tiles through shared memory
-__global__ void __launch_bounds__(256)
-transpose_kernel(const float* __restrict__ src, int R, int Cc, float* __restrict__ dst, int accumulate) {
-  __shared__ float t[32][33];
-  const int r0 = blockIdx.y * 32, c0 = blockIdx.x * 32;
-  const size_t b = blockIdx.z;
-  for (int k = threadIdx.y; k < 32; k += 8) {
-    const int r = r0 + k, c = c0 + threadIdx.x;
-    if (r < R && c < Cc) t[k][threadIdx.x] = __ldg(src + (b * R + r) * Cc + c);
-  }
-  __syncthreads();
-  for (int k = threadIdx.y; k < 32; k += 8) {
-    const int c = c0 + k, r = r0 + threadIdx.x;
-    if (r < R && c < Cc) {
-      const size_t o = (b * Cc + c) * R + r;
-      dst[o] = accumulate ? dst[o] + t[threadIdx.x][k] : t[threadIdx.x][k];
-    }
-  }
-}
 
 // relu(bilinear upsample by S) of f [B,h,w,C] -> pair [B,Sh,Sw,C]; one thread per 4 channels
 __global__ void __launch_bounds__(256)
@@ -219,14 +179,6 @@ act_backward_kernel(const ActBackward a) {
   }
 }
 
-__global__ void bias_reduce_kernel(const float* __restrict__ partial, int chunks, int C, float* __restrict__ g_b) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= C) return;
-  float s = 0.f;
-  for (int k = 0; k < chunks; ++k) s += partial[(size_t)k * C + c];
-  g_b[c] += s;
-}
-
 // a saved activation as fp32: hi + lo of a pair, or relu(u)
 __global__ void __launch_bounds__(256)
 unpack_kernel(const __nv_bfloat16* __restrict__ hi, const __nv_bfloat16* __restrict__ lo,
@@ -258,8 +210,6 @@ struct Layout {
   float* bpart;        // partial bias sums
 };
 
-static size_t chunks(size_t M) { return (M + kRows - 1) / kRows; }
-
 static void layout(const nfi_encoder_params& P, Bump& b, Layout& L) {
   memset(&L, 0, sizeof(L));
   const size_t B = P.batch, C = P.channels, hw = (size_t)P.height * P.width;
@@ -281,7 +231,7 @@ static void layout(const nfi_encoder_params& P, Bump& b, Layout& L) {
     const size_t pc = synth::wgrad3x3_partial_floats(P.batch, H, W, P.channels, P.channels);
     const size_t p4 = synth::wgrad3x3_partial_floats(P.batch, H, W, kMaps, P.channels);
     part = pc > p4 ? pc : p4;
-    bchunks = chunks(M);
+    bchunks = blocks(M, kRows);
   }
   if (P.latent_regressor) {
     L.wl = b.pair(wsz);
@@ -289,7 +239,7 @@ static void layout(const nfi_encoder_params& P, Bump& b, Layout& L) {
     L.ul = b.take(Ml * C);
     const size_t pl = synth::wgrad3x3_partial_floats(P.batch, P.height, P.width, P.channels, P.channels);
     part = part > pl ? part : pl;
-    bchunks = bchunks > chunks(Ml) ? bchunks : chunks(Ml);
+    bchunks = bchunks > blocks(Ml, kRows) ? bchunks : blocks(Ml, kRows);
   }
   if (P.save) {
     const size_t big = P.pose_regressor ? M : Ml;
@@ -335,22 +285,12 @@ static int check(const nfi_encoder_params& P, char* err, size_t err_len) {
   return 0;
 }
 
-// [B][R][Cc] -> [B][Cc][R]
-static void transpose(const float* src, int B, int R, int Cc, float* dst, bool accumulate, cudaStream_t st) {
-  transpose_kernel<<<dim3((unsigned)((Cc + 31) / 32), (unsigned)((R + 31) / 32), (unsigned)B), dim3(32, 8), 0,
-                     st>>>(src, R, Cc, dst, accumulate ? 1 : 0);
-}
-
 // the pair of a gradient with relu' applied, and its sum over positions into g_b (if set)
 static int act_backward(ActBackward a, float* g_b, cudaStream_t st, char* err, size_t err_len) {
-  const int n = (int)chunks((size_t)a.M);
+  const int n = (int)blocks((size_t)a.M, kRows);
   act_backward_kernel<<<n, 256, 0, st>>>(a);
   NFI_LAUNCH_CHECK(cudaGetLastError());
-  if (g_b != nullptr) {
-    bias_reduce_kernel<<<(a.C + 255) / 256, 256, 0, st>>>(a.partial, n, a.C, g_b);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
-  }
-  return 0;
+  return synth::bias_reduce(a.partial, n, a.C, g_b, st, err, err_len);
 }
 
 }  // namespace
@@ -402,10 +342,13 @@ int forward(const nfi_encoder_params& P, cudaStream_t st, char* err, size_t err_
     NFI_LAUNCH_CHECK(
         cudaMemcpyAsync(L.w4p, P.post4_w, (size_t)kMaps * C * 9 * sizeof(float), cudaMemcpyDeviceToDevice, st));
     NFI_LAUNCH_CHECK(cudaMemcpyAsync(L.b4p, P.post4_b, kMaps * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    if (int rc = synth::prep_weights3x3(P.post0_w, C, C, 0, L.w0.hi, L.w0.lo, st, err, err_len)) return rc;
-    if (int rc = synth::prep_weights3x3(P.post2_w, C, C, 0, L.w2.hi, L.w2.lo, st, err, err_len)) return rc;
-    if (int rc = synth::prep_weights3x3(L.w4p, kMapsN, C, 0, L.w4.hi, L.w4.lo, st, err, err_len)) return rc;
-    transpose(P.features, B, C, h * w, L.fcl, false, st);
+    if (int rc = synth::prep_weights(P.post0_w, C, C, 9, 9 * C, 1.f, synth::kTapCoCi, L.w0, st, err, err_len))
+      return rc;
+    if (int rc = synth::prep_weights(P.post2_w, C, C, 9, 9 * C, 1.f, synth::kTapCoCi, L.w2, st, err, err_len))
+      return rc;
+    if (int rc = synth::prep_weights(L.w4p, kMapsN, C, 9, 9 * C, 1.f, synth::kTapCoCi, L.w4, st, err, err_len))
+      return rc;
+    if (int rc = synth::transpose(P.features, B, C, h * w, nullptr, 0, L.fcl, st, err, err_len)) return rc;
     upsample_relu_kernel<<<flat_grid(M * C / 4), 256, 0, st>>>(L.fcl, B, h, w, C, kScale, L.x0.hi, L.x0.lo);
     NFI_LAUNCH_CHECK(cudaGetLastError());
     if (int rc = synth::conv3x3(B, H, W, C, C, L.x0, L.w0, P.post0_b, nullptr, L.a1, st, err, err_len)) return rc;
@@ -415,8 +358,8 @@ int forward(const nfi_encoder_params& P, cudaStream_t st, char* err, size_t err_
     NFI_LAUNCH_CHECK(cudaGetLastError());
   }
   if (P.latent_regressor) {
-    if (int rc = synth::prep_weights3x3(P.wpre_w, C, C, 0, L.wl.hi, L.wl.lo, st, err, err_len)) return rc;
-    transpose(P.features_latent, B, C, h * w, L.fcl, false, st);
+    if (int rc = synth::prep_weights(P.wpre_w, C, C, 9, 9 * C, 1.f, synth::kTapCoCi, L.wl, st, err, err_len)) return rc;
+    if (int rc = synth::transpose(P.features_latent, B, C, h * w, nullptr, 0, L.fcl, st, err, err_len)) return rc;
     upsample_relu_kernel<<<flat_grid(Ml * C / 4), 256, 0, st>>>(L.fcl, B, h, w, C, 1, L.xl.hi, L.xl.lo);
     NFI_LAUNCH_CHECK(cudaGetLastError());
     if (int rc = synth::conv3x3(B, h, w, C, C, L.xl, L.wl, P.wpre_b, L.ul, none, st, err, err_len)) return rc;
@@ -441,16 +384,19 @@ int backward(const nfi_encoder_params& P, const float* g_maps, const float* g_po
   const int B = P.batch, h = P.height, w = P.width, C = P.channels, H = kScale * h, W = kScale * w;
   const int M = B * H * W, Ml = B * h * w;
   if (P.pose_regressor) {
-    if (int rc = synth::prep_weights3x3(P.post0_w, C, C, 1, L.t0.hi, L.t0.lo, st, err, err_len)) return rc;
-    if (int rc = synth::prep_weights3x3(P.post2_w, C, C, 1, L.t2.hi, L.t2.lo, st, err, err_len)) return rc;
-    if (int rc = synth::prep_weights3x3(L.w4p, kMapsG, C, 1, L.t4.hi, L.t4.lo, st, err, err_len)) return rc;
+    if (int rc = synth::prep_weights(P.post0_w, C, C, 9, 9 * C, 1.f, synth::kTapCiCo, L.t0, st, err, err_len))
+      return rc;
+    if (int rc = synth::prep_weights(P.post2_w, C, C, 9, 9 * C, 1.f, synth::kTapCiCo, L.t2, st, err, err_len))
+      return rc;
+    if (int rc = synth::prep_weights(L.w4p, kMapsG, C, 9, 9 * C, 1.f, synth::kTapCiCo, L.t4, st, err, err_len))
+      return rc;
     ActBackward a;
     memset(&a, 0, sizeof(a));
     a.M = M; a.partial = L.bpart;
     // post[4]: g_maps as the zero-padded pair
     a.C = kMaps; a.out_C = kMapsG; a.g = g_maps; a.hi = L.g4.hi; a.lo = L.g4.lo;
     if (int rc = act_backward(a, G.g_post4_b, st, err, err_len)) return rc;
-    if (int rc = synth::wgrad3x3(B, H, W, kMaps, C, kMapsG, L.g4, L.a2, P.post4_w, L.part, G.g_post4_w, st, err,
+    if (int rc = synth::wgrad3x3(B, H, W, kMaps, C, kMapsG, L.g4, L.a2, L.part, G.g_post4_w, st, err,
                                  err_len))
       return rc;
     const bool below2 = G.g_post2_w || G.g_post2_b || G.g_post0_w || G.g_post0_b || G.g_features;
@@ -460,7 +406,7 @@ int backward(const nfi_encoder_params& P, const float* g_maps, const float* g_po
       // post[2]
       a.C = C; a.out_C = C; a.g = L.d; a.mask_hi = L.a2.hi; a.hi = L.g.hi; a.lo = L.g.lo;
       if (int rc = act_backward(a, G.g_post2_b, st, err, err_len)) return rc;
-      if (int rc = synth::wgrad3x3(B, H, W, C, C, C, L.g, L.a1, P.post2_w, L.part, G.g_post2_w, st, err, err_len))
+      if (int rc = synth::wgrad3x3(B, H, W, C, C, C, L.g, L.a1, L.part, G.g_post2_w, st, err, err_len))
         return rc;
     }
     if (below0) {
@@ -468,7 +414,7 @@ int backward(const nfi_encoder_params& P, const float* g_maps, const float* g_po
       // post[0]
       a.mask_hi = L.a1.hi;
       if (int rc = act_backward(a, G.g_post0_b, st, err, err_len)) return rc;
-      if (int rc = synth::wgrad3x3(B, H, W, C, C, C, L.g, L.x0, P.post0_w, L.part, G.g_post0_w, st, err, err_len))
+      if (int rc = synth::wgrad3x3(B, H, W, C, C, C, L.g, L.x0, L.part, G.g_post0_w, st, err, err_len))
         return rc;
     }
     if (G.g_features) {
@@ -476,26 +422,25 @@ int backward(const nfi_encoder_params& P, const float* g_maps, const float* g_po
       upsample_adjoint_kernel<<<flat_grid((size_t)Ml * C / 4), 256, 0, st>>>(L.d, L.x0.hi, B, h, w, C, kScale,
                                                                              L.fcl);
       NFI_LAUNCH_CHECK(cudaGetLastError());
-      transpose(L.fcl, B, h * w, C, G.g_features, true, st);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
+      if (int rc = synth::transpose(L.fcl, B, h * w, C, nullptr, 1, G.g_features, st, err, err_len)) return rc;
     }
   }
   if (P.latent_regressor) {
-    if (int rc = synth::prep_weights3x3(P.wpre_w, C, C, 1, L.tl.hi, L.tl.lo, st, err, err_len)) return rc;
+    if (int rc = synth::prep_weights(P.wpre_w, C, C, 9, 9 * C, 1.f, synth::kTapCiCo, L.tl, st, err, err_len)) return rc;
     ActBackward a;
     memset(&a, 0, sizeof(a));
     a.M = Ml; a.C = C; a.out_C = C; a.partial = L.bpart;
     a.g_img = g_pooled; a.per_img = h * w; a.g_scale = 1.f / (float)(h * w);
     a.mask_u = L.ul; a.hi = L.g.hi; a.lo = L.g.lo;
     if (int rc = act_backward(a, G.g_wpre_b, st, err, err_len)) return rc;
-    if (int rc = synth::wgrad3x3(B, h, w, C, C, C, L.g, L.xl, P.wpre_w, L.part, G.g_wpre_w, st, err, err_len))
+    if (int rc = synth::wgrad3x3(B, h, w, C, C, C, L.g, L.xl, L.part, G.g_wpre_w, st, err, err_len))
       return rc;
     if (G.g_features_latent) {
       if (int rc = synth::conv3x3_adjoint(B, h, w, C, C, L.g, L.tl, L.d, st, err, err_len)) return rc;
       upsample_adjoint_kernel<<<flat_grid((size_t)Ml * C / 4), 256, 0, st>>>(L.d, L.xl.hi, B, h, w, C, 1, L.fcl);
       NFI_LAUNCH_CHECK(cudaGetLastError());
-      transpose(L.fcl, B, h * w, C, G.g_features_latent, true, st);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
+      if (int rc = synth::transpose(L.fcl, B, h * w, C, nullptr, 1, G.g_features_latent, st, err, err_len))
+        return rc;
     }
   }
   return 0;

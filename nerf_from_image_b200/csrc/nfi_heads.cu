@@ -37,11 +37,6 @@ __device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float 
                "f"(c), "f"(d)
                : "memory");
 }
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-  return v;
-}
 
 struct Smem {
   float* W1t;  // [32][64]  W1t[c*64 + j] = W1[j][c]

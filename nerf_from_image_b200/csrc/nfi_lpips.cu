@@ -49,12 +49,6 @@ constexpr float kEps = 1e-10f;    // normalize_tensor
 
 inline bool pooled_after(int l) { return kTapOf[l] >= 0 && l < kConvs - 1; }
 
-__device__ __forceinline__ float warp_sum(float v) {  // butterfly: every lane holds the same bits
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 // ---------------------------------------------------------------- conv1_1 forward
 // One thread per (position, 8 output channels); the 8 threads of a position read the same 27 inputs.
 __global__ void __launch_bounds__(256)
@@ -455,8 +449,8 @@ int forward(const nfi_lpips_params& P, cudaStream_t st, char* err, size_t err_le
   if (const int rc = setup(P, L, err, err_len)) return rc;
   const int N = P.n, H = P.height, W = P.width, B2 = 2 * N;
   for (int l = 1; l < kConvs; ++l)
-    if (const int rc = synth::prep_weights3x3(P.conv_w[l], kCout[l], kCin[l], 0, L.wf[l].hi, L.wf[l].lo, st,
-                                              err, err_len))
+    if (const int rc = synth::prep_weights(P.conv_w[l], kCout[l], kCin[l], 9, 9 * kCin[l], 1.f, synth::kTapCoCi, L.wf[l],
+                                           st, err, err_len))
       return rc;
   conv11_forward_kernel<<<flat_grid((size_t)B2 * H * W * 8), 256, 0, st>>>(
       P.in0, P.in1, N, H, W, P.conv_w[0], P.conv_b[0], P.shift, P.scale, L.u[0], L.act[0].hi, L.act[0].lo);
@@ -507,8 +501,8 @@ int backward(const nfi_lpips_params& P, const float* g_dist, float* grad_in0, fl
   if (const int rc = setup(P, L, err, err_len)) return rc;
   const int N = P.n, H = P.height, W = P.width, B = grad_in1 ? 2 * N : N;
   for (int l = 1; l < kConvs; ++l)
-    if (const int rc = synth::prep_weights3x3(P.conv_w[l], kCout[l], kCin[l], 1, L.wt[l].hi, L.wt[l].lo, st,
-                                              err, err_len))
+    if (const int rc = synth::prep_weights(P.conv_w[l], kCout[l], kCin[l], 9, 9 * kCin[l], 1.f, synth::kTapCiCo, L.wt[l],
+                                           st, err, err_len))
       return rc;
   const float* gin = nullptr;  // gradient of layer l's relu(u), or of the pool output after it
   int cur = 0;

@@ -1,5 +1,6 @@
 // What the units on the synthesis network's bf16-pair conv kernels share (nfi_synth.cu, nfi_lpips.cu,
-// nfi_encoder.cu): the pair split, the workspace walk and the launch-grid helpers.
+// nfi_encoder.cu, nfi_disc.cu, nfi_segformer.cu): the pair split, the small device helpers, the
+// workspace walk and the launch-grid helpers.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -16,6 +17,28 @@ __device__ __forceinline__ void split_bf16(float t, __nv_bfloat16& hi, __nv_bflo
   lo = __float2bfloat16_rn(t - __bfloat162float(hi));
 }
 __device__ __forceinline__ float relu(float x) { return x > 0.f ? x : 0.f; }
+__device__ __forceinline__ float lrelu(float x, float slope) { return x > 0.f ? x : slope * x; }
+// lrelu' at the pre-activation u
+__device__ __forceinline__ float lrelu_grad(float u, float slope) { return u > 0.f ? 1.f : slope; }
+
+// PyTorch's upsample_bilinear2d source index for align_corners=False with a given scale factor
+// (area_pixel_compute_source_index with scale 1 / factor): the two taps and their weights
+__device__ __forceinline__ void src_index(int dst, float inv_s, int in, int& i0, int& i1, float& l0, float& l1) {
+  float s = inv_s * ((float)dst + 0.5f) - 0.5f;
+  if (s < 0.f) s = 0.f;
+  i0 = (int)s;
+  i1 = i0 + (i0 < in - 1 ? 1 : 0);
+  l1 = s - (float)i0;
+  l0 = 1.f - l1;
+}
+// The weight with which destination index `dst` reads source index `src` (both taps may be `src`
+// at the clamped last row)
+__device__ __forceinline__ float src_weight(int dst, int src, float inv_s, int in) {
+  int i0, i1;
+  float l0, l1;
+  src_index(dst, inv_s, in, i0, i1, l0, l1);
+  return (i0 == src ? l0 : 0.f) + (i1 == src ? l1 : 0.f);
+}
 
 // A tensor as two bf16 tensors of its shape, hi and lo of split_bf16
 struct Pair {

@@ -6,13 +6,13 @@
 // Forward, stage i at r = H / 2^(i+2) (M = B r^2 tokens, C = 64 / 128 / 320 / 512):
 //   pe1_kernel / phases_kernel + conv_down3x3   patch embed (7x7 s4 in fp32 / 3x3 s2 on the conv kernel)
 //   ln_kernel        s = x + scale (y + bias), LN(s) -> the next GEMM's pair (and the stream, stats)
-//   conv1x1          q, kv, proj, fc1, fc2 (RAW, weights by prep_kernel)
+//   conv1x1          q, kv, proj, fc1, fc2 (RAW, weights by synth::prep_weights)
 //   s2d_kernel       sr x sr space-to-depth of norm1's pair, then conv1x1 with K = sr^2 C, ln_kernel
 //   attn_kernel      softmax(q k^T / 8) v per (image, head, 32-query chunk), keys in shared memory
 //   dw_gelu_kernel   depthwise 3x3 of (fc1 + bias), + bias, exact GELU -> pair (pre-GELU kept)
 //   head             linear_c_i and linear_fuse's slice i at stage i's resolution (conv1x1),
 //                    upsample_sum_kernel (bilinear to r_0, summed, + fuse bias), linear_pred,
-//                    transpose_kernel -> features [B,out,r0,r0]
+//                    synth::transpose -> features [B,out,r0,r0]
 // Backward (every sum over positions in a fixed order; no atomics): the same walk reversed.
 //   act_kernel           a gradient times the drop-path scale -> pair, per-chunk column sums
 //   wgrad_tc_kernel      every GEMM's weight gradient (wgrad1x1, wgrad_down3x3)
@@ -53,10 +53,6 @@ constexpr int kLnRows = 8;     // rows per ln_backward_kernel chunk (one per war
 constexpr int kPe1 = 7, kPe1In = 3, kPe1W = kDims[0] * kPe1In * kPe1 * kPe1;  // 9408 weights
 constexpr float kEpsBlock = 1e-6f, kEpsEmbed = 1e-5f;  // block / stage norms; patch embed / attn.norm
 
-__device__ __forceinline__ float warp_sum(float v) {
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
 __device__ __forceinline__ float warp_max(float v) {
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
@@ -326,31 +322,6 @@ __global__ void __launch_bounds__(256) act_kernel(const Act a) {
       a.partial[(size_t)blockIdx.x * a.C + c] = t;
     }
   }
-}
-
-// A layer's weight w[co][ci][t] (row pitch ld) as the GEMM pair [cout][taps cin], K index t cin + ci
-// (transposed 0), or [taps cin][cout] (transposed 1)
-__global__ void prep_kernel(const float* __restrict__ w, int cout, int cin, int taps, int ld, int transposed,
-                            __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo) {
-  const int K = cin * taps;
-  const size_t n = (size_t)cout * K;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const int co = (int)(i / K), rr = (int)(i % K), ci = rr / taps, t = rr % taps;
-    const size_t k = (size_t)t * cin + ci;
-    const size_t d = transposed ? k * cout + co : (size_t)co * K + k;
-    split_bf16(__ldg(w + (size_t)co * ld + rr), hi[d], lo[d]);
-  }
-}
-
-// g_w[co][ci][t] (row pitch ld) += tmp[co][t cin + ci] (layout 0, the GEMM's) or tmp[ci][co][t] (1)
-__global__ void wgrad_finish_kernel(const float* __restrict__ tmp, int cout, int cin, int taps, int ld, int layout,
-                                    float* __restrict__ g_w) {
-  const int K = cin * taps;
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (size_t)cout * K) return;
-  const int co = (int)(i / K), rr = (int)(i % K), ci = rr / taps, t = rr % taps;
-  const size_t s = layout ? ((size_t)ci * cout + co) * taps + t : (size_t)co * K + (size_t)t * cin + ci;
-  g_w[(size_t)co * ld + rr] += tmp[s];
 }
 
 // norm1's pair [B,r,r,C] -> [B,r/sr,r/sr,sr^2 C] (rows beyond Mr of `rows` zero), column
@@ -626,23 +597,7 @@ dw_reduce_kernel(const float* __restrict__ partial, int chunks, int C, float* __
   if (t == 9 && g_b) g_b[c] += s;
 }
 
-// ---- decoder head.  PyTorch's upsample_bilinear2d source index (align_corners=False) at an
-// integer scale: the two taps and their weights
-__device__ __forceinline__ void src_index(int dst, float inv_s, int in, int& i0, int& i1, float& l0, float& l1) {
-  float s = inv_s * ((float)dst + 0.5f) - 0.5f;
-  if (s < 0.f) s = 0.f;
-  i0 = (int)s;
-  i1 = i0 + (i0 < in - 1 ? 1 : 0);
-  l1 = s - (float)i0;
-  l0 = 1.f - l1;
-}
-__device__ __forceinline__ float src_weight(int dst, int src, float inv_s, int in) {
-  int i0, i1;
-  float l0, l1;
-  src_index(dst, inv_s, in, i0, i1, l0, l1);
-  return (i0 == src ? l0 : 0.f) + (i1 == src ? l1 : 0.f);
-}
-
+// ---- decoder head
 struct Head4 {
   const float* d[kStages];  // linear_fuse's slice of stage i at r0 >> i, [B,r_i,r_i,768]
 };
@@ -704,26 +659,8 @@ upsample_adjoint_kernel(const float* __restrict__ g, int B, int h, int S, int ro
   }
 }
 
-// src [B][R][Cc] -> dst [B][Cc][R] (+ bias[c] where set): 32 x 32 tiles through shared memory
-__global__ void __launch_bounds__(256)
-transpose_kernel(const float* __restrict__ src, int R, int Cc, const float* __restrict__ bias, float* __restrict__ dst) {
-  __shared__ float t[32][33];
-  const int r0 = blockIdx.y * 32, c0 = blockIdx.x * 32;
-  const size_t b = blockIdx.z;
-  for (int k = threadIdx.y; k < 32; k += 8) {
-    const int r = r0 + k, c = c0 + threadIdx.x;
-    if (r < R && c < Cc) t[k][threadIdx.x] = __ldg(src + (b * R + r) * Cc + c) + (bias ? __ldg(bias + c) : 0.f);
-  }
-  __syncthreads();
-  for (int k = threadIdx.y; k < 32; k += 8) {
-    const int c = c0 + k, r = r0 + threadIdx.x;
-    if (r < R && c < Cc) dst[(b * Cc + c) * R + r] = t[threadIdx.x][k];
-  }
-}
-
 // ---------------------------------------------------------------- host side
 static size_t rnd(size_t m) { return (m + kRows - 1) / kRows * kRows; }
-static unsigned chunks(size_t m, int per) { return (unsigned)((m + per - 1) / per); }
 
 struct Shape {
   int r, N, C, heads, sr, rr, Nk, K;  // map side, tokens per image, width, heads, sr, reduced side, keys, sr^2 C
@@ -895,15 +832,15 @@ static void layout(const nfi_segformer_params& P, Bump& b, Layout& L) {
     if (s.sr > 1) partmax = mx(partmax, synth::wgrad1x1_partial_floats((int)(s.Mrp / kRows), 16, s.C, s.K));
     partmax = mx(partmax, synth::wgrad1x1_partial_floats(B16, 16, kDec, s.C));
     partmax = mx(partmax, synth::wgrad1x1_partial_floats(B16, 16, kDec, kDec));
-    bpmax = mx(bpmax, (size_t)chunks(s.Mp, kChunk) * mx(4 * C, kDec));
-    bpmax = mx(bpmax, (size_t)chunks(s.M, kLnRows) * 2 * C);
-    bpmax = mx(bpmax, (size_t)chunks(s.M, kChunk) * 10 * 4 * C);
-    apmax = mx(apmax, (size_t)B * s.heads * chunks(s.N, kQ) * 2 * s.Nk * kD);
+    bpmax = mx(bpmax, (size_t)blocks(s.Mp, kChunk) * mx(4 * C, kDec));
+    bpmax = mx(bpmax, (size_t)blocks(s.M, kLnRows) * 2 * C);
+    bpmax = mx(bpmax, (size_t)blocks(s.M, kChunk) * 10 * 4 * C);
+    apmax = mx(apmax, (size_t)B * s.heads * blocks(s.N, kQ) * 2 * s.Nk * kD);
   }
   const Shape& s0 = sh[0];
   partmax = mx(partmax, synth::wgrad1x1_partial_floats((int)(s0.Mp / kRows), 16, out, kDec));
-  bpmax = mx(bpmax, (size_t)chunks(s0.Mp, kChunk) * out);
-  bpmax = mx(bpmax, (size_t)chunks(s0.M, kRows) * kPe1W);
+  bpmax = mx(bpmax, (size_t)blocks(s0.Mp, kChunk) * out);
+  bpmax = mx(bpmax, (size_t)blocks(s0.M, kRows) * kPe1W);
   upmax = mx(upmax, s0.M * out);
 
   Blk shared_blk;
@@ -1036,46 +973,40 @@ static int gemm(size_t Mp, int K, int N, Pair in, Pair w, float* out, cudaStream
 // g_w [cout][cin] += g^T x over Mp rows
 static int wgrad(size_t Mp, int cout, int cin, Pair g, Pair x, float* part, float* g_w, cudaStream_t st, char* err,
                  size_t len) {
-  return synth::wgrad1x1((int)(Mp / kRows), 16, cout, cin, g, x, g_w, part, g_w, st, err, len);
+  return synth::wgrad1x1((int)(Mp / kRows), 16, cout, cin, g, x, part, g_w, st, err, len);
 }
-static int prep(const float* w, int cout, int cin, int taps, int ld, int transposed, Pair out, cudaStream_t st,
-                char* err, size_t err_len) {
-  prep_kernel<<<flat_grid((size_t)cout * cin * taps), 256, 0, st>>>(w, cout, cin, taps, ld, transposed, out.hi,
-                                                                    out.lo);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  return 0;
+// a linear layer's weight [cout][cin] (row pitch ld) as the pair [cout][cin] of its GEMM, or
+// [cin][cout] (transposed) of its data gradient's
+static int prep(const float* w, int cout, int cin, int ld, bool transposed, Pair out, cudaStream_t st, char* err,
+                size_t err_len) {
+  return synth::prep_weights(w, cout, cin, 1, ld, 1.f, transposed ? synth::kTapCiCo : synth::kTapCoCi, out, st, err,
+                             err_len);
 }
 static int ln(const LnFwd& a, cudaStream_t st, char* err, size_t err_len) {
-  ln_kernel<<<chunks((size_t)a.rows, 8), 256, 0, st>>>(a);
+  ln_kernel<<<blocks((size_t)a.rows, 8), 256, 0, st>>>(a);
   NFI_LAUNCH_CHECK(cudaGetLastError());
   return 0;
 }
 static int reduce(const float* partial, int n_chunks, int stride, int n, float* out, cudaStream_t st, char* err,
                   size_t err_len) {
   if (out == nullptr) return 0;
-  reduce_kernel<<<chunks((size_t)n, 32), 256, 0, st>>>(partial, n_chunks, stride, n, out);
+  reduce_kernel<<<blocks((size_t)n, 32), 256, 0, st>>>(partial, n_chunks, stride, n, out);
   NFI_LAUNCH_CHECK(cudaGetLastError());
   return 0;
 }
 // the LN backward and its affine gradients
 static int ln_backward(const LnBwd& a, float* g_w, float* g_b, cudaStream_t st, char* err, size_t err_len) {
-  const unsigned n = chunks((size_t)a.M, kLnRows);
+  const unsigned n = blocks((size_t)a.M, kLnRows);
   ln_backward_kernel<<<n, 256, 0, st>>>(a);
   NFI_LAUNCH_CHECK(cudaGetLastError());
   if (int rc = reduce(a.partial, (int)n, 2 * a.C, a.C, g_w, st, err, err_len)) return rc;
   return reduce(a.partial + a.C, (int)n, 2 * a.C, a.C, g_b, st, err, err_len);
 }
 static int act(const Act& a, float* g_b, cudaStream_t st, char* err, size_t err_len) {
-  const unsigned n = chunks((size_t)a.rows, kChunk);
+  const unsigned n = blocks((size_t)a.rows, kChunk);
   act_kernel<<<dim3(n, (unsigned)(a.C / 32)), 256, 0, st>>>(a);
   NFI_LAUNCH_CHECK(cudaGetLastError());
   return g_b ? reduce(a.partial, (int)n, a.C, a.C, g_b, st, err, err_len) : 0;
-}
-static int finish(const float* tmp, int cout, int cin, int taps, int ld, int lay, float* g_w, cudaStream_t st,
-                  char* err, size_t err_len) {
-  wgrad_finish_kernel<<<chunks((size_t)cout * cin * taps, 256), 256, 0, st>>>(tmp, cout, cin, taps, ld, lay, g_w);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  return 0;
 }
 
 }  // namespace
@@ -1099,7 +1030,8 @@ int forward(const nfi_segformer_params& P, cudaStream_t st, char* err, size_t er
       phases_kernel<<<flat_grid((size_t)4 * B * (s.r + 1) * (s.r + 1) * Cp), 256, 0, st>>>(L.s[i - 1].feat, B, s.r,
                                                                                           Cp, S.ph.hi, S.ph.lo);
       NFI_LAUNCH_CHECK(cudaGetLastError());
-      if (int rc = synth::prep_weights3x3(W[pe], C, Cp, 0, L.w.hi, L.w.lo, st, err, err_len)) return rc;
+      if (int rc = synth::prep_weights(W[pe], C, Cp, 9, 9 * Cp, 1.f, synth::kTapCoCi, L.w, st, err, err_len))
+        return rc;
       if (int rc = synth::conv_down3x3(B, s.r, Cp, C, S.ph, L.w, S.pe, st, err, err_len)) return rc;
     }
     NFI_LAUNCH_CHECK(cudaGetLastError());
@@ -1121,13 +1053,15 @@ int forward(const nfi_segformer_params& P, cudaStream_t st, char* err, size_t er
       const int nb = X.blk[i][k], o2 = nb + blk_off(s.sr);
       const float* sc_a = P.drop_scales ? P.drop_scales + (size_t)(2 * gk) * B : nullptr;
       const float* sc_m = P.drop_scales ? P.drop_scales + (size_t)(2 * gk + 1) * B : nullptr;
-      if (int rc = prep(W[nb + kQw], C, C, 1, C, 0, L.w, st, err, err_len)) return rc;
+      if (int rc = prep(W[nb + kQw], C, C, C, false, L.w, st, err, err_len)) return rc;
       if (int rc = gemm(s.Mp, C, C, K.a1, L.w, K.q, st, err, err_len)) return rc;
       Pair kvin = K.a1;
       if (s.sr > 1) {
         s2d_kernel<<<flat_grid(s.Mrp * s.K), 256, 0, st>>>(K.a1, B, s.r, s.sr, C, (int)s.Mrp, K.sd);
         NFI_LAUNCH_CHECK(cudaGetLastError());
-        if (int rc = prep(W[nb + kSrW], C, C, s.sr * s.sr, s.K, 0, L.w, st, err, err_len)) return rc;
+        if (int rc = synth::prep_weights(W[nb + kSrW], C, C, s.sr * s.sr, s.K, 1.f, synth::kCoTapCi, L.w, st, err,
+                                         err_len))
+          return rc;
         if (int rc = gemm(s.Mrp, s.K, C, K.sd, L.w, K.sr, st, err, err_len)) return rc;
         memset(&a, 0, sizeof(a));
         a.M = (int)s.Mr; a.rows = (int)s.Mrp; a.C = C; a.per_img = s.Nk;
@@ -1136,10 +1070,10 @@ int forward(const nfi_segformer_params& P, cudaStream_t st, char* err, size_t er
         if (int rc = ln(a, st, err, err_len)) return rc;
         kvin = K.xr;
       }
-      if (int rc = prep(W[nb + kKv], 2 * C, C, 1, C, 0, L.w, st, err, err_len)) return rc;
+      if (int rc = prep(W[nb + kKv], 2 * C, C, C, false, L.w, st, err, err_len)) return rc;
       if (int rc = gemm(s.Mkv, C, 2 * C, kvin, L.w, K.kv, st, err, err_len)) return rc;
       NFI_LAUNCH_CHECK(cudaFuncSetAttribute(attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem));
-      attn_kernel<<<dim3(chunks(s.N, kQ), s.heads, B), 256, kAttnSmem, st>>>(K.q, W[nb + kQw + 1], K.kv,
+      attn_kernel<<<dim3(blocks(s.N, kQ), s.heads, B), 256, kAttnSmem, st>>>(K.q, W[nb + kQw + 1], K.kv,
                                                                               W[nb + kKv + 1], s.N, s.Nk, C, K.o, K.op);
       NFI_LAUNCH_CHECK(cudaGetLastError());
       if (s.Mp > s.M) {
@@ -1147,19 +1081,19 @@ int forward(const nfi_segformer_params& P, cudaStream_t st, char* err, size_t er
         NFI_LAUNCH_CHECK(cudaMemsetAsync(K.op.hi + s.M * C, 0, pad, st));
         NFI_LAUNCH_CHECK(cudaMemsetAsync(K.op.lo + s.M * C, 0, pad, st));
       }
-      if (int rc = prep(W[nb + kProj], C, C, 1, C, 0, L.w, st, err, err_len)) return rc;
+      if (int rc = prep(W[nb + kProj], C, C, C, false, L.w, st, err, err_len)) return rc;
       if (int rc = gemm(s.Mp, C, C, K.op, L.w, L.y, st, err, err_len)) return rc;
       memset(&a, 0, sizeof(a));
       a.M = (int)s.M; a.rows = (int)s.Mp; a.C = C; a.per_img = s.N;
       a.x = K.x; a.y = L.y; a.bias = W[nb + kProj + 1]; a.scale = sc_a; a.s_out = K.x1;
       a.w = W[o2]; a.b = W[o2 + 1]; a.eps = kEpsBlock; a.pair = K.a2; a.stats = K.st2;
       if (int rc = ln(a, st, err, err_len)) return rc;
-      if (int rc = prep(W[o2 + 2], 4 * C, C, 1, C, 0, L.w, st, err, err_len)) return rc;
+      if (int rc = prep(W[o2 + 2], 4 * C, C, C, false, L.w, st, err, err_len)) return rc;
       if (int rc = gemm(s.Mp, C, 4 * C, K.a2, L.w, K.h, st, err, err_len)) return rc;
       dw_gelu_kernel<<<flat_grid(s.Mp * 4 * C), 256, 0, st>>>(K.h, W[o2 + 3], W[o2 + 4], W[o2 + 5], B, s.r, 4 * C,
                                                               (int)s.Mp, K.z, K.g);
       NFI_LAUNCH_CHECK(cudaGetLastError());
-      if (int rc = prep(W[o2 + 6], C, 4 * C, 1, 4 * C, 0, L.w, st, err, err_len)) return rc;
+      if (int rc = prep(W[o2 + 6], C, 4 * C, 4 * C, false, L.w, st, err, err_len)) return rc;
       if (int rc = gemm(s.Mp, 4 * C, C, K.g, L.w, L.y, st, err, err_len)) return rc;
       // the residual, then the next norm: the next block's norm1, or the stage norm
       const bool last = k + 1 == P.depths[i];
@@ -1181,13 +1115,13 @@ int forward(const nfi_segformer_params& P, cudaStream_t st, char* err, size_t er
   for (int i = 0; i < kStages; ++i) {
     const Shape s = shape(P, i);
     StageBufs& S = L.s[i];
-    if (int rc = prep(W[X.lc[i]], kDec, s.C, 1, s.C, 0, L.w, st, err, err_len)) return rc;
+    if (int rc = prep(W[X.lc[i]], kDec, s.C, s.C, false, L.w, st, err, err_len)) return rc;
     if (int rc = gemm(s.Mp, s.C, kDec, S.fp, L.w, L.y, st, err, err_len)) return rc;
     Act c;
     memset(&c, 0, sizeof(c));
     c.M = (int)s.M; c.rows = (int)s.Mp; c.C = kDec; c.per_img = s.N; c.g = L.y; c.bias = W[X.lc[i] + 1]; c.out = S.cp;
     if (int rc = act(c, nullptr, st, err, err_len)) return rc;
-    if (int rc = prep(W[X.fuse] + (kStages - 1 - i) * kDec, kDec, kDec, 1, kStages * kDec, 0, L.w, st, err, err_len))
+    if (int rc = prep(W[X.fuse] + (kStages - 1 - i) * kDec, kDec, kDec, kStages * kDec, false, L.w, st, err, err_len))
       return rc;
     if (int rc = gemm(s.Mp, kDec, kDec, S.cp, L.w, S.d, st, err, err_len)) return rc;
     hd.d[i] = S.d;
@@ -1195,12 +1129,9 @@ int forward(const nfi_segformer_params& P, cudaStream_t st, char* err, size_t er
   const Shape s0 = shape(P, 0);
   upsample_sum_kernel<<<flat_grid(s0.Mp * kDec), 256, 0, st>>>(hd, B, s0.r, W[X.fuse + 1], (int)s0.Mp, L.u);
   NFI_LAUNCH_CHECK(cudaGetLastError());
-  if (int rc = prep(W[X.pred], out, kDec, 1, kDec, 0, L.w, st, err, err_len)) return rc;
+  if (int rc = prep(W[X.pred], out, kDec, kDec, false, L.w, st, err, err_len)) return rc;
   if (int rc = gemm(s0.Mp, kDec, out, L.u, L.w, L.pred, st, err, err_len)) return rc;
-  transpose_kernel<<<dim3(chunks(out, 32), chunks(s0.N, 32), B), dim3(32, 8), 0, st>>>(L.pred, s0.N, out,
-                                                                                       W[X.pred + 1], P.features);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  return 0;
+  return synth::transpose(L.pred, B, s0.N, out, W[X.pred + 1], 0, P.features, st, err, err_len);
 }
 
 int backward(const nfi_segformer_params& P, const float* g_features, float* const* G, cudaStream_t st, char* err,
@@ -1220,15 +1151,13 @@ int backward(const nfi_segformer_params& P, const float* g_features, float* cons
   const int B = P.batch, H = P.height, out = P.out_features;
   const Shape s0 = shape(P, 0);
   // ---- head
-  transpose_kernel<<<dim3(chunks(s0.N, 32), chunks(out, 32), B), dim3(32, 8), 0, st>>>(g_features, out, s0.N,
-                                                                                       nullptr, L.gpe);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  if (int rc = synth::transpose(g_features, B, out, s0.N, nullptr, 0, L.gpe, st, err, err_len)) return rc;
   Act c;
   memset(&c, 0, sizeof(c));
   c.M = (int)s0.M; c.rows = (int)s0.Mp; c.C = out; c.per_img = s0.N; c.g = L.gpe; c.out = L.gy; c.partial = L.bpart;
   if (int rc = act(c, G[X.pred + 1], st, err, err_len)) return rc;
   if (int rc = wgrad(s0.Mp, out, kDec, L.gy, L.u, L.part, G[X.pred], st, err, err_len)) return rc;
-  if (int rc = prep(W[X.pred], out, kDec, 1, kDec, 1, L.w, st, err, err_len)) return rc;
+  if (int rc = prep(W[X.pred], out, kDec, kDec, true, L.w, st, err, err_len)) return rc;
   if (int rc = gemm(s0.Mp, out, kDec, L.gy, L.w, L.ga, st, err, err_len)) return rc;
   memset(&c, 0, sizeof(c));
   c.M = (int)s0.M; c.rows = (int)s0.Mp; c.C = kDec; c.per_img = s0.N; c.g = L.ga; c.partial = L.bpart;
@@ -1245,20 +1174,18 @@ int backward(const nfi_segformer_params& P, const float* g_features, float* cons
       NFI_LAUNCH_CHECK(cudaGetLastError());
     }
     const float* wf = W[X.fuse] + (kStages - 1 - i) * kDec;
-    if (G[X.fuse]) {
-      NFI_LAUNCH_CHECK(cudaMemsetAsync(L.wtmp, 0, (size_t)kDec * kDec * sizeof(float), st));
-      if (int rc = wgrad(s.Mp, kDec, kDec, L.gh, S.cp, L.part, L.wtmp, st, err, err_len)) return rc;
-      if (int rc = finish(L.wtmp, kDec, kDec, 1, kStages * kDec, 0, G[X.fuse] + (kStages - 1 - i) * kDec, st, err,
-                          err_len))
-        return rc;
-    }
-    if (int rc = prep(wf, kDec, kDec, 1, kStages * kDec, 1, L.w, st, err, err_len)) return rc;
+    float* gf = G[X.fuse] ? G[X.fuse] + (kStages - 1 - i) * kDec : nullptr;
+    if (int rc = synth::wgrad_terms(gf, 1, [&](int) {
+          return wgrad(s.Mp, kDec, kDec, L.gh, S.cp, L.part, L.wtmp, st, err, err_len);
+        }, kDec, kDec, 1, kStages * kDec, 1.f, synth::kCoCiTap, L.wtmp, st, err, err_len))
+      return rc;
+    if (int rc = prep(wf, kDec, kDec, kStages * kDec, true, L.w, st, err, err_len)) return rc;
     if (int rc = gemm(s.Mp, kDec, kDec, L.gh, L.w, L.gln, st, err, err_len)) return rc;
     memset(&c, 0, sizeof(c));
     c.M = (int)s.M; c.rows = (int)s.Mp; c.C = kDec; c.per_img = s.N; c.g = L.gln; c.out = L.gy; c.partial = L.bpart;
     if (int rc = act(c, G[X.lc[i] + 1], st, err, err_len)) return rc;
     if (int rc = wgrad(s.Mp, kDec, s.C, L.gy, S.fp, L.part, G[X.lc[i]], st, err, err_len)) return rc;
-    if (int rc = prep(W[X.lc[i]], kDec, s.C, 1, s.C, 1, L.w, st, err, err_len)) return rc;
+    if (int rc = prep(W[X.lc[i]], kDec, s.C, s.C, true, L.w, st, err, err_len)) return rc;
     if (int rc = gemm(s.Mp, kDec, s.C, L.gy, L.w, L.gfeat[i], st, err, err_len)) return rc;
   }
   // ---- stages, last to first
@@ -1285,21 +1212,21 @@ int backward(const nfi_segformer_params& P, const float* g_features, float* cons
       c.partial = L.bpart;
       if (int rc = act(c, G[o2 + 7], st, err, err_len)) return rc;
       if (int rc = wgrad(s.Mp, C, 4 * C, L.gy, K.g, L.part, G[o2 + 6], st, err, err_len)) return rc;
-      if (int rc = prep(W[o2 + 6], C, 4 * C, 1, 4 * C, 1, L.w, st, err, err_len)) return rc;
+      if (int rc = prep(W[o2 + 6], C, 4 * C, 4 * C, true, L.w, st, err, err_len)) return rc;
       if (int rc = gemm(s.Mp, C, 4 * C, L.gy, L.w, L.ga, st, err, err_len)) return rc;
-      const unsigned ndw = chunks(s.M, kChunk);
+      const unsigned ndw = blocks(s.M, kChunk);
       dw_backward_kernel<<<dim3(ndw, (unsigned)(4 * C / 32)), 256, 0, st>>>(L.ga, K.z, K.h, W[o2 + 3], B, s.r, 4 * C, L.bpart);
       NFI_LAUNCH_CHECK(cudaGetLastError());
       if (G[o2 + 4] || G[o2 + 5]) {
-        dw_reduce_kernel<<<chunks((size_t)40 * C, 32), 256, 0, st>>>(L.bpart, (int)ndw, 4 * C, G[o2 + 4], G[o2 + 5]);
+        dw_reduce_kernel<<<blocks((size_t)40 * C, 32), 256, 0, st>>>(L.bpart, (int)ndw, 4 * C, G[o2 + 4], G[o2 + 5]);
         NFI_LAUNCH_CHECK(cudaGetLastError());
       }
-      const unsigned nadj = chunks(s.Mp, kChunk);
+      const unsigned nadj = blocks(s.Mp, kChunk);
       dw_adjoint_kernel<<<dim3(nadj, (unsigned)(4 * C / 32)), 256, 0, st>>>(L.ga, W[o2 + 4], B, s.r, 4 * C, (int)s.Mp, L.gh, L.bpart);
       NFI_LAUNCH_CHECK(cudaGetLastError());
       if (int rc = reduce(L.bpart, (int)nadj, 4 * C, 4 * C, G[o2 + 3], st, err, err_len)) return rc;
       if (int rc = wgrad(s.Mp, 4 * C, C, L.gh, K.a2, L.part, G[o2 + 2], st, err, err_len)) return rc;
-      if (int rc = prep(W[o2 + 2], 4 * C, C, 1, C, 1, L.w, st, err, err_len)) return rc;
+      if (int rc = prep(W[o2 + 2], 4 * C, C, C, true, L.w, st, err, err_len)) return rc;
       if (int rc = gemm(s.Mp, 4 * C, C, L.gh, L.w, L.gln, st, err, err_len)) return rc;
       memset(&n, 0, sizeof(n));
       n.M = (int)s.M; n.C = C; n.s = K.x1; n.stats = K.st2; n.w = W[o2]; n.g = L.gln; n.g_res = L.gx; n.out = L.gx;
@@ -1311,9 +1238,9 @@ int backward(const nfi_segformer_params& P, const float* g_features, float* cons
       c.partial = L.bpart;
       if (int rc = act(c, G[nb + kProj + 1], st, err, err_len)) return rc;
       if (int rc = wgrad(s.Mp, C, C, L.gy, K.op, L.part, G[nb + kProj], st, err, err_len)) return rc;
-      if (int rc = prep(W[nb + kProj], C, C, 1, C, 1, L.w, st, err, err_len)) return rc;
+      if (int rc = prep(W[nb + kProj], C, C, C, true, L.w, st, err, err_len)) return rc;
       if (int rc = gemm(s.Mp, C, C, L.gy, L.w, L.gln, st, err, err_len)) return rc;
-      const unsigned nq = chunks(s.N, kQ);
+      const unsigned nq = blocks(s.N, kQ);
       NFI_LAUNCH_CHECK(
           cudaFuncSetAttribute(attn_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnBwdSmem));
       attn_backward_kernel<<<dim3(nq, s.heads, B), 256, kAttnBwdSmem, st>>>(
@@ -1331,9 +1258,9 @@ int backward(const nfi_segformer_params& P, const float* g_features, float* cons
       if (int rc = act(c, G[nb + kKv + 1], st, err, err_len)) return rc;
       const Pair kvin = s.sr > 1 ? K.xr : K.a1;
       if (int rc = wgrad(s.Mkv, 2 * C, C, L.gkvp, kvin, L.part, G[nb + kKv], st, err, err_len)) return rc;
-      if (int rc = prep(W[nb + kQw], C, C, 1, C, 1, L.w, st, err, err_len)) return rc;
+      if (int rc = prep(W[nb + kQw], C, C, C, true, L.w, st, err, err_len)) return rc;
       if (int rc = gemm(s.Mp, C, C, L.gy, L.w, L.gln, st, err, err_len)) return rc;
-      if (int rc = prep(W[nb + kKv], 2 * C, C, 1, C, 1, L.w, st, err, err_len)) return rc;
+      if (int rc = prep(W[nb + kKv], 2 * C, C, C, true, L.w, st, err, err_len)) return rc;
       if (int rc = gemm(s.Mkv, 2 * C, C, L.gkvp, L.w, L.gxr, st, err, err_len)) return rc;
       const float* g2 = L.gxr;
       if (s.sr > 1) {
@@ -1345,12 +1272,13 @@ int backward(const nfi_segformer_params& P, const float* g_features, float* cons
         c.M = (int)s.Mr; c.rows = (int)s.Mrp; c.C = C; c.per_img = s.Nk; c.g = L.gxr; c.out = L.gsr;
         c.partial = L.bpart;
         if (int rc = act(c, G[nb + kSrW + 1], st, err, err_len)) return rc;
-        if (G[nb + kSrW]) {
-          NFI_LAUNCH_CHECK(cudaMemsetAsync(L.wtmp, 0, (size_t)C * s.K * sizeof(float), st));
-          if (int rc = wgrad(s.Mrp, C, s.K, L.gsr, K.sd, L.part, L.wtmp, st, err, err_len)) return rc;
-          if (int rc = finish(L.wtmp, C, C, s.sr * s.sr, s.K, 0, G[nb + kSrW], st, err, err_len)) return rc;
-        }
-        if (int rc = prep(W[nb + kSrW], C, C, s.sr * s.sr, s.K, 1, L.w, st, err, err_len)) return rc;
+        if (int rc = synth::wgrad_terms(G[nb + kSrW], 1, [&](int) {
+              return wgrad(s.Mrp, C, s.K, L.gsr, K.sd, L.part, L.wtmp, st, err, err_len);
+            }, C, C, s.sr * s.sr, s.K, 1.f, synth::kCoTapCi, L.wtmp, st, err, err_len))
+          return rc;
+        if (int rc = synth::prep_weights(W[nb + kSrW], C, C, s.sr * s.sr, s.K, 1.f, synth::kTapCiCo, L.w, st, err,
+                                         err_len))
+          return rc;
         if (int rc = gemm(s.Mrp, C, s.K, L.gsr, L.w, L.gsd, st, err, err_len)) return rc;
         d2s_kernel<<<flat_grid(s.Mr * s.K), 256, 0, st>>>(L.gsd, B, s.r, s.sr, C, L.gext);
         NFI_LAUNCH_CHECK(cudaGetLastError());
@@ -1372,8 +1300,8 @@ int backward(const nfi_segformer_params& P, const float* g_features, float* cons
       c.M = c.rows = (int)s.M; c.C = C; c.per_img = s.N; c.g = L.gx; c.partial = L.bpart;
       if (int rc = act(c, G[pe + 1], st, err, err_len)) return rc;
       if (G[pe]) {
-        const unsigned np = chunks(s.M, kRows);
-        pe1_wgrad_kernel<<<dim3(chunks(kPe1W, 256), np), 256, 0, st>>>(L.gx, P.image, B, H, s.r, L.bpart);
+        const unsigned np = blocks(s.M, kRows);
+        pe1_wgrad_kernel<<<dim3(blocks(kPe1W, 256), np), 256, 0, st>>>(L.gx, P.image, B, H, s.r, L.bpart);
         NFI_LAUNCH_CHECK(cudaGetLastError());
         if (int rc = reduce(L.bpart, (int)np, kPe1W, kPe1W, G[pe], st, err, err_len)) return rc;
       }
@@ -1382,13 +1310,12 @@ int backward(const nfi_segformer_params& P, const float* g_features, float* cons
       memset(&c, 0, sizeof(c));
       c.M = c.rows = (int)s.M; c.C = C; c.per_img = s.N; c.g = L.gx; c.out = L.gy; c.partial = L.bpart;
       if (int rc = act(c, G[pe + 1], st, err, err_len)) return rc;
-      if (G[pe]) {
-        NFI_LAUNCH_CHECK(cudaMemsetAsync(L.wtmp, 0, (size_t)9 * C * Cp * sizeof(float), st));
-        if (int rc = synth::wgrad_down3x3(B, s.r, Cp, C, S.ph, L.gy, W[pe], L.part, L.wtmp, st, err, err_len))
-          return rc;
-        if (int rc = finish(L.wtmp, C, Cp, 9, 9 * Cp, 1, G[pe], st, err, err_len)) return rc;
-      }
-      if (int rc = synth::prep_weights3x3(W[pe], C, Cp, 1, L.w.hi, L.w.lo, st, err, err_len)) return rc;
+      if (int rc = synth::wgrad_terms(G[pe], 1, [&](int) {
+            return synth::wgrad_down3x3(B, s.r, Cp, C, S.ph, L.gy, L.part, L.wtmp, st, err, err_len);
+          }, C, Cp, 9, 9 * Cp, 1.f, synth::kCiCoTap, L.wtmp, st, err, err_len))
+        return rc;
+      if (int rc = synth::prep_weights(W[pe], C, Cp, 9, 9 * Cp, 1.f, synth::kTapCiCo, L.w, st, err, err_len))
+        return rc;
       if (int rc = synth::conv_up3x3(B, s.r, C, Cp, L.gy, L.w, L.gpe, st, err, err_len)) return rc;
       crop_add_kernel<<<flat_grid((size_t)B * 4 * s.r * s.r * Cp), 256, 0, st>>>(L.gpe, B, s.r, Cp, L.gfeat[i - 1]);
       NFI_LAUNCH_CHECK(cudaGetLastError());

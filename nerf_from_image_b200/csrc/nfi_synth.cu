@@ -161,8 +161,8 @@ __device__ __forceinline__ void store_split4(__nv_bfloat16* hi, __nv_bfloat16* l
   *reinterpret_cast<uint2*>(hi + idx) = *reinterpret_cast<const uint2*>(h);
   *reinterpret_cast<uint2*>(lo + idx) = *reinterpret_cast<const uint2*>(l);
 }
-__device__ __forceinline__ float lrelu(float x) { return x > 0.f ? x : 0.2f * x; }
-__device__ __forceinline__ float lrelu(float x, float slope) { return x > 0.f ? x : slope * x; }
+
+constexpr float kSlope = 0.2f;  // the leaky ReLU's negative slope
 
 // value -> (value * style) as a bf16 hi / lo pair, 2 channels (4 bytes per tensor) at a time
 __device__ __forceinline__ void store_split2(__nv_bfloat16* hi, __nv_bfloat16* lo, size_t idx,
@@ -525,8 +525,8 @@ fir_act_kernel(const float* __restrict__ raw, int B, int OH, int OW, int N, Epil
   }
 }
 
-// weight [Cout,Cin,K,K] -> [K*K][Cout][Cin] hi / lo (K-major rows of the B operand) and
-// wsq[Cout][Cin] = sum over taps of W^2 (for the demodulation coefficients)
+// The forward's weight prep: weight [Cout,Cin,K,K] -> [K*K][Cout][Cin] hi / lo (K-major rows of the
+// B operand) and wsq[Cout][Cin] = sum over taps of W^2 (for the demodulation coefficients)
 __global__ void prep_weights_kernel(const float* __restrict__ w, int cout, int cin, int taps,
                                     __nv_bfloat16* __restrict__ w_hi,
                                     __nv_bfloat16* __restrict__ w_lo, float* __restrict__ wsq) {
@@ -589,22 +589,9 @@ __global__ void const_input_kernel(const float* __restrict__ cst, const float* _
 
 // ------------------------------------------------------------------ backward to the latents
 // The data gradients dx~ = conv^T(dacc, W) run on conv_tc_kernel (RAW mode) with the weights
-// re-laid-out below; everything between two GEMMs of a layer is ONE full-resolution pass
-// (act_backward_kernel), plus the FIR adjoint for the up layers.
-
-// weight [Cout,Cin,K,K] -> [K*K][Cin][Cout] hi / lo: the B operand of the data-gradient GEMM
-// (reduction over Cout).  The stride-1 layer's tap flip lives in the tap table, not here.
-__global__ void prep_weights_t_kernel(const float* __restrict__ w, int cout, int cin, int taps,
-                                      __nv_bfloat16* __restrict__ w_hi,
-                                      __nv_bfloat16* __restrict__ w_lo) {
-  const size_t total = (size_t)cout * cin;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
-       i += (size_t)gridDim.x * blockDim.x) {
-    const size_t ci = i / cout, o = i - ci * cout;   // output index (ci, o): o fastest
-    for (int t = 0; t < taps; ++t)
-      split_bf16(w[(o * cin + ci) * taps + t], w_hi[(size_t)t * total + i], w_lo[(size_t)t * total + i]);
-  }
-}
+// re-laid-out by prep_weights (kTapCiCo: the B operand of a GEMM that reduces over Cout; the
+// stride-1 layer's tap flip lives in the tap table); everything between two GEMMs of a layer is
+// ONE full-resolution pass (act_backward_kernel), plus the FIR adjoint for the up layers.
 
 struct ActBackward {
   const float* u;       // [B,HW,C] saved pre-activation of the layer
@@ -624,8 +611,6 @@ struct ActBackward {
   float* g_bias;           // [C]
   float* g_noise;          // [B,HW] (with noise)
 };
-
-__device__ __forceinline__ float lrelu_grad(float u) { return u > 0.f ? 1.f : 0.2f; }
 
 constexpr int kActChunk = 1024;  // positions per block of act_backward_kernel
 
@@ -666,8 +651,10 @@ act_backward_kernel(ActBackward e, int HW, int C, int chunk) {
 #define NFI_CONSUMER(dx, s, acc)                                                    \
   if (dx != nullptr) {                                                              \
     const float4 x = __ldg(reinterpret_cast<const float4*>(dx + idx));              \
-    acc.x = fmaf(x.x, lrelu(u.x), acc.x); acc.y = fmaf(x.y, lrelu(u.y), acc.y);     \
-    acc.z = fmaf(x.z, lrelu(u.z), acc.z); acc.w = fmaf(x.w, lrelu(u.w), acc.w);     \
+    acc.x = fmaf(x.x, lrelu(u.x, kSlope), acc.x);                                   \
+    acc.y = fmaf(x.y, lrelu(u.y, kSlope), acc.y);                                   \
+    acc.z = fmaf(x.z, lrelu(u.z, kSlope), acc.z);                                   \
+    acc.w = fmaf(x.w, lrelu(u.w, kSlope), acc.w);                                   \
     dv.x = fmaf(x.x, s.x, dv.x); dv.y = fmaf(x.y, s.y, dv.y);                       \
     dv.z = fmaf(x.z, s.z, dv.z); dv.w = fmaf(x.w, s.w, dv.w);                       \
   }
@@ -676,7 +663,7 @@ act_backward_kernel(ActBackward e, int HW, int C, int chunk) {
 #undef NFI_CONSUMER
       float4 g, out;
 #define NFI_G(cmp)                                                                   \
-  g.cmp = dv.cmp * lrelu_grad(u.cmp) * e.gain;                                       \
+  g.cmp = dv.cmp * lrelu_grad(u.cmp, kSlope) * e.gain;                               \
   sd.cmp = fmaf(g.cmp, u.cmp * inv_gain - nz - bi.cmp, sd.cmp);  /* acc d = u/gain - noise - bias */ \
   out.cmp = g.cmp * d.cmp;
       NFI_G(x) NFI_G(y) NFI_G(z) NFI_G(w)
@@ -1048,7 +1035,8 @@ __global__ void restyle_kernel(const float* __restrict__ u, const float* __restr
     const int g = (int)(i % groups);
     const int img = (int)(i / ((size_t)HW * groups));
     float4 v = __ldg(reinterpret_cast<const float4*>(u) + i);
-    v.x = lrelu(v.x); v.y = lrelu(v.y); v.z = lrelu(v.z); v.w = lrelu(v.w);
+    v.x = lrelu(v.x, kSlope); v.y = lrelu(v.y, kSlope);
+    v.z = lrelu(v.z, kSlope); v.w = lrelu(v.w, kSlope);
     const float4 sv = __ldg(reinterpret_cast<const float4*>(s + (size_t)img * C) + g);
     store_split4(hi, lo, i * 4, v, sv);
   }
@@ -1158,10 +1146,10 @@ __global__ void restyle_tangent_kernel(const float* __restrict__ u, const float*
     const float4 sv = __ldg(reinterpret_cast<const float4*>(s + (size_t)img * C) + g);
     const float4 sd = __ldg(reinterpret_cast<const float4*>(sdot + (size_t)img * C) + g);
     float4 x;
-    x.x = lrelu_grad(v.x) * vd.x * sv.x + lrelu(v.x) * sd.x;
-    x.y = lrelu_grad(v.y) * vd.y * sv.y + lrelu(v.y) * sd.y;
-    x.z = lrelu_grad(v.z) * vd.z * sv.z + lrelu(v.z) * sd.z;
-    x.w = lrelu_grad(v.w) * vd.w * sv.w + lrelu(v.w) * sd.w;
+    x.x = lrelu_grad(v.x, kSlope) * vd.x * sv.x + lrelu(v.x, kSlope) * sd.x;
+    x.y = lrelu_grad(v.y, kSlope) * vd.y * sv.y + lrelu(v.y, kSlope) * sd.y;
+    x.z = lrelu_grad(v.z, kSlope) * vd.z * sv.z + lrelu(v.z, kSlope) * sd.z;
+    x.w = lrelu_grad(v.w, kSlope) * vd.w * sv.w + lrelu(v.w, kSlope) * sd.w;
     store_split4(hi, lo, i * 4, x, one);
   }
 }
@@ -1237,7 +1225,7 @@ act_backward_tangent_kernel(ActBackwardTangent e, int HW, int C, int chunk) {
       float out[4], outt[4], gsum = 0.f;
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
-        const float v = lrelu(u[k]), lg = lrelu_grad(u[k]), vd = lg * ud[k];
+        const float v = lrelu(u[k], kSlope), lg = lrelu_grad(u[k], kSlope), vd = lg * ud[k];
         sum[0][k] = fmaf(xa[k], v, sum[0][k]);
         sum[1][k] = fmaf(xb[k], v, sum[1][k]);
         sum[3][k] += xta[k] * v + xa[k] * vd;
@@ -1885,15 +1873,15 @@ static BackwardScratch backward_scratch(const nfi_synth_params& P, Bump& ws, int
 static int prep_backward(const nfi_synth_params& P, const float* g_planes, const BackwardScratch& s,
                          cudaStream_t st, char* err, size_t err_len) {
   const int B = P.batch, R = P.img_resolution, NI = P.img_channels;
+  auto prep_t = [&](const float* w, int cout, int cin, int taps, Pair out) {
+    return prep_weights(w, cout, cin, taps, cin * taps, 1.f, kTapCiCo, out, st, err, err_len);
+  };
   for (int i = 0; i < P.num_blocks; ++i) {
     const int c = P.channels[i], ci = i ? P.channels[i - 1] : 0;
-    if (i)
-      prep_weights_t_kernel<<<blocks((size_t)c * ci, 256), 256, 0, st>>>(P.conv0[i].weight, c, ci, 9,
-                                                                         s.wt0[i].hi, s.wt0[i].lo);
-    prep_weights_t_kernel<<<blocks((size_t)c * c, 256), 256, 0, st>>>(P.conv1[i].weight, c, c, 9,
-                                                                       s.wt1[i].hi, s.wt1[i].lo);
-    prep_weights_t_kernel<<<blocks((size_t)NI * c, 256), 256, 0, st>>>(P.torgb[i].weight, NI, c, 1,
-                                                                       s.wtr[i].hi, s.wtr[i].lo);
+    if (i > 0)
+      if (const int rc = prep_t(P.conv0[i].weight, c, ci, 9, s.wt0[i])) return rc;
+    if (const int rc = prep_t(P.conv1[i].weight, c, c, 9, s.wt1[i])) return rc;
+    if (const int rc = prep_t(P.torgb[i].weight, NI, c, 1, s.wtr[i])) return rc;
   }
   planes_grad_kernel<<<flat_grid((size_t)B * R * R * NI), 256, 0, st>>>(g_planes, B, R, s.dimg[0],
                                                                         s.dimg_p.hi, s.dimg_p.lo);
@@ -2493,6 +2481,134 @@ int backward_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const nfi_sy
 }
 
 // ---- the narrow entries of nfi_synth_launch.h ----
+// Where element (co, ci, t) of a [cout][cin][taps] weight sits in `order`
+__device__ __forceinline__ size_t order_index(int order, int co, int ci, int t, int cout, int cin, int taps) {
+  switch (order) {
+    case kTapCoCi: return ((size_t)t * cout + co) * cin + ci;
+    case kTapCiCo: return ((size_t)t * cin + ci) * cout + co;
+    case kCoTapCi: return ((size_t)co * taps + t) * cin + ci;
+    case kCiCoTap: return ((size_t)ci * cout + co) * taps + t;
+    default: return ((size_t)co * cin + ci) * taps + t;  // kCoCiTap
+  }
+}
+
+// One thread per (co, ci), in the order of a tap plane of `order`, so that each tap's stores are
+// contiguous; it reads the taps of its weight row in order.
+__global__ void prep_pair_kernel(const float* __restrict__ w, int cout, int cin, int taps, int ld, float gain,
+                                 int order, __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo) {
+  const size_t n = (size_t)cout * cin;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const bool ci_major = order == kTapCiCo;
+    const int co = (int)(ci_major ? i % cout : i / cin), ci = (int)(ci_major ? i / cout : i % cin);
+    for (int t = 0; t < taps; ++t) {
+      const size_t d = order_index(order, co, ci, t, cout, cin, taps);
+      split_bf16(__ldg(w + (size_t)co * ld + (size_t)ci * taps + t) * gain, hi[d], lo[d]);
+    }
+  }
+}
+
+__global__ void finish_wgrad_kernel(const float* __restrict__ tmp, int cout, int cin, int taps, int ld, float gain,
+                                    int order, float* __restrict__ g_w) {
+  const int K = cin * taps;
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t)cout * K) return;
+  const int co = (int)(i / K), rr = (int)(i % K), ci = rr / taps, t = rr % taps;
+  g_w[(size_t)co * ld + rr] += gain * tmp[order_index(order, co, ci, t, cout, cin, taps)];
+}
+
+// g_w[i taps + t] += sum_split part[split][t][i] (split order fixed), i < n: the narrow weight
+// gradients' K-split partials.  One thread per i.
+__global__ void wgrad_sum_kernel(const float* __restrict__ part, int n_split, int taps, size_t n,
+                                 float* __restrict__ g_w) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  for (int tp = 0; tp < taps; ++tp) {
+    float acc = 0.f;
+    for (int sp = 0; sp < n_split; ++sp) acc += part[((size_t)sp * taps + tp) * n + i];
+    g_w[i * taps + tp] += acc;
+  }
+}
+
+__global__ void bias_reduce_kernel(const float* __restrict__ partial, int n_chunks, int C, float* __restrict__ g_b) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  float s = 0.f;
+  for (int k = 0; k < n_chunks; ++k) s += partial[(size_t)k * C + c];
+  g_b[c] += s;
+}
+
+// 32 x 32 tiles through shared memory
+__global__ void __launch_bounds__(256)
+transpose_kernel(const float* __restrict__ src, int R, int Cc, const float* __restrict__ bias, int accumulate,
+                 float* __restrict__ dst) {
+  __shared__ float t[32][33];
+  const int r0 = blockIdx.y * 32, c0 = blockIdx.x * 32;
+  const size_t b = blockIdx.z;
+  for (int k = threadIdx.y; k < 32; k += 8) {
+    const int r = r0 + k, c = c0 + threadIdx.x;
+    if (r < R && c < Cc) {
+      const float v = __ldg(src + (b * R + r) * Cc + c);
+      t[k][threadIdx.x] = bias ? v + __ldg(bias + c) : v;
+    }
+  }
+  __syncthreads();
+  for (int k = threadIdx.y; k < 32; k += 8) {
+    const int c = c0 + k, r = r0 + threadIdx.x;
+    if (r < R && c < Cc) {
+      const size_t o = (b * Cc + c) * R + r;
+      dst[o] = accumulate ? dst[o] + t[threadIdx.x][k] : t[threadIdx.x][k];
+    }
+  }
+}
+
+int prep_weights(const float* w, int cout, int cin, int taps, int ld, float gain, int order, Pair out,
+                 cudaStream_t st, char* err, size_t err_len) {
+  if (order != kTapCoCi && order != kTapCiCo && order != kCoTapCi) {
+    snprintf(err, err_len, "prep_weights: no operand order %d", order);
+    return 1;
+  }
+  prep_pair_kernel<<<flat_grid((size_t)cout * cin), 256, 0, st>>>(w, cout, cin, taps, ld, gain, order, out.hi,
+                                                                   out.lo);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  return 0;
+}
+
+int finish_wgrad(const float* tmp, int cout, int cin, int taps, int ld, float gain, int order, float* g_w,
+                 cudaStream_t st, char* err, size_t err_len) {
+  if (order != kCoCiTap && order != kCiCoTap && order != kCoTapCi) {
+    snprintf(err, err_len, "finish_wgrad: no gradient order %d", order);
+    return 1;
+  }
+  finish_wgrad_kernel<<<blocks((size_t)cout * cin * taps, 256), 256, 0, st>>>(tmp, cout, cin, taps, ld, gain, order,
+                                                                              g_w);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  return 0;
+}
+
+int bias_reduce(const float* partial, int n_chunks, int C, float* g_b, cudaStream_t st, char* err,
+                size_t err_len) {
+  if (g_b == nullptr) return 0;
+  bias_reduce_kernel<<<blocks(C, 256), 256, 0, st>>>(partial, n_chunks, C, g_b);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  return 0;
+}
+
+int transpose(const float* src, int B, int R, int Cc, const float* bias, int accumulate, float* dst,
+              cudaStream_t st, char* err, size_t err_len) {
+  transpose_kernel<<<dim3(blocks(Cc, 32), blocks(R, 32), (unsigned)B), dim3(32, 8), 0, st>>>(src, R, Cc, bias,
+                                                                                            accumulate, dst);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  return 0;
+}
+
+// The fixed-order sum of a narrow weight gradient's partials into g_w
+static int wgrad_sum(const WgradArgs& a, float* g_w, cudaStream_t st, char* err, size_t err_len) {
+  const size_t n = (size_t)a.cout * a.cin;
+  wgrad_sum_kernel<<<blocks(n, 256), 256, 0, st>>>(a.part, a.n_split, a.taps, n, g_w);
+  NFI_LAUNCH_CHECK(cudaGetLastError());
+  return 0;
+}
+
 int conv3x3(int B, int H, int W, int C, int N, Pair in, Pair w, const float* bias, float* u_out, Pair out,
             cudaStream_t st, char* err, size_t err_len) {
   ConvArgs a = conv3x3_args(B, C, N, H, W, kModeAct);
@@ -2509,25 +2625,14 @@ int conv3x3_adjoint(int B, int H, int W, int C, int N, Pair in, Pair w, float* r
   return launch_conv(a, in, w, 9, st, err, err_len);
 }
 
-int prep_weights3x3(const float* w, int cout, int cin, int transposed, __nv_bfloat16* hi,
-                    __nv_bfloat16* lo, cudaStream_t st, char* err, size_t err_len) {
-  const unsigned grid = blocks((size_t)cout * cin, 256);
-  if (transposed)
-    prep_weights_t_kernel<<<grid, 256, 0, st>>>(w, cout, cin, 9, hi, lo);
-  else
-    prep_weights_kernel<<<grid, 256, 0, st>>>(w, cout, cin, 9, hi, lo, nullptr);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  return 0;
-}
-
 size_t wgrad3x3_partial_floats(int B, int H, int W, int cout, int cin) {
   WgradArgs a = conv3x3_wgrad(cout, cin);
   plan_wgrad(a, B, H, W);
   return (size_t)a.n_split * a.taps * cout * cin;
 }
 
-int wgrad3x3(int B, int H, int W, int cout, int cin, int g_channels, Pair g, Pair x, const float* w,
-             float* partials, float* g_w, cudaStream_t st, char* err, size_t err_len) {
+int wgrad3x3(int B, int H, int W, int cout, int cin, int g_channels, Pair g, Pair x, float* partials,
+             float* g_w, cudaStream_t st, char* err, size_t err_len) {
   if (g_w == nullptr) return 0;
   if (g_channels < cout || g_channels % 8 != 0 || cin % 8 != 0) {
     snprintf(err, err_len, "conv weight gradient: unsupported channel counts (G %d for Cout %d, Cin %d)",
@@ -2538,10 +2643,7 @@ int wgrad3x3(int B, int H, int W, int cout, int cin, int g_channels, Pair g, Pai
   plan_wgrad(a, B, H, W);
   a.part = partials;
   if (const int rc = launch_wgrad(a, g, B, H, W, x, B, H, W, st, err, err_len, g_channels)) return rc;
-  wgrad_reduce_kernel<<<blocks((size_t)a.cout * a.cin, 256), 256, 0, st>>>(
-      partials, a.n_split, a.taps, a.cout, a.cin, w, nullptr, nullptr, nullptr, B, g_w);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  return 0;
+  return wgrad_sum(a, g_w, st, err, err_len);
 }
 
 int conv3x3_act(int B, int H, int W, int C, int N, Pair in, Pair w, const float* bias, float gain, float slope,
@@ -2579,17 +2681,14 @@ size_t wgrad_down3x3_partial_floats(int B, int h, int cin, int cout) {
   return (size_t)a.n_split * a.taps * cout * cin;
 }
 
-int wgrad_down3x3(int B, int h, int cin, int cout, Pair phases, Pair g, const float* w, float* partials,
-                  float* g_wt, cudaStream_t st, char* err, size_t err_len) {
+int wgrad_down3x3(int B, int h, int cin, int cout, Pair phases, Pair g, float* partials, float* g_wt,
+                  cudaStream_t st, char* err, size_t err_len) {
   if (g_wt == nullptr) return 0;
   WgradArgs a = conv0_wgrad(cin, cout, B);
   plan_wgrad(a, B, h, h);
   a.part = partials;
   if (const int rc = launch_wgrad(a, phases, 4 * B, h + 1, h + 1, g, B, h, h, st, err, err_len)) return rc;
-  wgrad_reduce_kernel<<<blocks((size_t)a.cout * a.cin, 256), 256, 0, st>>>(
-      partials, a.n_split, a.taps, a.cout, a.cin, w, nullptr, nullptr, nullptr, B, g_wt);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  return 0;
+  return wgrad_sum(a, g_wt, st, err, err_len);
 }
 
 size_t wgrad1x1_partial_floats(int B, int H, int cout, int cin) {
@@ -2598,17 +2697,14 @@ size_t wgrad1x1_partial_floats(int B, int H, int cout, int cin) {
   return (size_t)a.n_split * a.taps * cout * cin;
 }
 
-int wgrad1x1(int B, int H, int cout, int cin, Pair g, Pair x, const float* w, float* partials, float* g_w,
-             cudaStream_t st, char* err, size_t err_len) {
+int wgrad1x1(int B, int H, int cout, int cin, Pair g, Pair x, float* partials, float* g_w, cudaStream_t st,
+             char* err, size_t err_len) {
   if (g_w == nullptr) return 0;
   WgradArgs a = torgb_wgrad(cout, cin);
   plan_wgrad(a, B, H, H);
   a.part = partials;
   if (const int rc = launch_wgrad(a, g, B, H, H, x, B, H, H, st, err, err_len)) return rc;
-  wgrad_reduce_kernel<<<blocks((size_t)a.cout * a.cin, 256), 256, 0, st>>>(
-      partials, a.n_split, a.taps, a.cout, a.cin, w, nullptr, nullptr, nullptr, B, g_w);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  return 0;
+  return wgrad_sum(a, g_w, st, err, err_len);
 }
 
 }  // namespace synth

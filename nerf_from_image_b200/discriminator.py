@@ -394,25 +394,12 @@ def _fused_forward(self, x, iteration, pose=None, image=None, focal=None):
     return logits(bb, x, cmap, r1=r1)
 
 
-_FUSED_CLASSES = {}
-
-
-def _fused_class(base):
-    if base not in _FUSED_CLASSES:
-        _FUSED_CLASSES[base] = type('Fused' + base.__name__, (base,),
-                                    {'forward': _fused_forward, '_nfi_unfused_class': base,
-                                     '__module__': __name__})
-    return _FUSED_CLASSES[base]
-
-
 def enable_fused_discriminator(discriminator, enabled=True, r1=False):
     """Switches a reference ``Discriminator`` instance to the fused backbone (``enabled=False``
     switches it back); returns the instance.  ``r1=True`` also runs R1-shaped calls on the kernels,
     their double backward on ``nfi_disc_backward_hvp``; the flag is an instance attribute, so
     ``nn.DataParallel``'s replicas (which copy the instance's ``__dict__``) keep it."""
-    m = discriminator
-    base = getattr(type(m), '_nfi_unfused_class', type(m))
-    m.__class__ = _fused_class(base) if enabled else base
+    m = _lib.switch_class(discriminator, _fused_forward, enabled)
     if enabled and r1:
         m._nfi_r1 = True
     else:

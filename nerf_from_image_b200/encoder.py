@@ -211,25 +211,9 @@ def _fused_forward(self, x):
     return coords, segmentation, w
 
 
-_FUSED_CLASSES = {}
-
-
-def _fused_class(base):
-    if base not in _FUSED_CLASSES:
-        _FUSED_CLASSES[base] = type('Fused' + base.__name__, (base,),
-                                    {'forward': _fused_forward, '_nfi_unfused_class': base,
-                                     '__module__': __name__})
-    return _FUSED_CLASSES[base]
-
-
 def enable_fused_encoder(bootstrap_encoder, enabled=True):
     """Switches a reference ``BootstrapEncoder`` instance to the fused heads (``enabled=False``
     switches it back).  Checks the heads' layout now; returns the instance."""
-    m = bootstrap_encoder
-    base = getattr(type(m), '_nfi_unfused_class', type(m))
     if enabled:
-        head_convs(m)
-        m.__class__ = _fused_class(base)
-    else:
-        m.__class__ = base
-    return m
+        head_convs(bootstrap_encoder)
+    return _lib.switch_class(bootstrap_encoder, _fused_forward, enabled)

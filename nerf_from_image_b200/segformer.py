@@ -239,24 +239,9 @@ def _fused_forward(self, x):
     return segformer(self, x)
 
 
-_FUSED_CLASSES = {}
-
-
-def _fused_class(base):
-    if base not in _FUSED_CLASSES:
-        _FUSED_CLASSES[base] = type('Fused' + base.__name__, (base,),
-                                    {'forward': _fused_forward, '_nfi_unfused_class': base,
-                                     '__module__': __name__})
-    return _FUSED_CLASSES[base]
-
-
 def enable_fused_segformer(module, enabled=True):
     """Switches a reference ``Segformer`` instance to the fused forward (``enabled=False`` switches it
     back).  Checks the layout now; returns the instance."""
-    base = getattr(type(module), '_nfi_unfused_class', type(module))
     if enabled:
         layout(module)
-        module.__class__ = _fused_class(base)
-    else:
-        module.__class__ = base
-    return module
+    return _lib.switch_class(module, _fused_forward, enabled)
