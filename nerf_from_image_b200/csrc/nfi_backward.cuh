@@ -643,13 +643,12 @@ render_backward_simt(const nfi_render_params p, const nfi_render_grads g) {
 namespace simt {
 
 template <int NP, bool WG, bool VD>
-int launch_bwd(const nfi_render_params& p, const nfi_render_grads& g, cudaStream_t st, char* err,
-               size_t err_len) {
+int launch_bwd(const nfi_render_params& p, const nfi_render_grads& g, cudaStream_t st) {
   const size_t smem = bwd_smem_floats(NP, WG, VD) * sizeof(float);
   auto k = render_backward_simt<NP, WG, VD>;
-  NFI_LAUNCH_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  NFI_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   k<<<(unsigned)num_tiles(p), kThreads, smem, st>>>(p, g);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 
@@ -658,19 +657,18 @@ int launch_bwd(const nfi_render_params& p, const nfi_render_grads& g, cudaStream
 // render_backward_simt, for arguments nfi_render_backward has checked.  nfi_render.cu instantiates
 // it for VD = false, nfi_viewdir.cu for VD = true.
 template <bool VD>
-int launch_backward_simt(const nfi_render_params& p, const nfi_render_grads& g, cudaStream_t st,
-                         char* err, size_t err_len) {
+int launch_backward_simt(const nfi_render_params& p, const nfi_render_grads& g, cudaStream_t st) {
   const bool wg = g.grad_w1 || g.grad_b1 || g.grad_w2 || g.grad_b2 || g.grad_w3 || g.grad_b3;
   switch (nout_pad_of(p.n_attention)) {
-    case 4: return wg ? simt::launch_bwd<4, true, VD>(p, g, st, err, err_len)
-                      : simt::launch_bwd<4, false, VD>(p, g, st, err, err_len);
-    case 12: return wg ? simt::launch_bwd<12, true, VD>(p, g, st, err, err_len)
-                       : simt::launch_bwd<12, false, VD>(p, g, st, err, err_len);
-    default: return wg ? simt::launch_bwd<16, true, VD>(p, g, st, err, err_len)
-                       : simt::launch_bwd<16, false, VD>(p, g, st, err, err_len);
+    case 4: return wg ? simt::launch_bwd<4, true, VD>(p, g, st)
+                      : simt::launch_bwd<4, false, VD>(p, g, st);
+    case 12: return wg ? simt::launch_bwd<12, true, VD>(p, g, st)
+                       : simt::launch_bwd<12, false, VD>(p, g, st);
+    default: return wg ? simt::launch_bwd<16, true, VD>(p, g, st)
+                       : simt::launch_bwd<16, false, VD>(p, g, st);
   }
 }
 extern template int launch_backward_simt<true>(const nfi_render_params&, const nfi_render_grads&,
-                                               cudaStream_t, char*, size_t);
+                                               cudaStream_t);
 
 }  // namespace nfi

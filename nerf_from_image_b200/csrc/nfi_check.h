@@ -1,10 +1,13 @@
-// The CUDA-check macro of every launcher in the library, and the warp sum of every unit.  On its own
-// so that the render units take them without the bf16-pair header (nfi_pair.cuh).
+// The error channel of every unit in the library, and the warp sum of every unit.  On its own so
+// that the render units take them without the bf16-pair header (nfi_pair.cuh).
 #pragma once
 #include <cuda_runtime.h>
-#include <stdio.h>
 
 namespace nfi {
+// Formats a refusal into the library's thread-local error text (nfi_last_error, defined beside it
+// in nfi_render.cu) and returns 1.
+int fail(const char* fmt, ...) __attribute__((format(printf, 1, 2)));
+
 // butterfly: every lane holds the same bits
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
@@ -13,13 +16,11 @@ __device__ __forceinline__ float warp_sum(float v) {
 }
 }  // namespace nfi
 
-// A CUDA runtime call in a launcher, which reports into (err, err_len): on failure the call and
-// the CUDA error go there and the launcher returns 2.
-#define NFI_LAUNCH_CHECK(expr)                                                       \
+// A CUDA runtime call: on failure the call and the CUDA error go to the error text and the caller
+// returns 2.
+#define NFI_CUDA(expr)                                                               \
   do {                                                                               \
     cudaError_t e__ = (expr);                                                        \
-    if (e__ != cudaSuccess) {                                                        \
-      snprintf(err, err_len, "%s failed: %s", #expr, cudaGetErrorString(e__));       \
-      return 2;                                                                      \
-    }                                                                                \
+    if (e__ != cudaSuccess)                                                          \
+      return nfi::fail("%s failed: %s", #expr, cudaGetErrorString(e__)), 2;          \
   } while (0)

@@ -34,13 +34,12 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <math.h>
-#include <stdio.h>
 #include <string.h>
 
 #include <algorithm>
 
 #include "nfi_disc.h"
-#include "nfi_disc_launch.h"
+#include "nfi_disc_r1.h"
 #include "nfi_pair.cuh"
 #include "nfi_synth_launch.h"
 
@@ -723,52 +722,41 @@ static void layout(const nfi_disc_params& P, Bump& b, Layout& L) {
   if (P.save) reverse_layout(P, z, 1, b, L.rev);
 }
 
-static int check(const nfi_disc_params& P, char* err, size_t err_len) {
+static int check(const nfi_disc_params& P) {
   const int R = P.resolution;
-  if (P.batch <= 0 || P.batch % kGroup != 0 || P.batch > 4096) {
-    snprintf(err, err_len, "discriminator: B must be a positive multiple of 4 up to 4096, got %d", P.batch);
-    return 1;
-  }
-  if (R < 8 || R > 256 || (R & (R - 1)) != 0) {
-    snprintf(err, err_len, "discriminator: resolution must be a power of two in 8..256, got %d", R);
-    return 1;
-  }
-  if (P.img_channels < 1 || P.img_channels > 4) {
-    snprintf(err, err_len, "discriminator: img_channels must be in 1..4, got %d", P.img_channels);
-    return 1;
-  }
-  if (P.cmap_dim != 0 && P.cmap_dim != kC4) {
-    snprintf(err, err_len, "discriminator: cmap_dim must be 0 or 512, got %d", P.cmap_dim);
-    return 1;
-  }
-  if (P.save != 0 && P.save != 1) {
-    snprintf(err, err_len, "discriminator: save must be 0 or 1, got %d", P.save);
-    return 1;
-  }
+  if (P.batch <= 0 || P.batch % kGroup != 0 || P.batch > 4096)
+    return fail("discriminator: B must be a positive multiple of 4 up to 4096, got %d", P.batch);
+  if (R < 8 || R > 256 || (R & (R - 1)) != 0)
+    return fail("discriminator: resolution must be a power of two in 8..256, got %d", R);
+  if (P.img_channels < 1 || P.img_channels > 4)
+    return fail("discriminator: img_channels must be in 1..4, got %d", P.img_channels);
+  if (P.cmap_dim != 0 && P.cmap_dim != kC4) return fail("discriminator: cmap_dim must be 0 or 512, got %d", P.cmap_dim);
+  if (P.save != 0 && P.save != 1) return fail("discriminator: save must be 0 or 1, got %d", P.save);
   return 0;
 }
 
-static int setup(const nfi_disc_params& P, Layout& L, char* err, size_t err_len) {
-  if (const int rc = check(P, err, err_len)) return rc;
+size_t workspace_bytes(const nfi_disc_params& P) {
+  if (check(P)) return 0;
+  Bump b{nullptr, 0, 0};
+  Layout L;
+  layout(P, b, L);
+  return b.off + 1024;
+}
+
+static int setup(const nfi_disc_params& P, Layout& L) {
+  if (const int rc = check(P)) return rc;
   const int nb = n_blocks(P.resolution);
   bool ok = P.img && P.fromrgb_w && P.fromrgb_b && P.b4_conv_w && P.b4_conv_b && P.fc_w && P.fc_b && P.out_w &&
             P.out_b && P.logits && (P.cmap_dim == 0 || P.cmap);
   for (int i = 0; i < nb; ++i)
     ok = ok && P.conv0_w[i] && P.conv0_b[i] && P.conv1_w[i] && P.conv1_b[i] && P.skip_w[i];
-  if (!ok) {
-    snprintf(err, err_len, "discriminator: img, every weight and bias of the %d blocks and the 4x4 "
-                           "epilogue, logits, and cmap (with cmap_dim 512) are needed", nb);
-    return 1;
-  }
-  if (!P.workspace) {
-    snprintf(err, err_len, "discriminator: workspace missing");
-    return 1;
-  }
+  if (!ok)
+    return fail("discriminator: img, every weight and bias of the %d blocks and the 4x4 "
+                "epilogue, logits, and cmap (with cmap_dim 512) are needed", nb);
+  if (!P.workspace) return fail("discriminator: workspace missing");
   const size_t need = workspace_bytes(P);
-  if (P.workspace_bytes < need) {
-    snprintf(err, err_len, "discriminator: workspace too small (%zu < %zu bytes)", P.workspace_bytes, need);
-    return 1;
-  }
+  if (P.workspace_bytes < need)
+    return fail("discriminator: workspace too small (%zu < %zu bytes)", P.workspace_bytes, need);
   Bump b = aligned_bump(P.workspace, P.workspace_bytes);
   layout(P, b, L);
   return 0;
@@ -785,34 +773,34 @@ Pair shifted(Pair p, size_t n) { return Pair{p.hi + n, p.lo + n}; }
 static int epilogue_backward(const nfi_disc_params& P, const Layout& L, const Reverse& V, const float* g_logits,
                              const float* hf, const float* a4, const float* xs, float* gw_out, float* gw_fc,
                              float* gw_b4, float* gb_out, float* gb_fc, float* gb_b4, float* grad_cmap,
-                             cudaStream_t st, char* err, size_t err_len) {
+                             cudaStream_t st) {
   const int B = P.batch, N = P.cmap_dim ? P.cmap_dim : 1;
   float *g_out = V.g4[0], *g_hf = V.g4[1], *g_a4 = V.g4[2], *g_xs = V.g4[3];
   logits_backward_kernel<<<blocks((size_t)B * N, 256), 256, 0, st>>>(g_logits, L.out, P.cmap, B, P.cmap_dim,
                                                                      g_out, grad_cmap);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   const float g_out_w = 1.f / sqrtf((float)kC4), g_fc_w = 1.f / sqrtf((float)kFcIn);
   linear_dw_kernel<<<blocks((size_t)N * kC4, 256), 256, 0, st>>>(g_out, hf, g_out_w, B, kC4, N, gw_out, gb_out);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   linear_dx_kernel<<<blocks((size_t)B * kC4, 256), 256, 0, st>>>(g_out, P.out_w, g_out_w, B, kC4, N, g_hf);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   act_backward_kernel<<<flat_grid((size_t)B * kC4), 256, 0, st>>>(g_hf, L.uf, (size_t)B * kC4, kSqrt2, g_hf);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   linear_dw_kernel<<<blocks((size_t)kC4 * kFcIn, 256), 256, 0, st>>>(g_hf, a4, g_fc_w, B, kFcIn, kC4, gw_fc, gb_fc);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   linear_dx_kernel<<<blocks((size_t)B * kFcIn, 256), 256, 0, st>>>(g_hf, P.fc_w, g_fc_w, B, kFcIn, kC4, g_a4);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   act_backward_kernel<<<flat_grid((size_t)B * kFcIn), 256, 0, st>>>(g_a4, L.u4, (size_t)B * kFcIn, kSqrt2, g_a4);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   const float g4w = conv_gain(kCat, 3);
   if (gw_b4 || gb_b4) {
     b4_conv_dw_kernel<<<blocks((size_t)kC4 * kCat * 9, 256), 256, 0, st>>>(g_a4, xs, g4w, B, gw_b4, gb_b4);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
+    NFI_CUDA(cudaGetLastError());
   }
   b4_conv_dx_kernel<<<dim3(blocks(kCat, 256), (unsigned)B), 256, 0, st>>>(g_a4, P.b4_conv_w, g4w, g_xs);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   mbstd_backward_kernel<<<blocks((size_t)B / kGroup * kFcIn, 256), 256, 0, st>>>(g_xs, L.x4, B, V.gA);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 
@@ -829,7 +817,7 @@ struct Acts {
 // and g (x) a-dot.  A bias pairs with a constant, so its gradient, like the image's, takes the last
 // copy alone.  Below block 0 only what is asked for runs.
 static int reverse_walk(const nfi_disc_params& P, const Layout& L, const Reverse& V, int copies, const Acts* acts,
-                        float* grad_img, const nfi_disc_grads& G, cudaStream_t st, char* err, size_t err_len) {
+                        float* grad_img, const nfi_disc_grads& G, cudaStream_t st) {
   const int B = P.batch, R = P.resolution, nc = P.img_channels, nb = n_blocks(R);
   float* gy = V.gA;  // the gradient of the current block's output
   for (int i = nb - 1; i >= 0; --i) {
@@ -842,47 +830,46 @@ static int reverse_walk(const nfi_disc_params& P, const Layout& L, const Reverse
       out_backward_kernel<<<blocks(M, kRows), 256, 0, st>>>(gy + c * mo, L.u1[i], M, s.Co, V.gy.hi + c * mo,
                                                             V.gy.lo + c * mo, V.gu.hi + c * mo, V.gu.lo + c * mo,
                                                             V.bpart);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
+      NFI_CUDA(cudaGetLastError());
     }
-    if (int rc = synth::bias_reduce(V.bpart, blocks(M, kRows), s.Co, G.conv1_b[i], st, err, err_len)) return rc;
+    if (int rc = synth::bias_reduce(V.bpart, blocks(M, kRows), s.Co, G.conv1_b[i], st)) return rc;
     if (int rc = synth::wgrad_terms(G.conv1_w[i], copies, [&](int k) {
           return synth::wgrad_down3x3(B, s.h, s.C, s.Co, acts[k].ph[i], shifted(V.gu, (copies - 1 - k) * mo), V.part,
-                                      V.wtmp, st, err, err_len);
-        }, s.Co, s.C, 9, 9 * s.C, conv_gain(s.C, 3), synth::kCiCoTap, V.wtmp, st, err, err_len))
+                                      V.wtmp, st);
+        }, s.Co, s.C, 9, 9 * s.C, conv_gain(s.C, 3), synth::kCiCoTap, V.wtmp, st))
       return rc;
     if (int rc = synth::wgrad_terms(G.skip_w[i], copies, [&](int k) {
           return synth::wgrad1x1(B, s.h, s.Co, s.C, shifted(V.gy, (copies - 1 - k) * mo), acts[k].d[i], V.part,
-                                 V.wtmp, st, err, err_len);
-        }, s.Co, s.C, 1, s.C, conv_gain(s.C, 1) * kSkipGain, synth::kCoCiTap, V.wtmp, st, err, err_len))
+                                 V.wtmp, st);
+        }, s.Co, s.C, 1, s.C, conv_gain(s.C, 1) * kSkipGain, synth::kCoCiTap, V.wtmp, st))
       return rc;
     if (below || G.conv0_w[i] || G.conv0_b[i]) {
-      if (int rc = synth::prep_weights(P.conv1_w[i], s.Co, s.C, 9, 9 * s.C, conv_gain(s.C, 3), synth::kTapCiCo, V.t1,
-                                       st, err, err_len))
+      if (int rc = synth::prep_weights(P.conv1_w[i], s.Co, s.C, 9, 9 * s.C, conv_gain(s.C, 3), synth::kTapCiCo,
+                                       V.t1, st))
         return rc;
-      if (int rc = synth::conv_up3x3(copies * B, s.h, s.Co, s.C, V.gu, V.t1, V.gf, st, err, err_len)) return rc;
+      if (int rc = synth::conv_up3x3(copies * B, s.h, s.Co, s.C, V.gu, V.t1, V.gf, st)) return rc;
       for (int c = 0; c < copies; ++c) {
         fir_up_act_kernel<<<blocks(Mr, kRows), 256, 0, st>>>(V.gf + c * mf, L.a[i].hi, B, s.r, s.C,
                                                              V.g0.hi + c * mr, V.g0.lo + c * mr, V.bpart);
-        NFI_LAUNCH_CHECK(cudaGetLastError());
+        NFI_CUDA(cudaGetLastError());
       }
-      if (int rc = synth::bias_reduce(V.bpart, blocks(Mr, kRows), s.C, G.conv0_b[i], st, err, err_len)) return rc;
+      if (int rc = synth::bias_reduce(V.bpart, blocks(Mr, kRows), s.C, G.conv0_b[i], st)) return rc;
       if (int rc = synth::wgrad_terms(G.conv0_w[i], copies, [&](int k) {
             return synth::wgrad3x3(B, s.r, s.r, s.C, s.C, s.C, shifted(V.g0, (copies - 1 - k) * mr), acts[k].x[i],
-                                   V.part, V.wtmp, st, err, err_len);
-          }, s.C, s.C, 9, 9 * s.C, conv_gain(s.C, 3), synth::kCoCiTap, V.wtmp, st, err, err_len))
+                                   V.part, V.wtmp, st);
+          }, s.C, s.C, 9, 9 * s.C, conv_gain(s.C, 3), synth::kCoCiTap, V.wtmp, st))
         return rc;
     }
     if (!below) break;
-    if (int rc = synth::prep_weights(P.conv0_w[i], s.C, s.C, 9, 9 * s.C, conv_gain(s.C, 3), synth::kTapCiCo, V.t0,
-                                     st, err, err_len))
+    if (int rc = synth::prep_weights(P.conv0_w[i], s.C, s.C, 9, 9 * s.C, conv_gain(s.C, 3), synth::kTapCiCo, V.t0, st))
       return rc;
-    if (int rc = synth::conv3x3_adjoint(copies * B, s.r, s.r, s.C, s.C, V.g0, V.t0, gx, st, err, err_len)) return rc;
+    if (int rc = synth::conv3x3_adjoint(copies * B, s.r, s.r, s.C, s.C, V.g0, V.t0, gx, st)) return rc;
     if (int rc = synth::prep_weights(P.skip_w[i], s.Co, s.C, 1, s.C, conv_gain(s.C, 1) * kSkipGain, synth::kTapCiCo,
-                                     V.ts, st, err, err_len))
+                                     V.ts, st))
       return rc;
-    if (int rc = synth::conv1x1(copies * B, s.h, s.Co, s.C, V.gy, V.ts, V.gd, st, err, err_len)) return rc;
+    if (int rc = synth::conv1x1(copies * B, s.h, s.Co, s.C, V.gy, V.ts, V.gd, st)) return rc;
     fir_down_adjoint_kernel<<<flat_grid(copies * mr), 256, 0, st>>>(V.gd, copies * B, s.r, s.C, gx);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
+    NFI_CUDA(cudaGetLastError());
     gy = gx;
   }
   // ---- fromrgb: gy is now the gradient of its output
@@ -894,118 +881,97 @@ static int reverse_walk(const nfi_disc_params& P, const Layout& L, const Reverse
     if (!G.fromrgb_w && !g_b) continue;
     fromrgb_backward_kernel<<<n, 256, 0, st>>>(gy + (copies - 1 - k) * m0, L.x[0].hi, acts[k].img, B, nc, RR, C,
                                                V.bpart);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
+    NFI_CUDA(cudaGetLastError());
     fromrgb_reduce_kernel<<<blocks((size_t)C * (1 + nc), 256), 256, 0, st>>>(V.bpart, n, C, nc, grgb, G.fromrgb_w,
                                                                              g_b);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
+    NFI_CUDA(cudaGetLastError());
   }
   if (grad_img) {
     fromrgb_gimg_kernel<<<flat_grid((size_t)B * RR * 32), 256, 0, st>>>(gy + (copies - 1) * m0, L.x[0].hi,
                                                                         P.fromrgb_w, grgb, B, nc, RR, C, grad_img);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
+    NFI_CUDA(cudaGetLastError());
   }
   return 0;
 }
 
 }  // namespace
 
-size_t workspace_bytes(const nfi_disc_params& P) {
-  char err[160];
-  if (check(P, err, sizeof(err))) return 0;
-  Bump b{nullptr, 0, 0};
+int forward(const nfi_disc_params& P, cudaStream_t st) {
   Layout L;
-  layout(P, b, L);
-  return b.off + 1024;
-}
-
-int forward(const nfi_disc_params& P, cudaStream_t st, char* err, size_t err_len) {
-  Layout L;
-  if (const int rc = setup(P, L, err, err_len)) return rc;
+  if (const int rc = setup(P, L)) return rc;
   const int B = P.batch, R = P.resolution, nc = P.img_channels, nb = n_blocks(R);
   const int N = P.cmap_dim ? P.cmap_dim : 1;
   {
     const int C = channels(R);
     fromrgb_kernel<<<flat_grid((size_t)B * R * R * C), 256, 0, st>>>(
         P.img, B, nc, R * R, C, P.fromrgb_w, 1.f / sqrtf((float)nc), P.fromrgb_b, L.x[0].hi, L.x[0].lo);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
+    NFI_CUDA(cudaGetLastError());
   }
   for (int i = 0; i < nb; ++i) {
     const BlockShape s = shape(R, i);
     const size_t hh = (size_t)B * s.h * s.h;
-    if (int rc = synth::prep_weights(P.conv0_w[i], s.C, s.C, 9, 9 * s.C, conv_gain(s.C, 3), synth::kTapCoCi, L.w0,
-                                     st, err, err_len))
+    if (int rc = synth::prep_weights(P.conv0_w[i], s.C, s.C, 9, 9 * s.C, conv_gain(s.C, 3), synth::kTapCoCi, L.w0, st))
       return rc;
-    if (int rc = synth::prep_weights(P.conv1_w[i], s.Co, s.C, 9, 9 * s.C, conv_gain(s.C, 3), synth::kTapCoCi, L.w1,
-                                     st, err, err_len))
+    if (int rc = synth::prep_weights(P.conv1_w[i], s.Co, s.C, 9, 9 * s.C, conv_gain(s.C, 3), synth::kTapCoCi, L.w1, st))
       return rc;
     if (int rc = synth::prep_weights(P.skip_w[i], s.Co, s.C, 1, s.C, conv_gain(s.C, 1) * kSkipGain, synth::kTapCoCi,
-                                     L.ws, st, err, err_len))
+                                     L.ws, st))
       return rc;
-    if (int rc = synth::conv3x3_act(B, s.r, s.r, s.C, s.C, L.x[i], L.w0, P.conv0_b[i], kSqrt2, kSlope, L.a[i], st,
-                                    err, err_len))
+    if (int rc = synth::conv3x3_act(B, s.r, s.r, s.C, s.C, L.x[i], L.w0, P.conv0_b[i], kSqrt2, kSlope, L.a[i], st))
       return rc;
     fir_phases_kernel<<<flat_grid((size_t)4 * B * (s.h + 1) * (s.h + 1) * s.C), 256, 0, st>>>(
         L.a[i].hi, L.a[i].lo, B, s.r, s.C, L.ph[i].hi, L.ph[i].lo);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
-    if (int rc = synth::conv_down3x3(B, s.h, s.C, s.Co, L.ph[i], L.w1, L.raw1, st, err, err_len)) return rc;
+    NFI_CUDA(cudaGetLastError());
+    if (int rc = synth::conv_down3x3(B, s.h, s.C, s.Co, L.ph[i], L.w1, L.raw1, st)) return rc;
     fir_down_kernel<<<flat_grid(hh * s.C), 256, 0, st>>>(L.x[i].hi, L.x[i].lo, B, s.r, s.C, L.d[i].hi, L.d[i].lo);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
-    if (int rc = synth::conv1x1(B, s.h, s.C, s.Co, L.d[i], L.ws, L.raws, st, err, err_len)) return rc;
+    NFI_CUDA(cudaGetLastError());
+    if (int rc = synth::conv1x1(B, s.h, s.C, s.Co, L.d[i], L.ws, L.raws, st)) return rc;
     const bool last = i == nb - 1;
     block_out_kernel<<<flat_grid(hh * s.Co), 256, 0, st>>>(L.raw1, L.raws, P.conv1_b[i], hh * s.Co, s.Co, L.u1[i],
                                                            last ? nullptr : L.x[i + 1].hi,
                                                            last ? nullptr : L.x[i + 1].lo, last ? L.x4 : nullptr);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
+    NFI_CUDA(cudaGetLastError());
   }
   mbstd_kernel<<<B / kGroup, 256, 0, st>>>(L.x4, B, L.xs, L.sd);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   w4_kernel<<<flat_grid((size_t)kC4 * kCat * 9), 256, 0, st>>>(P.b4_conv_w, conv_gain(kCat, 3), L.wt4);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   b4_conv_kernel<<<dim3((unsigned)B, kC4 / 64), 256, 0, st>>>(L.xs, L.wt4, P.b4_conv_b, L.u4, L.a4);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   const unsigned bgrid = blocks(B, kLinImg);
   linear_kernel<<<dim3(kC4, bgrid), 256, 0, st>>>(L.a4, P.fc_w, 1.f / sqrtf((float)kFcIn), P.fc_b, B, kFcIn, kC4,
                                                   1, L.uf, L.hf);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   linear_kernel<<<dim3((unsigned)N, bgrid), 256, 0, st>>>(L.hf, P.out_w, 1.f / sqrtf((float)kC4), P.out_b, B, kC4,
                                                           N, 0, nullptr, L.out);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   logits_kernel<<<blocks(B, 128), 128, 0, st>>>(L.out, P.cmap, B, P.cmap_dim, P.logits);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 
 int backward(const nfi_disc_params& P, const float* g_logits, float* grad_img, float* grad_cmap,
-             const nfi_disc_grads& G, cudaStream_t st, char* err, size_t err_len) {
-  if (!P.save) {
-    snprintf(err, err_len, "discriminator backward: needs the workspace of a forward with save = 1");
-    return 1;
-  }
-  if (!g_logits) {
-    snprintf(err, err_len, "discriminator backward: g_logits must be set");
-    return 1;
-  }
+             const nfi_disc_grads& G, cudaStream_t st) {
+  if (!P.save) return fail("discriminator backward: needs the workspace of a forward with save = 1");
+  if (!g_logits) return fail("discriminator backward: g_logits must be set");
   Layout L;
-  if (const int rc = setup(P, L, err, err_len)) return rc;
+  if (const int rc = setup(P, L)) return rc;
   if (int rc = epilogue_backward(P, L, L.rev, g_logits, L.hf, L.a4, L.xs, G.out_w, G.fc_w, G.b4_conv_w, G.out_b,
-                                 G.fc_b, G.b4_conv_b, grad_cmap, st, err, err_len))
+                                 G.fc_b, G.b4_conv_b, grad_cmap, st))
     return rc;
   const Acts saved = {L.x, L.ph, L.d, P.img};
-  return reverse_walk(P, L, L.rev, 1, &saved, grad_img, G, st, err, err_len);
+  return reverse_walk(P, L, L.rev, 1, &saved, grad_img, G, st);
 }
 
-int saved_preactivation(const nfi_disc_params& P, int block, int which, float* out, cudaStream_t st, char* err,
-                        size_t err_len) {
+int saved_preactivation(const nfi_disc_params& P, int block, int which, float* out, cudaStream_t st) {
   const int nb = n_blocks(P.resolution);
   const bool ok = P.save && out != nullptr && block >= 0 && block <= nb && which >= 0 &&
                   ((block < nb && which <= 2 && (which > 0 || block == 0)) || (block == nb && which <= 1));
-  if (!ok) {
-    snprintf(err, err_len, "discriminator saved_preactivation: needs a saved forward, out, and a block in "
-                           "0..%d with which in 1..2 (0..2 for block 0, 0..1 for the 4x4 epilogue)", nb);
-    return 1;
-  }
+  if (!ok)
+    return fail("discriminator saved_preactivation: needs a saved forward, out, and a block in "
+                "0..%d with which in 1..2 (0..2 for block 0, 0..1 for the 4x4 epilogue)", nb);
   Layout L;
-  if (const int rc = setup(P, L, err, err_len)) return rc;
+  if (const int rc = setup(P, L)) return rc;
   const size_t B = P.batch;
   size_t n;
   const __nv_bfloat16 *hi = nullptr, *lo = nullptr;
@@ -1026,7 +992,7 @@ int saved_preactivation(const nfi_disc_params& P, int block, int which, float* o
     }
   }
   unpack_kernel<<<flat_grid(n), 256, 0, st>>>(hi, lo, u, n, out);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 
@@ -1191,31 +1157,21 @@ void hvp_layout(const nfi_disc_params& P, Bump& b, HvpLayout& L) {
 }  // namespace
 
 size_t hvp_scratch_bytes(const nfi_disc_params& P) {
-  char err[160];
-  if (check(P, err, sizeof(err))) return 0;
+  if (check(P)) return 0;
   Bump b{nullptr, 0, 0};
   HvpLayout H;
   hvp_layout(P, b, H);
   return b.off + 1024;
 }
 
-int backward_hvp(const nfi_disc_params& P, const nfi_disc_hvp& V, const nfi_disc_grads& G, cudaStream_t st,
-                 char* err, size_t err_len) {
-  if (P.save != 1) {
-    snprintf(err, err_len, "discriminator HVP: needs the workspace of a forward with save = 1");
-    return 1;
-  }
-  if (!V.g_logits || !V.t_img || !V.scratch) {
-    snprintf(err, err_len, "discriminator HVP: g_logits, t_img and scratch must be set");
-    return 1;
-  }
+int backward_hvp(const nfi_disc_params& P, const nfi_disc_hvp& V, const nfi_disc_grads& G, cudaStream_t st) {
+  if (P.save != 1) return fail("discriminator HVP: needs the workspace of a forward with save = 1");
+  if (!V.g_logits || !V.t_img || !V.scratch) return fail("discriminator HVP: g_logits, t_img and scratch must be set");
   Layout L;
-  if (const int rc = setup(P, L, err, err_len)) return rc;
+  if (const int rc = setup(P, L)) return rc;
   const size_t need = hvp_scratch_bytes(P);
-  if (V.scratch_bytes < need) {
-    snprintf(err, err_len, "discriminator HVP: scratch too small (%zu < %zu bytes)", V.scratch_bytes, need);
-    return 1;
-  }
+  if (V.scratch_bytes < need)
+    return fail("discriminator HVP: scratch too small (%zu < %zu bytes)", V.scratch_bytes, need);
   HvpLayout H;
   Bump sb = aligned_bump(V.scratch, V.scratch_bytes);
   hvp_layout(P, sb, H);
@@ -1223,80 +1179,116 @@ int backward_hvp(const nfi_disc_params& P, const nfi_disc_hvp& V, const nfi_disc
   const int N = P.cmap_dim ? P.cmap_dim : 1;
   const int C = channels(R), RR = R * R;
   const float grgb = 1.f / sqrtf((float)nc);
-  NFI_LAUNCH_CHECK(cudaMemsetAsync(H.zero, 0, kC4 * sizeof(float), st));
+  NFI_CUDA(cudaMemsetAsync(H.zero, 0, kC4 * sizeof(float), st));
   // ---- the tangent forward along t, on the saved branches
   fromrgb_tangent_kernel<<<flat_grid((size_t)B * RR * C), 256, 0, st>>>(V.t_img, B, nc, RR, C, P.fromrgb_w, grgb,
                                                                        L.x[0].hi, H.dx[0].hi, H.dx[0].lo);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   for (int i = 0; i < nb; ++i) {
     const BlockShape s = shape(R, i);
     const size_t rr = (size_t)B * s.r * s.r, hh = (size_t)B * s.h * s.h;
-    if (int rc = synth::prep_weights(P.conv0_w[i], s.C, s.C, 9, 9 * s.C, conv_gain(s.C, 3), synth::kTapCoCi, H.w0,
-                                     st, err, err_len))
+    if (int rc = synth::prep_weights(P.conv0_w[i], s.C, s.C, 9, 9 * s.C, conv_gain(s.C, 3), synth::kTapCoCi, H.w0, st))
       return rc;
-    if (int rc = synth::prep_weights(P.conv1_w[i], s.Co, s.C, 9, 9 * s.C, conv_gain(s.C, 3), synth::kTapCoCi, H.w1,
-                                     st, err, err_len))
+    if (int rc = synth::prep_weights(P.conv1_w[i], s.Co, s.C, 9, 9 * s.C, conv_gain(s.C, 3), synth::kTapCoCi, H.w1, st))
       return rc;
     if (int rc = synth::prep_weights(P.skip_w[i], s.Co, s.C, 1, s.C, conv_gain(s.C, 1) * kSkipGain, synth::kTapCoCi,
-                                     H.ws, st, err, err_len))
+                                     H.ws, st))
       return rc;
-    if (int rc = synth::conv3x3(B, s.r, s.r, s.C, s.C, H.dx[i], H.w0, H.zero, H.raw0, Pair{nullptr, nullptr}, st,
-                                err, err_len))
+    if (int rc = synth::conv3x3(B, s.r, s.r, s.C, s.C, H.dx[i], H.w0, H.zero, H.raw0, Pair{nullptr, nullptr}, st))
       return rc;
     act_tangent_kernel<<<flat_grid(rr * s.C), 256, 0, st>>>(H.raw0, L.a[i].hi, rr * s.C, kSqrt2, H.da[i].hi,
                                                             H.da[i].lo);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
+    NFI_CUDA(cudaGetLastError());
     fir_phases_kernel<<<flat_grid((size_t)4 * B * (s.h + 1) * (s.h + 1) * s.C), 256, 0, st>>>(
         H.da[i].hi, H.da[i].lo, B, s.r, s.C, H.dph[i].hi, H.dph[i].lo);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
-    if (int rc = synth::conv_down3x3(B, s.h, s.C, s.Co, H.dph[i], H.w1, H.raw1, st, err, err_len)) return rc;
+    NFI_CUDA(cudaGetLastError());
+    if (int rc = synth::conv_down3x3(B, s.h, s.C, s.Co, H.dph[i], H.w1, H.raw1, st)) return rc;
     fir_down_kernel<<<flat_grid(hh * s.C), 256, 0, st>>>(H.dx[i].hi, H.dx[i].lo, B, s.r, s.C, H.dd[i].hi,
                                                          H.dd[i].lo);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
-    if (int rc = synth::conv1x1(B, s.h, s.C, s.Co, H.dd[i], H.ws, H.raws, st, err, err_len)) return rc;
+    NFI_CUDA(cudaGetLastError());
+    if (int rc = synth::conv1x1(B, s.h, s.C, s.Co, H.dd[i], H.ws, H.raws, st)) return rc;
     const bool last = i == nb - 1;
     block_out_tangent_kernel<<<flat_grid(hh * s.Co), 256, 0, st>>>(
         H.raw1, H.raws, L.u1[i], hh * s.Co, last ? nullptr : H.dx[i + 1].hi, last ? nullptr : H.dx[i + 1].lo,
         last ? H.dx4 : nullptr);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
+    NFI_CUDA(cudaGetLastError());
   }
   mbstd_tangent_kernel<<<B / kGroup, 256, 0, st>>>(L.x4, H.dx4, B, H.dxs);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   b4_conv_kernel<<<dim3((unsigned)B, kC4 / 64), 256, 0, st>>>(H.dxs, L.wt4, H.zero, H.du4, H.junk);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   act_backward_kernel<<<flat_grid((size_t)B * kFcIn), 256, 0, st>>>(H.du4, L.u4, (size_t)B * kFcIn, 1.f, H.da4);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   const unsigned bgrid = blocks(B, kLinImg);
   const float g_out_w = 1.f / sqrtf((float)kC4), g_fc_w = 1.f / sqrtf((float)kFcIn);
   linear_kernel<<<dim3(kC4, bgrid), 256, 0, st>>>(H.da4, P.fc_w, g_fc_w, H.zero, B, kFcIn, kC4, 0, nullptr, H.dhf);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   act_backward_kernel<<<flat_grid((size_t)B * kC4), 256, 0, st>>>(H.dhf, L.uf, (size_t)B * kC4, kSqrt2, H.dhf);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   linear_kernel<<<dim3((unsigned)N, bgrid), 256, 0, st>>>(H.dhf, P.out_w, g_out_w, H.zero, B, kC4, N, 0, nullptr,
                                                           H.dout);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   if (V.grad_g_logits) {
     logits_kernel<<<blocks(B, 128), 128, 0, st>>>(H.dout, P.cmap, B, P.cmap_dim, H.jt);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
+    NFI_CUDA(cudaGetLastError());
     accumulate_kernel<<<blocks(B, 128), 128, 0, st>>>(H.jt, B, V.grad_g_logits);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
+    NFI_CUDA(cudaGetLastError());
   }
   if (V.grad_cmap && P.cmap_dim) {  // g_logits out-dot / sqrt N (g_out's write here is discarded)
     logits_backward_kernel<<<blocks((size_t)B * N, 256), 256, 0, st>>>(V.g_logits, H.dout, P.cmap, B, P.cmap_dim,
                                                                        H.junk, V.grad_cmap);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
+    NFI_CUDA(cudaGetLastError());
   }
   // ---- the reverse walk: the epilogue's g as in the first-order backward (its g-dot is zero, property
   // 2), the minibatch std's g-dot after it, then the blocks over the stacked [g; g-dot]
   if (int rc = epilogue_backward(P, L, H.rev, V.g_logits, H.dhf, H.da4, H.dxs, G.out_w, G.fc_w, G.b4_conv_w,
-                                 nullptr, nullptr, nullptr, nullptr, st, err, err_len))
+                                 nullptr, nullptr, nullptr, nullptr, st))
     return rc;
   mbstd_hvp_kernel<<<blocks((size_t)B / kGroup * kFcIn, 256), 256, 0, st>>>(H.rev.g4[3], L.x4, H.dx4, B,
                                                                             H.rev.gA + (size_t)B * kFcIn);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   const Acts acts[2] = {{L.x, L.ph, L.d, P.img}, {H.dx, H.dph, H.dd, V.t_img}};
-  return reverse_walk(P, L, H.rev, 2, acts, V.grad_img, G, st, err, err_len);
+  return reverse_walk(P, L, H.rev, 2, acts, V.grad_img, G, st);
 }
 
 }  // namespace disc
 }  // namespace nfi
+
+using nfi::fail;
+
+extern "C" {
+
+size_t nfi_disc_workspace_bytes(const nfi_disc_params* params) {
+  if (params == nullptr) return 0;
+  return nfi::disc::workspace_bytes(*params);
+}
+
+int nfi_disc_forward(const nfi_disc_params* params, void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  return nfi::disc::forward(*params, (cudaStream_t)stream);
+}
+
+int nfi_disc_backward(const nfi_disc_params* params, const float* g_logits, float* grad_img, float* grad_cmap,
+                      const nfi_disc_grads* grads, void* stream) {
+  if (params == nullptr || grads == nullptr) return fail("params / grads is NULL");
+  return nfi::disc::backward(*params, g_logits, grad_img, grad_cmap, *grads, (cudaStream_t)stream);
+}
+
+int nfi_disc_saved_preactivation(const nfi_disc_params* params, int32_t block, int32_t which, float* out,
+                                 void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  return nfi::disc::saved_preactivation(*params, block, which, out, (cudaStream_t)stream);
+}
+
+size_t nfi_disc_r1_scratch_bytes(const nfi_disc_params* params) {
+  if (params == nullptr) return 0;
+  return nfi::disc::hvp_scratch_bytes(*params);
+}
+
+int nfi_disc_backward_hvp(const nfi_disc_params* params, const nfi_disc_hvp* hvp, const nfi_disc_grads* grads,
+                          void* stream) {
+  if (params == nullptr || hvp == nullptr || grads == nullptr) return fail("params / hvp / grads is NULL");
+  return nfi::disc::backward_hvp(*params, *hvp, *grads, (cudaStream_t)stream);
+}
+
+}  // extern "C"

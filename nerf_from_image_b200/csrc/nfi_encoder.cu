@@ -28,11 +28,9 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <limits.h>
-#include <stdio.h>
 #include <string.h>
 
 #include "nfi_encoder.h"
-#include "nfi_encoder_launch.h"
 #include "nfi_pair.cuh"
 #include "nfi_synth_launch.h"
 
@@ -257,205 +255,173 @@ static void layout(const nfi_encoder_params& P, Bump& b, Layout& L) {
   }
 }
 
-static int check(const nfi_encoder_params& P, char* err, size_t err_len) {
+static int check(const nfi_encoder_params& P) {
   if (P.batch <= 0 || P.batch > 65535 || P.height <= 0 || P.width <= 0 || P.height > 1024 ||
-      P.width > 1024) {
-    snprintf(err, err_len, "encoder: B in 1..65535 and feature sizes in 1..1024 needed, got B %d, %d x %d",
-             P.batch, P.height, P.width);
-    return 1;
-  }
-  if ((size_t)P.batch * kScale * kScale * P.height * P.width > (size_t)INT_MAX) {
-    snprintf(err, err_len, "encoder: more than 2^31 image positions (B %d, %d x %d features)", P.batch,
-             P.height, P.width);
-    return 1;
-  }
-  if (P.channels <= 0 || P.channels % 64 != 0) {
-    snprintf(err, err_len, "encoder: channels must be a positive multiple of 64, got %d", P.channels);
-    return 1;
-  }
+      P.width > 1024)
+    return fail("encoder: B in 1..65535 and feature sizes in 1..1024 needed, got B %d, %d x %d",
+                P.batch, P.height, P.width);
+  if ((size_t)P.batch * kScale * kScale * P.height * P.width > (size_t)INT_MAX)
+    return fail("encoder: more than 2^31 image positions (B %d, %d x %d features)", P.batch, P.height, P.width);
+  if (P.channels <= 0 || P.channels % 64 != 0)
+    return fail("encoder: channels must be a positive multiple of 64, got %d", P.channels);
   if ((P.pose_regressor != 0 && P.pose_regressor != 1) || (P.latent_regressor != 0 && P.latent_regressor != 1) ||
-      !(P.pose_regressor || P.latent_regressor)) {
-    snprintf(err, err_len, "encoder: pose_regressor and latent_regressor are 0 or 1, and one is 1");
-    return 1;
-  }
-  if (P.save != 0 && P.save != 1) {
-    snprintf(err, err_len, "encoder: save must be 0 or 1, got %d", P.save);
-    return 1;
-  }
+      !(P.pose_regressor || P.latent_regressor))
+    return fail("encoder: pose_regressor and latent_regressor are 0 or 1, and one is 1");
+  if (P.save != 0 && P.save != 1) return fail("encoder: save must be 0 or 1, got %d", P.save);
   return 0;
 }
 
 // the pair of a gradient with relu' applied, and its sum over positions into g_b (if set)
-static int act_backward(ActBackward a, float* g_b, cudaStream_t st, char* err, size_t err_len) {
+static int act_backward(ActBackward a, float* g_b, cudaStream_t st) {
   const int n = (int)blocks((size_t)a.M, kRows);
   act_backward_kernel<<<n, 256, 0, st>>>(a);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  return synth::bias_reduce(a.partial, n, a.C, g_b, st, err, err_len);
+  NFI_CUDA(cudaGetLastError());
+  return synth::bias_reduce(a.partial, n, a.C, g_b, st);
 }
 
 }  // namespace
 
 size_t workspace_bytes(const nfi_encoder_params& P) {
-  char err[160];
-  if (check(P, err, sizeof(err))) return 0;
+  if (check(P)) return 0;
   Bump b{nullptr, 0, 0};
   Layout L;
   layout(P, b, L);
   return b.off + 1024;
 }
 
-static int setup(const nfi_encoder_params& P, Layout& L, char* err, size_t err_len) {
-  if (const int rc = check(P, err, err_len)) return rc;
+static int setup(const nfi_encoder_params& P, Layout& L) {
+  if (const int rc = check(P)) return rc;
   if (P.pose_regressor && (!P.features || !P.post0_w || !P.post0_b || !P.post2_w || !P.post2_b || !P.post4_w ||
-                           !P.post4_b || !P.maps)) {
-    snprintf(err, err_len, "encoder: the pose head needs features, post weights and biases, and maps");
-    return 1;
-  }
-  if (P.latent_regressor && (!P.features_latent || !P.wpre_w || !P.wpre_b || !P.pooled)) {
-    snprintf(err, err_len, "encoder: the latent head needs features_latent, w_regressor_pre's weight and "
-                           "bias, and pooled");
-    return 1;
-  }
-  if (!P.workspace) {
-    snprintf(err, err_len, "encoder: workspace missing");
-    return 1;
-  }
+                           !P.post4_b || !P.maps))
+    return fail("encoder: the pose head needs features, post weights and biases, and maps");
+  if (P.latent_regressor && (!P.features_latent || !P.wpre_w || !P.wpre_b || !P.pooled))
+    return fail("encoder: the latent head needs features_latent, w_regressor_pre's weight and "
+                "bias, and pooled");
+  if (!P.workspace) return fail("encoder: workspace missing");
   const size_t need = workspace_bytes(P);
-  if (P.workspace_bytes < need) {
-    snprintf(err, err_len, "encoder: workspace too small (%zu < %zu bytes)", P.workspace_bytes, need);
-    return 1;
-  }
+  if (P.workspace_bytes < need) return fail("encoder: workspace too small (%zu < %zu bytes)", P.workspace_bytes, need);
   Bump b = aligned_bump(P.workspace, P.workspace_bytes);
   layout(P, b, L);
   return 0;
 }
 
-int forward(const nfi_encoder_params& P, cudaStream_t st, char* err, size_t err_len) {
+int forward(const nfi_encoder_params& P, cudaStream_t st) {
   Layout L;
-  if (const int rc = setup(P, L, err, err_len)) return rc;
+  if (const int rc = setup(P, L)) return rc;
   const int B = P.batch, h = P.height, w = P.width, C = P.channels, H = kScale * h, W = kScale * w;
   const size_t M = (size_t)B * H * W, Ml = (size_t)B * h * w;
   const Pair none = {nullptr, nullptr};
   if (P.pose_regressor) {
-    NFI_LAUNCH_CHECK(cudaMemsetAsync(L.w4p, 0, (size_t)kMapsG * C * 9 * sizeof(float), st));
-    NFI_LAUNCH_CHECK(cudaMemsetAsync(L.b4p, 0, kMapsG * sizeof(float), st));
-    NFI_LAUNCH_CHECK(
-        cudaMemcpyAsync(L.w4p, P.post4_w, (size_t)kMaps * C * 9 * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    NFI_LAUNCH_CHECK(cudaMemcpyAsync(L.b4p, P.post4_b, kMaps * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    if (int rc = synth::prep_weights(P.post0_w, C, C, 9, 9 * C, 1.f, synth::kTapCoCi, L.w0, st, err, err_len))
+    NFI_CUDA(cudaMemsetAsync(L.w4p, 0, (size_t)kMapsG * C * 9 * sizeof(float), st));
+    NFI_CUDA(cudaMemsetAsync(L.b4p, 0, kMapsG * sizeof(float), st));
+    NFI_CUDA(
+cudaMemcpyAsync(L.w4p, P.post4_w, (size_t)kMaps * C * 9 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    NFI_CUDA(cudaMemcpyAsync(L.b4p, P.post4_b, kMaps * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    if (int rc = synth::prep_weights(P.post0_w, C, C, 9, 9 * C, 1.f, synth::kTapCoCi, L.w0, st))
       return rc;
-    if (int rc = synth::prep_weights(P.post2_w, C, C, 9, 9 * C, 1.f, synth::kTapCoCi, L.w2, st, err, err_len))
+    if (int rc = synth::prep_weights(P.post2_w, C, C, 9, 9 * C, 1.f, synth::kTapCoCi, L.w2, st))
       return rc;
-    if (int rc = synth::prep_weights(L.w4p, kMapsN, C, 9, 9 * C, 1.f, synth::kTapCoCi, L.w4, st, err, err_len))
+    if (int rc = synth::prep_weights(L.w4p, kMapsN, C, 9, 9 * C, 1.f, synth::kTapCoCi, L.w4, st))
       return rc;
-    if (int rc = synth::transpose(P.features, B, C, h * w, nullptr, 0, L.fcl, st, err, err_len)) return rc;
+    if (int rc = synth::transpose(P.features, B, C, h * w, nullptr, 0, L.fcl, st)) return rc;
     upsample_relu_kernel<<<flat_grid(M * C / 4), 256, 0, st>>>(L.fcl, B, h, w, C, kScale, L.x0.hi, L.x0.lo);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
-    if (int rc = synth::conv3x3(B, H, W, C, C, L.x0, L.w0, P.post0_b, nullptr, L.a1, st, err, err_len)) return rc;
-    if (int rc = synth::conv3x3(B, H, W, C, C, L.a1, L.w2, P.post2_b, nullptr, L.a2, st, err, err_len)) return rc;
-    if (int rc = synth::conv3x3(B, H, W, C, kMapsN, L.a2, L.w4, L.b4p, L.u4, none, st, err, err_len)) return rc;
+    NFI_CUDA(cudaGetLastError());
+    if (int rc = synth::conv3x3(B, H, W, C, C, L.x0, L.w0, P.post0_b, nullptr, L.a1, st)) return rc;
+    if (int rc = synth::conv3x3(B, H, W, C, C, L.a1, L.w2, P.post2_b, nullptr, L.a2, st)) return rc;
+    if (int rc = synth::conv3x3(B, H, W, C, kMapsN, L.a2, L.w4, L.b4p, L.u4, none, st)) return rc;
     maps_kernel<<<flat_grid(M), 256, 0, st>>>(L.u4, M, P.maps);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
+    NFI_CUDA(cudaGetLastError());
   }
   if (P.latent_regressor) {
-    if (int rc = synth::prep_weights(P.wpre_w, C, C, 9, 9 * C, 1.f, synth::kTapCoCi, L.wl, st, err, err_len)) return rc;
-    if (int rc = synth::transpose(P.features_latent, B, C, h * w, nullptr, 0, L.fcl, st, err, err_len)) return rc;
+    if (int rc = synth::prep_weights(P.wpre_w, C, C, 9, 9 * C, 1.f, synth::kTapCoCi, L.wl, st)) return rc;
+    if (int rc = synth::transpose(P.features_latent, B, C, h * w, nullptr, 0, L.fcl, st)) return rc;
     upsample_relu_kernel<<<flat_grid(Ml * C / 4), 256, 0, st>>>(L.fcl, B, h, w, C, 1, L.xl.hi, L.xl.lo);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
-    if (int rc = synth::conv3x3(B, h, w, C, C, L.xl, L.wl, P.wpre_b, L.ul, none, st, err, err_len)) return rc;
+    NFI_CUDA(cudaGetLastError());
+    if (int rc = synth::conv3x3(B, h, w, C, C, L.xl, L.wl, P.wpre_b, L.ul, none, st)) return rc;
     mean_pool_kernel<<<dim3((unsigned)(C / 64), (unsigned)B), 256, 0, st>>>(L.ul, h * w, C, P.pooled);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
+    NFI_CUDA(cudaGetLastError());
   }
   return 0;
 }
 
 int backward(const nfi_encoder_params& P, const float* g_maps, const float* g_pooled, const nfi_encoder_grads& G,
-             cudaStream_t st, char* err, size_t err_len) {
-  if (!P.save) {
-    snprintf(err, err_len, "encoder backward: needs the workspace of a forward with save = 1");
-    return 1;
-  }
-  if ((P.pose_regressor && !g_maps) || (P.latent_regressor && !g_pooled)) {
-    snprintf(err, err_len, "encoder backward: g_maps (pose head) and g_pooled (latent head) must be set");
-    return 1;
-  }
+             cudaStream_t st) {
+  if (!P.save) return fail("encoder backward: needs the workspace of a forward with save = 1");
+  if ((P.pose_regressor && !g_maps) || (P.latent_regressor && !g_pooled))
+    return fail("encoder backward: g_maps (pose head) and g_pooled (latent head) must be set");
   Layout L;
-  if (const int rc = setup(P, L, err, err_len)) return rc;
+  if (const int rc = setup(P, L)) return rc;
   const int B = P.batch, h = P.height, w = P.width, C = P.channels, H = kScale * h, W = kScale * w;
   const int M = B * H * W, Ml = B * h * w;
   if (P.pose_regressor) {
-    if (int rc = synth::prep_weights(P.post0_w, C, C, 9, 9 * C, 1.f, synth::kTapCiCo, L.t0, st, err, err_len))
+    if (int rc = synth::prep_weights(P.post0_w, C, C, 9, 9 * C, 1.f, synth::kTapCiCo, L.t0, st))
       return rc;
-    if (int rc = synth::prep_weights(P.post2_w, C, C, 9, 9 * C, 1.f, synth::kTapCiCo, L.t2, st, err, err_len))
+    if (int rc = synth::prep_weights(P.post2_w, C, C, 9, 9 * C, 1.f, synth::kTapCiCo, L.t2, st))
       return rc;
-    if (int rc = synth::prep_weights(L.w4p, kMapsG, C, 9, 9 * C, 1.f, synth::kTapCiCo, L.t4, st, err, err_len))
+    if (int rc = synth::prep_weights(L.w4p, kMapsG, C, 9, 9 * C, 1.f, synth::kTapCiCo, L.t4, st))
       return rc;
     ActBackward a;
     memset(&a, 0, sizeof(a));
     a.M = M; a.partial = L.bpart;
     // post[4]: g_maps as the zero-padded pair
     a.C = kMaps; a.out_C = kMapsG; a.g = g_maps; a.hi = L.g4.hi; a.lo = L.g4.lo;
-    if (int rc = act_backward(a, G.g_post4_b, st, err, err_len)) return rc;
-    if (int rc = synth::wgrad3x3(B, H, W, kMaps, C, kMapsG, L.g4, L.a2, L.part, G.g_post4_w, st, err,
-                                 err_len))
+    if (int rc = act_backward(a, G.g_post4_b, st)) return rc;
+    if (int rc = synth::wgrad3x3(B, H, W, kMaps, C, kMapsG, L.g4, L.a2, L.part, G.g_post4_w, st))
       return rc;
     const bool below2 = G.g_post2_w || G.g_post2_b || G.g_post0_w || G.g_post0_b || G.g_features;
     const bool below0 = G.g_post0_w || G.g_post0_b || G.g_features;
     if (below2) {
-      if (int rc = synth::conv3x3_adjoint(B, H, W, kMapsG, C, L.g4, L.t4, L.d, st, err, err_len)) return rc;
+      if (int rc = synth::conv3x3_adjoint(B, H, W, kMapsG, C, L.g4, L.t4, L.d, st)) return rc;
       // post[2]
       a.C = C; a.out_C = C; a.g = L.d; a.mask_hi = L.a2.hi; a.hi = L.g.hi; a.lo = L.g.lo;
-      if (int rc = act_backward(a, G.g_post2_b, st, err, err_len)) return rc;
-      if (int rc = synth::wgrad3x3(B, H, W, C, C, C, L.g, L.a1, L.part, G.g_post2_w, st, err, err_len))
+      if (int rc = act_backward(a, G.g_post2_b, st)) return rc;
+      if (int rc = synth::wgrad3x3(B, H, W, C, C, C, L.g, L.a1, L.part, G.g_post2_w, st))
         return rc;
     }
     if (below0) {
-      if (int rc = synth::conv3x3_adjoint(B, H, W, C, C, L.g, L.t2, L.d, st, err, err_len)) return rc;
+      if (int rc = synth::conv3x3_adjoint(B, H, W, C, C, L.g, L.t2, L.d, st)) return rc;
       // post[0]
       a.mask_hi = L.a1.hi;
-      if (int rc = act_backward(a, G.g_post0_b, st, err, err_len)) return rc;
-      if (int rc = synth::wgrad3x3(B, H, W, C, C, C, L.g, L.x0, L.part, G.g_post0_w, st, err, err_len))
+      if (int rc = act_backward(a, G.g_post0_b, st)) return rc;
+      if (int rc = synth::wgrad3x3(B, H, W, C, C, C, L.g, L.x0, L.part, G.g_post0_w, st))
         return rc;
     }
     if (G.g_features) {
-      if (int rc = synth::conv3x3_adjoint(B, H, W, C, C, L.g, L.t0, L.d, st, err, err_len)) return rc;
+      if (int rc = synth::conv3x3_adjoint(B, H, W, C, C, L.g, L.t0, L.d, st)) return rc;
       upsample_adjoint_kernel<<<flat_grid((size_t)Ml * C / 4), 256, 0, st>>>(L.d, L.x0.hi, B, h, w, C, kScale,
                                                                              L.fcl);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
-      if (int rc = synth::transpose(L.fcl, B, h * w, C, nullptr, 1, G.g_features, st, err, err_len)) return rc;
+      NFI_CUDA(cudaGetLastError());
+      if (int rc = synth::transpose(L.fcl, B, h * w, C, nullptr, 1, G.g_features, st)) return rc;
     }
   }
   if (P.latent_regressor) {
-    if (int rc = synth::prep_weights(P.wpre_w, C, C, 9, 9 * C, 1.f, synth::kTapCiCo, L.tl, st, err, err_len)) return rc;
+    if (int rc = synth::prep_weights(P.wpre_w, C, C, 9, 9 * C, 1.f, synth::kTapCiCo, L.tl, st)) return rc;
     ActBackward a;
     memset(&a, 0, sizeof(a));
     a.M = Ml; a.C = C; a.out_C = C; a.partial = L.bpart;
     a.g_img = g_pooled; a.per_img = h * w; a.g_scale = 1.f / (float)(h * w);
     a.mask_u = L.ul; a.hi = L.g.hi; a.lo = L.g.lo;
-    if (int rc = act_backward(a, G.g_wpre_b, st, err, err_len)) return rc;
-    if (int rc = synth::wgrad3x3(B, h, w, C, C, C, L.g, L.xl, L.part, G.g_wpre_w, st, err, err_len))
+    if (int rc = act_backward(a, G.g_wpre_b, st)) return rc;
+    if (int rc = synth::wgrad3x3(B, h, w, C, C, C, L.g, L.xl, L.part, G.g_wpre_w, st))
       return rc;
     if (G.g_features_latent) {
-      if (int rc = synth::conv3x3_adjoint(B, h, w, C, C, L.g, L.tl, L.d, st, err, err_len)) return rc;
+      if (int rc = synth::conv3x3_adjoint(B, h, w, C, C, L.g, L.tl, L.d, st)) return rc;
       upsample_adjoint_kernel<<<flat_grid((size_t)Ml * C / 4), 256, 0, st>>>(L.d, L.xl.hi, B, h, w, C, 1, L.fcl);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
-      if (int rc = synth::transpose(L.fcl, B, h * w, C, nullptr, 1, G.g_features_latent, st, err, err_len))
+      NFI_CUDA(cudaGetLastError());
+      if (int rc = synth::transpose(L.fcl, B, h * w, C, nullptr, 1, G.g_features_latent, st))
         return rc;
     }
   }
   return 0;
 }
 
-int saved_activation(const nfi_encoder_params& P, int layer, float* out, cudaStream_t st, char* err,
-                     size_t err_len) {
+int saved_activation(const nfi_encoder_params& P, int layer, float* out, cudaStream_t st) {
   if (!P.save || layer < 0 || layer > 4 || out == nullptr || (layer < 3 && !P.pose_regressor) ||
-      (layer >= 3 && !P.latent_regressor)) {
-    snprintf(err, err_len, "encoder saved_activation: needs a saved forward, a layer in 0..4 of a head it "
-                           "ran, out");
-    return 1;
-  }
+      (layer >= 3 && !P.latent_regressor))
+    return fail("encoder saved_activation: needs a saved forward, a layer in 0..4 of a head it "
+                "ran, out");
   Layout L;
-  if (const int rc = setup(P, L, err, err_len)) return rc;
+  if (const int rc = setup(P, L)) return rc;
   const size_t C = P.channels, hw = (size_t)P.height * P.width, n = (size_t)P.batch * hw * C;
   const Pair src[4] = {L.x0, L.a1, L.a2, L.xl};
   const size_t count = layer < 3 ? n * kScale * kScale : n;
@@ -463,9 +429,36 @@ int saved_activation(const nfi_encoder_params& P, int layer, float* out, cudaStr
     unpack_kernel<<<flat_grid(count), 256, 0, st>>>(nullptr, nullptr, L.ul, count, out);
   else
     unpack_kernel<<<flat_grid(count), 256, 0, st>>>(src[layer].hi, src[layer].lo, nullptr, count, out);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 
 }  // namespace encoder
 }  // namespace nfi
+
+using nfi::fail;
+
+extern "C" {
+
+size_t nfi_encoder_workspace_bytes(const nfi_encoder_params* params) {
+  if (params == nullptr) return 0;
+  return nfi::encoder::workspace_bytes(*params);
+}
+
+int nfi_encoder_forward(const nfi_encoder_params* params, void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  return nfi::encoder::forward(*params, (cudaStream_t)stream);
+}
+
+int nfi_encoder_backward(const nfi_encoder_params* params, const float* g_maps, const float* g_pooled,
+                         const nfi_encoder_grads* grads, void* stream) {
+  if (params == nullptr || grads == nullptr) return fail("params / grads is NULL");
+  return nfi::encoder::backward(*params, g_maps, g_pooled, *grads, (cudaStream_t)stream);
+}
+
+int nfi_encoder_saved_activation(const nfi_encoder_params* params, int32_t layer, float* out, void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  return nfi::encoder::saved_activation(*params, layer, out, (cudaStream_t)stream);
+}
+
+}  // extern "C"

@@ -6,10 +6,10 @@
 // fp32 SIMT arithmetic built from the same device functions as render_forward_simt
 // (nfi_common.cuh), so a point evaluated here and the same point evaluated along a ray agree.
 #include <cuda_runtime.h>
-#include <stdio.h>
+#include <string.h>
 
 #include "nfi_common.cuh"
-#include "nfi_field_launch.h"
+#include "nfi_render.h"
 #include "nfi_forward.cuh"
 
 namespace nfi {
@@ -111,14 +111,13 @@ sample_field_simt(const nfi_render_params p, const nfi_sample_params io) {
 }
 
 template <int NP, bool NORM>
-int run_sampler(const nfi_render_params& p, const nfi_sample_params& io, cudaStream_t st,
-                char* err, size_t err_len) {
+int run_sampler(const nfi_render_params& p, const nfi_sample_params& io, cudaStream_t st) {
   const size_t smem = fwd_smem_floats(NP, 0, false, NORM) * sizeof(float);
   auto k = sample_field_simt<NP, NORM>;
-  NFI_LAUNCH_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  NFI_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const dim3 grid((unsigned)((io.n_points + kThreads - 1) / kThreads), (unsigned)io.batch);
   k<<<grid, kThreads, smem, st>>>(p, io);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 
@@ -289,38 +288,99 @@ __global__ void pose_to_matrix_bwd_kernel(const float* __restrict__ z0,
 }  // namespace
 
 int launch_sample_field(const nfi_render_params& p, const nfi_sample_params& io, int nout_pad,
-                        cudaStream_t st, char* err, size_t err_len) {
+                        cudaStream_t st) {
   const bool norm = io.normals != nullptr;
   switch (nout_pad) {
     case 4:
-      return norm ? run_sampler<4, true>(p, io, st, err, err_len)
-                  : run_sampler<4, false>(p, io, st, err, err_len);
+      return norm ? run_sampler<4, true>(p, io, st) : run_sampler<4, false>(p, io, st);
     case 12:
-      return norm ? run_sampler<12, true>(p, io, st, err, err_len)
-                  : run_sampler<12, false>(p, io, st, err, err_len);
+      return norm ? run_sampler<12, true>(p, io, st) : run_sampler<12, false>(p, io, st);
     default:
-      return norm ? run_sampler<16, true>(p, io, st, err, err_len)
-                  : run_sampler<16, false>(p, io, st, err, err_len);
+      return norm ? run_sampler<16, true>(p, io, st) : run_sampler<16, false>(p, io, st);
   }
 }
 
 int launch_pose_to_matrix(const float* z0, const float* t2, const float* s, const float* q,
-                          int flipped, int batch, float* c2w, float* focal, cudaStream_t st,
-                          char* err, size_t err_len) {
+                          int flipped, int batch, float* c2w, float* focal, cudaStream_t st) {
   pose_to_matrix_kernel<<<(batch + 63) / 64, 64, 0, st>>>(z0, t2, s, q, flipped, batch, c2w,
                                                           focal);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 
 int launch_pose_to_matrix_backward(const float* z0, const float* t2, const float* s,
                                    const float* q, int flipped, int batch, const float* g_c2w,
                                    const float* g_focal, float* g_z0, float* g_t2, float* g_s,
-                                   float* g_q, cudaStream_t st, char* err, size_t err_len) {
+                                   float* g_q, cudaStream_t st) {
   pose_to_matrix_bwd_kernel<<<(batch + 63) / 64, 64, 0, st>>>(z0, t2, s, q, flipped, batch, g_c2w,
                                                               g_focal, g_z0, g_t2, g_s, g_q);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 
 }  // namespace nfi
+
+using nfi::fail;
+
+extern "C" {
+
+int nfi_sample_field(const nfi_sample_params* sp, void* stream) {
+  if (sp == nullptr) return fail("params is NULL");
+  if (sp->batch <= 0 || sp->batch > 65535 || sp->n_points <= 0) return fail("empty point set");
+  if (sp->n_points > ((int64_t)1 << 37)) return fail("too many points per image");
+  if (sp->plane_res < 2) return fail("plane_res must be >= 2");
+  if (sp->n_attention < 0 || sp->n_attention > NFI_MAX_ATTENTION)
+    return fail("attention_values must be in [0, 15]");
+  if (!(sp->scene_range > 0.f)) return fail("scene_range must be positive");
+  if (!sp->planes || !sp->w1 || !sp->b1 || !sp->w2 || !sp->b2 || !sp->points)
+    return fail("planes / decoder weights / points must be given");
+  if (sp->n_attention > 0 && !sp->palette)
+    return fail("palette missing (attention_values > 0)");
+  if (sp->use_sdf && (!sp->beta || !sp->alpha)) return fail("use_sdf needs beta and alpha");
+  if (sp->semantics && sp->n_attention <= 0)
+    return fail("'semantics' needs attention_values > 0");  // generator.py:673
+  if (sp->normals && !sp->use_sdf) return fail("'normals' needs use_sdf");  // generator.py:600
+  if (sp->bbox_debug && !sp->sigma) return fail("bbox_debug modifies sigma: request it");
+  if (!sp->sdf_distance && !sp->sigma && !sp->rgb && !sp->semantics && !sp->normals)
+    return fail("no sampler output requested");
+  nfi_render_params p;
+  memset(&p, 0, sizeof(p));
+  p.batch = sp->batch;
+  p.plane_res = sp->plane_res;
+  p.n_attention = sp->n_attention;
+  p.use_sdf = sp->use_sdf;
+  p.scene_range = sp->scene_range;
+  p.planes = sp->planes;
+  p.w1 = sp->w1;
+  p.b1 = sp->b1;
+  p.w2 = sp->w2;
+  p.b2 = sp->b2;
+  p.palette = sp->palette;
+  p.beta = sp->beta;
+  p.alpha = sp->alpha;
+  return nfi::launch_sample_field(p, *sp, nfi::nout_pad_of(p.n_attention), (cudaStream_t)stream);
+}
+
+int nfi_pose_to_matrix(const float* z0, const float* t2, const float* s, const float* q,
+                       int32_t camera_flipped, int32_t batch, float* c2w, float* focal,
+                       void* stream) {
+  if (batch <= 0) return fail("empty batch");
+  if (!t2 || !s || !q || !c2w) return fail("t2 / s / q / c2w must be given");
+  if (z0 && !focal) return fail("perspective pose (z0 given) needs the focal output");
+  return nfi::launch_pose_to_matrix(z0, t2, s, q, camera_flipped, batch, c2w, focal,
+                                    (cudaStream_t)stream);
+}
+
+int nfi_pose_to_matrix_backward(const float* z0, const float* t2, const float* s, const float* q,
+                                int32_t camera_flipped, int32_t batch, const float* g_c2w,
+                                const float* g_focal, float* g_z0, float* g_t2, float* g_s,
+                                float* g_q, void* stream) {
+  if (batch <= 0) return fail("empty batch");
+  if (!t2 || !s || !q || !g_c2w || !g_t2 || !g_s || !g_q)
+    return fail("t2 / s / q / g_c2w and the three gradient outputs must be given");
+  if (z0 && !g_z0) return fail("perspective pose (z0 given) needs g_z0");
+  return nfi::launch_pose_to_matrix_backward(z0, t2, s, q, camera_flipped, batch, g_c2w, g_focal,
+                                             g_z0, g_t2, g_s, g_q, (cudaStream_t)stream);
+}
+
+}  // extern "C"

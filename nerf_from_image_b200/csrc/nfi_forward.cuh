@@ -418,37 +418,32 @@ inline size_t num_tiles(const nfi_render_params& p) {
 namespace simt {
 
 template <int NP, int EX, bool FINE, bool NORM, bool VD>
-int launch_fwd(const nfi_render_params& p, size_t smem, cudaStream_t st, char* err,
-               size_t err_len) {
-  if (smem > 227 * 1024) {
-    snprintf(err, err_len, "depth_samples_per_ray too large for the shared-memory columns");
-    return 1;
-  }
+int launch_fwd(const nfi_render_params& p, size_t smem, cudaStream_t st) {
+  if (smem > 227 * 1024)
+    return fail("depth_samples_per_ray too large for the shared-memory columns");
   auto k = render_forward_simt<NP, EX, FINE, NORM, VD>;
-  NFI_LAUNCH_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  NFI_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   k<<<(unsigned)num_tiles(p), kThreads, smem, st>>>(p);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 
 template <int NP, int EX, bool VD>
-int fwd_fine(const nfi_render_params& p, bool normals, size_t smem, cudaStream_t st, char* err,
-             size_t err_len) {
+int fwd_fine(const nfi_render_params& p, bool normals, size_t smem, cudaStream_t st) {
   if (normals) {
-    if (p.fine_sampling) return launch_fwd<NP, EX, true, true, VD>(p, smem, st, err, err_len);
-    return launch_fwd<NP, EX, false, true, VD>(p, smem, st, err, err_len);
+    if (p.fine_sampling) return launch_fwd<NP, EX, true, true, VD>(p, smem, st);
+    return launch_fwd<NP, EX, false, true, VD>(p, smem, st);
   }
-  if (p.fine_sampling) return launch_fwd<NP, EX, true, false, VD>(p, smem, st, err, err_len);
-  return launch_fwd<NP, EX, false, false, VD>(p, smem, st, err, err_len);
+  if (p.fine_sampling) return launch_fwd<NP, EX, true, false, VD>(p, smem, st);
+  return launch_fwd<NP, EX, false, false, VD>(p, smem, st);
 }
 
 template <int NP, bool VD>
-int fwd_extra(const nfi_render_params& p, bool normals, size_t smem, cudaStream_t st, char* err,
-              size_t err_len) {
+int fwd_extra(const nfi_render_params& p, bool normals, size_t smem, cudaStream_t st) {
   switch (p.extra_mode) {
-    case NFI_EXTRA_COORDS: return fwd_fine<NP, 1, VD>(p, normals, smem, st, err, err_len);
-    case NFI_EXTRA_SEMANTICS: return fwd_fine<NP, 2, VD>(p, normals, smem, st, err, err_len);
-    default: return fwd_fine<NP, 0, VD>(p, normals, smem, st, err, err_len);
+    case NFI_EXTRA_COORDS: return fwd_fine<NP, 1, VD>(p, normals, smem, st);
+    case NFI_EXTRA_SEMANTICS: return fwd_fine<NP, 2, VD>(p, normals, smem, st);
+    default: return fwd_fine<NP, 0, VD>(p, normals, smem, st);
   }
 }
 
@@ -457,18 +452,16 @@ int fwd_extra(const nfi_render_params& p, bool normals, size_t smem, cudaStream_
 // render_forward_simt; `p.workspace` points at the scratch slabs (behind the weight-image header).
 // nfi_render.cu instantiates it for VD = false, nfi_viewdir.cu for VD = true.
 template <bool VD>
-int launch_forward_simt(const nfi_render_params& p, bool normals, cudaStream_t st, char* err,
-                        size_t err_len) {
+int launch_forward_simt(const nfi_render_params& p, bool normals, cudaStream_t st) {
   const int np = nout_pad_of(p.n_attention);
   const size_t smem =
       fwd_smem_floats(np, p.num_samples, p.fine_sampling != 0, normals, VD) * sizeof(float);
   switch (np) {
-    case 4: return simt::fwd_extra<4, VD>(p, normals, smem, st, err, err_len);
-    case 12: return simt::fwd_extra<12, VD>(p, normals, smem, st, err, err_len);
-    default: return simt::fwd_extra<16, VD>(p, normals, smem, st, err, err_len);
+    case 4: return simt::fwd_extra<4, VD>(p, normals, smem, st);
+    case 12: return simt::fwd_extra<12, VD>(p, normals, smem, st);
+    default: return simt::fwd_extra<16, VD>(p, normals, smem, st);
   }
 }
-extern template int launch_forward_simt<true>(const nfi_render_params&, bool, cudaStream_t, char*,
-                                              size_t);
+extern template int launch_forward_simt<true>(const nfi_render_params&, bool, cudaStream_t);
 
 }  // namespace nfi

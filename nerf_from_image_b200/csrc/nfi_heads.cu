@@ -21,11 +21,9 @@
 // against the render's 2.1 M: this is not a hot loop, it exists so that the GAN generator step
 // does not need the unfused decoder (and its autograd graph) at all.
 #include <cuda_runtime.h>
-#include <stdio.h>
 
 #include "nfi_common.cuh"
 #include "nfi_heads.h"
-#include "nfi_heads_launch.h"
 
 namespace nfi {
 namespace heads {
@@ -370,24 +368,55 @@ static unsigned grid_for(const nfi_sdf_points_params& p) {
   return (unsigned)(ctas < 1 ? 1 : ctas);
 }
 
-int launch_forward(const nfi_sdf_points_params& p, cudaStream_t st, char* err, size_t err_len) {
+int launch_forward(const nfi_sdf_points_params& p, cudaStream_t st) {
   const size_t smem = smem_floats(false) * sizeof(float);
-  NFI_LAUNCH_CHECK(cudaFuncSetAttribute(sdf_points_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)smem));
+  NFI_CUDA(cudaFuncSetAttribute(sdf_points_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                (int)smem));
   sdf_points_fwd_kernel<<<grid_for(p), kThreads, smem, st>>>(p);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 
-int launch_backward(const nfi_sdf_points_params& p, const nfi_sdf_points_grads& g, cudaStream_t st,
-                    char* err, size_t err_len) {
+int launch_backward(const nfi_sdf_points_params& p, const nfi_sdf_points_grads& g,
+                    cudaStream_t st) {
   const size_t smem = smem_floats(true) * sizeof(float);
-  NFI_LAUNCH_CHECK(cudaFuncSetAttribute(sdf_points_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)smem));
+  NFI_CUDA(cudaFuncSetAttribute(sdf_points_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                (int)smem));
   sdf_points_bwd_kernel<<<grid_for(p), kThreads, smem, st>>>(p, g);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 
 }  // namespace heads
 }  // namespace nfi
+
+using nfi::fail;
+
+extern "C" {
+
+static int check_sdf_points(const nfi_sdf_points_params* p) {
+  if (p == nullptr) return fail("params is NULL");
+  if (p->batch <= 0 || p->n_points <= 0 || p->plane_res < 2) return fail("empty batch / no points");
+  if (!p->planes || !p->w1 || !p->b1 || !p->w2 || !p->b2 || !p->points)
+    return fail("planes, decoder weights and points must be given");
+  if (!(p->scene_range > 0.f)) return fail("scene_range must be positive");
+  return 0;
+}
+
+int nfi_sdf_points_forward(const nfi_sdf_points_params* params, void* stream) {
+  if (const int rc = check_sdf_points(params)) return rc;
+  if (!params->d) return fail("output d must be given");
+  return nfi::heads::launch_forward(*params, (cudaStream_t)stream);
+}
+
+int nfi_sdf_points_backward(const nfi_sdf_points_params* params, const nfi_sdf_points_grads* grads,
+                            void* stream) {
+  if (const int rc = check_sdf_points(params)) return rc;
+  if (grads == nullptr) return fail("grads is NULL");
+  if (!grads->g_d && !grads->g_grad) return fail("no upstream gradient");
+  if (grads->grad_w1 && (!grads->grad_b1 || !grads->grad_w2_row0 || !grads->grad_b2_0))
+    return fail("decoder gradients come as a set: grad_w1, grad_b1, grad_w2_row0, grad_b2_0");
+  return nfi::heads::launch_backward(*params, *grads, (cudaStream_t)stream);
+}
+
+}  // extern "C"

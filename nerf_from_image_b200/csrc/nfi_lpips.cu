@@ -27,11 +27,9 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <math.h>
-#include <stdio.h>
 #include <string.h>
 
 #include "nfi_lpips.h"
-#include "nfi_lpips_launch.h"
 #include "nfi_pair.cuh"
 #include "nfi_synth_launch.h"
 
@@ -378,20 +376,11 @@ static void layout(const nfi_lpips_params& P, Bump& b, Layout& L) {
   }
 }
 
-static int check(const nfi_lpips_params& P, char* err, size_t err_len) {
-  if (P.n <= 0) {
-    snprintf(err, err_len, "lpips: N must be positive, got %d", P.n);
-    return 1;
-  }
-  if (P.height < 16 || P.width < 16 || P.height % 16 || P.width % 16) {
-    snprintf(err, err_len, "lpips: H and W must be multiples of 16 (four 2x2 pools), got %d x %d",
-             P.height, P.width);
-    return 1;
-  }
-  if (P.save < 0 || P.save > 2) {
-    snprintf(err, err_len, "lpips: save must be 0, 1 or 2, got %d", P.save);
-    return 1;
-  }
+static int check(const nfi_lpips_params& P) {
+  if (P.n <= 0) return fail("lpips: N must be positive, got %d", P.n);
+  if (P.height < 16 || P.width < 16 || P.height % 16 || P.width % 16)
+    return fail("lpips: H and W must be multiples of 16 (four 2x2 pools), got %d x %d", P.height, P.width);
+  if (P.save < 0 || P.save > 2) return fail("lpips: save must be 0, 1 or 2, got %d", P.save);
   return 0;
 }
 
@@ -410,58 +399,45 @@ static void tap_backward(const TapBackward& a, cudaStream_t st) {
 }  // namespace
 
 size_t workspace_bytes(const nfi_lpips_params& P) {
-  char err[128];
-  if (check(P, err, sizeof(err))) return 0;
+  if (check(P)) return 0;
   Bump b{nullptr, 0, 0};
   Layout L;
   layout(P, b, L);
   return b.off + 1024;
 }
 
-static int setup(const nfi_lpips_params& P, Layout& L, char* err, size_t err_len) {
-  if (const int rc = check(P, err, err_len)) return rc;
-  if (!P.in0 || !P.in1 || !P.shift || !P.scale || !P.out || !P.workspace) {
-    snprintf(err, err_len, "lpips: in0, in1, shift, scale, out and workspace must be set");
-    return 1;
-  }
+static int setup(const nfi_lpips_params& P, Layout& L) {
+  if (const int rc = check(P)) return rc;
+  if (!P.in0 || !P.in1 || !P.shift || !P.scale || !P.out || !P.workspace)
+    return fail("lpips: in0, in1, shift, scale, out and workspace must be set");
   for (int l = 0; l < kConvs; ++l)
-    if (!P.conv_w[l] || !P.conv_b[l]) {
-      snprintf(err, err_len, "lpips: conv %d weight / bias missing", l);
-      return 1;
-    }
+    if (!P.conv_w[l] || !P.conv_b[l]) return fail("lpips: conv %d weight / bias missing", l);
   for (int t = 0; t < kTaps; ++t)
-    if (!P.lin_w[t]) {
-      snprintf(err, err_len, "lpips: lin %d missing", t);
-      return 1;
-    }
+    if (!P.lin_w[t]) return fail("lpips: lin %d missing", t);
   const size_t need = workspace_bytes(P);
-  if (P.workspace_bytes < need) {
-    snprintf(err, err_len, "lpips: workspace too small (%zu < %zu bytes)", P.workspace_bytes, need);
-    return 1;
-  }
+  if (P.workspace_bytes < need) return fail("lpips: workspace too small (%zu < %zu bytes)", P.workspace_bytes, need);
   Bump b = aligned_bump(P.workspace, P.workspace_bytes);
   layout(P, b, L);
   return 0;
 }
 
-int forward(const nfi_lpips_params& P, cudaStream_t st, char* err, size_t err_len) {
+int forward(const nfi_lpips_params& P, cudaStream_t st) {
   Layout L;
-  if (const int rc = setup(P, L, err, err_len)) return rc;
+  if (const int rc = setup(P, L)) return rc;
   const int N = P.n, H = P.height, W = P.width, B2 = 2 * N;
   for (int l = 1; l < kConvs; ++l)
-    if (const int rc = synth::prep_weights(P.conv_w[l], kCout[l], kCin[l], 9, 9 * kCin[l], 1.f, synth::kTapCoCi, L.wf[l],
-                                           st, err, err_len))
+    if (const int rc = synth::prep_weights(P.conv_w[l], kCout[l], kCin[l], 9, 9 * kCin[l], 1.f, synth::kTapCoCi,
+                                           L.wf[l], st))
       return rc;
   conv11_forward_kernel<<<flat_grid((size_t)B2 * H * W * 8), 256, 0, st>>>(
       P.in0, P.in1, N, H, W, P.conv_w[0], P.conv_b[0], P.shift, P.scale, L.u[0], L.act[0].hi, L.act[0].lo);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   int cur = 0;
   for (int l = 1; l < kConvs; ++l) {
     const int h = H >> kLevel[l], w = W >> kLevel[l], t = kTapOf[l];
     const bool writes_pair = t < 0;  // a tap's relu(u) is read from u (head, pool)
     const Pair out = writes_pair ? L.act[cur ^ 1] : Pair{nullptr, nullptr};
-    if (const int rc = synth::conv3x3(B2, h, w, kCin[l], kCout[l], L.act[cur], L.wf[l], P.conv_b[l], L.u[l], out,
-                                      st, err, err_len))
+    if (const int rc = synth::conv3x3(B2, h, w, kCin[l], kCout[l], L.act[cur], L.wf[l], P.conv_b[l], L.u[l], out, st))
       return rc;
     if (t >= 0) {
       float* part = L.partial + L.taps.off[t];
@@ -472,37 +448,31 @@ int forward(const nfi_lpips_params& P, cudaStream_t st, char* err, size_t err_le
         case 256: head_forward<8>(L.u[l], N, hw, P.lin_w[t], part, nc, st); break;
         default: head_forward<16>(L.u[l], N, hw, P.lin_w[t], part, nc, st); break;
       }
-      NFI_LAUNCH_CHECK(cudaGetLastError());
+      NFI_CUDA(cudaGetLastError());
       if (pooled_after(l)) {
         pool_kernel<<<flat_grid((size_t)B2 * (h / 2) * (w / 2) * (kCout[l] / 4)), 256, 0, st>>>(
             L.u[l], B2, h, w, kCout[l], L.act[cur ^ 1].hi, L.act[cur ^ 1].lo);
-        NFI_LAUNCH_CHECK(cudaGetLastError());
+        NFI_CUDA(cudaGetLastError());
       }
     }
     cur ^= 1;
   }
   head_sum_kernel<<<(N + 255) / 256, 256, 0, st>>>(L.partial, L.taps, N, P.out);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 
-int backward(const nfi_lpips_params& P, const float* g_dist, float* grad_in0, float* grad_in1,
-             cudaStream_t st, char* err, size_t err_len) {
-  if (!P.save || (grad_in1 && P.save != 2)) {
-    snprintf(err, err_len, "lpips backward: needs the workspace of a forward with save = 1 (save = 2 "
-                           "for a gradient to in1)");
-    return 1;
-  }
-  if (!g_dist || !grad_in0) {
-    snprintf(err, err_len, "lpips backward: g_dist and grad_in0 must be set");
-    return 1;
-  }
+int backward(const nfi_lpips_params& P, const float* g_dist, float* grad_in0, float* grad_in1, cudaStream_t st) {
+  if (!P.save || (grad_in1 && P.save != 2))
+    return fail("lpips backward: needs the workspace of a forward with save = 1 (save = 2 "
+                "for a gradient to in1)");
+  if (!g_dist || !grad_in0) return fail("lpips backward: g_dist and grad_in0 must be set");
   Layout L;
-  if (const int rc = setup(P, L, err, err_len)) return rc;
+  if (const int rc = setup(P, L)) return rc;
   const int N = P.n, H = P.height, W = P.width, B = grad_in1 ? 2 * N : N;
   for (int l = 1; l < kConvs; ++l)
-    if (const int rc = synth::prep_weights(P.conv_w[l], kCout[l], kCin[l], 9, 9 * kCin[l], 1.f, synth::kTapCiCo, L.wt[l],
-                                           st, err, err_len))
+    if (const int rc = synth::prep_weights(P.conv_w[l], kCout[l], kCin[l], 9, 9 * kCin[l], 1.f, synth::kTapCiCo,
+                                           L.wt[l], st))
       return rc;
   const float* gin = nullptr;  // gradient of layer l's relu(u), or of the pool output after it
   int cur = 0;
@@ -520,31 +490,54 @@ int backward(const nfi_lpips_params& P, const float* g_dist, float* grad_in0, fl
       case 256: tap_backward<8>(a, st); break;
       default: tap_backward<16>(a, st); break;
     }
-    NFI_LAUNCH_CHECK(cudaGetLastError());
-    if (const int rc = synth::conv3x3_adjoint(B, h, w, kCout[l], kCin[l], L.dacc, L.wt[l], L.g[cur], st, err,
-                                              err_len))
+    NFI_CUDA(cudaGetLastError());
+    if (const int rc = synth::conv3x3_adjoint(B, h, w, kCout[l], kCin[l], L.dacc, L.wt[l], L.g[cur], st))
       return rc;
     gin = L.g[cur];
     cur ^= 1;
   }
   conv11_backward_kernel<<<flat_grid((size_t)B * H * W), 256, 0, st>>>(gin, L.u[0], N, B, H, W, P.conv_w[0],
                                                                       P.scale, grad_in0, grad_in1);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 
-int saved_preactivation(const nfi_lpips_params& P, int layer, float* out, cudaStream_t st, char* err,
-                        size_t err_len) {
-  if (!P.save || layer < 0 || layer >= kConvs || out == nullptr) {
-    snprintf(err, err_len, "lpips saved_preactivation: needs a saved forward, a layer in 0..12, out");
-    return 1;
-  }
+int saved_preactivation(const nfi_lpips_params& P, int layer, float* out, cudaStream_t st) {
+  if (!P.save || layer < 0 || layer >= kConvs || out == nullptr)
+    return fail("lpips saved_preactivation: needs a saved forward, a layer in 0..12, out");
   Layout L;
-  if (const int rc = setup(P, L, err, err_len)) return rc;
+  if (const int rc = setup(P, L)) return rc;
   const size_t n = (size_t)2 * P.n * ((size_t)P.height * P.width >> (2 * kLevel[layer])) * kCout[layer];
-  NFI_LAUNCH_CHECK(cudaMemcpyAsync(out, L.u[layer], n * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  NFI_CUDA(cudaMemcpyAsync(out, L.u[layer], n * sizeof(float), cudaMemcpyDeviceToDevice, st));
   return 0;
 }
 
 }  // namespace lpips
 }  // namespace nfi
+
+using nfi::fail;
+
+extern "C" {
+
+size_t nfi_lpips_workspace_bytes(const nfi_lpips_params* params) {
+  if (params == nullptr) return 0;
+  return nfi::lpips::workspace_bytes(*params);
+}
+
+int nfi_lpips_forward(const nfi_lpips_params* params, void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  return nfi::lpips::forward(*params, (cudaStream_t)stream);
+}
+
+int nfi_lpips_backward(const nfi_lpips_params* params, const float* g_dist, float* grad_in0, float* grad_in1,
+                       void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  return nfi::lpips::backward(*params, g_dist, grad_in0, grad_in1, (cudaStream_t)stream);
+}
+
+int nfi_lpips_saved_preactivation(const nfi_lpips_params* params, int32_t layer, float* out, void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  return nfi::lpips::saved_preactivation(*params, layer, out, (cudaStream_t)stream);
+}
+
+}  // extern "C"

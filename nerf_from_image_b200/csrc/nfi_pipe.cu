@@ -38,45 +38,45 @@ static __global__ void prep_weight_image_bwd(const float* __restrict__ w1, const
 // log2 e goes into layer 1 and the colour rows of layer 2; padded logits at -1e30
 template <>
 int prep_weight_images<false>(const nfi_render_params& p, unsigned char* wimg, bool bwd,
-                              cudaStream_t st, char* err, size_t err_len) {
+                              cudaStream_t st) {
   const int nout = nout_of(p.n_attention);
   const bool att = p.n_attention > 0;
   prep_weight_image<<<1, 256, 0, st>>>(p.w1, p.b1, p.w2, p.b2, nout, wimg, kLog2e,
                                        att ? kPadLogit : 0.f, att ? kLog2e : 1.f);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   if (bwd) {
     prep_weight_image_bwd<<<1, 256, 0, st>>>(p.w1, p.w2, nout, wimg + kBwdImageOffset);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
+    NFI_CUDA(cudaGetLastError());
   }
   return 0;
 }
 
-template int launch_pipe_forward<false>(const nfi_render_params&, unsigned char*, float*, unsigned, cudaStream_t, char*, size_t);
-template int launch_pipe_backward<false>(const nfi_render_params&, const nfi_render_grads&, unsigned char*, unsigned, cudaStream_t,
-                                         char*, size_t);
+template int launch_pipe_forward<false>(const nfi_render_params&, unsigned char*, float*, unsigned,
+                                        cudaStream_t);
+template int launch_pipe_backward<false>(const nfi_render_params&, const nfi_render_grads&,
+                                         unsigned char*, unsigned, cudaStream_t);
 
 namespace {
 
 template <int NP, bool PLANES>
 int run_wgrad(const nfi_render_params& p, const nfi_render_grads& g, unsigned char* wimg,
-              unsigned grid, cudaStream_t st, char* err, size_t err_len) {
+              unsigned grid, cudaStream_t st) {
   using Cfg = WgCfgT<PLANES>;
   auto k = render_wgrad_pipe<NP, PLANES>;
-  NFI_LAUNCH_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        Cfg::kSmBytes));
+  NFI_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmBytes));
   k<<<grid, Cfg::kThreadsTotal, Cfg::kSmBytes, st>>>(p, g, wimg,
                                                      reinterpret_cast<float*>(wimg + kWgAccOffset));
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 
 template <bool PLANES>
 int wgrad_np(const nfi_render_params& p, const nfi_render_grads& g, unsigned char* wimg,
-             unsigned grid, cudaStream_t st, char* err, size_t err_len) {
+             unsigned grid, cudaStream_t st) {
   switch (nout_pad_of(p.n_attention)) {
-    case 4: return run_wgrad<4, PLANES>(p, g, wimg, grid, st, err, err_len);
-    case 12: return run_wgrad<12, PLANES>(p, g, wimg, grid, st, err, err_len);
-    default: return run_wgrad<16, PLANES>(p, g, wimg, grid, st, err, err_len);
+    case 4: return run_wgrad<4, PLANES>(p, g, wimg, grid, st);
+    case 12: return run_wgrad<12, PLANES>(p, g, wimg, grid, st);
+    default: return run_wgrad<16, PLANES>(p, g, wimg, grid, st);
   }
 }
 
@@ -87,35 +87,34 @@ size_t pipe_scratch_bytes_per_cta(int num_samples, int nes) {
 }
 
 int launch_pipe_wgrad(const nfi_render_params& p, const nfi_render_grads& g, unsigned char* wimg,
-                      unsigned grid, bool planes, cudaStream_t st, char* err, size_t err_len) {
-  if (int rc = prep_weight_images<false>(p, wimg, true, st, err, err_len)) return rc;
-  return planes ? wgrad_np<true>(p, g, wimg, grid, st, err, err_len)
-                : wgrad_np<false>(p, g, wimg, grid, st, err, err_len);
+                      unsigned grid, bool planes, cudaStream_t st) {
+  if (int rc = prep_weight_images<false>(p, wimg, true, st)) return rc;
+  return planes ? wgrad_np<true>(p, g, wimg, grid, st) : wgrad_np<false>(p, g, wimg, grid, st);
 }
 
 int launch_pipe_normals(const nfi_render_params& p, unsigned char* wimg, unsigned char* wimg_bwd,
-                        unsigned grid, cudaStream_t st, char* err, size_t err_len) {
+                        unsigned grid, cudaStream_t st) {
   // render_normals_pipe needs layer 1 and the distance row of the plain image: row 0 of w2 with
   // or without a view.  A view render is done with its own image (stream order), so the plain
   // one takes its place.
   if (p.view_features)
-    if (int rc = prep_weight_images<false>(p, wimg, false, st, err, err_len)) return rc;
+    if (int rc = prep_weight_images<false>(p, wimg, false, st)) return rc;
   prep_weight_image_bwd<<<1, 256, 0, st>>>(p.w1, p.w2, nout_of(p.n_attention), wimg_bwd);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  NFI_LAUNCH_CHECK(cudaMemsetAsync(p.normals, 0,
-                                   (size_t)p.batch * p.height * p.width * 3 * sizeof(float), st));
+  NFI_CUDA(cudaGetLastError());
+  NFI_CUDA(cudaMemsetAsync(p.normals, 0,
+                           (size_t)p.batch * p.height * p.width * 3 * sizeof(float), st));
   using Cfg = BwdCfg<2>;
   constexpr int smem = Cfg::kSmBytes + (kBwdSlots * 128 + kHid) * (int)sizeof(float);
 #define NFI_NRM(NP)                                                                          \
   do {                                                                                       \
     auto k = render_normals_pipe<NP, 2>;                                                     \
-    NFI_LAUNCH_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); \
+    NFI_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));    \
     k<<<grid, Cfg::kThreadsTotal, smem, st>>>(p, wimg, wimg_bwd);                            \
   } while (0)
   const int np = nout_pad_of(p.n_attention);
   if (np == 4) NFI_NRM(4); else if (np == 12) NFI_NRM(12); else NFI_NRM(16);
 #undef NFI_NRM
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 

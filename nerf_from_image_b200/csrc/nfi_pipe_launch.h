@@ -13,24 +13,23 @@ namespace nfi {
 // `grid` persistent CTAs; `scratch` = pipe_scratch_bytes_per_cta per CTA
 template <bool VD>
 int launch_pipe_forward(const nfi_render_params& p, unsigned char* wimg, float* scratch,
-                        unsigned grid, cudaStream_t st, char* err, size_t err_len);
+                        unsigned grid, cudaStream_t st);
 size_t pipe_scratch_bytes_per_cta(int num_samples, int nes);
 // both weight images at `wimg` (nfi_layout.h), then render_backward_pipe: a frozen decoder (and
 // with a view a frozen mapper output); decoder gradients of `g` are not produced
 template <bool VD>
 int launch_pipe_backward(const nfi_render_params& p, const nfi_render_grads& g,
-                         unsigned char* wimg, unsigned grid, cudaStream_t st, char* err,
-                         size_t err_len);
+                         unsigned char* wimg, unsigned grid, cudaStream_t st);
 // decoder-weight gradients (grad_w1 / b1 / w2 / b2 of `g`, accumulated) on the tensor cores: both
 // weight images + render_wgrad_pipe, whose accumulator rows follow them (nfi_layout.h,
 // NFI_BACKWARD_WORKSPACE_BYTES in all).  The other gradients of `g` are produced only with
 // `planes`: ONE sweep for the whole generator step, grad_planes / grad_palette / grad_beta /
 // grad_alpha (no pose gradient).
 int launch_pipe_wgrad(const nfi_render_params& p, const nfi_render_grads& g, unsigned char* wimg,
-                      unsigned grid, bool planes, cudaStream_t st, char* err, size_t err_len);
+                      unsigned grid, bool planes, cudaStream_t st);
 // composited surface normals (params.normals, overwritten) after a render_forward_pipe launch of
 // the same params (z_fine and mask filled): render_normals_pipe, reading the plain weight image
 // at `wimg` (rebuilt there after a view render) and a backward image it builds at `wimg_bwd`
 int launch_pipe_normals(const nfi_render_params& p, unsigned char* wimg, unsigned char* wimg_bwd,
-                        unsigned grid, cudaStream_t st, char* err, size_t err_len);
+                        unsigned grid, cudaStream_t st);
 }  // namespace nfi

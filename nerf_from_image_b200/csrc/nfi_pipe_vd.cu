@@ -48,21 +48,22 @@ __global__ void prep_weight_image_vd_bwd(const float* __restrict__ w1, const flo
 // The backward image is in natural units throughout (nfi_layout.h).
 template <>
 int prep_weight_images<true>(const nfi_render_params& p, unsigned char* wimg, bool bwd,
-                             cudaStream_t st, char* err, size_t err_len) {
+                             cudaStream_t st) {
   const bool att = p.n_attention > 0;
   prep_weight_image_vd<<<1, 256, 0, st>>>(p.w1, p.b1, p.w2, p.b2, p.w3, p.b3, p.n_attention, wimg,
                                           kLog2e, att ? kLog2e : 1.f, att ? kPadLogit : 0.f);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   if (bwd) {
     prep_weight_image_vd_bwd<<<1, 256, 0, st>>>(p.w1, p.w2, p.w3, p.n_attention,
                                                 wimg + kVdBwdImageOffset);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
+    NFI_CUDA(cudaGetLastError());
   }
   return 0;
 }
 
-template int launch_pipe_forward<true>(const nfi_render_params&, unsigned char*, float*, unsigned, cudaStream_t, char*, size_t);
-template int launch_pipe_backward<true>(const nfi_render_params&, const nfi_render_grads&, unsigned char*, unsigned, cudaStream_t,
-                                         char*, size_t);
+template int launch_pipe_forward<true>(const nfi_render_params&, unsigned char*, float*, unsigned,
+                                       cudaStream_t);
+template int launch_pipe_backward<true>(const nfi_render_params&, const nfi_render_grads&,
+                                        unsigned char*, unsigned, cudaStream_t);
 
 }  // namespace nfi

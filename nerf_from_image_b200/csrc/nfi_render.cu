@@ -4,49 +4,21 @@
 //        (nerf_from_image_b200/csrc/build.sh).  No torch, no CPU fallback: on a
 //        machine without an sm_90 device every launch returns an error.
 #include <cuda_runtime.h>
+#include <stdarg.h>
 #include <stdio.h>
-#include <string.h>
 
 #include "nfi_backward.cuh"
 #include "nfi_weight_image.cuh"
-#include "nfi_field_launch.h"
 #include "nfi_pipe_launch.h"
 #include "nfi_render.h"
 #include "nfi_route.h"
-#include "nfi_heads.h"
-#include "nfi_heads_launch.h"
-#include "nfi_disc.h"
-#include "nfi_disc_launch.h"
-#include "nfi_encoder.h"
-#include "nfi_encoder_launch.h"
-#include "nfi_lpips.h"
-#include "nfi_lpips_launch.h"
-#include "nfi_segformer.h"
-#include "nfi_segformer_launch.h"
-#include "nfi_synth.h"
-#include "nfi_synth_launch.h"
 
 #define NFI_STR_(x) #x
 #define NFI_STR(x) NFI_STR_(x)
 
+using nfi::fail;
+
 namespace {
-
-thread_local char g_err[512] = "";
-
-int fail(const char* fmt, const char* detail = "") {
-  snprintf(g_err, sizeof(g_err), fmt, detail);
-  return 1;
-}
-
-#define NFI_CUDA(expr)                                                      \
-  do {                                                                      \
-    cudaError_t e__ = (expr);                                               \
-    if (e__ != cudaSuccess) {                                               \
-      snprintf(g_err, sizeof(g_err), "%s failed: %s", #expr,                \
-               cudaGetErrorString(e__));                                    \
-      return 2;                                                             \
-    }                                                                       \
-  } while (0)
 
 int check_params(const nfi_render_params* p) {
   if (p == nullptr) return fail("params is NULL");
@@ -244,7 +216,18 @@ planes_from_cl_kernel(const float* __restrict__ src, int RR, float* __restrict__
   }
 }
 
+// the text behind nfi_last_error, one per host thread
+thread_local char g_err[512] = "";
+
 }  // namespace
+
+int nfi::fail(const char* fmt, ...) {
+  va_list ap;
+  va_start(ap, fmt);
+  vsnprintf(g_err, sizeof(g_err), fmt, ap);
+  va_end(ap);
+  return 1;
+}
 
 extern "C" {
 
@@ -303,7 +286,7 @@ int nfi_render_forward(const nfi_render_params* params, void* stream) {
   for (int q = 0; q < p.n_peers; ++q)
     if (!p.peer_rgb[q] || !p.peer_depth[q] || !p.peer_mask[q]) return fail("peer output pointer is NULL");
   const nfi::Plan r = nfi::route_forward(p);
-  if (r.route == nfi::Route::kRefused) return fail(r.refusal);
+  if (r.route == nfi::Route::kRefused) return fail("%s", r.refusal);
   const FwdWorkspace ws = fwd_workspace(p, r);
   if ((is_pipe(r.route) || p.fine_sampling) && (!p.workspace || p.workspace_bytes < ws.total))
     return fail("workspace too small (see nfi_render_workspace_bytes)");
@@ -312,17 +295,17 @@ int nfi_render_forward(const nfi_render_params* params, void* stream) {
     nfi_render_params ps = p;  // SIMT scratch starts after the weight-image header
     if (ps.workspace) ps.workspace = wsp + ws.scratch;
     if (r.route == nfi::Route::kSimtVd)
-      return nfi::launch_forward_simt<true>(ps, nfi::wants_normals(p), st, g_err, sizeof(g_err));
-    return nfi::launch_forward_simt<false>(ps, nfi::wants_normals(p), st, g_err, sizeof(g_err));
+      return nfi::launch_forward_simt<true>(ps, nfi::wants_normals(p), st);
+    return nfi::launch_forward_simt<false>(ps, nfi::wants_normals(p), st);
   }
   unsigned grid = 0;
   if (int rc = persistent_grid(p, &grid)) return rc;
   float* scratch = (float*)(wsp + ws.scratch);
   const int rc = r.route == nfi::Route::kPipeVd
-                     ? nfi::launch_pipe_forward<true>(p, wsp, scratch, grid, st, g_err, sizeof(g_err))
-                     : nfi::launch_pipe_forward<false>(p, wsp, scratch, grid, st, g_err, sizeof(g_err));
+                     ? nfi::launch_pipe_forward<true>(p, wsp, scratch, grid, st)
+                     : nfi::launch_pipe_forward<false>(p, wsp, scratch, grid, st);
   if (rc || !r.normals_pipe) return rc;
-  return nfi::launch_pipe_normals(p, wsp, wsp + ws.normals_image, grid, st, g_err, sizeof(g_err));
+  return nfi::launch_pipe_normals(p, wsp, wsp + ws.normals_image, grid, st);
 }
 
 int nfi_decoder_forward(const float* features, int64_t n_points, const float* w1, const float* b1,
@@ -380,269 +363,23 @@ int nfi_render_backward(const nfi_render_params* params, const nfi_render_grads*
   cudaStream_t st = (cudaStream_t)stream;
   const nfi::Plan r = nfi::route_backward(p, g);
   switch (r.route) {
-    case nfi::Route::kRefused: return fail(r.refusal);
-    case nfi::Route::kSimt: return nfi::launch_backward_simt<false>(p, g, st, g_err, sizeof(g_err));
-    case nfi::Route::kSimtVd: return nfi::launch_backward_simt<true>(p, g, st, g_err, sizeof(g_err));
+    case nfi::Route::kRefused: return fail("%s", r.refusal);
+    case nfi::Route::kSimt: return nfi::launch_backward_simt<false>(p, g, st);
+    case nfi::Route::kSimtVd: return nfi::launch_backward_simt<true>(p, g, st);
     default: break;
   }
   unsigned char* ws = (unsigned char*)p.workspace;
   unsigned grid = 0;  // <= kMaxPersistentCtas: the accumulator rows are sized for that many CTAs
   if (int rc = persistent_grid(p, &grid)) return rc;
   if (r.route == nfi::Route::kPipeVd)
-    return nfi::launch_pipe_backward<true>(p, g, ws, grid, st, g_err, sizeof(g_err));
+    return nfi::launch_pipe_backward<true>(p, g, ws, grid, st);
   if (r.route == nfi::Route::kPipe || r.route == nfi::Route::kPipeAndWgrad) {
     nfi_render_grads g1 = g;  // the decoder gradients are render_wgrad_pipe's
     g1.grad_w1 = g1.grad_b1 = g1.grad_w2 = g1.grad_b2 = nullptr;
-    if (int rc = nfi::launch_pipe_backward<false>(p, g1, ws, grid, st, g_err, sizeof(g_err)))
-      return rc;
+    if (int rc = nfi::launch_pipe_backward<false>(p, g1, ws, grid, st)) return rc;
     if (r.route == nfi::Route::kPipe) return 0;
   }
-  return nfi::launch_pipe_wgrad(p, g, ws, grid, r.route == nfi::Route::kWgradOneSweep, st, g_err,
-                                sizeof(g_err));
-}
-
-int nfi_sample_field(const nfi_sample_params* sp, void* stream) {
-  if (sp == nullptr) return fail("params is NULL");
-  if (sp->batch <= 0 || sp->batch > 65535 || sp->n_points <= 0) return fail("empty point set");
-  if (sp->n_points > ((int64_t)1 << 37)) return fail("too many points per image");
-  if (sp->plane_res < 2) return fail("plane_res must be >= 2");
-  if (sp->n_attention < 0 || sp->n_attention > NFI_MAX_ATTENTION)
-    return fail("attention_values must be in [0, 15]");
-  if (!(sp->scene_range > 0.f)) return fail("scene_range must be positive");
-  if (!sp->planes || !sp->w1 || !sp->b1 || !sp->w2 || !sp->b2 || !sp->points)
-    return fail("planes / decoder weights / points must be given");
-  if (sp->n_attention > 0 && !sp->palette)
-    return fail("palette missing (attention_values > 0)");
-  if (sp->use_sdf && (!sp->beta || !sp->alpha)) return fail("use_sdf needs beta and alpha");
-  if (sp->semantics && sp->n_attention <= 0)
-    return fail("'semantics' needs attention_values > 0");  // generator.py:673
-  if (sp->normals && !sp->use_sdf) return fail("'normals' needs use_sdf");  // generator.py:600
-  if (sp->bbox_debug && !sp->sigma) return fail("bbox_debug modifies sigma: request it");
-  if (!sp->sdf_distance && !sp->sigma && !sp->rgb && !sp->semantics && !sp->normals)
-    return fail("no sampler output requested");
-  nfi_render_params p;
-  memset(&p, 0, sizeof(p));
-  p.batch = sp->batch;
-  p.plane_res = sp->plane_res;
-  p.n_attention = sp->n_attention;
-  p.use_sdf = sp->use_sdf;
-  p.scene_range = sp->scene_range;
-  p.planes = sp->planes;
-  p.w1 = sp->w1;
-  p.b1 = sp->b1;
-  p.w2 = sp->w2;
-  p.b2 = sp->b2;
-  p.palette = sp->palette;
-  p.beta = sp->beta;
-  p.alpha = sp->alpha;
-  return nfi::launch_sample_field(p, *sp, nfi::nout_pad_of(p.n_attention), (cudaStream_t)stream,
-                                  g_err, sizeof(g_err));
-}
-
-int nfi_pose_to_matrix(const float* z0, const float* t2, const float* s, const float* q,
-                       int32_t camera_flipped, int32_t batch, float* c2w, float* focal,
-                       void* stream) {
-  if (batch <= 0) return fail("empty batch");
-  if (!t2 || !s || !q || !c2w) return fail("t2 / s / q / c2w must be given");
-  if (z0 && !focal) return fail("perspective pose (z0 given) needs the focal output");
-  return nfi::launch_pose_to_matrix(z0, t2, s, q, camera_flipped, batch, c2w, focal,
-                                    (cudaStream_t)stream, g_err, sizeof(g_err));
-}
-
-int nfi_pose_to_matrix_backward(const float* z0, const float* t2, const float* s, const float* q,
-                                int32_t camera_flipped, int32_t batch, const float* g_c2w,
-                                const float* g_focal, float* g_z0, float* g_t2, float* g_s,
-                                float* g_q, void* stream) {
-  if (batch <= 0) return fail("empty batch");
-  if (!t2 || !s || !q || !g_c2w || !g_t2 || !g_s || !g_q)
-    return fail("t2 / s / q / g_c2w and the three gradient outputs must be given");
-  if (z0 && !g_z0) return fail("perspective pose (z0 given) needs g_z0");
-  return nfi::launch_pose_to_matrix_backward(z0, t2, s, q, camera_flipped, batch, g_c2w, g_focal,
-                                             g_z0, g_t2, g_s, g_q, (cudaStream_t)stream, g_err,
-                                             sizeof(g_err));
-}
-
-static int check_sdf_points(const nfi_sdf_points_params* p) {
-  if (p == nullptr) return fail("params is NULL");
-  if (p->batch <= 0 || p->n_points <= 0 || p->plane_res < 2) return fail("empty batch / no points");
-  if (!p->planes || !p->w1 || !p->b1 || !p->w2 || !p->b2 || !p->points)
-    return fail("planes, decoder weights and points must be given");
-  if (!(p->scene_range > 0.f)) return fail("scene_range must be positive");
-  return 0;
-}
-
-int nfi_sdf_points_forward(const nfi_sdf_points_params* params, void* stream) {
-  if (const int rc = check_sdf_points(params)) return rc;
-  if (!params->d) return fail("output d must be given");
-  return nfi::heads::launch_forward(*params, (cudaStream_t)stream, g_err, sizeof(g_err));
-}
-
-int nfi_sdf_points_backward(const nfi_sdf_points_params* params, const nfi_sdf_points_grads* grads,
-                            void* stream) {
-  if (const int rc = check_sdf_points(params)) return rc;
-  if (grads == nullptr) return fail("grads is NULL");
-  if (!grads->g_d && !grads->g_grad) return fail("no upstream gradient");
-  if (grads->grad_w1 && (!grads->grad_b1 || !grads->grad_w2_row0 || !grads->grad_b2_0))
-    return fail("decoder gradients come as a set: grad_w1, grad_b1, grad_w2_row0, grad_b2_0");
-  return nfi::heads::launch_backward(*params, *grads, (cudaStream_t)stream, g_err, sizeof(g_err));
-}
-
-size_t nfi_lpips_workspace_bytes(const nfi_lpips_params* params) {
-  if (params == nullptr) return 0;
-  return nfi::lpips::workspace_bytes(*params);
-}
-
-int nfi_lpips_forward(const nfi_lpips_params* params, void* stream) {
-  if (params == nullptr) return fail("params is NULL");
-  return nfi::lpips::forward(*params, (cudaStream_t)stream, g_err, sizeof(g_err));
-}
-
-int nfi_lpips_backward(const nfi_lpips_params* params, const float* g_dist, float* grad_in0, float* grad_in1,
-                       void* stream) {
-  if (params == nullptr) return fail("params is NULL");
-  return nfi::lpips::backward(*params, g_dist, grad_in0, grad_in1, (cudaStream_t)stream, g_err,
-                              sizeof(g_err));
-}
-
-int nfi_lpips_saved_preactivation(const nfi_lpips_params* params, int32_t layer, float* out, void* stream) {
-  if (params == nullptr) return fail("params is NULL");
-  return nfi::lpips::saved_preactivation(*params, layer, out, (cudaStream_t)stream, g_err, sizeof(g_err));
-}
-
-size_t nfi_encoder_workspace_bytes(const nfi_encoder_params* params) {
-  if (params == nullptr) return 0;
-  return nfi::encoder::workspace_bytes(*params);
-}
-
-int nfi_encoder_forward(const nfi_encoder_params* params, void* stream) {
-  if (params == nullptr) return fail("params is NULL");
-  return nfi::encoder::forward(*params, (cudaStream_t)stream, g_err, sizeof(g_err));
-}
-
-int nfi_encoder_backward(const nfi_encoder_params* params, const float* g_maps, const float* g_pooled,
-                         const nfi_encoder_grads* grads, void* stream) {
-  if (params == nullptr || grads == nullptr) return fail("params / grads is NULL");
-  return nfi::encoder::backward(*params, g_maps, g_pooled, *grads, (cudaStream_t)stream, g_err, sizeof(g_err));
-}
-
-int nfi_encoder_saved_activation(const nfi_encoder_params* params, int32_t layer, float* out, void* stream) {
-  if (params == nullptr) return fail("params is NULL");
-  return nfi::encoder::saved_activation(*params, layer, out, (cudaStream_t)stream, g_err, sizeof(g_err));
-}
-
-size_t nfi_segformer_workspace_bytes(const nfi_segformer_params* params) {
-  if (params == nullptr) return 0;
-  return nfi::segformer::workspace_bytes(*params);
-}
-
-int nfi_segformer_forward(const nfi_segformer_params* params, void* stream) {
-  if (params == nullptr) return fail("params is NULL");
-  return nfi::segformer::forward(*params, (cudaStream_t)stream, g_err, sizeof(g_err));
-}
-
-int nfi_segformer_backward(const nfi_segformer_params* params, const float* g_features, float* const* grads,
-                           void* stream) {
-  if (params == nullptr) return fail("params is NULL");
-  return nfi::segformer::backward(*params, g_features, grads, (cudaStream_t)stream, g_err, sizeof(g_err));
-}
-
-size_t nfi_disc_workspace_bytes(const nfi_disc_params* params) {
-  if (params == nullptr) return 0;
-  return nfi::disc::workspace_bytes(*params);
-}
-
-int nfi_disc_forward(const nfi_disc_params* params, void* stream) {
-  if (params == nullptr) return fail("params is NULL");
-  return nfi::disc::forward(*params, (cudaStream_t)stream, g_err, sizeof(g_err));
-}
-
-int nfi_disc_backward(const nfi_disc_params* params, const float* g_logits, float* grad_img, float* grad_cmap,
-                      const nfi_disc_grads* grads, void* stream) {
-  if (params == nullptr || grads == nullptr) return fail("params / grads is NULL");
-  return nfi::disc::backward(*params, g_logits, grad_img, grad_cmap, *grads, (cudaStream_t)stream, g_err,
-                             sizeof(g_err));
-}
-
-int nfi_disc_saved_preactivation(const nfi_disc_params* params, int32_t block, int32_t which, float* out,
-                                 void* stream) {
-  if (params == nullptr) return fail("params is NULL");
-  return nfi::disc::saved_preactivation(*params, block, which, out, (cudaStream_t)stream, g_err, sizeof(g_err));
-}
-
-size_t nfi_disc_r1_scratch_bytes(const nfi_disc_params* params) {
-  if (params == nullptr) return 0;
-  return nfi::disc::hvp_scratch_bytes(*params);
-}
-
-int nfi_disc_backward_hvp(const nfi_disc_params* params, const nfi_disc_hvp* hvp, const nfi_disc_grads* grads,
-                          void* stream) {
-  if (params == nullptr || hvp == nullptr || grads == nullptr) return fail("params / hvp / grads is NULL");
-  return nfi::disc::backward_hvp(*params, *hvp, *grads, (cudaStream_t)stream, g_err, sizeof(g_err));
-}
-
-size_t nfi_synthesis_workspace_bytes(const nfi_synth_params* params) {
-  if (params == nullptr) return 0;
-  return nfi::synth::workspace_bytes(*params);
-}
-
-int nfi_synthesis_forward(const nfi_synth_params* params, void* stream) {
-  if (params == nullptr) return fail("params is NULL");
-  if (params->batch <= 0) return fail("empty batch");
-  return nfi::synth::forward(*params, (cudaStream_t)stream, g_err, sizeof(g_err));
-}
-
-size_t nfi_synthesis_saved_workspace_bytes(const nfi_synth_params* params) {
-  if (params == nullptr) return 0;
-  return nfi::synth::saved_workspace_bytes(*params);
-}
-
-int nfi_synthesis_forward_saved(const nfi_synth_params* params, void* stream) {
-  if (params == nullptr) return fail("params is NULL");
-  if (params->batch <= 0) return fail("empty batch");
-  return nfi::synth::forward_saved(*params, (cudaStream_t)stream, g_err, sizeof(g_err));
-}
-
-int nfi_synthesis_backward(const nfi_synth_params* params, const nfi_synth_grads* grads, void* stream) {
-  if (params == nullptr) return fail("params is NULL");
-  if (grads == nullptr) return fail("grads is NULL");
-  if (params->batch <= 0) return fail("empty batch");
-  return nfi::synth::backward(*params, *grads, (cudaStream_t)stream, g_err, sizeof(g_err));
-}
-
-int nfi_synthesis_saved_preactivation(const nfi_synth_params* params, int32_t block, int32_t which,
-                                      float* out, void* stream) {
-  if (params == nullptr) return fail("params is NULL");
-  if (params->batch <= 0) return fail("empty batch");
-  return nfi::synth::saved_preactivation(*params, block, which, out, (cudaStream_t)stream, g_err,
-                                         sizeof(g_err));
-}
-
-size_t nfi_synthesis_param_workspace_bytes(const nfi_synth_params* params) {
-  if (params == nullptr) return 0;
-  return nfi::synth::param_workspace_bytes(*params);
-}
-
-int nfi_synthesis_backward_params(const nfi_synth_params* params, const nfi_synth_grads* grads,
-                                  const nfi_synth_param_grads* param_grads, void* stream) {
-  if (params == nullptr) return fail("params is NULL");
-  if (grads == nullptr) return fail("grads is NULL");
-  if (param_grads == nullptr) return fail("param_grads is NULL");
-  if (params->batch <= 0) return fail("empty batch");
-  return nfi::synth::backward_params(*params, *grads, *param_grads, (cudaStream_t)stream, g_err,
-                                     sizeof(g_err));
-}
-
-size_t nfi_synthesis_hvp_scratch_bytes(const nfi_synth_params* params) {
-  if (params == nullptr) return 0;
-  return nfi::synth::hvp_scratch_bytes(*params);
-}
-
-int nfi_synthesis_backward_hvp(const nfi_synth_params* params, const nfi_synth_hvp* hvp,
-                               const nfi_synth_param_grads* param_grads, void* stream) {
-  if (params == nullptr) return fail("params is NULL");
-  if (hvp == nullptr) return fail("hvp is NULL");
-  if (params->batch <= 0) return fail("empty batch");
-  return nfi::synth::backward_hvp(*params, *hvp, param_grads, (cudaStream_t)stream, g_err, sizeof(g_err));
+  return nfi::launch_pipe_wgrad(p, g, ws, grid, r.route == nfi::Route::kWgradOneSweep, st);
 }
 
 int nfi_render_forward_host(const nfi_render_params* hp, int32_t device) {
@@ -678,8 +415,7 @@ int nfi_render_forward_host(const nfi_render_params* hp, int32_t device) {
       if (pool_changed) cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &old_keep);
       if (cp) cudaStreamDestroy(cp);
       if (st) cudaStreamDestroy(st);
-      snprintf(g_err, sizeof(g_err), "host entry point set-up failed: %s", cudaGetErrorString(e0));
-      return 2;
+      return fail("host entry point set-up failed: %s", cudaGetErrorString(e0)), 2;
     }
   }
 
@@ -817,7 +553,7 @@ int nfi_render_forward_host(const nfi_render_params* hp, int32_t device) {
   if (pool_changed) cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &old_keep);
   if (e == cudaSuccess) e = e1;
   if (!rc && e != cudaSuccess) {
-    snprintf(g_err, sizeof(g_err), "render failed: %s", cudaGetErrorString(e));
+    fail("render failed: %s", cudaGetErrorString(e));
     rc = 2;
   }
   return rc;

@@ -26,12 +26,10 @@
 #include <cuda_runtime.h>
 #include <limits.h>
 #include <math.h>
-#include <stdio.h>
 #include <string.h>
 
 #include "nfi_pair.cuh"
 #include "nfi_segformer.h"
-#include "nfi_segformer_launch.h"
 #include "nfi_synth_launch.h"
 
 namespace nfi {
@@ -902,40 +900,27 @@ static void layout(const nfi_segformer_params& P, Bump& b, Layout& L) {
   }
 }
 
-static int check(const nfi_segformer_params& P, char* err, size_t err_len) {
+static int check(const nfi_segformer_params& P) {
   if (P.batch <= 0 || P.batch > 65535 || P.height != P.width || P.height < 32 || P.height > 256 ||
-      P.height % 32 != 0) {
-    snprintf(err, err_len, "segformer: B in 1..65535 and a square image with H a multiple of 32 in 32..256 "
-                           "needed, got B %d, %d x %d", P.batch, P.height, P.width);
-    return 1;
-  }
+      P.height % 32 != 0)
+    return fail("segformer: B in 1..65535 and a square image with H a multiple of 32 in 32..256 "
+                "needed, got B %d, %d x %d", P.batch, P.height, P.width);
   const size_t M0 = (size_t)P.batch * (P.height / 4) * (P.height / 4);
-  if (M0 * kDec > (size_t)INT_MAX || M0 * P.out_features > (size_t)INT_MAX) {
-    snprintf(err, err_len, "segformer: more than 2^31 head activations (B %d, %d x %d)", P.batch, P.height,
-             P.width);
-    return 1;
-  }
+  if (M0 * kDec > (size_t)INT_MAX || M0 * P.out_features > (size_t)INT_MAX)
+    return fail("segformer: more than 2^31 head activations (B %d, %d x %d)", P.batch, P.height, P.width);
   for (int i = 0; i < kStages; ++i)
-    if (P.depths[i] < 1 || P.depths[i] > kMaxDepth) {
-      snprintf(err, err_len, "segformer: depths in 1..%d, got %d in stage %d", kMaxDepth, P.depths[i], i + 1);
-      return 1;
-    }
-  if (P.out_features <= 0 || P.out_features % 64 != 0 || P.out_features > 4096) {
-    snprintf(err, err_len, "segformer: out_features must be a multiple of 64 in 64..4096, got %d", P.out_features);
-    return 1;
-  }
-  if (P.save != 0 && P.save != 1) {
-    snprintf(err, err_len, "segformer: save must be 0 or 1, got %d", P.save);
-    return 1;
-  }
+    if (P.depths[i] < 1 || P.depths[i] > kMaxDepth)
+      return fail("segformer: depths in 1..%d, got %d in stage %d", kMaxDepth, P.depths[i], i + 1);
+  if (P.out_features <= 0 || P.out_features % 64 != 0 || P.out_features > 4096)
+    return fail("segformer: out_features must be a multiple of 64 in 64..4096, got %d", P.out_features);
+  if (P.save != 0 && P.save != 1) return fail("segformer: save must be 0 or 1, got %d", P.save);
   return 0;
 }
 
 }  // namespace
 
 size_t workspace_bytes(const nfi_segformer_params& P) {
-  char err[160];
-  if (check(P, err, sizeof(err))) return 0;
+  if (check(P)) return 0;
   Bump b{nullptr, 0, 0};
   Layout L;
   layout(P, b, L);
@@ -944,77 +929,66 @@ size_t workspace_bytes(const nfi_segformer_params& P) {
 
 namespace {
 
-static int setup(const nfi_segformer_params& P, Layout& L, Index& X, char* err, size_t err_len) {
-  if (const int rc = check(P, err, err_len)) return rc;
-  if (!P.image || !P.params || !P.features || !P.workspace) {
-    snprintf(err, err_len, "segformer: image, params, features and workspace must be set");
-    return 1;
-  }
+static int setup(const nfi_segformer_params& P, Layout& L, Index& X) {
+  if (const int rc = check(P)) return rc;
+  if (!P.image || !P.params || !P.features || !P.workspace)
+    return fail("segformer: image, params, features and workspace must be set");
   X = index_of(P);
   for (int j = 0; j < X.total; ++j)
-    if (!P.params[j]) {
-      snprintf(err, err_len, "segformer: parameter %d of %d is NULL", j, X.total);
-      return 1;
-    }
+    if (!P.params[j]) return fail("segformer: parameter %d of %d is NULL", j, X.total);
   const size_t need = workspace_bytes(P);
-  if (P.workspace_bytes < need) {
-    snprintf(err, err_len, "segformer: workspace too small (%zu < %zu bytes)", P.workspace_bytes, need);
-    return 1;
-  }
+  if (P.workspace_bytes < need)
+    return fail("segformer: workspace too small (%zu < %zu bytes)", P.workspace_bytes, need);
   Bump b = aligned_bump(P.workspace, P.workspace_bytes);
   layout(P, b, L);
   return 0;
 }
 
 // one token GEMM: out [Mp,N] = in [Mp,K] w^T, w the pair [N][K]
-static int gemm(size_t Mp, int K, int N, Pair in, Pair w, float* out, cudaStream_t st, char* err, size_t len) {
-  return synth::conv1x1((int)(Mp / kRows), 16, K, N, in, w, out, st, err, len);
+static int gemm(size_t Mp, int K, int N, Pair in, Pair w, float* out, cudaStream_t st) {
+  return synth::conv1x1((int)(Mp / kRows), 16, K, N, in, w, out, st);
 }
 // g_w [cout][cin] += g^T x over Mp rows
-static int wgrad(size_t Mp, int cout, int cin, Pair g, Pair x, float* part, float* g_w, cudaStream_t st, char* err,
-                 size_t len) {
-  return synth::wgrad1x1((int)(Mp / kRows), 16, cout, cin, g, x, part, g_w, st, err, len);
+static int wgrad(size_t Mp, int cout, int cin, Pair g, Pair x, float* part, float* g_w, cudaStream_t st) {
+  return synth::wgrad1x1((int)(Mp / kRows), 16, cout, cin, g, x, part, g_w, st);
 }
 // a linear layer's weight [cout][cin] (row pitch ld) as the pair [cout][cin] of its GEMM, or
 // [cin][cout] (transposed) of its data gradient's
-static int prep(const float* w, int cout, int cin, int ld, bool transposed, Pair out, cudaStream_t st, char* err,
-                size_t err_len) {
-  return synth::prep_weights(w, cout, cin, 1, ld, 1.f, transposed ? synth::kTapCiCo : synth::kTapCoCi, out, st, err,
-                             err_len);
+static int prep(const float* w, int cout, int cin, int ld, bool transposed, Pair out, cudaStream_t st) {
+  return synth::prep_weights(w, cout, cin, 1, ld, 1.f, transposed ? synth::kTapCiCo : synth::kTapCoCi, out, st);
 }
-static int ln(const LnFwd& a, cudaStream_t st, char* err, size_t err_len) {
+static int ln(const LnFwd& a, cudaStream_t st) {
   ln_kernel<<<blocks((size_t)a.rows, 8), 256, 0, st>>>(a);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
-static int reduce(const float* partial, int n_chunks, int stride, int n, float* out, cudaStream_t st, char* err,
-                  size_t err_len) {
+static int reduce(const float* partial, int n_chunks, int stride, int n, float* out, cudaStream_t st) {
   if (out == nullptr) return 0;
   reduce_kernel<<<blocks((size_t)n, 32), 256, 0, st>>>(partial, n_chunks, stride, n, out);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 // the LN backward and its affine gradients
-static int ln_backward(const LnBwd& a, float* g_w, float* g_b, cudaStream_t st, char* err, size_t err_len) {
+static int ln_backward(const LnBwd& a, float* g_w, float* g_b, cudaStream_t st) {
   const unsigned n = blocks((size_t)a.M, kLnRows);
   ln_backward_kernel<<<n, 256, 0, st>>>(a);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  if (int rc = reduce(a.partial, (int)n, 2 * a.C, a.C, g_w, st, err, err_len)) return rc;
-  return reduce(a.partial + a.C, (int)n, 2 * a.C, a.C, g_b, st, err, err_len);
+  NFI_CUDA(cudaGetLastError());
+  if (int rc = reduce(a.partial, (int)n, 2 * a.C, a.C, g_w, st)) return rc;
+  return reduce(a.partial + a.C, (int)n, 2 * a.C, a.C, g_b, st);
 }
-static int act(const Act& a, float* g_b, cudaStream_t st, char* err, size_t err_len) {
+static int act(const Act& a, float* g_b, cudaStream_t st) {
   const unsigned n = blocks((size_t)a.rows, kChunk);
   act_kernel<<<dim3(n, (unsigned)(a.C / 32)), 256, 0, st>>>(a);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  return g_b ? reduce(a.partial, (int)n, a.C, a.C, g_b, st, err, err_len) : 0;
+  NFI_CUDA(cudaGetLastError());
+  return g_b ? reduce(a.partial, (int)n, a.C, a.C, g_b, st) : 0;
 }
 
 }  // namespace
 
-int forward(const nfi_segformer_params& P, cudaStream_t st, char* err, size_t err_len) {
+int forward(const nfi_segformer_params& P, cudaStream_t st) {
   Layout L;
   Index X;
-  if (const int rc = setup(P, L, X, err, err_len)) return rc;
+  if (const int rc = setup(P, L, X)) return rc;
   const float* const* W = P.params;
   const int B = P.batch, H = P.height, out = P.out_features;
   int gk = 0;  // blocks so far (the drop-path scale rows)
@@ -1029,72 +1003,71 @@ int forward(const nfi_segformer_params& P, cudaStream_t st, char* err, size_t er
       const int Cp = kDims[i - 1];
       phases_kernel<<<flat_grid((size_t)4 * B * (s.r + 1) * (s.r + 1) * Cp), 256, 0, st>>>(L.s[i - 1].feat, B, s.r,
                                                                                           Cp, S.ph.hi, S.ph.lo);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
-      if (int rc = synth::prep_weights(W[pe], C, Cp, 9, 9 * Cp, 1.f, synth::kTapCoCi, L.w, st, err, err_len))
+      NFI_CUDA(cudaGetLastError());
+      if (int rc = synth::prep_weights(W[pe], C, Cp, 9, 9 * Cp, 1.f, synth::kTapCoCi, L.w, st))
         return rc;
-      if (int rc = synth::conv_down3x3(B, s.r, Cp, C, S.ph, L.w, S.pe, st, err, err_len)) return rc;
+      if (int rc = synth::conv_down3x3(B, s.r, Cp, C, S.ph, L.w, S.pe, st)) return rc;
     }
-    NFI_LAUNCH_CHECK(cudaGetLastError());
+    NFI_CUDA(cudaGetLastError());
     LnFwd a;
     memset(&a, 0, sizeof(a));
     a.M = a.rows = (int)s.M; a.C = C; a.per_img = s.N;
     a.y = S.pe; a.bias = W[pe + 1]; a.s_out = S.pe; a.w = W[pe + 2]; a.b = W[pe + 3]; a.eps = kEpsEmbed;
     a.out = S.blk[0].x; a.stats = S.pst;
-    if (int rc = ln(a, st, err, err_len)) return rc;
+    if (int rc = ln(a, st)) return rc;
     // norm1 of block 0
     const int nb0 = X.blk[i][0];
     memset(&a, 0, sizeof(a));
     a.M = (int)s.M; a.rows = (int)s.Mp; a.C = C; a.per_img = s.N;
     a.x = S.blk[0].x; a.w = W[nb0 + kN1]; a.b = W[nb0 + kN1 + 1]; a.eps = kEpsBlock;
     a.pair = S.blk[0].a1; a.stats = S.blk[0].st1;
-    if (int rc = ln(a, st, err, err_len)) return rc;
+    if (int rc = ln(a, st)) return rc;
     for (int k = 0; k < P.depths[i]; ++k, ++gk) {
       Blk& K = S.blk[k];
       const int nb = X.blk[i][k], o2 = nb + blk_off(s.sr);
       const float* sc_a = P.drop_scales ? P.drop_scales + (size_t)(2 * gk) * B : nullptr;
       const float* sc_m = P.drop_scales ? P.drop_scales + (size_t)(2 * gk + 1) * B : nullptr;
-      if (int rc = prep(W[nb + kQw], C, C, C, false, L.w, st, err, err_len)) return rc;
-      if (int rc = gemm(s.Mp, C, C, K.a1, L.w, K.q, st, err, err_len)) return rc;
+      if (int rc = prep(W[nb + kQw], C, C, C, false, L.w, st)) return rc;
+      if (int rc = gemm(s.Mp, C, C, K.a1, L.w, K.q, st)) return rc;
       Pair kvin = K.a1;
       if (s.sr > 1) {
         s2d_kernel<<<flat_grid(s.Mrp * s.K), 256, 0, st>>>(K.a1, B, s.r, s.sr, C, (int)s.Mrp, K.sd);
-        NFI_LAUNCH_CHECK(cudaGetLastError());
-        if (int rc = synth::prep_weights(W[nb + kSrW], C, C, s.sr * s.sr, s.K, 1.f, synth::kCoTapCi, L.w, st, err,
-                                         err_len))
+        NFI_CUDA(cudaGetLastError());
+        if (int rc = synth::prep_weights(W[nb + kSrW], C, C, s.sr * s.sr, s.K, 1.f, synth::kCoTapCi, L.w, st))
           return rc;
-        if (int rc = gemm(s.Mrp, s.K, C, K.sd, L.w, K.sr, st, err, err_len)) return rc;
+        if (int rc = gemm(s.Mrp, s.K, C, K.sd, L.w, K.sr, st)) return rc;
         memset(&a, 0, sizeof(a));
         a.M = (int)s.Mr; a.rows = (int)s.Mrp; a.C = C; a.per_img = s.Nk;
         a.y = K.sr; a.bias = W[nb + kSrW + 1]; a.s_out = K.sr; a.w = W[nb + kSrN]; a.b = W[nb + kSrN + 1];
         a.eps = kEpsEmbed; a.pair = K.xr; a.stats = K.str;
-        if (int rc = ln(a, st, err, err_len)) return rc;
+        if (int rc = ln(a, st)) return rc;
         kvin = K.xr;
       }
-      if (int rc = prep(W[nb + kKv], 2 * C, C, C, false, L.w, st, err, err_len)) return rc;
-      if (int rc = gemm(s.Mkv, C, 2 * C, kvin, L.w, K.kv, st, err, err_len)) return rc;
-      NFI_LAUNCH_CHECK(cudaFuncSetAttribute(attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem));
+      if (int rc = prep(W[nb + kKv], 2 * C, C, C, false, L.w, st)) return rc;
+      if (int rc = gemm(s.Mkv, C, 2 * C, kvin, L.w, K.kv, st)) return rc;
+      NFI_CUDA(cudaFuncSetAttribute(attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem));
       attn_kernel<<<dim3(blocks(s.N, kQ), s.heads, B), 256, kAttnSmem, st>>>(K.q, W[nb + kQw + 1], K.kv,
                                                                               W[nb + kKv + 1], s.N, s.Nk, C, K.o, K.op);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
+      NFI_CUDA(cudaGetLastError());
       if (s.Mp > s.M) {
         const size_t pad = (s.Mp - s.M) * C * sizeof(__nv_bfloat16);
-        NFI_LAUNCH_CHECK(cudaMemsetAsync(K.op.hi + s.M * C, 0, pad, st));
-        NFI_LAUNCH_CHECK(cudaMemsetAsync(K.op.lo + s.M * C, 0, pad, st));
+        NFI_CUDA(cudaMemsetAsync(K.op.hi + s.M * C, 0, pad, st));
+        NFI_CUDA(cudaMemsetAsync(K.op.lo + s.M * C, 0, pad, st));
       }
-      if (int rc = prep(W[nb + kProj], C, C, C, false, L.w, st, err, err_len)) return rc;
-      if (int rc = gemm(s.Mp, C, C, K.op, L.w, L.y, st, err, err_len)) return rc;
+      if (int rc = prep(W[nb + kProj], C, C, C, false, L.w, st)) return rc;
+      if (int rc = gemm(s.Mp, C, C, K.op, L.w, L.y, st)) return rc;
       memset(&a, 0, sizeof(a));
       a.M = (int)s.M; a.rows = (int)s.Mp; a.C = C; a.per_img = s.N;
       a.x = K.x; a.y = L.y; a.bias = W[nb + kProj + 1]; a.scale = sc_a; a.s_out = K.x1;
       a.w = W[o2]; a.b = W[o2 + 1]; a.eps = kEpsBlock; a.pair = K.a2; a.stats = K.st2;
-      if (int rc = ln(a, st, err, err_len)) return rc;
-      if (int rc = prep(W[o2 + 2], 4 * C, C, C, false, L.w, st, err, err_len)) return rc;
-      if (int rc = gemm(s.Mp, C, 4 * C, K.a2, L.w, K.h, st, err, err_len)) return rc;
+      if (int rc = ln(a, st)) return rc;
+      if (int rc = prep(W[o2 + 2], 4 * C, C, C, false, L.w, st)) return rc;
+      if (int rc = gemm(s.Mp, C, 4 * C, K.a2, L.w, K.h, st)) return rc;
       dw_gelu_kernel<<<flat_grid(s.Mp * 4 * C), 256, 0, st>>>(K.h, W[o2 + 3], W[o2 + 4], W[o2 + 5], B, s.r, 4 * C,
                                                               (int)s.Mp, K.z, K.g);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
-      if (int rc = prep(W[o2 + 6], C, 4 * C, 4 * C, false, L.w, st, err, err_len)) return rc;
-      if (int rc = gemm(s.Mp, 4 * C, C, K.g, L.w, L.y, st, err, err_len)) return rc;
+      NFI_CUDA(cudaGetLastError());
+      if (int rc = prep(W[o2 + 6], C, 4 * C, 4 * C, false, L.w, st)) return rc;
+      if (int rc = gemm(s.Mp, 4 * C, C, K.g, L.w, L.y, st)) return rc;
       // the residual, then the next norm: the next block's norm1, or the stage norm
       const bool last = k + 1 == P.depths[i];
       memset(&a, 0, sizeof(a));
@@ -1107,7 +1080,7 @@ int forward(const nfi_segformer_params& P, cudaStream_t st, char* err, size_t er
         const int nn = X.blk[i][k + 1];
         a.s_out = N1.x; a.w = W[nn + kN1]; a.b = W[nn + kN1 + 1]; a.pair = N1.a1; a.stats = N1.st1;
       }
-      if (int rc = ln(a, st, err, err_len)) return rc;
+      if (int rc = ln(a, st)) return rc;
     }
   }
   // decoder head: linear_c_i and linear_fuse's slice at stage i's resolution
@@ -1115,78 +1088,71 @@ int forward(const nfi_segformer_params& P, cudaStream_t st, char* err, size_t er
   for (int i = 0; i < kStages; ++i) {
     const Shape s = shape(P, i);
     StageBufs& S = L.s[i];
-    if (int rc = prep(W[X.lc[i]], kDec, s.C, s.C, false, L.w, st, err, err_len)) return rc;
-    if (int rc = gemm(s.Mp, s.C, kDec, S.fp, L.w, L.y, st, err, err_len)) return rc;
+    if (int rc = prep(W[X.lc[i]], kDec, s.C, s.C, false, L.w, st)) return rc;
+    if (int rc = gemm(s.Mp, s.C, kDec, S.fp, L.w, L.y, st)) return rc;
     Act c;
     memset(&c, 0, sizeof(c));
     c.M = (int)s.M; c.rows = (int)s.Mp; c.C = kDec; c.per_img = s.N; c.g = L.y; c.bias = W[X.lc[i] + 1]; c.out = S.cp;
-    if (int rc = act(c, nullptr, st, err, err_len)) return rc;
-    if (int rc = prep(W[X.fuse] + (kStages - 1 - i) * kDec, kDec, kDec, kStages * kDec, false, L.w, st, err, err_len))
+    if (int rc = act(c, nullptr, st)) return rc;
+    if (int rc = prep(W[X.fuse] + (kStages - 1 - i) * kDec, kDec, kDec, kStages * kDec, false, L.w, st))
       return rc;
-    if (int rc = gemm(s.Mp, kDec, kDec, S.cp, L.w, S.d, st, err, err_len)) return rc;
+    if (int rc = gemm(s.Mp, kDec, kDec, S.cp, L.w, S.d, st)) return rc;
     hd.d[i] = S.d;
   }
   const Shape s0 = shape(P, 0);
   upsample_sum_kernel<<<flat_grid(s0.Mp * kDec), 256, 0, st>>>(hd, B, s0.r, W[X.fuse + 1], (int)s0.Mp, L.u);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
-  if (int rc = prep(W[X.pred], out, kDec, kDec, false, L.w, st, err, err_len)) return rc;
-  if (int rc = gemm(s0.Mp, kDec, out, L.u, L.w, L.pred, st, err, err_len)) return rc;
-  return synth::transpose(L.pred, B, s0.N, out, W[X.pred + 1], 0, P.features, st, err, err_len);
+  NFI_CUDA(cudaGetLastError());
+  if (int rc = prep(W[X.pred], out, kDec, kDec, false, L.w, st)) return rc;
+  if (int rc = gemm(s0.Mp, kDec, out, L.u, L.w, L.pred, st)) return rc;
+  return synth::transpose(L.pred, B, s0.N, out, W[X.pred + 1], 0, P.features, st);
 }
 
-int backward(const nfi_segformer_params& P, const float* g_features, float* const* G, cudaStream_t st, char* err,
-             size_t err_len) {
-  if (!P.save) {
-    snprintf(err, err_len, "segformer backward: needs the workspace of a forward with save = 1");
-    return 1;
-  }
-  if (!g_features || !G) {
-    snprintf(err, err_len, "segformer backward: g_features and grads must be set");
-    return 1;
-  }
+int backward(const nfi_segformer_params& P, const float* g_features, float* const* G, cudaStream_t st) {
+  if (!P.save) return fail("segformer backward: needs the workspace of a forward with save = 1");
+  if (!g_features || !G) return fail("segformer backward: g_features and grads must be set");
   Layout L;
   Index X;
-  if (const int rc = setup(P, L, X, err, err_len)) return rc;
+  if (const int rc = setup(P, L, X)) return rc;
   const float* const* W = P.params;
   const int B = P.batch, H = P.height, out = P.out_features;
   const Shape s0 = shape(P, 0);
   // ---- head
-  if (int rc = synth::transpose(g_features, B, out, s0.N, nullptr, 0, L.gpe, st, err, err_len)) return rc;
+  if (int rc = synth::transpose(g_features, B, out, s0.N, nullptr, 0, L.gpe, st)) return rc;
   Act c;
   memset(&c, 0, sizeof(c));
   c.M = (int)s0.M; c.rows = (int)s0.Mp; c.C = out; c.per_img = s0.N; c.g = L.gpe; c.out = L.gy; c.partial = L.bpart;
-  if (int rc = act(c, G[X.pred + 1], st, err, err_len)) return rc;
-  if (int rc = wgrad(s0.Mp, out, kDec, L.gy, L.u, L.part, G[X.pred], st, err, err_len)) return rc;
-  if (int rc = prep(W[X.pred], out, kDec, kDec, true, L.w, st, err, err_len)) return rc;
-  if (int rc = gemm(s0.Mp, out, kDec, L.gy, L.w, L.ga, st, err, err_len)) return rc;
+  if (int rc = act(c, G[X.pred + 1], st)) return rc;
+  if (int rc = wgrad(s0.Mp, out, kDec, L.gy, L.u, L.part, G[X.pred], st)) return rc;
+  if (int rc = prep(W[X.pred], out, kDec, kDec, true, L.w, st)) return rc;
+  if (int rc = gemm(s0.Mp, out, kDec, L.gy, L.w, L.ga, st)) return rc;
   memset(&c, 0, sizeof(c));
   c.M = (int)s0.M; c.rows = (int)s0.Mp; c.C = kDec; c.per_img = s0.N; c.g = L.ga; c.partial = L.bpart;
-  if (int rc = act(c, G[X.fuse + 1], st, err, err_len)) return rc;
+  if (int rc = act(c, G[X.fuse + 1], st)) return rc;
   for (int i = 0; i < kStages; ++i) {
     const Shape s = shape(P, i);
     const StageBufs& S = L.s[i];
     if (i == 0) {
       memset(&c, 0, sizeof(c));
       c.M = (int)s.M; c.rows = (int)s.Mp; c.C = kDec; c.per_img = s.N; c.g = L.ga; c.out = L.gh;
-      if (int rc = act(c, nullptr, st, err, err_len)) return rc;
+      if (int rc = act(c, nullptr, st)) return rc;
     } else {
       upsample_adjoint_kernel<<<flat_grid(s.Mp * kDec), 256, 0, st>>>(L.ga, B, s.r, 1 << i, (int)s.Mp, L.gh);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
+      NFI_CUDA(cudaGetLastError());
     }
     const float* wf = W[X.fuse] + (kStages - 1 - i) * kDec;
     float* gf = G[X.fuse] ? G[X.fuse] + (kStages - 1 - i) * kDec : nullptr;
     if (int rc = synth::wgrad_terms(gf, 1, [&](int) {
-          return wgrad(s.Mp, kDec, kDec, L.gh, S.cp, L.part, L.wtmp, st, err, err_len);
-        }, kDec, kDec, 1, kStages * kDec, 1.f, synth::kCoCiTap, L.wtmp, st, err, err_len))
+          return wgrad(s.Mp, kDec, kDec, L.gh, S.cp, L.part, L.wtmp, st);
+        }, kDec, kDec, 1, kStages * kDec, 1.f, synth::kCoCiTap, L.wtmp, st))
       return rc;
-    if (int rc = prep(wf, kDec, kDec, kStages * kDec, true, L.w, st, err, err_len)) return rc;
-    if (int rc = gemm(s.Mp, kDec, kDec, L.gh, L.w, L.gln, st, err, err_len)) return rc;
+    if (int rc = prep(wf, kDec, kDec, kStages * kDec, true, L.w, st)) return rc;
+    if (int rc = gemm(s.Mp, kDec, kDec, L.gh, L.w, L.gln, st)) return rc;
     memset(&c, 0, sizeof(c));
     c.M = (int)s.M; c.rows = (int)s.Mp; c.C = kDec; c.per_img = s.N; c.g = L.gln; c.out = L.gy; c.partial = L.bpart;
-    if (int rc = act(c, G[X.lc[i] + 1], st, err, err_len)) return rc;
-    if (int rc = wgrad(s.Mp, kDec, s.C, L.gy, S.fp, L.part, G[X.lc[i]], st, err, err_len)) return rc;
-    if (int rc = prep(W[X.lc[i]], kDec, s.C, s.C, true, L.w, st, err, err_len)) return rc;
-    if (int rc = gemm(s.Mp, kDec, s.C, L.gy, L.w, L.gfeat[i], st, err, err_len)) return rc;
+    if (int rc = act(c, G[X.lc[i] + 1], st)) return rc;
+    if (int rc = wgrad(s.Mp, kDec, s.C, L.gy, S.fp, L.part, G[X.lc[i]], st)) return rc;
+    if (int rc = prep(W[X.lc[i]], kDec, s.C, s.C, true, L.w, st)) return rc;
+    if (int rc = gemm(s.Mp, kDec, s.C, L.gy, L.w, L.gfeat[i], st)) return rc;
   }
   // ---- stages, last to first
   int gk = 0;
@@ -1199,7 +1165,7 @@ int backward(const nfi_segformer_params& P, const float* g_features, float* cons
     memset(&n, 0, sizeof(n));
     n.M = (int)s.M; n.C = C; n.s = S.xs; n.stats = S.stn; n.w = W[X.norm[i]]; n.g = L.gfeat[i]; n.out = L.gx;
     n.partial = L.bpart;
-    if (int rc = ln_backward(n, G[X.norm[i]], G[X.norm[i] + 1], st, err, err_len)) return rc;
+    if (int rc = ln_backward(n, G[X.norm[i]], G[X.norm[i] + 1], st)) return rc;
     for (int k = P.depths[i] - 1; k >= 0; --k) {
       --gk;
       const Blk& K = S.blk[k];
@@ -1210,115 +1176,114 @@ int backward(const nfi_segformer_params& P, const float* g_features, float* cons
       memset(&c, 0, sizeof(c));
       c.M = (int)s.M; c.rows = (int)s.Mp; c.C = C; c.per_img = s.N; c.g = L.gx; c.scale = sc_m; c.out = L.gy;
       c.partial = L.bpart;
-      if (int rc = act(c, G[o2 + 7], st, err, err_len)) return rc;
-      if (int rc = wgrad(s.Mp, C, 4 * C, L.gy, K.g, L.part, G[o2 + 6], st, err, err_len)) return rc;
-      if (int rc = prep(W[o2 + 6], C, 4 * C, 4 * C, true, L.w, st, err, err_len)) return rc;
-      if (int rc = gemm(s.Mp, C, 4 * C, L.gy, L.w, L.ga, st, err, err_len)) return rc;
+      if (int rc = act(c, G[o2 + 7], st)) return rc;
+      if (int rc = wgrad(s.Mp, C, 4 * C, L.gy, K.g, L.part, G[o2 + 6], st)) return rc;
+      if (int rc = prep(W[o2 + 6], C, 4 * C, 4 * C, true, L.w, st)) return rc;
+      if (int rc = gemm(s.Mp, C, 4 * C, L.gy, L.w, L.ga, st)) return rc;
       const unsigned ndw = blocks(s.M, kChunk);
       dw_backward_kernel<<<dim3(ndw, (unsigned)(4 * C / 32)), 256, 0, st>>>(L.ga, K.z, K.h, W[o2 + 3], B, s.r, 4 * C, L.bpart);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
+      NFI_CUDA(cudaGetLastError());
       if (G[o2 + 4] || G[o2 + 5]) {
         dw_reduce_kernel<<<blocks((size_t)40 * C, 32), 256, 0, st>>>(L.bpart, (int)ndw, 4 * C, G[o2 + 4], G[o2 + 5]);
-        NFI_LAUNCH_CHECK(cudaGetLastError());
+        NFI_CUDA(cudaGetLastError());
       }
       const unsigned nadj = blocks(s.Mp, kChunk);
       dw_adjoint_kernel<<<dim3(nadj, (unsigned)(4 * C / 32)), 256, 0, st>>>(L.ga, W[o2 + 4], B, s.r, 4 * C, (int)s.Mp, L.gh, L.bpart);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
-      if (int rc = reduce(L.bpart, (int)nadj, 4 * C, 4 * C, G[o2 + 3], st, err, err_len)) return rc;
-      if (int rc = wgrad(s.Mp, 4 * C, C, L.gh, K.a2, L.part, G[o2 + 2], st, err, err_len)) return rc;
-      if (int rc = prep(W[o2 + 2], 4 * C, C, C, true, L.w, st, err, err_len)) return rc;
-      if (int rc = gemm(s.Mp, 4 * C, C, L.gh, L.w, L.gln, st, err, err_len)) return rc;
+      NFI_CUDA(cudaGetLastError());
+      if (int rc = reduce(L.bpart, (int)nadj, 4 * C, 4 * C, G[o2 + 3], st)) return rc;
+      if (int rc = wgrad(s.Mp, 4 * C, C, L.gh, K.a2, L.part, G[o2 + 2], st)) return rc;
+      if (int rc = prep(W[o2 + 2], 4 * C, C, C, true, L.w, st)) return rc;
+      if (int rc = gemm(s.Mp, 4 * C, C, L.gh, L.w, L.gln, st)) return rc;
       memset(&n, 0, sizeof(n));
       n.M = (int)s.M; n.C = C; n.s = K.x1; n.stats = K.st2; n.w = W[o2]; n.g = L.gln; n.g_res = L.gx; n.out = L.gx;
       n.partial = L.bpart;
-      if (int rc = ln_backward(n, G[o2], G[o2 + 1], st, err, err_len)) return rc;
+      if (int rc = ln_backward(n, G[o2], G[o2 + 1], st)) return rc;
       // attention branch
       memset(&c, 0, sizeof(c));
       c.M = (int)s.M; c.rows = (int)s.Mp; c.C = C; c.per_img = s.N; c.g = L.gx; c.scale = sc_a; c.out = L.gy;
       c.partial = L.bpart;
-      if (int rc = act(c, G[nb + kProj + 1], st, err, err_len)) return rc;
-      if (int rc = wgrad(s.Mp, C, C, L.gy, K.op, L.part, G[nb + kProj], st, err, err_len)) return rc;
-      if (int rc = prep(W[nb + kProj], C, C, C, true, L.w, st, err, err_len)) return rc;
-      if (int rc = gemm(s.Mp, C, C, L.gy, L.w, L.gln, st, err, err_len)) return rc;
+      if (int rc = act(c, G[nb + kProj + 1], st)) return rc;
+      if (int rc = wgrad(s.Mp, C, C, L.gy, K.op, L.part, G[nb + kProj], st)) return rc;
+      if (int rc = prep(W[nb + kProj], C, C, C, true, L.w, st)) return rc;
+      if (int rc = gemm(s.Mp, C, C, L.gy, L.w, L.gln, st)) return rc;
       const unsigned nq = blocks(s.N, kQ);
-      NFI_LAUNCH_CHECK(
-          cudaFuncSetAttribute(attn_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnBwdSmem));
+      NFI_CUDA(
+  cudaFuncSetAttribute(attn_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnBwdSmem));
       attn_backward_kernel<<<dim3(nq, s.heads, B), 256, kAttnBwdSmem, st>>>(
           K.q, W[nb + kQw + 1], K.kv, W[nb + kKv + 1], K.o, L.gln, s.N, s.Nk, C, L.gq, L.apart);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
+      NFI_CUDA(cudaGetLastError());
       attn_reduce_kernel<<<flat_grid(s.Mr * 2 * C), 256, 0, st>>>(L.apart, B, s.heads, (int)nq, s.Nk, C, L.gkv);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
+      NFI_CUDA(cudaGetLastError());
       memset(&c, 0, sizeof(c));
       c.M = (int)s.M; c.rows = (int)s.Mp; c.C = C; c.per_img = s.N; c.g = L.gq; c.out = L.gy; c.partial = L.bpart;
-      if (int rc = act(c, G[nb + kQw + 1], st, err, err_len)) return rc;
-      if (int rc = wgrad(s.Mp, C, C, L.gy, K.a1, L.part, G[nb + kQw], st, err, err_len)) return rc;
+      if (int rc = act(c, G[nb + kQw + 1], st)) return rc;
+      if (int rc = wgrad(s.Mp, C, C, L.gy, K.a1, L.part, G[nb + kQw], st)) return rc;
       memset(&c, 0, sizeof(c));
       c.M = (int)s.Mr; c.rows = (int)s.Mkv; c.C = 2 * C; c.per_img = s.Nk; c.g = L.gkv; c.out = L.gkvp;
       c.partial = L.bpart;
-      if (int rc = act(c, G[nb + kKv + 1], st, err, err_len)) return rc;
+      if (int rc = act(c, G[nb + kKv + 1], st)) return rc;
       const Pair kvin = s.sr > 1 ? K.xr : K.a1;
-      if (int rc = wgrad(s.Mkv, 2 * C, C, L.gkvp, kvin, L.part, G[nb + kKv], st, err, err_len)) return rc;
-      if (int rc = prep(W[nb + kQw], C, C, C, true, L.w, st, err, err_len)) return rc;
-      if (int rc = gemm(s.Mp, C, C, L.gy, L.w, L.gln, st, err, err_len)) return rc;
-      if (int rc = prep(W[nb + kKv], 2 * C, C, C, true, L.w, st, err, err_len)) return rc;
-      if (int rc = gemm(s.Mkv, 2 * C, C, L.gkvp, L.w, L.gxr, st, err, err_len)) return rc;
+      if (int rc = wgrad(s.Mkv, 2 * C, C, L.gkvp, kvin, L.part, G[nb + kKv], st)) return rc;
+      if (int rc = prep(W[nb + kQw], C, C, C, true, L.w, st)) return rc;
+      if (int rc = gemm(s.Mp, C, C, L.gy, L.w, L.gln, st)) return rc;
+      if (int rc = prep(W[nb + kKv], 2 * C, C, C, true, L.w, st)) return rc;
+      if (int rc = gemm(s.Mkv, 2 * C, C, L.gkvp, L.w, L.gxr, st)) return rc;
       const float* g2 = L.gxr;
       if (s.sr > 1) {
         memset(&n, 0, sizeof(n));
         n.M = (int)s.Mr; n.C = C; n.s = K.sr; n.stats = K.str; n.w = W[nb + kSrN]; n.g = L.gxr; n.out = L.gxr;
         n.partial = L.bpart;
-        if (int rc = ln_backward(n, G[nb + kSrN], G[nb + kSrN + 1], st, err, err_len)) return rc;
+        if (int rc = ln_backward(n, G[nb + kSrN], G[nb + kSrN + 1], st)) return rc;
         memset(&c, 0, sizeof(c));
         c.M = (int)s.Mr; c.rows = (int)s.Mrp; c.C = C; c.per_img = s.Nk; c.g = L.gxr; c.out = L.gsr;
         c.partial = L.bpart;
-        if (int rc = act(c, G[nb + kSrW + 1], st, err, err_len)) return rc;
+        if (int rc = act(c, G[nb + kSrW + 1], st)) return rc;
         if (int rc = synth::wgrad_terms(G[nb + kSrW], 1, [&](int) {
-              return wgrad(s.Mrp, C, s.K, L.gsr, K.sd, L.part, L.wtmp, st, err, err_len);
-            }, C, C, s.sr * s.sr, s.K, 1.f, synth::kCoTapCi, L.wtmp, st, err, err_len))
+              return wgrad(s.Mrp, C, s.K, L.gsr, K.sd, L.part, L.wtmp, st);
+            }, C, C, s.sr * s.sr, s.K, 1.f, synth::kCoTapCi, L.wtmp, st))
           return rc;
-        if (int rc = synth::prep_weights(W[nb + kSrW], C, C, s.sr * s.sr, s.K, 1.f, synth::kTapCiCo, L.w, st, err,
-                                         err_len))
+        if (int rc = synth::prep_weights(W[nb + kSrW], C, C, s.sr * s.sr, s.K, 1.f, synth::kTapCiCo, L.w, st))
           return rc;
-        if (int rc = gemm(s.Mrp, C, s.K, L.gsr, L.w, L.gsd, st, err, err_len)) return rc;
+        if (int rc = gemm(s.Mrp, C, s.K, L.gsr, L.w, L.gsd, st)) return rc;
         d2s_kernel<<<flat_grid(s.Mr * s.K), 256, 0, st>>>(L.gsd, B, s.r, s.sr, C, L.gext);
-        NFI_LAUNCH_CHECK(cudaGetLastError());
+        NFI_CUDA(cudaGetLastError());
         g2 = L.gext;
       }
       memset(&n, 0, sizeof(n));
       n.M = (int)s.M; n.C = C; n.s = K.x; n.stats = K.st1; n.w = W[nb + kN1]; n.g = L.gln; n.g2 = g2;
       n.g_res = L.gx; n.out = L.gx; n.partial = L.bpart;
-      if (int rc = ln_backward(n, G[nb + kN1], G[nb + kN1 + 1], st, err, err_len)) return rc;
+      if (int rc = ln_backward(n, G[nb + kN1], G[nb + kN1 + 1], st)) return rc;
     }
     // patch embed: its norm, then the conv
     const int pe = X.pe[i];
     memset(&n, 0, sizeof(n));
     n.M = (int)s.M; n.C = C; n.s = S.pe; n.stats = S.pst; n.w = W[pe + 2]; n.g = L.gx; n.out = L.gx;
     n.partial = L.bpart;
-    if (int rc = ln_backward(n, G[pe + 2], G[pe + 3], st, err, err_len)) return rc;
+    if (int rc = ln_backward(n, G[pe + 2], G[pe + 3], st)) return rc;
     if (i == 0) {
       memset(&c, 0, sizeof(c));
       c.M = c.rows = (int)s.M; c.C = C; c.per_img = s.N; c.g = L.gx; c.partial = L.bpart;
-      if (int rc = act(c, G[pe + 1], st, err, err_len)) return rc;
+      if (int rc = act(c, G[pe + 1], st)) return rc;
       if (G[pe]) {
         const unsigned np = blocks(s.M, kRows);
         pe1_wgrad_kernel<<<dim3(blocks(kPe1W, 256), np), 256, 0, st>>>(L.gx, P.image, B, H, s.r, L.bpart);
-        NFI_LAUNCH_CHECK(cudaGetLastError());
-        if (int rc = reduce(L.bpart, (int)np, kPe1W, kPe1W, G[pe], st, err, err_len)) return rc;
+        NFI_CUDA(cudaGetLastError());
+        if (int rc = reduce(L.bpart, (int)np, kPe1W, kPe1W, G[pe], st)) return rc;
       }
     } else {
       const int Cp = kDims[i - 1];
       memset(&c, 0, sizeof(c));
       c.M = c.rows = (int)s.M; c.C = C; c.per_img = s.N; c.g = L.gx; c.out = L.gy; c.partial = L.bpart;
-      if (int rc = act(c, G[pe + 1], st, err, err_len)) return rc;
+      if (int rc = act(c, G[pe + 1], st)) return rc;
       if (int rc = synth::wgrad_terms(G[pe], 1, [&](int) {
-            return synth::wgrad_down3x3(B, s.r, Cp, C, S.ph, L.gy, L.part, L.wtmp, st, err, err_len);
-          }, C, Cp, 9, 9 * Cp, 1.f, synth::kCiCoTap, L.wtmp, st, err, err_len))
+            return synth::wgrad_down3x3(B, s.r, Cp, C, S.ph, L.gy, L.part, L.wtmp, st);
+          }, C, Cp, 9, 9 * Cp, 1.f, synth::kCiCoTap, L.wtmp, st))
         return rc;
-      if (int rc = synth::prep_weights(W[pe], C, Cp, 9, 9 * Cp, 1.f, synth::kTapCiCo, L.w, st, err, err_len))
+      if (int rc = synth::prep_weights(W[pe], C, Cp, 9, 9 * Cp, 1.f, synth::kTapCiCo, L.w, st))
         return rc;
-      if (int rc = synth::conv_up3x3(B, s.r, C, Cp, L.gy, L.w, L.gpe, st, err, err_len)) return rc;
+      if (int rc = synth::conv_up3x3(B, s.r, C, Cp, L.gy, L.w, L.gpe, st)) return rc;
       crop_add_kernel<<<flat_grid((size_t)B * 4 * s.r * s.r * Cp), 256, 0, st>>>(L.gpe, B, s.r, Cp, L.gfeat[i - 1]);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
+      NFI_CUDA(cudaGetLastError());
     }
   }
   return 0;
@@ -1326,3 +1291,25 @@ int backward(const nfi_segformer_params& P, const float* g_features, float* cons
 
 }  // namespace segformer
 }  // namespace nfi
+
+using nfi::fail;
+
+extern "C" {
+
+size_t nfi_segformer_workspace_bytes(const nfi_segformer_params* params) {
+  if (params == nullptr) return 0;
+  return nfi::segformer::workspace_bytes(*params);
+}
+
+int nfi_segformer_forward(const nfi_segformer_params* params, void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  return nfi::segformer::forward(*params, (cudaStream_t)stream);
+}
+
+int nfi_segformer_backward(const nfi_segformer_params* params, const float* g_features, float* const* grads,
+                           void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  return nfi::segformer::backward(*params, g_features, grads, (cudaStream_t)stream);
+}
+
+}  // extern "C"

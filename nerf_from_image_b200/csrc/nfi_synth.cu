@@ -35,7 +35,6 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <math.h>
-#include <stdio.h>
 #include <string.h>
 
 #include "nfi_pair.cuh"
@@ -1380,17 +1379,11 @@ static int pick_bn(int N) {
 }
 
 // One convolution launch.  `in` [map_B (default B),H,W,C] pair, weights [taps9][N][C] pair.
-static int launch_conv(ConvArgs& a, Pair in, Pair wt, int w_taps, cudaStream_t st, char* err,
-                       size_t err_len, int map_B = 0) {
-  if (encode_fn() == nullptr) {
-    snprintf(err, err_len, "cuTensorMapEncodeTiled is not available from this driver");
-    return 1;
-  }
+static int launch_conv(ConvArgs& a, Pair in, Pair wt, int w_taps, cudaStream_t st, int map_B = 0) {
+  if (encode_fn() == nullptr) return fail("cuTensorMapEncodeTiled is not available from this driver");
   a.BN = pick_bn(a.N);
-  if (a.BN == 0 || a.C % 8 != 0) {  // (TMA: row pitch a multiple of 16 bytes)
-    snprintf(err, err_len, "synthesis conv: unsupported channel counts (Cin %d, Cout %d)", a.C, a.N);
-    return 1;
-  }
+  if (a.BN == 0 || a.C % 8 != 0)  // (TMA: row pitch a multiple of 16 bytes)
+    return fail("synthesis conv: unsupported channel counts (Cin %d, Cout %d)", a.C, a.N);
   a.n_tiles_n = a.N / a.BN;
   int m_tiles = 0;
   for (int p = 0; p < a.n_phases; ++p) {
@@ -1405,17 +1398,14 @@ static int launch_conv(ConvArgs& a, Pair in, Pair wt, int w_taps, cudaStream_t s
   CUtensorMap tAh, tAl, tWh, tWl;
   if (map_B == 0) map_B = a.B;
   if (!make_act_map(&tAh, in.hi, map_B, a.H, a.W, a.C) || !make_act_map(&tAl, in.lo, map_B, a.H, a.W, a.C) ||
-      !make_w_map(&tWh, wt.hi, w_taps, a.N, a.C, a.BN) || !make_w_map(&tWl, wt.lo, w_taps, a.N, a.C, a.BN)) {
-    snprintf(err, err_len, "cuTensorMapEncodeTiled failed (B %d H %d W %d C %d N %d)", a.B, a.H, a.W,
-             a.C, a.N);
-    return 1;
-  }
+      !make_w_map(&tWh, wt.hi, w_taps, a.N, a.C, a.BN) || !make_w_map(&tWl, wt.lo, w_taps, a.N, a.C, a.BN))
+    return fail("cuTensorMapEncodeTiled failed (B %d H %d W %d C %d N %d)", a.B, a.H, a.W, a.C, a.N);
   const int smem = kStages * (2 * kATile + 2 * a.BN * 128) + 128 +
                    ((a.mode == kModeRgb && a.skip != nullptr) ? kSkipBytes : 0);
-  NFI_LAUNCH_CHECK(cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  NFI_CUDA(cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   const int grid = n_tiles < sm_count() ? n_tiles : sm_count();
   conv_tc_kernel<<<grid, kConvThreads, smem, st>>>(tAh, tAl, tWh, tWl, a, n_tiles);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 
@@ -1442,27 +1432,21 @@ static int plan_wgrad(WgradArgs& a, int B, int DH, int DW) {
 // One weight-gradient GEMM (plan_wgrad'ed `a`): G [gB,gH,gW,g_channels (default cout)] and
 // X [B,xH,xW,cin] pairs.
 static int launch_wgrad(WgradArgs& a, Pair g, int gB, int gH, int gW, Pair x, int B, int xH, int xW,
-                        cudaStream_t st, char* err, size_t err_len, int g_channels = 0) {
-  if (encode_fn() == nullptr) {
-    snprintf(err, err_len, "cuTensorMapEncodeTiled is not available from this driver");
-    return 1;
-  }
+                        cudaStream_t st, int g_channels = 0) {
+  if (encode_fn() == nullptr) return fail("cuTensorMapEncodeTiled is not available from this driver");
   const int n_items = a.n_co * a.n_ci * a.taps * a.n_split;
   if (g_channels == 0) g_channels = a.cout;
   CUtensorMap tGh, tGl, tXh, tXl;
   if (!make_act_map(&tGh, g.hi, gB, gH, gW, g_channels, kWgTileH) ||
       !make_act_map(&tGl, g.lo, gB, gH, gW, g_channels, kWgTileH) ||
       !make_act_map(&tXh, x.hi, B, xH, xW, a.cin, kWgTileH) ||
-      !make_act_map(&tXl, x.lo, B, xH, xW, a.cin, kWgTileH)) {
-    snprintf(err, err_len, "cuTensorMapEncodeTiled failed (weight gradient, Cout %d Cin %d)", a.cout,
-             a.cin);
-    return 1;
-  }
+      !make_act_map(&tXl, x.lo, B, xH, xW, a.cin, kWgTileH))
+    return fail("cuTensorMapEncodeTiled failed (weight gradient, Cout %d Cin %d)", a.cout, a.cin);
   const int smem = kWgStages * kWgStage + 128;
-  NFI_LAUNCH_CHECK(cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  NFI_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   const int grid = n_items < 2 * sm_count() ? n_items : 2 * sm_count();
   wgrad_tc_kernel<<<grid, kWgThreads, smem, st>>>(tGh, tGl, tXh, tXl, a, n_items);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 
@@ -1591,28 +1575,17 @@ static WgradArgs conv0_wgrad(int cout, int cin, int nimg) {
   return a;
 }
 
-static int check_params(const nfi_synth_params& P, char* err, size_t err_len) {
+static int check_params(const nfi_synth_params& P) {
   const int R = P.img_resolution;
   int nb = 0;
   for (int r = 4; r <= R; r <<= 1) ++nb;
-  if (R < 8 || (R & (R - 1)) || nb != P.num_blocks || nb > NFI_SYNTH_MAX_BLOCKS) {
-    snprintf(err, err_len, "synthesis: img_resolution %d / num_blocks %d inconsistent", R, P.num_blocks);
-    return 1;
-  }
-  if (P.img_channels != 96) {
-    snprintf(err, err_len, "synthesis: img_channels must be 96 (3 planes x 32), got %d", P.img_channels);
-    return 1;
-  }
-  if (P.num_ws < 2 * nb) {
-    snprintf(err, err_len, "synthesis: ws has %d rows, need %d", P.num_ws, 2 * nb);
-    return 1;
-  }
+  if (R < 8 || (R & (R - 1)) || nb != P.num_blocks || nb > NFI_SYNTH_MAX_BLOCKS)
+    return fail("synthesis: img_resolution %d / num_blocks %d inconsistent", R, P.num_blocks);
+  if (P.img_channels != 96) return fail("synthesis: img_channels must be 96 (3 planes x 32), got %d", P.img_channels);
+  if (P.num_ws < 2 * nb) return fail("synthesis: ws has %d rows, need %d", P.num_ws, 2 * nb);
   for (int i = 0; i < nb; ++i)
-    if (P.channels[i] % 32 != 0 || pick_bn(P.channels[i]) == 0) {
-      snprintf(err, err_len, "synthesis: block %d has %d channels (need a multiple of 32 that tiles)", i,
-               P.channels[i]);
-      return 1;
-    }
+    if (P.channels[i] % 32 != 0 || pick_bn(P.channels[i]) == 0)
+      return fail("synthesis: block %d has %d channels (need a multiple of 32 that tiles)", i, P.channels[i]);
   return 0;
 }
 
@@ -1634,8 +1607,7 @@ struct Saved {
 
 // Runs (or, with dry, only lays out) the whole network.  With `sv`, the forward also stores every
 // layer's pre-activation u (the save mode) and `sv` receives the pointers the backward reads.
-static int run(const nfi_synth_params& P, Bump& ws, cudaStream_t st, bool dry, char* err, size_t err_len,
-               Saved* sv = nullptr) {
+static int run(const nfi_synth_params& P, Bump& ws, cudaStream_t st, bool dry, Saved* sv = nullptr) {
   const int B = P.batch, nb = P.num_blocks, D = P.w_dim;
   const float sqrt2 = 1.4142135623730951f;
 
@@ -1718,7 +1690,7 @@ static int run(const nfi_synth_params& P, Bump& ws, cudaStream_t st, bool dry, c
       if (!dry) {
         ConvArgs a = conv_up_args(B, cin, cout, hin);
         a.out_raw = raw;
-        const int rc = launch_conv(a, x, w0[i], 9, st, err, err_len);
+        const int rc = launch_conv(a, x, w0[i], 9, st);
         if (rc) return rc;
         ActEpilogue e;
         memset(&e, 0, sizeof(e));
@@ -1728,7 +1700,7 @@ static int run(const nfi_synth_params& P, Bump& ws, cudaStream_t st, bool dry, c
         e.u_out = sv ? sv->u0[i] : nullptr;
         const size_t total = (size_t)B * (res / 2) * (res / 2) * (cout / 4);
         fir_act_kernel<<<flat_grid(total), 256, 0, st>>>(raw, B, res, res, cout, e);
-        NFI_LAUNCH_CHECK(cudaGetLastError());
+        NFI_CUDA(cudaGetLastError());
       }
       x = y;
     }
@@ -1744,7 +1716,7 @@ static int run(const nfi_synth_params& P, Bump& ws, cudaStream_t st, bool dry, c
       a.act.style_a = style_rgb[i]; a.act.a_hi = xr.hi; a.act.a_lo = xr.lo;
       if (!last) { a.act.style_b = style0[i + 1]; a.act.b_hi = xn.hi; a.act.b_lo = xn.lo; }
       a.act.u_out = sv ? sv->u1[i] : nullptr;
-      const int rc = launch_conv(a, x, w1[i], 9, st, err, err_len);
+      const int rc = launch_conv(a, x, w1[i], 9, st);
       if (rc) return rc;
     }
     // ToRGB (1x1, K = cout) + bias + upsampled running image
@@ -1753,7 +1725,7 @@ static int run(const nfi_synth_params& P, Bump& ws, cudaStream_t st, bool dry, c
       ConvArgs a = torgb_args(B, cout, P.img_channels, res, kModeRgb);
       a.act.bias = P.torgb[i].bias;
       a.skip = img_prev; a.img = img; a.planes = last ? P.planes : nullptr;
-      const int rc = launch_conv(a, xr, wrgb[i], 1, st, err, err_len);
+      const int rc = launch_conv(a, xr, wrgb[i], 1, st);
       if (rc) return rc;
     }
     img_prev = img;
@@ -1766,31 +1738,26 @@ static int run(const nfi_synth_params& P, Bump& ws, cudaStream_t st, bool dry, c
 // 1024 bytes an entry may lose aligning the caller's pointer
 template <class Layout>
 static size_t sized(const nfi_synth_params& P, Layout layout) {
-  char err[256];
-  if (check_params(P, err, sizeof(err))) return 0;
+  if (check_params(P)) return 0;
   Bump b{nullptr, 0, 0};
-  layout(b, err, sizeof(err));
+  layout(b);
   return b.off + 1024;
 }
 
 size_t workspace_bytes(const nfi_synth_params& P) {
-  return sized(P, [&](Bump& b, char* err, size_t err_len) { run(P, b, nullptr, true, err, err_len); });
+  return sized(P, [&](Bump& b) { run(P, b, nullptr, true); });
 }
 
-int forward(const nfi_synth_params& P, cudaStream_t st, char* err, size_t err_len) {
-  const int rc = check_params(P, err, err_len);
+int forward(const nfi_synth_params& P, cudaStream_t st) {
+  const int rc = check_params(P);
   if (rc) return rc;
-  if (P.ws == nullptr || P.const_input == nullptr || P.planes == nullptr || P.workspace == nullptr) {
-    snprintf(err, err_len, "synthesis: ws, const_input, planes and workspace must be set");
-    return 1;
-  }
+  if (P.ws == nullptr || P.const_input == nullptr || P.planes == nullptr || P.workspace == nullptr)
+    return fail("synthesis: ws, const_input, planes and workspace must be set");
   const size_t need = workspace_bytes(P);
-  if (P.workspace_bytes < need) {
-    snprintf(err, err_len, "synthesis: workspace too small (%zu < %zu bytes)", P.workspace_bytes, need);
-    return 1;
-  }
+  if (P.workspace_bytes < need)
+    return fail("synthesis: workspace too small (%zu < %zu bytes)", P.workspace_bytes, need);
   Bump b = aligned_bump(P.workspace, P.workspace_bytes);
-  return run(P, b, st, false, err, err_len);
+  return run(P, b, st, false);
 }
 
 // ---- backward ----
@@ -1870,11 +1837,10 @@ static BackwardScratch backward_scratch(const nfi_synth_params& P, Bump& ws, int
 
 // The walk's operands that do not depend on it: every layer's W^T pair, and the planes' gradient
 // as the last block's image gradient dimg[0] (fp32 and pair)
-static int prep_backward(const nfi_synth_params& P, const float* g_planes, const BackwardScratch& s,
-                         cudaStream_t st, char* err, size_t err_len) {
+static int prep_backward(const nfi_synth_params& P, const float* g_planes, const BackwardScratch& s, cudaStream_t st) {
   const int B = P.batch, R = P.img_resolution, NI = P.img_channels;
   auto prep_t = [&](const float* w, int cout, int cin, int taps, Pair out) {
-    return prep_weights(w, cout, cin, taps, cin * taps, 1.f, kTapCiCo, out, st, err, err_len);
+    return prep_weights(w, cout, cin, taps, cin * taps, 1.f, kTapCiCo, out, st);
   };
   for (int i = 0; i < P.num_blocks; ++i) {
     const int c = P.channels[i], ci = i ? P.channels[i - 1] : 0;
@@ -1885,7 +1851,7 @@ static int prep_backward(const nfi_synth_params& P, const float* g_planes, const
   }
   planes_grad_kernel<<<flat_grid((size_t)B * R * R * NI), 256, 0, st>>>(g_planes, B, R, s.dimg[0],
                                                                         s.dimg_p.hi, s.dimg_p.lo);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 
@@ -1895,8 +1861,7 @@ static int prep_backward(const nfi_synth_params& P, const float* g_planes, const
 // on dimg before the running image's adjoint overwrites it, conv1 on its dacc pair, conv0 on the
 // raw-gradient phases.  It also takes the rebuilt layer input x~ and the GEMM partials.
 static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, const Saved& sv, Bump& ws,
-                        cudaStream_t st, bool dry, char* err, size_t err_len,
-                        const nfi_synth_param_grads* PG = nullptr) {
+                        cudaStream_t st, bool dry, const nfi_synth_param_grads* PG = nullptr) {
   const int B = P.batch, nb = P.num_blocks, D = P.w_dim, NI = P.img_channels;
   const float sqrt2 = 1.4142135623730951f;
   const BackwardScratch s = backward_scratch(P, ws, 1, PG != nullptr, PG != nullptr);
@@ -1907,21 +1872,18 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
   const auto &ds0 = s.ds0[0], &ds1 = s.ds1[0], &dsr = s.dsr[0], &dd0 = s.dd0[0], &dd1 = s.dd1[0];
   const Pair dimg_p = s.dimg_p, xt = s.xt;
 
-  NFI_LAUNCH_CHECK(cudaMemsetAsync(s.sums, 0, s.n_sums * sizeof(float), st));
-  if (const int rc = prep_backward(P, G.g_planes, s, st, err, err_len)) return rc;
+  NFI_CUDA(cudaMemsetAsync(s.sums, 0, s.n_sums * sizeof(float), st));
+  if (const int rc = prep_backward(P, G.g_planes, s, st)) return rc;
 
   auto act_backward = [&](ActBackward& e, int HW, int C) -> int {
-    if (C % 4 != 0 || C / 4 > 256) {
-      snprintf(err, err_len, "synthesis backward: %d channels unsupported", C);
-      return 1;
-    }
+    if (C % 4 != 0 || C / 4 > 256) return fail("synthesis backward: %d channels unsupported", C);
     const int chunk = kActChunk;
     dim3 grid((unsigned)((HW + chunk - 1) / chunk), (unsigned)B);
     if (PG)
       act_backward_kernel<true><<<grid, 256, 0, st>>>(e, HW, C, chunk);
     else
       act_backward_kernel<false><<<grid, 256, 0, st>>>(e, HW, C, chunk);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
+    NFI_CUDA(cudaGetLastError());
     return 0;
   };
   auto to_ws = [&](const float* ds, const nfi_synth_layer& L, int cin, int row, float gain) {
@@ -1943,10 +1905,10 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
                    const float* d, const float* s, float* g_w) -> int {
     plan_wgrad(a, B, D_, D_);
     a.part = part;
-    if (const int rc = launch_wgrad(a, g, gB, gH, gH, xt, B, D_, D_, st, err, err_len)) return rc;
+    if (const int rc = launch_wgrad(a, g, gB, gH, gH, xt, B, D_, D_, st)) return rc;
     wgrad_reduce_kernel<<<blocks((size_t)a.cout * a.cin, 256), 256, 0, st>>>(
         part, a.n_split, a.taps, a.cout, a.cin, w, dd, d, s, B, g_w);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
+    NFI_CUDA(cudaGetLastError());
     return 0;
   };
 
@@ -1958,7 +1920,7 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
     {
       ConvArgs a = torgb_args(B, NI, c, res, kModeRaw);
       a.out_raw = bufA;
-      const int rc = launch_conv(a, dimg_p, wtr[i], 1, st, err, err_len);
+      const int rc = launch_conv(a, dimg_p, wtr[i], 1, st);
       if (rc) return rc;
     }
     if (PG) {  // ToRGB bias and weight: sum dimg, and dimg against x~ = lrelu(u1) s_rgb
@@ -1978,7 +1940,7 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
       const int h = res / 2;
       upsample_adjoint_kernel<<<flat_grid((size_t)B * h * h * NI), 256, 0, st>>>(
           dimg[cur], B, h, h, NI, dimg[cur ^ 1], dimg_p.hi, dimg_p.lo);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
+      NFI_CUDA(cudaGetLastError());
       cur ^= 1;
     }
     // conv1: consumers ToRGB (style_rgb) and, below the last block, conv0 of block i+1 (bufC)
@@ -2010,7 +1972,7 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
       // dx~ of conv1 = conv^T(dacc, W1) -> bufA
       ConvArgs a = conv3x3_args(B, c, c, res, res, kModeRaw, true);
       a.out_raw = bufA;
-      const int rc = launch_conv(a, pb, wt1[i], 9, st, err, err_len);
+      const int rc = launch_conv(a, pb, wt1[i], 9, st);
       if (rc) return rc;
       if (PG && PG->conv1[i].g_weight != nullptr) {  // dacc against x~ = lrelu(u0) s1 (const s1)
         if (i)
@@ -2032,7 +1994,7 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
           sv.wsq1[0], sv.style1[0], dd1[0], sv.dco1[0], c, c, B, ds1[0]);
       to_ws(ds1[0], P.conv1[0], c, sv.row1[0], 1.f);
       if (PG) affine(ds1[0], PG->conv1[0], c, sv.row1[0], 1.f);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
+      NFI_CUDA(cudaGetLastError());
       break;
     }
     // conv0 (up): its one consumer is conv1 -> dacc fp32 in bufB, ds1 and dd0
@@ -2062,7 +2024,7 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
                  reinterpret_cast<__nv_bfloat16*>(bufA) + (size_t)4 * B * (h + 1) * (h + 1) * c};
       fir_adjoint_kernel<<<flat_grid((size_t)4 * B * (h + 1) * (h + 1) * (c / 4)), 256, 0, st>>>(
           bufB, B, res, res, c, ph.hi, ph.lo);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
+      NFI_CUDA(cudaGetLastError());
       if (PG && PG->conv0[i].g_weight != nullptr) {
         // raw gradient at (2i+ky, 2j+kx) = phase (ky%2, kx%2) at (i + ky/2, j + kx/2), against
         // x~ = lrelu(u1 of block i-1) s0 on the low-resolution grid
@@ -2074,24 +2036,24 @@ static int run_backward(const nfi_synth_params& P, const nfi_synth_grads& G, con
       }
       ConvArgs a = conv_up_adjoint_args(B, c, ci, h);
       a.out_raw = bufC;
-      const int rc = launch_conv(a, ph, wt0[i], 9, st, err, err_len, 4 * B);
+      const int rc = launch_conv(a, ph, wt0[i], 9, st, 4 * B);
       if (rc) return rc;
     }
   }
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 
-static int saved_layout(const nfi_synth_params& P, Bump& b, Saved& sv, char* err, size_t err_len) {
-  return run(P, b, nullptr, true, err, err_len, &sv);
+static int saved_layout(const nfi_synth_params& P, Bump& b, Saved& sv) {
+  return run(P, b, nullptr, true, &sv);
 }
 
 // The saved forward and, after it, the backward's scratch (with PG, the parameter backward's)
 static size_t backward_bytes(const nfi_synth_params& P, const nfi_synth_param_grads* PG) {
-  return sized(P, [&](Bump& b, char* err, size_t err_len) {
+  return sized(P, [&](Bump& b) {
     Saved sv{};
-    saved_layout(P, b, sv, err, err_len);
-    run_backward(P, nfi_synth_grads{}, sv, b, nullptr, true, err, err_len, PG);
+    saved_layout(P, b, sv);
+    run_backward(P, nfi_synth_grads{}, sv, b, nullptr, true, PG);
   });
 }
 
@@ -2102,19 +2064,14 @@ size_t param_workspace_bytes(const nfi_synth_params& P) {
   return backward_bytes(P, &pg);
 }
 
-static int check_saved(const nfi_synth_params& P, char* err, size_t err_len) {
-  const int rc = check_params(P, err, err_len);
+static int check_saved(const nfi_synth_params& P) {
+  const int rc = check_params(P);
   if (rc) return rc;
-  if (P.ws == nullptr || P.const_input == nullptr || P.planes == nullptr || P.workspace == nullptr) {
-    snprintf(err, err_len, "synthesis: ws, const_input, planes and workspace must be set");
-    return 1;
-  }
+  if (P.ws == nullptr || P.const_input == nullptr || P.planes == nullptr || P.workspace == nullptr)
+    return fail("synthesis: ws, const_input, planes and workspace must be set");
   const size_t need = saved_workspace_bytes(P);
-  if (P.workspace_bytes < need) {
-    snprintf(err, err_len, "synthesis: saved workspace too small (%zu < %zu bytes)", P.workspace_bytes,
-             need);
-    return 1;
-  }
+  if (P.workspace_bytes < need)
+    return fail("synthesis: saved workspace too small (%zu < %zu bytes)", P.workspace_bytes, need);
   return 0;
 }
 
@@ -2122,68 +2079,54 @@ static int check_saved(const nfi_synth_params& P, char* err, size_t err_len) {
 // workspace's size; g_planes and g_ws where G is given; the parameter backward's larger workspace
 // with `param_ws`), then the Bump over the aligned workspace and, where `sv` is given, the saved
 // forward's pointers, which leave the Bump past the saved forward.
-static int open_saved(const nfi_synth_params& P, const nfi_synth_grads* G, bool param_ws, Bump& b,
-                      Saved* sv, char* err, size_t err_len) {
-  if (const int rc = check_saved(P, err, err_len)) return rc;
-  if (G != nullptr && (G->g_planes == nullptr || G->g_ws == nullptr)) {
-    snprintf(err, err_len, "synthesis backward: g_planes and g_ws must be set");
-    return 1;
-  }
+static int open_saved(const nfi_synth_params& P, const nfi_synth_grads* G, bool param_ws, Bump& b, Saved* sv) {
+  if (const int rc = check_saved(P)) return rc;
+  if (G != nullptr && (G->g_planes == nullptr || G->g_ws == nullptr))
+    return fail("synthesis backward: g_planes and g_ws must be set");
   if (param_ws) {
     const size_t need = param_workspace_bytes(P);
-    if (P.workspace_bytes < need) {
-      snprintf(err, err_len, "synthesis parameter backward: workspace too small (%zu < %zu bytes)",
-               P.workspace_bytes, need);
-      return 1;
-    }
+    if (P.workspace_bytes < need)
+      return fail("synthesis parameter backward: workspace too small (%zu < %zu bytes)", P.workspace_bytes, need);
   }
   b = aligned_bump(P.workspace, P.workspace_bytes);
   if (sv == nullptr) return 0;
   *sv = Saved{};
-  return saved_layout(P, b, *sv, err, err_len);
+  return saved_layout(P, b, *sv);
 }
 
-int forward_saved(const nfi_synth_params& P, cudaStream_t st, char* err, size_t err_len) {
+int forward_saved(const nfi_synth_params& P, cudaStream_t st) {
   Bump b;
-  if (const int rc = open_saved(P, nullptr, false, b, nullptr, err, err_len)) return rc;
+  if (const int rc = open_saved(P, nullptr, false, b, nullptr)) return rc;
   Saved sv{};
-  return run(P, b, st, false, err, err_len, &sv);
+  return run(P, b, st, false, &sv);
 }
 
-int backward(const nfi_synth_params& P, const nfi_synth_grads& G, cudaStream_t st, char* err,
-             size_t err_len) {
+int backward(const nfi_synth_params& P, const nfi_synth_grads& G, cudaStream_t st) {
   Bump b;
   Saved sv;
-  if (const int rc = open_saved(P, &G, false, b, &sv, err, err_len)) return rc;
-  return run_backward(P, G, sv, b, st, false, err, err_len);
+  if (const int rc = open_saved(P, &G, false, b, &sv)) return rc;
+  return run_backward(P, G, sv, b, st, false);
 }
 
-int saved_preactivation(const nfi_synth_params& P, int block, int which, float* out, cudaStream_t st,
-                        char* err, size_t err_len) {
+int saved_preactivation(const nfi_synth_params& P, int block, int which, float* out, cudaStream_t st) {
   Bump b;
   Saved sv;
-  if (const int rc = open_saved(P, nullptr, false, b, &sv, err, err_len)) return rc;
-  if (block < 0 || block >= P.num_blocks || (which != 0 && which != 1) || (which == 0 && block == 0)) {
-    snprintf(err, err_len, "synthesis pre-activation: no layer (block %d, which %d)", block, which);
-    return 1;
-  }
-  if (out == nullptr) {
-    snprintf(err, err_len, "synthesis pre-activation: out must be set");
-    return 1;
-  }
+  if (const int rc = open_saved(P, nullptr, false, b, &sv)) return rc;
+  if (block < 0 || block >= P.num_blocks || (which != 0 && which != 1) || (which == 0 && block == 0))
+    return fail("synthesis pre-activation: no layer (block %d, which %d)", block, which);
+  if (out == nullptr) return fail("synthesis pre-activation: out must be set");
   const int res = 4 << block;
   const size_t n = (size_t)P.batch * res * res * P.channels[block];
-  NFI_LAUNCH_CHECK(cudaMemcpyAsync(out, which ? sv.u1[block] : sv.u0[block], n * sizeof(float),
-                            cudaMemcpyDeviceToDevice, st));
+  NFI_CUDA(cudaMemcpyAsync(out, which ? sv.u1[block] : sv.u0[block], n * sizeof(float), cudaMemcpyDeviceToDevice, st));
   return 0;
 }
 
 int backward_params(const nfi_synth_params& P, const nfi_synth_grads& G, const nfi_synth_param_grads& PG,
-                    cudaStream_t st, char* err, size_t err_len) {
+                    cudaStream_t st) {
   Bump b;
   Saved sv;
-  if (const int rc = open_saved(P, &G, true, b, &sv, err, err_len)) return rc;
-  return run_backward(P, G, sv, b, st, false, err, err_len, &PG);
+  if (const int rc = open_saved(P, &G, true, b, &sv)) return rc;
+  return run_backward(P, G, sv, b, st, false, &PG);
 }
 
 
@@ -2194,7 +2137,7 @@ int backward_params(const nfi_synth_params& P, const nfi_synth_grads& G, const n
 // against W^T, the weight GEMMs on [dacc; dacc-dot] against [x~-dot; x~] (one sum over 2B images
 // is the product rule's two terms).  Buffers as in run_backward, with room for 2B images.
 static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Saved& sv, Bump& ws,
-                   cudaStream_t st, bool dry, char* err, size_t err_len, const nfi_synth_param_grads* PG) {
+                   cudaStream_t st, bool dry, const nfi_synth_param_grads* PG) {
   const int B = P.batch, B2 = 2 * B, nb = P.num_blocks, D = P.w_dim, NI = P.img_channels;
   const float sqrt2 = 1.4142135623730951f;
   // xt is [x~-dot; x~]: the tangent conv's input, the weight GEMMs' X
@@ -2223,7 +2166,7 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
   const auto &ds0 = s.ds0, &ds1 = s.ds1, &dsr = s.dsr, &dd0 = s.dd0, &dd1 = s.dd1;  // [0]: q, [1]: q-dot
   const Pair dimg_p = s.dimg_p, xt = s.xt;
 
-  NFI_LAUNCH_CHECK(cudaMemsetAsync(s.sums, 0, s.n_sums * sizeof(float), st));
+  NFI_CUDA(cudaMemsetAsync(s.sums, 0, s.n_sums * sizeof(float), st));
   // ---- tangent forward ----
   auto style_dot = [&](const nfi_synth_layer& L, int c, int row, float gain, float* out) {
     styles_kernel<<<blocks((size_t)B * c * 32, 256), 256, 0, st>>>(H.t_ws + (size_t)row * D, P.num_ws * D, D,
@@ -2256,11 +2199,11 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
       restyle_dot(sv.u1[i - 1], ud1[i - 1], sv.style0[i], sd0[i], h * h, ci, xt);
       ConvArgs a = conv_up_args(B, ci, c, h);
       a.out_raw = bufA;
-      if (const int rc = launch_conv(a, xt, sv.w0[i], 9, st, err, err_len)) return rc;
+      if (const int rc = launch_conv(a, xt, sv.w0[i], 9, st)) return rc;
       const size_t total = (size_t)B * h * h * (c / 4);
       fir_act_kernel<<<flat_grid(total), 256, 0, st>>>(bufA, B, res, res, c,
                                                        tangent_epi(P.conv0[i], sv.dco0[i], ddot0[i], sv.u0[i], ud0[i]));
-      NFI_LAUNCH_CHECK(cudaGetLastError());
+      NFI_CUDA(cudaGetLastError());
       restyle_dot(sv.u0[i], ud0[i], sv.style1[i], sd1[i], HW, c, xt);
     } else {  // b4.const does not depend on ws: x~-dot = const s-dot
       const_input_kernel<<<blocks((size_t)B * 16 * c, 256), 256, 0, st>>>(P.const_input, sd1[0], B, c, xt.hi,
@@ -2268,23 +2211,20 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
     }
     ConvArgs a = conv3x3_args(B, c, c, res, res, kModeRaw);
     a.out_raw = bufA;
-    if (const int rc = launch_conv(a, xt, sv.w1[i], 9, st, err, err_len)) return rc;
+    if (const int rc = launch_conv(a, xt, sv.w1[i], 9, st)) return rc;
     tangent_act_kernel<<<flat_grid((size_t)B * HW * c / 4), 256, 0, st>>>(
         bufA, B, HW, c, tangent_epi(P.conv1[i], sv.dco1[i], ddot1[i], sv.u1[i], ud1[i]));
-    NFI_LAUNCH_CHECK(cudaGetLastError());
+    NFI_CUDA(cudaGetLastError());
   }
 
   // ---- the backward and its tangent, last block first ----
-  if (const int rc = prep_backward(P, H.g_planes, s, st, err, err_len)) return rc;
+  if (const int rc = prep_backward(P, H.g_planes, s, st)) return rc;
 
   auto act_backward = [&](ActBackwardTangent& e, int HW, int C) -> int {
-    if (C % 4 != 0 || C / 4 > 256) {
-      snprintf(err, err_len, "synthesis HVP: %d channels unsupported", C);
-      return 1;
-    }
+    if (C % 4 != 0 || C / 4 > 256) return fail("synthesis HVP: %d channels unsupported", C);
     dim3 grid((unsigned)((HW + kActChunk - 1) / kActChunk), (unsigned)B);
     act_backward_tangent_kernel<<<grid, 256, 0, st>>>(e, HW, C, kActChunk);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
+    NFI_CUDA(cudaGetLastError());
     return 0;
   };
   // the ws gradient is the tangent's (the style gradient's tangent through styles_kernel's
@@ -2312,14 +2252,14 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
                    const float* d, const float* ddot, const float* s, const float* sdot, float* g_w) -> int {
     plan_wgrad(a, nimg, D_, D_);
     a.part = part;
-    if (const int rc = launch_wgrad(a, g, gB, gH, gH, xt, nimg, D_, D_, st, err, err_len)) return rc;
+    if (const int rc = launch_wgrad(a, g, gB, gH, gH, xt, nimg, D_, D_, st)) return rc;
     if (dd == nullptr)
       wgrad_reduce_kernel<<<blocks((size_t)a.cout * a.cin, 256), 256, 0, st>>>(
           part, a.n_split, a.taps, a.cout, a.cin, w, nullptr, nullptr, nullptr, B, g_w);
     else
       wgrad_reduce_tangent_kernel<<<blocks((size_t)a.cout * a.cin, 256), 256, 0, st>>>(
           part, a.n_split, a.taps, a.cout, a.cin, w, dd[0], dd[1], d, ddot, s, sdot, B, g_w);
-    NFI_LAUNCH_CHECK(cudaGetLastError());
+    NFI_CUDA(cudaGetLastError());
     return 0;
   };
 
@@ -2331,7 +2271,7 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
     {  // ToRGB: dx~ = dimg Wrgb^T -> bufA (its tangent is 0: dimg does not depend on ws)
       ConvArgs a = torgb_args(B, NI, c, res, kModeRaw);
       a.out_raw = bufA;
-      if (const int rc = launch_conv(a, dimg_p, wtr[i], 1, st, err, err_len)) return rc;
+      if (const int rc = launch_conv(a, dimg_p, wtr[i], 1, st)) return rc;
     }
     if (PG && PG->torgb[i].g_weight != nullptr) {  // dimg against x~-dot of ToRGB
       restyle_dot(sv.u1[i], ud1[i], sv.style_rgb[i], sdr[i], HW, c, xt);
@@ -2344,7 +2284,7 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
       const int h = res / 2;
       upsample_adjoint_kernel<<<flat_grid((size_t)B * h * h * NI), 256, 0, st>>>(
           dimg[cur], B, h, h, NI, dimg[cur ^ 1], dimg_p.hi, dimg_p.lo);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
+      NFI_CUDA(cudaGetLastError());
       cur ^= 1;
     }
     // conv1: consumers ToRGB and conv0 of block i+1 ([dx~; dx~-dot] in bufC) -> [dacc; dacc-dot]
@@ -2379,7 +2319,7 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
     {  // [dx~; dx~-dot] of conv1 = conv^T([dacc; dacc-dot], W1) -> bufA
       ConvArgs a = conv3x3_args(B2, c, c, res, res, kModeRaw, true);
       a.out_raw = bufA;
-      if (const int rc = launch_conv(a, pb, wt1[i], 9, st, err, err_len)) return rc;
+      if (const int rc = launch_conv(a, pb, wt1[i], 9, st)) return rc;
     }
     if (PG && PG->conv1[i].g_weight != nullptr) {  // [dacc; dacc-dot] against [x~-dot; x~]
       if (i) {
@@ -2407,7 +2347,7 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
       float* dd[2] = {dd1[0][0], dd1[1][0]};
       demod(sv.wsq1[0], sv.style1[0], sd1[0], dd, sv.dco1[0], ddot1[0], c, c, ds1[0][0], ds1[1][0]);
       outputs(ds1[0][0], ds1[1][0], P.conv1[0], c, sv.row1[0], 1.f, PG ? &PG->conv1[0] : nullptr);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
+      NFI_CUDA(cudaGetLastError());
       break;
     }
     {  // conv0 (up): one consumer, conv1 -> [dacc; dacc-dot] fp32 in bufB
@@ -2433,7 +2373,7 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
       const size_t nph = (size_t)4 * B2 * (h + 1) * (h + 1) * c;
       Pair ph = {reinterpret_cast<__nv_bfloat16*>(bufA), reinterpret_cast<__nv_bfloat16*>(bufA) + nph};
       fir_adjoint_kernel<<<flat_grid(nph / 4), 256, 0, st>>>(bufB, B2, res, res, c, ph.hi, ph.lo);
-      NFI_LAUNCH_CHECK(cudaGetLastError());
+      NFI_CUDA(cudaGetLastError());
       if (PG && PG->conv0[i].g_weight != nullptr) {
         const size_t nl = (size_t)B * h * h * ci;
         restyle_dot(sv.u1[i - 1], ud1[i - 1], sv.style0[i], sd0[i], h * h, ci, xt);
@@ -2447,37 +2387,31 @@ static int run_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const Save
       }
       ConvArgs a = conv_up_adjoint_args(B2, c, ci, h);
       a.out_raw = bufC;
-      if (const int rc = launch_conv(a, ph, wt0[i], 9, st, err, err_len, 4 * B2)) return rc;
+      if (const int rc = launch_conv(a, ph, wt0[i], 9, st, 4 * B2)) return rc;
     }
   }
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 
 size_t hvp_scratch_bytes(const nfi_synth_params& P) {
-  return sized(P, [&](Bump& b, char* err, size_t err_len) {
+  return sized(P, [&](Bump& b) {
     const Saved sv{};  // (the dry walk reads no saved pointer)
     const nfi_synth_param_grads pg{};
-    run_hvp(P, nfi_synth_hvp{}, sv, b, nullptr, true, err, err_len, &pg);
+    run_hvp(P, nfi_synth_hvp{}, sv, b, nullptr, true, &pg);
   });
 }
 
-int backward_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const nfi_synth_param_grads* PG,
-                 cudaStream_t st, char* err, size_t err_len) {
+int backward_hvp(const nfi_synth_params& P, const nfi_synth_hvp& H, const nfi_synth_param_grads* PG, cudaStream_t st) {
   Bump b;
   Saved sv;
-  if (const int rc = open_saved(P, nullptr, false, b, &sv, err, err_len)) return rc;
-  if (H.g_planes == nullptr || H.t_ws == nullptr || H.g_ws == nullptr || H.scratch == nullptr) {
-    snprintf(err, err_len, "synthesis HVP: g_planes, t_ws, g_ws and scratch must be set");
-    return 1;
-  }
+  if (const int rc = open_saved(P, nullptr, false, b, &sv)) return rc;
+  if (H.g_planes == nullptr || H.t_ws == nullptr || H.g_ws == nullptr || H.scratch == nullptr)
+    return fail("synthesis HVP: g_planes, t_ws, g_ws and scratch must be set");
   const size_t need = hvp_scratch_bytes(P);
-  if (H.scratch_bytes < need) {
-    snprintf(err, err_len, "synthesis HVP: scratch too small (%zu < %zu bytes)", H.scratch_bytes, need);
-    return 1;
-  }
+  if (H.scratch_bytes < need) return fail("synthesis HVP: scratch too small (%zu < %zu bytes)", H.scratch_bytes, need);
   Bump s = aligned_bump(H.scratch, H.scratch_bytes);
-  return run_hvp(P, H, sv, s, st, false, err, err_len, PG);
+  return run_hvp(P, H, sv, s, st, false, PG);
 }
 
 // ---- the narrow entries of nfi_synth_launch.h ----
@@ -2562,67 +2496,60 @@ transpose_kernel(const float* __restrict__ src, int R, int Cc, const float* __re
 }
 
 int prep_weights(const float* w, int cout, int cin, int taps, int ld, float gain, int order, Pair out,
-                 cudaStream_t st, char* err, size_t err_len) {
-  if (order != kTapCoCi && order != kTapCiCo && order != kCoTapCi) {
-    snprintf(err, err_len, "prep_weights: no operand order %d", order);
-    return 1;
-  }
+                 cudaStream_t st) {
+  if (order != kTapCoCi && order != kTapCiCo && order != kCoTapCi)
+    return fail("prep_weights: no operand order %d", order);
   prep_pair_kernel<<<flat_grid((size_t)cout * cin), 256, 0, st>>>(w, cout, cin, taps, ld, gain, order, out.hi,
                                                                    out.lo);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 
 int finish_wgrad(const float* tmp, int cout, int cin, int taps, int ld, float gain, int order, float* g_w,
-                 cudaStream_t st, char* err, size_t err_len) {
-  if (order != kCoCiTap && order != kCiCoTap && order != kCoTapCi) {
-    snprintf(err, err_len, "finish_wgrad: no gradient order %d", order);
-    return 1;
-  }
+                 cudaStream_t st) {
+  if (order != kCoCiTap && order != kCiCoTap && order != kCoTapCi)
+    return fail("finish_wgrad: no gradient order %d", order);
   finish_wgrad_kernel<<<blocks((size_t)cout * cin * taps, 256), 256, 0, st>>>(tmp, cout, cin, taps, ld, gain, order,
                                                                               g_w);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 
-int bias_reduce(const float* partial, int n_chunks, int C, float* g_b, cudaStream_t st, char* err,
-                size_t err_len) {
+int bias_reduce(const float* partial, int n_chunks, int C, float* g_b, cudaStream_t st) {
   if (g_b == nullptr) return 0;
   bias_reduce_kernel<<<blocks(C, 256), 256, 0, st>>>(partial, n_chunks, C, g_b);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 
-int transpose(const float* src, int B, int R, int Cc, const float* bias, int accumulate, float* dst,
-              cudaStream_t st, char* err, size_t err_len) {
+int transpose(const float* src, int B, int R, int Cc, const float* bias, int accumulate, float* dst, cudaStream_t st) {
   transpose_kernel<<<dim3(blocks(Cc, 32), blocks(R, 32), (unsigned)B), dim3(32, 8), 0, st>>>(src, R, Cc, bias,
                                                                                             accumulate, dst);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 
 // The fixed-order sum of a narrow weight gradient's partials into g_w
-static int wgrad_sum(const WgradArgs& a, float* g_w, cudaStream_t st, char* err, size_t err_len) {
+static int wgrad_sum(const WgradArgs& a, float* g_w, cudaStream_t st) {
   const size_t n = (size_t)a.cout * a.cin;
   wgrad_sum_kernel<<<blocks(n, 256), 256, 0, st>>>(a.part, a.n_split, a.taps, n, g_w);
-  NFI_LAUNCH_CHECK(cudaGetLastError());
+  NFI_CUDA(cudaGetLastError());
   return 0;
 }
 
 int conv3x3(int B, int H, int W, int C, int N, Pair in, Pair w, const float* bias, float* u_out, Pair out,
-            cudaStream_t st, char* err, size_t err_len) {
+            cudaStream_t st) {
   ConvArgs a = conv3x3_args(B, C, N, H, W, kModeAct);
   a.act.bias = bias; a.act.gain = 1.f; a.act.slope = 0.f;
   a.act.a_hi = out.hi; a.act.a_lo = out.lo;
   a.act.u_out = u_out;
-  return launch_conv(a, in, w, 9, st, err, err_len);
+  return launch_conv(a, in, w, 9, st);
 }
 
-int conv3x3_adjoint(int B, int H, int W, int C, int N, Pair in, Pair w, float* raw_out, cudaStream_t st,
-                    char* err, size_t err_len) {
+int conv3x3_adjoint(int B, int H, int W, int C, int N, Pair in, Pair w, float* raw_out, cudaStream_t st) {
   ConvArgs a = conv3x3_args(B, C, N, H, W, kModeRaw, true);
   a.out_raw = raw_out;
-  return launch_conv(a, in, w, 9, st, err, err_len);
+  return launch_conv(a, in, w, 9, st);
 }
 
 size_t wgrad3x3_partial_floats(int B, int H, int W, int cout, int cin) {
@@ -2632,47 +2559,41 @@ size_t wgrad3x3_partial_floats(int B, int H, int W, int cout, int cin) {
 }
 
 int wgrad3x3(int B, int H, int W, int cout, int cin, int g_channels, Pair g, Pair x, float* partials,
-             float* g_w, cudaStream_t st, char* err, size_t err_len) {
+             float* g_w, cudaStream_t st) {
   if (g_w == nullptr) return 0;
-  if (g_channels < cout || g_channels % 8 != 0 || cin % 8 != 0) {
-    snprintf(err, err_len, "conv weight gradient: unsupported channel counts (G %d for Cout %d, Cin %d)",
-             g_channels, cout, cin);
-    return 1;
-  }
+  if (g_channels < cout || g_channels % 8 != 0 || cin % 8 != 0)
+    return fail("conv weight gradient: unsupported channel counts (G %d for Cout %d, Cin %d)", g_channels, cout, cin);
   WgradArgs a = conv3x3_wgrad(cout, cin);
   plan_wgrad(a, B, H, W);
   a.part = partials;
-  if (const int rc = launch_wgrad(a, g, B, H, W, x, B, H, W, st, err, err_len, g_channels)) return rc;
-  return wgrad_sum(a, g_w, st, err, err_len);
+  if (const int rc = launch_wgrad(a, g, B, H, W, x, B, H, W, st, g_channels)) return rc;
+  return wgrad_sum(a, g_w, st);
 }
 
 int conv3x3_act(int B, int H, int W, int C, int N, Pair in, Pair w, const float* bias, float gain, float slope,
-                Pair out, cudaStream_t st, char* err, size_t err_len) {
+                Pair out, cudaStream_t st) {
   ConvArgs a = conv3x3_args(B, C, N, H, W, kModeAct);
   a.act.bias = bias; a.act.gain = gain; a.act.slope = slope;
   a.act.a_hi = out.hi; a.act.a_lo = out.lo;
-  return launch_conv(a, in, w, 9, st, err, err_len);
+  return launch_conv(a, in, w, 9, st);
 }
 
-int conv_down3x3(int B, int h, int C, int N, Pair phases, Pair w, float* raw_out, cudaStream_t st, char* err,
-                 size_t err_len) {
+int conv_down3x3(int B, int h, int C, int N, Pair phases, Pair w, float* raw_out, cudaStream_t st) {
   ConvArgs a = conv_up_adjoint_args(B, C, N, h);
   a.out_raw = raw_out;
-  return launch_conv(a, phases, w, 9, st, err, err_len, 4 * B);
+  return launch_conv(a, phases, w, 9, st, 4 * B);
 }
 
-int conv_up3x3(int B, int h, int C, int N, Pair in, Pair w, float* raw_out, cudaStream_t st, char* err,
-               size_t err_len) {
+int conv_up3x3(int B, int h, int C, int N, Pair in, Pair w, float* raw_out, cudaStream_t st) {
   ConvArgs a = conv_up_args(B, C, N, h);
   a.out_raw = raw_out;
-  return launch_conv(a, in, w, 9, st, err, err_len);
+  return launch_conv(a, in, w, 9, st);
 }
 
-int conv1x1(int B, int H, int C, int N, Pair in, Pair w, float* raw_out, cudaStream_t st, char* err,
-            size_t err_len) {
+int conv1x1(int B, int H, int C, int N, Pair in, Pair w, float* raw_out, cudaStream_t st) {
   ConvArgs a = torgb_args(B, C, N, H, kModeRaw);
   a.out_raw = raw_out;
-  return launch_conv(a, in, w, 1, st, err, err_len);
+  return launch_conv(a, in, w, 1, st);
 }
 
 size_t wgrad_down3x3_partial_floats(int B, int h, int cin, int cout) {
@@ -2681,14 +2602,13 @@ size_t wgrad_down3x3_partial_floats(int B, int h, int cin, int cout) {
   return (size_t)a.n_split * a.taps * cout * cin;
 }
 
-int wgrad_down3x3(int B, int h, int cin, int cout, Pair phases, Pair g, float* partials, float* g_wt,
-                  cudaStream_t st, char* err, size_t err_len) {
+int wgrad_down3x3(int B, int h, int cin, int cout, Pair phases, Pair g, float* partials, float* g_wt, cudaStream_t st) {
   if (g_wt == nullptr) return 0;
   WgradArgs a = conv0_wgrad(cin, cout, B);
   plan_wgrad(a, B, h, h);
   a.part = partials;
-  if (const int rc = launch_wgrad(a, phases, 4 * B, h + 1, h + 1, g, B, h, h, st, err, err_len)) return rc;
-  return wgrad_sum(a, g_wt, st, err, err_len);
+  if (const int rc = launch_wgrad(a, phases, 4 * B, h + 1, h + 1, g, B, h, h, st)) return rc;
+  return wgrad_sum(a, g_wt, st);
 }
 
 size_t wgrad1x1_partial_floats(int B, int H, int cout, int cin) {
@@ -2697,15 +2617,83 @@ size_t wgrad1x1_partial_floats(int B, int H, int cout, int cin) {
   return (size_t)a.n_split * a.taps * cout * cin;
 }
 
-int wgrad1x1(int B, int H, int cout, int cin, Pair g, Pair x, float* partials, float* g_w, cudaStream_t st,
-             char* err, size_t err_len) {
+int wgrad1x1(int B, int H, int cout, int cin, Pair g, Pair x, float* partials, float* g_w, cudaStream_t st) {
   if (g_w == nullptr) return 0;
   WgradArgs a = torgb_wgrad(cout, cin);
   plan_wgrad(a, B, H, H);
   a.part = partials;
-  if (const int rc = launch_wgrad(a, g, B, H, H, x, B, H, H, st, err, err_len)) return rc;
-  return wgrad_sum(a, g_w, st, err, err_len);
+  if (const int rc = launch_wgrad(a, g, B, H, H, x, B, H, H, st)) return rc;
+  return wgrad_sum(a, g_w, st);
 }
 
 }  // namespace synth
 }  // namespace nfi
+
+using nfi::fail;
+
+extern "C" {
+
+size_t nfi_synthesis_workspace_bytes(const nfi_synth_params* params) {
+  if (params == nullptr) return 0;
+  return nfi::synth::workspace_bytes(*params);
+}
+
+int nfi_synthesis_forward(const nfi_synth_params* params, void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  if (params->batch <= 0) return fail("empty batch");
+  return nfi::synth::forward(*params, (cudaStream_t)stream);
+}
+
+size_t nfi_synthesis_saved_workspace_bytes(const nfi_synth_params* params) {
+  if (params == nullptr) return 0;
+  return nfi::synth::saved_workspace_bytes(*params);
+}
+
+int nfi_synthesis_forward_saved(const nfi_synth_params* params, void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  if (params->batch <= 0) return fail("empty batch");
+  return nfi::synth::forward_saved(*params, (cudaStream_t)stream);
+}
+
+int nfi_synthesis_backward(const nfi_synth_params* params, const nfi_synth_grads* grads, void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  if (grads == nullptr) return fail("grads is NULL");
+  if (params->batch <= 0) return fail("empty batch");
+  return nfi::synth::backward(*params, *grads, (cudaStream_t)stream);
+}
+
+int nfi_synthesis_saved_preactivation(const nfi_synth_params* params, int32_t block, int32_t which,
+                                      float* out, void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  if (params->batch <= 0) return fail("empty batch");
+  return nfi::synth::saved_preactivation(*params, block, which, out, (cudaStream_t)stream);
+}
+
+size_t nfi_synthesis_param_workspace_bytes(const nfi_synth_params* params) {
+  if (params == nullptr) return 0;
+  return nfi::synth::param_workspace_bytes(*params);
+}
+
+int nfi_synthesis_backward_params(const nfi_synth_params* params, const nfi_synth_grads* grads,
+                                  const nfi_synth_param_grads* param_grads, void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  if (grads == nullptr) return fail("grads is NULL");
+  if (param_grads == nullptr) return fail("param_grads is NULL");
+  if (params->batch <= 0) return fail("empty batch");
+  return nfi::synth::backward_params(*params, *grads, *param_grads, (cudaStream_t)stream);
+}
+
+size_t nfi_synthesis_hvp_scratch_bytes(const nfi_synth_params* params) {
+  if (params == nullptr) return 0;
+  return nfi::synth::hvp_scratch_bytes(*params);
+}
+
+int nfi_synthesis_backward_hvp(const nfi_synth_params* params, const nfi_synth_hvp* hvp,
+                               const nfi_synth_param_grads* param_grads, void* stream) {
+  if (params == nullptr) return fail("params is NULL");
+  if (hvp == nullptr) return fail("hvp is NULL");
+  if (params->batch <= 0) return fail("empty batch");
+  return nfi::synth::backward_hvp(*params, *hvp, param_grads, (cudaStream_t)stream);
+}
+
+}  // extern "C"

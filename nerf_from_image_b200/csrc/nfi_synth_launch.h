@@ -1,33 +1,16 @@
-// Entry points of the synthesis-network translation unit (nfi_synth.cu), compiled in parallel
-// with the rest of the library.
+// The narrow entries of the synthesis-network translation unit (nfi_synth.cu), which serve the
+// networks other than the synthesis (the LPIPS VGG stack, nfi_lpips.cu; the encoder heads,
+// nfi_encoder.cu; the discriminator, nfi_disc.cu; the SegFormer backbone, nfi_segformer.cu).  Every
+// kernel they launch is compiled in nfi_synth.cu alone.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stddef.h>
 
 #include "nfi_pair.cuh"
-#include "nfi_synth.h"
 
 namespace nfi {
 namespace synth {
-size_t workspace_bytes(const nfi_synth_params& p);
-int forward(const nfi_synth_params& p, cudaStream_t st, char* err, size_t err_len);
-size_t saved_workspace_bytes(const nfi_synth_params& p);
-int forward_saved(const nfi_synth_params& p, cudaStream_t st, char* err, size_t err_len);
-int backward(const nfi_synth_params& p, const nfi_synth_grads& g, cudaStream_t st, char* err,
-             size_t err_len);
-int saved_preactivation(const nfi_synth_params& p, int block, int which, float* out, cudaStream_t st,
-                        char* err, size_t err_len);
-size_t param_workspace_bytes(const nfi_synth_params& p);
-int backward_params(const nfi_synth_params& p, const nfi_synth_grads& g,
-                    const nfi_synth_param_grads& pg, cudaStream_t st, char* err, size_t err_len);
-size_t hvp_scratch_bytes(const nfi_synth_params& p);
-int backward_hvp(const nfi_synth_params& p, const nfi_synth_hvp& h, const nfi_synth_param_grads* pg,
-                 cudaStream_t st, char* err, size_t err_len);
-
-// The narrow entries below serve the networks other than the synthesis (the LPIPS VGG stack,
-// nfi_lpips.cu; the encoder heads, nfi_encoder.cu; the discriminator, nfi_disc.cu; the SegFormer
-// backbone, nfi_segformer.cu).  Every kernel they launch is compiled in nfi_synth.cu alone.
 
 // Orders of a layer's weight w[co][ci][t] (t: its taps) as a GEMM operand or a weight gradient
 enum WeightOrder {
@@ -40,34 +23,31 @@ enum WeightOrder {
 
 // w[co ld + ci taps + t] gain -> the pair `out` in `order` (kTapCoCi, kTapCiCo or kCoTapCi).  With
 // gain 1 the pair is split from w's own values.
-int prep_weights(const float* w, int cout, int cin, int taps, int ld, float gain, int order, Pair out,
-                 cudaStream_t st, char* err, size_t err_len);
+int prep_weights(const float* w, int cout, int cin, int taps, int ld, float gain, int order, Pair out, cudaStream_t st);
 
 // g_w[co ld + ci taps + t] += gain tmp, tmp in `order` (kCoCiTap, kCiCoTap or kCoTapCi)
 int finish_wgrad(const float* tmp, int cout, int cin, int taps, int ld, float gain, int order, float* g_w,
-                 cudaStream_t st, char* err, size_t err_len);
+                 cudaStream_t st);
 
 // g_w += gain (the sum over terms k < n of wgrad(k)): each term's weight GEMM adds into tmp (cout cin
 // taps floats in `order`, zeroed first), then one finish_wgrad.  The terms are summed before the
 // gain, in term order.  A null g_w launches nothing.
 template <class Wgrad>
 int wgrad_terms(float* g_w, int n, Wgrad&& wgrad, int cout, int cin, int taps, int ld, float gain, int order,
-                float* tmp, cudaStream_t st, char* err, size_t err_len) {
+                float* tmp, cudaStream_t st) {
   if (g_w == nullptr) return 0;
-  NFI_LAUNCH_CHECK(cudaMemsetAsync(tmp, 0, (size_t)cout * cin * taps * sizeof(float), st));
+  NFI_CUDA(cudaMemsetAsync(tmp, 0, (size_t)cout * cin * taps * sizeof(float), st));
   for (int k = 0; k < n; ++k)
     if (int rc = wgrad(k)) return rc;
-  return finish_wgrad(tmp, cout, cin, taps, ld, gain, order, g_w, st, err, err_len);
+  return finish_wgrad(tmp, cout, cin, taps, ld, gain, order, g_w, st);
 }
 
 // g_b[c] += sum over chunks k < n_chunks of partial[k C + c], in chunk order.  A null g_b launches
 // nothing.
-int bias_reduce(const float* partial, int n_chunks, int C, float* g_b, cudaStream_t st, char* err,
-                size_t err_len);
+int bias_reduce(const float* partial, int n_chunks, int C, float* g_b, cudaStream_t st);
 
 // src [B][R][Cc] (+ bias[c], where bias is set) -> dst [B][Cc][R], or dst += it with `accumulate`
-int transpose(const float* src, int B, int R, int Cc, const float* bias, int accumulate, float* dst,
-              cudaStream_t st, char* err, size_t err_len);
+int transpose(const float* src, int B, int R, int Cc, const float* bias, int accumulate, float* dst, cudaStream_t st);
 
 // A plain stride-1, pad-1 3x3 convolution on conv_tc_kernel.  `in` is [B,H,W,C] as a bf16 pair of
 // plain values.
@@ -76,9 +56,8 @@ int transpose(const float* src, int B, int R, int Cc, const float* bias, int acc
 //   conv3x3_adjoint: the data gradient of such a conv, weights [9][N=Cin][C=Cout] (prep_weights,
 //            kTapCiCo), taps flipped -> raw_out fp32 [B,H,W,N]
 int conv3x3(int B, int H, int W, int C, int N, Pair in, Pair w, const float* bias, float* u_out, Pair out,
-            cudaStream_t st, char* err, size_t err_len);
-int conv3x3_adjoint(int B, int H, int W, int C, int N, Pair in, Pair w, float* raw_out, cudaStream_t st,
-                    char* err, size_t err_len);
+            cudaStream_t st);
+int conv3x3_adjoint(int B, int H, int W, int C, int N, Pair in, Pair w, float* raw_out, cudaStream_t st);
 
 // The weight gradient of such a conv on wgrad_tc_kernel:
 //   g_w[co,ci,ky,kx] += sum_{b,y,x} G[b,y,x,co] X[b,y+ky-1,x+kx-1,ci]
@@ -88,7 +67,7 @@ int conv3x3_adjoint(int B, int H, int W, int C, int N, Pair in, Pair w, float* r
 // fixed order: two calls on the same inputs give the same bits.  A null g_w launches nothing.
 size_t wgrad3x3_partial_floats(int B, int H, int W, int cout, int cin);
 int wgrad3x3(int B, int H, int W, int cout, int cin, int g_channels, Pair g, Pair x, float* partials,
-             float* g_w, cudaStream_t st, char* err, size_t err_len);
+             float* g_w, cudaStream_t st);
 
 // The discriminator's and SegFormer's layers, on the same two kernels:
 //   conv3x3_act: conv3x3 with the ACT epilogue's gain and negative slope: lrelu(gain (conv + bias))
@@ -103,18 +82,13 @@ int wgrad3x3(int B, int H, int W, int cout, int cin, int g_channels, Pair g, Pai
 //   wgrad1x1: g_w[co,ci] += sum over positions of g[.,co] x[.,ci], both [B,H,H,.]
 // (the partials and g_w as for wgrad3x3)
 int conv3x3_act(int B, int H, int W, int C, int N, Pair in, Pair w, const float* bias, float gain, float slope,
-                Pair out, cudaStream_t st, char* err, size_t err_len);
-int conv_down3x3(int B, int h, int C, int N, Pair phases, Pair w, float* raw_out, cudaStream_t st, char* err,
-                 size_t err_len);
-int conv_up3x3(int B, int h, int C, int N, Pair in, Pair w, float* raw_out, cudaStream_t st, char* err,
-               size_t err_len);
-int conv1x1(int B, int H, int C, int N, Pair in, Pair w, float* raw_out, cudaStream_t st, char* err,
-            size_t err_len);
+                Pair out, cudaStream_t st);
+int conv_down3x3(int B, int h, int C, int N, Pair phases, Pair w, float* raw_out, cudaStream_t st);
+int conv_up3x3(int B, int h, int C, int N, Pair in, Pair w, float* raw_out, cudaStream_t st);
+int conv1x1(int B, int H, int C, int N, Pair in, Pair w, float* raw_out, cudaStream_t st);
 size_t wgrad_down3x3_partial_floats(int B, int h, int cin, int cout);
-int wgrad_down3x3(int B, int h, int cin, int cout, Pair phases, Pair g, float* partials, float* g_wt,
-                  cudaStream_t st, char* err, size_t err_len);
+int wgrad_down3x3(int B, int h, int cin, int cout, Pair phases, Pair g, float* partials, float* g_wt, cudaStream_t st);
 size_t wgrad1x1_partial_floats(int B, int H, int cout, int cin);
-int wgrad1x1(int B, int H, int cout, int cin, Pair g, Pair x, float* partials, float* g_w, cudaStream_t st,
-             char* err, size_t err_len);
+int wgrad1x1(int B, int H, int cout, int cin, Pair g, Pair x, float* partials, float* g_w, cudaStream_t st);
 }  // namespace synth
 }  // namespace nfi

@@ -5,7 +5,7 @@
 #include "nfi_backward.cuh"
 
 namespace nfi {
-template int launch_forward_simt<true>(const nfi_render_params&, bool, cudaStream_t, char*, size_t);
+template int launch_forward_simt<true>(const nfi_render_params&, bool, cudaStream_t);
 template int launch_backward_simt<true>(const nfi_render_params&, const nfi_render_grads&,
-                                        cudaStream_t, char*, size_t);
+                                        cudaStream_t);
 }  // namespace nfi
