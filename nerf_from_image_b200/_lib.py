@@ -328,6 +328,24 @@ SEGFORMER_EXPORTS = {
                                               ctypes.c_void_p, ctypes.c_void_p]),
 }
 
+PNP_MAX_FOCALS, PNP_RECORD_DOUBLES = 64, 9
+
+
+class PnpParams(ctypes.Structure):
+    """struct nfi_pnp_params (include/nfi_pnp.h)."""
+    _fields_ = [(n, ctypes.c_int32) for n in ('batch', 'height', 'width', 'n_focals', 'refine')] + [
+        ('coords', ctypes.c_void_p), ('coords_stride', ctypes.c_int64 * 4)] + [
+        (n, ctypes.c_void_p) for n in ('mask', 'focals', 'world2cam', 'focal', 'error', 'record',
+                                       'workspace')] + [
+        ('workspace_bytes', ctypes.c_size_t)]
+
+
+# include/nfi_pnp.h (tests/test_pnp_abi.py)
+PNP_EXPORTS = {
+    'nfi_pnp_workspace_bytes': (ctypes.c_size_t, [ctypes.POINTER(PnpParams)]),
+    'nfi_pnp_solve': (ctypes.c_int, [ctypes.POINTER(PnpParams), ctypes.c_void_p]),
+}
+
 _lib = None
 _lock = threading.Lock()
 
@@ -370,7 +388,8 @@ def load():
             for name, (restype, argtypes) in (list(EXPORTS.items()) + list(LPIPS_EXPORTS.items())
                                        + list(ENCODER_EXPORTS.items()) + list(DISC_EXPORTS.items())
                                        + list(DISC_R1_EXPORTS.items())
-                                       + list(SEGFORMER_EXPORTS.items())):
+                                       + list(SEGFORMER_EXPORTS.items())
+                                       + list(PNP_EXPORTS.items())):
                 fn = getattr(lib, name, None)
                 if fn is None and os.environ.get('NFI_LIB_PATH'):
                     continue  # an older build under test lacks the newer entry points
